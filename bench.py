@@ -1,13 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- SSD300 images/sec (forward + DecodeDetections) on N B200s, plus the reference CPU arm.
+"""bench.py -- SSD300 images/sec (forward + DecodeDetections) on N H100s, plus the reference CPU arm.
 
   python bench.py --gpus 1 --steps 20 --warmup 3                   # this framework (one JSON line on stdout)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W                     # N ranks, NCCL, weak scaling (32 images / GPU)
   python bench.py --impl reference --steps 3 --warmup 1             # the reference's CPU path (oracle port) on host cores
+  python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR # also write the last timed step's detections to DIR
 
 Workload (BASELINE.json configs[1]): SSD300, batch 32 synthetic 300x300x3 float32 images, 21 classes, 8732 priors,
-he_normal random weights, DecodeDetections(conf 0.01, iou 0.45, top_k 200, nms cap 400).
+he_normal random weights, DecodeDetections(conf 0.01, iou 0.45, top_k 200, nms cap 400).  The images are normalised by the
+model's preprocessing ((x - mean) / 127.5): on raw 0..255 pixels the random weights drive the box offsets into the hundreds,
+every confidence to 1.0 and the decoded boxes to infinity, which no trained detector produces.
 A step = one forward + decode of one batch.  `value` = images/s with inputs resident in HBM (CUDA events, max over
 ranks); `e2e` = the same through SSDModel.predict with pinned host images copied H2D and the (B,200,6) result copied
 D2H inside the timed region.
@@ -25,11 +28,12 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 SC300 = [0.1, 0.2, 0.37, 0.54, 0.71, 0.88, 1.05]
+STDDEV = [127.5, 127.5, 127.5]       # divide_by_stddev of the inference workload (see above)
 BATCH = 32
 N_CLASSES = 20
 METRIC = 'SSD300 images/sec (fwd+decode)'
-WORKLOAD = ('SSD300 inference, batch 32 per GPU, synthetic 300x300x3 float32, 21 classes, 8732 priors, he_normal random '
-            'weights, DecodeDetections(0.01/0.45/200/400)')
+WORKLOAD = ('SSD300 inference, batch 32 per GPU, synthetic 300x300x3 float32 normalised by (x - mean) / 127.5, 21 classes, '
+            '8732 priors, he_normal random weights, DecodeDetections(0.01/0.45/200/400)')
 
 
 def _peaks():
@@ -38,7 +42,14 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return d, 'measured (MEASURED_PEAKS.json)'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback (B200_PROFILING.md)'
+    # NVIDIA's H100 SXM data sheet (a 700 W card): HBM3 bandwidth and dense BF16 tensor rate, peaks rather than sustained rates
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'H100 SXM data sheet (700 W)'
+
+
+def _tensor_peak(peaks):
+    """(TFLOP/s, key): the measured sustained bf16 rate where MEASURED_PEAKS.json has one, else the data-sheet peak."""
+    key = 'bf16_tflops_sustained' if 'bf16_tflops_sustained' in peaks else 'bf16_tflops'
+    return peaks[key], key
 
 
 def _weights():
@@ -53,7 +64,7 @@ class ClockSampler:
     """Samples SM clock / throttle reasons with NVML while the timed region runs."""
 
     def __init__(self, index):
-        self.samples, self.reasons, self.max_mhz = [], set(), None
+        self.samples, self.reasons, self.max_mhz, self.power_limit_w = [], set(), None, None
         self._stop = threading.Event()
         self._t = None
         try:
@@ -62,6 +73,7 @@ class ClockSampler:
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
         except Exception:
             self.nv = None
 
@@ -92,7 +104,8 @@ class ClockSampler:
             self._stop.set()
             self._t.join()
         med = float(np.median(self.samples)) if self.samples else None
-        return {'sm_mhz': med, 'sm_max_mhz': self.max_mhz, 'reasons': sorted(self.reasons), 'samples': len(self.samples)}
+        return {'sm_mhz': med, 'sm_max_mhz': self.max_mhz, 'power_limit_w': self.power_limit_w, 'reasons': sorted(self.reasons),
+                'samples': len(self.samples)}
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -106,7 +119,7 @@ def _decode_one(y):
     C++ in TensorFlow -- runs through the C restatement oracle/tf_nms.c (bit-identical to the NumPy one, which stays the fallback
     where no compiler exists): a Python NMS loop would make the CPU arm slower than the reference really is."""
     from oracle.decoder import decode_layer, tf_nms_c
-    with np.errstate(all='ignore'):                 # random weights produce inf/NaN boxes (handled as TensorFlow does)
+    with np.errstate(all='ignore'):                 # random weights can produce inf/NaN boxes (handled as TensorFlow does)
         return decode_layer(y, 0.01, 0.45, 200, 400, True, 300, 300, nms=tf_nms_c)
 
 
@@ -130,7 +143,7 @@ def cpu_reference_step(images, weights, pool=None):
     followed by the DecodeDetections restatement (NumPy + the C NMS of oracle/tf_nms.c; one image per worker process).  Returns the
     (n,200,6) detections."""
     from oracle.model import ssd_vgg_forward
-    y = ssd_vgg_forward(images, weights, 300, N_CLASSES, scales=SC300)
+    y = ssd_vgg_forward(images, weights, 300, N_CLASSES, scales=SC300, divide_by_stddev=STDDEV)
     if pool is None:
         return _decode_one(y)
     return np.concatenate(pool.map(_decode_one, [y[i:i + 1] for i in range(y.shape[0])]), axis=0)
@@ -145,9 +158,9 @@ def _pick_threads(x, w):
     best, best_t = None, 0
     for t in sorted({min(ncpu, c) for c in (8, 16, 32, 64, ncpu)}):
         torch.set_num_threads(t)
-        ssd_vgg_forward(x[:1], w, 300, N_CLASSES, scales=SC300)           # warm the thread pool
+        ssd_vgg_forward(x[:1], w, 300, N_CLASSES, scales=SC300, divide_by_stddev=STDDEV)           # warm the thread pool
         t0 = time.perf_counter()
-        ssd_vgg_forward(x, w, 300, N_CLASSES, scales=SC300)
+        ssd_vgg_forward(x, w, 300, N_CLASSES, scales=SC300, divide_by_stddev=STDDEV)
         dt = time.perf_counter() - t0
         if best is None or dt < best:
             best, best_t = dt, t
@@ -169,7 +182,7 @@ def time_cpu_reference(n_images, reps, warmup):
     t_fwd = t_dec = 0.0
     for _ in range(reps):
         t0 = time.perf_counter()
-        y = ssd_vgg_forward(x, w, 300, N_CLASSES, scales=SC300)
+        y = ssd_vgg_forward(x, w, 300, N_CLASSES, scales=SC300, divide_by_stddev=STDDEV)
         t1 = time.perf_counter()
         pool.map(_decode_one, [y[i:i + 1] for i in range(y.shape[0])])
         t2 = time.perf_counter()
@@ -289,7 +302,7 @@ def micro_benchmarks(peaks):
     ms = _time_cuda(train_step, iters=5, warm=2)
     fl = 3.0 * mt.flops(Bt)[0]
     out['train_step_ssd300_b32'] = {'ms': ms, 'images_per_s': Bt * 1e3 / ms, 'algorithmic_TFLOPs': fl / ms / 1e9,
-                                    'frac_tensor_peak': fl / ms / 1e9 / peaks['bf16_tflops_sustained'], 'n_params': tr.n_params}
+                                    'frac_tensor_peak': fl / ms / 1e9 / _tensor_peak(peaks)[0], 'n_params': tr.n_params}
     return out
 
 
@@ -365,7 +378,7 @@ def dist_extras(world, rank, peaks, model_inf_weights):
     # --- configs 1/2 as the survey partitions them: a FIXED global batch of 32 images, 32 / world per rank (strong scaling)
     if 32 % world == 0:
         bl = 32 // world
-        ms_ = ssd_300((300, 300, 3), 20, mode='inference', scales=SC300)
+        ms_ = ssd_300((300, 300, 3), 20, mode='inference', scales=SC300, divide_by_stddev=STDDEV)
         ms_.set_weights(model_inf_weights)
         lo, hi = shard_bounds(32, rank, world)
         xs = [torch.from_numpy(synth.synth_images(200 + i, 32, 300, 300)[lo:hi]).cuda() for i in range(2)]
@@ -450,18 +463,21 @@ def run_ours(args):
     peaks, peaks_src = _peaks()
 
     precision = 'bf16' if args.fast else 'bf16x3'
-    model = ssd_300((300, 300, 3), N_CLASSES, mode='inference', scales=SC300, precision=precision)
+    model = ssd_300((300, 300, 3), N_CLASSES, mode='inference', scales=SC300, divide_by_stddev=STDDEV, precision=precision)
     model.set_weights(_weights())
-    # several distinct input batches so that a step never finds its images in L2 (4 x 34.6 MB > 126 MB L2)
+    # several distinct input batches so that a step never finds its images in L2 (4 x 34.6 MB > 50 MB L2)
     n_in = 4
     host = [torch.from_numpy(synth.synth_images(100 * rank + i, BATCH, 300, 300)).pin_memory() for i in range(n_in)]
     dev = [h.cuda() for h in host]
     from ssd_keras_b200.distributed import all_gather_detections
 
+    last = {}
+
     def step_device(i):
         out = model.predict_device(dev[i % n_in])
         if world > 1:
             out = all_gather_detections(out)            # decoded boxes of every rank (SURVEY 8e, C2)
+        last['out'] = out
         return out
 
     pinned_out = torch.empty((world * BATCH, 200, 6), dtype=torch.float32).pin_memory()
@@ -508,6 +524,10 @@ def run_ours(args):
         return ms, clocks, launches
 
     ms_dev, clocks, launches = timed(step_device, args.steps, max(args.warmup, 3))
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step: the (world*32, 200, 6) float32 detections [class, conf, xmin, ymin, xmax, ymax]
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'detections.npy'), last['out'].float().cpu().numpy())
     # end to end: one untimed pipelined pass, then K batches in ONE timed pipelined pass (K uploads + K downloads inside it)
     run_e2e(max(args.warmup, 3))
     barrier()
@@ -522,7 +542,7 @@ def run_ours(args):
     ips = world * BATCH * args.steps / (ms_dev * 1e-3)
     ips_e2e = world * BATCH * args.steps / (ms_e2e * 1e-3)
 
-    # dominant kernel: the tcgen05 convolution.  Time of all conv launches of one step via CUDA events on the launch
+    # dominant kernel: the wgmma convolution.  Time of all conv launches of one step via CUDA events on the launch
     # stream (instrumented passes outside the timed region).
     model.set_timing(BATCH, True)
     conv_ms = []
@@ -533,32 +553,21 @@ def run_ours(args):
     model.set_timing(BATCH, False)
     conv_ms = float(np.median(conv_ms))
     fl_algo, fl_issued = model.flops(BATCH)
-    peak = peaks.get('bf16_tflops_sustained', peaks.get('bf16_tflops'))
-    traffic, traffic_src = None, None
-    for name in ('r02_conv_traffic.json', 'r01_conv_traffic.json'):       # newest ncu --set full capture of this workload first
-        tp = os.path.join(ROOT, 'profiles', name)
-        if os.path.exists(tp):
-            with open(tp) as f:
-                tj = json.load(f)
-            traffic = tj.get('dram_bytes_per_step')
-            traffic_src = 'profiles/%s (dram read+write bytes of the %d conv launches of one step, ncu --set full; %s)' % (
-                name, tj.get('launches_per_step', 0), tj.get('source', ''))
-            break
-    roofline = {'bound': 'tensor', 'kernel': 'conv_tcgen05_kernel (all conv launches of one step)',
+    peak, peak_key = _tensor_peak(peaks)
+    roofline = {'bound': 'tensor', 'kernel': 'conv_wgmma_kernel (all conv launches of one step)',
                 'achieved': fl_algo / conv_ms / 1e9, 'peak': peak, 'unit': 'TFLOP/s', 'frac': fl_algo / conv_ms / 1e9 / peak,
-                'peak_source': peaks_src + ', bf16_tflops_sustained', 'traffic': traffic, 'traffic_unit': 'bytes per step',
-                'traffic_source': traffic_src,
+                'peak_source': peaks_src + ', ' + peak_key,
                 'algorithmic_tflop_per_step': fl_algo / 1e12, 'issued_mma_tflop_per_step': fl_issued / 1e12,
                 'issued_tflops': fl_issued / conv_ms / 1e9, 'issued_frac': fl_issued / conv_ms / 1e9 / peak,
                 'conv_ms_per_step': conv_ms}
 
     line = {'metric': METRIC, 'value': ips, 'unit': 'images/s', 'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3),
             'ms_per_step': ms_dev / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-            'dtype': 'bf16x3 (bf16 hi+lo operands, 3 tcgen05 MMAs per product, fp32 accumulate)' if not args.fast else 'bf16',
-            'data': 'synthetic',
+            'dtype': 'bf16x3 (bf16 hi+lo operands, 3 wgmma MMAs per product, fp32 accumulate)' if not args.fast else 'bf16',
+            'data': 'synthetic', 'gpu': torch.cuda.get_device_name(local),
             'config': {'workload': WORKLOAD, 'global_batch': world * BATCH, 'parallelism': 'dp%d' % world, 'precision': precision,
                        'l2': 'no explicit flush: %d distinct 34.6 MB input batches are rotated and each step streams >4 GB of '
-                             'activations through the 126 MB L2' % n_in},
+                             'activations through the 50 MB L2' % n_in},
             'e2e': {'value': ips_e2e, 'unit': 'images/s', 'h2d_bytes_per_step': world * BATCH * 300 * 300 * 3 * 4,
                     'd2h_bytes_per_step': world * BATCH * 200 * 6 * 4, 'ms_per_step': ms_e2e / args.steps,
                     'note': 'SSDModel.predict_stream (the pipeline behind predict / predict_generator) on pinned-host inputs: the H2D '
@@ -622,6 +631,7 @@ def main():
     ap.add_argument('--fast', action='store_true', help='single-pass bf16 convolutions instead of bf16x3')
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-micro', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last timed step\'s detections to DIR/detections.npy (float32)')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * ssdk.h -- C-ABI of the B200-native SSD hot path (libssdk.so).
+ * ssdk.h -- C-ABI of the H100-native SSD hot path (libssdk.so).
  *
  * The reference (pierluigiferrari/ssd_keras) is pure Python: it has no FFI / plugin
  * interface of its own, so the drop-in boundary is its public Python surface (SURVEY.md
@@ -266,7 +266,7 @@ int ssdk_ssd_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true_dev, const
 /* ------------------------------------------------------------------------------------------
  * Model graph.  Replaces ssd_300 (models/keras_ssd300.py:31-457), ssd_512 (models/keras_ssd512.py:31-477)
  * and build_model (models/keras_ssd7.py:30-430) + L2Normalization
- * (keras_layers/keras_layer_L2Normalization.py:61-63): a static plan of tcgen05 implicit-GEMM
+ * (keras_layers/keras_layer_L2Normalization.py:61-63): a static plan of wgmma implicit-GEMM
  * convolutions, pooling, normalisation and the head epilogue producing (B,P,C+12).
  * The graph is described layer by layer by the host (Python mirrors the reference builders).
  * ------------------------------------------------------------------------------------------ */
@@ -321,7 +321,7 @@ int ssdk_l2_normalize(ssdk_ctx* ctx, const float* x_dev, long long rows, int C, 
 
 /* Stand-alone Conv2D forward (what every `Conv2D(...)` of models/keras_ssd300.py:274-335 computes; SURVEY 8b `ssdk_conv2d_fwd`):
  * y = act(conv(x, kernel) + bias) on float32 NHWC device tensors, kernel HWIO / bias on the HOST (copied and packed by the call).
- * x (B,H,W,Cin) -> y (B,Ho,Wo,Cout), Ho = (H + pad_t + pad_b - dilation*(kh-1) - 1)/stride + 1.  Runs the same tcgen05 plan the
+ * x (B,H,W,Cin) -> y (B,Ho,Wo,Cout), Ho = (H + pad_t + pad_b - dilation*(kh-1) - 1)/stride + 1.  Runs the same wgmma plan the
  * model graphs use (precision 0 = bf16x3, 1 = bf16) as a one-layer graph built and destroyed inside the call: it synchronises
  * the stream and allocates -- a utility for tests and interop; steady-state users describe their layers to ssdk_model_create. */
 int ssdk_conv2d_fwd(ssdk_ctx* ctx, const float* x_dev, int B, int H, int W, int Cin, const float* kernel_hwio_host,

@@ -1,4 +1,4 @@
-"""ssd_keras_b200 -- the SSD detection hot path of pierluigiferrari/ssd_keras on NVIDIA B200 (sm_100a).
+"""ssd_keras_b200 -- the SSD detection hot path of pierluigiferrari/ssd_keras on NVIDIA H100 (sm_90a).
 
 The sub-packages mirror the reference's module layout, so ``from ssd_keras_b200.models.keras_ssd300 import ssd_300``
 replaces ``from models.keras_ssd300 import ssd_300`` and so on.  The hot path -- model forward / backward, encoder, decoders,

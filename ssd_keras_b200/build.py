@@ -1,7 +1,8 @@
-"""Build libssdk.so (sm_100a only) in-tree with nvcc.
+"""Build libssdk.so (sm_90a only) in-tree with nvcc.
 
 ``python -m ssd_keras_b200.build`` or ``build_library()``.  nvcc cross-compiles without a GPU.
-The resulting ``ssd_keras_b200/_lib/libssdk.so`` is git-ignored but travels to the GPU box.
+The resulting ``ssd_keras_b200/_lib/libssdk.so`` is git-ignored; the stamp next to it holds a digest of the sources and flags, so
+a build from other sources or for another architecture is never reused.
 """
 import concurrent.futures
 import hashlib
@@ -15,7 +16,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIBDIR = os.path.join(HERE, '_lib')
 LIB = os.path.join(LIBDIR, 'libssdk.so')
 
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-Xcompiler', '-ffp-contract=off',
           '-Xcudafe', '--diag_suppress=177', '-Xcudafe', '--diag_suppress=550']
 # exactness-critical files: no FMA contraction on the device either
@@ -50,6 +51,7 @@ def _digest():
                 h.update(open(os.path.join(root, f), 'rb').read())
     h.update(repr(SOURCES).encode())
     h.update(repr(COMMON).encode())
+    h.update(repr(ARCH).encode())
     return h.hexdigest()
 
 

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libssdk.so (B200 / sm_100a).
+// Shared host/device helpers for libssdk.so (H100 / sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -52,7 +52,7 @@ struct Scratch {
 
 struct ssdk_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int64_t launches = 0;
   ssdk::Scratch ws[4];          // decode / loss / nms workspaces
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for

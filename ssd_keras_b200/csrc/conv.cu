@@ -1,8 +1,8 @@
-// tcgen05 implicit-GEMM convolution for sm_100a plus the small data-movement kernels around it.
+// wgmma implicit-GEMM convolution for sm_90a plus the small data-movement kernels around it.
 // Reference ops: Conv2D / MaxPooling2D / Lambda preprocessing / L2Normalization / Reshape+softmax+Concat in
 // models/keras_ssd300.py:263-419, keras_layers/keras_layer_L2Normalization.py:61-63.
 //
-// conv_tcgen05_kernel -- persistent, warp-specialised (DESIGN.md section "conv"):
+// conv_wgmma_kernel -- persistent, 256 threads = two warpgroups (DESIGN.md section "conv"):
 //   GEMM view   D[M = output pixels, N = Cout] = sum over (tap, cin-block) A_tap[M, 64] * W_tap[N, 64]^T.
 //   "im2col in the TMA descriptor": the activation tensor is a zero-bordered NHWC buffer viewed as a 2-D
 //   matrix [B*Hp*Wp, C]; the A tile of filter tap (kh, kw) for output rows [m0, m0+128) is simply rows
@@ -10,12 +10,11 @@
 //   padding / dilation come for free (the border is zero, rows past the end are TMA zero-filled).
 //   Outputs are computed for every position of the padded grid ("virtual rows"); the epilogue stores the
 //   valid ones, and m-tiles without any valid row are not scheduled.
-//   warp 0: TMA producer (one elected lane)      warp 1: tcgen05.mma issuer (one lane)
-//   warp 2: TMEM allocator                        warps 4-7: epilogue (tcgen05.ld -> bias/BN/act -> store)
-//   smem ring of `stages` {A_hi, A_lo, W_hi, W_lo} 128B-swizzled K-major tiles, full/empty mbarriers;
-//   two TMEM accumulators (2*BN columns) so the epilogue of tile i overlaps the main loop of tile i+1.
+//   One thread issues the TMA loads of a ring of `stages` {A_hi, A_lo, W_hi, W_lo} 128B-swizzled K-major tiles (full / empty
+//   mbarriers); each warpgroup runs wgmma m64nBNk16 on its 64 rows with fp32 accumulators in registers.  After the K loop the
+//   accumulators go through shared memory (over the drained ring) to an epilogue with one thread per row (bias/BN/act -> store).
 //   Precision: operands are bf16 "hi + lo" pairs; three MMAs per k-step (hi*hi, hi*lo, lo*hi) accumulate
-//   in fp32 TMEM, which reproduces an fp32 convolution to ~1e-5 relative (split=0 issues hi*hi only).
+//   in fp32, which reproduces an fp32 convolution to ~1e-5 relative (split=0 issues hi*hi only).
 #include "conv.cuh"
 #include "tc.cuh"
 #include <cudaTypedefs.h>
@@ -80,84 +79,57 @@ int make_tmap_4d(CUtensorMap* out, const void* base, const uint64_t dims_[4], co
   return SSDK_OK;
 }
 
-static constexpr int kBM = 128;          // UMMA M (rows per tile)
+static constexpr int kBM = 128;          // output rows per tile: two warpgroups of 64
 static constexpr int kBK = 64;           // channels per k-block = one 128-byte swizzle atom of bf16
 static constexpr int kATile = kBM * kBK * 2;   // 16 KB
+static constexpr int kAccPad = 4;        // the fp32 accumulator tile in shared memory has rows of BN + 4 floats (conflict-free reads)
+static constexpr int kParBytes = 3 * 256 * (int)sizeof(float);   // bias | bn scale | bn shift of one n-tile
 
-static int mt_of(const ConvArgs& a) { return a.mt > 1 ? a.mt : 1; }
-static size_t slot_a_bytes(const ConvArgs& a) { return (size_t)(a.slab_rows + (mt_of(a) - 1) * kBM) * kBK * 2 * (a.split ? 2 : 1); }
-static size_t slot_b_bytes(const ConvArgs& a) { return (size_t)a.BN * kBK * 2 * (a.split ? 2 : 1); }
-static size_t epi_param_bytes(const ConvArgs& a) { return ((size_t)a.cout * 3 * sizeof(float) + 127) / 128 * 128; }   // bias | bn scale | bn shift
-size_t conv_smem_bytes(const ConvArgs& a) { return 1024 + slot_a_bytes(a) * a.stages_a + slot_b_bytes(a) * a.stages_b + 512 + epi_param_bytes(a); }
-// Two rings: A slabs (one per (kh, channel block), shared by the KW taps of that row) and weight tiles (one per tap).
+static size_t stage_bytes(const ConvArgs& a) { return ((size_t)kATile + (size_t)a.BN * kBK * 2) * (a.split ? 2 : 1); }
+// (+32 floats: the 32-column chunk reads of the epilogue may run past the end of a row whose width is not a multiple of 64)
+static size_t acc_tile_bytes(int BN) { return ((size_t)kBM * (BN + kAccPad) + 32) * sizeof(float); }
+static size_t ring_bytes(const ConvArgs& a) { return std::max(stage_bytes(a) * a.stages, acc_tile_bytes(a.BN)); }
+size_t conv_smem_bytes(const ConvArgs& a) { return 1024 + ring_bytes(a) + 256 + kParBytes; }
+// As many ring stages ({A_hi, A_lo, W_hi, W_lo} per k-iteration) as shared memory holds, 2 ... 6.
 void conv_pick_stages(ConvArgs& a) {
-  const size_t budget = 218 * 1024 - 1536 - epi_param_bytes(a);
-  if (a.resident_b) {                       // weights resident: stages_b counts the tiles, the rest goes to A slabs
-    a.stages_b = a.KH * a.KW * a.kblocks;
-    a.stages_a = 2;
-    while (a.stages_a < 4 && slot_a_bytes(a) * (a.stages_a + 1) + slot_b_bytes(a) * a.stages_b <= budget) ++a.stages_a;
-    return;
-  }
-  a.stages_a = 2; a.stages_b = 2;
-  int max_a = 4, max_b = 6;
-  if (const char* e = getenv("SSDK_SA_MAX")) max_a = atoi(e);
-  if (const char* e = getenv("SSDK_SB_MAX")) max_b = atoi(e);
-  bool grew = true;
-  while (grew) {
-    grew = false;
-    if (a.stages_b < max_b && slot_a_bytes(a) * a.stages_a + slot_b_bytes(a) * (a.stages_b + 1) <= budget) { ++a.stages_b; grew = true; }
-    if (a.stages_a < max_a && slot_a_bytes(a) * (a.stages_a + 1) + slot_b_bytes(a) * a.stages_b <= budget) { ++a.stages_a; grew = true; }
+  a.stages = 2;
+  while (a.stages < 6) {
+    ++a.stages;
+    if (conv_smem_bytes(a) > 227 * 1024) { --a.stages; break; }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors (PTX wrappers: tc.cuh)
-// ------------------------------------------------------------------------------------------------
-// K-major, 128B-swizzled operand tile: start address, SBO = 1024 B (8 rows x 128 B), descriptor version 1 (sm_100)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t addr, int bo_mode = 0) {
-  uint64_t d = 0;
-  const uint32_t phase = (addr >> 7) & 0x7u;          // start row inside the 8-row (1024 B) swizzle atom
-  if (bo_mode == 1) d |= (uint64_t)phase << 49;       // [49,52) base offset
-  else if (bo_mode == 2) d |= (uint64_t)((8u - phase) & 7u) << 49;
-  d |= (uint64_t)((addr >> 4) & 0x3FFFu);            // [0,14)  start address >> 4
-  d |= (uint64_t)0 << 16;                            // [16,30) leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)((1024u >> 4) & 0x3FFFu) << 32;     // [32,46) stride byte offset
-  d |= (uint64_t)1 << 46;                            // [46,48) version = 1
-  d |= (uint64_t)2 << 61;                            // [61,64) layout = SWIZZLE_128B
-  return d;
-}
-// constant upper part of that descriptor: SBO = 1024 B at [32,46), version 1 at [46,48), SWIZZLE_128B at [61,64)
-static constexpr uint64_t kDescHi = ((uint64_t)(1024u >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-  // c_format F32 (bit 4), a/b format BF16 (bits 7, 10), K-major A and B, N>>3 at bit 17, M>>4 at bit 24
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kBM >> 4) << 24);
-}
 __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == SSDK_ACT_RELU) return fmaxf(x, 0.f);
   if (act == SSDK_ACT_ELU) return x > 0.f ? x : expm1f(x);
   return x;
 }
 
-// Accumulator read: 32 columns of this thread's TMEM lane; with a separate cross-term accumulator (`xoff` columns further)
-// the two partial sums are added here in fp32 round-to-nearest.
-__device__ __forceinline__ void ld_acc32(uint32_t taddr, uint32_t xoff, uint32_t (&v)[32]) {
-  if (!xoff) { tmem_ld32(taddr, v); return; }
-  {
-    uint32_t w[32];
-    tmem_ld32_nowait(taddr, v);            // both loads in flight, one wait (SSDK: the epilogue of 256-wide tiles with a cross-term
-    tmem_ld32_nowait(taddr + xoff, w);     // accumulator does not overlap the next tile's MMAs, so its latency is on the critical path)
-    tmem_ld_wait();
+// 32 accumulator columns of this thread's row of the shared-memory accumulator tile
+__device__ __forceinline__ void ld_acc32(const float* p, float (&v)[32]) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
+  for (int q = 0; q < 8; ++q) {
+    const float4 t = reinterpret_cast<const float4*>(p)[q];
+    v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+  }
+}
+
+// Accumulator fragment of one warpgroup (64 rows x BN) -> rows [64 * wg, +64) of the shared-memory tile (row pitch BN + kAccPad)
+template <int BN>
+__device__ __forceinline__ void store_acc_tile(const float (&acc)[BN / 2], float* s_acc, int wg, int warp, int lane) {
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(s_acc + (size_t)r0 * (BN + kAccPad) + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(s_acc + (size_t)(r0 + 8) * (BN + kAccPad) + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
   }
 }
 
 // Predictor-head epilogue for a compile-time row width CP4 = n_classes + 4 (25: Pascal VOC, the benchmark configuration): one thread =
 // one pixel = n_boxes prior rows.  With CP4 known the accumulator columns of a box are compile-time register indices, so each box
-// costs one sweep: <= 2 TMEM loads, C bias adds, C exponentials (kept in registers), one reciprocal, C+12 stores.
+// costs one sweep: <= 2 loads of 32 columns, C bias adds, C exponentials (kept in registers), one reciprocal, C+12 stores.
 template <int CP4>
-__device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, uint32_t t_row, uint32_t xoff, bool valid, int n, int pix,
-                                               const float* s_bias) {
+__device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, const float* arow, int n, int pix, const float* s_bias) {
   constexpr int C = CP4 - 4, RW = C + 12;
 #pragma unroll
   for (int bx = 0; bx < 8; ++bx) {
@@ -166,15 +138,14 @@ __device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, uint32_t t_
     const int c_lo = bx * CP4;                                   // compile-time after unrolling
     const int k_lo = c_lo >> 5, k_hi = (c_lo + CP4 - 1) >> 5;
     if (c_lo + CP4 > kMaxCol) break;
-    uint32_t v0[32], v1[32];
-    ld_acc32(t_row + (uint32_t)(k_lo * 32), xoff, v0);
-    if (k_hi != k_lo) ld_acc32(t_row + (uint32_t)(k_hi * 32), xoff, v1);
-    if (!valid) continue;
+    float v0[32], v1[32];
+    ld_acc32(arow + k_lo * 32, v0);
+    if (k_hi != k_lo) ld_acc32(arow + k_hi * 32, v1);
     float e[CP4];
 #pragma unroll
     for (int r = 0; r < CP4; ++r) {
       const int col = c_lo + r;
-      e[r] = __uint_as_float(((col >> 5) == k_lo) ? v0[col & 31] : v1[col & 31]) + s_bias[col];
+      e[r] = (((col >> 5) == k_lo) ? v0[col & 31] : v1[col & 31]) + s_bias[col];
     }
     float mx = e[0];
 #pragma unroll
@@ -196,18 +167,17 @@ __device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, uint32_t t_
 }
 
 // Epilogue of the activation-producing launches: bias / folded BatchNorm / activation -> bf16 hi+lo planes, 8 channels per
-// 16-byte store.  BWD adds what the data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
-template <bool BWD, bool PIPE = false>
-__device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, uint32_t xoff, int ncols, int n0, size_t o, bool valid,
-                                          const float* s_bias, const float* s_scale, const float* s_shift) {
+// 16-byte store.  `acc`, `sb`, `ss`, `sh` and output element `o` all start at this thread's first column.  BWD adds what the
+// data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
+template <bool BWD>
+__device__ __forceinline__ void epi_split(const ConvArgs& args, const float* acc, int ncols, size_t o, const float* sb,
+                                          const float* ss, const float* sh) {
   if (!BWD && !args.bn_scale && args.act == SSDK_ACT_RELU && args.out_lo) {
     // the common forward case (bias + ReLU, hi/lo planes) without per-element branches: packed conversions (two values per
-    // cvt.rn.bf16x2.f32), biases fetched four at a time, and 32-byte stores (one full sector per lane and instruction: a thread's
-    // row is 2*Cout bytes of its own, so 16-byte stores leave every sector half written per instruction).  Bit-identical to the
-    // generic path below.
-    const bool wide = (args.out_Cs % 16 == 0) && ((n0 & 15) == 0);
-    // one chunk of 32 accumulator columns: bias + ReLU, hi/lo split, stores
-    auto process = [&](const uint32_t (&vr)[32], int c0) {
+    // cvt.rn.bf16x2.f32) and biases fetched four at a time.  Bit-identical to the generic path below.
+    for (int c0 = 0; c0 < ncols; c0 += 32) {
+      float vr[32];
+      ld_acc32(acc + c0, vr);
 #pragma unroll
       for (int g2 = 0; g2 < 2; ++g2) {
         uint32_t ph[8], pl[8];
@@ -215,13 +185,13 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, 
         for (int h = 0; h < 2; ++h) {
           const int g = g2 * 2 + h;
           if (c0 + g * 8 < ncols) {
-            const float4 b0 = *reinterpret_cast<const float4*>(s_bias + n0 + c0 + g * 8);
-            const float4 b1 = *reinterpret_cast<const float4*>(s_bias + n0 + c0 + g * 8 + 4);
+            const float4 b0 = *reinterpret_cast<const float4*>(sb + c0 + g * 8);
+            const float4 b1 = *reinterpret_cast<const float4*>(sb + c0 + g * 8 + 4);
             const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-              const float f0 = fmaxf(__uint_as_float(vr[g * 8 + j * 2]) + bb[j * 2], 0.f);
-              const float f1 = fmaxf(__uint_as_float(vr[g * 8 + j * 2 + 1]) + bb[j * 2 + 1], 0.f);
+              const float f0 = fmaxf(vr[g * 8 + j * 2] + bb[j * 2], 0.f);
+              const float f1 = fmaxf(vr[g * 8 + j * 2 + 1] + bb[j * 2 + 1], 0.f);
               const __nv_bfloat162 hh = __floats2bfloat162_rn(f0, f1);
               const uint32_t hp = *reinterpret_cast<const uint32_t*>(&hh);
               const __nv_bfloat162 ll = __floats2bfloat162_rn(f0 - __uint_as_float(hp << 16), f1 - __uint_as_float(hp & 0xffff0000u));
@@ -230,12 +200,7 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, 
           }
         }
         const int cA = c0 + g2 * 16;
-        if (wide && cA + 16 <= ncols) {
-          asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(args.out_hi + o + cA), "r"(ph[0]), "r"(ph[1]), "r"(ph[2]),
-                       "r"(ph[3]), "r"(ph[4]), "r"(ph[5]), "r"(ph[6]), "r"(ph[7]) : "memory");
-          asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(args.out_lo + o + cA), "r"(pl[0]), "r"(pl[1]), "r"(pl[2]),
-                       "r"(pl[3]), "r"(pl[4]), "r"(pl[5]), "r"(pl[6]), "r"(pl[7]) : "memory");
-        } else {
+        {
           if (cA < ncols) {
             *reinterpret_cast<uint4*>(args.out_hi + o + cA) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
             *reinterpret_cast<uint4*>(args.out_lo + o + cA) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
@@ -246,49 +211,12 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, 
           }
         }
       }
-    
-    };
-    if constexpr (PIPE) {
-      // software-pipelined accumulator reads (conv_tcgen05_kernel): the TMEM loads of chunk c+1 are issued before chunk c is converted
-      // and stored, so their latency hides behind that work (tcgen05.wait::ld waits for every load this thread has issued).  It
-      // matters for the 256-wide tiles with a cross-term accumulator: they have ONE accumulator set, so their epilogue does not run
-      // under the next tile's MMAs.  args.epi_pipe (SSDK_EPI_PIPE): 2 = as described (default), 1 = both loads of a chunk in flight
-      // but no prefetch, 0 = one load at a time.
-      const int pipe = args.epi_pipe;
-      uint32_t va[32], vb[32];
-      if (pipe == 2) {
-        tmem_ld32_nowait(t_row, va);
-        if (xoff) tmem_ld32_nowait(t_row + xoff, vb);
-      }
-      for (int c0 = 0; c0 < ncols; c0 += 32) {
-        uint32_t vr[32];
-        if (pipe != 2) {
-          tmem_ld32_nowait(t_row + (uint32_t)c0, va);
-          if (pipe == 0) tmem_ld_wait();
-          if (xoff) tmem_ld32_nowait(t_row + (uint32_t)c0 + xoff, vb);
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) vr[j] = xoff ? __float_as_uint(__uint_as_float(va[j]) + __uint_as_float(vb[j])) : va[j];
-        if (pipe == 2 && c0 + 32 < ncols) {
-          tmem_ld32_nowait(t_row + (uint32_t)(c0 + 32), va);
-          if (xoff) tmem_ld32_nowait(t_row + (uint32_t)(c0 + 32) + xoff, vb);
-        }
-        if (valid) process(vr, c0);
-      }
-    } else {
-      for (int c0 = 0; c0 < ncols; c0 += 32) {
-        uint32_t vr[32];
-        ld_acc32(t_row + (uint32_t)c0, xoff, vr);
-        if (valid) process(vr, c0);
-      }
     }
     return;
   }
   for (int c0 = 0; c0 < ncols; c0 += 32) {
-    uint32_t vr[32];
-    ld_acc32(t_row + (uint32_t)c0, xoff, vr);
-    if (!valid) continue;
+    float vr[32];
+    ld_acc32(acc + c0, vr);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       if (c0 + g * 8 < ncols) {
@@ -307,9 +235,9 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, 
           float f[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int col = n0 + c0 + g * 8 + j * 2 + e;
-            float xv = __uint_as_float(vr[g * 8 + j * 2 + e]) + s_bias[col];
-            if (args.bn_scale) xv = xv * s_scale[col] + s_shift[col];
+            const int col = c0 + g * 8 + j * 2 + e;
+            float xv = vr[g * 8 + j * 2 + e] + sb[col];
+            if (args.bn_scale) xv = xv * ss[col] + sh[col];
             xv = apply_act(xv, args.act);
             if (BWD) {
               if (!(__uint_as_float(((mkw[j] >> (e * 16)) & 0xffffu) << 16) > 0.f)) xv = 0.f;       // ReLU'(forward value)
@@ -333,318 +261,208 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, uint32_t t_row, 
 // ------------------------------------------------------------------------------------------------
 // The convolution kernel
 // ------------------------------------------------------------------------------------------------
+// MODE (ConvArgs::split / acc_split as a compile-time constant, so that every wgmma of the K loop is issued on a uniform path):
+//   kSingle  one bf16 product per k-step;
+//   kSplitXS bf16x3, the cross terms (hi*lo, lo*hi) accumulate in their own registers and are added to the hi*hi sum after the
+//            K loop: the large accumulator takes one rounding add per k-step instead of three (deep-K layers: fc6, fc7,
+//            conv6_2 ... stay within 1e-4 of an fp32 convolution).
+enum { kSingle = 0, kSplitXS = 2 };
+template <int BN, int MODE>
 __global__ void __launch_bounds__(256, 1)
-conv_tcgen05_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-                    const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
-                    const __grid_constant__ ConvArgs args) {
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+                  const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                  const __grid_constant__ ConvArgs args) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int SA = args.stages_a, SB = args.stages_b, BN = args.BN, split = args.split;
-  const int MT = args.mt > 1 ? args.mt : 1;                            // m-tiles per work unit
-  const uint32_t a_plane = (uint32_t)(args.slab_rows + (MT - 1) * kBM) * kBK * 2;   // one A slab plane (hi or lo)
-  const uint32_t a_box = (uint32_t)args.slab_rows * kBK * 2;           // bytes one TMA box delivers
-  const uint32_t b_tile = (uint32_t)BN * kBK * 2;
-  const uint32_t slot_a = a_plane * (split ? 2 : 1), slot_b = b_tile * (split ? 2 : 1);
-  const uint32_t ring_b = smem_base + slot_a * SA;
-  const uint32_t bar_base = ring_b + slot_b * SB;
-  // barrier slots (8 B each): fullA[SA] | emptyA[SA] | fullB[SB] | emptyB[SB] | tmem_full[2] | tmem_empty[2] | tmem ptr
-  auto fullA = [&](int s) { return bar_base + 8u * s; };
-  auto emptyA = [&](int s) { return bar_base + 8u * (SA + s); };
-  auto fullB = [&](int s) { return bar_base + 8u * (2 * SA + s); };
-  auto emptyB = [&](int s) { return bar_base + 8u * (2 * SA + SB + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * SA + 2 * SB + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * SA + 2 * SB + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * SA + 2 * SB + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_dyn + (tmem_slot - smem_u32(smem_dyn)));
-  // epilogue parameters live in shared memory (L1 is almost entirely carved out for the rings, global loads would miss)
-  float* s_bias = reinterpret_cast<float*>(smem_dyn + (bar_base + 512u - smem_u32(smem_dyn)));
-  float* s_scale = s_bias + args.cout;
-  float* s_shift = s_scale + args.cout;
-  for (int i = threadIdx.x; i < args.cout; i += blockDim.x) {
-    s_bias[i] = args.bias ? args.bias[i] : 0.f;
-    if (args.bn_scale) { s_scale[i] = args.bn_scale[i]; s_shift[i] = args.bn_shift[i]; }
-  }
+  unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
+  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  constexpr bool split = MODE == kSplitXS;
+  const int S = args.stages;
+  constexpr uint32_t kBTile = (uint32_t)BN * kBK * 2;
+  const uint32_t b_off = (uint32_t)kATile * (split ? 2u : 1u);            // stage: A_hi | A_lo | W_hi | W_lo
+  const uint32_t stage = b_off + kBTile * (split ? 2u : 1u);
+  const uint32_t ring = max(stage * (uint32_t)S, ((uint32_t)kBM * (BN + kAccPad) + 32u) * 4u);
+  const uint32_t bar_base = smem_base + ring;
+  auto full = [&](uint32_t s) { return bar_base + 8u * s; };
+  auto empty = [&](uint32_t s) { return bar_base + 8u * ((uint32_t)S + s); };
+  float* s_acc = reinterpret_cast<float*>(smem_al);                       // after the main loop of a tile: [128][BN + kAccPad]
+  float* s_bias = reinterpret_cast<float*>(smem_al + ring + 256);
+  float* s_scale = s_bias + BN;
+  float* s_shift = s_scale + BN;
 
-  int tmem_cols = 32;
-  const int XS = args.acc_split ? 2 : 1;                               // accumulators per output tile (main | cross terms)
-  const int NB = args.acc_bufs == 1 ? 1 : 2;                           // accumulator sets
-  while (tmem_cols < NB * XS * MT * BN) tmem_cols <<= 1;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_a_hi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_b_hi)) : "memory");
-    if (split) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_a_lo)) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_b_lo)) : "memory");
-    }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < SA; ++s) { mbar_init(fullA(s), 1); mbar_init(emptyA(s), 1); }
-    for (int s = 0; s < SB; ++s) { mbar_init(fullB(s), 1); mbar_init(emptyB(s), 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
+  if (tid == 0) {
+    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_b_hi);
+    if (split) { prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_lo); }
+    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }   // empty: one arrival per warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   const int KS = args.k_split > 1 ? args.k_split : 1;
   const int total_tiles = args.n_tiles_m * args.n_tiles_n * KS;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      int sa = 0, sb = 0; uint32_t pa = 0, pb = 0;
-      if (args.resident_b && (int)blockIdx.x < total_tiles) {      // every weight tile once, each on its own barrier
-        for (int i = 0; i < SB; ++i) {
-          const uint32_t db = ring_b + slot_b * i;
-          mbar_expect_tx(fullB(i), slot_b);
-          tma_load_2d(db, &tm_b_hi, i * kBK + args.b_k_offset, 0, fullB(i));
-          if (split) tma_load_2d(db + b_tile, &tm_b_lo, i * kBK + args.b_k_offset, 0, fullB(i));
-        }
-      }
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        const int tt = t / KS, ks = t - tt * KS;
-        const int m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
-        const int n0 = (tt % args.n_tiles_n) * BN;
-        const int kb0 = KS > 1 ? ks * args.kb_per : 0;
-        const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
-        for (int kh = 0; kh < args.KH; ++kh) {
-          const int row0 = m0 + args.row_shift[kh];
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(emptyA(sa), pa ^ 1u);
-            const uint32_t da = smem_base + slot_a * sa;
-            mbar_expect_tx(fullA(sa), a_box * (uint32_t)MT * (split ? 2u : 1u));
-            for (int mt = 0; mt < MT; ++mt) {                // the second box overlaps the first by slab_rows-128 identical rows
-              tma_load_2d(da + mt * kATile, &tm_a_hi, kb * kBK, row0 + mt * kBM, fullA(sa));
-              if (split) tma_load_2d(da + a_plane + mt * kATile, &tm_a_lo, kb * kBK, row0 + mt * kBM, fullA(sa));
-            }
-            if (++sa == SA) { sa = 0; pa ^= 1u; }
-            for (int kw = 0; kw < args.KW && !args.resident_b; ++kw) {
-              mbar_wait(emptyB(sb), pb ^ 1u);
-              const uint32_t db = ring_b + slot_b * sb;
-              mbar_expect_tx(fullB(sb), slot_b);
-              const int kcol = ((kh * args.KW + kw) * args.kblocks + kb) * kBK + args.b_k_offset;
-              tma_load_2d(db, &tm_b_hi, kcol, n0, fullB(sb));
-              if (split) tma_load_2d(db + b_tile, &tm_b_lo, kcol, n0, fullB(sb));
-              if (++sb == SB) { sb = 0; pb ^= 1u; }
-            }
-          }
-        }
-      }
+  uint32_t g = 0;                                                          // ring uses so far (slot = g % S, phase = g / S)
+  float acc[BN / 2], accx[split ? BN / 2 : 1];
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const int tt = t / KS, ks = t - tt * KS;
+    const int m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
+    const int n0 = (tt % args.n_tiles_n) * BN;
+    const int kb0 = KS > 1 ? ks * args.kb_per : 0;
+    const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
+    const int nkb = kb1 - kb0, nk = args.KH * args.KW * nkb;
+    for (int i = tid; i < BN; i += blockDim.x) {
+      const int col = n0 + i;
+      s_bias[i] = (args.bias && col < args.cout) ? args.bias[col] : 0.f;
+      if (args.bn_scale) { s_scale[i] = col < args.cout ? args.bn_scale[col] : 0.f; s_shift[i] = col < args.cout ? args.bn_shift[col] : 0.f; }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    int sa = 0, sb = 0; uint32_t pa = 0, pb = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
-      const int tt = t / KS, ks = t - tt * KS;
-      const int n0 = (tt % args.n_tiles_n) * BN;
-      const int kb0 = KS > 1 ? ks * args.kb_per : 0;
-      const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
-      const int acc = NB == 2 ? (it & 1) : 0;
-      const uint32_t acc_phase = (uint32_t)(NB == 2 ? (it >> 1) : it) & 1u;
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tc_fence_after();
-      int n_eff = args.cout - n0;
-      n_eff = n_eff > BN ? BN : ((n_eff + 15) & ~15);
-      const uint32_t idesc = make_idesc(n_eff);
-      const uint32_t idesc2 = make_idesc(BN + n_eff);       // fuse_b: [B_hi (BN rows, the tail zero-filled by TMA) ; B_lo (n_eff rows)]
-      const bool fuse_b = args.fuse_b != 0;
-      const uint32_t d_tmem = tmem_base + (uint32_t)(acc * XS * MT * BN);
-      const uint32_t x_cols = (uint32_t)((XS - 1) * BN);     // column offset of the cross-term accumulator
-      uint32_t accumulate = 0;
-      for (int kh = 0; kh < args.KH; ++kh) {
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(fullA(sa), pa);
-          const uint32_t a_hi = smem_base + slot_a * sa, a_lo = a_hi + a_plane;
-          const int ksteps = (kb == args.kblocks - 1) ? args.last_ksteps : 4;
-          for (int kw = 0; kw < args.KW; ++kw) {
-            int sbi = sb;
-            if (args.resident_b) { sbi = (kh * args.KW + kw) * args.kblocks + kb; if (it == 0) mbar_wait(fullB(sbi), 0); }
-            else mbar_wait(fullB(sb), pb);
-            tc_fence_after();
-            if (elect_one()) {
-              // The issuing thread is a single in-order instruction stream: for N <= 128 an MMA retires in 32-64 clocks, so the
-              // descriptor arithmetic between two issues must be a couple of integer adds.  Only the 14-bit start-address field
-              // (address >> 4) changes: +2 per k-step (32 B), +8*rows for a row-shifted tap, +1024 for the second m-tile.
-              const uint32_t bh = (ring_b + slot_b * sbi) >> 4, bl = bh + (b_tile >> 4);
-              const uint32_t ah = (a_hi + (uint32_t)(kw * args.kw_rows) * 128u) >> 4, al = ah + (a_plane >> 4);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                if (k < ksteps) {
-                  const uint64_t db = kDescHi | (uint64_t)(bh + 2 * k), dbl = kDescHi | (uint64_t)(bl + 2 * k);
-#pragma unroll
-                  for (int mt = 0; mt < 2; ++mt) {
-                    if (mt < MT) {
-                      const uint64_t da = kDescHi | (uint64_t)(ah + mt * (kATile >> 4) + 2 * k);
-                      const uint32_t d_main = d_tmem + (uint32_t)(mt * XS * BN);
-                      if (fuse_b) {
-                        tc_mma(d_main, da, db, idesc2, accumulate);          // [main | cross] (+)= A_hi * [B_hi ; B_lo]
-                        tc_mma(d_main + x_cols, kDescHi | (uint64_t)(al + mt * (kATile >> 4) + 2 * k), db, idesc, 1);
-                      } else {
-                        tc_mma(d_main, da, db, idesc, accumulate);
-                        if (split) {
-                          tc_mma(d_main + x_cols, da, dbl, idesc, XS == 2 ? accumulate : 1u);
-                          tc_mma(d_main + x_cols, kDescHi | (uint64_t)(al + mt * (kATile >> 4) + 2 * k), db, idesc, 1);
-                        }
-                      }
-                    }
-                  }
-                  accumulate = 1;
-                }
-              }
-              if (!args.resident_b) tc_commit(emptyB(sb));   // weight slot is free once these MMAs retire
-              if (kw == args.KW - 1) tc_commit(emptyA(sa));  // ... and the slab after its last tap
-            }
-            __syncwarp();
-            if (!args.resident_b && ++sb == SB) { sb = 0; pb ^= 1u; }
-          }
-          if (++sa == SA) { sa = 0; pa ^= 1u; }
-        }
+    // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +128) of the activation matrix
+    auto issue = [&](int i) {
+      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
+      mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
+      const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
+      const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
+      const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
+      const uint32_t dst = smem_base + stage * s;
+      mbar_expect_tx(full(s), stage);
+      tma_load_2d(dst, &tm_a_hi, kb * kBK, row, full(s));
+      tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, full(s));
+      if (split) {
+        tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, full(s));
+        tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, full(s));
       }
-      if (elect_one()) tc_commit(tfull_bar(acc));
+    };
+    // k-iteration j's MMAs are done: its stage goes back to the producer, which refills it with k-iteration j + S
+    auto release = [&](int j) {
       __syncwarp();
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int q = warp - 4;                                // TMEM lane quarter of this warp (== warp % 4)
-    int it = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++it) {
-      const int tt = t / KS;
-      const int m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
-      const int n0 = (tt % args.n_tiles_n) * BN;
-      const int acc = NB == 2 ? (it & 1) : 0;
-      const uint32_t acc_phase = (uint32_t)(NB == 2 ? (it >> 1) : it) & 1u;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      for (int mt = 0; mt < MT; ++mt) {
-      const int v = m0 + mt * kBM + q * 32 + lane;         // virtual row of this thread
-      bool valid = v < args.M_total;
-      int n = 0, y = 0, x = 0;
-      if (valid) {
-        n = v / args.rows_per_img;
-        const int r = v - n * args.rows_per_img;
-        y = r / args.in_Wp;
-        x = r - y * args.in_Wp;
-        valid = (y < args.Ho) && (x < args.Wo);
-      }
-      int ncols = args.cout - n0;
-      ncols = ncols > BN ? BN : ncols;
-      const uint32_t t_row = tmem_base + (uint32_t)((acc * MT + mt) * XS * BN) + ((uint32_t)(q * 32) << 16);
-      const uint32_t xoff = (uint32_t)((XS - 1) * BN);
-      if (args.epi == EPI_SPLIT) {
-        const size_t o = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + n0;
-        if (args.mask_hi || args.accumulate) epi_split<true>(args, t_row, xoff, ncols, n0, o, valid, s_bias, s_scale, s_shift);
-        else epi_split<false, true>(args, t_row, xoff, ncols, n0, o, valid, s_bias, s_scale, s_shift);
-      } else if (args.epi == EPI_ATOMIC) {
-        float* dstp = args.out_f32 + (size_t)v * args.out_ld + args.out_col_off + n0;
-        for (int c0 = 0; c0 < ncols; c0 += 32) {
-          uint32_t vr[32];
-          ld_acc32(t_row + (uint32_t)c0, xoff, vr);
-          if (valid) {
+      if (lane == 0) mbar_arrive(empty((g + (uint32_t)j) % (uint32_t)S));
+      if (tid == 0 && j + S < nk) issue(j + S);
+    };
+    if (tid == 0)
+      for (int i = 0; i < min(S, nk); ++i) issue(i);
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(accx);
+    // Every k-iteration issues all 4 k-steps of its 64-channel block: past the last real channel the A tile is TMA zero fill (or
+    // the zeros of a padded operand), so the loop body has no data-dependent branch around the wgmma.  One group stays in flight:
+    // the MMAs of iteration i are issued before the stage of iteration i-1 is released.
+    for (int i = 0; i < nk; ++i) {
+      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
+      mbar_wait(full(s), (gi / (uint32_t)S) & 1u);
+      const uint32_t a_hi = smem_base + stage * s + (uint32_t)wg * (kATile / 2), b_hi = smem_base + stage * s + b_off;
+      constexpr uint64_t kDesc = wgmma_desc_hi(16);
+      wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + j < ncols) atomicAdd(dstp + c0 + j, __uint_as_float(vr[j]));
-          }
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t sc = (i | k) ? 1u : 0u;
+        const uint64_t da = wgmma_desc(kDesc, a_hi + 32u * k), db = wgmma_desc(kDesc, b_hi + 32u * k);
+        Wgmma<BN, 0, 0>::mma(acc, da, db, sc);
+        if constexpr (split) {
+          Wgmma<BN, 0, 0>::mma(accx, da, wgmma_desc(kDesc, b_hi + kBTile + 32u * k), sc);
+          Wgmma<BN, 0, 0>::mma(accx, wgmma_desc(kDesc, a_hi + kATile + 32u * k), db, 1u);
         }
-      } else if (args.epi == EPI_HEAD) {
-        // one thread = one pixel = n_boxes prior rows.  Per box three sweeps over its C+4 accumulator columns (TMEM reads are cheap
-        // and this warp group runs under the MMAs of the next tile): maximum, sum of exponentials, normalised store.
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (i > 0) release(i - 1);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(accx);
+    if (nk > 0) release(nk - 1);
+    g += (uint32_t)nk;
+    if constexpr (split) {
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) acc[j] += accx[j];
+    }
+
+    // ===================== epilogue: registers -> shared-memory tile -> one thread per row (and half of the columns) =====
+    __syncthreads();                                                       // both warpgroups are done with the ring
+    store_acc_tile<BN>(acc, s_acc, wg, warp, lane);
+    __syncthreads();
+    const int r = tid & (kBM - 1), half = tid >> 7;
+    const int v = m0 + r;                                                  // virtual row of this thread
+    bool valid = v < args.M_total;
+    int n = 0, y = 0, x = 0;
+    if (valid) {
+      n = v / args.rows_per_img;
+      const int rr = v - n * args.rows_per_img;
+      y = rr / args.in_Wp;
+      x = rr - y * args.in_Wp;
+      valid = (y < args.Ho) && (x < args.Wo);
+    }
+    const float* arow = s_acc + (size_t)r * (BN + kAccPad);
+    const int ncols = min(BN, args.cout - n0);
+    const int h0 = half * (BN / 2), nh = min(BN / 2, ncols - h0);       // this thread's columns: [h0, h0 + nh)
+    if (valid && args.epi == EPI_HEAD) {
+      if (half == 0) {
         const int C = args.head_C, CP4 = C + 4, RW = C + 12;
         const int pix = y * args.Wo + x;
-        if (CP4 == 25 && args.head_nb <= 8) { epi_head_fixed<25>(args, t_row, xoff, valid, n, pix, s_bias); continue; }
-        for (int bx = 0; bx < args.head_nb; ++bx) {
-          const int c_lo = bx * CP4, c_hi = c_lo + CP4;
-          const int k_lo = c_lo >> 5, k_hi = (c_hi - 1) >> 5;
-          float mx = -INFINITY;
-          for (int k = k_lo; k <= k_hi; ++k) {
-            uint32_t vr[32];
-            ld_acc32(t_row + (uint32_t)(k * 32), xoff, vr);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int col = k * 32 + j;
-              if (col >= c_lo && col < c_lo + C) mx = fmaxf(mx, __uint_as_float(vr[j]) + s_bias[col]);
+        if (CP4 == 25 && args.head_nb <= 8) {
+          epi_head_fixed<25>(args, arow, n, pix, s_bias);
+        } else {
+          for (int bx = 0; bx < args.head_nb; ++bx) {
+            const int c_lo = bx * CP4;
+            float mx = -INFINITY;
+            for (int c = c_lo; c < c_lo + C; ++c) mx = fmaxf(mx, arow[c] + s_bias[c]);
+            float sum = 0.f;
+            for (int c = c_lo; c < c_lo + C; ++c) sum += expf(arow[c] + s_bias[c] - mx);
+            const int prior = args.head_prior_off + pix * args.head_nb + bx;
+            float* dst = args.out_f32 + ((size_t)n * args.head_P + prior) * RW;
+            for (int rc = 0; rc < CP4; ++rc) {
+              const float val = arow[c_lo + rc] + s_bias[c_lo + rc];
+              dst[rc] = rc < C ? expf(val - mx) / sum : val;
             }
-          }
-          float sum = 0.f;
-          for (int k = k_lo; k <= k_hi; ++k) {
-            uint32_t vr[32];
-            ld_acc32(t_row + (uint32_t)(k * 32), xoff, vr);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int col = k * 32 + j;
-              if (col >= c_lo && col < c_lo + C) sum += expf(__uint_as_float(vr[j]) + s_bias[col] - mx);
-            }
-          }
-          const int prior = args.head_prior_off + pix * args.head_nb + bx;
-          float* dst = args.out_f32 + ((size_t)n * args.head_P + prior) * RW;
-          for (int k = k_lo; k <= k_hi; ++k) {
-            uint32_t vr[32];
-            ld_acc32(t_row + (uint32_t)(k * 32), xoff, vr);
-            if (valid) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int col = k * 32 + j;
-                if (col >= c_lo && col < c_hi) {
-                  const float v = __uint_as_float(vr[j]) + s_bias[col];
-                  const int r = col - c_lo;
-                  dst[r] = r < C ? expf(v - mx) / sum : v;
-                }
-              }
-            }
-          }
-          if (valid) {
             const float4 an = __ldg(reinterpret_cast<const float4*>(args.head_anchors) + prior);
             dst[C + 4] = an.x; dst[C + 5] = an.y; dst[C + 6] = an.z; dst[C + 7] = an.w;
             dst[C + 8] = args.head_var[0]; dst[C + 9] = args.head_var[1]; dst[C + 10] = args.head_var[2]; dst[C + 11] = args.head_var[3];
           }
         }
-      } else {
-        const size_t o = (((size_t)n * args.Ho + y) * args.Wo + x) * (size_t)args.cout + n0;
-        for (int c0 = 0; c0 < ncols; c0 += 32) {
-          uint32_t vr[32];
-          ld_acc32(t_row + (uint32_t)c0, xoff, vr);
-          if (valid) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (c0 + j < ncols) {
-                const int col = n0 + c0 + j;
-                float xv = __uint_as_float(vr[j]) + s_bias[col];
-                args.out_f32[o + c0 + j] = apply_act(xv, args.act);
-              }
-            }
-          }
-        }
       }
-      }   // mt
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
+    } else if (valid && nh > 0) {
+      if (args.epi == EPI_SPLIT) {
+        const size_t o = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + n0 + h0;
+        if (args.mask_hi || args.accumulate) epi_split<true>(args, arow + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
+        else epi_split<false>(args, arow + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
+      } else if (args.epi == EPI_ATOMIC) {
+        float* dstp = args.out_f32 + (size_t)v * args.out_ld + args.out_col_off + n0 + h0;
+        for (int j = 0; j < nh; ++j) atomicAdd(dstp + j, arow[h0 + j]);
+      } else {
+        const size_t o = (((size_t)n * args.Ho + y) * args.Wo + x) * (size_t)args.cout + n0 + h0;
+        for (int j = 0; j < nh; ++j) args.out_f32[o + j] = apply_act(arow[h0 + j] + s_bias[h0 + j], args.act);
+      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+    fence_proxy_async();                                                   // the next tile's TMA writes over s_acc
+    __syncthreads();
   }
 }
 
-int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int grid_cap) {
+template <int BN, int MODE>
+static int launch_conv_bn(const ConvLaunch& L, int grid, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_tcgen05_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
+  conv_wgmma_kernel<BN, MODE><<<grid, 256, L.smem, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
+  return SSDK_OK;
+}
+
+int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int grid_cap) {
   // the kernel is persistent with a static stride over its work units: any grid size computes the same result
   const int grid = grid_cap > 0 ? std::max(1, std::min(L.grid, grid_cap)) : L.grid;
-  conv_tcgen05_kernel<<<grid, 256, L.smem, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
+  const bool split = L.args.split != 0;
+  SSDK_REQUIRE(!split || L.args.acc_split, "internal: bf16x3 conv plans carry the cross-term accumulator");
+  SSDK_REQUIRE(split || L.args.BN != 160, "internal: 160-wide conv tiles are for bf16x3 predictor heads");
+  int rc;
+  switch (L.args.BN) {
+    case 64: rc = split ? launch_conv_bn<64, kSplitXS>(L, grid, stream) : launch_conv_bn<64, kSingle>(L, grid, stream); break;
+    case 128: rc = split ? launch_conv_bn<128, kSplitXS>(L, grid, stream) : launch_conv_bn<128, kSingle>(L, grid, stream); break;
+    case 160: rc = launch_conv_bn<160, kSplitXS>(L, grid, stream); break;
+    case 256:
+      SSDK_REQUIRE(!split, "internal: 256-wide conv tiles have no cross-term accumulator");
+      rc = launch_conv_bn<256, kSingle>(L, grid, stream);
+      break;
+    default: set_error("internal: conv tile width %d", L.args.BN); return SSDK_ERR_INVALID;
+  }
+  if (rc) return rc;
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
@@ -882,7 +700,6 @@ int launch_conv_direct(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const
   }
   const size_t total = (size_t)out.B * out.H * ((out.W + kDirectPx - 1) / kDirectPx) * (out.C / 16);
   const unsigned blocks = (unsigned)((total + 255) / 256);
-  // (a fully unrolled <3, 3> instantiation was measured slower on B200: 771 vs 683 us for conv1_1 at batch 32)
   conv_direct_kernel<0, 0><<<blocks, 256, smem, stream>>>(in, out, w, bias, bn_scale, bn_shift, act, kh, kw, dil, pad_t, pad_l);
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());
@@ -892,14 +709,12 @@ int launch_conv_direct(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const
 // ------------------------------------------------------------------------------------------------
 // conv_first_kernel: the image-facing layer (Cin <= 4: conv1_1 3x3x3 of models/keras_ssd300.py:263, conv1 5x5x3 of
 // models/keras_ssd7.py:277) on the tensor cores.  K = taps * 4 (channels padded to 4) is far too thin for the TMA ring of
-// conv_tcgen05_kernel -- an explicit im2col would write and re-read ten times the layer's input -- so the A tile is GATHERED:
-//   warps  0- 7  epilogue, two groups of four (TMEM lane quarter = warp % 4), group g drains accumulator g
-//   warps  8-15  gather, two groups of 128 threads; thread = one output pixel: reads the taps' 8-byte (4-channel) hi / lo words
-//                from the zero-bordered input planes (L1/L2 hits: every word is used by taps of neighbouring pixels) and writes
-//                them K-major into the 128B-swizzled A stage; group g fills the stages of tiles g, g+2, ...
-//   warp   16    TMEM allocation, tcgen05.mma issue (<= 8 k-steps x 3 products per tile), commits
-// The weights (K-major, swizzled image prepared on the host) stay in shared memory for the whole launch.  The layer is bound by
-// writing its output (B*H*W*Cout*4 bytes of hi+lo planes); the epilogue is the one of the other activation-producing launches.
+// conv_wgmma_kernel -- an explicit im2col would write and re-read ten times the layer's input -- so the A tile is GATHERED.
+// Per 128-pixel tile: 256 threads gather (thread = one output pixel and one plane: the taps' 8-byte (4-channel) hi or lo words
+// from the zero-bordered input planes, L1/L2 hits since every word is used by taps of neighbouring pixels) into the K-major
+// 128B-swizzled A tile; two warpgroups issue wgmma on 64 rows each; the accumulators go through shared memory to the epilogue
+// of the other activation-producing launches.  The weights (K-major, swizzled image prepared on the host) stay in shared memory
+// for the whole launch.  The layer is bound by writing its output (B*H*W*Cout*4 bytes of hi+lo planes).
 // ------------------------------------------------------------------------------------------------
 struct FirstArgs {
   ActBuf in;
@@ -907,169 +722,115 @@ struct FirstArgs {
   int KH, KW, dil, pad_t, pad_l;
   int tap_off[32];            // element offset of tap t's 4-channel word relative to the output pixel's own word in the input planes
                               // (the planes' zero border covers every tap: checked on the host)
-  int kblocks, ksteps;        // 64-wide blocks / 16-wide MMA steps that cover taps * 4
-  int BN, stages, split;
+  int kblocks;                // 64-wide blocks that cover taps * 4 (1 or 2; a template parameter of the kernel, as is split)
+  int split;
   long long M;                // B * Ho * Wo output pixels
   int n_tiles, Ho, Wo;
   ConvArgs epi;               // bias / bn / act / output planes as the shared epilogue expects them
 };
-constexpr int kFirstThreads = 17 * 32;
 
-__global__ void __launch_bounds__(kFirstThreads, 1) conv_first_kernel(const __grid_constant__ FirstArgs fa) {
+int first_bn(int cout) { return cout <= 64 ? 64 : 128; }
+static size_t first_smem_bytes(int kblocks, int BN, int split) {
+  return 1024 + ((size_t)kblocks * kATile + (size_t)kblocks * BN * 128) * (split ? 2 : 1) + acc_tile_bytes(BN) + (size_t)3 * BN * sizeof(float);
+}
+
+template <int BN, int KB, bool SPLIT>
+__global__ void __launch_bounds__(256, 1) conv_first_kernel(const __grid_constant__ FirstArgs fa) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int SA = fa.stages, BN = fa.BN, split = fa.split, KB = fa.kblocks;
-  const uint32_t a_plane = (uint32_t)KB * kATile;                      // one stage plane (hi or lo)
-  const uint32_t a_stage = a_plane * (split ? 2 : 1);
+  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  constexpr bool split = SPLIT;
+  const uint32_t a_plane = (uint32_t)KB * kATile;                      // A tile: hi plane | lo plane
   const uint32_t b_block = (uint32_t)BN * 128u;                        // one k-block of the weight tile
   const uint32_t b_plane = b_block * KB;
-  const uint32_t ring_b = smem_base + a_stage * SA;
-  const uint32_t bar_base = ring_b + b_plane * (split ? 2 : 1);
-  auto fullA = [&](int i) { return bar_base + 8u * i; };
-  auto emptyA = [&](int i) { return bar_base + 8u * (SA + i); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * SA + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * SA + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * SA + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_al + (tmem_slot - smem_base));
-  float* s_bias = reinterpret_cast<float*>(smem_al + (bar_base + 256u - smem_base));
-  float* s_scale = s_bias + fa.epi.cout;
-  float* s_shift = s_scale + fa.epi.cout;
-  for (int i = threadIdx.x; i < fa.epi.cout; i += blockDim.x) {
-    s_bias[i] = fa.epi.bias ? fa.epi.bias[i] : 0.f;
-    if (fa.epi.bn_scale) { s_scale[i] = fa.epi.bn_scale[i]; s_shift[i] = fa.epi.bn_shift[i]; }
+  const uint32_t a_base = smem_base, b_base = a_base + a_plane * (split ? 2 : 1);
+  float* s_acc = reinterpret_cast<float*>(smem_al + (b_base + b_plane * (split ? 2 : 1) - smem_base));
+  float* s_bias = s_acc + (size_t)kBM * (BN + kAccPad) + 32;
+  float* s_scale = s_bias + BN;
+  float* s_shift = s_scale + BN;
+  for (int i = tid; i < BN; i += blockDim.x) {
+    const bool in = i < fa.epi.cout;
+    s_bias[i] = (in && fa.epi.bias) ? fa.epi.bias[i] : 0.f;
+    if (fa.epi.bn_scale) { s_scale[i] = in ? fa.epi.bn_scale[i] : 0.f; s_shift[i] = in ? fa.epi.bn_shift[i] : 0.f; }
   }
   {   // resident weights: straight copy of the swizzled images
     const uint4* src_h = reinterpret_cast<const uint4*>(fa.w_hi);
     const uint4* src_l = reinterpret_cast<const uint4*>(fa.w_lo);
-    uint4* dst = reinterpret_cast<uint4*>(smem_al + (ring_b - smem_base));
+    uint4* dst = reinterpret_cast<uint4*>(smem_al + (b_base - smem_base));
     const int n16 = (int)(b_plane >> 4);
-    for (int i = threadIdx.x; i < n16; i += blockDim.x) { dst[i] = src_h[i]; if (split) dst[n16 + i] = src_l[i]; }
+    for (int i = tid; i < n16; i += blockDim.x) { dst[i] = src_h[i]; if (split) dst[n16 + i] = src_l[i]; }
   }
-  int tmem_cols = 32;
-  while (tmem_cols < 2 * BN) tmem_cols <<= 1;
-  if (warp == 16) {
-    if (lane == 0) {
-      for (int i = 0; i < SA; ++i) { mbar_init(fullA(i), 128); mbar_init(emptyA(i), 1); }
-      for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // the weight copy above is read by the MMA (async proxy)
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   const int taps = fa.KH * fa.KW;
-
-  if (warp == 16) {
-    // ===================== MMA issuer =====================
-    const uint32_t idesc = make_idesc(BN);
-    int it = 0;
-    for (int t = blockIdx.x; t < fa.n_tiles; t += gridDim.x, ++it) {
-      const int st = it % SA;
-      const int acc = it & 1;
-      mbar_wait(fullA(st), (uint32_t)(it / SA) & 1u);
-      mbar_wait(tempty_bar(acc), ((uint32_t)(it >> 1) & 1u) ^ 1u);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + (uint32_t)(acc * BN);
-        const uint32_t a0 = smem_base + a_stage * st;
-        for (int ks = 0; ks < fa.ksteps; ++ks) {
-          const int kb = ks >> 2, k = ks & 3;
-          const uint32_t ah = (a0 + (uint32_t)kb * kATile) >> 4, bh = (ring_b + (uint32_t)kb * b_block) >> 4;
-          const uint64_t da = kDescHi | (uint64_t)(ah + 2 * k), db = kDescHi | (uint64_t)(bh + 2 * k);
-          tc_mma(d, da, db, idesc, ks ? 1u : 0u);
-          if (split) {
-            tc_mma(d, da, kDescHi | (uint64_t)(bh + (b_plane >> 4) + 2 * k), idesc, 1u);
-            tc_mma(d, kDescHi | (uint64_t)(ah + (a_plane >> 4) + 2 * k), db, idesc, 1u);
-          }
-        }
-        tc_commit(emptyA(st));
-        tc_commit(tfull_bar(acc));
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 8) {
+  constexpr int slots = KB * 16;                                       // 8-byte (4-channel) K slots; slots >= taps hold zeros
+  const int r = tid & (kBM - 1), plane = tid >> 7;                     // gather / epilogue row; gather plane (0 hi, 1 lo)
+  const __nv_bfloat16* src_plane = plane ? fa.in.lo : fa.in.hi;
+  unsigned char* a_dst = smem_al + (a_base - smem_base) + plane * a_plane;
+  float acc[BN / 2];
+  for (int t = blockIdx.x; t < fa.n_tiles; t += gridDim.x) {
     // ===================== gather =====================
-    const int grp = (warp - 8) >> 2;
-    const int r = ((warp - 8) & 3) * 32 + lane;                        // row of the tile
-    const int slots = fa.ksteps * 4;                                   // 8-byte (4-channel) K slots; slots >= taps hold zeros
-    int it = 0;
-    for (int t = blockIdx.x; t < fa.n_tiles; t += gridDim.x, ++it) {
-      if ((it & 1) != grp) continue;
-      const int st = it % SA;
-      const long long v = (long long)t * kBM + r;
-      const bool valid = v < fa.M;
-      int n = 0, y = 0, x = 0;
-      if (valid) {
-        n = (int)(v / ((long long)fa.Ho * fa.Wo));
-        const int rem = (int)(v - (long long)n * fa.Ho * fa.Wo);
-        y = rem / fa.Wo; x = rem - y * fa.Wo;
-      }
+    const long long v = (long long)t * kBM + r;
+    const bool valid = v < fa.M;
+    int n = 0, y = 0, x = 0;
+    if (valid) {
+      n = (int)(v / ((long long)fa.Ho * fa.Wo));
+      const int rem = (int)(v - (long long)n * fa.Ho * fa.Wo);
+      y = rem / fa.Wo; x = rem - y * fa.Wo;
+    }
+    if (plane == 0 || split) {
       const size_t src0 = valid ? act_index(fa.in, n, y, x) : 0;
       // all loads of a round are issued before the first store (twelve taps = the whole 3x3 kernel in one round trip)
       constexpr int kRound = 12;
-      uint2 h[kRound], l[kRound];
+      uint2 w[kRound];
       for (int s0 = 0; s0 < slots; s0 += kRound) {
 #pragma unroll
         for (int j = 0; j < kRound; ++j) {
           const int tap = s0 + j;
-          h[j] = make_uint2(0, 0); l[j] = make_uint2(0, 0);
-          if (valid && tap < taps) {
-            const long long src = (long long)src0 + fa.tap_off[tap];
-            h[j] = __ldg(reinterpret_cast<const uint2*>(fa.in.hi + src));
-            if (split) l[j] = __ldg(reinterpret_cast<const uint2*>(fa.in.lo + src));
-          }
+          w[j] = make_uint2(0, 0);
+          if (valid && tap < taps) w[j] = __ldg(reinterpret_cast<const uint2*>(src_plane + (long long)src0 + fa.tap_off[tap]));
         }
-        if (s0 == 0) mbar_wait(emptyA(st), ((uint32_t)(it / SA) & 1u) ^ 1u);   // (the loads above do not touch the stage)
-        unsigned char* stage = smem_al + (a_stage * st);
 #pragma unroll
         for (int j = 0; j < kRound; ++j) {
           const int tap = s0 + j;
           if (tap < slots) {
             const uint32_t off = (uint32_t)(tap >> 4) * kATile + (uint32_t)r * 128u + ((uint32_t)(((tap >> 1) & 7) ^ (r & 7)) << 4) + (uint32_t)(tap & 1) * 8u;
-            *reinterpret_cast<uint2*>(stage + off) = h[j];
-            if (split) *reinterpret_cast<uint2*>(stage + a_plane + off) = l[j];
+            *reinterpret_cast<uint2*>(a_dst + off) = w[j];
           }
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> visible to the MMA's async proxy
-      mbar_arrive(fullA(st));
     }
-  } else {
-    // ===================== epilogue =====================
-    const int grp = warp >> 2, q = warp & 3;
-    int it = 0;
-    for (int t = blockIdx.x; t < fa.n_tiles; t += gridDim.x, ++it) {
-      if ((it & 1) != grp) continue;
-      const int acc = it & 1;
-      mbar_wait(tfull_bar(acc), (uint32_t)(it >> 1) & 1u);
-      tc_fence_after();
-      const long long v = (long long)t * kBM + q * 32 + lane;
-      const bool valid = v < fa.M;
-      size_t o = 0;
-      if (valid) {
-        const int n = (int)(v / ((long long)fa.Ho * fa.Wo));
-        const int rem = (int)(v - (long long)n * fa.Ho * fa.Wo);
-        const int y = rem / fa.Wo, x = rem - y * fa.Wo;
-        o = (((size_t)n * fa.epi.out_Hp + (y + fa.epi.out_pad)) * fa.epi.out_Wp + (x + fa.epi.out_pad)) * fa.epi.out_Cs;
+    fence_proxy_async();                                               // generic-proxy stores -> visible to wgmma (async proxy)
+    __syncthreads();
+    // ===================== MMA: warpgroup wg computes rows [64 wg, +64) =====================
+    {
+      constexpr uint64_t kDesc = wgmma_desc_hi(16);
+      wgmma_fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < KB * 4; ++ks) {                             // every k-step of the k-blocks: uniform issue
+        const int kb = ks >> 2, k = ks & 3;
+        const uint32_t ah = a_base + (uint32_t)kb * kATile + (uint32_t)wg * (kATile / 2) + 32u * k;
+        const uint32_t bh = b_base + (uint32_t)kb * b_block + 32u * k;
+        const uint64_t da = wgmma_desc(kDesc, ah), db = wgmma_desc(kDesc, bh);
+        Wgmma<BN, 0, 0>::mma(acc, da, db, ks ? 1u : 0u);
+        if constexpr (split) {
+          Wgmma<BN, 0, 0>::mma(acc, da, wgmma_desc(kDesc, bh + b_plane), 1u);
+          Wgmma<BN, 0, 0>::mma(acc, wgmma_desc(kDesc, ah + a_plane), db, 1u);
+        }
       }
-      const uint32_t t_row = tmem_base + (uint32_t)(acc * BN) + ((uint32_t)(q * 32) << 16);
-      epi_split<false>(fa.epi, t_row, 0u, fa.epi.cout, 0, o, valid, s_bias, s_scale, s_shift);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 16) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+    store_acc_tile<BN>(acc, s_acc, wg, warp, lane);
+    __syncthreads();
+    // ===================== epilogue: thread = (row, half of the columns) =====================
+    const int h0 = plane * (BN / 2), nh = min(BN / 2, fa.epi.cout - h0);
+    if (valid && nh > 0) {
+      const size_t o = (((size_t)n * fa.epi.out_Hp + (y + fa.epi.out_pad)) * fa.epi.out_Wp + (x + fa.epi.out_pad)) * fa.epi.out_Cs + h0;
+      epi_split<false>(fa.epi, s_acc + (size_t)r * (BN + kAccPad) + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
+    }
+    __syncthreads();                                                   // the A tile and s_acc are rewritten by the next tile
   }
 }
 
@@ -1096,6 +857,22 @@ bool first_border_ok(const ActBuf& in, int kh, int kw, int dil, int pad_t, int p
 }
 int first_tc_supported(int taps, int cin, int cout) { return cin <= 4 && taps * 4 <= 128 && cout % 8 == 0 && cout <= 128; }
 
+template <int BN, int KB, bool SPLIT>
+static int launch_first_bn(const FirstArgs& fa, int grid, size_t smem, cudaStream_t stream) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_first_kernel<BN, KB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  conv_first_kernel<BN, KB, SPLIT><<<grid, 256, smem, stream>>>(fa);
+  return SSDK_OK;
+}
+template <int BN>
+static int launch_first_kb(const FirstArgs& fa, int grid, size_t smem, cudaStream_t stream) {
+  if (fa.kblocks == 1) return fa.split ? launch_first_bn<BN, 1, true>(fa, grid, smem, stream) : launch_first_bn<BN, 1, false>(fa, grid, smem, stream);
+  return fa.split ? launch_first_bn<BN, 2, true>(fa, grid, smem, stream) : launch_first_bn<BN, 2, false>(fa, grid, smem, stream);
+}
+
 int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
                       const float* bias, const float* bn_scale, const float* bn_shift, int act, int kh, int kw, int dil, int pad_t,
                       int pad_l, cudaStream_t stream) {
@@ -1109,26 +886,19 @@ int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const 
     fa.tap_off[t] = (dy * in.Wp() + dx) * in.Cs;
   }
   const int K = kh * kw * 4;
-  fa.ksteps = (K + 15) / 16; fa.kblocks = (K + 63) / 64;
-  fa.BN = (out.C + 15) / 16 * 16;
+  fa.kblocks = (K + 63) / 64;
+  SSDK_REQUIRE(fa.kblocks <= 2, "image-facing convolution: more than 128 K columns");
+  const int BN = first_bn(out.C);
   fa.split = (in.lo && w_lo) ? 1 : 0;
   fa.M = (long long)out.B * out.H * out.W; fa.Ho = out.H; fa.Wo = out.W;
   fa.n_tiles = (int)((fa.M + kBM - 1) / kBM);
-  const size_t a_stage = (size_t)fa.kblocks * kATile * (fa.split ? 2 : 1);
-  const size_t b_bytes = (size_t)fa.kblocks * fa.BN * 128 * (fa.split ? 2 : 1);
-  const size_t fixed = 1024 + b_bytes + 256 + ((size_t)out.C * 3 * sizeof(float) + 127) / 128 * 128 + 128;
-  fa.stages = (int)std::min<size_t>(4, (200 * 1024 - fixed) / a_stage);
-  SSDK_REQUIRE(fa.stages >= 2, "image-facing convolution: the gathered A tile does not fit in shared memory twice");
   fa.epi.cout = out.C; fa.epi.bias = bias; fa.epi.bn_scale = bn_scale; fa.epi.bn_shift = bn_shift; fa.epi.act = act;
   fa.epi.out_hi = out.hi; fa.epi.out_lo = out.lo; fa.epi.out_Hp = out.Hp(); fa.epi.out_Wp = out.Wp(); fa.epi.out_pad = out.pad; fa.epi.out_Cs = out.Cs;
-  const size_t smem = fixed + a_stage * fa.stages;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_first_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
+  const size_t smem = first_smem_bytes(fa.kblocks, BN, fa.split);
+  SSDK_REQUIRE(smem <= 227 * 1024, "image-facing convolution: %zu bytes of shared memory", smem);
   const int grid = std::min(fa.n_tiles, ctx->sm_count);
-  conv_first_kernel<<<grid, kFirstThreads, smem, stream>>>(fa);
+  const int rc = BN == 64 ? launch_first_kb<64>(fa, grid, smem, stream) : launch_first_kb<128>(fa, grid, smem, stream);
+  if (rc) return rc;
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

@@ -10,7 +10,7 @@ namespace ssdk {
 
 // An activation tensor: NHWC, channel-padded to a multiple of 8, spatially padded with a zero border
 // of `pad` pixels, stored as TWO bf16 planes: value = hi + lo (lo is absent in single-pass bf16 mode).
-// hi + lo carries 16 significant bits, which keeps the tcgen05 path within ~1e-5 of an fp32 conv.
+// hi + lo carries 16 significant bits, which keeps the tensor-core path within ~1e-5 of an fp32 conv.
 struct ActBuf {
   __nv_bfloat16* hi = nullptr;
   __nv_bfloat16* lo = nullptr;
@@ -38,25 +38,17 @@ struct ConvArgs {
   int rows_per_img;     // rows of the virtual grid per image
   int in_Wp;            // virtual row pitch
   int Ho, Wo, B;        // valid extent: virtual (y, x) is a real output iff y < Ho && x < Wo
-  int KH, KW, kblocks;  // K loop = KH * kblocks A-slabs, each feeding KW weight tiles (taps (kh, 0..KW-1))
-  int last_ksteps;      // UMMA k-steps (of 16) in the last k-block of every tap (1..4)
+  int KH, KW, kblocks;  // K loop = KH * KW taps x kblocks channel blocks of 64
   int row_shift[8];     // row offset of tap (kh, kw=0)
-  int kw_rows;          // rows between consecutive kw taps (= dilation); tap kw reads slab rows [kw*kw_rows, +128)
-  int slab_rows;        // rows per A slab = round_up8(128 + (KW-1)*kw_rows) <= 256
-  int stages_a, stages_b;
-  int acc_split;        // 1: the two cross terms (hi*lo, lo*hi) accumulate in their own TMEM columns and are added in the epilogue
-  int fuse_b;           // 1 (needs acc_split): A_hi * [B_hi ; B_lo] as ONE MMA of N = BN + n into [main | cross], then A_lo * B_hi into cross
-  int acc_bufs;         // accumulator sets in TMEM (2: the epilogue of tile i overlaps the MMAs of tile i+1; 1 when columns run out)
-  int resident_b;       // 1: all KH*KW*kblocks weight tiles of the (single) n-tile stay in shared memory for the whole launch
-  int mt;               // m-tiles per work unit (1 or 2): with 2, every weight tile feeds two 128-row MMAs (halves the weight traffic)
-  int bo_mode;          // how the UMMA descriptor's base-offset field is filled for row-shifted A tiles (debug knob)
-  int epi_pipe;         // forward epilogue: 2 = TMEM loads of the next 32 columns issued before the current ones are converted / stored, 1 / 0 = experiment knobs
+  int kw_rows;          // rows between consecutive kw taps (= dilation)
+  int stages;           // TMA ring depth
   int n_tiles_m;        // number of entries in tile_list
   int n_tiles_n;
   const int* tile_list; // m-tile indices that contain at least one valid row
-  int BN;               // accumulator tile width (64/128/256); TMA box rows of the weight tile
+  int BN;               // accumulator tile width (64/128/160/256: the wgmma N); TMA box rows of the weight tile
   int cout;
   int split;            // 1: bf16x3 (hi*hi + hi*lo + lo*hi), 0: single bf16 pass
+  int acc_split;        // 1 (always with split): the cross terms accumulate apart from hi*hi and are added after the K loop
   // epilogue
   int epi;
   const float* bias; const float* bn_scale; const float* bn_shift;
@@ -105,6 +97,7 @@ int launch_conv_direct(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const
                        const float* bn_shift, int act, int kh, int kw, int dil, int pad_t, int pad_l, cudaStream_t stream);
 // image-facing layer on the tensor cores (gathered A tile, weights resident in shared memory as a swizzled image)
 int first_tc_supported(int taps, int cin, int cout);
+int first_bn(int cout);     // weight-image rows (wgmma N) of the image-facing layer
 bool first_border_ok(const ActBuf& in, int kh, int kw, int dil, int pad_t, int pad_l);
 void first_weight_image(const float* hwio, int taps, int cin, int cout, int BN, int kblocks, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
 int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,

@@ -1,4 +1,4 @@
-// Decode path on sm_100a: offset decode, confidence threshold, greedy IoU-NMS and top-k.
+// Decode path on sm_90a: offset decode, confidence threshold, greedy IoU-NMS and top-k.
 // Reference: keras_layers/keras_layer_DecodeDetections.py:109-265, keras_layer_DecodeDetectionsFast.py:111-248,
 // ssd_encoder_decoder/ssd_output_decoder.py:77-333.
 //

@@ -1,4 +1,4 @@
-// SSDInputEncoder hot path on sm_100a: pairwise IoU, greedy bipartite + multi matching, neutral boxes and offset
+// SSDInputEncoder hot path on sm_90a: pairwise IoU, greedy bipartite + multi matching, neutral boxes and offset
 // encoding.  Reference: ssd_encoder_decoder/ssd_input_encoder.py:277-418,
 // bounding_box_utils/bounding_box_utils.py:283-383, ssd_encoder_decoder/matching_utils.py:22-116.
 //

@@ -1,4 +1,4 @@
-// SSDLoss on sm_100a as ONE kernel (forward, backward, or both).  Reference: keras_loss_function/keras_ssd_loss.py:53-211.
+// SSDLoss on sm_90a as ONE kernel (forward, backward, or both).  Reference: keras_loss_function/keras_ssd_loss.py:53-211.
 //
 // ssd_loss_kernel is a persistent cooperative kernel (all CTAs co-resident, grid-wide barriers between phases):
 //   phase A  tiles of 128 prediction rows stream through shared memory with cp.async.bulk + mbarrier (two stages), one thread

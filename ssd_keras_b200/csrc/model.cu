@@ -65,7 +65,7 @@ int build_conv(ssdk_model* m, int li) {
     L.bn_eps = d.bn_eps > 0.f ? d.bn_eps : 1e-3f;
     L.bn_momentum = (d.bn_momentum > 0.f && d.bn_momentum < 1.f) ? d.bn_momentum : 0.99f;
   }
-  // experiment knob (inference plans only): route the image-facing layer through im2col (K = 27 -> 32) + the tcgen05 GEMM instead
+  // experiment knob (inference plans only): route the image-facing layer through im2col (K = 27 -> 32) + the implicit GEMM instead
   if (L.direct && !m->training && getenv("SSDK_NO_DIRECT")) L.direct = false;
   if (L.direct) {
     int rc = upload_f32(m, &L.w_f32, d.kernel, (size_t)taps * cin * cout); if (rc) return rc;
@@ -82,7 +82,7 @@ int build_conv(ssdk_model* m, int li) {
     if (!m->training && first_tc_supported(taps, cin, cout) && d.dilation >= 1 && first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l) &&
         !getenv("SSDK_NO_FIRST_TC")) {
       std::vector<uint16_t> whi, wlo;
-      const int K = taps * 4, BN = (cout + 15) / 16 * 16;
+      const int K = taps * 4, BN = first_bn(cout);
       first_weight_image(d.kernel, taps, cin, cout, BN, (K + 63) / 64, whi, wlo);
       rc = dev_alloc(m, &L.w_hi, whi.size(), false); if (rc) return rc;
       SSDK_CHECK_CUDA(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
@@ -100,18 +100,16 @@ int build_conv(ssdk_model* m, int li) {
   const int Ho = L.H, Wo = L.W;
   ConvGeom g;
   g.Ho = Ho; g.Wo = Wo; g.B = m->B; g.cout = cout;
-  int kblocks, ktot;
+  int kblocks;
   if (L.im2col) {
     L.Kpad = (taps * cin + 7) / 8 * 8;
     kblocks = (L.Kpad + 63) / 64;
-    ktot = L.Kpad;
     size_t n = (size_t)m->B * Ho * Wo * L.Kpad + 64 * 8;
     int rc = dev_alloc(m, &L.col_hi, n, true); if (rc) return rc;
     if (m->split) { rc = dev_alloc(m, &L.col_lo, n, true); if (rc) return rc; }
     g.a_hi = L.col_hi; g.a_lo = L.col_lo; g.a_inner = L.Kpad; g.a_rows = (uint64_t)m->B * Ho * Wo;
   } else {
     kblocks = (ia.Cs + 63) / 64;
-    ktot = ia.Cs;
     g.in = &ia; g.kh = d.kh; g.kw = d.kw; g.dilation = d.dilation; g.pad_t = d.pad_t; g.pad_l = d.pad_l;
     SSDK_REQUIRE(ia.pad >= std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)), "internal: activation border too small");
   }
@@ -127,7 +125,7 @@ int build_conv(ssdk_model* m, int li) {
     rc = dev_alloc(m, &L.w_lo, wlo.size(), false); if (rc) return rc;
     SSDK_CHECK_CUDA(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
   }
-  rc = plan_conv_gemm(m, cl, g, L.w_hi, L.w_lo, Krow, kblocks, (ktot - (kblocks - 1) * 64 + 15) / 16, &L.tile_list);
+  rc = plan_conv_gemm(m, cl, g, L.w_hi, L.w_lo, Krow, kblocks, &L.tile_list);
   if (rc) return rc;
   if (m->training) {          // fp32 master kernel, HWIO, with the conf/loc kernels of a head fused per box like the packed planes
     std::vector<float> master((size_t)taps * cin * cout);
@@ -222,7 +220,7 @@ int plan_overlap(ssdk_model* m) {
   m->overlap_from = -1; m->grid_cap = 0;
   if (m->training) return SSDK_OK;
   if (const char* e = getenv("SSDK_OVERLAP")) { if (!atoi(e)) return SSDK_OK; }
-  int R = m->ctx->sm_count / 3 + 1;      // 50 of 148: measured on B200 against sm_count / 4 (5.76 / 5.91 ms vs 5.84 / 5.95 ms per step)
+  int R = m->ctx->sm_count / 3 + 1;
   if (const char* e = getenv("SSDK_OVERLAP_R")) R = atoi(e);
   std::vector<int> kind(n, 0), grid(n, 0), input(n, -1);
   for (int i = 0; i < n; ++i) {
@@ -249,7 +247,7 @@ namespace ssdk {
 
 // Geometry, tile list, pipeline depths and TMA descriptors of one implicit-GEMM launch.  The caller fills the epilogue.
 int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
-                   size_t krow, int kblocks, int last_ksteps, int** tile_list_out) {
+                   size_t krow, int kblocks, int** tile_list_out) {
   ConvArgs& a = cl.args;
   memset(&a, 0, sizeof(a));
   const __nv_bfloat16* a_hi; const __nv_bfloat16* a_lo;
@@ -257,7 +255,7 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   if (!g.in) {
     SSDK_REQUIRE(g.a_rows < (1ull << 31), "GEMM with too many rows");
     a.M_total = (int)g.a_rows; a.rows_per_img = g.Ho * g.Wo; a.in_Wp = g.Wo;
-    a.KH = 1; a.KW = 1; a.row_shift[0] = 0; a.kw_rows = 1; a.slab_rows = 128;
+    a.KH = 1; a.KW = 1; a.row_shift[0] = 0; a.kw_rows = 1;
     a_hi = g.a_hi; a_lo = g.a_lo; a_inner = g.a_inner; a_rows = g.a_rows;
   } else {
     const ActBuf& ia = *g.in;
@@ -265,8 +263,6 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
     a.M_total = g.B * ia.Hp() * ia.Wp(); a.rows_per_img = ia.Hp() * ia.Wp(); a.in_Wp = ia.Wp();
     SSDK_REQUIRE(g.kh <= 8 && g.kw <= 8, "conv kernel %dx%d is larger than the supported 8x8", g.kh, g.kw);
     a.KH = g.kh; a.KW = g.kw; a.kw_rows = g.dilation;
-    a.slab_rows = (128 + (g.kw - 1) * g.dilation + 7) / 8 * 8;
-    SSDK_REQUIRE(a.slab_rows <= 256, "conv kernel width x dilation too large for one TMA box");
     for (int kh = 0; kh < g.kh; ++kh) {
       a.row_shift[kh] = (kh * g.dilation - g.pad_t + ia.pad) * ia.Wp() + (0 - g.pad_l + ia.pad);
       SSDK_REQUIRE(a.row_shift[kh] >= 0, "internal: activation border too small for this convolution");
@@ -274,15 +270,19 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
     a_hi = ia.hi; a_lo = ia.lo; a_inner = ia.Cs; a_rows = (uint64_t)a.M_total;
   }
   a.kblocks = kblocks;
-  a.last_ksteps = last_ksteps;
   a.Ho = g.Ho; a.Wo = g.Wo; a.B = g.B;
   a.cout = g.cout;
   a.BN = g.cout <= 64 ? 64 : (g.cout <= 128 ? 128 : 256);
   a.split = m->split;
   a.k_split = 1;
-  if (a.BN == 256 && g.cout % 128 == 0) {                       // (not the predictor heads: their epilogue needs all boxes in one tile)
-    // 256-wide tiles on few m-tiles leave the last wave of the persistent grid mostly empty (conv5_x: 220 units on 148 SMs);
-    // 128-wide tiles double the units.  Pick by the number of full-width waves (SSDK_BN_MAX forces, SSDK_BN_AUTO=0 disables).
+  if (a.split && a.BN == 256) {
+    // bf16x3 tiles carry the cross-term accumulator (acc_split), which fits in registers up to 160 columns: 160-wide tiles for
+    // the predictor heads of <= 160 columns (6 boxes x 25 for VOC: the fused head epilogue needs all boxes of a pixel in one
+    // tile), 128-wide tiles otherwise
+    a.BN = g.cout <= 160 ? 160 : 128;
+  } else if (a.BN == 256 && g.cout % 128 == 0) {                // (not the predictor heads: their epilogue needs all boxes in one tile)
+    // 256-wide tiles on few m-tiles leave the last wave of the persistent grid mostly empty; 128-wide tiles double the units.
+    // Pick the width with fewer tile-columns per SM over all waves (a partial last wave costs a whole one).
     long long n_valid = 0;
     for (long long t = 0; t < (a.M_total + 127) / 128; ++t) {
       bool any = false;
@@ -296,65 +296,20 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
     }
     const int sms = m->ctx->sm_count;
     const long long u256 = n_valid * ((g.cout + 255) / 256), u128 = n_valid * ((g.cout + 127) / 128);
-    // measured on B200 (same-box A/B, SSDK_BN_MAX=128): a 128-wide tile costs 15-18 % more per FLOP than a 256-wide one (its MMAs
-    // sit at the shared-memory operand bandwidth: conv3_x 460 -> 542 us, conv4_x 513 -> 588 us), so it only pays where the
-    // 256-wide grid wastes more than that: conv5_x (220 units on 148 SMs) 178 -> 168 us, conv6_2 / conv7_2 / conv8_2 54 -> 39,
-    // 34 -> 25, 32 -> 24 us
     const double t256 = (double)((u256 + sms - 1) / sms) * 256.0;
-    double pen = 1.18;                                  // SSDK_BN128_PENALTY: experiment knob for this factor
-    if (const char* e = getenv("SSDK_BN128_PENALTY")) pen = atof(e);
-    const double t128 = (double)((u128 + sms - 1) / sms) * 128.0 * pen;
-    bool use128 = t128 < 0.95 * t256;
-    if (const char* e = getenv("SSDK_BN_AUTO")) { if (!atoi(e)) use128 = false; }
-    if (const char* e = getenv("SSDK_BN_MAX")) use128 = atoi(e) <= 128;
+    const double t128 = (double)((u128 + sms - 1) / sms) * 128.0;
+    const bool use128 = t128 < t256;
     if (use128) a.BN = 128;
   }
+  a.acc_split = a.split;
   a.n_tiles_n = (g.cout + a.BN - 1) / a.BN;
-  // two m-tiles per work unit when the accumulators fit (2 buffers x 2 tiles x BN <= 512 TMEM columns): the 64/128-channel
-  // layers are bound by re-fetching the weight tiles from L2 for every m-tile, pairing halves that traffic
   const int n_m = (a.M_total + 127) / 128;
-  a.mt = 1;
-  { const char* e = getenv("SSDK_MT"); const int want = e ? atoi(e) : 2;
-    if (want >= 2 && g.in && a.BN <= 128 && n_m >= 8 * m->ctx->sm_count) a.mt = 2; }
-  // 64 -> 64 channel layers (conv1_2 and its data gradient): all nine weight tiles fit in shared memory next to two A slabs.
-  // Keeping them resident removes ~40% of the layer's L2->SM traffic, but forces one m-tile per unit and measured SLOWER on
-  // B200 (7.69 vs 7.56 ms/step): the layer is bound by the shared-memory operand bandwidth of N = 64 MMAs, not by L2.
-  // Kept behind SSDK_RESIDENT=1 for experiments.
-  { const char* e = getenv("SSDK_RESIDENT"); const int want = e ? atoi(e) : 0;
-    const size_t wbytes = (size_t)a.KH * a.KW * kblocks * a.BN * 64 * 2 * (a.split ? 2 : 1);
-    const size_t abytes = (size_t)a.slab_rows * 64 * 2 * (a.split ? 2 : 1);
-    if (want && g.in && a.n_tiles_n == 1 && a.BN == 64 && n_m >= 8 * m->ctx->sm_count && wbytes + 2 * abytes + 4096 <= 218 * 1024) { a.resident_b = 1; a.mt = 1; } }
-  // deep-K layers: the tensor core adds into the fp32 accumulator with truncation, ~0.5 ulp of bias per MMA; keeping the two
-  // small cross terms in their own accumulator leaves only the hi*hi third of the adds on the large one (DESIGN.md 3.1)
-  a.acc_bufs = 2; a.acc_split = 0;
-  { const char* e = getenv("SSDK_ACC_SPLIT"); const int want = e ? atoi(e) : 1;       // on: +3.5% step time, 3x less bias
-    if (want && a.split && a.KH * a.KW * kblocks >= 32) {
-      a.acc_split = 1;
-      a.mt = 1;                     // paired m-tiles + cross-term accumulator would need 4 accumulators per unit; deep-K layers
-                                    // re-fetch few weight bytes per MMA anyway, so they keep one m-tile and both accumulator sets
-      if (2 * 2 * a.mt * a.BN > 512) a.acc_bufs = 1;
-      if (a.acc_bufs * 2 * a.mt * a.BN > 512) { a.acc_split = 0; a.acc_bufs = 2; }
-    } }
-  // The hi and lo planes of a weight tile lie back to back in a ring slot and the cross-term accumulator follows the main one in
-  // TMEM, so for BN <= 128 the products A_hi*B_hi and A_hi*B_lo are ONE MMA of N = 2*BN (operand [B_hi ; B_lo], result
-  // [main | cross]); A_lo*B_hi follows into the cross columns.  Two issues instead of three per k-step, and the A_hi tile is read
-  // from shared memory once instead of twice: N = 64 MMAs are bound by the operand bandwidth (4 KB of A + 2 KB of B per 32 clocks),
-  // the combined one moves 8 KB per 64 clocks.  Tiles without a cross-term accumulator get one when the columns are there
-  // (64-wide tiles with paired m-tiles: 2 sets x 2 tiles x 2 x 64 = 512).  SSDK_FUSE_B=0 restores three MMAs.
-  a.fuse_b = 0;
-  { const char* e = getenv("SSDK_FUSE_B"); const int want = e ? atoi(e) : 1;
-    if (want && a.split && a.BN <= 128) {
-      if (!a.acc_split && 2 * 2 * a.mt * a.BN <= 512) { a.acc_split = 1; a.acc_bufs = 2; }
-      if (a.acc_split) a.fuse_b = 1;
-    } }
   conv_pick_stages(a);
-  { const char* e = getenv("SSDK_BO_MODE"); a.bo_mode = e ? atoi(e) : 0; }
-  { const char* e = getenv("SSDK_EPI_PIPE"); a.epi_pipe = e ? atoi(e) : 2; }
   // m-tiles that hold at least one valid output row
   std::vector<int> tiles;
-  for (int t = 0; t < n_m; t += a.mt) {
+  for (int t = 0; t < n_m; ++t) {
     bool any = false;
-    for (int r = 0; r < 128 * a.mt && !any; ++r) {
+    for (int r = 0; r < 128 && !any; ++r) {
       long long v = (long long)t * 128 + r;
       if (v >= a.M_total) break;
       int rr = (int)(v % a.rows_per_img);
@@ -369,24 +324,21 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   a.tile_list = tl;
   if (tile_list_out) *tile_list_out = tl;
   const uint64_t a_ld = (!g.in && g.a_ld) ? g.a_ld : a_inner;
-  rc = make_tmap_2d(&cl.a_hi, a_hi, a_inner, a_rows, a_ld * 2, 64, (uint32_t)a.slab_rows); if (rc) return rc;
+  rc = make_tmap_2d(&cl.a_hi, a_hi, a_inner, a_rows, a_ld * 2, 64, 128); if (rc) return rc;
   rc = make_tmap_2d(&cl.b_hi, w_hi, krow, (uint64_t)g.cout, krow * 2, 64, (uint32_t)a.BN); if (rc) return rc;
   if (m->split) {
-    rc = make_tmap_2d(&cl.a_lo, a_lo, a_inner, a_rows, a_ld * 2, 64, (uint32_t)a.slab_rows); if (rc) return rc;
+    rc = make_tmap_2d(&cl.a_lo, a_lo, a_inner, a_rows, a_ld * 2, 64, 128); if (rc) return rc;
     rc = make_tmap_2d(&cl.b_lo, w_lo, krow, (uint64_t)g.cout, krow * 2, 64, (uint32_t)a.BN); if (rc) return rc;
   } else { cl.a_lo = cl.a_hi; cl.b_lo = cl.b_hi; }
   const int total_tiles = a.n_tiles_m * a.n_tiles_n;
   cl.grid = std::max(1, std::min(total_tiles, m->ctx->sm_count));
   cl.smem = conv_smem_bytes(a);
-  SSDK_REQUIRE((a.acc_bufs == 1 ? 1 : 2) * (a.acc_split ? 2 : 1) * a.mt * a.BN <= 512,
-               "internal: conv plan needs %d TMEM columns", (a.acc_bufs == 1 ? 1 : 2) * (a.acc_split ? 2 : 1) * a.mt * a.BN);
   SSDK_REQUIRE(cl.smem <= 227 * 1024, "internal: conv plan needs %zu bytes of shared memory", cl.smem);
   double issued = 0;
   for (int nt = 0; nt < a.n_tiles_n; ++nt) {
-    int ne = std::min(a.BN, ((g.cout - nt * a.BN) + 15) / 16 * 16);
-    // MMA columns per product: 3 x ne, or (BN + ne) + ne with the fused weight operand
-    const double cols = !m->split ? ne : (a.fuse_b ? (double)(a.BN + 2 * ne) : 3.0 * ne);
-    issued += 2.0 * a.n_tiles_m * a.mt * 128.0 * cols * (double)(a.KH * a.KW) * ((kblocks - 1) * 64 + a.last_ksteps * 16);
+    // every tile issues the full BN columns (the weight rows past cout are TMA zero fill) and all 64 channels of every k-block,
+    // 3 products with split planes
+    issued += 2.0 * a.n_tiles_m * 128.0 * a.BN * (m->split ? 3.0 : 1.0) * (double)(a.KH * a.KW) * (kblocks * 64);
   }
   cl.flops_issued = issued;
   return SSDK_OK;
@@ -398,8 +350,8 @@ extern "C" int ssdk_model_create(ssdk_ctx* ctx, const ssdk_model_desc* desc, ssd
   SSDK_REQUIRE(ctx && desc && out && desc->layers && desc->n_layers > 0, "ssdk_model_create: bad argument");
   SSDK_REQUIRE(desc->batch > 0 && desc->img_height > 0 && desc->img_width > 0, "ssdk_model_create: bad input shape");
   SSDK_REQUIRE(desc->precision == 0 || desc->precision == 1, "ssdk_model_create: precision must be 0 (bf16x3) or 1 (bf16)");
-  SSDK_REQUIRE(ctx->prop.major == 10, "libssdk's convolution kernels need an sm_100 (Blackwell) GPU, found sm_%d%d; there is no fallback",
-               ctx->prop.major, ctx->prop.minor);
+  SSDK_REQUIRE(ctx->prop.major == 9 && ctx->prop.minor == 0,
+               "libssdk's convolution kernels need an sm_90 (Hopper) GPU, found sm_%d%d; there is no fallback", ctx->prop.major, ctx->prop.minor);
   SSDK_CHECK_CUDA(cudaSetDevice(ctx->device));
   ssdk_model* m = new ssdk_model();
   m->ctx = ctx; m->B = desc->batch; m->H = desc->img_height; m->W = desc->img_width; m->Cimg = desc->img_channels;

@@ -121,6 +121,6 @@ int launch_bn_forward(ssdk_ctx* ctx, LayerPlan& L, int act, cudaStream_t s);
 int launch_bn_backward(ssdk_ctx* ctx, LayerPlan& L, int act, const ActBuf& g, float* dgamma, float* dbeta, cudaStream_t s);
 
 int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
-                   size_t krow, int kblocks, int last_ksteps, int** tile_list_out);
+                   size_t krow, int kblocks, int** tile_list_out);
 
 }  // namespace ssdk

@@ -1,8 +1,8 @@
-// Training step for the SSD graphs on sm_100a: backward pass + SGD.  Replaces what TensorFlow/Keras do for the reference
+// Training step for the SSD graphs on sm_90a: backward pass + SGD.  Replaces what TensorFlow/Keras do for the reference
 // in fit_generator (autodiff of models/keras_ssd300.py:263-419 and keras_loss_function/keras_ssd_loss.py:98-211, the
 // l2 kernel regulariser models/keras_ssd300.py:274 and SGD(lr, momentum) ssd300_training.ipynb:169).
 //
-// Every convolution gradient runs on the SAME tcgen05 implicit-GEMM kernel as the forward pass (conv.cu):
+// Every convolution gradient runs on the SAME wgmma implicit-GEMM kernel as the forward pass (conv.cu):
 //   data gradient    dX = conv(dZ, W rotated by 180 degrees with in/out channels swapped), padding dilation*(k-1)-pad;
 //                    the epilogue multiplies by ReLU'(forward value) and accumulates when a tensor has several consumers.
 //   weight gradient  dW[co][tap][ci] = sum_v dZT[co][v] * XT[ci][v + shift(tap)]: both operands are transposed once into
@@ -587,7 +587,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
         ConvGeom gg;
         gg.in = &T.g; gg.kh = 1; gg.kw = 1; gg.dilation = 1; gg.pad_t = 0; gg.pad_l = 0;
         gg.Ho = L.H; gg.Wo = L.W; gg.B = m->B; gg.cout = kcol;
-        rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, (T.g.Cs - (T.w2_kblocks - 1) * 64 + 15) / 16, &T.dgrad_tiles);
+        rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, &T.dgrad_tiles);
         if (rc) return fail(rc);
         ConvArgs& a = T.dgrad.args;
         a.epi = EPI_F32; a.bias = nullptr; a.act = SSDK_ACT_NONE; a.out_f32 = T.dcol;
@@ -603,7 +603,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       gg.in = &T.g; gg.kh = d.kh; gg.kw = d.kw; gg.dilation = d.dilation;
       gg.pad_t = d.dilation * (d.kh - 1) - d.pad_t; gg.pad_l = d.dilation * (d.kw - 1) - d.pad_l;
       gg.Ho = PL.H; gg.Wo = PL.W; gg.B = m->B; gg.cout = T.cin;
-      rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, (T.g.Cs - (T.w2_kblocks - 1) * 64 + 15) / 16, &T.dgrad_tiles);
+      rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, &T.dgrad_tiles);
       if (rc) return fail(rc);
       ConvArgs& a = T.dgrad.args;
       a.epi = EPI_SPLIT; a.bias = nullptr; a.act = SSDK_ACT_NONE;
@@ -659,7 +659,6 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
     const int n_gemm = L.im2col ? 1 : T.taps;
     const int ncols = L.im2col ? L.Kpad : T.cin;            // N of the GEMM
     const int kblocks = (int)((T.Kv + 63) / 64);
-    const int last_ksteps = (int)((T.Kv - (long long)(kblocks - 1) * 64 + 15) / 16);
     T.wgrad.resize(n_gemm); T.wgrad_res.assign(n_gemm, 0);
     for (int tp = 0; tp < n_gemm; ++tp) {
       ConvGeom wg;
@@ -667,7 +666,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       wg.Ho = T.cout; wg.Wo = 1; wg.B = 1; wg.cout = ncols;
       ConvLaunch& cl = T.wgrad[tp];
       // the transposed operands are [channels][ldT] with zeros in [Kv, ldT)
-      rc = plan_conv_gemm(m, cl, wg, t->xT_hi, t->xT_lo, (size_t)T.ldT, kblocks, last_ksteps, nullptr);
+      rc = plan_conv_gemm(m, cl, wg, t->xT_hi, t->xT_lo, (size_t)T.ldT, kblocks, nullptr);
       if (rc) return fail(rc);
       ConvArgs& a = cl.args;
       a.epi = EPI_ATOMIC; a.bias = nullptr; a.act = SSDK_ACT_NONE;

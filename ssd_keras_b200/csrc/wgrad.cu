@@ -1,17 +1,15 @@
-// Weight gradient of a stride-1 convolution on tcgen05, straight from the NHWC activation / gradient tensors (no transposes):
+// Weight gradient of a stride-1 convolution on wgmma, straight from the NHWC activation / gradient tensors (no transposes):
 //   dW[co][kh][kw][ci] = sum over output pixels p of dZ[p][co] * X[p + (kh, kw)*dilation - pad][ci]
 // (the cuDNN wgrad the reference gets through TensorFlow's autodiff of models/keras_ssd300.py:274-361).
 //
-// GEMM view: M = co (128 per tile), N = (kw, ci) -- KW accumulators of BNc input channels each, side by side in TMEM --
-// K = output pixels.  Both operands are "MN-major": a K row (one pixel) holds 64 contiguous channels = one 128-byte line, which
-// is exactly how NHWC tensors lie in HBM, so a K-block of 64 pixels is ONE 4-D TMA box {64 channels, bw, bh, 1 image}
-// (bw * bh = 64) per 64-channel group.  The X box is bw + (KW-1)*dilation pixels wide: the KW taps of a kernel row read the
-// same slab at a K-row offset of kw*dilation lines (UMMA descriptor start address + 128 B per line, swizzle phase follows the
-// absolute shared-memory address, base_offset 0).  Borders are physical zeros, everything further out is TMA zero fill, and
-// dZ is zero outside the valid outputs, so no masking is needed.  The pixel axis is split across CTAs (split-K); partial
-// sums are reduced into the fp32 gradient buffer with vector atomics (red.global.add.v4.f32).
-// Work unit = (co tile, ci tile, kh, k-split); persistent CTAs; warp 0 TMA, warp 1 MMA, warp 2 TMEM alloc, warps 4-7 epilogue.
-// Precision as in conv.cu: bf16 hi+lo operands, hi*hi + hi*lo + lo*hi into fp32 TMEM.
+// GEMM view: M = co (128 per tile, 64 per warpgroup), N = ci (BNc per tile), K = output pixels.  Both operands are "MN-major": a
+// K row (one pixel) holds 64 contiguous channels = one 128-byte line, which is exactly how NHWC tensors lie in HBM, so a K-block
+// of 64 pixels is ONE 4-D TMA box {64 channels, bw, bh, 1 image} (bw * bh = 64) per 64-channel group; the X box of tap (kh, kw)
+// is the same patch shifted by (kw, kh) * dilation.  Borders are physical zeros, everything further out is TMA zero fill, and
+// dZ is zero outside the valid outputs, so no masking is needed.  The pixel axis is split across CTAs (split-K); partial sums
+// are reduced into the fp32 gradient buffer with vector atomics (red.global.add.v2.f32) straight from the accumulator registers.
+// Work unit = (co tile, ci tile, tap, k-split); persistent CTAs; one thread issues the TMA ring, two warpgroups issue wgmma.
+// Precision as in conv.cu: bf16 hi+lo operands, hi*hi + hi*lo + lo*hi into fp32 accumulators.
 #include "wgrad.cuh"
 #include "tc.cuh"
 #include <cudaTypedefs.h>
@@ -23,185 +21,120 @@ namespace {
 
 constexpr int kBoxA = 64 * 128;            // one {64 channels x 64 pixels} box: 8 KB
 
-// MN-major, 128B-swizzled operand: a K row is one 128-byte line (64 channels); 8 lines form a 1024-byte swizzle atom (SBO);
-// the next 64-channel group starts `lbo` bytes further (LBO).
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t addr, uint32_t lbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3FFFu);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((1024u >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;                            // descriptor version 1 (sm_100)
-  d |= (uint64_t)2 << 61;                            // SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ uint32_t make_idesc_mn(int n) {
-  // c F32 (bit 4), a/b BF16 (bits 7, 10), a/b MN-major (bits 15, 16), N>>3 at 17, M>>4 at 24
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
+template <int BNc, bool SPLIT>
 __global__ void __launch_bounds__(256, 1)
-wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tm_g_hi, const __grid_constant__ CUtensorMap tm_g_lo,
-                     const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
-                     const __grid_constant__ WgradArgs args) {
+wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tm_g_hi, const __grid_constant__ CUtensorMap tm_g_lo,
+                   const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
+                   const __grid_constant__ WgradArgs args) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int S = args.stages, split = args.split, KW = args.KW, BNc = args.BNc;
-  const int nA = args.a_boxes, nB = BNc / 64;
-  const uint32_t a_plane = (uint32_t)nA * kBoxA, b_plane = (uint32_t)nB * args.slab_bytes;
-  const uint32_t stage_bytes = (a_plane + b_plane) * (split ? 2u : 1u);
-  const uint32_t bar_base = smem_base + stage_bytes * S;
-  auto full = [&](int s) { return bar_base + 8u * s; };
-  auto empty = [&](int s) { return bar_base + 8u * (S + s); };
-  const uint32_t tfull = bar_base + 8u * (2 * S), tempty = bar_base + 8u * (2 * S + 1);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * S + 2);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_dyn + (tmem_slot - smem_u32(smem_dyn)));
+  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  constexpr bool split = SPLIT;
+  const int S = args.stages, KW = args.KW;
+  constexpr int nB = BNc / 64;
+  const int nA = args.a_boxes;
+  // stage: dZ_hi (2 boxes) | dZ_lo | X_hi (nB boxes) | X_lo
+  const uint32_t a_plane = 2u * kBoxA, b_plane = (uint32_t)nB * kBoxA;
+  const uint32_t b_off = a_plane * (split ? 2u : 1u);
+  const uint32_t stage = (a_plane + b_plane) * (split ? 2u : 1u);
+  const uint32_t bar_base = smem_base + stage * S;
+  auto full = [&](uint32_t s) { return bar_base + 8u * s; };
+  auto empty = [&](uint32_t s) { return bar_base + 8u * ((uint32_t)S + s); };
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_g_hi)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tm_x_hi)) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-    mbar_init(tfull, 1); mbar_init(tempty, 4);
+  if (tid == 0) {
+    prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_x_hi);
+    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  const int total_units = args.co_tiles * args.ci_tiles * args.KH * args.k_split;
+  const int taps = args.KH * KW;
+  const int total_units = args.co_tiles * args.ci_tiles * taps * args.k_split;
   const int patches_per_img = args.px_tiles * args.py_tiles;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      int s = 0; uint32_t ph = 0;
-      for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
-        const int ks = u % args.k_split; int r = u / args.k_split;
-        const int kh = r % args.KH; r /= args.KH;
-        const int ci0 = (r % args.ci_tiles) * BNc, co0 = (r / args.ci_tiles) * 128;
-        const int p0 = ks * args.patches_per_split, p1 = min(args.total_patches, p0 + args.patches_per_split);
-        for (int p = p0; p < p1; ++p) {
-          const int n = p / patches_per_img; const int q = p - n * patches_per_img;
-          const int py = q / args.px_tiles, px = q - py * args.px_tiles;
-          const int x0 = px * args.bw, y0 = py * args.bh;
-          mbar_wait(empty(s), ph ^ 1u);
-          const uint32_t dst = smem_base + stage_bytes * s;
-          mbar_expect_tx(full(s), args.tx_bytes);
-          for (int pl = 0; pl < (split ? 2 : 1); ++pl) {
-            const CUtensorMap* tg = pl ? &tm_g_lo : &tm_g_hi;
-            const CUtensorMap* tx = pl ? &tm_x_lo : &tm_x_hi;
-            const uint32_t da = dst + pl * a_plane, db = dst + (split ? 2u : 1u) * a_plane + pl * b_plane;
-            for (int i = 0; i < nA; ++i) tma_load_4d(da + i * kBoxA, tg, co0 + 64 * i, x0 + args.g_pad, y0 + args.g_pad, n, full(s));
-            for (int j = 0; j < nB; ++j)
-              tma_load_4d(db + j * args.slab_bytes, tx, ci0 + 64 * j, x0 + args.x_off, y0 + kh * args.dil + args.y_off, n, full(s));
-          }
-          if (++s == S) { s = 0; ph ^= 1u; }
-        }
+  // with cout <= 64 there is one dZ box: the second warpgroup multiplies it again (a uniform wgmma path) and stores nothing
+  const bool active = wg < nA;
+  const uint32_t a_box = active ? (uint32_t)wg * kBoxA : 0u;
+  uint32_t g = 0;
+  float acc[BNc / 2];
+  for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+    const int ks = u % args.k_split; int r = u / args.k_split;
+    const int tap = r % taps; r /= taps;
+    const int kh = tap / KW, kw = tap - kh * KW;
+    const int ci0 = (r % args.ci_tiles) * BNc, co0 = (r / args.ci_tiles) * 128;
+    const int p0 = ks * args.patches_per_split, p1 = min(args.total_patches, p0 + args.patches_per_split);
+    const int nk = p1 - p0;
+    auto issue = [&](int i) {
+      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
+      mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
+      const int p = p0 + i;
+      const int n = p / patches_per_img; const int q = p - n * patches_per_img;
+      const int py = q / args.px_tiles, px = q - py * args.px_tiles;
+      const int x0 = px * args.bw, y0 = py * args.bh;
+      const uint32_t dst = smem_base + stage * s;
+      mbar_expect_tx(full(s), args.tx_bytes);
+      for (int pl = 0; pl < (split ? 2 : 1); ++pl) {
+        const CUtensorMap* tg = pl ? &tm_g_lo : &tm_g_hi;
+        const CUtensorMap* tx = pl ? &tm_x_lo : &tm_x_hi;
+        const uint32_t da = dst + pl * a_plane, db = dst + b_off + pl * b_plane;
+        for (int a = 0; a < nA; ++a) tma_load_4d(da + a * kBoxA, tg, co0 + 64 * a, x0 + args.g_pad, y0 + args.g_pad, n, full(s));
+        for (int j = 0; j < nB; ++j)
+          tma_load_4d(db + j * kBoxA, tx, ci0 + 64 * j, x0 + kw * args.dil + args.x_off, y0 + kh * args.dil + args.y_off, n, full(s));
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    int s = 0; uint32_t ph = 0;
-    int it = 0;
-    const uint32_t idesc = make_idesc_mn(BNc);
-    const int slab_w = args.bw + (KW - 1) * args.dil;
-    const uint64_t desc_a = make_desc_mn(0, kBoxA), desc_b = make_desc_mn(0, args.slab_bytes);
-    uint32_t krow[4];                                       // first slab line (in 16-byte units) of each 16-pixel k-step
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { const int line = (k * 16) / args.bw; krow[k] = (uint32_t)(line * slab_w + (k * 16 - line * args.bw)) * 8u; }
-    for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++it) {
-      const int ks = u % args.k_split;
-      const int p0 = ks * args.patches_per_split, p1 = min(args.total_patches, p0 + args.patches_per_split);
-      mbar_wait(tempty, (uint32_t)(it & 1) ^ 1u);            // the epilogue has drained the previous unit's accumulators
-      tc_fence_after();
-      uint32_t accumulate = 0;
-      for (int p = p0; p < p1; ++p) {
-        mbar_wait(full(s), ph);
-        tc_fence_after();
-        if (elect_one()) {
-          // descriptor = constant upper word | (address >> 4): a couple of integer adds between two MMA issues
-          const uint32_t a_hi = (smem_base + stage_bytes * s) >> 4, a_lo = a_hi + (a_plane >> 4);
-          const uint32_t b_hi = a_hi + (((split ? 2u : 1u) * a_plane) >> 4), b_lo = b_hi + (b_plane >> 4);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {                       // 4 UMMA k-steps of 16 pixels
-            const uint64_t dah = desc_a | (uint64_t)(a_hi + 128u * k), dal = desc_a | (uint64_t)(a_lo + 128u * k);
-            for (int kw = 0; kw < KW; ++kw) {
-              const uint32_t bo = krow[k] + (uint32_t)(kw * args.dil) * 8u;
-              const uint64_t dbh = desc_b | (uint64_t)(b_hi + bo);
-              const uint32_t d_tmem = tmem_base + (uint32_t)(kw * BNc);
-              tc_mma(d_tmem, dah, dbh, idesc, accumulate);
-              if (split) {
-                tc_mma(d_tmem, dah, desc_b | (uint64_t)(b_lo + bo), idesc, 1);
-                tc_mma(d_tmem, dal, dbh, idesc, 1);
-              }
-            }
-            accumulate = 1;
-          }
-          tc_commit(empty(s));
-        }
-        __syncwarp();
-        if (++s == S) { s = 0; ph ^= 1u; }
-      }
-      if (elect_one()) tc_commit(tfull);
+    };
+    auto release = [&](int j) {                                  // patch j's MMAs are done: refill its stage with patch j + S
       __syncwarp();
+      if (lane == 0) mbar_arrive(empty((g + (uint32_t)j) % (uint32_t)S));
+      if (tid == 0 && j + S < nk) issue(j + S);
+    };
+    if (tid == 0)
+      for (int i = 0; i < min(S, nk); ++i) issue(i);
+    wgmma_fence_acc(acc);
+    for (int i = 0; i < nk; ++i) {                                 // one wgmma group stays in flight
+      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
+      mbar_wait(full(s), (gi / (uint32_t)S) & 1u);
+      constexpr uint64_t kDescA = wgmma_desc_hi(kBoxA), kDescB = wgmma_desc_hi(kBoxA);
+      const uint32_t a_hi = smem_base + stage * s + a_box, b_hi = smem_base + stage * s + b_off;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {                                 // 4 k-steps of 16 pixels = 2048 bytes of each box
+        const uint64_t dah = wgmma_desc(kDescA, a_hi + 2048u * k), dbh = wgmma_desc(kDescB, b_hi + 2048u * k);
+        Wgmma<BNc, 1, 1>::mma(acc, dah, dbh, (i | k) ? 1u : 0u);
+        if constexpr (split) {
+          Wgmma<BNc, 1, 1>::mma(acc, dah, wgmma_desc(kDescB, b_hi + b_plane + 2048u * k), 1u);
+          Wgmma<BNc, 1, 1>::mma(acc, wgmma_desc(kDescA, a_hi + a_plane + 2048u * k), dbh, 1u);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (i > 0) release(i - 1);
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue: TMEM -> atomics into dW[co][tap][ci] =====================
-    const int q = warp - 4;
-    int it = 0;
-    for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++it) {
-      int r = u / args.k_split;
-      const int kh = r % args.KH; r /= args.KH;
-      const int ci0 = (r % args.ci_tiles) * BNc, co0 = (r / args.ci_tiles) * 128;
-      mbar_wait(tfull, (uint32_t)(it & 1));
-      tc_fence_after();
-      const int co = co0 + q * 32 + lane;
-      const bool valid = co < args.cout;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16);
-      for (int kw = 0; kw < KW; ++kw) {
-        float* dst = args.dw + ((size_t)co * args.taps + (kh * KW + kw)) * args.cin + ci0;
-        for (int c0 = 0; c0 < BNc; c0 += 32) {
-          uint32_t vr[32];
-          tmem_ld32(t_row + (uint32_t)(kw * BNc + c0), vr);
-          if (valid) {
-            // the parameter spans of the flat gradient buffer are only 4-byte aligned in general (head biases of 6*25 floats)
-            const unsigned al = (unsigned)(reinterpret_cast<uintptr_t>(dst) & 15u);
-            if (al == 0) {
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (nk > 0) release(nk - 1);
+    g += (uint32_t)nk;
+    // ===================== epilogue: accumulator registers -> atomics into dW[co][tap][ci] =====================
+    if (active && nk > 0) {
+      const int co_a = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c = 2 * (lane & 3);
 #pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                red_add_v4(dst + c0 + j, __uint_as_float(vr[j]), __uint_as_float(vr[j + 1]), __uint_as_float(vr[j + 2]), __uint_as_float(vr[j + 3]));
-            } else if ((al & 7u) == 0) {
+      for (int h = 0; h < 2; ++h) {
+        const int co = co_a + 8 * h;
+        if (co < args.cout) {
+          float* dst = args.dw + ((size_t)co * taps + tap) * args.cin + ci0 + c;
+          // the parameter spans of the flat gradient buffer are only 4-byte aligned in general (head biases of 6*25 floats)
+          const bool al8 = (reinterpret_cast<uintptr_t>(dst) & 7u) == 0;
 #pragma unroll
-              for (int j = 0; j < 32; j += 2) red_add_v2(dst + c0 + j, __uint_as_float(vr[j]), __uint_as_float(vr[j + 1]));
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) atomicAdd(dst + c0 + j, __uint_as_float(vr[j]));
-            }
+          for (int j = 0; j < BNc / 8; ++j) {
+            const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+            if (al8) red_add_v2(dst + 8 * j, v0, v1);
+            else { atomicAdd(dst + 8 * j, v0); atomicAdd(dst + 8 * j + 1, v1); }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
   }
 }
 
@@ -254,7 +187,7 @@ int plan_wgrad(ssdk_ctx* ctx, WgradLaunch& L, const ActBuf& X, const ActBuf& G, 
   a.ci_tiles = X.C / a.BNc;
   a.co_tiles = (G.C + 127) / 128;
   a.a_boxes = G.C <= 64 ? 1 : 2;
-  // pixel patches: bw x bh = 64, bw a multiple of 16 (one UMMA k-step never straddles a patch line)
+  // pixel patches: bw x bh = 64, bw a multiple of 16 (one wgmma k-step never straddles a patch line)
   int best_bw = 16; double best = 1e30;
   for (int bw : {64, 32, 16}) {
     const int bh = 64 / bw;
@@ -266,14 +199,12 @@ int plan_wgrad(ssdk_ctx* ctx, WgradLaunch& L, const ActBuf& X, const ActBuf& G, 
   a.total_patches = G.B * a.px_tiles * a.py_tiles;
   a.g_pad = G.pad;
   a.x_off = X.pad - pad_l; a.y_off = X.pad - pad_t;
-  const int slab_w = a.bw + (KW - 1) * dil;
-  a.slab_bytes = (uint32_t)((a.bh * slab_w * 128 + 1023) / 1024 * 1024);
-  const size_t stage = ((size_t)a.a_boxes * kBoxA + (size_t)(a.BNc / 64) * a.slab_bytes) * (a.split ? 2 : 1);
-  a.tx_bytes = (uint32_t)(((size_t)a.a_boxes * kBoxA + (size_t)(a.BNc / 64) * a.bh * slab_w * 128) * (a.split ? 2 : 1));
+  const size_t stage = ((size_t)2 * kBoxA + (size_t)(a.BNc / 64) * kBoxA) * (a.split ? 2 : 1);
+  a.tx_bytes = (uint32_t)(((size_t)a.a_boxes * kBoxA + (size_t)(a.BNc / 64) * kBoxA) * (a.split ? 2 : 1));
   a.stages = (int)std::min<size_t>(6, (220 * 1024) / stage);
   if (a.stages < 2) { set_error("wgrad: stage of %zu bytes does not fit twice in shared memory", stage); return SSDK_ERR_UNSUPPORTED; }
   L.smem = 1024 + stage * a.stages + 256;
-  const int base_units = a.co_tiles * a.ci_tiles * KH;
+  const int base_units = a.co_tiles * a.ci_tiles * KH * KW;
   int ks = std::max(1, (2 * ctx->sm_count + base_units - 1) / base_units);
   ks = std::min(ks, std::max(1, a.total_patches / 4));
   a.patches_per_split = (a.total_patches + ks - 1) / ks;
@@ -283,7 +214,7 @@ int plan_wgrad(ssdk_ctx* ctx, WgradLaunch& L, const ActBuf& X, const ActBuf& G, 
   const uint64_t gd[4] = {(uint64_t)G.Cs, (uint64_t)G.Wp(), (uint64_t)G.Hp(), (uint64_t)G.B};
   const uint64_t xd[4] = {(uint64_t)X.Cs, (uint64_t)X.Wp(), (uint64_t)X.Hp(), (uint64_t)X.B};
   const uint32_t gb[4] = {64, (uint32_t)a.bw, (uint32_t)a.bh, 1};
-  const uint32_t xb[4] = {64, (uint32_t)slab_w, (uint32_t)a.bh, 1};
+  const uint32_t xb[4] = {64, (uint32_t)a.bw, (uint32_t)a.bh, 1};
   int rc = make_tmap_4d(&L.g_hi, G.hi, gd, gb); if (rc) return rc;
   rc = make_tmap_4d(&L.x_hi, X.hi, xd, xb); if (rc) return rc;
   if (a.split) {
@@ -294,13 +225,22 @@ int plan_wgrad(ssdk_ctx* ctx, WgradLaunch& L, const ActBuf& X, const ActBuf& G, 
   return SSDK_OK;
 }
 
-int launch_wgrad(ssdk_ctx* ctx, const WgradLaunch& L, cudaStream_t stream) {
+template <int BNc, bool SPLIT>
+static int launch_wgrad_bn(const WgradLaunch& L, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_tcgen05_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<BNc, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  wgrad_tcgen05_kernel<<<L.grid, 256, L.smem, stream>>>(L.g_hi, L.g_lo, L.x_hi, L.x_lo, L.args);
+  wgrad_wgmma_kernel<BNc, SPLIT><<<L.grid, 256, L.smem, stream>>>(L.g_hi, L.g_lo, L.x_hi, L.x_lo, L.args);
+  return SSDK_OK;
+}
+
+int launch_wgrad(ssdk_ctx* ctx, const WgradLaunch& L, cudaStream_t stream) {
+  const bool sp = L.args.split != 0;
+  const int rc = L.args.BNc == 128 ? (sp ? launch_wgrad_bn<128, true>(L, stream) : launch_wgrad_bn<128, false>(L, stream))
+                                   : (sp ? launch_wgrad_bn<64, true>(L, stream) : launch_wgrad_bn<64, false>(L, stream));
+  if (rc) return rc;
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

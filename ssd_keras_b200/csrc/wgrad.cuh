@@ -1,4 +1,4 @@
-// Interface of the tcgen05 weight-gradient kernel (wgrad.cu) used by train.cu.
+// Interface of the wgmma weight-gradient kernel (wgrad.cu) used by train.cu.
 #pragma once
 #include "conv.cuh"
 
@@ -7,12 +7,11 @@ namespace ssdk {
 struct WgradArgs {
   int KH, KW, dil, split;
   int cin, cout, taps;
-  int BNc;                 // input channels per accumulator (64 or 128); KW accumulators side by side in TMEM
+  int BNc;                 // input channels per tile (64 or 128: the wgmma N)
   int ci_tiles, co_tiles, a_boxes;
   int bw, bh;              // pixel patch of one K-block (bw * bh = 64)
   int px_tiles, py_tiles, total_patches;
-  int g_pad, x_off, y_off; // TMA coordinates: dZ box at (x0 + g_pad, y0 + g_pad), X slab at (x0 + x_off, y0 + kh*dil + y_off)
-  uint32_t slab_bytes;     // one 64-channel X slab in shared memory (rounded up to the 1024-byte swizzle atom)
+  int g_pad, x_off, y_off; // TMA coordinates: dZ box at (x0 + g_pad, y0 + g_pad), X box at (x0 + kw*dil + x_off, y0 + kh*dil + y_off)
   uint32_t tx_bytes;       // bytes one stage's TMA loads deliver
   int stages;
   int k_split, patches_per_split;

@@ -1,4 +1,4 @@
-"""``Evaluator`` on B200 (reference ``eval_utils/average_precision_evaluator.py:36-905``): Pascal-VOC average precision.
+"""``Evaluator`` on H100 (reference ``eval_utils/average_precision_evaluator.py:36-905``): Pascal-VOC average precision.
 
 The expensive step of the reference is ``match_predictions`` (:538-736): for every class, a Python loop over all predictions in
 descending confidence with an element-wise ``iou`` against the ground truth of the prediction's image.  Here it is two stable

@@ -1,4 +1,4 @@
-"""``DecodeDetections`` on B200 (reference ``keras_layers/keras_layer_DecodeDetections.py:27-283``):
+"""``DecodeDetections`` on H100 (reference ``keras_layers/keras_layer_DecodeDetections.py:27-283``):
 a callable with the reference layer's constructor arguments; ``layer(y_pred)`` maps a float32 CUDA
 tensor ``(B, P, C+12)`` to ``(B, top_k, 6)`` rows ``[class_id, confidence, xmin, ymin, xmax, ymax]``,
 sorted by confidence and zero padded, through ``ssdk_decode`` (``csrc/decode.cu``)."""

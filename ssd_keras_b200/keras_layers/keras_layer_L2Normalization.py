@@ -1,4 +1,4 @@
-"""``L2Normalization`` on B200 (reference ``keras_layers/keras_layer_L2Normalization.py:25-70``):
+"""``L2Normalization`` on H100 (reference ``keras_layers/keras_layer_L2Normalization.py:25-70``):
 ``x * rsqrt(max(sum_c x^2, 1e-12)) * gamma_c`` over the channel axis of an NHWC tensor, computed by
 ``ssdk_l2_normalize`` (``l2norm_f32_kernel`` in ``csrc/conv.cu``).  Inside ``ssd_300`` / ``ssd_512`` the same
 arithmetic runs on the split-bf16 activation planes (``l2norm_kernel``)."""

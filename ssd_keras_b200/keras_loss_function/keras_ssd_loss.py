@@ -1,4 +1,4 @@
-"""``SSDLoss`` on B200 (reference ``keras_loss_function/keras_ssd_loss.py:22-211``), computed by
+"""``SSDLoss`` on H100 (reference ``keras_loss_function/keras_ssd_loss.py:22-211``), computed by
 ``csrc/loss.cu``.  ``compute_loss`` takes / returns torch CUDA tensors (NumPy arrays are accepted and
 copied) and is differentiable with respect to ``y_pred`` through a ``torch.autograd.Function`` whose
 backward is the hand-written ``ssdk_ssd_loss_bwd`` kernel.

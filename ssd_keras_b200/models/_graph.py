@@ -1,7 +1,7 @@
 """Host-side graph description shared by ``ssd_300`` / ``ssd_512`` / ``build_model``.
 
 The builders mirror the reference functions' arguments and produce an ``SSDModel`` whose forward pass
-is a static plan of hand-written sm_100a kernels inside libssdk.so (``ssdk_model_*``).  The object offers
+is a static plan of hand-written sm_90a kernels inside libssdk.so (``ssdk_model_*``).  The object offers
 the part of the Keras ``Model`` surface that the reference's callers use: ``predict``, ``get_layer(name)
 .output_shape``, ``load_weights`` / ``set_weights`` / ``get_weights``.
 """

@@ -1,7 +1,7 @@
-"""``ssd_300`` on B200 -- same signature as the reference builder (``models/keras_ssd300.py:31-59``).
+"""``ssd_300`` on H100 -- same signature as the reference builder (``models/keras_ssd300.py:31-59``).
 
 Returns an ``SSDModel`` (see ``_graph.py``) instead of a Keras ``Model``: VGG-16 (atrous fc6/fc7) + extra
-layers + L2Normalization + six fused conf/loc predictor heads, executed as tcgen05 implicit-GEMM kernels."""
+layers + L2Normalization + six fused conf/loc predictor heads, executed as wgmma implicit-GEMM kernels."""
 
 from .. import _ffi
 from ._graph import SSDModel, Spec, records_config, resolve_box_args, same_pad, tf_same_pool_pad

@@ -1,4 +1,4 @@
-"""``ssd_512`` on B200 -- same signature as the reference builder (``models/keras_ssd512.py:31-60``):
+"""``ssd_512`` on H100 -- same signature as the reference builder (``models/keras_ssd512.py:31-60``):
 the SSD300 graph with seven predictor layers (extra stride-2 stages and the 4x4 'valid' conv10_2, :312-321)."""
 from ._graph import SSDModel, records_config, resolve_box_args
 from .keras_ssd300 import _extra, _finish, _input_spec, _vgg_base

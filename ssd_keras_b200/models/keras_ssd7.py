@@ -1,4 +1,4 @@
-"""``build_model`` (SSD7) on B200 -- same signature as the reference builder (``models/keras_ssd7.py:30-53``);
+"""``build_model`` (SSD7) on H100 -- same signature as the reference builder (``models/keras_ssd7.py:30-53``);
 ``ssd_7`` is an alias.  Seven conv + BatchNormalization(eps 1e-3, folded) + ELU stages with 'valid' 2x2 pools and
 four predictor heads on conv4..conv7 (:277-331)."""
 from .. import _ffi

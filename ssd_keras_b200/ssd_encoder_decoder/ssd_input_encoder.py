@@ -1,4 +1,4 @@
-"""``SSDInputEncoder`` on B200: same constructor / call surface as the reference class
+"""``SSDInputEncoder`` on H100: same constructor / call surface as the reference class
 (``ssd_encoder_decoder/ssd_input_encoder.py:36-57, 277``), computed by the CUDA kernels in
 ``csrc/encode.cu`` through ``ssdk_encode``.  Host side is argument validation and packing only.
 """

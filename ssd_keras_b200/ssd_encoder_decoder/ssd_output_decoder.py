@@ -1,4 +1,4 @@
-"""``decode_detections`` / ``decode_detections_fast`` on B200 (reference
+"""``decode_detections`` / ``decode_detections_fast`` on H100 (reference
 ``ssd_encoder_decoder/ssd_output_decoder.py:111-333``), computed by ``csrc/decode.cu`` through ``ssdk_decode``.
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-"""Training step on B200: what ``model.compile(optimizer=SGD(lr, momentum), loss=SSDLoss().compute_loss)`` +
+"""Training step on H100: what ``model.compile(optimizer=SGD(lr, momentum), loss=SSDLoss().compute_loss)`` +
 ``train_on_batch`` do in the reference (``ssd300_training.ipynb:169-173``), through ``ssdk_train_backward`` /
 ``ssdk_train_apply`` (``csrc/train.cu``).  Data-parallel: every rank runs the same step on its shard and the flat
 gradient buffer is summed with ONE NCCL all-reduce before the update (replica-local loss, SURVEY.md section 8e(i)).
@@ -149,9 +149,9 @@ class SSDTrainer:
         """forward + loss + backward + gradient exchange + SGD update.  Returns the per-image loss tensor (B,).
         With several ranks the flat gradient buffer is all-reduced either in buckets, from the top of the network down, each as
         soon as its layers have been differentiated (NCCL on its own stream under the weight / data gradient kernels of the lower
-        layers), or in one call after the backward pass.  ``overlap=None`` picks: measured on B200 at 2 ranks the whole 105 MB
-        exchange costs 0.5 ms alone while NCCL's kernels delay the persistent 148-CTA conv launches by more than that when they
-        run side by side, so the bucketed exchange is used from 4 ranks on (SSDK_GRAD_OVERLAP=0/1 overrides; SSDK_OVERLAP is the two-stream schedule of inference plans)."""
+        layers), or in one call after the backward pass.  ``overlap=None`` picks: at 2 ranks the whole exchange is short while
+        NCCL's kernels share the SMs with the persistent (one CTA per SM) conv launches when they run side by side, so the
+        bucketed exchange is used from 4 ranks on (SSDK_GRAD_OVERLAP=0/1 overrides; SSDK_OVERLAP is the two-stream schedule of inference plans)."""
         import os
         import torch.distributed as dist
         on = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): CUDA encode / decode / loss / IoU through the C-ABI,
+"""GPU parity tests (run with -m gpu on an H100): CUDA encode / decode / loss / IoU through the C-ABI,
 checked against the oracle and the committed golden fixtures.  Bars: bit-exact for match assignments, class
 ids and NMS survivor indices; 1e-6..1e-4 relative (stated per test) for float32 coordinates and losses."""
 import numpy as np

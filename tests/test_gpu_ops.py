@@ -1,5 +1,5 @@
 """GPU tests for the stand-alone layer calls ``ssdk_conv2d_fwd`` / ``ssdk_maxpool`` (SURVEY 8b) through ``ssd_keras_b200.ops``:
-the same tcgen05 plan the model graphs use, run as a one-layer graph, against float64 torch-CPU references of the Keras layers
+the same wgmma plan the model graphs use, run as a one-layer graph, against float64 torch-CPU references of the Keras layers
 (``Conv2D`` / ``MaxPooling2D`` as used in models/keras_ssd300.py:274-335).  Tolerance of the bf16x3 convolution: 1e-4 of the
 tensor's max magnitude (the bar of tests/test_gpu_model.py); max-pooling of bf16-exact inputs is exact."""
 import numpy as np

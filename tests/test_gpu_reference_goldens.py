@@ -87,7 +87,7 @@ def _vgg_w(seed, variant, n_cls):
 
 def _close_to_builder(y, rows, colsum, stride):
     """Element-wise: the oracle's own pin against the builders is rtol 2e-3 / atol 1e-4 (two float32 evaluation orders through
-    ~23 layers); the tcgen05 path adds its own <= 1.5e-4 on the probabilities (tests/test_gpu_model.py), hence atol 3e-4.
+    ~23 layers); the wgmma path adds its own <= 1.5e-4 on the probabilities (tests/test_gpu_model.py), hence atol 3e-4.
     Column sums over all P rows: the bf16x3 accumulation error is systematic (truncating fp32 adds), so it does not average
     out -- bounded by 3e-5 per row on top of the float32 summation noise."""
     np.testing.assert_allclose(y[:, ::stride], rows, rtol=2e-3, atol=3e-4)

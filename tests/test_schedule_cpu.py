@@ -1,5 +1,5 @@
 """Host logic of the two-stream schedule of inference plans (csrc/model.cu: overlap_assign, exported as ssdk_schedule_preview), on the
-launch grids of the SSD300 batch-32 plan (profiles/r02_launches_step_final.csv) and on edge cases.  No device needed."""
+launch grids of an SSD300 batch-32 plan on a 148-SM device and on edge cases.  No device needed."""
 import ctypes as C
 
 import numpy as np

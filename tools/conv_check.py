@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Debug harness for the tcgen05 conv path: small graphs, every layer compared with torch-CPU float32.
+"""Debug harness for the wgmma conv path: small graphs, every layer compared with torch-CPU float32.
 Each case runs in its own process so that a device trap in one case cannot poison the others.
 Usage (GPU box):  python tools/conv_check.py            # all cases
                   python tools/conv_check.py --case 3   # one case, in-process

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Encoder timing sweep (one B200): config 5 (P=1e5, G=128, B=256) and config 3 (SSD300, B=32, G=8) over the tile-set /
+"""Encoder timing sweep (one GPU): config 5 (P=1e5, G=128, B=256) and config 3 (SSD300, B=32, G=8) over the tile-set /
 tiles-per-CTA knobs.  CUDA events around back-to-back calls into a preallocated output; prints one JSON line per variant."""
 import json
 import os
