@@ -355,6 +355,31 @@ int ssdk_model_flops(const ssdk_model* m, double* out_algorithmic, double* out_i
 int ssdk_model_set_timing(ssdk_model* m, int enable);
 int ssdk_model_last_conv_ms(ssdk_model* m, float* out_ms);
 
+/* Read-only view of the launch plan ssdk_model_create chose for one convolution or head (host only, no device work), so that a
+ * test can pin the kernel variant it exercises.  Non-convolution layers report kernel = SSDK_PLAN_NONE and zeros. */
+enum ssdk_plan_kernel {
+  SSDK_PLAN_NONE = 0,
+  SSDK_PLAN_GEMM = 1,          /* conv_wgmma_kernel on the zero-bordered activation (implicit GEMM) */
+  SSDK_PLAN_IM2COL_GEMM = 2,   /* im2col_kernel / im2col8_kernel, then conv_wgmma_kernel on the column matrix */
+  SSDK_PLAN_FIRST_TC = 3,      /* conv_first_kernel: image-facing layer, gathered A tile, tensor cores */
+  SSDK_PLAN_DIRECT = 4         /* conv_direct_kernel: fp32 FMAs on the float32 master kernel */
+};
+enum ssdk_plan_epilogue { SSDK_PLAN_EPI_SPLIT = 0, SSDK_PLAN_EPI_F32 = 1, SSDK_PLAN_EPI_ATOMIC = 2, SSDK_PLAN_EPI_HEAD = 3 };
+typedef struct ssdk_layer_plan {
+  int kernel;                  /* ssdk_plan_kernel */
+  int bn;                      /* wgmma N of the tile (GEMM / FIRST_TC) */
+  int split;                   /* 1: bf16x3 (hi*hi + hi*lo + lo*hi), 0: one bf16 product */
+  int stages;                  /* TMA ring depth (GEMM) */
+  int kblocks;                 /* 64-wide K blocks per tap (GEMM: of the input channels or of the im2col row; FIRST_TC: of taps*4) */
+  int n_tiles_m, n_tiles_n;    /* scheduled 128-row m-tiles and BN-wide n-tiles */
+  int grid;                    /* CTAs of the (persistent) launch */
+  int k_split;                 /* work units per tile along K */
+  int epilogue;                /* ssdk_plan_epilogue, of GEMM launches */
+  int head_fused;              /* 1: softmax / anchors / variances in the GEMM epilogue, straight into y_pred */
+  int im2col_vec8;             /* IM2COL_GEMM: 1 = im2col8_kernel (8 channels per thread), 0 = im2col_kernel */
+} ssdk_layer_plan;
+int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_plan* out);
+
 /* ------------------------------------------------------------------------------------------
  * Training step (BASELINE config 3).  Replaces what Keras/TensorFlow do for the reference in model.fit_generator:
  * autodiff of the graph (models/keras_ssd300.py:263-419) and of SSDLoss (keras_ssd_loss.py:98-211), the kernel_regularizer
@@ -398,6 +423,30 @@ int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, float beta2, f
 int ssdk_trainer_read_bn_stats(ssdk_trainer* t, int layer, float* mean_dev, float* var_dev, void* stream);
 /* Copy the current float32 master parameters (same order / layout as the gradients) to out_dev. */
 int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream);
+
+/* Read-only view of the backward launches ssdk_trainer_create planned for one convolution or head (host only). */
+enum ssdk_dgrad_path { SSDK_DGRAD_NONE = 0, SSDK_DGRAD_GEMM = 1 /* implicit GEMM into the producer's gradient planes */,
+                       SSDK_DGRAD_STRIDED = 2 /* GEMM to an fp32 column matrix, then col2im */ };
+enum ssdk_wgrad_path { SSDK_WGRAD_NONE = 0, SSDK_WGRAD_NATIVE = 1 /* wgrad_wgmma_kernel on dZ / X in place */,
+                       SSDK_WGRAD_TRANSPOSED = 2 /* one GEMM per tap on transposed copies of dZ / X */,
+                       SSDK_WGRAD_IM2COL = 3 /* one GEMM on transposed copies of dZ and the im2col matrix */,
+                       SSDK_WGRAD_DIRECT = 4 /* fp32 image-facing weight-gradient kernel */ };
+typedef struct ssdk_backward_plan {
+  int dgrad;                   /* ssdk_dgrad_path */
+  int dgrad_bn;                /* wgmma N of the data-gradient GEMM */
+  int dgrad_mask;              /* 1: ReLU'(producer output) applied in the epilogue */
+  int dgrad_accumulate;        /* 1: added to a gradient another consumer of the producer already wrote */
+  int dgrad_n_tiles_m, dgrad_n_tiles_n, dgrad_grid;
+  int wgrad;                   /* ssdk_wgrad_path */
+  int wgrad_bn;                /* NATIVE: input channels per tile (BNc); TRANSPOSED / IM2COL: GEMM tile width */
+  int a_boxes;                 /* NATIVE: 64-row output-channel boxes per tile */
+  int bw, bh;                  /* NATIVE: pixel patch of one K block (bw * bh = 64) */
+  int co_tiles, ci_tiles;      /* NATIVE: output- / input-channel tiles */
+  int k_split;                 /* work units per tile along the pixel axis */
+  int n_gemms;                 /* TRANSPOSED / IM2COL: GEMM launches */
+  int stages, grid;
+} ssdk_backward_plan;
+int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_backward_plan* out);
 
 #ifdef __cplusplus
 }

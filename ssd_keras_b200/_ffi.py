@@ -74,7 +74,44 @@ class ModelDesc(C.Structure):
                 ('precision', C.c_int), ('anchors_f32', c_float_p), ('variances', C.c_float * 4), ('training', C.c_int)]
 
 
-OP_INPUT, OP_CONV, OP_MAXPOOL, OP_L2NORM, OP_HEAD = range(5)
+class LayerPlan(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ('kernel', 'bn', 'split', 'stages', 'kblocks', 'n_tiles_m', 'n_tiles_n', 'grid', 'k_split',
+                                       'epilogue', 'head_fused', 'im2col_vec8')]
+
+
+class TrainerLayerPlan(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ('dgrad', 'dgrad_bn', 'dgrad_mask', 'dgrad_accumulate', 'dgrad_n_tiles_m', 'dgrad_n_tiles_n',
+                                       'dgrad_grid', 'wgrad', 'wgrad_bn', 'a_boxes', 'bw', 'bh', 'co_tiles', 'ci_tiles', 'k_split',
+                                       'n_gemms', 'stages', 'grid')]
+
+
+PLAN_KERNELS = {0: None, 1: 'gemm', 2: 'im2col_gemm', 3: 'first_tc', 4: 'direct'}
+PLAN_EPILOGUES = {0: 'split', 1: 'f32', 2: 'atomic', 3: 'head'}
+DGRAD_PATHS = {0: None, 1: 'gemm', 2: 'strided'}
+WGRAD_PATHS = {0: None, 1: 'native', 2: 'transposed', 3: 'im2col', 4: 'direct'}
+
+
+def model_layer_plan(handle, layer):
+    """The launch plan of one layer of a model plan, as a dict (ssdk_model_layer_plan)."""
+    p = LayerPlan()
+    check(lib().ssdk_model_layer_plan(handle, int(layer), C.byref(p)))
+    out = {n: getattr(p, n) for n, _ in LayerPlan._fields_}
+    out['kernel'] = PLAN_KERNELS[p.kernel]
+    out['epilogue'] = PLAN_EPILOGUES[p.epilogue]
+    return out
+
+
+def trainer_layer_plan(handle, layer):
+    """The backward launches of one layer of a trainer, as a dict (ssdk_trainer_layer_plan)."""
+    p = TrainerLayerPlan()
+    check(lib().ssdk_trainer_layer_plan(handle, int(layer), C.byref(p)))
+    out = {n: getattr(p, n) for n, _ in TrainerLayerPlan._fields_}
+    out['dgrad'] = DGRAD_PATHS[p.dgrad]
+    out['wgrad'] = WGRAD_PATHS[p.wgrad]
+    return out
+
+
+OP_INPUT, OP_CONV, OP_MAXPOOL, OP_L2NORM, OP_HEAD, OP_TENSOR = range(6)
 ACT_NONE, ACT_RELU, ACT_ELU = range(3)
 
 _lib = None
@@ -145,6 +182,8 @@ def lib():
             L.ssdk_model_flops.argtypes = [vp, c_double_p, c_double_p]
             L.ssdk_model_set_timing.argtypes = [vp, C.c_int]
             L.ssdk_model_last_conv_ms.argtypes = [vp, c_float_p]
+            L.ssdk_model_layer_plan.argtypes = [vp, C.c_int, C.POINTER(LayerPlan)]
+            L.ssdk_model_layer_plan.restype = C.c_int
         if hasattr(L, 'ssdk_trainer_create'):
             L.ssdk_trainer_create.argtypes = [vp, vp, C.POINTER(vp)]
             L.ssdk_trainer_destroy.argtypes = [vp]
@@ -165,6 +204,8 @@ def lib():
             L.ssdk_train_backward_layers.restype = C.c_int
             L.ssdk_train_apply.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, vp]
             L.ssdk_trainer_read_params.argtypes = [vp, vp, vp]
+            L.ssdk_trainer_layer_plan.argtypes = [vp, C.c_int, C.POINTER(TrainerLayerPlan)]
+            L.ssdk_trainer_layer_plan.restype = C.c_int
             for name in ('ssdk_trainer_create', 'ssdk_trainer_destroy', 'ssdk_trainer_num_params', 'ssdk_trainer_param_span',
                          'ssdk_train_backward', 'ssdk_train_apply', 'ssdk_trainer_read_params'):
                 getattr(L, name).restype = C.c_int

@@ -581,10 +581,14 @@ __global__ void im2col8_kernel(ActBuf in, __nv_bfloat16* __restrict__ out_hi, __
   if (out_lo) *reinterpret_cast<uint4*>(out_lo + row * Kpad + k) = l;
 }
 
+bool im2col_vec8_ok(const ActBuf& in, int Kpad, const void* out_hi, const void* out_lo) {
+  return in.C % 8 == 0 && in.Cs == in.C && Kpad % 8 == 0 && (reinterpret_cast<uintptr_t>(out_hi) & 15) == 0 &&
+         (!out_lo || (reinterpret_cast<uintptr_t>(out_lo) & 15) == 0);
+}
+
 int launch_im2col(ssdk_ctx* ctx, const ActBuf& in, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, int Ho, int Wo, int kh, int kw,
-                  int stride, int dil, int pad_t, int pad_l, int Kpad, cudaStream_t stream) {
-  if (in.C % 8 == 0 && in.Cs == in.C && Kpad % 8 == 0 && (reinterpret_cast<uintptr_t>(out_hi) & 15) == 0 &&
-      (!out_lo || (reinterpret_cast<uintptr_t>(out_lo) & 15) == 0)) {
+                  int stride, int dil, int pad_t, int pad_l, int Kpad, bool vec8, cudaStream_t stream) {
+  if (vec8) {
     const size_t total8 = (size_t)in.B * Ho * Wo * (Kpad / 8);
     im2col8_kernel<<<(unsigned)((total8 + 255) / 256), 256, 0, stream>>>(in, out_hi, out_lo, Ho, Wo, kh, kw, stride, dil, pad_t, pad_l, Kpad);
     SSDK_COUNT_LAUNCH(ctx);
@@ -730,6 +734,14 @@ struct FirstArgs {
 };
 
 int first_bn(int cout) { return cout <= 64 ? 64 : 128; }
+FirstPlan first_plan(const ActBuf& out, int kh, int kw, int sm_count) {
+  FirstPlan fp;
+  fp.BN = first_bn(out.C);
+  fp.kblocks = (kh * kw * 4 + 63) / 64;
+  fp.n_tiles = (int)(((long long)out.B * out.H * out.W + kBM - 1) / kBM);
+  fp.grid = std::min(fp.n_tiles, sm_count);
+  return fp;
+}
 static size_t first_smem_bytes(int kblocks, int BN, int split) {
   return 1024 + ((size_t)kblocks * kATile + (size_t)kblocks * BN * 128) * (split ? 2 : 1) + acc_tile_bytes(BN) + (size_t)3 * BN * sizeof(float);
 }
@@ -873,7 +885,7 @@ static int launch_first_kb(const FirstArgs& fa, int grid, size_t smem, cudaStrea
   return fa.split ? launch_first_bn<BN, 2, true>(fa, grid, smem, stream) : launch_first_bn<BN, 2, false>(fa, grid, smem, stream);
 }
 
-int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
+int launch_conv_first(ssdk_ctx* ctx, const FirstPlan& fp, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
                       const float* bias, const float* bn_scale, const float* bn_shift, int act, int kh, int kw, int dil, int pad_t,
                       int pad_l, cudaStream_t stream) {
   FirstArgs fa;
@@ -885,18 +897,17 @@ int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const 
     const int dy = (t / kw) * dil - pad_t, dx = (t % kw) * dil - pad_l;
     fa.tap_off[t] = (dy * in.Wp() + dx) * in.Cs;
   }
-  const int K = kh * kw * 4;
-  fa.kblocks = (K + 63) / 64;
+  fa.kblocks = fp.kblocks;
   SSDK_REQUIRE(fa.kblocks <= 2, "image-facing convolution: more than 128 K columns");
-  const int BN = first_bn(out.C);
+  const int BN = fp.BN;
   fa.split = (in.lo && w_lo) ? 1 : 0;
   fa.M = (long long)out.B * out.H * out.W; fa.Ho = out.H; fa.Wo = out.W;
-  fa.n_tiles = (int)((fa.M + kBM - 1) / kBM);
+  fa.n_tiles = fp.n_tiles;
   fa.epi.cout = out.C; fa.epi.bias = bias; fa.epi.bn_scale = bn_scale; fa.epi.bn_shift = bn_shift; fa.epi.act = act;
   fa.epi.out_hi = out.hi; fa.epi.out_lo = out.lo; fa.epi.out_Hp = out.Hp(); fa.epi.out_Wp = out.Wp(); fa.epi.out_pad = out.pad; fa.epi.out_Cs = out.Cs;
   const size_t smem = first_smem_bytes(fa.kblocks, BN, fa.split);
   SSDK_REQUIRE(smem <= 227 * 1024, "image-facing convolution: %zu bytes of shared memory", smem);
-  const int grid = std::min(fa.n_tiles, ctx->sm_count);
+  const int grid = fp.grid;
   const int rc = BN == 64 ? launch_first_kb<64>(fa, grid, smem, stream) : launch_first_kb<128>(fa, grid, smem, stream);
   if (rc) return rc;
   SSDK_COUNT_LAUNCH(ctx);

@@ -91,16 +91,22 @@ int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int gri
 // elementwise / data movement kernels
 int launch_preprocess(ssdk_ctx* ctx, const float* images, int B, int H, int W, int Cimg, const float* mean, const float* stddev,
                       const int* swap, const ActBuf& out, cudaStream_t stream);
+// im2col8_kernel (8 channels per thread) applies when the input holds a multiple of 8 channels unpadded and the column planes are
+// 16-byte aligned; decided once when the plan is built, launch_im2col runs the recorded choice
+bool im2col_vec8_ok(const ActBuf& in, int Kpad, const void* out_hi, const void* out_lo);
 int launch_im2col(ssdk_ctx* ctx, const ActBuf& in, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, int Ho, int Wo, int kh, int kw,
-                  int stride, int dil, int pad_t, int pad_l, int Kpad, cudaStream_t stream);
+                  int stride, int dil, int pad_t, int pad_l, int Kpad, bool vec8, cudaStream_t stream);
 int launch_conv_direct(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const float* w, const float* bias, const float* bn_scale,
                        const float* bn_shift, int act, int kh, int kw, int dil, int pad_t, int pad_l, cudaStream_t stream);
 // image-facing layer on the tensor cores (gathered A tile, weights resident in shared memory as a swizzled image)
 int first_tc_supported(int taps, int cin, int cout);
 int first_bn(int cout);     // weight-image rows (wgmma N) of the image-facing layer
+// launch shape of conv_first_kernel, chosen when the plan is built
+struct FirstPlan { int BN = 0, kblocks = 0, n_tiles = 0, grid = 0; };
+FirstPlan first_plan(const ActBuf& out, int kh, int kw, int sm_count);
 bool first_border_ok(const ActBuf& in, int kh, int kw, int dil, int pad_t, int pad_l);
 void first_weight_image(const float* hwio, int taps, int cin, int cout, int BN, int kblocks, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo);
-int launch_conv_first(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
+int launch_conv_first(ssdk_ctx* ctx, const FirstPlan& fp, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
                       const float* bias, const float* bn_scale, const float* bn_shift, int act, int kh, int kw, int dil, int pad_t,
                       int pad_l, cudaStream_t stream);
 int launch_maxpool(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, int kh, int kw, int stride, int pad_t, int pad_l,

@@ -82,8 +82,8 @@ int build_conv(ssdk_model* m, int li) {
     if (!m->training && first_tc_supported(taps, cin, cout) && d.dilation >= 1 && first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l) &&
         !getenv("SSDK_NO_FIRST_TC")) {
       std::vector<uint16_t> whi, wlo;
-      const int K = taps * 4, BN = first_bn(cout);
-      first_weight_image(d.kernel, taps, cin, cout, BN, (K + 63) / 64, whi, wlo);
+      L.first = first_plan(L.out, d.kh, d.kw, m->ctx->sm_count);
+      first_weight_image(d.kernel, taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
       rc = dev_alloc(m, &L.w_hi, whi.size(), false); if (rc) return rc;
       SSDK_CHECK_CUDA(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
       if (m->split) {
@@ -107,6 +107,7 @@ int build_conv(ssdk_model* m, int li) {
     size_t n = (size_t)m->B * Ho * Wo * L.Kpad + 64 * 8;
     int rc = dev_alloc(m, &L.col_hi, n, true); if (rc) return rc;
     if (m->split) { rc = dev_alloc(m, &L.col_lo, n, true); if (rc) return rc; }
+    L.im2col_vec8 = im2col_vec8_ok(ia, L.Kpad, L.col_hi, L.col_lo);
     g.a_hi = L.col_hi; g.a_lo = L.col_lo; g.a_inner = L.Kpad; g.a_rows = (uint64_t)m->B * Ho * Wo;
   } else {
     kblocks = (ia.Cs + 63) / 64;
@@ -473,6 +474,29 @@ extern "C" int ssdk_model_layer_shape(const ssdk_model* m, int layer, int* h, in
   return SSDK_OK;
 }
 
+extern "C" int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_plan* out) {
+  SSDK_REQUIRE(m && out && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_plan: bad argument");
+  memset(out, 0, sizeof(*out));
+  const LayerPlan& L = m->layers[layer];
+  if (L.d.op != SSDK_OP_CONV && L.d.op != SSDK_OP_HEAD) return SSDK_OK;
+  out->split = m->split;
+  if (L.direct && L.first_tc) {
+    out->kernel = SSDK_PLAN_FIRST_TC;
+    out->bn = L.first.BN; out->kblocks = L.first.kblocks;
+    out->n_tiles_m = L.first.n_tiles; out->n_tiles_n = 1;
+    out->grid = L.first.grid; out->k_split = 1;
+    return SSDK_OK;
+  }
+  if (L.direct) { out->kernel = SSDK_PLAN_DIRECT; out->split = 0; return SSDK_OK; }
+  const ConvArgs& a = L.launch.args;
+  out->kernel = L.im2col ? SSDK_PLAN_IM2COL_GEMM : SSDK_PLAN_GEMM;
+  out->bn = a.BN; out->split = a.split; out->stages = a.stages; out->kblocks = a.kblocks;
+  out->n_tiles_m = a.n_tiles_m; out->n_tiles_n = a.n_tiles_n; out->grid = L.launch.grid; out->k_split = a.k_split > 1 ? a.k_split : 1;
+  out->epilogue = a.epi; out->head_fused = L.head_fused ? 1 : 0;
+  out->im2col_vec8 = L.im2col && L.im2col_vec8 ? 1 : 0;
+  return SSDK_OK;
+}
+
 extern "C" int ssdk_model_flops(const ssdk_model* m, double* algo, double* issued) {
   SSDK_REQUIRE(m, "ssdk_model_flops: NULL model");
   if (algo) *algo = m->flops_algo;
@@ -549,7 +573,7 @@ extern "C" int ssdk_model_forward(ssdk_model* m, const float* images_dev, float*
         const LayerPlan& in = m->layers[d.input];
         if (L.direct) {
           if (L.first_tc)
-            rc = launch_conv_first(ctx, in.out, L.out, L.w_hi, L.w_lo, L.bias, L.bn_scale, L.bn_shift, d.act, d.kh, d.kw, d.dilation, d.pad_t,
+            rc = launch_conv_first(ctx, L.first, in.out, L.out, L.w_hi, L.w_lo, L.bias, L.bn_scale, L.bn_shift, d.act, d.kh, d.kw, d.dilation, d.pad_t,
                                    d.pad_l, stream);
           else
           rc = launch_conv_direct(ctx, in.out, L.bn_train ? L.z : L.out, L.w_f32, L.bias, L.bn_scale, L.bn_shift, L.bn_train ? (int)SSDK_ACT_NONE : d.act,
@@ -559,7 +583,7 @@ extern "C" int ssdk_model_forward(ssdk_model* m, const float* images_dev, float*
           break;
         }
         if (L.im2col) {
-          rc = launch_im2col(ctx, in.out, L.col_hi, L.col_lo, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t, d.pad_l, L.Kpad, stream);
+          rc = launch_im2col(ctx, in.out, L.col_hi, L.col_lo, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t, d.pad_l, L.Kpad, L.im2col_vec8, stream);
           if (rc) return rc;
         }
         if (m->timing) cudaEventRecord(L.ev0, stream);

@@ -24,6 +24,8 @@ struct LayerPlan {
   bool im2col = false;
   bool direct = false;                // fp32 SIMT path for the image-facing conv (Cin < 8)
   bool first_tc = false;           // direct layer of an inference plan on the tensor cores (conv_first_kernel)
+  FirstPlan first;                    // its launch shape (first_tc)
+  bool im2col_vec8 = false;           // im2col path: im2col8_kernel rather than im2col_kernel
   float* w_f32 = nullptr;
   int Kpad = 0;
   __nv_bfloat16* col_hi = nullptr; __nv_bfloat16* col_lo = nullptr;

@@ -450,6 +450,7 @@ struct TLayer {
   __nv_bfloat16 *w2_hi = nullptr, *w2_lo = nullptr; size_t w2_krow = 0; int w2_kblocks = 0;
   int* dgrad_tiles = nullptr;
   bool dgrad_strided = false;               // stride != 1: col-gradient GEMM (dZ * W^T) + col2im
+  int dgrad_relu_mask = 0;                  // col2im zeroes the gradient where the ReLU producer's output is <= 0
   float* dcol = nullptr; int dcol_ld = 0;
   // weight gradient
   bool wg_native = false;                   // stride-1 layers: wgrad.cu reads dZ / X in place (no transposed copies)
@@ -500,6 +501,8 @@ int launch_repack(ssdk_ctx* ctx, const float* w, int taps, int cin, int cout, in
 }
 
 bool is_conv(int op) { return op == SSDK_OP_CONV || op == SSDK_OP_HEAD; }
+// graph sources (preprocessed images, or a caller tensor): no producer, no parameters, no gradient
+bool is_source(int op) { return op == SSDK_OP_INPUT || op == SSDK_OP_TENSOR; }
 
 }  // namespace
 
@@ -540,7 +543,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
   for (int i = 0; i < n; ++i) {
     LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
-    if (L.d.op == SSDK_OP_INPUT) continue;
+    if (is_source(L.d.op)) continue;
     ActBuf& g = T.g;
     if (L.d.op == SSDK_OP_HEAD) { g.B = m->B; g.H = L.H; g.W = L.W; g.C = L.C; g.Cs = (L.C + 7) / 8 * 8; g.pad = 1; }
     else { g = L.out; g.hi = nullptr; g.lo = nullptr; }
@@ -556,11 +559,11 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
     LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
     const ssdk_layer_desc& d = L.d;
-    if (d.op == SSDK_OP_INPUT) continue;
+    if (is_source(d.op)) continue;
     const int pi = d.input;
     LayerPlan& PL = m->layers[pi];
     TLayer& PT = t->tl[pi];
-    const bool prod_needs_grad = PL.d.op != SSDK_OP_INPUT;
+    const bool prod_needs_grad = !is_source(PL.d.op);
     if (d.op == SSDK_OP_L2NORM) { rc = t_alloc(t, &T.vgamma, (size_t)L.C, true); if (rc) return fail(rc); }
     if (!is_conv(d.op)) { if (prod_needs_grad) written[pi] = 1; continue; }
     rc = t_alloc(t, &T.vw, (size_t)T.cout * T.taps * T.cin, true); if (rc) return fail(rc);
@@ -577,6 +580,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       if (d.stride != 1) {
         // dCol[M][taps*cin] = dZ[M][cout] * W^T, then col2im
         T.has_dgrad = true; T.dgrad_strided = true;
+        T.dgrad_relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
         const int kcol = T.taps * T.cin;
         T.w2_kblocks = (T.g.Cs + 63) / 64;
         T.w2_krow = (size_t)T.w2_kblocks * 64;
@@ -727,6 +731,37 @@ extern "C" int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int whi
 
 extern "C" float* ssdk_trainer_grad_buffer(ssdk_trainer* t) { return t ? t->grad : nullptr; }
 
+extern "C" int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_backward_plan* out) {
+  SSDK_REQUIRE(t && out && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_layer_plan: bad argument");
+  memset(out, 0, sizeof(*out));
+  const TLayer& T = t->tl[layer];
+  const LayerPlan& L = t->m->layers[layer];
+  if (!is_conv(L.d.op)) return SSDK_OK;
+  if (T.has_dgrad) {
+    const ConvArgs& a = T.dgrad.args;
+    out->dgrad = T.dgrad_strided ? SSDK_DGRAD_STRIDED : SSDK_DGRAD_GEMM;
+    out->dgrad_bn = a.BN;
+    out->dgrad_mask = T.dgrad_strided ? T.dgrad_relu_mask : (a.mask_hi != nullptr);
+    out->dgrad_accumulate = a.accumulate;
+    out->dgrad_n_tiles_m = a.n_tiles_m; out->dgrad_n_tiles_n = a.n_tiles_n; out->dgrad_grid = T.dgrad.grid;
+  }
+  if (L.direct) { out->wgrad = SSDK_WGRAD_DIRECT; return SSDK_OK; }
+  if (T.wg_native) {
+    const WgradArgs& w = T.wg.args;
+    out->wgrad = SSDK_WGRAD_NATIVE;
+    out->wgrad_bn = w.BNc; out->a_boxes = w.a_boxes; out->bw = w.bw; out->bh = w.bh;
+    out->co_tiles = w.co_tiles; out->ci_tiles = w.ci_tiles; out->k_split = w.k_split > 1 ? w.k_split : 1;
+    out->stages = w.stages; out->grid = T.wg.grid;
+    return SSDK_OK;
+  }
+  if (T.wgrad.empty()) return SSDK_OK;
+  const ConvLaunch& c = T.wgrad[0];
+  out->wgrad = L.im2col ? SSDK_WGRAD_IM2COL : SSDK_WGRAD_TRANSPOSED;
+  out->wgrad_bn = c.args.BN; out->k_split = c.args.k_split > 1 ? c.args.k_split : 1;
+  out->n_gemms = (int)T.wgrad.size(); out->stages = c.args.stages; out->grid = c.grid;
+  return SSDK_OK;
+}
+
 namespace {
 
 int do_transpose(ssdk_trainer* t, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int src_ld, long long src_rows, const TMap& mp,
@@ -797,11 +832,11 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
     const ssdk_layer_desc& d = L.d;
-    if (d.op == SSDK_OP_INPUT) continue;
+    if (is_source(d.op)) continue;
     const int pi = d.input;
     LayerPlan& PL = m->layers[pi];
     TLayer& PT = t->tl[pi];
-    const bool prod_needs_grad = PL.d.op != SSDK_OP_INPUT;
+    const bool prod_needs_grad = !is_source(PL.d.op);
     const int relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
     if (d.op == SSDK_OP_HEAD) {
       const size_t total = (size_t)m->B * L.H * L.W * d.n_boxes;
@@ -872,7 +907,7 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       rc = launch_conv(ctx, T.dgrad, s); if (rc) return rc;
       const size_t total = (size_t)PT.g.B * PT.g.H * PT.g.W * PT.g.C;
       col2im_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(T.dcol, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t, d.pad_l, T.dcol_ld,
-                                                                     PL.out, PT.g, relu_mask, written[pi] ? 1 : 0);
+                                                                     PL.out, PT.g, T.dgrad_relu_mask, written[pi] ? 1 : 0);
       SSDK_COUNT_LAUNCH(ctx);
       written[pi] = 1;
     } else if (T.has_dgrad) {

@@ -1,9 +1,20 @@
-"""GPU tests for the stand-alone layer calls ``ssdk_conv2d_fwd`` / ``ssdk_maxpool`` (SURVEY 8b) through ``ssd_keras_b200.ops``:
-the same wgmma plan the model graphs use, run as a one-layer graph, against float64 torch-CPU references of the Keras layers
-(``Conv2D`` / ``MaxPooling2D`` as used in models/keras_ssd300.py:274-335).  Tolerance of the bf16x3 convolution: 1e-4 of the
-tensor's max magnitude (the bar of tests/test_gpu_model.py); max-pooling of bf16-exact inputs is exact."""
+"""GPU tests of the convolution kernels and of the stand-alone layer calls (SURVEY 8b).
+
+Convolutions: every case of tests/conv_cases.py FORWARD_CASES is a one-layer graph whose plan must be the variant the case
+declares (ssdk_model_layer_plan).  Its output is compared element by element with the operand-exact float64 reference of
+oracle/opexact.py: the same bf16 hi / lo split products the kernel issues, with the bound kappa * A + unit * |y_ref| derived
+there (fp32 accumulation plus the output store).  The same comparison is repeated against perturbed references -- a dropped
+cross term, tap, 64-channel k-block or bias -- and each of these must fail, so the bound is tight enough to see a stale ring
+stage or a lost K range.  Set SSDK_KERNEL_ERRORS_LOG to a file name to record every measured ratio (tests/conv_cases.py).
+
+``CASES`` below is kept as a check of the ``ops.conv2d`` API (argument handling, padding modes, the one-layer plan it builds
+and destroys) against plain float64 convolutions at 1e-4 of the tensor's max; the kernels themselves are held to the
+operand-exact bound above.  Max-pooling of bf16-exact inputs is exact."""
 import numpy as np
 import pytest
+
+import conv_cases as cc
+from oracle import opexact
 
 pytestmark = pytest.mark.gpu
 
@@ -29,6 +40,47 @@ def _ref_conv(x, k, b, stride, dil, pads, act):
     elif act == 'elu':
         y = F.elu(y)
     return y.permute(0, 2, 3, 1).numpy()
+
+
+@pytest.mark.parametrize('case', cc.FORWARD_CASES, ids=[c['name'] for c in cc.FORWARD_CASES])
+def test_conv_kernel_variant_within_operand_exact_bound(case, monkeypatch):
+    import torch
+    for k, v in case['env'].items():
+        monkeypatch.setenv(k, v)
+    x, w, b, scale, shift = cc.case_data(case, seed=sum(map(ord, case['name'])))
+    layer = dict(cout=case['cout'], k=case['k'], stride=case['stride'], dil=case['dil'], pads=case['pads'], act=case['act'],
+                 kernel=w, bias=b, bn_scale=scale, bn_shift=shift)
+    g = cc.Graph(case['B'], case['H'], case['W'], case['cin'], [layer], prec=case['prec'])
+    try:
+        plan = g.plan(1)
+        cc.assert_plan(plan, case['expect'], case['name'])
+        if case['persistent']:
+            units = plan['n_tiles_m'] * plan['n_tiles_n'] * plan['k_split']
+            sms = torch.cuda.get_device_properties(0).multi_processor_count
+            assert plan['grid'] == sms and units >= 3 * sms, (plan, sms)
+            nk = case['k'] * case['k'] * plan['kblocks']
+            assert (nk < plan['stages']) if case['persistent'] == 'nk<stages' else (nk % plan['stages'] != 0), (nk, plan)
+        g.forward(x)
+        x_st = g.read(0)                                # the input as conv_direct_kernel reads it (hi + lo, or hi)
+        y = g.read(1)
+    finally:
+        g.close()
+    mode = 'fp32' if plan['kernel'] == 'direct' else case['prec']
+    if mode != 'fp32':
+        x_st = x                                        # the tensor-core kernels read split(x): split the input itself
+    geo = dict(stride=case['stride'], dil=case['dil'], pads=case['pads'], mode=mode, act=case['act'], bn_scale=scale, bn_shift=shift)
+    taps = case['k'] * case['k']
+    y_ref, A, pert = opexact.conv_ref(x_st, w, b, perturb=cc.perturbations(plan, taps, case['cin'], mode == 'bf16x3', b), **geo)
+    n_steps = cc.n_steps_of(plan, taps, case['cin'])
+    store = 'bf16' if case['prec'] == 'bf16' else 'split'
+    bnd = opexact.bound(y_ref, A, n_steps, store)
+    ratio = opexact.err_ratio(y, y_ref, bnd)
+    perturbed = {p[0]: opexact.err_ratio(y, yp, bnd) for p, yp in pert.items()}
+    cc.log_ratio(dict(test='forward', case=case['name'], kernel=plan['kernel'], bn=plan['bn'], split=plan['split'],
+                      ratio=ratio, perturbed=perturbed))
+    assert ratio <= 1.0, (case['name'], ratio)
+    for k, r in perturbed.items():
+        assert r > 1.0, '%s: the bound does not see a dropped %s (ratio %.3g)' % (case['name'], k, r)
 
 
 CASES = [
@@ -75,7 +127,7 @@ def test_conv2d_single_pass_mode_and_errors():
     y1 = ops.conv2d(x, ker, None, precision='bf16').cpu().numpy()
     ref = _ref_conv(x, ker, None, 1, 1, (1, 1, 1, 1), None)
     assert np.abs(y3 - ref).max() / np.abs(ref).max() < 1e-4
-    assert 1e-4 < np.abs(y1 - ref).max() / np.abs(ref).max() < 5e-2          # one bf16 pass: ~3e-3, and really a different path
+    assert np.abs(y1 - ref).max() / np.abs(ref).max() > 1e-4                  # one bf16 pass is really a different path
     with pytest.raises(ValueError):
         ops.conv2d(x, ker[:, :, :8], None)
     with pytest.raises(ValueError):
