@@ -354,6 +354,8 @@ int ssdk_model_flops(const ssdk_model* m, double* out_algorithmic, double* out_i
 /* Time of the conv kernels of the last forward in ms (CUDA events on `stream`), when enabled. */
 int ssdk_model_set_timing(ssdk_model* m, int enable);
 int ssdk_model_last_conv_ms(ssdk_model* m, float* out_ms);
+/* Time in ms of one layer's convolution launch in the last timed forward (0 for layers without a conv_wgmma_kernel launch). */
+int ssdk_model_layer_ms(const ssdk_model* m, int layer, float* out_ms);
 
 /* Read-only view of the launch plan ssdk_model_create chose for one convolution or head (host only, no device work), so that a
  * test can pin the kernel variant it exercises.  Non-convolution layers report kernel = SSDK_PLAN_NONE and zeros. */

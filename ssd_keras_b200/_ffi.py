@@ -182,6 +182,7 @@ def lib():
             L.ssdk_model_flops.argtypes = [vp, c_double_p, c_double_p]
             L.ssdk_model_set_timing.argtypes = [vp, C.c_int]
             L.ssdk_model_last_conv_ms.argtypes = [vp, c_float_p]
+            L.ssdk_model_layer_ms.argtypes = [vp, C.c_int, c_float_p]
             L.ssdk_model_layer_plan.argtypes = [vp, C.c_int, C.POINTER(LayerPlan)]
             L.ssdk_model_layer_plan.restype = C.c_int
         if hasattr(L, 'ssdk_trainer_create'):

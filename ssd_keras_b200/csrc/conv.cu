@@ -2,7 +2,7 @@
 // Reference ops: Conv2D / MaxPooling2D / Lambda preprocessing / L2Normalization / Reshape+softmax+Concat in
 // models/keras_ssd300.py:263-419, keras_layers/keras_layer_L2Normalization.py:61-63.
 //
-// conv_wgmma_kernel -- persistent, 256 threads = two warpgroups (DESIGN.md section "conv"):
+// conv_wgmma_kernel -- persistent, 384 threads = a TMA producer warpgroup + two wgmma consumer warpgroups (DESIGN.md section "conv"):
 //   GEMM view   D[M = output pixels, N = Cout] = sum over (tap, cin-block) A_tap[M, 64] * W_tap[N, 64]^T.
 //   "im2col in the TMA descriptor": the activation tensor is a zero-bordered NHWC buffer viewed as a 2-D
 //   matrix [B*Hp*Wp, C]; the A tile of filter tap (kh, kw) for output rows [m0, m0+128) is simply rows
@@ -10,9 +10,9 @@
 //   padding / dilation come for free (the border is zero, rows past the end are TMA zero-filled).
 //   Outputs are computed for every position of the padded grid ("virtual rows"); the epilogue stores the
 //   valid ones, and m-tiles without any valid row are not scheduled.
-//   One thread issues the TMA loads of a ring of `stages` {A_hi, A_lo, W_hi, W_lo} 128B-swizzled K-major tiles (full / empty
-//   mbarriers); each warpgroup runs wgmma m64nBNk16 on its 64 rows with fp32 accumulators in registers.  After the K loop the
-//   accumulators go through shared memory (over the drained ring) to an epilogue with one thread per row (bias/BN/act -> store).
+//   One producer thread keeps a ring of `stages` {A_hi, A_lo, W_hi, W_lo} 128B-swizzled K-major tiles (full / empty mbarriers)
+//   filled across tile boundaries; each consumer warpgroup runs wgmma m64nBNk16 on its 64 rows with fp32 accumulators in
+//   registers.  Activation outputs are stored from the registers; head / fp32 / atomic outputs go through a shared-memory tile.
 //   Precision: operands are bf16 "hi + lo" pairs; three MMAs per k-step (hi*hi, hi*lo, lo*hi) accumulate
 //   in fp32, which reproduces an fp32 convolution to ~1e-5 relative (split=0 issues hi*hi only).
 #include "conv.cuh"
@@ -166,13 +166,51 @@ __device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, const float
   }
 }
 
-// Epilogue of the activation-producing launches: bias / folded BatchNorm / activation -> bf16 hi+lo planes, 8 channels per
-// 16-byte store.  `acc`, `sb`, `ss`, `sh` and output element `o` all start at this thread's first column.  BWD adds what the
-// data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
+// One group of 8 output channels of the activation-producing epilogues: bias / folded BatchNorm / activation -> bf16 hi+lo planes,
+// one 16-byte store per plane.  `v`, `sb`, `ss`, `sh` and output element `o` start at the group's first column.  BWD adds what
+// the data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
 template <bool BWD>
+__device__ __forceinline__ void epi_split8(const ConvArgs& args, const float* v, size_t o, const float* sb, const float* ss,
+                                           const float* sh) {
+  uint32_t ph[4], pl[4];
+  uint4 mk = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u), oh = make_uint4(0, 0, 0, 0), ol = oh;
+  if (BWD) {
+    if (args.mask_hi) mk = *reinterpret_cast<const uint4*>(args.mask_hi + o);
+    if (args.accumulate) {
+      oh = *reinterpret_cast<const uint4*>(args.out_hi + o);
+      if (args.out_lo) ol = *reinterpret_cast<const uint4*>(args.out_lo + o);
+    }
+  }
+  const uint32_t mkw[4] = {mk.x, mk.y, mk.z, mk.w}, ohw[4] = {oh.x, oh.y, oh.z, oh.w}, olw[4] = {ol.x, ol.y, ol.z, ol.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float f[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int col = j * 2 + e;
+      float xv = v[col] + sb[col];
+      if (args.bn_scale) xv = xv * ss[col] + sh[col];
+      xv = apply_act(xv, args.act);
+      if (BWD) {
+        if (!(__uint_as_float(((mkw[j] >> (e * 16)) & 0xffffu) << 16) > 0.f)) xv = 0.f;       // ReLU'(forward value)
+        xv += __uint_as_float(((ohw[j] >> (e * 16)) & 0xffffu) << 16) + __uint_as_float(((olw[j] >> (e * 16)) & 0xffffu) << 16);
+      }
+      f[e] = xv;
+    }
+    __nv_bfloat16 h0 = __float2bfloat16_rn(f[0]), h1 = __float2bfloat16_rn(f[1]);
+    __nv_bfloat16 l0 = __float2bfloat16_rn(f[0] - __bfloat162float(h0));
+    __nv_bfloat16 l1 = __float2bfloat16_rn(f[1] - __bfloat162float(h1));
+    ph[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
+    pl[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
+  }
+  *reinterpret_cast<uint4*>(args.out_hi + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
+  if (args.out_lo) *reinterpret_cast<uint4*>(args.out_lo + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+}
+
+// Row epilogue of conv_first_kernel (one thread = one row of the shared-memory accumulator tile, `ncols` columns from `acc`).
 __device__ __forceinline__ void epi_split(const ConvArgs& args, const float* acc, int ncols, size_t o, const float* sb,
                                           const float* ss, const float* sh) {
-  if (!BWD && !args.bn_scale && args.act == SSDK_ACT_RELU && args.out_lo) {
+  if (!args.bn_scale && args.act == SSDK_ACT_RELU && args.out_lo) {
     // the common forward case (bias + ReLU, hi/lo planes) without per-element branches: packed conversions (two values per
     // cvt.rn.bf16x2.f32) and biases fetched four at a time.  Bit-identical to the generic path below.
     for (int c0 = 0; c0 < ncols; c0 += 32) {
@@ -218,43 +256,8 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, const float* acc
     float vr[32];
     ld_acc32(acc + c0, vr);
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      if (c0 + g * 8 < ncols) {
-        uint32_t ph[4], pl[4];
-        uint4 mk = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u), oh = make_uint4(0, 0, 0, 0), ol = oh;
-        if (BWD) {
-          if (args.mask_hi) mk = *reinterpret_cast<const uint4*>(args.mask_hi + o + c0 + g * 8);
-          if (args.accumulate) {
-            oh = *reinterpret_cast<const uint4*>(args.out_hi + o + c0 + g * 8);
-            if (args.out_lo) ol = *reinterpret_cast<const uint4*>(args.out_lo + o + c0 + g * 8);
-          }
-        }
-        const uint32_t mkw[4] = {mk.x, mk.y, mk.z, mk.w}, ohw[4] = {oh.x, oh.y, oh.z, oh.w}, olw[4] = {ol.x, ol.y, ol.z, ol.w};
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float f[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int col = c0 + g * 8 + j * 2 + e;
-            float xv = vr[g * 8 + j * 2 + e] + sb[col];
-            if (args.bn_scale) xv = xv * ss[col] + sh[col];
-            xv = apply_act(xv, args.act);
-            if (BWD) {
-              if (!(__uint_as_float(((mkw[j] >> (e * 16)) & 0xffffu) << 16) > 0.f)) xv = 0.f;       // ReLU'(forward value)
-              xv += __uint_as_float(((ohw[j] >> (e * 16)) & 0xffffu) << 16) + __uint_as_float(((olw[j] >> (e * 16)) & 0xffffu) << 16);
-            }
-            f[e] = xv;
-          }
-          __nv_bfloat16 h0 = __float2bfloat16_rn(f[0]), h1 = __float2bfloat16_rn(f[1]);
-          __nv_bfloat16 l0 = __float2bfloat16_rn(f[0] - __bfloat162float(h0));
-          __nv_bfloat16 l1 = __float2bfloat16_rn(f[1] - __bfloat162float(h1));
-          ph[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-          pl[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-        }
-        *reinterpret_cast<uint4*>(args.out_hi + o + c0 + g * 8) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-        if (args.out_lo) *reinterpret_cast<uint4*>(args.out_lo + o + c0 + g * 8) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-      }
-    }
+    for (int g = 0; g < 4; ++g)
+      if (c0 + g * 8 < ncols) epi_split8<false>(args, vr + g * 8, o + c0 + g * 8, sb + c0 + g * 8, ss + c0 + g * 8, sh + c0 + g * 8);
   }
 }
 
@@ -267,15 +270,41 @@ __device__ __forceinline__ void epi_split(const ConvArgs& args, const float* acc
 //            K loop: the large accumulator takes one rounding add per k-step instead of three (deep-K layers: fc6, fc7,
 //            conv6_2 ... stay within 1e-4 of an fp32 convolution).
 enum { kSingle = 0, kSplitXS = 2 };
+static constexpr int kConvThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma consumers of rows [0, 64) / [64, 128)
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the two consumer warpgroups
+
+// The 8 accumulator columns [8j, 8j + 8) of a quad's rows, j = jp + (q & 1), row half h = q >> 1, gathered into lane q (= lane % 4)
+// of the quad: a 4 x 4 transpose of float2 pairs.  Lane p holds columns 8j + 2p + {0, 1} of rows r and r + 8 (d[4j + 2h + e]).
+template <int N>
+__device__ __forceinline__ void quad_gather8(const float (&acc)[N], int jp, int q, float (&v)[8]) {
+  const float2 c00 = make_float2(acc[4 * jp], acc[4 * jp + 1]), c01 = make_float2(acc[4 * jp + 2], acc[4 * jp + 3]);
+  const float2 c10 = make_float2(acc[4 * jp + 4], acc[4 * jp + 5]), c11 = make_float2(acc[4 * jp + 6], acc[4 * jp + 7]);
+  float2 rcv[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const int u = q ^ r;                                                   // the unit 2h + jj that lane q ^ r gathers
+    const float2 s = (u & 1) ? ((u & 2) ? c11 : c10) : ((u & 2) ? c01 : c00);
+    rcv[r].x = __shfl_xor_sync(0xffffffffu, s.x, r);
+    rcv[r].y = __shfl_xor_sync(0xffffffffu, s.y, r);
+  }
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {                                            // columns 2p, 2p + 1 came from lane p = q ^ r
+    const int r = q ^ p;
+    const float2 t = r == 0 ? rcv[0] : (r == 1 ? rcv[1] : (r == 2 ? rcv[2] : rcv[3]));
+    v[2 * p] = t.x; v[2 * p + 1] = t.y;
+  }
+}
+
 template <int BN, int MODE>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                   const __grid_constant__ ConvArgs args) {
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
-  const int tid = threadIdx.x, wg = tid >> 7, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
   constexpr bool split = MODE == kSplitXS;
   const int S = args.stages;
   constexpr uint32_t kBTile = (uint32_t)BN * kBK * 2;
@@ -285,59 +314,93 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const uint32_t bar_base = smem_base + ring;
   auto full = [&](uint32_t s) { return bar_base + 8u * s; };
   auto empty = [&](uint32_t s) { return bar_base + 8u * ((uint32_t)S + s); };
-  float* s_acc = reinterpret_cast<float*>(smem_al);                       // after the main loop of a tile: [128][BN + kAccPad]
+  const uint32_t staged_free = bar_base + 16u * (uint32_t)S;              // staged epilogues: the tile over the ring has been read
+  float* s_acc = reinterpret_cast<float*>(smem_al);                       // staged epilogues, after a tile's K loop: [128][BN + kAccPad]
   float* s_bias = reinterpret_cast<float*>(smem_al + ring + 256);
   float* s_scale = s_bias + BN;
   float* s_shift = s_scale + BN;
+  // EPI_SPLIT stores from the accumulator registers; the other epilogues go through a shared-memory tile over the ring, so the
+  // producer holds the next tile's loads until that tile has been read
+  const bool staged = args.epi != EPI_SPLIT;
 
   if (tid == 0) {
     prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_b_hi);
     if (split) { prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_lo); }
-    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }   // empty: one arrival per warp
+    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }   // empty: one arrival per consumer warp
+    mbar_init(staged_free, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   const int KS = args.k_split > 1 ? args.k_split : 1;
   const int total_tiles = args.n_tiles_m * args.n_tiles_n * KS;
-  uint32_t g = 0;                                                          // ring uses so far (slot = g % S, phase = g / S)
+  // work unit t -> output rows [m0, m0 + 128), columns [n0, n0 + BN), k-blocks [kb0, kb0 + nkb), nk = taps * nkb k-iterations
+  auto unit = [&](int t, int& m0, int& n0, int& kb0, int& nkb) {
+    const int tt = t / KS, ks = t - tt * KS;
+    m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
+    n0 = (tt % args.n_tiles_n) * BN;
+    kb0 = KS > 1 ? ks * args.kb_per : 0;
+    const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
+    nkb = kb1 - kb0;
+  };
+
+  if (wg == 0) {
+    // ===================== producer: one thread walks the tile schedule and keeps the ring full across tile boundaries =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (tid != 0) return;
+    uint32_t g = 0;                                                        // ring uses so far (slot = g % S, phase = g / S)
+    uint32_t lt = 0;                                                       // tiles of this CTA so far
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
+      int m0, n0, kb0, nkb;
+      unit(t, m0, n0, kb0, nkb);
+      const int nk = args.KH * args.KW * nkb;
+      if (staged && lt > 0) mbar_wait(staged_free, (lt - 1) & 1u);
+      // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +128) of the activation matrix
+      for (int i = 0; i < nk; ++i) {
+        const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
+        mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
+        const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
+        const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
+        const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
+        const uint32_t dst = smem_base + stage * s;
+        mbar_expect_tx(full(s), stage);
+        tma_load_2d(dst, &tm_a_hi, kb * kBK, row, full(s));
+        tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, full(s));
+        if (split) {
+          tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, full(s));
+          tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, full(s));
+        }
+      }
+      g += (uint32_t)nk;
+    }
+    return;
+  }
+
+  // ===================== consumers: warpgroup cw computes rows [64 cw, +64) of every tile =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1, ctid = tid - 128, cwarp = (tid >> 5) & 3;
+  uint32_t g = 0;
   float acc[BN / 2], accx[split ? BN / 2 : 1];
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-    const int tt = t / KS, ks = t - tt * KS;
-    const int m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
-    const int n0 = (tt % args.n_tiles_n) * BN;
-    const int kb0 = KS > 1 ? ks * args.kb_per : 0;
-    const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
-    const int nkb = kb1 - kb0, nk = args.KH * args.KW * nkb;
-    for (int i = tid; i < BN; i += blockDim.x) {
-      const int col = n0 + i;
-      s_bias[i] = (args.bias && col < args.cout) ? args.bias[col] : 0.f;
-      if (args.bn_scale) { s_scale[i] = col < args.cout ? args.bn_scale[col] : 0.f; s_shift[i] = col < args.cout ? args.bn_shift[col] : 0.f; }
-    }
-    // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +128) of the activation matrix
-    auto issue = [&](int i) {
-      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
-      mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
-      const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
-      const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
-      const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
-      const uint32_t dst = smem_base + stage * s;
-      mbar_expect_tx(full(s), stage);
-      tma_load_2d(dst, &tm_a_hi, kb * kBK, row, full(s));
-      tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, full(s));
-      if (split) {
-        tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, full(s));
-        tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, full(s));
+    int m0, n0, kb0, nkb;
+    unit(t, m0, n0, kb0, nkb);
+    const int nk = args.KH * args.KW * nkb;
+    if (staged)
+      for (int i = ctid; i < BN; i += 256) {
+        const int col = n0 + i;
+        s_bias[i] = (args.bias && col < args.cout) ? args.bias[col] : 0.f;
+        if (args.bn_scale) { s_scale[i] = col < args.cout ? args.bn_scale[col] : 0.f; s_shift[i] = col < args.cout ? args.bn_shift[col] : 0.f; }
       }
-    };
-    // k-iteration j's MMAs are done: its stage goes back to the producer, which refills it with k-iteration j + S
+    // k-iteration j's MMAs are done: its stage goes back to the producer
     auto release = [&](int j) {
       __syncwarp();
       if (lane == 0) mbar_arrive(empty((g + (uint32_t)j) % (uint32_t)S));
-      if (tid == 0 && j + S < nk) issue(j + S);
     };
-    if (tid == 0)
-      for (int i = 0; i < min(S, nk); ++i) issue(i);
+    // (the first k-step overwrites the accumulators; zeroing them here only ends their live range at the previous epilogue)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (split ? BN / 2 : 1); ++j) accx[j] = 0.f;
     wgmma_fence_acc(acc);
     wgmma_fence_acc(accx);
     // Every k-iteration issues all 4 k-steps of its 64-channel block: past the last real channel the A tile is TMA zero fill (or
@@ -346,7 +409,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     for (int i = 0; i < nk; ++i) {
       const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
       mbar_wait(full(s), (gi / (uint32_t)S) & 1u);
-      const uint32_t a_hi = smem_base + stage * s + (uint32_t)wg * (kATile / 2), b_hi = smem_base + stage * s + b_off;
+      const uint32_t a_hi = smem_base + stage * s + (uint32_t)cw * (kATile / 2), b_hi = smem_base + stage * s + b_off;
       constexpr uint64_t kDesc = wgmma_desc_hi(16);
       wgmma_fence();
 #pragma unroll
@@ -372,12 +435,50 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 #pragma unroll
       for (int j = 0; j < BN / 2; ++j) acc[j] += accx[j];
     }
+    const int ncols = min(BN, args.cout - n0);
 
-    // ===================== epilogue: registers -> shared-memory tile -> one thread per row (and half of the columns) =====
-    __syncthreads();                                                       // both warpgroups are done with the ring
-    store_acc_tile<BN>(acc, s_acc, wg, warp, lane);
-    __syncthreads();
-    const int r = tid & (kBM - 1), half = tid >> 7;
+    if (!staged) {
+      // ===================== EPI_SPLIT from the registers: a quad exchange gives each lane 8 consecutive columns of one row ====
+      const int q = lane & 3;
+      const int v = m0 + cw * 64 + cwarp * 16 + (lane >> 2) + 8 * (q >> 1);   // virtual row of this lane's stores
+      bool valid = v < args.M_total;
+      int n = 0, y = 0, x = 0;
+      if (valid) {
+        n = v / args.rows_per_img;
+        const int rr = v - n * args.rows_per_img;
+        y = rr / args.in_Wp;
+        x = rr - y * args.in_Wp;
+        valid = (y < args.Ho) && (x < args.Wo);
+      }
+      const size_t o_row = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + n0;
+      const bool bwd = args.mask_hi || args.accumulate;
+#pragma unroll
+      for (int jp = 0; jp < BN / 8; jp += 2) {
+        float vr[8];
+        quad_gather8(acc, jp, q, vr);
+        const int c0 = 8 * (jp + (q & 1));
+        if (valid && c0 < ncols) {
+          float sb[8], ss[8], sh[8];
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            const int col = n0 + c0 + e;
+            const bool in = col < args.cout;
+            sb[e] = (args.bias && in) ? __ldg(args.bias + col) : 0.f;
+            ss[e] = (args.bn_scale && in) ? __ldg(args.bn_scale + col) : 0.f;
+            sh[e] = (args.bn_scale && in) ? __ldg(args.bn_shift + col) : 0.f;
+          }
+          if (bwd) epi_split8<true>(args, vr, o_row + c0, sb, ss, sh);
+          else epi_split8<false>(args, vr, o_row + c0, sb, ss, sh);
+        }
+      }
+      continue;
+    }
+
+    // ===================== staged epilogues: registers -> shared-memory tile -> one thread per row (and half of the columns) ==
+    consumer_sync();                                                       // both warpgroups are done with the ring
+    store_acc_tile<BN>(acc, s_acc, cw, cwarp, lane);
+    consumer_sync();
+    const int r = ctid & (kBM - 1), half = ctid >> 7;
     const int v = m0 + r;                                                  // virtual row of this thread
     bool valid = v < args.M_total;
     int n = 0, y = 0, x = 0;
@@ -389,7 +490,6 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       valid = (y < args.Ho) && (x < args.Wo);
     }
     const float* arow = s_acc + (size_t)r * (BN + kAccPad);
-    const int ncols = min(BN, args.cout - n0);
     const int h0 = half * (BN / 2), nh = min(BN / 2, ncols - h0);       // this thread's columns: [h0, h0 + nh)
     if (valid && args.epi == EPI_HEAD) {
       if (half == 0) {
@@ -417,11 +517,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
         }
       }
     } else if (valid && nh > 0) {
-      if (args.epi == EPI_SPLIT) {
-        const size_t o = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + n0 + h0;
-        if (args.mask_hi || args.accumulate) epi_split<true>(args, arow + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
-        else epi_split<false>(args, arow + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
-      } else if (args.epi == EPI_ATOMIC) {
+      if (args.epi == EPI_ATOMIC) {
         float* dstp = args.out_f32 + (size_t)v * args.out_ld + args.out_col_off + n0 + h0;
         for (int j = 0; j < nh; ++j) atomicAdd(dstp + j, arow[h0 + j]);
       } else {
@@ -430,7 +526,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       }
     }
     fence_proxy_async();                                                   // the next tile's TMA writes over s_acc
-    __syncthreads();
+    consumer_sync();
+    if (ctid == 0) mbar_arrive(staged_free);
   }
 }
 
@@ -441,7 +538,7 @@ static int launch_conv_bn(const ConvLaunch& L, int grid, cudaStream_t stream) {
     SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  conv_wgmma_kernel<BN, MODE><<<grid, 256, L.smem, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
+  conv_wgmma_kernel<BN, MODE><<<grid, kConvThreads, L.smem, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
   return SSDK_OK;
 }
 
@@ -840,7 +937,7 @@ __global__ void __launch_bounds__(256, 1) conv_first_kernel(const __grid_constan
     const int h0 = plane * (BN / 2), nh = min(BN / 2, fa.epi.cout - h0);
     if (valid && nh > 0) {
       const size_t o = (((size_t)n * fa.epi.out_Hp + (y + fa.epi.out_pad)) * fa.epi.out_Wp + (x + fa.epi.out_pad)) * fa.epi.out_Cs + h0;
-      epi_split<false>(fa.epi, s_acc + (size_t)r * (BN + kAccPad) + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
+      epi_split(fa.epi, s_acc + (size_t)r * (BN + kAccPad) + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
     }
     __syncthreads();                                                   // the A tile and s_acc are rewritten by the next tile
   }

@@ -524,6 +524,16 @@ extern "C" int ssdk_model_last_conv_ms(ssdk_model* m, float* out_ms) {
   return SSDK_OK;
 }
 
+extern "C" int ssdk_model_layer_ms(const ssdk_model* m, int layer, float* out_ms) {
+  SSDK_REQUIRE(m && out_ms && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_ms: bad argument");
+  const LayerPlan& L = m->layers[layer];
+  *out_ms = 0.f;
+  if (!L.ev0 || L.direct) return SSDK_OK;
+  SSDK_CHECK_CUDA(cudaEventSynchronize(L.ev1));
+  SSDK_CHECK_CUDA(cudaEventElapsedTime(out_ms, L.ev0, L.ev1));
+  return SSDK_OK;
+}
+
 extern "C" int ssdk_model_forward(ssdk_model* m, const float* images_dev, float* y_pred_dev, void* stream_) {
   SSDK_REQUIRE(m && images_dev, "ssdk_model_forward: NULL argument");
   SSDK_REQUIRE(m->P == 0 || y_pred_dev, "ssdk_model_forward: y_pred_dev is NULL");

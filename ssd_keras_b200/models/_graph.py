@@ -501,6 +501,16 @@ class SSDModel(KerasTrainingMixin):
         _ffi.check(_ffi.lib().ssdk_model_last_conv_ms(self._plan(batch)['handle'], C.byref(v)))
         return v.value
 
+    def layer_ms(self, batch, name):
+        """Time in ms of one layer's conv_wgmma_kernel launch in the last forward with timing enabled (0.0 for other layers)."""
+        v = C.c_float()
+        _ffi.check(_ffi.lib().ssdk_model_layer_ms(self._plan(batch)['handle'], self.index[name], C.byref(v)))
+        return v.value
+
+    def layer_plan(self, batch, name):
+        """The launch plan ssdk_model_create chose for one layer, as a dict (see _ffi.model_layer_plan)."""
+        return _ffi.model_layer_plan(self._plan(batch)['handle'], self.index[name])
+
 
 # ---------------------------------------------------------------------------------------------
 # argument handling shared by the three builders (reference: models/keras_ssd300.py:183-240)
