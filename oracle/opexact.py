@@ -1,7 +1,7 @@
 """Operand-exact float64 references of the tensor-core convolutions, with a per-element error bound.
 
 The convolution kernels do not multiply float32 operands.  They multiply the 16-bit split of each operand,
-``hi = bf16_rne(x)``, ``lo = bf16_rne(x - hi)`` (pack_kernel, pack_weights, first_weight_image, the hi/lo activation planes),
+``hi = bf16_rne(x)``, ``lo = bf16_rne(x - hi)`` (pack_kernel, repack_kernel, first_weight_image, the hi/lo activation planes),
 and issue hi*hi + hi*lo + lo*hi per k-step in bf16x3 mode, hi*hi in bf16 mode.  A reference that multiplies the unrounded
 float32 operands has to absorb the representation error of the split as well as the arithmetic, which needs bars of 1e-4 of
 the tensor's max (bf16x3) or 5e-2 (bf16).  The references here multiply the same split operands in float64.  The kernel's
@@ -37,7 +37,7 @@ UNIT = {'split': 2.0 ** -15, 'bf16': 2.0 ** -7, 'f32': 2.0 ** -23}
 
 
 def bf16_rne(x):
-    """float32 -> float32 values rounded to bfloat16, round to nearest even (the f2bf of model.cuh, __float2bfloat16_rn)."""
+    """float32 -> float32 values rounded to bfloat16, round to nearest even (the f2bf of conv.cuh, __float2bfloat16_rn)."""
     x = np.ascontiguousarray(x, dtype=np.float32)
     u = x.view(np.uint32).astype(np.uint64)
     nan = (u & 0x7fffffff) > 0x7f800000

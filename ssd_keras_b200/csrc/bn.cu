@@ -12,35 +12,6 @@ namespace ssdk {
 
 namespace {
 
-__device__ __forceinline__ size_t aidx(const ActBuf& a, int n, int y, int x) {
-  return (((size_t)n * a.Hp() + (y + a.pad)) * a.Wp() + (x + a.pad)) * a.Cs;
-}
-__device__ __forceinline__ void load8(const ActBuf& a, size_t i, float (&v)[8]) {
-  const uint4 h = *reinterpret_cast<const uint4*>(a.hi + i);
-  uint4 l = make_uint4(0, 0, 0, 0);
-  if (a.lo) l = *reinterpret_cast<const uint4*>(a.lo + i);
-  const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-  for (int e = 0; e < 8; ++e)
-    v[e] = __uint_as_float(((hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu) << 16) + __uint_as_float(((lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu) << 16);
-}
-__device__ __forceinline__ void store8(const ActBuf& a, size_t i, const float (&v)[8]) {
-  uint32_t ph[4], pl[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(v[2 * j]), h1 = __float2bfloat16_rn(v[2 * j + 1]);
-    const __nv_bfloat16 l0 = __float2bfloat16_rn(v[2 * j] - __bfloat162float(h0)), l1 = __float2bfloat16_rn(v[2 * j + 1] - __bfloat162float(h1));
-    ph[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    pl[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  }
-  *reinterpret_cast<uint4*>(a.hi + i) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-  if (a.lo) *reinterpret_cast<uint4*>(a.lo + i) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-}
-__device__ __forceinline__ float act_fwd(float y, int act) {
-  if (act == SSDK_ACT_RELU) return fmaxf(y, 0.f);
-  if (act == SSDK_ACT_ELU) return y > 0.f ? y : expm1f(y);
-  return y;
-}
 __device__ __forceinline__ float act_bwd(float a, int act) {      // derivative expressed through the activation's OUTPUT a
   if (act == SSDK_ACT_RELU) return a > 0.f ? 1.f : 0.f;
   if (act == SSDK_ACT_ELU) return a > 0.f ? 1.f : a + 1.f;       // d/dy (e^y - 1) = e^y = a + 1
@@ -73,7 +44,7 @@ __global__ void __launch_bounds__(256) bn_stats_kernel(ActBuf z, double* __restr
     const Elem el = elem_of(z, e, groups);
     g = el.g;
     float v[8];
-    load8(z, aidx(z, el.n, el.y, el.x) + (size_t)el.g * 8, v);
+    split_load8(z.hi, z.lo, act_index(z, el.n, el.y, el.x) + (size_t)el.g * 8, v);
 #pragma unroll
     for (int k = 0; k < 8; ++k) { s[k] += (double)v[k]; q[k] += (double)v[k] * (double)v[k]; }
   }
@@ -108,14 +79,14 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(ActBuf z, ActBuf out, con
   if (e >= total) return;
   const Elem el = elem_of(z, e, groups);
   float v[8], o[8];
-  load8(z, aidx(z, el.n, el.y, el.x) + (size_t)el.g * 8, v);
+  split_load8(z.hi, z.lo, act_index(z, el.n, el.y, el.x) + (size_t)el.g * 8, v);
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int c = el.g * 8 + k;
     o[k] = 0.f;
-    if (c < z.C) o[k] = act_fwd(gamma[c] * ((v[k] - bmean[c]) * brstd[c]) + beta[c], act);
+    if (c < z.C) o[k] = apply_act(gamma[c] * ((v[k] - bmean[c]) * brstd[c]) + beta[c], act);
   }
-  store8(out, aidx(out, el.n, el.y, el.x) + (size_t)el.g * 8, o);
+  split_store8(out.hi, out.lo, act_index(out, el.n, el.y, el.x) + (size_t)el.g * 8, o);
 }
 
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(ActBuf z, ActBuf a, ActBuf g, const float* __restrict__ bmean, const float* __restrict__ brstd,
@@ -133,9 +104,9 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(ActBuf z, ActBuf a, 
     const Elem el = elem_of(z, e, groups);
     gg = el.g;
     float zv[8], av[8], dv[8];
-    load8(z, aidx(z, el.n, el.y, el.x) + (size_t)el.g * 8, zv);
-    load8(a, aidx(a, el.n, el.y, el.x) + (size_t)el.g * 8, av);
-    load8(g, aidx(g, el.n, el.y, el.x) + (size_t)el.g * 8, dv);
+    split_load8(z.hi, z.lo, act_index(z, el.n, el.y, el.x) + (size_t)el.g * 8, zv);
+    split_load8(a.hi, a.lo, act_index(a, el.n, el.y, el.x) + (size_t)el.g * 8, av);
+    split_load8(g.hi, g.lo, act_index(g, el.n, el.y, el.x) + (size_t)el.g * 8, dv);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const int c = el.g * 8 + k;
@@ -164,10 +135,10 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(ActBuf z, ActBuf a, A
   if (e >= total) return;
   const Elem el = elem_of(z, e, groups);
   float zv[8], av[8], dv[8], o[8];
-  const size_t iz = aidx(z, el.n, el.y, el.x) + (size_t)el.g * 8, ig = aidx(g, el.n, el.y, el.x) + (size_t)el.g * 8;
-  load8(z, iz, zv);
-  load8(a, aidx(a, el.n, el.y, el.x) + (size_t)el.g * 8, av);
-  load8(g, ig, dv);
+  const size_t iz = act_index(z, el.n, el.y, el.x) + (size_t)el.g * 8, ig = act_index(g, el.n, el.y, el.x) + (size_t)el.g * 8;
+  split_load8(z.hi, z.lo, iz, zv);
+  split_load8(a.hi, a.lo, act_index(a, el.n, el.y, el.x) + (size_t)el.g * 8, av);
+  split_load8(g.hi, g.lo, ig, dv);
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const int c = el.g * 8 + k;
@@ -179,7 +150,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(ActBuf z, ActBuf a, A
       o[k] = gamma[c] * brstd[c] * (dy - m1 - xh * m2);
     }
   }
-  store8(g, ig, o);
+  split_store8(g.hi, g.lo, ig, o);
 }
 
 __global__ void zero_acc_kernel(double* acc, int n) {

@@ -99,12 +99,6 @@ void conv_pick_stages(ConvArgs& a) {
   }
 }
 
-__device__ __forceinline__ float apply_act(float x, int act) {
-  if (act == SSDK_ACT_RELU) return fmaxf(x, 0.f);
-  if (act == SSDK_ACT_ELU) return x > 0.f ? x : expm1f(x);
-  return x;
-}
-
 // 32 accumulator columns of this thread's row of the shared-memory accumulator tile
 __device__ __forceinline__ void ld_acc32(const float* p, float (&v)[32]) {
 #pragma unroll
@@ -167,98 +161,41 @@ __device__ __forceinline__ void epi_head_fixed(const ConvArgs& args, const float
 }
 
 // One group of 8 output channels of the activation-producing epilogues: bias / folded BatchNorm / activation -> bf16 hi+lo planes,
-// one 16-byte store per plane.  `v`, `sb`, `ss`, `sh` and output element `o` start at the group's first column.  BWD adds what
-// the data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
+// one 16-byte store per plane.  `v`, `sb`, `ss`, `sh` hold the group's accumulators and parameters, `o` is the output element of
+// its first column.  BWD adds what the data-gradient launches need: ReLU'(forward value) mask and accumulation into the output.
 template <bool BWD>
-__device__ __forceinline__ void epi_split8(const ConvArgs& args, const float* v, size_t o, const float* sb, const float* ss,
-                                           const float* sh) {
-  uint32_t ph[4], pl[4];
-  uint4 mk = make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u), oh = make_uint4(0, 0, 0, 0), ol = oh;
+__device__ __forceinline__ void epi_split8(const ConvArgs& args, const float (&v)[8], size_t o, const float (&sb)[8], const float (&ss)[8],
+                                           const float (&sh)[8]) {
+  float mk[8], old[8], f[8];
   if (BWD) {
-    if (args.mask_hi) mk = *reinterpret_cast<const uint4*>(args.mask_hi + o);
-    if (args.accumulate) {
-      oh = *reinterpret_cast<const uint4*>(args.out_hi + o);
-      if (args.out_lo) ol = *reinterpret_cast<const uint4*>(args.out_lo + o);
+    unpack8(args.mask_hi ? *reinterpret_cast<const uint4*>(args.mask_hi + o) : make_uint4(0x3f803f80u, 0x3f803f80u, 0x3f803f80u, 0x3f803f80u), mk);
+    if (args.accumulate) split_load8(args.out_hi, args.out_lo, o, old);
+    else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) old[e] = 0.f;
     }
   }
-  const uint32_t mkw[4] = {mk.x, mk.y, mk.z, mk.w}, ohw[4] = {oh.x, oh.y, oh.z, oh.w}, olw[4] = {ol.x, ol.y, ol.z, ol.w};
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float f[2];
+  for (int e = 0; e < 8; ++e) f[e] = v[e] + sb[e];
+  if (args.bn_scale) {
 #pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int col = j * 2 + e;
-      float xv = v[col] + sb[col];
-      if (args.bn_scale) xv = xv * ss[col] + sh[col];
-      xv = apply_act(xv, args.act);
-      if (BWD) {
-        if (!(__uint_as_float(((mkw[j] >> (e * 16)) & 0xffffu) << 16) > 0.f)) xv = 0.f;       // ReLU'(forward value)
-        xv += __uint_as_float(((ohw[j] >> (e * 16)) & 0xffffu) << 16) + __uint_as_float(((olw[j] >> (e * 16)) & 0xffffu) << 16);
-      }
-      f[e] = xv;
-    }
-    __nv_bfloat16 h0 = __float2bfloat16_rn(f[0]), h1 = __float2bfloat16_rn(f[1]);
-    __nv_bfloat16 l0 = __float2bfloat16_rn(f[0] - __bfloat162float(h0));
-    __nv_bfloat16 l1 = __float2bfloat16_rn(f[1] - __bfloat162float(h1));
-    ph[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    pl[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
+    for (int e = 0; e < 8; ++e) f[e] = f[e] * ss[e] + sh[e];
   }
-  *reinterpret_cast<uint4*>(args.out_hi + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-  if (args.out_lo) *reinterpret_cast<uint4*>(args.out_lo + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+  apply_act8(f, args.act);
+  if (BWD) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      if (!(mk[e] > 0.f)) f[e] = 0.f;                                     // ReLU'(forward value)
+      f[e] += old[e];
+    }
+  }
+  split_store8(args.out_hi, args.out_lo, o, f);
 }
 
-// Row epilogue of conv_first_kernel (one thread = one row of the shared-memory accumulator tile, `ncols` columns from `acc`).
-__device__ __forceinline__ void epi_split(const ConvArgs& args, const float* acc, int ncols, size_t o, const float* sb,
-                                          const float* ss, const float* sh) {
-  if (!args.bn_scale && args.act == SSDK_ACT_RELU && args.out_lo) {
-    // the common forward case (bias + ReLU, hi/lo planes) without per-element branches: packed conversions (two values per
-    // cvt.rn.bf16x2.f32) and biases fetched four at a time.  Bit-identical to the generic path below.
-    for (int c0 = 0; c0 < ncols; c0 += 32) {
-      float vr[32];
-      ld_acc32(acc + c0, vr);
-#pragma unroll
-      for (int g2 = 0; g2 < 2; ++g2) {
-        uint32_t ph[8], pl[8];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int g = g2 * 2 + h;
-          if (c0 + g * 8 < ncols) {
-            const float4 b0 = *reinterpret_cast<const float4*>(sb + c0 + g * 8);
-            const float4 b1 = *reinterpret_cast<const float4*>(sb + c0 + g * 8 + 4);
-            const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float f0 = fmaxf(vr[g * 8 + j * 2] + bb[j * 2], 0.f);
-              const float f1 = fmaxf(vr[g * 8 + j * 2 + 1] + bb[j * 2 + 1], 0.f);
-              const __nv_bfloat162 hh = __floats2bfloat162_rn(f0, f1);
-              const uint32_t hp = *reinterpret_cast<const uint32_t*>(&hh);
-              const __nv_bfloat162 ll = __floats2bfloat162_rn(f0 - __uint_as_float(hp << 16), f1 - __uint_as_float(hp & 0xffff0000u));
-              ph[h * 4 + j] = hp; pl[h * 4 + j] = *reinterpret_cast<const uint32_t*>(&ll);
-            }
-          }
-        }
-        const int cA = c0 + g2 * 16;
-        {
-          if (cA < ncols) {
-            *reinterpret_cast<uint4*>(args.out_hi + o + cA) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-            *reinterpret_cast<uint4*>(args.out_lo + o + cA) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-          }
-          if (cA + 8 < ncols) {
-            *reinterpret_cast<uint4*>(args.out_hi + o + cA + 8) = make_uint4(ph[4], ph[5], ph[6], ph[7]);
-            *reinterpret_cast<uint4*>(args.out_lo + o + cA + 8) = make_uint4(pl[4], pl[5], pl[6], pl[7]);
-          }
-        }
-      }
-    }
-    return;
-  }
-  for (int c0 = 0; c0 < ncols; c0 += 32) {
-    float vr[32];
-    ld_acc32(acc + c0, vr);
-#pragma unroll
-    for (int g = 0; g < 4; ++g)
-      if (c0 + g * 8 < ncols) epi_split8<false>(args, vr + g * 8, o + c0 + g * 8, sb + c0 + g * 8, ss + c0 + g * 8, sh + c0 + g * 8);
-  }
+// 8 consecutive floats of shared memory (16-byte aligned)
+__device__ __forceinline__ void ld_f8(const float* p, float (&v)[8]) {
+  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -565,23 +502,6 @@ int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int gri
   return SSDK_OK;
 }
 
-// ------------------------------------------------------------------------------------------------
-// helpers: split store
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void split_store(const ActBuf& o, size_t idx, float v) {
-  __nv_bfloat16 h = __float2bfloat16_rn(v);
-  o.hi[idx] = h;
-  if (o.lo) o.lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
-}
-__device__ __forceinline__ float split_load(const ActBuf& a, size_t idx) {
-  float v = __bfloat162float(a.hi[idx]);
-  if (a.lo) v += __bfloat162float(a.lo[idx]);
-  return v;
-}
-__device__ __forceinline__ size_t act_index(const ActBuf& a, int n, int y, int x) {
-  return (((size_t)n * a.Hp() + (y + a.pad)) * a.Wp() + (x + a.pad)) * a.Cs;
-}
-
 // (x - mean) / std, channel swap (models/keras_ssd300.py:247-272) -> split bf16 planes
 __global__ void preprocess_kernel(const float* __restrict__ img, int B, int H, int W, int Cimg, float3 mean, float3 inv_std,
                                   int has_std, int3 swap, ActBuf out) {
@@ -601,19 +521,11 @@ __global__ void preprocess_kernel(const float* __restrict__ img, int B, int H, i
   const int sw[3] = {swap.x, swap.y, swap.z};
   const size_t o = act_index(out, n, y, x);
   if (out.Cs == 8 && Cimg == 3) {               // one 16-byte word per plane and pixel (channels 3..7 are zero)
-    const float w0 = v[sw[0]], w1 = v[sw[1]], w2 = v[sw[2]];
-    const __nv_bfloat162 h01 = __floats2bfloat162_rn(w0, w1);
-    const __nv_bfloat16 h2 = __float2bfloat16_rn(w2);
-    const uint32_t hp = *reinterpret_cast<const uint32_t*>(&h01);
-    *reinterpret_cast<uint4*>(out.hi + o) = make_uint4(hp, (uint32_t)__bfloat16_as_ushort(h2), 0u, 0u);
-    if (out.lo) {
-      const __nv_bfloat162 l01 = __floats2bfloat162_rn(w0 - __uint_as_float(hp << 16), w1 - __uint_as_float(hp & 0xffff0000u));
-      const __nv_bfloat16 l2 = __float2bfloat16_rn(w2 - __bfloat162float(h2));
-      *reinterpret_cast<uint4*>(out.lo + o) = make_uint4(*reinterpret_cast<const uint32_t*>(&l01), (uint32_t)__bfloat16_as_ushort(l2), 0u, 0u);
-    }
+    const float w[8] = {v[sw[0]], v[sw[1]], v[sw[2]], 0.f, 0.f, 0.f, 0.f, 0.f};
+    split_store8(out.hi, out.lo, o, w);
     return;
   }
-  for (int c = 0; c < Cimg && c < 3; ++c) split_store(out, o + c, v[sw[c]]);
+  for (int c = 0; c < Cimg && c < 3; ++c) split_store(out.hi, out.lo, o + c, v[sw[c]]);
 }
 
 int launch_preprocess(ssdk_ctx* ctx, const float* images, int B, int H, int W, int Cimg, const float* mean, const float* stddev,
@@ -765,28 +677,18 @@ __global__ void __launch_bounds__(256) conv_direct_kernel(ActBuf in, ActBuf out,
   for (int p = 0; p < kDirectPx; ++p) {
     const int xo = xo0 + p;
     if (xo >= out.W) break;
-    uint32_t ph[8], pl[8];
+    const size_t o = act_index(out, n, yo, xo) + (size_t)g * 16;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float f[2];
+    for (int h = 0; h < 2; ++h) {
+      float f[8];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int col = g * 16 + j * 2 + e;
-        float xv = acc[p][j * 2 + e] + __ldg(bias + col);
+      for (int e = 0; e < 8; ++e) {
+        const int col = g * 16 + h * 8 + e;
+        float xv = acc[p][h * 8 + e] + __ldg(bias + col);
         if (bn_scale) xv = xv * __ldg(bn_scale + col) + __ldg(bn_shift + col);
         f[e] = apply_act(xv, act);
       }
-      __nv_bfloat16 h0 = __float2bfloat16_rn(f[0]), h1 = __float2bfloat16_rn(f[1]);
-      __nv_bfloat16 l0 = __float2bfloat16_rn(f[0] - __bfloat162float(h0)), l1 = __float2bfloat16_rn(f[1] - __bfloat162float(h1));
-      ph[j] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-      pl[j] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-    }
-    const size_t o = act_index(out, n, yo, xo) + (size_t)g * 16;
-    *reinterpret_cast<uint4*>(out.hi + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-    *reinterpret_cast<uint4*>(out.hi + o + 8) = make_uint4(ph[4], ph[5], ph[6], ph[7]);
-    if (out.lo) {
-      *reinterpret_cast<uint4*>(out.lo + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-      *reinterpret_cast<uint4*>(out.lo + o + 8) = make_uint4(pl[4], pl[5], pl[6], pl[7]);
+      split_store8(out.hi, out.lo, o + h * 8, f);
     }
   }
 }
@@ -937,7 +839,15 @@ __global__ void __launch_bounds__(256, 1) conv_first_kernel(const __grid_constan
     const int h0 = plane * (BN / 2), nh = min(BN / 2, fa.epi.cout - h0);
     if (valid && nh > 0) {
       const size_t o = (((size_t)n * fa.epi.out_Hp + (y + fa.epi.out_pad)) * fa.epi.out_Wp + (x + fa.epi.out_pad)) * fa.epi.out_Cs + h0;
-      epi_split(fa.epi, s_acc + (size_t)r * (BN + kAccPad) + h0, nh, o, s_bias + h0, s_scale + h0, s_shift + h0);
+      const float* arow = s_acc + (size_t)r * (BN + kAccPad) + h0;
+#pragma unroll 4
+      for (int c0 = 0; c0 < nh; c0 += 8) {
+        float v[8], sb[8], ss[8], sh[8];
+        ld_f8(arow + c0, v);
+        ld_f8(s_bias + h0 + c0, sb);
+        if (fa.epi.bn_scale) { ld_f8(s_scale + h0 + c0, ss); ld_f8(s_shift + h0 + c0, sh); }
+        epi_split8<false>(fa.epi, v, o + c0, sb, ss, sh);
+      }
     }
     __syncthreads();                                                   // the A tile and s_acc are rewritten by the next tile
   }
@@ -947,9 +857,6 @@ __global__ void __launch_bounds__(256, 1) conv_first_kernel(const __grid_constan
 // k = tap * 4 + c.  HWIO kernel in.
 void first_weight_image(const float* hwio, int taps, int cin, int cout, int BN, int kblocks, std::vector<uint16_t>& hi, std::vector<uint16_t>& lo) {
   hi.assign((size_t)kblocks * BN * 64, 0); lo.assign((size_t)kblocks * BN * 64, 0);
-  auto f2bf = [](float f) { uint32_t u; memcpy(&u, &f, 4); if ((u & 0x7f800000u) == 0x7f800000u) return (uint16_t)(u >> 16);
-                            u += 0x7fffu + ((u >> 16) & 1u); return (uint16_t)(u >> 16); };
-  auto bf2f = [](uint16_t h) { uint32_t u = (uint32_t)h << 16; float f; memcpy(&f, &u, 4); return f; };
   for (int o = 0; o < cout; ++o)
     for (int t = 0; t < taps; ++t)
       for (int c = 0; c < cin; ++c) {
@@ -1122,10 +1029,10 @@ __global__ void l2norm_kernel(ActBuf in, ActBuf out, const float* __restrict__ g
   const int x = (int)(pix % in.W); const int y = (int)((pix / in.W) % in.H); const int n = (int)(pix / ((size_t)in.W * in.H));
   const size_t s = act_index(in, n, y, x), o = act_index(out, n, y, x);
   float ss = 0.f;
-  for (int c = lane; c < in.C; c += 32) { float v = split_load(in, s + c); ss += v * v; }
+  for (int c = lane; c < in.C; c += 32) { float v = split_load(in.hi, in.lo, s + c); ss += v * v; }
   ss = warp_sum(ss);
   const float inv = rsqrtf(fmaxf(ss, 1e-12f));
-  for (int c = lane; c < in.C; c += 32) split_store(out, o + c, split_load(in, s + c) * inv * __ldg(gamma + c));
+  for (int c = lane; c < in.C; c += 32) split_store(out.hi, out.lo, o + c, split_load(in.hi, in.lo, s + c) * inv * __ldg(gamma + c));
 }
 
 // The same with eight channels (16 bytes of each plane) per lane and step: up to 512 channels stay in registers between the two
@@ -1145,16 +1052,9 @@ __global__ void __launch_bounds__(256) l2norm8_kernel(ActBuf in, ActBuf out, con
 #pragma unroll
     for (int e = 0; e < 8; ++e) v[k][e] = 0.f;
     if (c < in.C) {
-      const uint4 h4 = *reinterpret_cast<const uint4*>(in.hi + s + c);
-      uint4 l4 = make_uint4(0, 0, 0, 0);
-      if (in.lo) l4 = *reinterpret_cast<const uint4*>(in.lo + s + c);
-      const uint32_t hw[4] = {h4.x, h4.y, h4.z, h4.w}, lw[4] = {l4.x, l4.y, l4.z, l4.w};
+      split_load8(in.hi, in.lo, s + c, v[k]);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const uint32_t hb = (hw[e >> 1] >> ((e & 1) * 16)) & 0xffffu, lb = (lw[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
-        v[k][e] = __uint_as_float(hb << 16) + __uint_as_float(lb << 16);
-        ss += v[k][e] * v[k][e];
-      }
+      for (int e = 0; e < 8; ++e) ss += v[k][e] * v[k][e];
     }
   }
   ss = warp_sum(ss);
@@ -1165,17 +1065,10 @@ __global__ void __launch_bounds__(256) l2norm8_kernel(ActBuf in, ActBuf out, con
     if (c < in.C) {
       const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + c)), g1 = __ldg(reinterpret_cast<const float4*>(gamma + c + 4));
       const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-      uint32_t ph[4], pl[4];
+      float f[8];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float f0 = v[k][j * 2] * inv * gm[j * 2], f1 = v[k][j * 2 + 1] * inv * gm[j * 2 + 1];
-        const __nv_bfloat162 hh = __floats2bfloat162_rn(f0, f1);
-        const uint32_t hp = *reinterpret_cast<const uint32_t*>(&hh);
-        const __nv_bfloat162 ll = __floats2bfloat162_rn(f0 - __uint_as_float(hp << 16), f1 - __uint_as_float(hp & 0xffff0000u));
-        ph[j] = hp; pl[j] = *reinterpret_cast<const uint32_t*>(&ll);
-      }
-      *reinterpret_cast<uint4*>(out.hi + o + c) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-      if (out.lo) *reinterpret_cast<uint4*>(out.lo + o + c) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+      for (int e = 0; e < 8; ++e) f[e] = v[k][e] * inv * gm[e];
+      split_store8(out.hi, out.lo, o + c, f);
     }
   }
 }
@@ -1250,7 +1143,7 @@ __global__ void unpack_kernel(ActBuf in, float* __restrict__ out) {
   if (i >= total) return;
   const int c = (int)(i % in.C); const size_t pix = i / in.C;
   const int x = (int)(pix % in.W); const int y = (int)((pix / in.W) % in.H); const int n = (int)(pix / ((size_t)in.W * in.H));
-  out[i] = split_load(in, act_index(in, n, y, x) + c);
+  out[i] = split_load(in.hi, in.lo, act_index(in, n, y, x) + c);
 }
 
 // float32 NHWC tensor -> split bf16 planes of an activation buffer (SSDK_OP_TENSOR); channels beyond C stay zero
@@ -1260,7 +1153,7 @@ __global__ void pack_kernel(const float* __restrict__ in, ActBuf out) {
   if (i >= total) return;
   const int c = (int)(i % out.C); const size_t pix = i / out.C;
   const int x = (int)(pix % out.W); const int y = (int)((pix / out.W) % out.H); const int n = (int)(pix / ((size_t)out.W * out.H));
-  split_store(out, act_index(out, n, y, x) + c, in[i]);
+  split_store(out.hi, out.lo, act_index(out, n, y, x) + c, in[i]);
 }
 
 int launch_pack(ssdk_ctx* ctx, const float* in, const ActBuf& out, cudaStream_t stream) {

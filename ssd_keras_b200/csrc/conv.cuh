@@ -28,6 +28,83 @@ struct ActBuf {
   size_t elems() const { return rows() * Cs; }
 };
 
+// The hi + lo plane format of activations, gradients and packed weights: hi = bf16(v), lo = bf16(v - hi), both rounded to nearest
+// even; lo is a null plane in single-pass bf16 mode.  The helpers below are the only code that rounds values into the format or
+// reads them back (max-pooling, transposes and gathers move raw 16-bit halves).  They contain no multiply-add, so the per-file
+// --fmad settings cannot change their results.
+inline uint16_t f2bf(float f) {                  // host: round-to-nearest-even float -> bf16; a NaN stays a (quiet) NaN
+  uint32_t u; memcpy(&u, &f, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);
+  u += 0x7fffu + ((u >> 16) & 1u);
+  return (uint16_t)(u >> 16);
+}
+inline float bf2f(uint16_t h) { uint32_t u = (uint32_t)h << 16; float f; memcpy(&f, &u, 4); return f; }
+
+#ifdef __CUDACC__
+// element index of channel 0 of pixel (n, y, x) in a zero-bordered NHWC plane
+__device__ __forceinline__ size_t act_index(const ActBuf& a, int n, int y, int x) {
+  return (((size_t)n * a.Hp() + (y + a.pad)) * a.Wp() + (x + a.pad)) * a.Cs;
+}
+// one element: hi, plus lo when that plane exists
+__device__ __forceinline__ float split_load(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t i) {
+  float v = __bfloat162float(hi[i]);
+  if (lo) v += __bfloat162float(lo[i]);
+  return v;
+}
+__device__ __forceinline__ void split_store(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t i, float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hi[i] = h;
+  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+// 8 channels = one 16-byte word per plane: a word of one plane -> 8 values, and 8 values -> the hi and lo words
+__device__ __forceinline__ void unpack8(uint4 w, float (&v)[8]) {
+  const uint32_t u[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) { v[2 * j] = __uint_as_float(u[j] << 16); v[2 * j + 1] = __uint_as_float(u[j] & 0xffff0000u); }
+}
+__device__ __forceinline__ void pack8(const float (&v)[8], uint4& hi, uint4& lo) {
+  uint32_t h[4], l[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const __nv_bfloat162 hh = __floats2bfloat162_rn(v[2 * j], v[2 * j + 1]);
+    h[j] = *reinterpret_cast<const uint32_t*>(&hh);
+    const __nv_bfloat162 ll = __floats2bfloat162_rn(v[2 * j] - __uint_as_float(h[j] << 16), v[2 * j + 1] - __uint_as_float(h[j] & 0xffff0000u));
+    l[j] = *reinterpret_cast<const uint32_t*>(&ll);
+  }
+  hi = make_uint4(h[0], h[1], h[2], h[3]);
+  lo = make_uint4(l[0], l[1], l[2], l[3]);
+}
+// v = hi + lo of 8 channels (a missing lo plane reads as a zero word); `i` is a multiple of 8
+__device__ __forceinline__ void split_load8(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t i, float (&v)[8]) {
+  float l[8];
+  unpack8(*reinterpret_cast<const uint4*>(hi + i), v);
+  if (lo) unpack8(*reinterpret_cast<const uint4*>(lo + i), l);
+#pragma unroll
+  for (int e = 0; e < 8; ++e) v[e] += lo ? l[e] : 0.f;
+}
+__device__ __forceinline__ void split_store8(__nv_bfloat16* hi, __nv_bfloat16* lo, size_t i, const float (&v)[8]) {
+  uint4 h, l;
+  pack8(v, h, l);
+  *reinterpret_cast<uint4*>(hi + i) = h;
+  if (lo) *reinterpret_cast<uint4*>(lo + i) = l;
+}
+__device__ __forceinline__ float apply_act(float x, int act) {
+  if (act == SSDK_ACT_RELU) return fmaxf(x, 0.f);
+  if (act == SSDK_ACT_ELU) return x > 0.f ? x : expm1f(x);
+  return x;
+}
+// the same on 8 values with one branch on `act`, not one per value
+__device__ __forceinline__ void apply_act8(float (&v)[8], int act) {
+  if (act == SSDK_ACT_RELU) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = apply_act(v[e], SSDK_ACT_RELU);
+  } else if (act == SSDK_ACT_ELU) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) v[e] = apply_act(v[e], SSDK_ACT_ELU);
+  }
+}
+#endif
+
 enum { EPI_SPLIT = 0, EPI_F32 = 1, EPI_ATOMIC = 2, EPI_HEAD = 3 };
 
 constexpr int kMaxTaps = 25;

@@ -1,43 +1,34 @@
 // Static execution plan for the SSD graphs (models/keras_ssd300.py:263-419, keras_ssd512.py, keras_ssd7.py:266-393).
 // The host (Python, mirroring the reference builders) describes the graph layer by layer; this file sizes the
-// zero-bordered activation buffers, packs the weights into K-major bf16 hi/lo planes, builds the TMA descriptors
+// zero-bordered activation buffers, packs the weights into K-major bf16 hi/lo planes on the device, builds the TMA descriptors
 // and tile lists once, and replays the kernel sequence on every forward call.
 #include "model.cuh"
+#include <memory>
 
 using namespace ssdk;
 
 namespace {
 
-// Pack an HWIO float32 kernel (optionally two kernels fused per box: conf + loc) into K-major bf16 hi/lo planes
-// [cout][taps][kblocks*64] (virtual path) or [cout][kblocks*64] with k = (kh*KW+kw)*cin + c (im2col path).
-void pack_weights(const LayerPlan& L, int cin, int cout, int taps, int kblocks, bool im2col, int Ctot,
-                  std::vector<uint16_t>& hi, std::vector<uint16_t>& lo, std::vector<float>& bias) {
-  const ssdk_layer_desc& d = L.d;
-  const size_t Krow = im2col ? (size_t)kblocks * 64 : (size_t)taps * kblocks * 64;
-  hi.assign((size_t)cout * Krow, 0); lo.assign((size_t)cout * Krow, 0);
+// fp32 master kernel, HWIO [taps][cin][cout], and bias of a conv layer.  A head fuses its conf and loc kernels (and biases) per
+// box as [C logits | 4 offsets], the order of its output channels; every packed weight plane is made from this master.
+void fused_master(const ssdk_layer_desc& d, int cin, int cout, int Ctot, std::vector<float>& w, std::vector<float>& bias) {
+  const size_t K = (size_t)d.kh * d.kw * cin;
+  w.assign(K * cout, 0.f);
   bias.assign(cout, 0.f);
-  const bool head = d.op == SSDK_OP_HEAD;
-  const int nb = d.n_boxes;
-  const int c_conf = head ? nb * Ctot : cout;       // channels of the first kernel
-  const int c_loc = head ? nb * 4 : 0;
   for (int o = 0; o < cout; ++o) {
-    const float* ker; int oc, ocn;
-    if (!head) { ker = d.kernel; oc = o; ocn = c_conf; bias[o] = d.bias ? d.bias[o] : 0.f; }
-    else {
-      const int b = o / (Ctot + 4), r = o % (Ctot + 4);
-      if (r < Ctot) { ker = d.kernel; oc = b * Ctot + r; ocn = c_conf; bias[o] = d.bias ? d.bias[oc] : 0.f; }
-      else { ker = d.kernel2; oc = b * 4 + (r - Ctot); ocn = c_loc; bias[o] = d.bias2 ? d.bias2[oc] : 0.f; }
+    const float* ker = d.kernel; const float* b = d.bias;
+    int oc = o, ocn = cout;                             // column of `ker`, and its number of columns
+    if (d.op == SSDK_OP_HEAD) {
+      const int box = o / (Ctot + 4), r = o % (Ctot + 4);
+      if (r < Ctot) { oc = box * Ctot + r; ocn = d.n_boxes * Ctot; }
+      else { ker = d.kernel2; b = d.bias2; oc = box * 4 + (r - Ctot); ocn = d.n_boxes * 4; }
     }
-    for (int t = 0; t < taps; ++t)
-      for (int c = 0; c < cin; ++c) {
-        const float w = ker[((size_t)t * cin + c) * ocn + oc];       // HWIO: ((kh*KW+kw)*cin + c)*cout + o
-        const size_t k = im2col ? (size_t)t * cin + c : (size_t)t * kblocks * 64 + c;
-        const uint16_t h = f2bf(w);
-        hi[(size_t)o * Krow + k] = h;
-        lo[(size_t)o * Krow + k] = f2bf(w - bf2f(h));
-      }
+    if (b) bias[o] = b[oc];
+    for (size_t k = 0; k < K; ++k) w[k * cout + o] = ker[k * ocn + oc];
   }
 }
+
+struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
 
 int build_conv(ssdk_model* m, int li) {
   LayerPlan& L = m->layers[li];
@@ -51,6 +42,8 @@ int build_conv(ssdk_model* m, int li) {
   SSDK_REQUIRE(taps <= kMaxTaps, "conv kernel %dx%d is larger than the supported %d taps", d.kh, d.kw, kMaxTaps);
   SSDK_REQUIRE(head || cout % 8 == 0, "conv output channels must be a multiple of 8 (got %d)", cout);
   L.direct = !head && cin <= 4 && d.stride == 1 && cout % 16 == 0 && (size_t)taps * cin * cout * 4 <= 96 * 1024 && ia.Cs == 8;
+  std::vector<float> master, bias;
+  fused_master(d, cin, cout, m->Ctot, master, bias);
   // conv + BatchNormalization in a training plan: the conv writes its raw output z, batch statistics follow (bn.cu)
   L.bn_train = m->training && !head && d.bn_gamma && d.bn_beta && d.bn_mean && d.bn_var;
   if (L.bn_train) {
@@ -68,9 +61,8 @@ int build_conv(ssdk_model* m, int li) {
   // experiment knob (inference plans only): route the image-facing layer through im2col (K = 27 -> 32) + the implicit GEMM instead
   if (L.direct && !m->training && getenv("SSDK_NO_DIRECT")) L.direct = false;
   if (L.direct) {
-    int rc = upload_f32(m, &L.w_f32, d.kernel, (size_t)taps * cin * cout); if (rc) return rc;
-    std::vector<float> b0(cout, 0.f);
-    rc = upload_f32(m, &L.bias, d.bias ? d.bias : b0.data(), cout); if (rc) return rc;
+    int rc = upload_f32(m, &L.w_f32, master.data(), master.size()); if (rc) return rc;
+    rc = upload_f32(m, &L.bias, bias.data(), bias.size()); if (rc) return rc;
     if (d.bn_scale && d.bn_shift && !L.bn_train) {
       rc = upload_f32(m, &L.bn_scale, d.bn_scale, cout); if (rc) return rc;
       rc = upload_f32(m, &L.bn_shift, d.bn_shift, cout); if (rc) return rc;
@@ -83,7 +75,7 @@ int build_conv(ssdk_model* m, int li) {
         !getenv("SSDK_NO_FIRST_TC")) {
       std::vector<uint16_t> whi, wlo;
       L.first = first_plan(L.out, d.kh, d.kw, m->ctx->sm_count);
-      first_weight_image(d.kernel, taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
+      first_weight_image(master.data(), taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
       rc = dev_alloc(m, &L.w_hi, whi.size(), false); if (rc) return rc;
       SSDK_CHECK_CUDA(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
       if (m->split) {
@@ -115,35 +107,24 @@ int build_conv(ssdk_model* m, int li) {
     SSDK_REQUIRE(ia.pad >= std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)), "internal: activation border too small");
   }
   L.kblocks = kblocks;
-  // weights
-  std::vector<uint16_t> whi, wlo; std::vector<float> bias;
-  pack_weights(L, cin, cout, taps, kblocks, L.im2col, m->Ctot, whi, wlo, bias);
-  const size_t Krow = whi.size() / cout;
-  L.w_krow = Krow;
-  int rc = dev_alloc(m, &L.w_hi, whi.size(), false); if (rc) return rc;
-  SSDK_CHECK_CUDA(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
-  if (m->split) {
-    rc = dev_alloc(m, &L.w_lo, wlo.size(), false); if (rc) return rc;
-    SSDK_CHECK_CUDA(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
-  }
-  rc = plan_conv_gemm(m, cl, g, L.w_hi, L.w_lo, Krow, kblocks, &L.tile_list);
-  if (rc) return rc;
-  if (m->training) {          // fp32 master kernel, HWIO, with the conf/loc kernels of a head fused per box like the packed planes
-    std::vector<float> master((size_t)taps * cin * cout);
-    for (int t = 0; t < taps; ++t)
-      for (int c = 0; c < cin; ++c)
-        for (int o = 0; o < cout; ++o) {
-          float w;
-          if (!head) w = d.kernel[((size_t)t * cin + c) * cout + o];
-          else {
-            const int b = o / (m->Ctot + 4), r = o % (m->Ctot + 4);
-            w = r < m->Ctot ? d.kernel[((size_t)t * cin + c) * (d.n_boxes * m->Ctot) + b * m->Ctot + r]
-                            : d.kernel2[((size_t)t * cin + c) * (d.n_boxes * 4) + b * 4 + (r - m->Ctot)];
-          }
-          master[((size_t)t * cin + c) * cout + o] = w;
-        }
+  // weights: forward planes packed on the device from the master, which training plans keep for the optimiser
+  L.w_krow = L.im2col ? (size_t)kblocks * 64 : (size_t)taps * kblocks * 64;
+  int rc = dev_alloc(m, &L.w_hi, (size_t)cout * L.w_krow, false); if (rc) return rc;
+  if (m->split) { rc = dev_alloc(m, &L.w_lo, (size_t)cout * L.w_krow, false); if (rc) return rc; }
+  std::unique_ptr<float, CudaFree> scratch;         // the master of an inference plan, freed once the planes are packed
+  float* w_dev = nullptr;
+  if (m->training) {
     rc = upload_f32(m, &L.w_f32, master.data(), master.size()); if (rc) return rc;
+    w_dev = L.w_f32;
+  } else {
+    SSDK_CHECK_CUDA(cudaMalloc(&w_dev, master.size() * sizeof(float)));
+    scratch.reset(w_dev);
+    SSDK_CHECK_CUDA(cudaMemcpy(w_dev, master.data(), master.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
+  rc = launch_repack(m->ctx, w_dev, taps, cin, cout, L.im2col ? PACK_FWD_IM2COL : PACK_FWD, kblocks, L.w_krow, L.w_hi, L.w_lo, 0);
+  if (rc) return rc;
+  rc = plan_conv_gemm(m, cl, g, L.w_hi, L.w_lo, L.w_krow, kblocks, &L.tile_list);
+  if (rc) return rc;
   rc = upload_f32(m, &L.bias, bias.data(), bias.size()); if (rc) return rc;
   a.bias = L.bias;
   if (d.bn_scale && d.bn_shift && !head && !L.bn_train) {
@@ -245,6 +226,37 @@ int plan_overlap(ssdk_model* m) {
 }  // namespace
 
 namespace ssdk {
+
+// One element of the packed planes per thread: row `row`, K index `k` of `layout` <- the master element it holds (or 0)
+__global__ void repack_kernel(const float* __restrict__ w, int taps, int cin, int cout, WeightLayout layout, int kblocks, size_t krow,
+                              int rows, __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)rows * krow) return;
+  const int row = (int)(i / krow); const size_t k = i % krow;
+  float val = 0.f;
+  if (layout == PACK_FWD) {
+    const int t = (int)(k / ((size_t)kblocks * 64)), c = (int)(k % ((size_t)kblocks * 64));
+    if (t < taps && c < cin) val = w[((size_t)t * cin + c) * cout + row];
+  } else if (layout == PACK_FWD_IM2COL) {
+    if (k < (size_t)taps * cin) val = w[k * cout + row];
+  } else if (layout == PACK_DGRAD) {
+    const int t2 = (int)(k / ((size_t)kblocks * 64)), co = (int)(k % ((size_t)kblocks * 64));
+    if (t2 < taps && co < cout) val = w[((size_t)(taps - 1 - t2) * cin + row) * cout + co];
+  } else {
+    if (k < (size_t)cout) val = w[(size_t)row * cout + k];
+  }
+  split_store(hi, lo, i, val);
+}
+
+int launch_repack(ssdk_ctx* ctx, const float* w, int taps, int cin, int cout, WeightLayout layout, int kblocks, size_t krow,
+                  __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t s) {
+  const int rows = layout == PACK_DGRAD ? cin : layout == PACK_DGRAD_COL ? taps * cin : cout;
+  const size_t total = (size_t)rows * krow;
+  repack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w, taps, cin, cout, layout, kblocks, krow, rows, hi, lo);
+  SSDK_COUNT_LAUNCH(ctx);
+  SSDK_CHECK_CUDA(cudaGetLastError());
+  return SSDK_OK;
+}
 
 // Geometry, tile list, pipeline depths and TMA descriptors of one implicit-GEMM launch.  The caller fills the epilogue.
 int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,

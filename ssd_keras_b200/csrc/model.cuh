@@ -8,14 +8,6 @@
 
 namespace ssdk {
 
-inline uint16_t f2bf(float f) {                  // round-to-nearest-even float -> bf16
-  uint32_t u; memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);   // NaN
-  u += 0x7fffu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-inline float bf2f(uint16_t h) { uint32_t u = (uint32_t)h << 16; float f; memcpy(&f, &u, 4); return f; }
-
 struct LayerPlan {
   ssdk_layer_desc d{};
   int H = 0, W = 0, C = 0;            // logical output shape
@@ -124,5 +116,16 @@ int launch_bn_backward(ssdk_ctx* ctx, LayerPlan& L, int act, const ActBuf& g, fl
 
 int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
                    size_t krow, int kblocks, int** tile_list_out);
+
+// Layouts of the packed K-major bf16 hi / lo weight planes, all made on the device from the fp32 HWIO master [taps][cin][cout]
+// (defined in model.cu).  Every row is zero-padded to `krow` elements.
+enum WeightLayout {
+  PACK_FWD,          // forward, implicit GEMM: [cout][tap][kblocks * 64 over cin]
+  PACK_FWD_IM2COL,   // forward, im2col GEMM: [cout][k = tap * cin + c]
+  PACK_DGRAD,        // data gradient: the kernel rotated by 180 degrees, in / out swapped: [cin][taps - 1 - tap][kblocks * 64 over cout]
+  PACK_DGRAD_COL,    // col-gradient GEMM of a strided convolution, W^T: [k = tap * cin + c][cout]
+};
+int launch_repack(ssdk_ctx* ctx, const float* w, int taps, int cin, int cout, WeightLayout layout, int kblocks, size_t krow,
+                  __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t s);
 
 }  // namespace ssdk

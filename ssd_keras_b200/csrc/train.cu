@@ -18,23 +18,6 @@ using namespace ssdk;
 
 namespace {
 
-// ---------------------------------------------------------------------------------------------
-// device helpers
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ size_t aidx(const ActBuf& a, int n, int y, int x) {
-  return (((size_t)n * a.Hp() + (y + a.pad)) * a.Wp() + (x + a.pad)) * a.Cs;
-}
-__device__ __forceinline__ float ld2(const ActBuf& a, size_t i) {
-  float v = __bfloat162float(a.hi[i]);
-  if (a.lo) v += __bfloat162float(a.lo[i]);
-  return v;
-}
-__device__ __forceinline__ void st2(const ActBuf& a, size_t i, float v) {
-  __nv_bfloat16 h = __float2bfloat16_rn(v);
-  a.hi[i] = h;
-  if (a.lo) a.lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-}
-
 // dst[c][v] = src[row(v)][c] (or 0), v in [0, Kv): K-major operands for the weight-gradient GEMMs.
 struct TMap {
   int identity;             // row(v) = v
@@ -132,37 +115,13 @@ __global__ void head_bwd_kernel(const float* __restrict__ head, const float* __r
   float dot = 0.f;
   for (int c = lane; c < C; c += 32) dot += (expf(src[c] - mx) / sum) * d[c];
   dot = warp_sum(dot);
-  const size_t o = aidx(g, n, y, x) + (size_t)b * (C + 4);
-  for (int c = lane; c < C; c += 32) { const float p = expf(src[c] - mx) / sum; st2(g, o + c, p * (d[c] - dot)); }
-  if (lane < 4) st2(g, o + C + lane, d[C + lane]);
+  const size_t o = act_index(g, n, y, x) + (size_t)b * (C + 4);
+  for (int c = lane; c < C; c += 32) { const float p = expf(src[c] - mx) / sum; split_store(g.hi, g.lo, o + c, p * (d[c] - dot)); }
+  if (lane < 4) split_store(g.hi, g.lo, o + C + lane, d[C + lane]);
 }
 
 // Max-pool backward (gather form): gin(n,y,x,c) (+)= sum over windows whose FIRST maximum is (y,x) of gout; optional ReLU' mask.
 // One thread per (input pixel, 8 channels): 16-byte loads of the hi / lo planes.
-__device__ __forceinline__ void ld8(const ActBuf& a, size_t i, float (&v)[8]) {
-  const uint4 h = *reinterpret_cast<const uint4*>(a.hi + i);
-  const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
-#pragma unroll
-  for (int e = 0; e < 4; ++e) { v[2 * e] = __uint_as_float(hw[e] << 16); v[2 * e + 1] = __uint_as_float(hw[e] & 0xffff0000u); }
-  if (a.lo) {
-    const uint4 l = *reinterpret_cast<const uint4*>(a.lo + i);
-    const uint32_t lw[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) { v[2 * e] += __uint_as_float(lw[e] << 16); v[2 * e + 1] += __uint_as_float(lw[e] & 0xffff0000u); }
-  }
-}
-__device__ __forceinline__ void st8(const ActBuf& a, size_t i, const float (&v)[8]) {
-  uint32_t hw[4], lw[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const __nv_bfloat16 h0 = __float2bfloat16_rn(v[2 * e]), h1 = __float2bfloat16_rn(v[2 * e + 1]);
-    hw[e] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-    const __nv_bfloat16 l0 = __float2bfloat16_rn(v[2 * e] - __bfloat162float(h0)), l1 = __float2bfloat16_rn(v[2 * e + 1] - __bfloat162float(h1));
-    lw[e] = (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
-  }
-  *reinterpret_cast<uint4*>(a.hi + i) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-  if (a.lo) *reinterpret_cast<uint4*>(a.lo + i) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-}
 __global__ void __launch_bounds__(256) pool_bwd_kernel(ActBuf in, ActBuf gout, ActBuf gin, int Hout, int Wout, int KH, int KW, int stride,
                                                        int pad_t, int pad_l, int relu_mask, int accumulate) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -172,7 +131,7 @@ __global__ void __launch_bounds__(256) pool_bwd_kernel(ActBuf in, ActBuf gout, A
   const int c = (int)(i % CG) * 8; const size_t pix = i / CG;
   const int x = (int)(pix % in.W); const int y = (int)((pix / in.W) % in.H); const int n = (int)(pix / ((size_t)in.W * in.H));
   float v[8], acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  ld8(in, aidx(in, n, y, x) + c, v);
+  split_load8(in.hi, in.lo, act_index(in, n, y, x) + c, v);
   const int yo_lo = max(0, (y + pad_t - KH + stride) / stride), yo_hi = min(Hout - 1, (y + pad_t) / stride);
   const int xo_lo = max(0, (x + pad_l - KW + stride) / stride), xo_hi = min(Wout - 1, (x + pad_l) / stride);
   for (int yo = yo_lo; yo <= yo_hi; ++yo) {
@@ -190,7 +149,7 @@ __global__ void __launch_bounds__(256) pool_bwd_kernel(ActBuf in, ActBuf gout, A
           const int xx = x0 + kx;
           if (xx < 0 || xx >= in.W || (yy == y && xx == x)) continue;
           float u[8];
-          ld8(in, aidx(in, n, yy, xx) + c, u);
+          split_load8(in.hi, in.lo, act_index(in, n, yy, xx) + c, u);
           const bool before = (yy < y) || (yy == y && xx < x);
 #pragma unroll
           for (int e = 0; e < 8; ++e) if (u[e] > v[e] || (u[e] == v[e] && before)) first &= ~(1u << e);
@@ -198,24 +157,24 @@ __global__ void __launch_bounds__(256) pool_bwd_kernel(ActBuf in, ActBuf gout, A
       }
       if (first) {
         float g[8];
-        ld8(gout, aidx(gout, n, yo, xo) + c, g);
+        split_load8(gout.hi, gout.lo, act_index(gout, n, yo, xo) + c, g);
 #pragma unroll
         for (int e = 0; e < 8; ++e) if (first & (1u << e)) acc[e] += g[e];
       }
     }
   }
-  const size_t o = aidx(gin, n, y, x) + c;
+  const size_t o = act_index(gin, n, y, x) + c;
   if (relu_mask) {
 #pragma unroll
     for (int e = 0; e < 8; ++e) if (!(v[e] > 0.f)) acc[e] = 0.f;
   }
   if (accumulate) {
     float old[8];
-    ld8(gin, o, old);
+    split_load8(gin.hi, gin.lo, o, old);
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[e] += old[e];
   }
-  st8(gin, o, acc);
+  split_store8(gin.hi, gin.lo, o, acc);
 }
 
 // L2Normalization backward (y_c = gamma_c * x_c * s, s = rsqrt(max(sum x^2, 1e-12))): one warp per pixel.
@@ -226,24 +185,24 @@ __global__ void l2norm_bwd_kernel(ActBuf x, ActBuf gy, ActBuf gx, const float* _
   const size_t total = (size_t)x.B * x.H * x.W;
   if (pix >= total) return;
   const int xx = (int)(pix % x.W); const int yy = (int)((pix / x.W) % x.H); const int n = (int)(pix / ((size_t)x.W * x.H));
-  const size_t sx = aidx(x, n, yy, xx), sg = aidx(gy, n, yy, xx), so = aidx(gx, n, yy, xx);
+  const size_t sx = act_index(x, n, yy, xx), sg = act_index(gy, n, yy, xx), so = act_index(gx, n, yy, xx);
   float ss = 0.f, dot = 0.f;
   for (int c = lane; c < x.C; c += 32) {
-    const float v = ld2(x, sx + c);
+    const float v = split_load(x.hi, x.lo, sx + c);
     ss += v * v;
-    dot += gamma[c] * ld2(gy, sg + c) * v;
+    dot += gamma[c] * split_load(gy.hi, gy.lo, sg + c) * v;
   }
   ss = warp_sum(ss); dot = warp_sum(dot);
   const bool clamped = !(ss > 1e-12f);
   const float s = rsqrtf(fmaxf(ss, 1e-12f));
   for (int c = lane; c < x.C; c += 32) {
-    const float v = ld2(x, sx + c), d = ld2(gy, sg + c);
+    const float v = split_load(x.hi, x.lo, sx + c), d = split_load(gy.hi, gy.lo, sg + c);
     float g = s * gamma[c] * d;
     if (!clamped) g -= v * s * s * s * dot;
     atomicAdd(ggamma + c, d * v * s);
     if (relu_mask && !(v > 0.f)) g = 0.f;
-    if (accumulate) g += ld2(gx, so + c);
-    st2(gx, so + c, g);
+    if (accumulate) g += split_load(gx.hi, gx.lo, so + c);
+    split_store(gx.hi, gx.lo, so + c, g);
   }
 }
 
@@ -269,10 +228,10 @@ __global__ void col2im_kernel(const float* __restrict__ dcol, int Ho, int Wo, in
       acc += dcol[(((size_t)n * Ho + yo) * Wo + xo) * ld + (size_t)(kh * KW + kw) * gin.C + c];
     }
   }
-  const size_t o = aidx(gin, n, y, x) + c;
-  if (relu_mask && !(ld2(fwd, aidx(fwd, n, y, x) + c) > 0.f)) acc = 0.f;
-  if (accumulate) acc += ld2(gin, o);
-  st2(gin, o, acc);
+  const size_t o = act_index(gin, n, y, x) + c;
+  if (relu_mask && !(split_load(fwd.hi, fwd.lo, act_index(fwd, n, y, x) + c) > 0.f)) acc = 0.f;
+  if (accumulate) acc += split_load(gin.hi, gin.lo, o);
+  split_store(gin.hi, gin.lo, o, acc);
 }
 
 // Weight gradient of the image-facing conv (Cin <= 4): gw[co][tap][ci] += sum_pix dZ[pix][co] * X[pix + tap][ci].
@@ -294,12 +253,12 @@ __global__ void __launch_bounds__(256) wgrad_direct_kernel(ActBuf in, ActBuf g, 
       const int y = yo + kh * dil - pad_t;
       if (y < 0 || y >= in.H) continue;
       const int xo_lo = max(0, pad_l - kw * dil), xo_hi = min(g.W, in.W + pad_l - kw * dil);
-      size_t xi = aidx(in, n, y, xo_lo + kw * dil - pad_l) + c;
-      size_t go = aidx(g, n, yo, xo_lo) + cg;
+      size_t xi = act_index(in, n, y, xo_lo + kw * dil - pad_l) + c;
+      size_t go = act_index(g, n, yo, xo_lo) + cg;
       for (int xo = xo_lo; xo < xo_hi; ++xo, xi += in.Cs, go += g.Cs) {
-        const float xv = ld2(in, xi);
+        const float xv = split_load(in.hi, in.lo, xi);
         float gv[8];
-        ld8(g, go, gv);
+        split_load8(g.hi, g.lo, go, gv);
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc[e] += xv * gv[e];
       }
@@ -333,7 +292,7 @@ __global__ void __launch_bounds__(256) wgrad_direct3x3_kernel(ActBuf in, ActBuf 
     for (int r = r0; r < r1; ++r) {
       const int n = r / g.H, yo = r - n * g.H;
       for (int xo = pl; xo < g.W; xo += PL) {
-        const size_t go = aidx(g, n, yo, xo) + 2 * cq;
+        const size_t go = act_index(g, n, yo, xo) + 2 * cq;
         const uint32_t gh = *reinterpret_cast<const uint32_t*>(g.hi + go);
         float g0 = __uint_as_float(gh << 16), g1 = __uint_as_float(gh & 0xffff0000u);
         if (g.lo) {
@@ -395,32 +354,6 @@ __global__ void sgd_kernel_flat(float* __restrict__ w, float* __restrict__ v, co
   const float nv = mom * v[i] - lr * g[i] * scale;
   v[i] = nv;
   w[i] += nv;
-}
-
-// master HWIO -> packed K-major bf16 hi/lo planes.  mode 0: forward virtual path [cout][tap][kblocks*64];
-// mode 1: forward im2col path [cout][k = tap*cin + c]; mode 2: data-gradient kernel [cin][taps-1-tap][kb2*64 over cout];
-// mode 3: [tap*cin + c][cout] (col-gradient GEMM of strided convolutions).
-__global__ void repack_kernel(const float* __restrict__ w, int taps, int cin, int cout, int mode, int kblocks, size_t krow, int rows,
-                              __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t total = (size_t)rows * krow;
-  if (i >= total) return;
-  const int row = (int)(i / krow); const size_t k = i % krow;
-  float val = 0.f;
-  if (mode == 0) {
-    const int t = (int)(k / ((size_t)kblocks * 64)), c = (int)(k % ((size_t)kblocks * 64));
-    if (t < taps && c < cin) val = w[((size_t)t * cin + c) * cout + row];
-  } else if (mode == 1) {
-    if (k < (size_t)taps * cin) val = w[k * cout + row];
-  } else if (mode == 2) {
-    const int t2 = (int)(k / ((size_t)kblocks * 64)), co = (int)(k % ((size_t)kblocks * 64));
-    if (t2 < taps && co < cout) val = w[((size_t)(taps - 1 - t2) * cin + row) * cout + co];
-  } else {                      // mode 3: W^T for the col-gradient GEMM of strided convs: [k = tap*cin + c][cout]
-    if (k < (size_t)cout) val = w[(size_t)row * cout + k];
-  }
-  const __nv_bfloat16 h = __float2bfloat16_rn(val);
-  hi[i] = h;
-  if (lo) lo[i] = __float2bfloat16_rn(val - __bfloat162float(h));
 }
 
 __global__ void hwio_to_ohwi_kernel(const float* __restrict__ w, int taps, int cin, int cout, float* __restrict__ out) {
@@ -491,18 +424,28 @@ int t_alloc(ssdk_trainer* t, T** out, size_t count, bool zero) {
   return SSDK_OK;
 }
 
-int launch_repack(ssdk_ctx* ctx, const float* w, int taps, int cin, int cout, int mode, int kblocks, size_t krow, int rows,
-                  __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t s) {
-  const size_t total = (size_t)rows * krow;
-  repack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w, taps, cin, cout, mode, kblocks, krow, rows, hi, lo);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
-}
-
 bool is_conv(int op) { return op == SSDK_OP_CONV || op == SSDK_OP_HEAD; }
 // graph sources (preprocessed images, or a caller tensor): no producer, no parameters, no gradient
 bool is_source(int op) { return op == SSDK_OP_INPUT || op == SSDK_OP_TENSOR; }
+
+// The bf16 planes of conv layer i from its fp32 master: the forward planes (the image-facing direct kernel reads the master
+// itself) and the data-gradient planes
+int repack_layer(ssdk_trainer* t, int i, cudaStream_t s) {
+  ssdk_model* m = t->m;
+  const TLayer& T = t->tl[i];
+  const LayerPlan& L = m->layers[i];
+  int rc;
+  if (!L.direct) {
+    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, L.im2col ? PACK_FWD_IM2COL : PACK_FWD, L.kblocks, L.w_krow, L.w_hi, L.w_lo, s);
+    if (rc) return rc;
+  }
+  if (T.has_dgrad) {
+    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, T.dgrad_strided ? PACK_DGRAD_COL : PACK_DGRAD, T.w2_kblocks, T.w2_krow, T.w2_hi,
+                       T.w2_lo, s);
+    if (rc) return rc;
+  }
+  return SSDK_OK;
+}
 
 }  // namespace
 
@@ -691,14 +634,8 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       cl.grid = std::max(1, std::min(units * a.k_split, m->ctx->sm_count));
     }
   }
-  // rotated kernels for the data gradients
-  for (int i = 0; i < n; ++i) {
-    TLayer& T = t->tl[i];
-    if (!T.has_dgrad) continue;
-    if (T.dgrad_strided) rc = launch_repack(m->ctx, m->layers[i].w_f32, T.taps, T.cin, T.cout, 3, T.w2_kblocks, T.w2_krow, T.taps * T.cin, T.w2_hi, T.w2_lo, 0);
-    else rc = launch_repack(m->ctx, m->layers[i].w_f32, T.taps, T.cin, T.cout, 2, T.w2_kblocks, T.w2_krow, T.cin, T.w2_hi, T.w2_lo, 0);
-    if (rc) return fail(rc);
-  }
+  for (int i = 0; i < n; ++i)
+    if (is_conv(m->layers[i].d.op)) { rc = repack_layer(t, i, 0); if (rc) return fail(rc); }
   SSDK_CHECK_CUDA(cudaDeviceSynchronize());
   *out = t;
   return SSDK_OK;
@@ -946,14 +883,7 @@ extern "C" int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float
       sgd_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_beta, T.m_bnb, t->grad + T.off_bnb, (size_t)T.cout, lr, momentum, grad_scale);
       SSDK_COUNT_LAUNCH(ctx); SSDK_COUNT_LAUNCH(ctx);
     }
-    if (!L.direct) {
-      rc = launch_repack(ctx, L.w_f32, T.taps, T.cin, T.cout, L.im2col ? 1 : 0, L.kblocks, L.w_krow, T.cout, L.w_hi, L.w_lo, s); if (rc) return rc;
-    }
-    if (T.has_dgrad) {
-      if (T.dgrad_strided) rc = launch_repack(ctx, L.w_f32, T.taps, T.cin, T.cout, 3, T.w2_kblocks, T.w2_krow, T.taps * T.cin, T.w2_hi, T.w2_lo, s);
-      else rc = launch_repack(ctx, L.w_f32, T.taps, T.cin, T.cout, 2, T.w2_kblocks, T.w2_krow, T.cin, T.w2_hi, T.w2_lo, s);
-      if (rc) return rc;
-    }
+    rc = repack_layer(t, (int)i, s); if (rc) return rc;
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
@@ -982,22 +912,6 @@ __global__ void adam_kernel_flat(float* __restrict__ w, float* __restrict__ m1, 
   const float b = b2 * m2[i] + (1.f - b2) * grad * grad;
   m1[i] = a; m2[i] = b;
   w[i] -= lr_t * a / (sqrtf(b) + eps);
-}
-
-int repack_after_update(ssdk_trainer* t, int i, cudaStream_t s) {
-  ssdk_model* m = t->m;
-  TLayer& T = t->tl[i];
-  LayerPlan& L = m->layers[i];
-  int rc;
-  if (!L.direct) {
-    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, L.im2col ? 1 : 0, L.kblocks, L.w_krow, T.cout, L.w_hi, L.w_lo, s); if (rc) return rc;
-  }
-  if (T.has_dgrad) {
-    if (T.dgrad_strided) rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, 3, T.w2_kblocks, T.w2_krow, T.taps * T.cin, T.w2_hi, T.w2_lo, s);
-    else rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, 2, T.w2_kblocks, T.w2_krow, T.cin, T.w2_hi, T.w2_lo, s);
-    if (rc) return rc;
-  }
-  return SSDK_OK;
 }
 
 }  // namespace
@@ -1031,7 +945,7 @@ extern "C" int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, flo
       adam_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_beta, T.m_bnb, T.v_bnb, t->grad + T.off_bnb, (size_t)T.cout, lr_t, beta1, beta2, eps, grad_scale);
       SSDK_COUNT_LAUNCH(ctx); SSDK_COUNT_LAUNCH(ctx);
     }
-    rc = repack_after_update(t, (int)i, s); if (rc) return rc;
+    rc = repack_layer(t, (int)i, s); if (rc) return rc;
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

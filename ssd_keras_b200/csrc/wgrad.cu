@@ -149,15 +149,14 @@ __global__ void __launch_bounds__(256) bias_grad_kernel(const __nv_bfloat16* __r
   if (rl < RL) {
     const long long r0 = (long long)blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
     for (long long r = r0 + rl; r < r1; r += RL) {
-      const uint4 h = *reinterpret_cast<const uint4*>(hi + r * Cs + c);
-      const uint32_t hw[4] = {h.x, h.y, h.z, h.w};
+      float v[8];
+      unpack8(*reinterpret_cast<const uint4*>(hi + r * Cs + c), v);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) { acc[2 * e] += __uint_as_float(hw[e] << 16); acc[2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u); }
+      for (int e = 0; e < 8; ++e) acc[e] += v[e];
       if (lo) {
-        const uint4 l = *reinterpret_cast<const uint4*>(lo + r * Cs + c);
-        const uint32_t lw[4] = {l.x, l.y, l.z, l.w};
+        unpack8(*reinterpret_cast<const uint4*>(lo + r * Cs + c), v);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) { acc[2 * e] += __uint_as_float(lw[e] << 16); acc[2 * e + 1] += __uint_as_float(lw[e] & 0xffff0000u); }
+        for (int e = 0; e < 8; ++e) acc[e] += v[e];
       }
     }
 #pragma unroll

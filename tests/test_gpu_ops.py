@@ -134,6 +134,20 @@ def test_conv2d_single_pass_mode_and_errors():
         ops.conv2d(x, ker, None, strides=2, padding='same')
     with pytest.raises(Exception):
         ops.conv2d(x, ker[..., :12], None)                                    # 12 output channels: not a multiple of 8
+    # a NaN weight of the image-facing layer whose payload lies in the low 16 bits stays NaN in its bf16 weight image (not Inf);
+    # no activation: ReLU would turn the NaN into 0
+    x3 = rng.standard_normal((1, 9, 10, 3)).astype(np.float32)
+    k3 = (rng.standard_normal((3, 3, 3, 16)) * 0.1).astype(np.float32)
+    k3.view(np.uint32)[1, 1, 2, 5] = 0x7f800001                             # centre tap: reaches every output pixel
+    g = cc.Graph(1, 9, 10, 3, [dict(cout=16, k=3, pads=(1, 1, 1, 1), act=None, kernel=k3)], prec='bf16')
+    try:
+        cc.assert_plan(g.plan(1), dict(kernel='first_tc', split=0), 'nan_weight')
+        g.forward(x3)
+        y3 = g.read(1)
+    finally:
+        g.close()
+    assert np.isnan(y3[..., 5]).all() and not np.isinf(y3).any()
+    assert np.isfinite(np.delete(y3, 5, axis=-1)).all()
 
 
 @pytest.mark.parametrize('shape,pool,stride,padding', [
