@@ -349,6 +349,11 @@ int ssdk_model_layer_shape(const ssdk_model* m, int layer, int* out_h, int* out_
 int ssdk_model_forward(ssdk_model* m, const float* images_dev, float* y_pred_dev, void* stream);
 /* Copy a layer's activation (B,h,w,c) as float32 NHWC to out_dev (tests: per-layer parity). */
 int ssdk_model_read_layer(ssdk_model* m, int layer, float* out_dev, void* stream);
+/* The raw bf16 activation planes of a layer (what the next launches read, value = hi + lo), borders and padding channels
+ * included: geometry (padded rows Hp, row pitch Wp, stored channels Cs, border pad; a plane holds B*Hp*Wp*Cs values), and a
+ * copy of hi and lo (lo_dev may be NULL; single-pass bf16 plans have no lo plane).  Heads have no planes. */
+int ssdk_model_layer_planes_shape(const ssdk_model* m, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad);
+int ssdk_model_read_layer_planes(ssdk_model* m, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream);
 /* FLOPs of one forward pass (2*MACs of every conv, SURVEY 8d) and MMA flops actually issued. */
 int ssdk_model_flops(const ssdk_model* m, double* out_algorithmic, double* out_issued);
 /* Time of the conv kernels of the last forward in ms (CUDA events on `stream`), when enabled. */
@@ -401,6 +406,15 @@ int ssdk_trainer_num_params(const ssdk_trainer* t, long long* out_n);
  * gamma (3) or beta (4) inside the flat buffers */
 int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int which, long long* out_offset, long long* out_count);
 float* ssdk_trainer_grad_buffer(ssdk_trainer* t);
+/* Read-only views of a layer's output gradient (the planes the backward pass writes and the next launches read).
+ *   ssdk_trainer_grad_shape        stored geometry of the planes: padded rows Hp, padded row pitch Wp, stored channels Cs
+ *                                  (multiple of 8), zero border pad; a plane holds B*Hp*Wp*Cs bf16 values.
+ *   ssdk_trainer_read_grad         hi + lo as float32 NHWC (B,H,W,C) into out_dev.
+ *   ssdk_trainer_read_grad_planes  the raw bf16 planes, borders and padding channels included; lo_dev may be NULL and is left
+ *                                  untouched by a single-pass bf16 trainer, which has no lo plane. */
+int ssdk_trainer_grad_shape(const ssdk_trainer* t, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad);
+int ssdk_trainer_read_grad(ssdk_trainer* t, int layer, float* out_dev, void* stream);
+int ssdk_trainer_read_grad_planes(ssdk_trainer* t, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream);
 int ssdk_train_backward(ssdk_trainer* t, const float* y_true_dev, const float* y_pred_dev, int neg_pos_ratio, int n_neg_min,
                         float alpha, float* out_loss_dev /* [B] */, void* stream);
 /* The step in pieces, for overlapping the gradient exchange with the backward pass:
@@ -423,6 +437,9 @@ int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, float beta2, f
                           void* stream);
 /* Moving mean / variance of a BatchNormalization layer as the training passes left them (float32 [cout] each). */
 int ssdk_trainer_read_bn_stats(ssdk_trainer* t, int layer, float* mean_dev, float* var_dev, void* stream);
+/* The raw convolution output z (B,h,w,c) a BatchNormalization layer normalised in the last forward pass, hi + lo as float32
+ * NHWC (read-only; what the BatchNormalization backward reads). */
+int ssdk_trainer_read_bn_input(ssdk_trainer* t, int layer, float* out_dev, void* stream);
 /* Copy the current float32 master parameters (same order / layout as the gradients) to out_dev. */
 int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream);
 
@@ -447,6 +464,8 @@ typedef struct ssdk_backward_plan {
   int k_split;                 /* work units per tile along the pixel axis */
   int n_gemms;                 /* TRANSPOSED / IM2COL: GEMM launches */
   int stages, grid;
+  int kv;                      /* TRANSPOSED / IM2COL: pixels on the GEMM's K axis (the padded grid); NATIVE: 64-pixel patches */
+  int direct_fast;             /* DIRECT: 1 = wgrad_direct3x3_kernel (3x3x3 fast path), 0 = wgrad_direct_kernel */
 } ssdk_backward_plan;
 int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_backward_plan* out);
 

@@ -27,6 +27,23 @@ logit itself and of its difference to the row max (2**-22 * max|logit|).
 Gradients over a chain of GEMMs use the same bound.  A is the float64 autograd of the same graph run on absolute values:
 |x|, |w|, |dy|, with the ReLU masks as 0/1.
 
+Backward launches (``*_bwd_ref``, ``dgrad_ref``, ``wgrad_ref``) take the operands the kernel reads: the stored forward planes
+(hi + lo, as float32), the stored gradient planes (hi and lo separately, so no re-split is needed), the float32 masters.  Each
+returns (ref, A, {perturbation: ref'}) and is judged with the same form |g - ref| <= kappa * A + unit * |ref|:
+
+3. GEMMs (data and weight gradients) follow 1. with their own k-step counts.  dgrad: ``n_steps_gemm(taps, kblocks of dZ)``, and
+   one more for the old value a second consumer already wrote.  The strided data gradient stores the one-tap column GEMM in fp32
+   and col2im adds up to ``taps`` of those, one fp32 rounding each: ``n_steps_gemm(1, kblocks) + taps``.  The weight gradient
+   puts all three products of a k-step on one accumulator (wgrad_wgmma_kernel: ``4 * patches per split * products`` k-steps)
+   or runs the pixel axis through conv_wgmma_kernel (cross terms apart: ``4 * K blocks per split``); the ``k_split`` partial
+   sums meet in fp32 atomics (``n_steps_wgrad``).  The X operand is the stored planes themselves, not a re-split of hi + lo.
+4. fp32 sums (wgrad_direct, bias_grad_kernel, rowsum_kernel, col2im, pool routing, the gamma gradient).  Adding N terms in
+   any order loses at most (N - 1) * 2**-24 * sum |term| (every partial sum is bounded by the sum of absolute terms); a
+   rounded product adds 2**-24 * |term|.  So n_steps = N + 1 in kappa = 2**-22 * (n_steps + 1) is a bound, whatever order
+   the atomics take.
+5. Pointwise chains (softmax backward, L2Normalization backward) carry a relative error per fp32 operation; each is
+   written as kappa * A with A the sum of the absolute values of the terms, see the functions.
+
 The module is CPU only: NumPy for the bit-level rounding, torch float64 for the convolutions.
 """
 import numpy as np
@@ -181,3 +198,338 @@ def softmax_ref(z, A_z, n_steps, n_classes):
     p = e / e.sum(axis=-1, keepdims=True)
     delta = (kappa(n_steps) * A_z).max(axis=-1, keepdims=True) + 2.0 ** -22 * np.abs(z).max(axis=-1, keepdims=True)
     return p, p * (np.expm1(2.0 * delta) + (n_classes + 8) * 2.0 ** -23)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# backward launches
+# ------------------------------------------------------------------------------------------------------------------------------
+def bf16_bits_to_f32(u16):
+    """uint16 bf16 bit patterns -> float32 values."""
+    return (np.asarray(u16, np.uint16).astype(np.uint32) << 16).view(np.float32)
+
+
+def n_steps_wgrad(plan, products):
+    """k-steps behind one weight-gradient element, from ssdk_trainer_layer_plan.  NATIVE (wgrad_wgmma_kernel): ``kv`` 64-pixel
+    patches, all ``products`` of a k-step on one accumulator.  TRANSPOSED / IM2COL (conv_wgmma_kernel on a K axis of ``kv``
+    pixels, ceil(kv / 64) K blocks): the cross products have accumulators of their own, added in the epilogue, so the main
+    accumulator takes 4 k-steps per K block.  Either way the axis is cut into k_split ranges of at most ceil(units /
+    (k_split - 1)) units each, whose partial sums meet in fp32 atomics."""
+    ks = plan['k_split']
+    units, per_unit = (plan['kv'], 4 * products) if plan['wgrad'] == 'native' else (-(-plan['kv'] // 64), 4)
+    per = units if ks == 1 else min(units, -(-units // (ks - 1)))
+    return per_unit * per + ks
+
+
+def _dconv_tap(dz, w, t, in_hw, stride, dil, pads, c0=0, c1=None):
+    """Contribution of tap t (dZ channels [c0, c1)) to the data gradient: dz (B,Ho,Wo,Cout) x w[kh,kw,:,c0:c1]^T scattered
+    onto the (B,H,W,Cin) input grid."""
+    pt, pl, _, _ = pads
+    KH, KW, cin, cout = w.shape
+    kh, kw = divmod(t, KW)
+    c1 = cout if c1 is None else min(c1, cout)
+    B, Ho, Wo, _ = dz.shape
+    H, W = in_hw
+    out = np.zeros((B, H + 2 * (pt + dil * KH + stride), W + 2 * (pl + dil * KW + stride), cin))
+    v = np.einsum('bhwo,co->bhwc', np.asarray(dz[..., c0:c1], np.float64), np.asarray(w[kh, kw, :, c0:c1], np.float64))
+    y0, x0 = kh * dil, kw * dil                                    # padded-input position of output (0, 0) under this tap
+    out[:, y0:y0 + stride * (Ho - 1) + 1:stride, x0:x0 + stride * (Wo - 1) + 1:stride] += v
+    return out[:, pt:pt + H, pl:pl + W]
+
+
+def _dconv(dz, w, in_hw, stride, dil, pads):
+    return sum(_dconv_tap(dz, w, t, in_hw, stride, dil, pads) for t in range(w.shape[0] * w.shape[1]))
+
+
+def _planes(p):
+    """(hi, lo) float32 planes; lo None -> zeros (single-pass bf16 gradients)."""
+    hi, lo = p
+    return np.asarray(hi, np.float32), (np.zeros_like(hi, np.float32) if lo is None else np.asarray(lo, np.float32))
+
+
+def _terms(a, b, mode):
+    """Products the kernel issues for split operands a = (hi, lo), b = (hi, lo)."""
+    return [(a[0], b[0]), (a[0], b[1]), (a[1], b[0])] if mode == 'bf16x3' else [(a[0], b[0])]
+
+
+def _mask_acc(v, A, mask, old):
+    if mask is not None:
+        v, A = v * (mask > 0), A * (mask > 0)
+    if old is not None:
+        v, A = v + old, A + np.abs(old)
+    return v, A
+
+
+def dgrad_ref(dz, w, in_hw, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', mask=None, old=None, perturb=()):
+    """Data gradient of one convolution -> (ref, A, {perturbation: ref'}), float64 (B,H,W,Cin).
+
+    dz: the layer's gradient planes (hi, lo) as float32 (B,Ho,Wo,Cout), lo None in bf16 mode.  w: float32 HWIO master (split
+    here as the data-gradient planes are packed).  mask: the ReLU producer's stored output (the gradient is zeroed where it is
+    not > 0) or None.  old: the producer's gradient before the launch (accumulation) or None.  perturb: ('cross',) drops
+    dZ_hi * W_lo; ('tap', t) drops tap t; ('kblock', t, kb) drops dZ channels [64 kb, 64 kb + 64) of tap t (one K block of
+    the GEMM); ('mask',) leaves the mask out; ('old',) leaves the old value out."""
+    d = _planes(dz)
+    terms = _terms(d, split(w), mode)
+    geo = dict(in_hw=in_hw, stride=stride, dil=dil, pads=pads)
+    z = sum(_dconv(a, k, **geo) for a, k in terms)
+    A = sum(_dconv(np.abs(a), np.abs(k), **geo) for a, k in terms)
+    out = {}
+    for p in perturb:
+        zp, mp, op = z, mask, old
+        if p[0] == 'cross':
+            zp = z - _dconv(*terms[1], **geo)
+        elif p[0] == 'tap':
+            zp = z - sum(_dconv_tap(a, k, p[1], **geo) for a, k in terms)
+        elif p[0] == 'kblock':
+            zp = z - sum(_dconv_tap(a, k, p[1], c0=64 * p[2], c1=64 * p[2] + 64, **geo) for a, k in terms)
+        elif p[0] == 'mask':
+            mp = None
+        elif p[0] == 'old':
+            op = None
+        out[p] = _mask_acc(zp, A, mp, op)[0]
+    ref, A = _mask_acc(z, A, mask, old)
+    return ref, A, out
+
+
+def n_steps_dgrad(plan, taps, kblocks):
+    """k-steps behind one data-gradient element (section 3)."""
+    if plan['dgrad'] == 'strided':
+        return n_steps_gemm(1, kblocks) + taps + plan['dgrad_accumulate']
+    return n_steps_gemm(taps, kblocks) + plan['dgrad_accumulate']
+
+
+def _wgrad_tap(x, dz, t, KH, KW, stride, dil, pads, pix=None):
+    """dW[:, tap t, :] = sum over output pixels of dz (B,Ho,Wo,Cout) x the tap's window of x -> (Cout, Cin); pix: optional
+    (B,Ho,Wo) 0/1 weights of the output pixels."""
+    pt, pl, pb, pr = pads
+    kh, kw = divmod(t, KW)
+    B, Ho, Wo, _ = dz.shape
+    xp = np.pad(np.asarray(x, np.float64), ((0, 0), (pt, pb + stride + dil * KH), (pl, pr + stride + dil * KW), (0, 0)))
+    win = xp[:, kh * dil:kh * dil + stride * (Ho - 1) + 1:stride, kw * dil:kw * dil + stride * (Wo - 1) + 1:stride]
+    d = np.asarray(dz, np.float64) if pix is None else np.asarray(dz, np.float64) * pix[..., None]
+    return np.einsum('bhwc,bhwo->oc', win, d)
+
+
+def wgrad_ref(x, dz, KH, KW, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', perturb=()):
+    """Weight gradient -> (ref, A, {perturbation: ref'}), float64 (Cout, KH, KW, Cin) (the flat buffer's OHWI layout).
+
+    x: the layer's input as stored: its planes (hi, lo) as float32 (lo None in bf16 mode), or float32 hi + lo values to be
+    split here.  Pass the planes: where lo is exactly half an ulp of hi, split(hi + lo) may trade that half ulp between the
+    planes, which moves hi * dZ_lo by 2**-16 of the product -- more than the accumulation bound when a sparse (ReLU) input
+    channel has few non-zero products.  dz: the gradient planes (hi, lo).  mode 'fp32':
+    wgrad_direct_kernel, fp32 products of the unsplit hi + lo values.  perturb: ('cross',) drops X_hi * dZ_lo; ('tap', t);
+    ('kblock', kb) drops input channels [64 kb, 64 kb + 64) of every tap (one wgmma N block); ('pixels', n, y0, x0, h, w)
+    drops an h x w block of output pixels of image n (with h x w = bh x bw at the origin: one K block of the native kernel);
+    ('first', n, m) drops the first m output pixels of image n in row-major order (the first K block of the im2col GEMM)."""
+    g = _planes(dz)
+    xs = _planes(x) if isinstance(x, tuple) else split(x)
+    if mode == 'fp32':
+        terms = [(xs[0].astype(np.float64) + xs[1], g[0].astype(np.float64) + g[1])]
+    else:
+        terms = _terms(xs, g, mode)
+    taps = KH * KW
+    geo = dict(KH=KH, KW=KW, stride=stride, dil=dil, pads=pads)
+
+    def full(pix=None, c=None, skip_tap=None, which=None):
+        out = np.zeros((dz[0].shape[-1], taps, xs[0].shape[-1]))
+        for a, d in (terms if which is None else which):
+            for t in range(taps):
+                if t != skip_tap:
+                    out[:, t] += _wgrad_tap(a, d, t, pix=pix, **geo)
+        if c is not None:
+            out[:, :, c] = 0.0
+        return out
+    ref = full()
+    A = full(which=[(np.abs(a), np.abs(d)) for a, d in terms])
+    out = {}
+    for p in perturb:
+        if p[0] == 'cross':
+            out[p] = ref - full(which=[terms[1]])
+        elif p[0] == 'tap':
+            out[p] = full(skip_tap=p[1])
+        elif p[0] == 'kblock':
+            out[p] = full(c=slice(64 * p[1], 64 * p[1] + 64))
+        elif p[0] == 'pixels':
+            pix = np.ones(dz[0].shape[:3])
+            pix[p[1], p[2]:p[2] + p[4], p[3]:p[3] + p[5]] = 0
+            out[p] = full(pix=pix)
+        elif p[0] == 'first':
+            pix = np.ones(dz[0].shape[:3])
+            pix[p[1]].reshape(-1)[:p[2]] = 0
+            out[p] = full(pix=pix)
+    shape = (-1, KH, KW, xs[0].shape[-1])
+    return ref.reshape(shape), A.reshape(shape), {k: v.reshape(shape) for k, v in out.items()}
+
+
+def bias_grad_ref(dz, perturb=()):
+    """Bias gradient (bias_grad_kernel, rowsum_kernel): fp32 sum of hi and lo over all pixels -> (ref, A, n_steps, {...}).
+    perturb: ('lo',) leaves the lo plane out; ('row', n, y) leaves pixel row y of image n out."""
+    g = _planes(dz)
+    ref = g[0].astype(np.float64).sum(axis=(0, 1, 2)) + g[1].astype(np.float64).sum(axis=(0, 1, 2))
+    A = np.abs(g[0]).astype(np.float64).sum(axis=(0, 1, 2)) + np.abs(g[1]).astype(np.float64).sum(axis=(0, 1, 2))
+    out = {}
+    for p in perturb:
+        if p[0] == 'lo':
+            out[p] = g[0].astype(np.float64).sum(axis=(0, 1, 2))
+        elif p[0] == 'row':
+            out[p] = ref - g[0][p[1], p[2]].astype(np.float64).sum(0) - g[1][p[1], p[2]].astype(np.float64).sum(0)
+    return ref, A, 2 * int(np.prod(g[0].shape[:3])), out
+
+
+def pool_route(x, gout, KH, KW, stride, pad_t, pad_l, last=False):
+    """Max-pool backward routing in float64: each output's gradient goes to the FIRST maximum of its window (row-major scan,
+    strict '>', out-of-range taps skipped); last=True routes ties to the last maximum.  -> (routed, sum of |routed|,
+    windows per input element)."""
+    x = np.asarray(x, np.float64)
+    B, H, W, Cc = x.shape
+    _, Ho, Wo, _ = gout.shape
+    g = np.asarray(gout, np.float64)
+    out, A, cnt = np.zeros_like(x), np.zeros_like(x), np.zeros_like(x)
+    bi, ci = np.meshgrid(np.arange(B), np.arange(Cc), indexing='ij')
+    for yo in range(Ho):
+        for xo in range(Wo):
+            ys = [y for y in range(yo * stride - pad_t, yo * stride - pad_t + KH) if 0 <= y < H]
+            xs = [xx for xx in range(xo * stride - pad_l, xo * stride - pad_l + KW) if 0 <= xx < W]
+            pos = [(y, xx) for y in ys for xx in xs]                   # row-major scan order
+            win = np.stack([x[:, y, xx] for y, xx in pos], axis=-1)     # (B, C, taps)
+            k = win.shape[-1] - 1 - np.argmax(win[..., ::-1], axis=-1) if last else np.argmax(win, axis=-1)
+            py = np.array([p[0] for p in pos])[k]
+            px = np.array([p[1] for p in pos])[k]
+            np.add.at(out, (bi, py, px, ci), g[:, yo, xo])
+            np.add.at(A, (bi, py, px, ci), np.abs(g[:, yo, xo]))
+            np.add.at(cnt, (bi, py, px, ci), 1.0)
+    return out, A, cnt
+
+
+def pool_bwd_ref(x, gout, KH, KW, stride, pad_t, pad_l, relu_mask=False, old=None, perturb=()):
+    """pool_bwd_kernel -> (ref, A, n_steps, {...}).  x: the pool's input as stored (hi + lo); gout: the pool's gradient (hi + lo).
+    n_steps: the most windows that route to one element, plus the accumulation.  perturb: ('last',) ties to the last
+    maximum; ('mask',), ('old',)."""
+    r, A, cnt = pool_route(x, gout, KH, KW, stride, pad_t, pad_l)
+    mask = x if relu_mask else None
+    out = {}
+    for p in perturb:
+        if p[0] == 'last':
+            out[p] = _mask_acc(pool_route(x, gout, KH, KW, stride, pad_t, pad_l, last=True)[0], A, mask, old)[0]
+        elif p[0] == 'mask':
+            out[p] = _mask_acc(r, A, None, old)[0]
+        elif p[0] == 'old':
+            out[p] = _mask_acc(r, A, mask, None)[0]
+    ref, A = _mask_acc(r, A, mask, old)
+    return ref, A, int(cnt.max()) + (old is not None), out
+
+
+def l2norm_bwd_ref(x, gy, gamma, relu_mask=False, old=None, perturb=()):
+    """l2norm_bwd_kernel -> (gx_ref, A, kappa, gamma_ref, A_gamma, n_steps_gamma, {...}), float64.
+
+    y_c = gamma_c x_c s, s = rsqrt(max(sum x^2, 1e-12)): gx_c = s gamma_c d_c - x_c s^3 dot, dot = sum_c gamma_c d_c x_c; a
+    clamped pixel (sum x^2 <= 1e-12) keeps s gamma_c d_c only.  dgamma_c = sum over pixels of d_c x_c s.
+    Bound of gx: sum x^2 and dot are fp32 sums of C products (relative (C + 1) 2**-24 of their absolute sums); rsqrtf adds
+    2 ulps, so s carries (C/2 + 3) 2**-23 and s^3 three times that; the remaining multiplies, the subtraction and the
+    accumulation add a few roundings.  kappa = (3 C + 32) 2**-23 with A = s |gamma d| + |x| s^3 sum|gamma d x| (+ |old|)
+    covers all of them.  dgamma: a product of three factors (s as above) summed over N pixels in fp32 atomics ->
+    n_steps = N + C/2 + 6.  perturb: ('proj',) drops the projection term x s^3 dot."""
+    x = np.asarray(x, np.float64)
+    d = np.asarray(gy, np.float64)
+    gm = np.asarray(gamma, np.float64)
+    Cc = x.shape[-1]
+    ss = (x * x).sum(-1, keepdims=True)
+    clamped = ~(ss > 1e-12)
+    s = 1.0 / np.sqrt(np.maximum(ss, 1e-12))
+    dot = (gm * d * x).sum(-1, keepdims=True)
+    t1 = s * gm * d
+    t2 = np.where(clamped, 0.0, x * s ** 3 * dot)
+    A = np.abs(t1) + np.where(clamped, 0.0, np.abs(x) * s ** 3 * (np.abs(gm * d * x)).sum(-1, keepdims=True))
+    mask = x if relu_mask else None
+    out = {}
+    for p in perturb:
+        if p[0] == 'proj':
+            out[p] = _mask_acc(t1, A, mask, old)[0]
+        elif p[0] == 'mask':
+            out[p] = _mask_acc(t1 - t2, A, None, old)[0]
+        elif p[0] == 'old':
+            out[p] = _mask_acc(t1 - t2, A, mask, None)[0]
+    ref, A = _mask_acc(t1 - t2, A, mask, old)
+    gg = (d * x * s).reshape(-1, Cc).sum(0)
+    Ag = np.abs(d * x * s).reshape(-1, Cc).sum(0)
+    npix = int(np.prod(x.shape[:-1]))
+    return ref, A, (3 * Cc + 32) * 2.0 ** -23, gg, Ag, npix + Cc // 2 + 6, out
+
+
+def head_bwd_ref(logits, dy, n_boxes, n_classes, perturb=()):
+    """head_bwd_kernel -> (ref, A, kappa, {...}), float64 (B,H,W,n_boxes*(C+4)).
+
+    logits: the head's stored fp32 output (B,H,W,n_boxes*(C+4)); dy: d loss / d y_pred rows of this head, (B,H,W,n_boxes,>=C+4).
+    Class columns: p_c (d_c - dot), dot = sum p d; offsets pass d through.  Bound: expf is within 2 ulps, so each p carries a
+    relative e_p = (C + 8) 2**-22 (C exponentials in the sum, the max, the quotient); dot adds (C + 2) 2**-23 of S = sum p|d|;
+    the difference and the product one rounding each.  |err| <= (2 e_p + (C + 4) 2**-23) p (|d| + S): kappa = (5 C + 36) 2**-23,
+    A = p (|d| + S).  perturb: ('dot',) drops the dot term."""
+    Cc = n_classes
+    B, H, W, _ = logits.shape
+    z = np.asarray(logits, np.float64).reshape(B, H, W, n_boxes, Cc + 4)
+    d = np.asarray(dy, np.float64)[..., :Cc + 4]
+    e = np.exp(z[..., :Cc] - z[..., :Cc].max(-1, keepdims=True))
+    p = e / e.sum(-1, keepdims=True)
+    dot = (p * d[..., :Cc]).sum(-1, keepdims=True)
+    S = (p * np.abs(d[..., :Cc])).sum(-1, keepdims=True)
+
+    def rows(cls):
+        return np.concatenate([cls, d[..., Cc:]], axis=-1).reshape(B, H, W, -1)
+    ref = rows(p * (d[..., :Cc] - dot))
+    A = rows(p * (np.abs(d[..., :Cc]) + S)) * np.tile(np.concatenate([np.ones(Cc), np.zeros(4)]), n_boxes)
+    out = {}
+    for q in perturb:
+        if q[0] == 'dot':
+            out[q] = rows(p * d[..., :Cc])
+    return ref, A, (5 * Cc + 36) * 2.0 ** -23, out
+
+
+def bn_bwd_ref(z, a, da, gamma, act=None, eps=1e-3, perturb=()):
+    """BatchNormalization backward (bn_bwd_reduce_kernel + bn_bwd_apply_kernel) -> (dz_ref, A, kappa, dgamma_ref, dbeta_ref,
+    A_dgamma, A_dbeta, kappa_params, {...}), float64.
+
+    z: the stored raw convolution output (hi + lo); a: the stored activation output; da: d loss / d a (the gradient planes the
+    launch read).  The batch statistics are recomputed in float64 from z (biased variance over B, H, W).
+        dy = da * act'(a)  (ReLU: a > 0; ELU: a + 1 where a <= 0, written through the output like the kernel),
+        x^ = (z - mean) * rstd,  m1 = mean(dy),  m2 = mean(dy x^),  dz = gamma rstd (dy - m1 - x^ m2),
+        dgamma = sum dy x^,  dbeta = sum dy.
+    Bound: the kernel holds mean and rstd in fp32 (2**-24 relative each, from float64 statistics), forms dy with one rounding,
+    x^ with two (the subtraction and the product; the mean's rounding adds 2**-24 |mean| rstd), m1 and m2 as float64 sums rounded
+    once to fp32, and dz with three more roundings.  dy - m1 - x^ m2 cancels, so every term is bounded on absolute values:
+    with X = (|z - mean| + |mean|) rstd >= |x^| and its error, S1 = mean |dy| and S2 = mean(|dy| X),
+        |dz - dz_ref| <= 16 * 2**-23 * |gamma| rstd (|dy| + S1 + X (S2 + |m2|))  (kappa = 2**-19, A the factor after it).
+    The parameter gradients are float64 sums of fp32 terms dy x^ (each within 6 * 2**-23 of |dy| X) and dy, rounded once:
+    kappa_params = 8 * 2**-23 with A = sum |dy| X and sum |dy|.  perturb: ('m1',) and ('m2',) drop those terms; ('elu1',)
+    replaces act' by 1."""
+    z = np.asarray(z, np.float64)
+    a = np.asarray(a, np.float64)
+    da = np.asarray(da, np.float64)
+    gm = np.asarray(gamma, np.float64)
+    axes = tuple(range(z.ndim - 1))
+    mean = z.mean(axes)
+    rstd = 1.0 / np.sqrt(z.var(axes) + float(np.float32(eps)))
+    xh = (z - mean) * rstd
+    X = (np.abs(z - mean) + np.abs(mean)) * rstd
+
+    def deriv(unit_elu=False):
+        if act == 'relu':
+            return (a > 0).astype(np.float64)
+        if act == 'elu' and not unit_elu:
+            return np.where(a > 0, 1.0, a + 1.0)
+        return np.ones_like(a)
+
+    def dz_of(dy, drop=None):
+        m1, m2 = dy.mean(axes), (dy * xh).mean(axes)
+        return gm * rstd * (dy - (0 if drop == 'm1' else m1) - (0 if drop == 'm2' else xh * m2))
+    dy = da * deriv()
+    ref = dz_of(dy)
+    m2 = (dy * xh).mean(axes)
+    A = np.abs(gm) * rstd * (np.abs(dy) + np.abs(dy).mean(axes) + X * ((np.abs(dy) * X).mean(axes) + np.abs(m2)))
+    out = {}
+    for p in perturb:
+        if p[0] in ('m1', 'm2'):
+            out[p] = dz_of(dy, p[0])
+        elif p[0] == 'elu1':
+            out[p] = dz_of(da * deriv(unit_elu=True))
+    dgamma, dbeta = (dy * xh).sum(axes), dy.sum(axes)
+    Ag, Ab = (np.abs(dy) * X).sum(axes), np.abs(dy).sum(axes)
+    return ref, A, 16 * 2.0 ** -23, dgamma, dbeta, Ag, Ab, 8 * 2.0 ** -23, out

@@ -82,7 +82,7 @@ class LayerPlan(C.Structure):
 class TrainerLayerPlan(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('dgrad', 'dgrad_bn', 'dgrad_mask', 'dgrad_accumulate', 'dgrad_n_tiles_m', 'dgrad_n_tiles_n',
                                        'dgrad_grid', 'wgrad', 'wgrad_bn', 'a_boxes', 'bw', 'bh', 'co_tiles', 'ci_tiles', 'k_split',
-                                       'n_gemms', 'stages', 'grid')]
+                                       'n_gemms', 'stages', 'grid', 'kv', 'direct_fast')]
 
 
 PLAN_KERNELS = {0: None, 1: 'gemm', 2: 'im2col_gemm', 3: 'first_tc', 4: 'direct'}
@@ -185,6 +185,10 @@ def lib():
             L.ssdk_model_layer_ms.argtypes = [vp, C.c_int, c_float_p]
             L.ssdk_model_layer_plan.argtypes = [vp, C.c_int, C.POINTER(LayerPlan)]
             L.ssdk_model_layer_plan.restype = C.c_int
+            L.ssdk_model_layer_planes_shape.argtypes = [vp, C.c_int, c_int_p, c_int_p, c_int_p, c_int_p]
+            L.ssdk_model_read_layer_planes.argtypes = [vp, C.c_int, vp, vp, vp]
+            L.ssdk_model_layer_planes_shape.restype = C.c_int
+            L.ssdk_model_read_layer_planes.restype = C.c_int
         if hasattr(L, 'ssdk_trainer_create'):
             L.ssdk_trainer_create.argtypes = [vp, vp, C.POINTER(vp)]
             L.ssdk_trainer_destroy.argtypes = [vp]
@@ -207,6 +211,12 @@ def lib():
             L.ssdk_trainer_read_params.argtypes = [vp, vp, vp]
             L.ssdk_trainer_layer_plan.argtypes = [vp, C.c_int, C.POINTER(TrainerLayerPlan)]
             L.ssdk_trainer_layer_plan.restype = C.c_int
+            L.ssdk_trainer_grad_shape.argtypes = [vp, C.c_int, c_int_p, c_int_p, c_int_p, c_int_p]
+            L.ssdk_trainer_read_grad.argtypes = [vp, C.c_int, vp, vp]
+            L.ssdk_trainer_read_grad_planes.argtypes = [vp, C.c_int, vp, vp, vp]
+            L.ssdk_trainer_read_bn_input.argtypes = [vp, C.c_int, vp, vp]
+            for name in ('ssdk_trainer_grad_shape', 'ssdk_trainer_read_grad', 'ssdk_trainer_read_grad_planes', 'ssdk_trainer_read_bn_input'):
+                getattr(L, name).restype = C.c_int
             for name in ('ssdk_trainer_create', 'ssdk_trainer_destroy', 'ssdk_trainer_num_params', 'ssdk_trainer_param_span',
                          'ssdk_train_backward', 'ssdk_train_apply', 'ssdk_trainer_read_params'):
                 getattr(L, name).restype = C.c_int

@@ -652,6 +652,24 @@ extern "C" int ssdk_model_read_layer(ssdk_model* m, int layer, float* out_dev, v
   return launch_unpack(m->ctx, L.out, out_dev, stream);
 }
 
+extern "C" int ssdk_model_layer_planes_shape(const ssdk_model* m, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad) {
+  SSDK_REQUIRE(m && out_hp && out_wp && out_cs && out_pad && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_planes_shape: bad argument");
+  const ActBuf& o = m->layers[layer].out;
+  SSDK_REQUIRE(o.hi, "ssdk_model_layer_planes_shape: layer %d has no activation planes", layer);
+  *out_hp = o.Hp(); *out_wp = o.Wp(); *out_cs = o.Cs; *out_pad = o.pad;
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_model_read_layer_planes(ssdk_model* m, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream) {
+  SSDK_REQUIRE(m && hi_dev && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_read_layer_planes: bad argument");
+  const ActBuf& o = m->layers[layer].out;
+  SSDK_REQUIRE(o.hi, "ssdk_model_read_layer_planes: layer %d has no activation planes", layer);
+  const size_t bytes = o.elems() * sizeof(uint16_t);
+  SSDK_CHECK_CUDA(cudaMemcpyAsync(hi_dev, o.hi, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  if (lo_dev && o.lo) SSDK_CHECK_CUDA(cudaMemcpyAsync(lo_dev, o.lo, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return SSDK_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Stand-alone layer calls (SURVEY 8b: ssdk_conv2d_fwd, ssdk_maxpool): a one-layer graph through the same plan builder
 // ---------------------------------------------------------------------------------------------------------------------

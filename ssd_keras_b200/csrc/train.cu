@@ -384,6 +384,7 @@ struct TLayer {
   int* dgrad_tiles = nullptr;
   bool dgrad_strided = false;               // stride != 1: col-gradient GEMM (dZ * W^T) + col2im
   int dgrad_relu_mask = 0;                  // col2im zeroes the gradient where the ReLU producer's output is <= 0
+  int dgrad_col2im_accumulate = 0;          // col2im adds to a gradient another consumer of the producer already wrote
   float* dcol = nullptr; int dcol_ld = 0;
   // weight gradient
   bool wg_native = false;                   // stride-1 layers: wgrad.cu reads dZ / X in place (no transposed copies)
@@ -395,6 +396,13 @@ struct TLayer {
   TMap dy_map{}, x_map{};
   float* vgamma = nullptr;
 };
+
+// wgrad_direct3x3_kernel's conditions: 3x3 undilated taps over 3 input channels, an even cout that fits its shared accumulators, and a
+// zero border wide enough that every tap is a constant offset from the window origin
+bool direct_fast3(const ssdk_layer_desc& d, const ActBuf& X, int cin, int cout) {
+  return d.kh == 3 && d.kw == 3 && d.dilation == 1 && cin == 3 && X.Cs >= 4 && cout % 2 == 0 && cout <= 512 && X.pad >= d.pad_t &&
+         X.pad >= d.pad_l && X.pad >= 2 - d.pad_t && X.pad >= 2 - d.pad_l;
+}
 
 }  // namespace
 
@@ -538,6 +546,7 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
         if (rc) return fail(rc);
         ConvArgs& a = T.dgrad.args;
         a.epi = EPI_F32; a.bias = nullptr; a.act = SSDK_ACT_NONE; a.out_f32 = T.dcol;
+        T.dgrad_col2im_accumulate = written[pi] ? 1 : 0;
         written[pi] = 1;
         goto wgrad_plan;
       }
@@ -668,6 +677,32 @@ extern "C" int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int whi
 
 extern "C" float* ssdk_trainer_grad_buffer(ssdk_trainer* t) { return t ? t->grad : nullptr; }
 
+extern "C" int ssdk_trainer_grad_shape(const ssdk_trainer* t, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad) {
+  SSDK_REQUIRE(t && out_hp && out_wp && out_cs && out_pad && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_grad_shape: bad argument");
+  const TLayer& T = t->tl[layer];
+  SSDK_REQUIRE(T.has_g, "ssdk_trainer_grad_shape: layer %d has no gradient planes", layer);
+  *out_hp = T.g.Hp(); *out_wp = T.g.Wp(); *out_cs = T.g.Cs; *out_pad = T.g.pad;
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_trainer_read_grad(ssdk_trainer* t, int layer, float* out_dev, void* stream) {
+  SSDK_REQUIRE(t && out_dev && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_read_grad: bad argument");
+  const TLayer& T = t->tl[layer];
+  SSDK_REQUIRE(T.has_g, "ssdk_trainer_read_grad: layer %d has no gradient planes", layer);
+  return launch_unpack(t->m->ctx, T.g, out_dev, (cudaStream_t)stream);
+}
+
+extern "C" int ssdk_trainer_read_grad_planes(ssdk_trainer* t, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream) {
+  SSDK_REQUIRE(t && hi_dev && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_read_grad_planes: bad argument");
+  const TLayer& T = t->tl[layer];
+  SSDK_REQUIRE(T.has_g, "ssdk_trainer_read_grad_planes: layer %d has no gradient planes", layer);
+  const size_t bytes = T.g.elems() * sizeof(uint16_t);
+  cudaStream_t s = (cudaStream_t)stream;
+  SSDK_CHECK_CUDA(cudaMemcpyAsync(hi_dev, T.g.hi, bytes, cudaMemcpyDeviceToDevice, s));
+  if (lo_dev && T.g.lo) SSDK_CHECK_CUDA(cudaMemcpyAsync(lo_dev, T.g.lo, bytes, cudaMemcpyDeviceToDevice, s));
+  return SSDK_OK;
+}
+
 extern "C" int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_backward_plan* out) {
   SSDK_REQUIRE(t && out && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_layer_plan: bad argument");
   memset(out, 0, sizeof(*out));
@@ -679,23 +714,27 @@ extern "C" int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_ba
     out->dgrad = T.dgrad_strided ? SSDK_DGRAD_STRIDED : SSDK_DGRAD_GEMM;
     out->dgrad_bn = a.BN;
     out->dgrad_mask = T.dgrad_strided ? T.dgrad_relu_mask : (a.mask_hi != nullptr);
-    out->dgrad_accumulate = a.accumulate;
+    out->dgrad_accumulate = T.dgrad_strided ? T.dgrad_col2im_accumulate : a.accumulate;
     out->dgrad_n_tiles_m = a.n_tiles_m; out->dgrad_n_tiles_n = a.n_tiles_n; out->dgrad_grid = T.dgrad.grid;
   }
-  if (L.direct) { out->wgrad = SSDK_WGRAD_DIRECT; return SSDK_OK; }
+  if (L.direct) {
+    out->wgrad = SSDK_WGRAD_DIRECT;
+    out->direct_fast = direct_fast3(L.d, t->m->layers[L.d.input].out, T.cin, T.cout) ? 1 : 0;
+    return SSDK_OK;
+  }
   if (T.wg_native) {
     const WgradArgs& w = T.wg.args;
     out->wgrad = SSDK_WGRAD_NATIVE;
     out->wgrad_bn = w.BNc; out->a_boxes = w.a_boxes; out->bw = w.bw; out->bh = w.bh;
     out->co_tiles = w.co_tiles; out->ci_tiles = w.ci_tiles; out->k_split = w.k_split > 1 ? w.k_split : 1;
-    out->stages = w.stages; out->grid = T.wg.grid;
+    out->stages = w.stages; out->grid = T.wg.grid; out->kv = w.total_patches;
     return SSDK_OK;
   }
   if (T.wgrad.empty()) return SSDK_OK;
   const ConvLaunch& c = T.wgrad[0];
   out->wgrad = L.im2col ? SSDK_WGRAD_IM2COL : SSDK_WGRAD_TRANSPOSED;
   out->wgrad_bn = c.args.BN; out->k_split = c.args.k_split > 1 ? c.args.k_split : 1;
-  out->n_gemms = (int)T.wgrad.size(); out->stages = c.args.stages; out->grid = c.grid;
+  out->n_gemms = (int)T.wgrad.size(); out->stages = c.args.stages; out->grid = c.grid; out->kv = (int)T.Kv;
   return SSDK_OK;
 }
 
@@ -807,10 +846,16 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     if (L.direct) {
       const int K = T.taps * T.cin;
       const size_t smem = (size_t)K * T.cout * sizeof(float);
+      // the plan admits direct layers whose fp32 [K][Cout] accumulator needs up to 96 KB (model.cu, as conv_direct_kernel)
+      static bool attr_set = false;
+      if (!attr_set) {
+        SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct3x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        attr_set = true;
+      }
       const int total_rows = T.g.B * T.g.H;
       const int rpb = std::max(1, (total_rows + 8 * ctx->sm_count - 1) / (8 * ctx->sm_count));
-      const bool fast3 = d.kh == 3 && d.kw == 3 && d.dilation == 1 && T.cin == 3 && PL.out.Cs >= 4 && T.cout % 2 == 0 && T.cout <= 512 &&
-                         PL.out.pad >= d.pad_t && PL.out.pad >= d.pad_l && PL.out.pad >= 2 - d.pad_t && PL.out.pad >= 2 - d.pad_l;
+      const bool fast3 = direct_fast3(d, PL.out, T.cin, T.cout);
       if (fast3) wgrad_direct3x3_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, t->grad + T.off_w, d.pad_t, d.pad_l, rpb);
       else wgrad_direct_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, t->grad + T.off_w, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
       SSDK_COUNT_LAUNCH(ctx);
@@ -958,6 +1003,13 @@ extern "C" int ssdk_trainer_read_bn_stats(ssdk_trainer* t, int layer, float* mea
   SSDK_CHECK_CUDA(cudaMemcpyAsync(mean_dev, L.bn_mmean, (size_t)L.C * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream_));
   SSDK_CHECK_CUDA(cudaMemcpyAsync(var_dev, L.bn_mvar, (size_t)L.C * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream_));
   return SSDK_OK;
+}
+
+extern "C" int ssdk_trainer_read_bn_input(ssdk_trainer* t, int layer, float* out_dev, void* stream_) {
+  SSDK_REQUIRE(t && out_dev && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_read_bn_input: bad argument");
+  LayerPlan& L = t->m->layers[layer];
+  SSDK_REQUIRE(L.bn_train, "ssdk_trainer_read_bn_input: layer %d has no BatchNormalization", layer);
+  return launch_unpack(t->m->ctx, L.z, out_dev, (cudaStream_t)stream_);
 }
 
 extern "C" int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream_) {

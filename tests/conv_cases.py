@@ -1,4 +1,5 @@
-"""Case tables and the GPU harness of the convolution tests (tests/test_gpu_ops.py, tests/test_gpu_conv_heads.py).
+"""Case tables and the GPU harness of the convolution tests (tests/test_gpu_ops.py, tests/test_gpu_conv_heads.py,
+tests/test_gpu_backward_kernels.py).
 
 Every case is a small graph described to ssdk_model_create directly: a float32 tensor input (any channel count) and the layer
 under test.  The tables are plain data, so that a CPU test can check that together they reach every kernel variant the plan
@@ -139,23 +140,30 @@ class Graph:
             d = descs[i]
             d.op = L.get('op', _ffi.OP_CONV)
             d.input = L.get('input', i - 1)
-            d.cout, d.kh, d.kw = L.get('cout', 0), L['k'], L['k']
+            d.cout, d.kh, d.kw = L.get('cout', 0), L.get('k', 0), L.get('k', 0)
             d.stride, d.dilation = L.get('stride', 1), L.get('dil', 1)
-            d.pad_t, d.pad_l, d.pad_b, d.pad_r = L['pads']
+            d.pad_t, d.pad_l, d.pad_b, d.pad_r = L.get('pads', (0, 0, 0, 0))
             d.act, d.n_boxes = ACTS[L.get('act')], L.get('n_boxes', 0)
-            d.kernel = fptr(L['kernel'])
+            if L.get('kernel') is not None:                   # conv / head kernel, or an L2Normalization's gamma
+                d.kernel = fptr(L['kernel'])
             if L.get('bias') is not None:
                 d.bias = fptr(L['bias'])
             if L.get('kernel2') is not None:
                 d.kernel2, d.bias2 = fptr(L['kernel2']), fptr(L['bias2'])
             if L.get('bn_scale') is not None:
                 d.bn_scale, d.bn_shift = fptr(L['bn_scale']), fptr(L['bn_shift'])
+            if L.get('bn_gamma') is not None:                 # raw BatchNormalization parameters (training plans: bn_train)
+                d.bn_gamma, d.bn_beta = fptr(L['bn_gamma']), fptr(L['bn_beta'])
+                d.bn_mean, d.bn_var = fptr(L['bn_mean']), fptr(L['bn_var'])
+                d.bn_eps, d.bn_momentum = L.get('bn_eps', 1e-3), L.get('bn_momentum', 0.99)
         anc = fptr(anchors if anchors is not None else np.zeros(4, np.float32))
         md = _ffi.ModelDesc(B, H, W, cin, n_classes, n, descs, 0 if prec == 'bf16x3' else 1, anc,
                             (C.c_float * 4)(*[float(v) for v in variances]), 1 if training else 0)
         self.h = C.c_void_p()
         self.t = None
         _ffi.check(_ffi.lib().ssdk_model_create(_ffi.context(), C.byref(md), C.byref(self.h)))
+        self.split = prec == 'bf16x3'
+        self.grad_layers = list(range(1, n))                   # every layer but the tensor input has gradient planes
         P = C.c_int()
         _ffi.check(_ffi.lib().ssdk_model_num_priors(self.h, C.byref(P)))
         self.P = P.value
@@ -178,6 +186,71 @@ class Graph:
             self.t = C.c_void_p()
             _ffi.check(L.ssdk_trainer_create(self.h, _ffi.dptr(self.grad), C.byref(self.t)))
         return _ffi.trainer_layer_plan(self.t, layer)
+
+    def planes(self, layer):
+        """The raw forward activation planes of a layer -> (hi, lo, pad), uint16 (B, Hp, Wp, Cs), lo None in bf16 mode."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        hp, wp, cs, pad = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        _ffi.check(_ffi.lib().ssdk_model_layer_planes_shape(self.h, layer, C.byref(hp), C.byref(wp), C.byref(cs), C.byref(pad)))
+        shape = (self.B, hp.value, wp.value, cs.value)
+        hi = torch.empty(shape, dtype=torch.int16, device='cuda')
+        lo = torch.empty(shape, dtype=torch.int16, device='cuda') if self.split else None
+        _ffi.check(_ffi.lib().ssdk_model_read_layer_planes(self.h, layer, _ffi.dptr(hi), _ffi.dptr(lo), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return hi.cpu().numpy().view(np.uint16), (None if lo is None else lo.cpu().numpy().view(np.uint16)), pad.value
+
+    def grad_planes(self, layer):
+        """The raw gradient planes of a layer -> (hi, lo) uint16 arrays (B, Hp, Wp, Cs), lo None in bf16 mode, and the pad."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        hp, wp, cs, pad = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        _ffi.check(_ffi.lib().ssdk_trainer_grad_shape(self.t, layer, C.byref(hp), C.byref(wp), C.byref(cs), C.byref(pad)))
+        shape = (self.B, hp.value, wp.value, cs.value)
+        hi = torch.empty(shape, dtype=torch.int16, device='cuda')
+        lo = torch.empty(shape, dtype=torch.int16, device='cuda') if self.split else None
+        _ffi.check(_ffi.lib().ssdk_trainer_read_grad_planes(self.t, layer, _ffi.dptr(hi), _ffi.dptr(lo), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return hi.cpu().numpy().view(np.uint16), (None if lo is None else lo.cpu().numpy().view(np.uint16)), pad.value
+
+    def read_grad(self, layer):
+        """hi + lo of a layer's gradient as float32 (B,H,W,C) (ssdk_trainer_read_grad)."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        h, w, c = C.c_int(), C.c_int(), C.c_int()
+        _ffi.check(_ffi.lib().ssdk_model_layer_shape(self.h, layer, C.byref(h), C.byref(w), C.byref(c)))
+        out = torch.empty((self.B, h.value, w.value, c.value), dtype=torch.float32, device='cuda')
+        _ffi.check(_ffi.lib().ssdk_trainer_read_grad(self.t, layer, _ffi.dptr(out), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return out.cpu().numpy()
+
+    def read_bn_input(self, layer):
+        """The raw convolution output z a BatchNormalization layer normalised (ssdk_trainer_read_bn_input)."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        h, w, c = C.c_int(), C.c_int(), C.c_int()
+        _ffi.check(_ffi.lib().ssdk_model_layer_shape(self.h, layer, C.byref(h), C.byref(w), C.byref(c)))
+        out = torch.empty((self.B, h.value, w.value, c.value), dtype=torch.float32, device='cuda')
+        _ffi.check(_ffi.lib().ssdk_trainer_read_bn_input(self.t, layer, _ffi.dptr(out), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return out.cpu().numpy()
+
+    def snapshot(self):
+        """Every gradient buffer (raw planes) and the flat parameter gradient."""
+        import torch
+        torch.cuda.synchronize()
+        planes = {i: self.grad_planes(i) for i in self.grad_layers}
+        return planes, self.grad.cpu().numpy().copy()
+
+    def step(self, layer, dy):
+        """Run the backward launches of one layer (ssdk_train_backward_layers(t, dy, layer, layer)) -> (before, after) snapshots.
+        A pass must start at the top layer and go down one layer per call."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        before = self.snapshot()
+        _ffi.check(_ffi.lib().ssdk_train_backward_layers(self.t, _ffi.dptr(dy), layer, layer, _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return before, self.snapshot()
 
     def forward(self, x, width=0):
         """x float32 (B,H,W,cin) -> y_pred (B,P,width) or None."""
@@ -252,3 +325,25 @@ def perturbations(plan, taps, cin, split_products, bias):
 def assert_plan(plan, expect, name):
     for key, v in expect.items():
         assert plan[key] == v, '%s: plan %s = %r, expected %r (full plan %r)' % (name, key, plan[key], v, plan)
+
+
+def plane_values(planes):
+    """(hi, lo, pad) raw planes -> (hi, lo) float32 arrays of the whole padded grid (lo None stays None)."""
+    hi, lo, _ = planes
+    return opexact.bf16_bits_to_f32(hi), (None if lo is None else opexact.bf16_bits_to_f32(lo))
+
+
+def interior(planes, H, W, C_):
+    """The (B,H,W,C) values of raw planes -> (hi, lo) float32, lo None in bf16 mode."""
+    hi, lo = plane_values(planes)
+    pad = planes[2]
+    cut = (slice(None), slice(pad, pad + H), slice(pad, pad + W), slice(0, C_))
+    return hi[cut], (None if lo is None else lo[cut])
+
+
+def outside(planes, H, W, C_):
+    """The stored values outside the (B,H,W,C) interior: zero border and padding channels, both planes."""
+    pad = planes[2]
+    keep = np.ones(planes[0].shape, bool)
+    keep[:, pad:pad + H, pad:pad + W, :C_] = False
+    return [p[keep] for p in planes[:2] if p is not None]

@@ -172,3 +172,278 @@ def test_head_case_table_reaches_every_variant():
     unfused = [(c, e) for c, e in hv if not e['head_fused']]
     assert any(c['env'].get('SSDK_NO_HEAD_FUSION') == '1' for c, e in unfused)
     assert any(c['nb'] * (c['C'] + 4) == 200 and c['prec'] == 'bf16x3' and not c['env'] for c, e in unfused)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# backward references
+# ------------------------------------------------------------------------------------------------------------------------------
+def _conv_t(x, w, stride, dil, pads):
+    pt, pl, pb, pr = pads
+    xt = torch.nn.functional.pad(x.permute(0, 3, 1, 2), (pl, pr, pt, pb))
+    return torch.nn.functional.conv2d(xt, w.permute(3, 2, 0, 1), stride=stride, dilation=dil).permute(0, 2, 3, 1)
+
+
+@pytest.mark.parametrize('k,stride,dil,pads', [(3, 1, 1, (1, 1, 1, 1)), (3, 1, 1, (0, 0, 2, 2)), (4, 1, 1, (0, 0, 0, 0)),
+                                               (3, 1, 3, (3, 3, 3, 3)), (3, 2, 1, (1, 1, 1, 1)), (3, 2, 1, (0, 0, 0, 0)),
+                                               (5, 1, 1, (2, 2, 2, 2))])
+def test_backward_references_equal_float64_autograd(k, stride, dil, pads):
+    rng = np.random.default_rng(k * 10 + stride + dil)
+    B, H, W, cin, cout = 2, 9, 8, 16, 24
+    x = rng.standard_normal((B, H, W, cin)).astype(np.float32)
+    w = rng.standard_normal((k, k, cin, cout)).astype(np.float32)
+    xt = torch.from_numpy(x.astype(np.float64)).requires_grad_()
+    wh, wl = opexact.split(w)
+    wt = torch.from_numpy(wh.astype(np.float64) + wl).requires_grad_()
+    y = _conv_t(xt, wt, stride, dil, pads)
+    dz = opexact.split(rng.standard_normal(y.shape).astype(np.float32))
+    # bf16x3 drops dZ_lo * W_lo: autograd of the graph on dZ_hi (with W_hi + W_lo) plus dZ_lo (with W_hi)
+    gx_hi = torch.autograd.grad(y, xt, torch.from_numpy(dz[0].astype(np.float64)), retain_graph=True)[0].numpy()
+    wt_hi = torch.from_numpy(wh.astype(np.float64))
+    xl = torch.from_numpy(x.astype(np.float64)).requires_grad_()
+    gx_lo = torch.autograd.grad(_conv_t(xl, wt_hi, stride, dil, pads), xl, torch.from_numpy(dz[1].astype(np.float64)))[0].numpy()
+    mask = rng.standard_normal((B, H, W, cin)).astype(np.float32)
+    old = rng.standard_normal((B, H, W, cin))
+    ref, A, _ = opexact.dgrad_ref(dz, w, (H, W), stride=stride, dil=dil, pads=pads, mask=mask, old=old)
+    np.testing.assert_allclose(ref, (gx_hi + gx_lo) * (mask > 0) + old, rtol=1e-12, atol=1e-12)
+    # weight gradient on the split operands: X_hi dZ_hi + X_hi dZ_lo + X_lo dZ_hi
+    xh, xlo = opexact.split(x)
+    want = 0
+    for a, d in [(xh, dz[0]), (xh, dz[1]), (xlo, dz[0])]:
+        wv = torch.from_numpy(w.astype(np.float64)).requires_grad_()
+        want = want + torch.autograd.grad(_conv_t(torch.from_numpy(a.astype(np.float64)), wv, stride, dil, pads), wv,
+                                          torch.from_numpy(d.astype(np.float64)))[0].numpy()
+    ref, A, _ = opexact.wgrad_ref(x, dz, k, k, stride=stride, dil=dil, pads=pads)
+    np.testing.assert_allclose(ref, want.transpose(3, 0, 1, 2), rtol=1e-12, atol=1e-12)
+
+
+def test_dgrad_and_wgrad_bounds_accept_fp32_and_reject_perturbations():
+    rng = np.random.default_rng(3)
+    B, H, W, cin, cout, k = 2, 10, 9, 16, 80, 3
+    pads = (1, 1, 1, 1)
+    x = rng.standard_normal((B, H, W, cin)).astype(np.float32)
+    w = (rng.standard_normal((k, k, cin, cout)) * 0.2).astype(np.float32)
+    dz = opexact.split(rng.standard_normal((B, H, W, cout)).astype(np.float32))
+    mask = rng.standard_normal((B, H, W, cin)).astype(np.float32)
+    old = opexact.bf16_rne(rng.standard_normal((B, H, W, cin)).astype(np.float32)).astype(np.float64)
+    pert = [('cross',), ('tap', 4), ('kblock', 4, 1), ('mask',), ('old',)]
+    ref, A, perts = opexact.dgrad_ref(dz, w, (H, W), pads=pads, mask=mask, old=old, perturb=pert)
+    # fp32 emulation: the same products, summed in float32 (torch float32 autograd), then mask, accumulation and the split store
+    wh, wl = opexact.split(w)
+    got = 0
+    for d, kk in [(dz[0], wh), (dz[0], wl), (dz[1], wh)]:
+        xt = torch.zeros((B, H, W, cin), dtype=torch.float32, requires_grad=True)
+        got = got + torch.autograd.grad(_conv_t(xt, torch.from_numpy(kk), 1, 1, pads), xt, torch.from_numpy(d))[0]
+    got = (got.numpy() * (mask > 0) + old.astype(np.float32)).astype(np.float32)
+    got = np.sum(opexact.split(got), axis=0, dtype=np.float64)
+    bnd = opexact.bound(ref, A, opexact.n_steps_gemm(9, 2) + 1, 'split')
+    assert opexact.err_ratio(got, ref, bnd) <= 1.0
+    for p, r in perts.items():
+        assert opexact.err_ratio(got, r, bnd) > 1.0, p
+    plan = dict(wgrad='transposed', kv=B * (H + 2) * 16, k_split=1)
+    ref, A, perts = opexact.wgrad_ref(x, dz, k, k, pads=pads, perturb=[('cross',), ('tap', 4), ('kblock', 0), ('pixels', 0, 0, 0, 8, 8)])
+    xh, xlo = opexact.split(x)
+    got = 0
+    for a, d in [(xh, dz[0]), (xh, dz[1]), (xlo, dz[0])]:
+        wv = torch.zeros((k, k, cin, cout), dtype=torch.float32, requires_grad=True)
+        got = got + torch.autograd.grad(_conv_t(torch.from_numpy(a), wv, 1, 1, pads), wv, torch.from_numpy(d))[0]
+    got = got.numpy().transpose(3, 0, 1, 2)
+    bnd = opexact.bound(ref, A, opexact.n_steps_wgrad(plan, 3), 'f32')
+    assert opexact.err_ratio(got, ref, bnd) <= 1.0
+    for p, r in perts.items():
+        assert opexact.err_ratio(got, r, bnd) > 1.0, p
+
+
+def test_perturbed_backward_references_equal_recomputed_ones():
+    rng = np.random.default_rng(4)
+    B, H, W, cin, cout, k = 1, 7, 6, 8, 72, 3
+    pads = (1, 1, 1, 1)
+    w = rng.standard_normal((k, k, cin, cout)).astype(np.float32)
+    dz = opexact.split(rng.standard_normal((B, H, W, cout)).astype(np.float32))
+    _, _, perts = opexact.dgrad_ref(dz, w, (H, W), pads=pads, perturb=[('tap', 4), ('kblock', 4, 1)])
+    w_tap = w.copy()
+    w_tap[1, 1] = 0
+    np.testing.assert_allclose(perts[('tap', 4)], opexact.dgrad_ref(dz, w_tap, (H, W), pads=pads)[0], rtol=1e-12, atol=1e-12)
+    d_blk = [d.copy() for d in dz]
+    full = opexact.dgrad_ref(dz, w, (H, W), pads=pads)[0]
+    for d in d_blk:
+        d[..., 64:] = 0
+    w_t = np.zeros_like(w)
+    w_t[1, 1] = w[1, 1]
+    only_blk = opexact.dgrad_ref(dz, w_t, (H, W), pads=pads)[0] - opexact.dgrad_ref(d_blk, w_t, (H, W), pads=pads)[0]
+    np.testing.assert_allclose(perts[('kblock', 4, 1)], full - only_blk, rtol=1e-12, atol=1e-12)
+
+
+def _pool_loop(x, g, KH, KW, s, pt, pl, last=False):
+    B, H, W, Cc = x.shape
+    out = np.zeros(x.shape)
+    for b in range(B):
+        for c in range(Cc):
+            for yo in range(g.shape[1]):
+                for xo in range(g.shape[2]):
+                    best, at = None, None
+                    for ky in range(KH):
+                        for kx in range(KW):
+                            y, xx = yo * s - pt + ky, xo * s - pl + kx
+                            if 0 <= y < H and 0 <= xx < W:
+                                v = x[b, y, xx, c]
+                                if best is None or v > best or (last and v == best):
+                                    best, at = v, (y, xx)
+                    out[b, at[0], at[1], c] += g[b, yo, xo, c]
+    return out
+
+
+@pytest.mark.parametrize('KH,s,pads', [(2, 2, (0, 0, 0, 0)), (2, 2, (0, 0, 1, 1)), (3, 1, (1, 1, 1, 1))])
+def test_pool_route_matches_a_literal_loop_on_ties(KH, s, pads):
+    rng = np.random.default_rng(KH + s)
+    x = rng.integers(-2, 3, (2, 7, 9, 3)).astype(np.float32)
+    Ho, Wo = (7 + pads[0] + pads[2] - KH) // s + 1, (9 + pads[1] + pads[3] - KH) // s + 1
+    g = rng.standard_normal((2, Ho, Wo, 3))
+    r, _, _ = opexact.pool_route(x, g, KH, KH, s, pads[0], pads[1])
+    np.testing.assert_allclose(r, _pool_loop(x, g, KH, KH, s, pads[0], pads[1]), rtol=1e-12, atol=1e-12)
+    rl, _, _ = opexact.pool_route(x, g, KH, KH, s, pads[0], pads[1], last=True)
+    np.testing.assert_allclose(rl, _pool_loop(x, g, KH, KH, s, pads[0], pads[1], last=True), rtol=1e-12, atol=1e-12)
+    assert not np.allclose(r, rl), 'the inputs must contain tied maxima'
+    old = rng.standard_normal(x.shape)
+    ref, A, steps, perts = opexact.pool_bwd_ref(x, g, KH, KH, s, pads[0], pads[1], relu_mask=True, old=old,
+                                                perturb=[('last',), ('mask',), ('old',)])
+    np.testing.assert_allclose(ref, r * (x > 0) + old, rtol=1e-12, atol=1e-12)
+    bnd = opexact.bound(ref, A, steps, 'split')
+    got = np.sum(opexact.split((r * (x > 0)).astype(np.float32) + old.astype(np.float32)), axis=0, dtype=np.float64)
+    assert opexact.err_ratio(got, ref, np.maximum(bnd, 1e-300)) <= 1.0
+    for p, v in perts.items():
+        assert opexact.err_ratio(got, v, np.maximum(bnd, 1e-300)) > 1.0, p
+
+
+def test_l2norm_and_head_backward_references_equal_autograd():
+    rng = np.random.default_rng(5)
+    x = rng.standard_normal((2, 4, 5, 12))
+    x[0, 1, 1] = 0.0                                                     # the clamped branch
+    gy = rng.standard_normal(x.shape)
+    gamma = rng.uniform(0.5, 20, 12)
+    xt, gt = torch.from_numpy(x).requires_grad_(), torch.from_numpy(gamma).requires_grad_()
+    y = gt * xt * torch.rsqrt(torch.clamp((xt * xt).sum(-1, keepdim=True), min=1e-12))
+    gx, gg = torch.autograd.grad(y, (xt, gt), torch.from_numpy(gy))
+    ref, A, kap, gref, gA, gsteps, perts = opexact.l2norm_bwd_ref(x, gy, gamma, perturb=[('proj',)])
+    np.testing.assert_allclose(ref, gx.numpy(), rtol=1e-10, atol=1e-10)
+    np.testing.assert_allclose(gref, gg.numpy(), rtol=1e-10, atol=1e-10)
+    # fp32 emulation of the kernel passes, dropping the projection does not
+    x32, d32, g32 = x.astype(np.float32), gy.astype(np.float32), gamma.astype(np.float32)
+    ss = (x32 * x32).sum(-1, keepdims=True, dtype=np.float32)
+    s = (1 / np.sqrt(np.maximum(ss, np.float32(1e-12)))).astype(np.float32)
+    dot = (g32 * d32 * x32).sum(-1, keepdims=True, dtype=np.float32)
+    got = s * g32 * d32 - np.where(ss > 1e-12, x32 * s * s * s * dot, 0)
+    bnd = kap * A + opexact.UNIT['f32'] * np.abs(ref)
+    assert opexact.err_ratio(got, ref, np.maximum(bnd, 1e-300)) <= 1.0
+    assert opexact.err_ratio(got, perts[('proj',)], np.maximum(bnd, 1e-300)) > 1.0
+    # head: softmax backward on the class columns, pass-through on the offsets
+    nb, Cc = 3, 21
+    z = rng.standard_normal((2, 3, 4, nb * (Cc + 4))) * 4
+    dy = rng.standard_normal((2, 3, 4, nb, Cc + 12))
+    zt = torch.from_numpy(z.reshape(2, 3, 4, nb, Cc + 4)).requires_grad_()
+    out = torch.cat([torch.softmax(zt[..., :Cc], -1), zt[..., Cc:]], -1)
+    want = torch.autograd.grad(out, zt, torch.from_numpy(dy[..., :Cc + 4]))[0].numpy().reshape(z.shape)
+    ref, A, kap, perts = opexact.head_bwd_ref(z, dy, nb, Cc, perturb=[('dot',)])
+    np.testing.assert_allclose(ref, want, rtol=1e-10, atol=1e-12)
+    z32 = z.reshape(2, 3, 4, nb, Cc + 4).astype(np.float32)
+    e = np.exp(z32[..., :Cc] - z32[..., :Cc].max(-1, keepdims=True))
+    p = e / e.sum(-1, keepdims=True, dtype=np.float32)
+    d32 = dy.astype(np.float32)
+    cls = p * (d32[..., :Cc] - (p * d32[..., :Cc]).sum(-1, keepdims=True, dtype=np.float32))
+    got = np.concatenate([cls, d32[..., Cc:Cc + 4]], -1).reshape(z.shape)
+    bnd = np.maximum(kap * A + opexact.UNIT['f32'] * np.abs(ref), 1e-300)
+    assert opexact.err_ratio(got, ref, bnd) <= 1.0
+    assert opexact.err_ratio(got, perts[('dot',)], bnd) > 1.0
+
+
+def test_backward_case_table_reaches_every_variant():
+    import test_gpu_backward_kernels as tb
+    seen = {}
+    for c in tb.BACKWARD_CASES:
+        for i, e in c['expect'].items():
+            seen.setdefault(c['prec'], []).append(e)
+    allp = [e for v in seen.values() for e in v]
+
+    def has(prec=None, **kv):
+        pool_ = allp if prec is None else seen.get(prec, [])
+        return any(all(e.get(k) == v for k, v in kv.items()) for e in pool_)
+    for bn in (64, 128, 160):
+        assert has('bf16x3', dgrad='gemm', dgrad_bn=bn), bn
+    for bn in (64, 128, 256):
+        assert has('bf16', dgrad='gemm', dgrad_bn=bn), bn
+    for m in (0, 1):
+        for a in (0, 1):
+            assert has(dgrad='strided', dgrad_mask=m, dgrad_accumulate=a), ('strided', m, a)
+            assert has(dgrad='gemm', dgrad_mask=m, dgrad_accumulate=a), ('gemm', m, a)
+    assert has('bf16', dgrad='strided') and has('bf16x3', dgrad='strided')
+    assert has(wgrad='native', k_split=1) and has(wgrad='native', min_k_split=2)
+    assert has(wgrad='transposed', k_split=1) and has(wgrad='transposed', min_k_split=2)
+    assert has(wgrad='direct', direct_fast=1) and has(wgrad='direct', direct_fast=0)
+    for bw in (16, 32, 64):
+        assert has(wgrad='native', bw=bw), bw
+    assert has(wgrad='native', wgrad_bn=64) and has(wgrad='native', wgrad_bn=128) and has('bf16', wgrad='native')
+    assert has(wgrad='native', a_boxes=1) and has(wgrad='native', a_boxes=2) and has(wgrad='native', co_tiles=2)
+    assert has(wgrad='native', ci_tiles=2)
+    assert has('bf16x3', wgrad='transposed') and has('bf16', wgrad='transposed') and has(wgrad='transposed', n_gemms=16)
+    assert has(wgrad='im2col')
+    im2col = [(c, L) for c in tb.BACKWARD_CASES for i, e in c['expect'].items() if e.get('wgrad') == 'im2col'
+              for L in [c['layers'][i - 1]]]
+    assert any(L['stride'] == 2 for c, L in im2col)
+    assert any(L['stride'] == 1 and c['cin'] == 3 and L['input'] in (None, 0) and L['cout'] == 40 for c, L in im2col)
+    # BatchNormalization backward: ELU, ReLU and no activation, C = 24 and 136, both precisions
+    bn = [(c['prec'], L['act'], L['cout']) for c in tb.BACKWARD_CASES for L in c['layers'] if L.get('bn')]
+    assert {a for _, a, _ in bn} == {'elu', 'relu', None} and {24, 136} <= {co for _, _, co in bn}
+    assert {p for p, _, _ in bn} == {'bf16x3', 'bf16'}
+    names = {c['name'] for c in tb.BACKWARD_CASES}
+    for n in ('native_unaligned_dw_span', 'direct3x3_cin3_cout480_51840B', 'direct5x5_cin3_cout176_52800B', 'direct_cin1',
+              'direct3x3_dil2_cin4', 'im2col_cin3_cout40', 'l2norm_linear_zero_pixel', 'l2norm_mask_acc', 'heads_voc25_two',
+              'pool2x2_even_mask', 'pool2x2_odd_endpad_linear_acc', 'pool3x3_s1_p1_mask_acc'):
+        assert n in names, n
+    assert any(c['env'].get('SSDK_WGRAD_TRANSPOSED') == '1' for c in tb.BACKWARD_CASES)
+    # the odd head in front of the unaligned case makes the next span start at an odd float offset
+    c = next(c for c in tb.BACKWARD_CASES if c['name'] == 'native_unaligned_dw_span')
+    assert (c['layers'][0]['nb'] * (c['C'] + 4) * (9 * c['cin'] + 1)) % 2 == 1
+
+
+
+def test_bn_backward_reference_equals_autograd_and_its_bound_rejects_perturbations():
+    rng = np.random.default_rng(6)
+    B, H, W, Cc = 2, 5, 6, 24
+    z = (rng.standard_normal((B, H, W, Cc)) * 2 + 0.5).astype(np.float32)
+    gamma = rng.uniform(0.5, 1.5, Cc).astype(np.float32)
+    beta = (rng.standard_normal(Cc) * 0.2).astype(np.float32)
+    da = rng.standard_normal((B, H, W, Cc)).astype(np.float32)
+    eps = 1e-3
+    for act in ('elu', 'relu', None):
+        zt = torch.from_numpy(z.astype(np.float64)).requires_grad_()
+        gt = torch.from_numpy(gamma.astype(np.float64)).requires_grad_()
+        bt = torch.from_numpy(beta.astype(np.float64)).requires_grad_()
+        mean, var = zt.mean((0, 1, 2)), zt.var((0, 1, 2), unbiased=False)
+        y = gt * (zt - mean) / torch.sqrt(var + float(np.float32(eps))) + bt
+        a = torch.nn.functional.elu(y) if act == 'elu' else torch.relu(y) if act == 'relu' else y
+        gz, gg, gb = torch.autograd.grad(a, (zt, gt, bt), torch.from_numpy(da.astype(np.float64)))
+        a64 = a.detach().numpy()
+        pert = [('m1',), ('m2',)] + ([('elu1',)] if act == 'elu' else [])
+        ref, A, kap, dgam, dbet, Ag, Ab, kp, perts = opexact.bn_bwd_ref(z, a64, da, gamma, act=act, eps=eps, perturb=pert)
+        np.testing.assert_allclose(ref, gz.numpy(), rtol=1e-9, atol=1e-12)
+        np.testing.assert_allclose(dgam, gg.numpy(), rtol=1e-9, atol=1e-12)
+        np.testing.assert_allclose(dbet, gb.numpy(), rtol=1e-9, atol=1e-12)
+        # fp32 emulation of bn_bwd_reduce_kernel + bn_bwd_apply_kernel (fp32 mean / rstd, float64 sums)
+        mean32 = z.astype(np.float64).mean((0, 1, 2)).astype(np.float32)
+        rstd32 = (1.0 / np.sqrt(z.astype(np.float64).var((0, 1, 2)) + np.float32(eps))).astype(np.float32)
+        a32 = a64.astype(np.float32)
+        d = np.where(a32 > 0, np.float32(1), a32 + np.float32(1)) if act == 'elu' else (a32 > 0).astype(np.float32) if act == 'relu' \
+            else np.ones_like(a32)
+        dy = (da * d).astype(np.float32)
+        xh = ((z - mean32) * rstd32).astype(np.float32)
+        m1 = dy.astype(np.float64).mean((0, 1, 2)).astype(np.float32)
+        m2 = (dy * xh).astype(np.float64).mean((0, 1, 2)).astype(np.float32)
+        got = (gamma * rstd32 * (dy - m1 - xh * m2)).astype(np.float32)
+        bnd = kap * A + opexact.UNIT['split'] * np.abs(ref)
+        assert opexact.err_ratio(got, ref, bnd) <= 1.0, act
+        for p, r in perts.items():
+            assert opexact.err_ratio(got, r, bnd) > 1.0, (act, p)
+        g32 = (dy * xh).astype(np.float64).sum((0, 1, 2)).astype(np.float32)
+        assert opexact.err_ratio(g32, dgam, kp * Ag) <= 1.0
+        # each perturbed reference equals one recomputed without the dropped part
+        if act == 'elu':
+            np.testing.assert_allclose(perts[('elu1',)], opexact.bn_bwd_ref(z, a64, da, gamma, act=None, eps=eps)[0], rtol=1e-12, atol=1e-12)
