@@ -442,6 +442,10 @@ int ssdk_trainer_read_bn_stats(ssdk_trainer* t, int layer, float* mean_dev, floa
 int ssdk_trainer_read_bn_input(ssdk_trainer* t, int layer, float* out_dev, void* stream);
 /* Copy the current float32 master parameters (same order / layout as the gradients) to out_dev. */
 int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream);
+/* Copy one slot of the optimiser state (same order / layout as the gradients, kernels OHWI) to out_dev (read-only):
+ * slot 0 = the SGD velocity or the Adam first moment m, slot 1 = the Adam second moment v (an error before the first Adam
+ * update, and for any other slot). */
+int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out_dev, void* stream);
 
 /* Read-only view of the backward launches ssdk_trainer_create planned for one convolution or head (host only). */
 enum ssdk_dgrad_path { SSDK_DGRAD_NONE = 0, SSDK_DGRAD_GEMM = 1 /* implicit GEMM into the producer's gradient planes */,

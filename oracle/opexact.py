@@ -44,6 +44,41 @@ returns (ref, A, {perturbation: ref'}) and is judged with the same form |g - ref
 5. Pointwise chains (softmax backward, L2Normalization backward) carry a relative error per fp32 operation; each is
    written as kappa * A with A the sum of the absolute values of the terms, see the functions.
 
+The optimiser updates and the training-phase forward launches that are not convolutions (``sgd_ref``, ``adam_ref``,
+``bn_fwd_ref``, ``l2norm_fwd_ref``, ``pool_fwd_ref``, ``preprocess_ref``) take the operands the launch read and return
+per-element bounds.  train.cu, bn.cu and conv.cu build with --fmad=true, so the compiler may contract a product and an add into
+one FMA: every bound counts a product and an add as two roundings, which covers the contracted form (one rounding) as well.
+u = 2**-24 is the unit roundoff of fp32; a rounding of a value t loses at most u |t|.  expm1f is within 1 ulp, rsqrtf within
+2 ulps, sqrtf and division are correctly rounded.
+
+6. SGD (sgd_kernel_w / sgd_kernel_flat): grad = g s + 2 l2 w, v' = mom v - lr grad, w' = w + v'.  Six roundings (g s, 2 l2 w,
+   their sum, lr grad, mom v, the difference), each at most u times A_v = |mom v| + |lr| (|g s| + 2 l2 |w|), which bounds every
+   intermediate:  |v' - v'_ref| <= 8 u A_v.  w' adds one rounding of its own, the store; as everywhere in this module one unit
+   of the stored format (2**-23 for fp32) is added:  |v' - v'_ref| <= 8 u A_v + 2**-23 |v'_ref|, the same for w'.
+7. Adam (adam_kernel_w / adam_kernel_flat): grad as in 6.; m' = b1 m + (1 - b1) grad (1 - b1 is exact for b1 in [1/2, 1]);
+   v' = b2 v + (1 - b2) grad^2; w' = w - lr_t m' / (sqrtf(v') + eps), lr_t = fp32(fp32(sqrt(1 - b2^t) / (1 - b1^t)) lr).
+   m' carries the 3 roundings of grad and 3 of its own: |m' - m'_ref| <= 8 u A_m, A_m = |b1 m| + (1 - b1) G, G = |g s| + 2 l2 |w|.
+   v' has no cancellation but grad's error enters squared (6 u) and v' adds 4 roundings: |v' - v'_ref| <= 16 u A_v,
+   A_v = b2 v + (1 - b2) G^2.  The denominator D = sqrt(v') + eps moves by E_D = e_v / (sqrt(v'_ref) + sqrt(max(v'_ref - e_v, 0)))
+   + 2 u D (|sqrt x - sqrt y| = |x - y| / (sqrt x + sqrt y), the square root and the add).  The numerator N = lr_t m' moves by
+   lr_t e_m + 3 u |N| (lr_t's two roundings and the product).  The quotient adds one rounding: |N/D - N_ref/D_ref| <=
+   e_N / (D - E_D) + |N| E_D / (D (D - E_D)) + u |N/D|, and w' one more, the store (one unit, 2**-23 |w'_ref|, for each array).
+8. BatchNormalization forward (bn_stats_kernel, bn_finalize_kernel, bn_apply_kernel): the batch sums are float64; mean and
+   rstd = 1 / sqrt(var + eps) are rounded to fp32 once (u each).  var = E[z^2] - mean^2 from float64 sums of N terms loses at
+   most (N + 4) 2**-53 (E[z^2] + 2 |mean| E|z|); rstd then carries that over 2 (var + eps) as a relative r on top.  a = act(gamma ((z - mean) rstd) + beta): with
+   X = (|z - mean| + |mean|) rstd, the subtraction, the mean's rounding, rstd's rounding and the product lose 4 u X, the
+   gamma product and the beta add 2 u (|gamma| X + |beta|); ReLU and ELU are 1-Lipschitz, expm1f adds 2 u |a|.
+   |a - a_ref| <= 8 u (|gamma| X (1 + r / 8u) + |beta|) + 2 u |a_ref| + unit |a_ref|.  The moving statistics follow the
+   recurrence of bn_finalize_kernel, x' = mom x + (1 - mom) s with s the fp32 batch mean or the unbiased variance var N / (N - 1):
+   four roundings of at most A = |mom x| + |(1 - mom) s|, |x' - x'_ref| <= 8 u A + 2**-23 |x'_ref| (the batch variance's own r
+   included).
+9. L2Normalization forward (l2norm_kernel, l2norm8_kernel): y = x s gamma, s = rsqrtf(max(sum x^2, 1e-12)).  The sum of C
+   non-negative squares loses at most (C + 1) u of itself whatever the order; rsqrtf adds 4 u and halves the sum's error; the two
+   products 2 u.  |y - y_ref| <= ((C + 1) / 2 + 8) u |y_ref| + unit |y_ref|.  A clamped pixel (sum x^2 <= 1e-12 in fp32) takes
+   s = rsqrt(1e-12): max is continuous, so the reference uses the same formula in float64.
+10. Max-pooling and the input preprocessing move or compute values without an accumulation: ``pool_fwd_ref`` (the hi and lo
+   planes of the first maximum of hi + lo) and ``preprocess_ref`` ((x - mean) / std in fp32, channel swap, split) are bit-exact.
+
 The module is CPU only: NumPy for the bit-level rounding, torch float64 for the convolutions.
 """
 import numpy as np
@@ -117,7 +152,8 @@ def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3',
              perturb=()):
     """Operand-exact reference of one convolution + epilogue -> (y_ref, A, {perturbation: perturbed y_ref}), float64 NHWC.
 
-    x: the layer's input as the kernel reads it, float32 NHWC (split here exactly as the kernel's planes were).
+    x: the layer's input as the kernel reads it, float32 NHWC (split here exactly as the kernel's planes were), or the stored
+    planes (hi, lo) of a layer output as float32 (lo None in bf16 mode), multiplied as they are.
     w: the float32 HWIO kernel the plan was given.  mode: 'bf16x3' | 'bf16' (split products) or 'fp32' (conv_direct_kernel).
     perturb: perturbations for the sensitivity checks, each a tuple -- ('cross',) drops hi*lo; ('tap', t) drops tap t;
     ('taps', t0, t1) drops taps [t0, t1) (one 64-column K block of conv_first_kernel: 16 taps x 4 channels);
@@ -126,12 +162,13 @@ def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3',
     A perturbed reference differs from y_ref by the dropped products only; it is judged with the unperturbed bound."""
     geo = dict(stride=stride, dil=dil, pads=pads)
     if mode == 'fp32':
-        x32, w32 = np.asarray(x, np.float32), np.asarray(w, np.float32)
+        x32 = np.sum(_planes(x), axis=0, dtype=np.float32) if isinstance(x, tuple) else np.asarray(x, np.float32)
+        w32 = np.asarray(w, np.float32)
         terms = [(x32, w32)]
         z = conv64(x32, w32, **geo)
         A = conv64(np.abs(x32), np.abs(w32), **geo)
     else:
-        xh, xl = split(x)
+        xh, xl = _planes(x) if isinstance(x, tuple) else split(x)
         wh, wl = split(w)
         if mode == 'bf16x3':
             terms = [(xh, wh), (xh, wl), (xl, wh)]
@@ -533,3 +570,208 @@ def bn_bwd_ref(z, a, da, gamma, act=None, eps=1e-3, perturb=()):
     dgamma, dbeta = (dy * xh).sum(axes), dy.sum(axes)
     Ag, Ab = (np.abs(dy) * X).sum(axes), np.abs(dy).sum(axes)
     return ref, A, 16 * 2.0 ** -23, dgamma, dbeta, Ag, Ab, 8 * 2.0 ** -23, out
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# optimiser updates and the training-phase forward launches that are not convolutions (sections 6 - 10)
+# ------------------------------------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24
+
+
+def _f64(a):
+    """float32 operands (or Python scalars the launch receives as float) -> their float64 values."""
+    return np.asarray(a, np.float32).astype(np.float64)
+
+
+def state_ratio(got, ref, bnd):
+    """max |got - ref| / bound over the arrays of an update ({'w': ..., 'm': ...}); a zero bound admits only exact values."""
+    r = 0.0
+    for k in ref:
+        b = np.maximum(np.asarray(bnd[k], np.float64), np.finfo(np.float64).tiny)
+        r = max(r, err_ratio(np.asarray(got[k], np.float64).reshape(ref[k].shape), ref[k], b))
+    return r
+
+
+def _grad(g, w, l2, scale, kernel_shape, p):
+    """The gradient an update reads (section 6) and G = |g s| + 2 l2 |w|; p: the perturbation that changes it, or None."""
+    g, w = _f64(g), _f64(w)
+    if p == ('hwio',):                                               # the flat gradient indexed like the HWIO master
+        cout, kh, kw, cin = kernel_shape
+        g = g.reshape(kh, kw, cin, cout).transpose(3, 0, 1, 2).reshape(g.shape)
+    s = 1.0 if p == ('no_scale',) else float(np.float32(scale))
+    l2 = float(np.float32(l2))
+    if kernel_shape is None:
+        l2 = l2 if p == ('l2_all',) else 0.0
+    elif p == ('no_l2',):
+        l2 = 0.0
+    return g * s + 2.0 * l2 * w, np.abs(g * s) + 2.0 * l2 * np.abs(w)
+
+
+def sgd_ref(w, v, g, lr, momentum, l2=0.0, scale=1.0, kernel_shape=None, perturb=()):
+    """One SGD update of one parameter span (sgd_kernel_w / sgd_kernel_flat) -> (ref, bound, {perturbation: ref'}), each a dict
+    {'w': new master, 'v': new velocity}, float64.
+
+    w, v, g: the master, the velocity and the gradient as the launch read them, in the gradient's layout (kernels OHWI, as
+    ssdk_trainer_read_params / ssdk_trainer_read_opt_state return them).  kernel_shape: (cout, kh, kw, cin) of a conv / head kernel,
+    whose update carries the l2 term; None for biases and gammas.  Bound: section 6.  perturb: ('no_l2',) drops the l2 term;
+    ('l2_all',) applies it to a bias / gamma span; ('no_scale',) ignores grad_scale; ('no_momentum',) drops the carried velocity;
+    ('hwio',) reads the gradient at the HWIO index."""
+    lr, mom = float(np.float32(lr)), float(np.float32(momentum))
+    w64, v64 = _f64(w), _f64(v)
+
+    def update(p=None):
+        grad, G = _grad(g, w, l2, scale, kernel_shape, p)
+        nv = (0.0 if p == ('no_momentum',) else mom * v64) - lr * grad
+        return {'w': w64 + nv, 'v': nv}, G
+    ref, G = update()
+    A = np.abs(mom * v64) + abs(lr) * G
+    unit = UNIT['f32']
+    bnd = {'v': 8 * U32 * A + unit * np.abs(ref['v']), 'w': 8 * U32 * A + unit * np.abs(ref['w'])}
+    return ref, bnd, {p: update(p)[0] for p in perturb}
+
+
+def adam_lr_t(lr, beta1, beta2, t):
+    """Keras' lr_t = lr sqrt(1 - b2^t) / (1 - b1^t) in float64 from the float32 operands."""
+    b1, b2 = float(np.float32(beta1)), float(np.float32(beta2))
+    return float(np.float32(lr)) * np.sqrt(1.0 - b2 ** t) / (1.0 - b1 ** t)
+
+
+def adam_ref(w, m, v, g, lr, beta1, beta2, eps, t, l2=0.0, scale=1.0, kernel_shape=None, perturb=()):
+    """One Adam update of one parameter span (adam_kernel_w / adam_kernel_flat) -> (ref, bound, {perturbation: ref'}), each a dict
+    {'w': new master, 'm': new first moment, 'v': new second moment}, float64.
+
+    w, m, v, g: as read before the launch, in the gradient's layout; t: the step the update was given (from 1).  Bound: section
+    7.  perturb: the perturbations of sgd_ref that change the gradient, and ('t-1',), ('t+1',) (lr_t of the neighbouring step),
+    ('eps_in_root',) (w -= lr_t m / sqrt(v + eps)), ('no_m',), ('no_v',) (a moment not carried)."""
+    b1, b2, e = float(np.float32(beta1)), float(np.float32(beta2)), float(np.float32(eps))
+    w64, m64, v64 = _f64(w), _f64(m), _f64(v)
+
+    def update(p=None):
+        grad, G = _grad(g, w, l2, scale, kernel_shape, p)
+        a = (0.0 if p == ('no_m',) else b1 * m64) + (1.0 - b1) * grad
+        b = (0.0 if p == ('no_v',) else b2 * v64) + (1.0 - b2) * grad * grad
+        tt = t - 1 if p == ('t-1',) else t + 1 if p == ('t+1',) else t
+        den = np.sqrt(b + e) if p == ('eps_in_root',) else np.sqrt(b) + e
+        return {'w': w64 - adam_lr_t(lr, b1, b2, tt) * a / den, 'm': a, 'v': b}, G
+    ref, G = update()
+    lr_t = adam_lr_t(lr, b1, b2, t)
+    e_m = 8 * U32 * (np.abs(b1 * m64) + (1.0 - b1) * G)
+    e_v = 16 * U32 * (b2 * v64 + (1.0 - b2) * G * G)
+    vr = ref['v']
+    D = np.sqrt(vr) + e
+    with np.errstate(divide='ignore', invalid='ignore'):
+        e_sqrt = np.minimum(np.sqrt(e_v), np.where(e_v > 0, e_v / (np.sqrt(vr) + np.sqrt(np.maximum(vr - e_v, 0.0))), 0.0))
+    e_D = e_sqrt + 2 * U32 * D
+    N = lr_t * np.abs(ref['m'])
+    e_N = lr_t * e_m + 3 * U32 * N
+    D_lo = D - e_D
+    e_step = e_N / D_lo + N * e_D / (D * D_lo) + U32 * N / D
+    unit = UNIT['f32']
+    bnd = {'w': e_step + unit * np.abs(ref['w']), 'm': e_m + unit * np.abs(ref['m']), 'v': e_v + unit * np.abs(vr)}
+    return ref, bnd, {p: update(p)[0] for p in perturb}
+
+
+def bn_fwd_ref(z, gamma, beta, mmean, mvar, act=None, eps=1e-3, momentum=0.99, z_prev=None, perturb=()):
+    """BatchNormalization forward in the training phase (bn_stats_kernel, bn_finalize_kernel, bn_apply_kernel) -> (a_ref, A,
+    kappa, stats_ref, stats_bound, {perturbation: (a', stats')}), float64.  |a - a_ref| <= kappa A + unit |a_ref| (section 8).
+
+    z: the raw convolution output the pass normalised (ssdk_trainer_read_bn_input); mmean, mvar: the moving statistics read
+    before the pass.  stats: {'mean': moving mean after the pass, 'var': moving variance}.  perturb: ('acc',) the accumulator of
+    the previous pass (whose input was z_prev) is not cleared, so its sums are added in; ('biased',) the moving average takes the
+    biased variance; ('no_eps',) rstd = 1 / sqrt(var)."""
+    z = _f64(z)
+    axes = tuple(range(z.ndim - 1))
+    N = float(np.prod(z.shape[:-1]))
+    gm, bt, e, mom = _f64(gamma), _f64(beta), float(np.float32(eps)), float(np.float32(momentum))
+    mm, mv = _f64(mmean), _f64(mvar)
+
+    def run(p=None):
+        s1, s2 = z.sum(axes), (z * z).sum(axes)
+        if p == ('acc',):
+            zp = _f64(z_prev)
+            s1, s2 = s1 + zp.sum(axes), s2 + (zp * zp).sum(axes)
+        mean = s1 / N
+        var = np.maximum(s2 / N - mean * mean, 0.0)
+        rstd = 1.0 / np.sqrt(var + (0.0 if p == ('no_eps',) else e))
+        y = gm * (z - mean) * rstd + bt
+        a = np.maximum(y, 0.0) if act == 'relu' else np.where(y > 0, y, np.expm1(np.minimum(y, 0.0))) if act == 'elu' else y
+        unb = var if p == ('biased',) else var * N / (N - 1.0) if N > 1 else var
+        return a, {'mean': mom * mm + (1.0 - mom) * mean, 'var': mom * mv + (1.0 - mom) * unb}, mean, var, rstd
+    a, stats, mean, var, rstd = run()
+    ez2 = (z * z).mean(axes)
+    r = (N + 4) * 2.0 ** -53 * (ez2 + 2 * np.abs(mean) * np.abs(z).mean(axes)) / (var + e) / 2
+    X = (np.abs(z - mean) + np.abs(mean)) * rstd
+    kap = 8 * U32
+    A = np.abs(gm) * X * (1.0 + r / kap) + np.abs(bt) + (2 * U32 / kap) * np.abs(a)
+    unb = var * N / (N - 1.0) if N > 1 else var
+    sb = {'mean': kap * (np.abs(mom * mm) + (1.0 - mom) * np.abs(mean)) + UNIT['f32'] * np.abs(stats['mean']),
+          'var': kap * (np.abs(mom * mv) + (1.0 - mom) * unb * (1.0 + 2 * r / kap)) + UNIT['f32'] * np.abs(stats['var'])}
+    out = {}
+    for p in perturb:
+        ap, sp = run(p)[:2]
+        out[p] = (ap, sp)
+    return a, A, kap, stats, sb, out
+
+
+def l2norm_fwd_ref(x, gamma, perturb=()):
+    """L2Normalization forward (l2norm_kernel, l2norm8_kernel) -> (y_ref, kappa * |y_ref|, {perturbation: y'}), float64; add
+    unit |y_ref| of the store (section 9).  x: the layer's input as stored (hi + lo).  perturb: ('no_gamma',);
+    ('gamma_shift',) channel c takes gamma[c + 1]."""
+    x = _f64(x)
+    gm = _f64(gamma)
+    Cc = x.shape[-1]
+    s = 1.0 / np.sqrt(np.maximum((x * x).sum(-1, keepdims=True), float(np.float32(1e-12))))
+    y = x * s * gm
+    out = {}
+    for p in perturb:
+        if p == ('no_gamma',):
+            out[p] = x * s
+        elif p == ('gamma_shift',):
+            out[p] = x * s * np.roll(gm, -1)
+    return y, ((Cc + 1) / 2.0 + 8) * U32 * np.abs(y), out
+
+
+def pool_fwd_ref(hi, lo, KH, KW, stride, pad_t, pad_l, Ho, Wo, perturb=()):
+    """Max-pool forward (maxpool_kernel, maxpool2x2_kernel), bit-exact -> (hi_out, lo_out, {perturbation: (hi', lo')}), float32.
+
+    hi, lo: the input planes' values (B,H,W,C) (lo None in bf16 mode).  Each output takes both planes of the FIRST maximum of
+    hi + lo in its window (row-major scan, strict '>', taps outside the input skipped: TF 'same' padding).  perturb: ('hi_only',)
+    compares hi alone; ('lo_tie',) keeps the hi plane but takes lo from the last tap whose hi is the window's largest hi."""
+    hi = np.asarray(hi, np.float32)
+    lo = np.zeros_like(hi) if lo is None else np.asarray(lo, np.float32)
+    v = hi.astype(np.float64) + lo
+    B, H, W, Cc = hi.shape
+    bi, ci = np.meshgrid(np.arange(B), np.arange(Cc), indexing='ij')
+    res = {k: (np.zeros((B, Ho, Wo, Cc), np.float32), np.zeros((B, Ho, Wo, Cc), np.float32)) for k in [None] + list(perturb)}
+    for yo in range(Ho):
+        for xo in range(Wo):
+            pos = [(y, xx) for y in range(yo * stride - pad_t, yo * stride - pad_t + KH) if 0 <= y < H
+                   for xx in range(xo * stride - pad_l, xo * stride - pad_l + KW) if 0 <= xx < W]
+            py, px = np.array([p[0] for p in pos]), np.array([p[1] for p in pos])
+
+            def pick(vals, last=False):
+                win = np.stack([vals[:, y, xx] for y, xx in pos], axis=-1)
+                k = win.shape[-1] - 1 - np.argmax(win[..., ::-1], axis=-1) if last else np.argmax(win, axis=-1)
+                return (bi, py[k], px[k], ci)
+            first = pick(v)
+            for key, (ho, lo_) in res.items():
+                if key == ('hi_only',):
+                    at = pick(hi.astype(np.float64))
+                    ho[:, yo, xo], lo_[:, yo, xo] = hi[at], lo[at]
+                elif key == ('lo_tie',):
+                    ho[:, yo, xo], lo_[:, yo, xo] = hi[first], lo[pick(hi.astype(np.float64), last=True)]
+                else:
+                    ho[:, yo, xo], lo_[:, yo, xo] = hi[first], lo[first]
+    out = res.pop(None)
+    return out[0], out[1], res
+
+
+def preprocess_ref(img, mean=None, std=None, swap=None):
+    """The input layer (preprocess_kernel), bit-exact -> (hi, lo) float32 (B,H,W,3): t = x - mean, t = t / std in fp32 (each
+    correctly rounded), output channel c = t[swap[c]], split into the two planes."""
+    x = np.asarray(img, np.float32)
+    t = x - (np.zeros(3, np.float32) if mean is None else np.asarray(mean, np.float32))
+    if std is not None:
+        t = (t / np.asarray(std, np.float32)).astype(np.float32)
+    t = t[..., list(swap) if swap is not None else [0, 1, 2]]
+    return split(t)

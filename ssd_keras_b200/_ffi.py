@@ -215,7 +215,9 @@ def lib():
             L.ssdk_trainer_read_grad.argtypes = [vp, C.c_int, vp, vp]
             L.ssdk_trainer_read_grad_planes.argtypes = [vp, C.c_int, vp, vp, vp]
             L.ssdk_trainer_read_bn_input.argtypes = [vp, C.c_int, vp, vp]
-            for name in ('ssdk_trainer_grad_shape', 'ssdk_trainer_read_grad', 'ssdk_trainer_read_grad_planes', 'ssdk_trainer_read_bn_input'):
+            L.ssdk_trainer_read_opt_state.argtypes = [vp, C.c_int, vp, vp]
+            for name in ('ssdk_trainer_grad_shape', 'ssdk_trainer_read_grad', 'ssdk_trainer_read_grad_planes', 'ssdk_trainer_read_bn_input',
+                         'ssdk_trainer_read_opt_state'):
                 getattr(L, name).restype = C.c_int
             for name in ('ssdk_trainer_create', 'ssdk_trainer_destroy', 'ssdk_trainer_num_params', 'ssdk_trainer_param_span',
                          'ssdk_train_backward', 'ssdk_train_apply', 'ssdk_trainer_read_params'):

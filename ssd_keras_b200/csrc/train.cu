@@ -415,6 +415,7 @@ struct ssdk_trainer {
   long long xT_elems = 0, dyT_elems = 0;
   float* dypred = nullptr;                  // [B*P*(C+12)]
   std::vector<char> written;                // backward pass state: which activations already hold a partial gradient
+  bool adam = false;                        // an Adam update ran: the second moments exist
   std::vector<void*> allocs;
 };
 
@@ -991,6 +992,33 @@ extern "C" int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, flo
       SSDK_COUNT_LAUNCH(ctx); SSDK_COUNT_LAUNCH(ctx);
     }
     rc = repack_layer(t, (int)i, s); if (rc) return rc;
+  }
+  t->adam = true;
+  SSDK_CHECK_CUDA(cudaGetLastError());
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out_dev, void* stream_) {
+  SSDK_REQUIRE(t && out_dev, "ssdk_trainer_read_opt_state: NULL argument");
+  SSDK_REQUIRE(slot == 0 || (slot == 1 && t->adam),
+               "ssdk_trainer_read_opt_state: slot %d does not exist (0: SGD velocity / Adam first moment, 1: Adam second moment, "
+               "after an Adam update)", slot);
+  ssdk_model* m = t->m;
+  cudaStream_t s = (cudaStream_t)stream_;
+  for (size_t i = 0; i < t->tl.size(); ++i) {
+    TLayer& T = t->tl[i];
+    LayerPlan& L = m->layers[i];
+    if (T.off_g >= 0)
+      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_g, slot ? T.v2gamma : T.vgamma, (size_t)L.C * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (T.off_w < 0) continue;
+    const size_t nw = (size_t)T.taps * T.cin * T.cout;
+    hwio_to_ohwi_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(slot ? T.v2w : T.vw, T.taps, T.cin, T.cout, out_dev + T.off_w);
+    SSDK_COUNT_LAUNCH(m->ctx);
+    SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_b, slot ? T.v2b : T.vb, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    if (T.off_bng >= 0) {
+      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bng, slot ? T.v_bng : T.m_bng, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
+      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bnb, slot ? T.v_bnb : T.m_bnb, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    }
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

@@ -66,12 +66,14 @@ class SSDTrainer:
 
     def _detach(self):
         """Called by the model before it destroys its plans (``set_weights`` / ``load_weights``): the native trainer points
-        into the training plan.  Optimiser state (momentum) does not survive; the next step starts from the new weights."""
+        into the training plan.  Optimiser state (momentum, Adam's moments and its step count) does not survive; the next step
+        starts from the new weights as a fresh trainer's first step would."""
         if self.handle is not None:
             _ffi.lib().ssdk_trainer_destroy(self.handle)
         self.handle = None
         self.plan = None
         self._dirty = False
+        self.iterations = 0
 
     def __del__(self):
         try:

@@ -1,5 +1,5 @@
 """Case tables and the GPU harness of the convolution tests (tests/test_gpu_ops.py, tests/test_gpu_conv_heads.py,
-tests/test_gpu_backward_kernels.py).
+tests/test_gpu_backward_kernels.py, tests/test_gpu_train_step_kernels.py).
 
 Every case is a small graph described to ssdk_model_create directly: a float32 tensor input (any channel count) and the layer
 under test.  The tables are plain data, so that a CPU test can check that together they reach every kernel variant the plan
@@ -123,7 +123,9 @@ class Graph:
     """A tensor input plus conv / head layers, planned by ssdk_model_create (inference plan)."""
 
     def __init__(self, B, H, W, cin, layers, prec='bf16x3', n_classes=0, anchors=None, variances=(0.1, 0.1, 0.2, 0.2),
-                 training=False):
+                 training=False, input_layer=None):
+        """input_layer: None (a float32 tensor input), or dict(mean=, stddev=, swap=) of a model input layer (preprocess_kernel;
+        each entry may be None)."""
         from ssd_keras_b200 import _ffi
         self.B, self.H, self.W, self.cin = B, H, W, cin
         self._keep = []
@@ -135,6 +137,17 @@ class Graph:
             a = np.ascontiguousarray(a, dtype=np.float32)
             self._keep.append(a)
             return _ffi.np_ptr(a, C.c_float)
+
+        if input_layer is not None:
+            descs[0].op = _ffi.OP_INPUT
+            if input_layer.get('mean') is not None:
+                descs[0].mean = fptr(input_layer['mean'])
+            if input_layer.get('stddev') is not None:
+                descs[0].stddev = fptr(input_layer['stddev'])
+            if input_layer.get('swap') is not None:
+                sw = np.ascontiguousarray(input_layer['swap'], dtype=np.int32)
+                self._keep.append(sw)
+                descs[0].swap = _ffi.np_ptr(sw, C.c_int)
 
         for i, L in enumerate(layers, start=1):
             d = descs[i]
@@ -175,6 +188,12 @@ class Graph:
     def backward_plan(self, layer):
         """The trainer's backward plan of a layer (training graphs; the trainer is created on first use)."""
         from ssd_keras_b200 import _ffi
+        self.trainer()
+        return _ffi.trainer_layer_plan(self.t, layer)
+
+    def trainer(self):
+        """The trainer of a training graph, created on first use over a flat gradient buffer the test owns (self.grad)."""
+        from ssd_keras_b200 import _ffi
         if self.t is None:
             import torch
             L = _ffi.lib()
@@ -185,7 +204,47 @@ class Graph:
             self.grad = torch.zeros(n.value, dtype=torch.float32, device='cuda')
             self.t = C.c_void_p()
             _ffi.check(L.ssdk_trainer_create(self.h, _ffi.dptr(self.grad), C.byref(self.t)))
-        return _ffi.trainer_layer_plan(self.t, layer)
+        return self.t
+
+    def apply(self, optimizer, lr, l2=0.0, scale=1.0, momentum=0.9, beta1=0.9, beta2=0.999, eps=1e-8, step=1):
+        """One optimiser update from the flat gradient buffer (ssdk_train_apply / ssdk_train_apply_adam)."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        torch.cuda.synchronize()
+        if optimizer == 'adam':
+            _ffi.check(_ffi.lib().ssdk_train_apply_adam(self.trainer(), lr, beta1, beta2, eps, l2, scale, step, _ffi.stream_ptr()))
+        else:
+            _ffi.check(_ffi.lib().ssdk_train_apply(self.trainer(), lr, momentum, l2, scale, _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+
+    def _flat(self, fn, *args):
+        import torch
+        from ssd_keras_b200 import _ffi
+        out = torch.full_like(self.grad, float('nan'))
+        _ffi.check(fn(self.trainer(), *args, _ffi.dptr(out), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return out.cpu().numpy()
+
+    def params(self):
+        """The float32 master parameters in the gradient's layout (ssdk_trainer_read_params)."""
+        from ssd_keras_b200 import _ffi
+        return self._flat(_ffi.lib().ssdk_trainer_read_params)
+
+    def opt_state(self, slot):
+        """One slot of the optimiser state in the gradient's layout (ssdk_trainer_read_opt_state): 0 = SGD velocity / Adam m,
+        1 = Adam v."""
+        from ssd_keras_b200 import _ffi
+        return self._flat(_ffi.lib().ssdk_trainer_read_opt_state, int(slot))
+
+    def bn_stats(self, layer, C_):
+        """(moving mean, moving variance) of a BatchNormalization layer (ssdk_trainer_read_bn_stats)."""
+        import torch
+        from ssd_keras_b200 import _ffi
+        mu = torch.empty((C_,), dtype=torch.float32, device='cuda')
+        var = torch.empty_like(mu)
+        _ffi.check(_ffi.lib().ssdk_trainer_read_bn_stats(self.trainer(), layer, _ffi.dptr(mu), _ffi.dptr(var), _ffi.stream_ptr()))
+        torch.cuda.synchronize()
+        return mu.cpu().numpy(), var.cpu().numpy()
 
     def planes(self, layer):
         """The raw forward activation planes of a layer -> (hi, lo, pad), uint16 (B, Hp, Wp, Cs), lo None in bf16 mode."""

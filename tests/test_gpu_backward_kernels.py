@@ -183,7 +183,7 @@ def _build(case, seed=0):
             Ho = (H + pads[0] + pads[2] - dil * (k - 1) - 1) // stride + 1
             Wo = (W + pads[1] + pads[3] - dil * (k - 1) - 1) // stride + 1
             info[i] = dict(op=op, input=inp, k=k, pads=pads, stride=stride, dil=dil, w=master, act=spec.get('act'),
-                           bn_gamma=layers[-1].get('bn_gamma'))
+                           bn_gamma=layers[-1].get('bn_gamma'), bn_beta=layers[-1].get('bn_beta'))
             if op == 'head':
                 info[i].update(nb=spec['nb'], prior_off=P)
                 P += Ho * Wo * spec['nb']

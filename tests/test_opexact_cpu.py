@@ -447,3 +447,242 @@ def test_bn_backward_reference_equals_autograd_and_its_bound_rejects_perturbatio
         # each perturbed reference equals one recomputed without the dropped part
         if act == 'elu':
             np.testing.assert_allclose(perts[('elu1',)], opexact.bn_bwd_ref(z, a64, da, gamma, act=None, eps=eps)[0], rtol=1e-12, atol=1e-12)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# optimiser updates and the training-phase forward launches (sections 6 - 10 of oracle/opexact.py)
+# ------------------------------------------------------------------------------------------------------------------------------
+def _fma(a, b, c, contract):
+    """a * b + c in fp32: one rounding (an FMA, emulated exactly enough in float64) or two."""
+    a, b, c = np.float32(a), np.float32(b), np.float32(c)
+    if contract:
+        return (a.astype(np.float64) * b + c).astype(np.float32)
+    return (a * b).astype(np.float32) + c
+
+
+def _opt_operands(rng, n):
+    g = (rng.choice([-1.0, 1.0], n) * 10.0 ** rng.uniform(-9, 2, n)).astype(np.float32)
+    g[rng.random(n) < 0.1] = 0
+    w = (rng.standard_normal(n) * 0.1).astype(np.float32)
+    return w, g
+
+
+KSHAPE = (5, 3, 3, 4)                                                 # OHWI: distinct cout, taps and cin
+
+
+def _grad32(w, g, l2, s, ks, contract):
+    if ks is not None:                                                # the kernel reads g at the OHWI index of HWIO element i
+        g = g.reshape(ks)
+    return _fma(np.float32(2 * np.float32(l2)), w, (g.reshape(w.shape) * np.float32(s)).astype(np.float32), contract)
+
+
+@pytest.mark.parametrize('contract', [False, True])
+@pytest.mark.parametrize('kernel', [True, False])
+def test_sgd_reference_loop_emulation_and_perturbations(contract, kernel):
+    rng = np.random.default_rng(31 + contract)
+    n = int(np.prod(KSHAPE))
+    ks = KSHAPE if kernel else None
+    w, _ = _opt_operands(rng, n)
+    v = np.zeros(n, np.float32)
+    for t, (lr, s, l2) in enumerate([(1e-2, 1.0, 5e-4), (5e-3, 0.5, 5e-4), (2e-3, 0.5, 0.0)], start=1):
+        _, g = _opt_operands(rng, n)
+        perts = [('hwio',), ('no_l2',)] if kernel else [('l2_all',)]
+        perts = [p for p in perts if l2 or p not in (('no_l2',), ('l2_all',))] + ([('no_scale',)] if s != 1 else []) + \
+            ([('no_momentum',)] if t > 1 else [])
+        ref, bnd, pv = opexact.sgd_ref(w, v, g, lr, 0.9, l2=l2, scale=s, kernel_shape=ks, perturb=perts)
+        # a literal float64 loop over the HWIO master, gradient read at the OHWI index
+        want_w, want_v = np.zeros(n), np.zeros(n)
+        for co in range(KSHAPE[0]):
+            for kh in range(3):
+                for kw in range(3):
+                    for ci in range(KSHAPE[3]):
+                        i = ((co * 3 + kh) * 3 + kw) * KSHAPE[3] + ci
+                        gr = float(g[i]) * float(np.float32(s)) + (2 * float(np.float32(l2)) * float(w[i]) if kernel else 0.0)
+                        want_v[i] = float(np.float32(0.9)) * float(v[i]) - float(np.float32(lr)) * gr
+                        want_w[i] = float(w[i]) + want_v[i]
+        np.testing.assert_allclose(ref['v'], want_v, rtol=1e-13, atol=1e-300)
+        np.testing.assert_allclose(ref['w'], want_w, rtol=1e-13, atol=1e-300)
+        # fp32 emulation of sgd_kernel_w / sgd_kernel_flat
+        gr = _grad32(w, g, l2, s, ks, contract) if kernel else (g * np.float32(s)).astype(np.float32)
+        nv = _fma(np.float32(0.9), v, -(np.float32(lr) * gr).astype(np.float32), contract)
+        got = {'w': (w + nv).astype(np.float32), 'v': nv}
+        assert opexact.state_ratio(got, ref, bnd) <= 1.0, t
+        for p, r in pv.items():
+            assert opexact.state_ratio(got, r, bnd) > 1.0, (t, p)
+        w, v = got['w'], got['v']
+
+
+@pytest.mark.parametrize('contract', [False, True])
+def test_adam_reference_loop_emulation_and_perturbations(contract):
+    rng = np.random.default_rng(41 + contract)
+    n = int(np.prod(KSHAPE))
+    w, _ = _opt_operands(rng, n)
+    w[:40] = 0                                                       # no l2 term at the first step: grad = g s exactly
+    m = np.zeros(n, np.float32)
+    v = np.zeros(n, np.float32)
+    b1, b2, eps = np.float32(0.9), np.float32(0.999), np.float32(1e-8)
+    for t, (lr, s, l2) in enumerate([(1e-3, 1.0, 5e-4), (2e-3, 0.5, 5e-4), (1e-3, 1.0, 0.0), (5e-4, 0.5, 0.0), (1e-3, 1.0, 5e-4)], 1):
+        _, g = _opt_operands(rng, n)
+        perts = [('t+1',), ('eps_in_root',)] + ([('t-1',), ('no_m',), ('no_v',)] if t > 1 else [])
+        ref, bnd, pv = opexact.adam_ref(w, m, v, g, lr, b1, b2, eps, t, l2=l2, scale=s, kernel_shape=KSHAPE, perturb=perts)
+        # literal float64 loop, Keras' formulas
+        lr_t = float(np.float32(lr)) * np.sqrt(1 - float(b2) ** t) / (1 - float(b1) ** t)
+        for i in range(n):
+            gr = float(g[i]) * float(np.float32(s)) + 2 * float(np.float32(l2)) * float(w[i])
+            mi = float(b1) * float(m[i]) + (1 - float(b1)) * gr
+            vi = float(b2) * float(v[i]) + (1 - float(b2)) * gr * gr
+            assert abs(ref['m'][i] - mi) <= 1e-13 * abs(mi) and abs(ref['v'][i] - vi) <= 1e-13 * abs(vi)
+            wi = float(w[i]) - lr_t * mi / (np.sqrt(vi) + float(eps))
+            assert abs(ref['w'][i] - wi) <= 1e-13 * abs(wi)
+        # fp32 emulation of adam_kernel_w
+        lr_t32 = np.float32(np.float32(np.sqrt(1.0 - float(b2) ** t) / (1.0 - float(b1) ** t)) * np.float32(lr))
+        gr = _grad32(w, g, l2, s, KSHAPE, contract)
+        a = _fma(b1, m, ((np.float32(1) - b1) * gr).astype(np.float32), contract)
+        b = _fma(b2, v, ((np.float32(1) - b2) * gr * gr).astype(np.float32), contract)
+        den = (np.sqrt(b) + eps).astype(np.float32)
+        w = (w - ((lr_t32 * a).astype(np.float32) / den).astype(np.float32)).astype(np.float32)
+        got = {'w': w, 'm': a, 'v': b}
+        assert opexact.state_ratio(got, ref, bnd) <= 1.0, t
+        for p, r in pv.items():
+            assert opexact.state_ratio(got, r, bnd) > 1.0, (t, p)
+        if t == 1:
+            assert np.any(np.sqrt(b) < eps) and np.any(np.sqrt(b) > 1e3 * eps), 'eps must matter for some elements and not for others'
+        m, v = a, b
+
+
+@pytest.mark.parametrize('act', ['elu', 'relu', None])
+def test_bn_forward_reference_emulation_and_perturbations(act):
+    rng = np.random.default_rng(7)
+    B, H, W, Cc = 2, 5, 6, 24
+    gamma = rng.uniform(0.5, 1.5, Cc).astype(np.float32)
+    beta = (rng.standard_normal(Cc) * 0.2).astype(np.float32)
+    mm, mv = np.zeros(Cc, np.float32), np.ones(Cc, np.float32)
+    z_prev = None
+    for p in range(3):
+        z = np.sum(opexact.split((rng.standard_normal((B, H, W, Cc)) * 0.1 + 0.05 * p).astype(np.float32)), axis=0, dtype=np.float32)
+        perts = [('biased',), ('no_eps',)] + ([('acc',)] if z_prev is not None else [])
+        ref, A, kap, st, sb, pv = opexact.bn_fwd_ref(z, gamma, beta, mm, mv, act=act, z_prev=z_prev, perturb=perts)
+        # float64 autograd-free check: torch's batch_norm in training mode on float64
+        zt = torch.from_numpy(z.astype(np.float64)).permute(0, 3, 1, 2)
+        rm, rv = torch.from_numpy(mm.astype(np.float64)), torch.from_numpy(mv.astype(np.float64))
+        y = torch.nn.functional.batch_norm(zt, rm, rv, torch.from_numpy(gamma.astype(np.float64)), torch.from_numpy(beta.astype(np.float64)),
+                                           training=True, momentum=1 - float(np.float32(0.99)), eps=float(np.float32(1e-3)))
+        y = torch.nn.functional.elu(y) if act == 'elu' else torch.relu(y) if act == 'relu' else y
+        np.testing.assert_allclose(ref, y.permute(0, 2, 3, 1).numpy(), rtol=1e-10, atol=1e-12)
+        np.testing.assert_allclose(st['mean'], rm.numpy(), rtol=1e-10, atol=1e-14)
+        np.testing.assert_allclose(st['var'], rv.numpy(), rtol=1e-10, atol=1e-14)
+        # fp32 emulation of bn_finalize_kernel + bn_apply_kernel, stored as hi + lo
+        z64 = z.astype(np.float64)
+        mean, var = z64.mean((0, 1, 2)), np.maximum((z64 * z64).mean((0, 1, 2)) - z64.mean((0, 1, 2)) ** 2, 0)
+        bm, br = mean.astype(np.float32), (1 / np.sqrt(var + float(np.float32(1e-3)))).astype(np.float32)
+        yy = (gamma * ((z - bm).astype(np.float32) * br).astype(np.float32)).astype(np.float32) + beta
+        a32 = np.maximum(yy, 0) if act == 'relu' else np.where(yy > 0, yy, np.expm1(np.minimum(yy, 0)).astype(np.float32)) if act == 'elu' else yy
+        got = np.sum(opexact.split(a32.astype(np.float32)), axis=0, dtype=np.float64)
+        N = B * H * W
+        mom = np.float32(0.99)
+        gst = {'mean': (mom * mm + (np.float32(1) - mom) * bm).astype(np.float32),
+               'var': (mom * mv + (np.float32(1) - mom) * (var * N / (N - 1)).astype(np.float32)).astype(np.float32)}
+        bnd = kap * A + opexact.UNIT['split'] * np.abs(ref)
+        assert opexact.err_ratio(got, ref, bnd) <= 1.0 and opexact.state_ratio(gst, st, sb) <= 1.0, (act, p)
+        for k, (ap, sp) in pv.items():
+            assert max(opexact.err_ratio(got, ap, bnd), opexact.state_ratio(gst, sp, sb)) > 1.0, (act, p, k)
+        mm, mv, z_prev = gst['mean'], gst['var'], z
+
+
+@pytest.mark.parametrize('Cc', [32, 20, 520])
+def test_l2norm_forward_reference_emulation_and_perturbations(Cc):
+    rng = np.random.default_rng(Cc)
+    x = rng.standard_normal((2, 3, 4, Cc)).astype(np.float32)
+    x[0, 1, 1] = 0
+    x[1, 2, 3] = (rng.standard_normal(Cc) * 1e-8).astype(np.float32)
+    gamma = rng.uniform(0.5, 20, Cc).astype(np.float32)
+    ref, err, pv = opexact.l2norm_fwd_ref(x, gamma, perturb=[('no_gamma',), ('gamma_shift',)])
+    xt = torch.from_numpy(x.astype(np.float64))
+    want = xt * torch.rsqrt(torch.clamp((xt * xt).sum(-1, keepdim=True), min=float(np.float32(1e-12)))) * torch.from_numpy(gamma.astype(np.float64))
+    np.testing.assert_allclose(ref, want.numpy(), rtol=1e-12, atol=0)
+    bnd = np.maximum(err + opexact.UNIT['split'] * np.abs(ref), 1e-300)
+    for order in (1, -1):                                              # two summation orders, as l2norm_kernel and l2norm8_kernel
+        ss = np.zeros(x.shape[:-1], np.float32)
+        for c in range(Cc)[::order]:
+            ss = _fma(x[..., c], x[..., c], ss, order > 0)
+        inv = (1 / np.sqrt(np.maximum(ss, np.float32(1e-12)).astype(np.float64)) * (1 + 2 ** -22)).astype(np.float32)   # rsqrtf, 1 ulp off
+        got = np.sum(opexact.split((x * inv[..., None]).astype(np.float32) * gamma), axis=0, dtype=np.float64)
+        assert opexact.err_ratio(got, ref, bnd) <= 1.0, order
+        for p, r in pv.items():
+            assert opexact.err_ratio(got, r, bnd) > 1.0, (order, p)
+    assert not np.any(ref[0, 1, 1]) and np.all(ref[1, 2, 3] != 0)
+
+
+@pytest.mark.parametrize('k,s,pads', [(2, 2, (0, 0, 0, 0)), (2, 2, (0, 0, 1, 1)), (3, 1, (1, 1, 1, 1)), (3, 2, (0, 0, 0, 0))])
+def test_pool_forward_reference_matches_a_literal_loop(k, s, pads):
+    import test_gpu_train_step_kernels as ts
+    rng = np.random.default_rng(k + s)
+    H, W = 7, 9
+    x = ts._tie_input(rng, (2, H, W, 3))
+    hi, lo = opexact.split(x)
+    Ho, Wo = (H + pads[0] + pads[2] - k) // s + 1, (W + pads[1] + pads[3] - k) // s + 1
+    rh, rl, pv = opexact.pool_fwd_ref(hi, lo, k, k, s, pads[0], pads[1], Ho, Wo, perturb=[('hi_only',), ('lo_tie',)])
+    for b in range(2):
+        for c in range(3):
+            for yo in range(Ho):
+                for xo in range(Wo):
+                    best, at = -np.inf, None
+                    for ky in range(k):
+                        for kx in range(k):
+                            y, xx = yo * s - pads[0] + ky, xo * s - pads[1] + kx
+                            if 0 <= y < H and 0 <= xx < W and float(hi[b, y, xx, c]) + float(lo[b, y, xx, c]) > best:
+                                best, at = float(hi[b, y, xx, c]) + float(lo[b, y, xx, c]), (y, xx)
+                    assert rh[b, yo, xo, c] == hi[b, at[0], at[1], c] and rl[b, yo, xo, c] == lo[b, at[0], at[1], c]
+    for p, (ph, pl) in pv.items():
+        assert not (np.array_equal(ph, rh) and np.array_equal(pl, rl)), p
+
+
+def test_preprocess_reference_matches_a_literal_loop():
+    rng = np.random.default_rng(2)
+    img = rng.uniform(0, 255, (2, 3, 4, 3)).astype(np.float32)
+    mean, std, swap = (123.68, 116.779, 103.939), (58.393, 57.12, 57.375), (2, 1, 0)
+    for m_, s_, w_ in ((mean, None, None), (mean, std, None), (mean, std, swap)):
+        hi, lo = opexact.preprocess_ref(img, m_, s_, w_)
+        sw = w_ or (0, 1, 2)
+        for idx in np.ndindex(img.shape[:3]):
+            for c in range(3):
+                t = np.float32(img[idx + (sw[c],)]) - np.float32(m_[sw[c]])
+                if s_ is not None:
+                    t = np.float32(t / np.float32(s_[sw[c]]))
+                h = opexact.bf16_rne(np.array([t], np.float32))[0]
+                assert hi[idx + (c,)] == h and lo[idx + (c,)] == opexact.bf16_rne(np.array([t - h], np.float32))[0]
+
+
+def test_train_step_case_tables_reach_every_variant():
+    import test_gpu_train_step_kernels as ts
+    # optimiser: both optimisers x both precisions over a graph holding every parameter kind; every kernel span is
+    # a conv or head kernel with distinct cout, taps and cin (a transposed index lands on another element)
+    assert {(c['optimizer'], c['prec']) for c in ts.OPT_CASES} == {(o, p) for o in ('sgd', 'adam') for p in ('bf16x3', 'bf16')}
+    L = ts.OPT_LAYERS
+    assert L[0]['op'] == 'conv' and L[0]['input'] is None                 # image-facing: the direct kernel (3 input channels)
+    assert any(x['op'] == 'conv' and x['k'] == 3 and x['stride'] == 1 and not x['bn'] and x['cout'] not in (9, 24) for x in L[1:])
+    assert any(x['op'] == 'conv' and x['bn'] and x['act'] == 'elu' for x in L)
+    assert any(x['op'] == 'l2' for x in L) and any(x['op'] == 'head' for x in L) and any(x.get('stride') == 2 for x in L)
+    assert len(ts.SGD_STEPS) >= 3 and len(ts.ADAM_STEPS) >= 5
+    for steps in (ts.SGD_STEPS, ts.ADAM_STEPS):
+        assert {s for _, s, _ in steps} == {1.0, 0.5} and {l for _, _, l in steps} == {0.0, 5e-4}
+        assert len({lr for lr, _, _ in steps}) > 1
+    # re-pack: every WeightLayout, the direct kernel's master and the head interleave
+    fwd = {ts.REPACK_LAYOUTS[e['fwd']] for e in ts.REPACK_EXPECT.values()}
+    dgr = {ts.DGRAD_LAYOUTS[e['dgrad']] for e in ts.REPACK_EXPECT.values() if e['dgrad']}
+    assert fwd == {'master', 'PACK_FWD', 'PACK_FWD_IM2COL'} and dgr == {'PACK_DGRAD', 'PACK_DGRAD_COL'}
+    assert ts.REPACK_LAYERS[-1]['op'] == 'head'
+    # max-pool and L2Normalization: both kernels each
+    assert {ts.pool_kernel_of(c['H'], c['W'], c['k'], c['stride'], c['pads']) for c in ts.POOL_CASES} == {'maxpool2x2', 'maxpool'}
+    assert any(c['H'] == 75 and c['pads'] == (0, 0, 1, 1) for c in ts.POOL_CASES)
+    ks = {ts.l2norm_kernel_of(c['C'], -(-c['C'] // 8) * 8): c['C'] for c in ts.L2_CASES}
+    assert set(ks) == {'l2norm8', 'l2norm'} and {20, 520} <= {c['C'] for c in ts.L2_CASES}
+    # BatchNormalization: ELU / ReLU / none, C = 24 and 136, both precisions, both branches of bn_grid
+    bn = [(c, x) for c in ts.BN_CASES for x in c['layers'] if x['bn']]
+    assert {x['act'] for _, x in bn} == {'elu', 'relu', None} and {24, 136} <= {x['cout'] for _, x in bn}
+    assert {c['prec'] for c in ts.BN_CASES} == {'bf16x3', 'bf16'}
+    branches = {ts.bn_grid(c['B'], c['H'], c['W'], x['cout'])[1] for c, x in bn}
+    assert branches == {1, 2}
+    assert ts.bn_grid(1, 10, 10, 136) == (17, 2)
+    # preprocessing: mean only, mean + std, and the BGR swap
+    assert [(c['stddev'] is not None, c['swap'] is not None) for c in ts.PRE_CASES] == [(False, False), (True, False), (True, True)]
