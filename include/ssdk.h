@@ -165,6 +165,27 @@ typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, const int* offsets_in_dev, int B, int total_in,
                         const ssdk_box_op* ops_dev, int max_ops, float* gt_out_dev, int* offsets_out_dev, int* out_stats_dev,
                         void* stream);
+/* The image half of the same op lists: ConvertTo3Channels (object_detection_2d_photometric_ops.py:88-108; gray is replicated,
+ * RGBA drops alpha, applied first), the image arithmetic of CropPad (:266-313) and Flip, and uint8 cv2.resize, into a float32
+ * NHWC batch of [0,255] integers (what ssdk_model_forward takes).  The image fields live in flag bits the box kernel never reads:
+ *   CROP_PAD  flags bits 8-31: background R, G, B bytes (0 = black, as CropPad's default; SSDExpand uses 123,117,104)
+ *   RESIZE    flags bits 8-15: cv2 interpolation code, INTER_NEAREST = 0 or INTER_LINEAR = 1 (an exact 2x linear downscale
+ *             takes INTER_AREA's fast path, as cv2 does); any other code is an error
+ *   FILTER    nothing to do for images
+ * src_dev: the B uint8 images packed back to back, image b at bytes src_offsets_host[b] .. src_offsets_host[b+1] (host, [B+1]),
+ * of shape src_hwc_host[3b..3b+2] = h, w, c with c in {1, 3, 4}.  ops_host: [B*max_ops] on the HOST (a list ends at
+ * SSDK_BOXOP_END or after max_ops entries).  out_dev: [B*out_h*out_w*3] float32.
+ * Checked on the host before anything is enqueued (SSDK_ERR_INVALID, nothing written): sizes positive, B <= 65535, offsets
+ * consistent with the shapes; each CROP_PAD integer with a positive size and overlapping its input (CropPad's own test, :270-271);
+ * each flip's a0 equal to the canvas width / height at that point; at most one RESIZE, from the canvas size reached at that point,
+ * and no crop / pad / flip after it; the final size out_h x out_w; a supported interpolation code; and all pads of one list that
+ * reach past their input use one background colour (bands of different colours are not represented).
+ * The crops, pads and flips before the resize are composed on the host into one integer map per image; one kernel launch
+ * evaluates the whole list without an intermediate image.  The descriptors go to the device with one asynchronous copy from
+ * pinned staging owned by the context (a ring of four buffers: the call waits only if the upload of the call four calls earlier
+ * has not run yet); like the encoder, one context must not run this on two streams at the same time. */
+int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const long long* src_offsets_host, const int* src_hwc_host, int B,
+                         const ssdk_box_op* ops_host, int max_ops, int out_h, int out_w, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Evaluation.  Replaces the per-prediction Python loop of Evaluator.match_predictions

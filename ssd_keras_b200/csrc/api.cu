@@ -40,6 +40,10 @@ extern "C" int ssdk_ctx_create(int device, ssdk_ctx** out) {
 extern "C" int ssdk_ctx_destroy(ssdk_ctx* ctx) {
   if (!ctx) return SSDK_OK;
   for (auto& w : ctx->ws) w.release();
+  for (auto& s : ctx->img_stage) {
+    if (s.done) { cudaEventSynchronize(s.done); cudaEventDestroy(s.done); }
+    if (s.ptr) cudaFreeHost(s.ptr);
+  }
   delete ctx;
   return SSDK_OK;
 }

@@ -54,10 +54,15 @@ struct ssdk_ctx {
   int device = 0;
   int sm_count = 132;
   int64_t launches = 0;
-  ssdk::Scratch ws[4];          // decode / loss / nms workspaces
+  ssdk::Scratch ws[5];          // decode / loss / nms / box assembly / image descriptor workspaces
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for
   int loss_parity = 0;          // which of its two histogram sets the next loss call uses (the other one is being cleared)
   cudaDeviceProp prop{};
+  // Pinned staging for the per-image descriptors of ssdk_assemble_images: a ring of buffers, each with an event recorded after
+  // its upload, so that the host can run up to kImgStages calls ahead of the device before a buffer has to be waited for.
+  static constexpr int kImgStages = 4;
+  struct HostStage { void* ptr = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; } img_stage[kImgStages];
+  int img_stage_next = 0;
 };
 
 #define SSDK_COUNT_LAUNCH(ctx) do { (ctx)->launches++; } while (0)
