@@ -51,11 +51,11 @@ one FMA: every bound counts a product and an add as two roundings, which covers 
 u = 2**-24 is the unit roundoff of fp32; a rounding of a value t loses at most u |t|.  expm1f is within 1 ulp, rsqrtf within
 2 ulps, sqrtf and division are correctly rounded.
 
-6. SGD (sgd_kernel_w / sgd_kernel_flat): grad = g s + 2 l2 w, v' = mom v - lr grad, w' = w + v'.  Six roundings (g s, 2 l2 w,
+6. SGD (sgd_kernel<true> / sgd_kernel<false>): grad = g s + 2 l2 w, v' = mom v - lr grad, w' = w + v'.  Six roundings (g s, 2 l2 w,
    their sum, lr grad, mom v, the difference), each at most u times A_v = |mom v| + |lr| (|g s| + 2 l2 |w|), which bounds every
    intermediate:  |v' - v'_ref| <= 8 u A_v.  w' adds one rounding of its own, the store; as everywhere in this module one unit
    of the stored format (2**-23 for fp32) is added:  |v' - v'_ref| <= 8 u A_v + 2**-23 |v'_ref|, the same for w'.
-7. Adam (adam_kernel_w / adam_kernel_flat): grad as in 6.; m' = b1 m + (1 - b1) grad (1 - b1 is exact for b1 in [1/2, 1]);
+7. Adam (adam_kernel<true> / adam_kernel<false>): grad as in 6.; m' = b1 m + (1 - b1) grad (1 - b1 is exact for b1 in [1/2, 1]);
    v' = b2 v + (1 - b2) grad^2; w' = w - lr_t m' / (sqrtf(v') + eps), lr_t = fp32(fp32(sqrt(1 - b2^t) / (1 - b1^t)) lr).
    m' carries the 3 roundings of grad and 3 of its own: |m' - m'_ref| <= 8 u A_m, A_m = |b1 m| + (1 - b1) G, G = |g s| + 2 l2 |w|.
    v' has no cancellation but grad's error enters squared (6 u) and v' adds 4 roundings: |v' - v'_ref| <= 16 u A_v,
@@ -608,7 +608,7 @@ def _grad(g, w, l2, scale, kernel_shape, p):
 
 
 def sgd_ref(w, v, g, lr, momentum, l2=0.0, scale=1.0, kernel_shape=None, perturb=()):
-    """One SGD update of one parameter span (sgd_kernel_w / sgd_kernel_flat) -> (ref, bound, {perturbation: ref'}), each a dict
+    """One SGD update of one parameter span (sgd_kernel<true> / sgd_kernel<false>) -> (ref, bound, {perturbation: ref'}), each a dict
     {'w': new master, 'v': new velocity}, float64.
 
     w, v, g: the master, the velocity and the gradient as the launch read them, in the gradient's layout (kernels OHWI, as
@@ -637,7 +637,7 @@ def adam_lr_t(lr, beta1, beta2, t):
 
 
 def adam_ref(w, m, v, g, lr, beta1, beta2, eps, t, l2=0.0, scale=1.0, kernel_shape=None, perturb=()):
-    """One Adam update of one parameter span (adam_kernel_w / adam_kernel_flat) -> (ref, bound, {perturbation: ref'}), each a dict
+    """One Adam update of one parameter span (adam_kernel<true> / adam_kernel<false>) -> (ref, bound, {perturbation: ref'}), each a dict
     {'w': new master, 'm': new first moment, 'v': new second moment}, float64.
 
     w, m, v, g: as read before the launch, in the gradient's layout; t: the step the update was given (from 1).  Bound: section

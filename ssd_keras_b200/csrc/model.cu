@@ -52,9 +52,9 @@ int build_conv(ssdk_model* m, int li) {
     rc = upload_f32(m, &L.bn_beta, d.bn_beta, cout); if (rc) return rc;
     rc = upload_f32(m, &L.bn_mmean, d.bn_mean, cout); if (rc) return rc;
     rc = upload_f32(m, &L.bn_mvar, d.bn_var, cout); if (rc) return rc;
-    rc = dev_alloc(m, &L.bn_bmean, cout, true); if (rc) return rc;
-    rc = dev_alloc(m, &L.bn_brstd, cout, true); if (rc) return rc;
-    rc = dev_alloc(m, &L.bn_acc, (size_t)2 * cout, true); if (rc) return rc;
+    rc = dev_alloc(m->allocs, &L.bn_bmean, cout, true); if (rc) return rc;
+    rc = dev_alloc(m->allocs, &L.bn_brstd, cout, true); if (rc) return rc;
+    rc = dev_alloc(m->allocs, &L.bn_acc, (size_t)2 * cout, true); if (rc) return rc;
     L.bn_eps = d.bn_eps > 0.f ? d.bn_eps : 1e-3f;
     L.bn_momentum = (d.bn_momentum > 0.f && d.bn_momentum < 1.f) ? d.bn_momentum : 0.99f;
   }
@@ -76,10 +76,10 @@ int build_conv(ssdk_model* m, int li) {
       std::vector<uint16_t> whi, wlo;
       L.first = first_plan(L.out, d.kh, d.kw, m->ctx->sm_count);
       first_weight_image(master.data(), taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
-      rc = dev_alloc(m, &L.w_hi, whi.size(), false); if (rc) return rc;
+      rc = dev_alloc(m->allocs, &L.w_hi, whi.size(), false); if (rc) return rc;
       SSDK_CHECK_CUDA(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
       if (m->split) {
-        rc = dev_alloc(m, &L.w_lo, wlo.size(), false); if (rc) return rc;
+        rc = dev_alloc(m->allocs, &L.w_lo, wlo.size(), false); if (rc) return rc;
         SSDK_CHECK_CUDA(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
       }
       L.first_tc = true;
@@ -97,8 +97,8 @@ int build_conv(ssdk_model* m, int li) {
     L.Kpad = (taps * cin + 7) / 8 * 8;
     kblocks = (L.Kpad + 63) / 64;
     size_t n = (size_t)m->B * Ho * Wo * L.Kpad + 64 * 8;
-    int rc = dev_alloc(m, &L.col_hi, n, true); if (rc) return rc;
-    if (m->split) { rc = dev_alloc(m, &L.col_lo, n, true); if (rc) return rc; }
+    int rc = dev_alloc(m->allocs, &L.col_hi, n, true); if (rc) return rc;
+    if (m->split) { rc = dev_alloc(m->allocs, &L.col_lo, n, true); if (rc) return rc; }
     L.im2col_vec8 = im2col_vec8_ok(ia, L.Kpad, L.col_hi, L.col_lo);
     g.a_hi = L.col_hi; g.a_lo = L.col_lo; g.a_inner = L.Kpad; g.a_rows = (uint64_t)m->B * Ho * Wo;
   } else {
@@ -109,8 +109,8 @@ int build_conv(ssdk_model* m, int li) {
   L.kblocks = kblocks;
   // weights: forward planes packed on the device from the master, which training plans keep for the optimiser
   L.w_krow = L.im2col ? (size_t)kblocks * 64 : (size_t)taps * kblocks * 64;
-  int rc = dev_alloc(m, &L.w_hi, (size_t)cout * L.w_krow, false); if (rc) return rc;
-  if (m->split) { rc = dev_alloc(m, &L.w_lo, (size_t)cout * L.w_krow, false); if (rc) return rc; }
+  int rc = dev_alloc(m->allocs, &L.w_hi, (size_t)cout * L.w_krow, false); if (rc) return rc;
+  if (m->split) { rc = dev_alloc(m->allocs, &L.w_lo, (size_t)cout * L.w_krow, false); if (rc) return rc; }
   std::unique_ptr<float, CudaFree> scratch;         // the master of an inference plan, freed once the planes are packed
   float* w_dev = nullptr;
   if (m->training) {
@@ -143,7 +143,7 @@ int build_conv(ssdk_model* m, int li) {
       L.head_fused = true;
     } else {
       a.epi = EPI_F32;
-      rc = dev_alloc(m, &L.head_f32, (size_t)m->B * Ho * Wo * cout, true); if (rc) return rc;
+      rc = dev_alloc(m->allocs, &L.head_f32, (size_t)m->B * Ho * Wo * cout, true); if (rc) return rc;
       a.out_f32 = L.head_f32;
     }
   } else {
@@ -332,7 +332,7 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   }
   a.n_tiles_m = (int)tiles.size();
   int* tl = nullptr;
-  int rc = dev_alloc(m, &tl, tiles.size(), false); if (rc) return rc;
+  int rc = dev_alloc(m->allocs, &tl, tiles.size(), false); if (rc) return rc;
   SSDK_CHECK_CUDA(cudaMemcpy(tl, tiles.data(), tiles.size() * sizeof(int), cudaMemcpyHostToDevice));
   a.tile_list = tl;
   if (tile_list_out) *tile_list_out = tl;

@@ -67,21 +67,22 @@ struct ssdk_model {
 
 namespace ssdk {
 
+// Device memory owned by a model or a trainer: `allocs` is its owner's list, freed when the owner is destroyed.
 template <typename T>
-inline int dev_alloc(ssdk_model* m, T** out, size_t count, bool zero) {
+inline int dev_alloc(std::vector<void*>& allocs, T** out, size_t count, bool zero) {
   void* p = nullptr;
   size_t bytes = count * sizeof(T);
   if (bytes == 0) bytes = 16;
   cudaError_t e = cudaMalloc(&p, bytes);
   if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSDK_ERR_NOMEM; }
+  allocs.push_back(p);
   if (zero) { e = cudaMemset(p, 0, bytes); if (e != cudaSuccess) { set_error("cudaMemset failed: %s", cudaGetErrorString(e)); return SSDK_ERR_CUDA; } }
-  m->allocs.push_back(p);
   *out = reinterpret_cast<T*>(p);
   return SSDK_OK;
 }
 
 inline int upload_f32(ssdk_model* m, float** out, const float* host, size_t n) {
-  int rc = dev_alloc(m, out, n, false);
+  int rc = dev_alloc(m->allocs, out, n, false);
   if (rc) return rc;
   SSDK_CHECK_CUDA(cudaMemcpy(*out, host, n * sizeof(float), cudaMemcpyHostToDevice));
   return SSDK_OK;
@@ -93,9 +94,9 @@ inline int alloc_act(ssdk_model* m, ActBuf& a, int B, int H, int W, int C, int p
   if (!m->training && pad > 0) { const char* e = getenv("SSDK_SHARED_BORDER"); a.shared = e ? (atoi(e) ? 1 : 0) : 1; }
   // slack: TMA boxes may start on the last rows; with a shared border the last row's right border lies behind the last image
   size_t n = a.elems() + std::max<size_t>(64 * 8, (size_t)(pad + 1) * a.Cs);
-  int rc = dev_alloc(m, &a.hi, n, true);
+  int rc = dev_alloc(m->allocs, &a.hi, n, true);
   if (rc) return rc;
-  if (m->split) { rc = dev_alloc(m, &a.lo, n, true); if (rc) return rc; }
+  if (m->split) { rc = dev_alloc(m->allocs, &a.lo, n, true); if (rc) return rc; }
   return SSDK_OK;
 }
 

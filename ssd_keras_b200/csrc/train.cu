@@ -334,26 +334,44 @@ __global__ void __launch_bounds__(256) wgrad_direct3x3_kernel(ActBuf in, ActBuf 
   }
 }
 
-// SGD with momentum (Keras: v = m*v - lr*g; w += v); kernels get the l2 regulariser's gradient 2*l2*w.
-// `w` is HWIO [taps][cin][cout]; the gradient is OHWI [cout][taps][cin].
-__global__ void sgd_kernel_w(float* __restrict__ w, float* __restrict__ v, const float* __restrict__ g, int taps, int cin, int cout,
-                             float lr, float mom, float l2, float scale) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t total = (size_t)taps * cin * cout;
-  if (i >= total) return;
+// The optimiser kernels update one parameter span.  KERNEL: a conv / head kernel, whose value and state are HWIO
+// [taps][cin][cout] while its gradient is OHWI [cout][taps][cin], and which alone gets the l2 regulariser's gradient 2*l2*w.
+// Vector spans (bias, gammas, beta) index all three alike.
+__device__ __forceinline__ size_t ohwi_index(size_t i, int taps, int cin, int cout) {
   const int co = (int)(i % cout); const size_t r = i / cout; const int ci = (int)(r % cin); const int t = (int)(r / cin);
-  const float grad = g[((size_t)co * taps + t) * cin + ci] * scale + 2.f * l2 * w[i];
-  const float nv = mom * v[i] - lr * grad;
+  return ((size_t)co * taps + t) * cin + ci;
+}
+
+// SGD with momentum (Keras: v = m*v - lr*g; w += v)
+template <bool KERNEL>
+__global__ void sgd_kernel(float* __restrict__ w, float* __restrict__ v, const float* __restrict__ g, size_t n, int taps, int cin, int cout,
+                           float lr, float mom, float l2, float scale) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float nv;
+  if constexpr (KERNEL) {
+    const float grad = g[ohwi_index(i, taps, cin, cout)] * scale + 2.f * l2 * w[i];
+    nv = mom * v[i] - lr * grad;
+  } else {
+    nv = mom * v[i] - lr * g[i] * scale;
+  }
   v[i] = nv;
   w[i] += nv;
 }
-__global__ void sgd_kernel_flat(float* __restrict__ w, float* __restrict__ v, const float* __restrict__ g, size_t n, float lr, float mom,
-                                float scale) {
+
+// Adam (Keras: m = b1*m + (1-b1)*g; v = b2*v + (1-b2)*g^2; w -= lr_t*m / (sqrt(v) + eps))
+template <bool KERNEL>
+__global__ void adam_kernel(float* __restrict__ w, float* __restrict__ m1, float* __restrict__ m2, const float* __restrict__ g, size_t n, int taps,
+                            int cin, int cout, float lr_t, float b1, float b2, float eps, float l2, float scale) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float nv = mom * v[i] - lr * g[i] * scale;
-  v[i] = nv;
-  w[i] += nv;
+  float grad;
+  if constexpr (KERNEL) grad = g[ohwi_index(i, taps, cin, cout)] * scale + 2.f * l2 * w[i];
+  else grad = g[i] * scale;
+  const float a = b1 * m1[i] + (1.f - b1) * grad;
+  const float b = b2 * m2[i] + (1.f - b2) * grad * grad;
+  m1[i] = a; m2[i] = b;
+  w[i] -= lr_t * a / (sqrtf(b) + eps);
 }
 
 __global__ void hwio_to_ohwi_kernel(const float* __restrict__ w, int taps, int cin, int cout, float* __restrict__ out) {
@@ -368,13 +386,7 @@ __global__ void hwio_to_ohwi_kernel(const float* __restrict__ w, int taps, int c
 // plan
 // ---------------------------------------------------------------------------------------------
 struct TLayer {
-  int li = -1, op = -1;
-  // parameters (conv / head): master kernel HWIO in L.w_f32, bias in L.bias (shared with the forward plan)
-  int cin = 0, cout = 0, taps = 0;
-  float *vw = nullptr, *vb = nullptr;       // momentum
-  long long off_w = -1, off_b = -1, off_g = -1, off_bng = -1, off_bnb = -1;
-  float *v2w = nullptr, *v2b = nullptr, *v2gamma = nullptr;     // Adam second moments (vw / vb / vgamma hold the first moments)
-  float *m_bng = nullptr, *v_bng = nullptr, *m_bnb = nullptr, *v_bnb = nullptr;   // BatchNormalization gamma / beta optimiser state
+  int cin = 0, cout = 0, taps = 0;          // conv / head kernel shape
   ActBuf g;                                 // gradient of this layer's output (pre-activation); same geometry as the output
   bool has_g = false;
   // data gradient
@@ -394,7 +406,16 @@ struct TLayer {
   std::vector<int> wgrad_res;               // tap shift mod 8: TMA needs 16-byte aligned K offsets, so XT is built once per residue
   long long Kv = 0, ldT = 0;
   TMap dy_map{}, x_map{};
-  float* vgamma = nullptr;
+};
+
+// One parameter span of the flat gradient buffer.  `which` is ssdk_trainer_param_span's code: 0 conv / head kernel, 1 bias,
+// 2 L2Normalization gamma, 3 / 4 BatchNormalization gamma / beta.  `value` is the fp32 parameter the layer plan reads
+// (L.w_f32, L.bias, L.gamma, L.bn_gamma, L.bn_beta).
+struct ParamSpan {
+  int layer = 0, which = 0;
+  long long off = 0, count = 0;
+  float* value = nullptr;
+  int taps = 0, cin = 0, cout = 0;          // kernel spans: the HWIO value is read and written as OHWI; 0: a vector span
 };
 
 // wgrad_direct3x3_kernel's conditions: 3x3 undilated taps over 3 input channels, an even cout that fits its shared accumulators, and a
@@ -409,33 +430,31 @@ bool direct_fast3(const ssdk_layer_desc& d, const ActBuf& X, int cin, int cout) 
 struct ssdk_trainer {
   ssdk_model* m = nullptr;
   std::vector<TLayer> tl;
-  float* grad = nullptr; bool own_grad = false;
+  std::vector<ParamSpan> params;            // the spans of the flat gradient buffer, in its order
+  float* grad = nullptr;
   long long n_params = 0;
+  // optimiser state in the flat buffer's spans, a kernel's HWIO like its value: [0] SGD velocity / Adam first moment, made with
+  // the trainer; [1] Adam second moment, made by the first Adam update
+  float* state[2] = {nullptr, nullptr};
   __nv_bfloat16 *xT_hi = nullptr, *xT_lo = nullptr, *dyT_hi = nullptr, *dyT_lo = nullptr;   // scratch, sized for the largest layer
-  long long xT_elems = 0, dyT_elems = 0;
   float* dypred = nullptr;                  // [B*P*(C+12)]
   std::vector<char> written;                // backward pass state: which activations already hold a partial gradient
-  bool adam = false;                        // an Adam update ran: the second moments exist
   std::vector<void*> allocs;
 };
 
 namespace {
 
-template <typename T>
-int t_alloc(ssdk_trainer* t, T** out, size_t count, bool zero) {
-  void* p = nullptr;
-  size_t bytes = std::max<size_t>(count * sizeof(T), 16);
-  cudaError_t e = cudaMalloc(&p, bytes);
-  if (e != cudaSuccess) { set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return SSDK_ERR_NOMEM; }
-  if (zero) cudaMemset(p, 0, bytes);
-  t->allocs.push_back(p);
-  *out = reinterpret_cast<T*>(p);
-  return SSDK_OK;
-}
-
 bool is_conv(int op) { return op == SSDK_OP_CONV || op == SSDK_OP_HEAD; }
 // graph sources (preprocessed images, or a caller tensor): no producer, no parameters, no gradient
 bool is_source(int op) { return op == SSDK_OP_INPUT || op == SSDK_OP_TENSOR; }
+
+const ParamSpan* find_span(const ssdk_trainer* t, int layer, int which) {
+  for (const ParamSpan& p : t->params)
+    if (p.layer == layer && p.which == which) return &p;
+  return nullptr;
+}
+// the gradient of a span the layer has
+float* span_grad(ssdk_trainer* t, int layer, int which) { return t->grad + find_span(t, layer, which)->off; }
 
 // The bf16 planes of conv layer i from its fp32 master: the forward planes (the image-facing direct kernel reads the master
 // itself) and the data-gradient planes
@@ -456,43 +475,41 @@ int repack_layer(ssdk_trainer* t, int i, cudaStream_t s) {
   return SSDK_OK;
 }
 
-}  // namespace
-
-extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_trainer** out) {
-  SSDK_REQUIRE(m && out, "ssdk_trainer_create: NULL argument");
-  SSDK_REQUIRE(m->training, "ssdk_trainer_create: the model plan was not created with training=1");
-  SSDK_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  ssdk_trainer* t = new ssdk_trainer();
-  t->m = m;
-  const int n = (int)m->layers.size();
-  t->tl.resize(n);
-  int rc = SSDK_OK;
-  auto fail = [&](int code) { ssdk_trainer_destroy(t); return code; };
-  // parameter spans
+// The parameter table in flat-buffer order (per layer: a conv / head's kernel, bias and BatchNormalization gamma / beta, or an
+// L2Normalization's gamma), the flat gradient buffer (the caller's, or the trainer's own) and optimiser slot 0.
+int plan_params(ssdk_trainer* t, float* flat_grad_dev) {
+  ssdk_model* m = t->m;
   long long off = 0;
-  for (int i = 0; i < n; ++i) {
+  auto add = [&](int i, int which, long long count, float* value, int taps = 0, int cin = 0, int cout = 0) {
+    t->params.push_back(ParamSpan{i, which, off, count, value, taps, cin, cout});
+    off += count;
+  };
+  for (int i = 0; i < (int)m->layers.size(); ++i) {
     LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
-    T.li = i; T.op = L.d.op;
     if (is_conv(L.d.op)) {
       if ((L.d.act == SSDK_ACT_ELU || L.bn_scale) && !L.bn_train) {
         set_error("training: layer %d has an ELU / folded BatchNormalization without the raw BatchNormalization parameters (bn_gamma, ...)", i);
-        return fail(SSDK_ERR_UNSUPPORTED);
+        return SSDK_ERR_UNSUPPORTED;
       }
       T.cin = m->layers[L.d.input].C; T.cout = L.C; T.taps = L.d.kh * L.d.kw;
-      T.off_w = off; off += (long long)T.cout * T.taps * T.cin;
-      T.off_b = off; off += T.cout;
-      if (L.bn_train) { T.off_bng = off; off += T.cout; T.off_bnb = off; off += T.cout; }
+      add(i, 0, (long long)T.cout * T.taps * T.cin, L.w_f32, T.taps, T.cin, T.cout);
+      add(i, 1, T.cout, L.bias);
+      if (L.bn_train) { add(i, 3, T.cout, L.bn_gamma); add(i, 4, T.cout, L.bn_beta); }
     } else if (L.d.op == SSDK_OP_L2NORM) {
-      T.off_g = off; off += L.C;
+      add(i, 2, L.C, L.gamma);
     }
   }
   t->n_params = off;
   if (flat_grad_dev) t->grad = flat_grad_dev;
-  else { rc = t_alloc(t, &t->grad, (size_t)off, true); if (rc) return fail(rc); t->own_grad = true; }
-  rc = t_alloc(t, &t->dypred, (size_t)m->B * m->P * (m->Ctot + 12), true); if (rc) return fail(rc);
-  // gradient buffers: same geometry as the forward outputs
-  for (int i = 0; i < n; ++i) {
+  else { int rc = dev_alloc(t->allocs, &t->grad, (size_t)off, true); if (rc) return rc; }
+  return dev_alloc(t->allocs, &t->state[0], (size_t)off, true);
+}
+
+// Gradient planes of every layer but the sources, in the geometry of its forward output
+int alloc_grad_planes(ssdk_trainer* t) {
+  ssdk_model* m = t->m;
+  for (int i = 0; i < (int)m->layers.size(); ++i) {
     LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
     if (is_source(L.d.op)) continue;
@@ -500,117 +517,106 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
     if (L.d.op == SSDK_OP_HEAD) { g.B = m->B; g.H = L.H; g.W = L.W; g.C = L.C; g.Cs = (L.C + 7) / 8 * 8; g.pad = 1; }
     else { g = L.out; g.hi = nullptr; g.lo = nullptr; }
     const size_t ne = g.elems() + 64 * 8;
-    rc = t_alloc(t, &g.hi, ne, true); if (rc) return fail(rc);
-    if (m->split) { rc = t_alloc(t, &g.lo, ne, true); if (rc) return fail(rc); }
+    int rc = dev_alloc(t->allocs, &g.hi, ne, true); if (rc) return rc;
+    if (m->split) { rc = dev_alloc(t->allocs, &g.lo, ne, true); if (rc) return rc; }
     T.has_g = true;
   }
-  // per conv: momentum, data-gradient plan, weight-gradient plans
-  std::vector<char> written(n, 0);            // does the producer's gradient buffer already hold a contribution?
-  long long max_xT = 0, max_dyT = 0;
-  for (int i = n - 1; i >= 0; --i) {
-    LayerPlan& L = m->layers[i];
-    TLayer& T = t->tl[i];
-    const ssdk_layer_desc& d = L.d;
-    if (is_source(d.op)) continue;
-    const int pi = d.input;
-    LayerPlan& PL = m->layers[pi];
-    TLayer& PT = t->tl[pi];
-    const bool prod_needs_grad = !is_source(PL.d.op);
-    if (d.op == SSDK_OP_L2NORM) { rc = t_alloc(t, &T.vgamma, (size_t)L.C, true); if (rc) return fail(rc); }
-    if (!is_conv(d.op)) { if (prod_needs_grad) written[pi] = 1; continue; }
-    rc = t_alloc(t, &T.vw, (size_t)T.cout * T.taps * T.cin, true); if (rc) return fail(rc);
-    rc = t_alloc(t, &T.vb, (size_t)T.cout, true); if (rc) return fail(rc);
-    if (L.bn_train) {
-      rc = t_alloc(t, &T.m_bng, (size_t)T.cout, true); if (rc) return fail(rc);
-      rc = t_alloc(t, &T.v_bng, (size_t)T.cout, true); if (rc) return fail(rc);
-      rc = t_alloc(t, &T.m_bnb, (size_t)T.cout, true); if (rc) return fail(rc);
-      rc = t_alloc(t, &T.v_bnb, (size_t)T.cout, true); if (rc) return fail(rc);
-    }
-    // ---- data gradient
-    if (prod_needs_grad) {
-      if (T.cin % 8 != 0) { set_error("training: input channels must be a multiple of 8 (layer %d)", i); return fail(SSDK_ERR_UNSUPPORTED); }
-      if (d.stride != 1) {
-        // dCol[M][taps*cin] = dZ[M][cout] * W^T, then col2im
-        T.has_dgrad = true; T.dgrad_strided = true;
-        T.dgrad_relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
-        const int kcol = T.taps * T.cin;
-        T.w2_kblocks = (T.g.Cs + 63) / 64;
-        T.w2_krow = (size_t)T.w2_kblocks * 64;
-        rc = t_alloc(t, &T.w2_hi, (size_t)kcol * T.w2_krow, true); if (rc) return fail(rc);
-        if (m->split) { rc = t_alloc(t, &T.w2_lo, (size_t)kcol * T.w2_krow, true); if (rc) return fail(rc); }
-        T.dcol_ld = kcol;
-        rc = t_alloc(t, &T.dcol, (size_t)m->B * L.H * L.W * kcol, true); if (rc) return fail(rc);
-        ConvGeom gg;
-        gg.in = &T.g; gg.kh = 1; gg.kw = 1; gg.dilation = 1; gg.pad_t = 0; gg.pad_l = 0;
-        gg.Ho = L.H; gg.Wo = L.W; gg.B = m->B; gg.cout = kcol;
-        rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, &T.dgrad_tiles);
-        if (rc) return fail(rc);
-        ConvArgs& a = T.dgrad.args;
-        a.epi = EPI_F32; a.bias = nullptr; a.act = SSDK_ACT_NONE; a.out_f32 = T.dcol;
-        T.dgrad_col2im_accumulate = written[pi] ? 1 : 0;
-        written[pi] = 1;
-        goto wgrad_plan;
-      }
-      T.has_dgrad = true;
-      T.w2_kblocks = (T.g.Cs + 63) / 64;
-      T.w2_krow = (size_t)T.taps * T.w2_kblocks * 64;
-      rc = t_alloc(t, &T.w2_hi, (size_t)T.cin * T.w2_krow, true); if (rc) return fail(rc);
-      if (m->split) { rc = t_alloc(t, &T.w2_lo, (size_t)T.cin * T.w2_krow, true); if (rc) return fail(rc); }
-      ConvGeom gg;
-      gg.in = &T.g; gg.kh = d.kh; gg.kw = d.kw; gg.dilation = d.dilation;
-      gg.pad_t = d.dilation * (d.kh - 1) - d.pad_t; gg.pad_l = d.dilation * (d.kw - 1) - d.pad_l;
-      gg.Ho = PL.H; gg.Wo = PL.W; gg.B = m->B; gg.cout = T.cin;
-      rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, &T.dgrad_tiles);
-      if (rc) return fail(rc);
-      ConvArgs& a = T.dgrad.args;
-      a.epi = EPI_SPLIT; a.bias = nullptr; a.act = SSDK_ACT_NONE;
-      a.out_hi = PT.g.hi; a.out_lo = PT.g.lo; a.out_Hp = PT.g.Hp(); a.out_Wp = PT.g.Wp(); a.out_pad = PT.g.pad; a.out_Cs = PT.g.Cs;
-      a.mask_hi = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? PL.out.hi : nullptr;
-      a.accumulate = written[pi] ? 1 : 0;
-      written[pi] = 1;
-    }
-    // ---- weight gradient
-    wgrad_plan:
-    if (L.direct) continue;                     // handled by wgrad_direct_kernel
-    const ActBuf& X = PL.out;
-    long long Kv;
-    if (!L.im2col && !getenv("SSDK_WGRAD_TRANSPOSED") && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
-      T.wg_native = true;
-      rc = plan_wgrad(m->ctx, T.wg, X, T.g, L.H, L.W, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, m->split, nullptr);
-      if (rc) return fail(rc);
-      continue;
-    }
-    if (L.im2col) {
-      Kv = (long long)m->B * L.H * L.W;
-      T.dy_map = TMap{0, L.H * L.W, L.W, L.H, L.W, T.g.Hp(), T.g.Wp(), T.g.pad};
-      T.x_map = TMap{1, 0, 0, 0, 0, 0, 0, 0};
-      max_xT = std::max(max_xT, (long long)L.Kpad * ((Kv + 7) / 8 * 8 + 64));
-    } else {
-      // the GEMM's pixel axis runs over X's padded grid with the row pitch rounded up to 8 elements: tap shifts are then
-      // kh*Wq + kw (+ const) and only the kw part can break TMA's 16-byte alignment -> one XT copy per distinct kw residue
-      const int Wq = (X.Wp() + 7) / 8 * 8;
-      T.Wq = Wq;
-      Kv = (long long)m->B * X.Hp() * Wq;
-      T.dy_map = TMap{0, X.Hp() * Wq, Wq, L.H, L.W, T.g.Hp(), T.g.Wp(), T.g.pad};
-      T.x_map = TMap{0, X.Hp() * Wq, Wq, X.Hp(), X.Wp(), X.Hp(), X.Wp(), 0};
-      max_xT = std::max(max_xT, (long long)X.Cs * ((Kv + 7) / 8 * 8 + 64));
-    }
-    T.Kv = Kv; T.ldT = (Kv + 7) / 8 * 8 + 64;
-    max_dyT = std::max(max_dyT, (long long)T.g.Cs * T.ldT);
+  return SSDK_OK;
+}
+
+// Data-gradient plan of conv layer i into its producer's gradient planes.  written[pi]: the backward pass has already written
+// a contribution of another consumer into them when it reaches layer i.
+int plan_dgrad(ssdk_trainer* t, int i, std::vector<char>& written) {
+  ssdk_model* m = t->m;
+  const LayerPlan& L = m->layers[i];
+  TLayer& T = t->tl[i];
+  const ssdk_layer_desc& d = L.d;
+  const int pi = d.input;
+  const LayerPlan& PL = m->layers[pi];
+  const TLayer& PT = t->tl[pi];
+  if (is_source(PL.d.op)) return SSDK_OK;
+  if (T.cin % 8 != 0) { set_error("training: input channels must be a multiple of 8 (layer %d)", i); return SSDK_ERR_UNSUPPORTED; }
+  const int relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
+  T.has_dgrad = true;
+  T.dgrad_strided = d.stride != 1;
+  T.w2_kblocks = (T.g.Cs + 63) / 64;
+  ConvGeom gg;
+  gg.in = &T.g; gg.B = m->B;
+  int rows, rc;                               // rows of the packed planes
+  if (T.dgrad_strided) {
+    // dCol[M][taps*cin] = dZ[M][cout] * W^T, then col2im
+    rows = T.dcol_ld = T.taps * T.cin;
+    T.w2_krow = (size_t)T.w2_kblocks * 64;
+    rc = dev_alloc(t->allocs, &T.dcol, (size_t)m->B * L.H * L.W * T.dcol_ld, true); if (rc) return rc;
+    gg.Ho = L.H; gg.Wo = L.W; gg.cout = T.dcol_ld;
+  } else {
+    rows = T.cin;
+    T.w2_krow = (size_t)T.taps * T.w2_kblocks * 64;
+    gg.kh = d.kh; gg.kw = d.kw; gg.dilation = d.dilation;
+    gg.pad_t = d.dilation * (d.kh - 1) - d.pad_t; gg.pad_l = d.dilation * (d.kw - 1) - d.pad_l;
+    gg.Ho = PL.H; gg.Wo = PL.W; gg.cout = T.cin;
   }
-  t->xT_elems = max_xT; t->dyT_elems = max_dyT;
-  rc = t_alloc(t, &t->xT_hi, (size_t)max_xT + 4096, true); if (rc) return fail(rc);
-  rc = t_alloc(t, &t->dyT_hi, (size_t)max_dyT + 4096, true); if (rc) return fail(rc);
-  if (m->split) {
-    rc = t_alloc(t, &t->xT_lo, (size_t)max_xT + 4096, true); if (rc) return fail(rc);
-    rc = t_alloc(t, &t->dyT_lo, (size_t)max_dyT + 4096, true); if (rc) return fail(rc);
+  rc = dev_alloc(t->allocs, &T.w2_hi, (size_t)rows * T.w2_krow, true); if (rc) return rc;
+  if (m->split) { rc = dev_alloc(t->allocs, &T.w2_lo, (size_t)rows * T.w2_krow, true); if (rc) return rc; }
+  rc = plan_conv_gemm(m, T.dgrad, gg, T.w2_hi, T.w2_lo, T.w2_krow, T.w2_kblocks, &T.dgrad_tiles);
+  if (rc) return rc;
+  ConvArgs& a = T.dgrad.args;
+  a.bias = nullptr; a.act = SSDK_ACT_NONE;
+  if (T.dgrad_strided) {
+    a.epi = EPI_F32; a.out_f32 = T.dcol;
+    T.dgrad_relu_mask = relu_mask;
+    T.dgrad_col2im_accumulate = written[pi];
+  } else {
+    a.epi = EPI_SPLIT;
+    a.out_hi = PT.g.hi; a.out_lo = PT.g.lo; a.out_Hp = PT.g.Hp(); a.out_Wp = PT.g.Wp(); a.out_pad = PT.g.pad; a.out_Cs = PT.g.Cs;
+    a.mask_hi = relu_mask ? PL.out.hi : nullptr;
+    a.accumulate = written[pi];
   }
-  // weight-gradient GEMM plans (need the scratch addresses)
-  for (int i = 0; i < n; ++i) {
-    LayerPlan& L = m->layers[i];
+  written[pi] = 1;
+  return SSDK_OK;
+}
+
+// Weight-gradient plan of conv layer i: wgrad.cu's GEMM on dZ / X in place, or the geometry of the transposed operands (their
+// GEMMs are planned by plan_transposed_gemms once the shared scratch is sized).  Direct layers need none.
+int plan_wgrad_layer(ssdk_trainer* t, int i, long long& max_xT, long long& max_dyT) {
+  ssdk_model* m = t->m;
+  const LayerPlan& L = m->layers[i];
+  TLayer& T = t->tl[i];
+  const ssdk_layer_desc& d = L.d;
+  if (L.direct) return SSDK_OK;               // handled by wgrad_direct_kernel
+  const ActBuf& X = m->layers[d.input].out;
+  if (!L.im2col && !getenv("SSDK_WGRAD_TRANSPOSED") && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
+    T.wg_native = true;
+    return plan_wgrad(m->ctx, T.wg, X, T.g, L.H, L.W, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, m->split, span_grad(t, i, 0));
+  }
+  if (L.im2col) {
+    T.Kv = (long long)m->B * L.H * L.W;
+    T.ldT = (T.Kv + 7) / 8 * 8 + 64;
+    T.dy_map = TMap{0, L.H * L.W, L.W, L.H, L.W, T.g.Hp(), T.g.Wp(), T.g.pad};
+    T.x_map = TMap{1, 0, 0, 0, 0, 0, 0, 0};
+    max_xT = std::max(max_xT, (long long)L.Kpad * T.ldT);
+  } else {
+    // the GEMM's pixel axis runs over X's padded grid with the row pitch rounded up to 8 elements: tap shifts are then
+    // kh*Wq + kw (+ const) and only the kw part can break TMA's 16-byte alignment -> one XT copy per distinct kw residue
+    const int Wq = (X.Wp() + 7) / 8 * 8;
+    T.Wq = Wq;
+    T.Kv = (long long)m->B * X.Hp() * Wq;
+    T.ldT = (T.Kv + 7) / 8 * 8 + 64;
+    T.dy_map = TMap{0, X.Hp() * Wq, Wq, L.H, L.W, T.g.Hp(), T.g.Wp(), T.g.pad};
+    T.x_map = TMap{0, X.Hp() * Wq, Wq, X.Hp(), X.Wp(), X.Hp(), X.Wp(), 0};
+    max_xT = std::max(max_xT, (long long)X.Cs * T.ldT);
+  }
+  max_dyT = std::max(max_dyT, (long long)T.g.Cs * T.ldT);
+  return SSDK_OK;
+}
+
+// The weight-gradient GEMMs of the transposed path (one per tap, or one for an im2col layer) on the shared scratch
+int plan_transposed_gemms(ssdk_trainer* t) {
+  ssdk_model* m = t->m;
+  for (int i = 0; i < (int)m->layers.size(); ++i) {
+    const LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
-    if (!is_conv(L.d.op) || L.direct) continue;
-    if (T.wg_native) { T.wg.args.dw = t->grad + T.off_w; continue; }
+    if (!is_conv(L.d.op) || L.direct || T.wg_native) continue;
     const ssdk_layer_desc& d = L.d;
     const ActBuf& X = m->layers[d.input].out;
     const int n_gemm = L.im2col ? 1 : T.taps;
@@ -623,11 +629,11 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       wg.Ho = T.cout; wg.Wo = 1; wg.B = 1; wg.cout = ncols;
       ConvLaunch& cl = T.wgrad[tp];
       // the transposed operands are [channels][ldT] with zeros in [Kv, ldT)
-      rc = plan_conv_gemm(m, cl, wg, t->xT_hi, t->xT_lo, (size_t)T.ldT, kblocks, nullptr);
-      if (rc) return fail(rc);
+      int rc = plan_conv_gemm(m, cl, wg, t->xT_hi, t->xT_lo, (size_t)T.ldT, kblocks, nullptr);
+      if (rc) return rc;
       ConvArgs& a = cl.args;
       a.epi = EPI_ATOMIC; a.bias = nullptr; a.act = SSDK_ACT_NONE;
-      a.out_f32 = t->grad + T.off_w;
+      a.out_f32 = span_grad(t, i, 0);
       if (L.im2col) { a.out_ld = T.taps * T.cin; a.out_col_off = 0; a.b_k_offset = 0; a.cout = T.taps * T.cin; a.n_tiles_n = (a.cout + a.BN - 1) / a.BN; }
       else {
         const int kh = tp / d.kw, kw = tp % d.kw;
@@ -644,9 +650,50 @@ extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_tra
       cl.grid = std::max(1, std::min(units * a.k_split, m->ctx->sm_count));
     }
   }
+  return SSDK_OK;
+}
+
+// Everything ssdk_trainer_create makes; on failure the caller destroys the partly made trainer
+int plan_trainer(ssdk_trainer* t, float* flat_grad_dev) {
+  ssdk_model* m = t->m;
+  const int n = (int)m->layers.size();
+  t->tl.resize(n);
+  int rc = plan_params(t, flat_grad_dev); if (rc) return rc;
+  rc = dev_alloc(t->allocs, &t->dypred, (size_t)m->B * m->P * (m->Ctot + 12), true); if (rc) return rc;
+  rc = alloc_grad_planes(t); if (rc) return rc;
+  // in the backward pass's order: does the producer's gradient buffer already hold a contribution?
+  std::vector<char> written(n, 0);
+  long long max_xT = 0, max_dyT = 0;
+  for (int i = n - 1; i >= 0; --i) {
+    const ssdk_layer_desc& d = m->layers[i].d;
+    if (is_source(d.op)) continue;
+    if (!is_conv(d.op)) { if (!is_source(m->layers[d.input].d.op)) written[d.input] = 1; continue; }
+    rc = plan_dgrad(t, i, written); if (rc) return rc;
+    rc = plan_wgrad_layer(t, i, max_xT, max_dyT); if (rc) return rc;
+  }
+  rc = dev_alloc(t->allocs, &t->xT_hi, (size_t)max_xT + 4096, true); if (rc) return rc;
+  rc = dev_alloc(t->allocs, &t->dyT_hi, (size_t)max_dyT + 4096, true); if (rc) return rc;
+  if (m->split) {
+    rc = dev_alloc(t->allocs, &t->xT_lo, (size_t)max_xT + 4096, true); if (rc) return rc;
+    rc = dev_alloc(t->allocs, &t->dyT_lo, (size_t)max_dyT + 4096, true); if (rc) return rc;
+  }
+  rc = plan_transposed_gemms(t); if (rc) return rc;
   for (int i = 0; i < n; ++i)
-    if (is_conv(m->layers[i].d.op)) { rc = repack_layer(t, i, 0); if (rc) return fail(rc); }
+    if (is_conv(m->layers[i].d.op)) { rc = repack_layer(t, i, 0); if (rc) return rc; }
   SSDK_CHECK_CUDA(cudaDeviceSynchronize());
+  return SSDK_OK;
+}
+
+}  // namespace
+
+extern "C" int ssdk_trainer_create(ssdk_model* m, float* flat_grad_dev, ssdk_trainer** out) {
+  SSDK_REQUIRE(m && out, "ssdk_trainer_create: NULL argument");
+  SSDK_REQUIRE(m->training, "ssdk_trainer_create: the model plan was not created with training=1");
+  SSDK_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  ssdk_trainer* t = new ssdk_trainer();
+  t->m = m;
+  const int rc = plan_trainer(t, flat_grad_dev);
+  if (rc) { ssdk_trainer_destroy(t); return rc; }
   *out = t;
   return SSDK_OK;
 }
@@ -666,13 +713,8 @@ extern "C" int ssdk_trainer_num_params(const ssdk_trainer* t, long long* out_n) 
 
 extern "C" int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int which, long long* out_offset, long long* out_count) {
   SSDK_REQUIRE(t && out_offset && out_count && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_param_span: bad argument");
-  const TLayer& T = t->tl[layer];
-  *out_offset = -1; *out_count = 0;
-  if (which == 0 && T.off_w >= 0) { *out_offset = T.off_w; *out_count = (long long)T.cout * T.taps * T.cin; }
-  else if (which == 1 && T.off_b >= 0) { *out_offset = T.off_b; *out_count = T.cout; }
-  else if (which == 2 && T.off_g >= 0) { *out_offset = T.off_g; *out_count = t->m->layers[layer].C; }
-  else if (which == 3 && T.off_bng >= 0) { *out_offset = T.off_bng; *out_count = T.cout; }
-  else if (which == 4 && T.off_bnb >= 0) { *out_offset = T.off_bnb; *out_count = T.cout; }
+  const ParamSpan* p = find_span(t, layer, which);
+  *out_offset = p ? p->off : -1; *out_count = p ? p->count : 0;
   return SSDK_OK;
 }
 
@@ -834,7 +876,7 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     if (d.op == SSDK_OP_L2NORM) {
       if (prod_needs_grad) {
         const size_t total = (size_t)PL.out.B * PL.out.H * PL.out.W;
-        l2norm_bwd_kernel<<<(unsigned)((total + 7) / 8), 256, 0, s>>>(PL.out, T.g, PT.g, L.gamma, t->grad + T.off_g, relu_mask, written[pi] ? 1 : 0);
+        l2norm_bwd_kernel<<<(unsigned)((total + 7) / 8), 256, 0, s>>>(PL.out, T.g, PT.g, L.gamma, span_grad(t, i, 2), relu_mask, written[pi] ? 1 : 0);
         SSDK_COUNT_LAUNCH(ctx);
         written[pi] = 1;
       }
@@ -842,7 +884,7 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     }
     // ---- conv + BatchNormalization + activation: the gradient planes hold d loss / d activation; turn them into the gradient of
     //      the raw conv output (and produce dgamma / dbeta) before the conv's own gradients are formed
-    if (L.bn_train) { rc = launch_bn_backward(ctx, L, d.act, T.g, t->grad + T.off_bng, t->grad + T.off_bnb, s); if (rc) return rc; }
+    if (L.bn_train) { rc = launch_bn_backward(ctx, L, d.act, T.g, span_grad(t, i, 3), span_grad(t, i, 4), s); if (rc) return rc; }
     // ---- convolution / head: weight + bias gradients
     if (L.direct) {
       const int K = T.taps * T.cin;
@@ -857,13 +899,13 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       const int total_rows = T.g.B * T.g.H;
       const int rpb = std::max(1, (total_rows + 8 * ctx->sm_count - 1) / (8 * ctx->sm_count));
       const bool fast3 = direct_fast3(d, PL.out, T.cin, T.cout);
-      if (fast3) wgrad_direct3x3_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, t->grad + T.off_w, d.pad_t, d.pad_l, rpb);
-      else wgrad_direct_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, t->grad + T.off_w, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
+      if (fast3) wgrad_direct3x3_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, span_grad(t, i, 0), d.pad_t, d.pad_l, rpb);
+      else wgrad_direct_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, span_grad(t, i, 0), d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
       SSDK_COUNT_LAUNCH(ctx);
-      rc = launch_bias_grad(ctx, T.g, t->grad + T.off_b, s); if (rc) return rc;
+      rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     } else if (T.wg_native) {
       rc = launch_wgrad(ctx, T.wg, s); if (rc) return rc;
-      rc = launch_bias_grad(ctx, T.g, t->grad + T.off_b, s); if (rc) return rc;
+      rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     } else {
       // transposed operands
       rc = do_transpose(t, T.g.hi, T.g.lo, T.g.Cs, (long long)T.g.rows(), T.dy_map, T.Kv, T.cout, t->dyT_hi, t->dyT_lo, T.ldT, s); if (rc) return rc;
@@ -882,7 +924,7 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
         }
       }
       dim3 gr(64, T.cout);
-      rowsum_kernel<<<gr, 256, 0, s>>>(t->dyT_hi, t->dyT_lo, T.ldT, T.Kv, t->grad + T.off_b);
+      rowsum_kernel<<<gr, 256, 0, s>>>(t->dyT_hi, t->dyT_lo, T.ldT, T.Kv, span_grad(t, i, 1));
       SSDK_COUNT_LAUNCH(ctx);
     }
     // ---- data gradient
@@ -903,122 +945,67 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
   return SSDK_OK;
 }
 
+// the spans of a conv / head layer end at span k: its bf16 planes can be re-packed from the updated master
+bool ends_conv_layer(const ssdk_trainer* t, size_t k) {
+  const int li = t->params[k].layer;
+  return is_conv(t->m->layers[li].d.op) && (k + 1 == t->params.size() || t->params[k + 1].layer != li);
+}
+
+// span p of `src` (its value, or its optimiser state) into out_dev, in the gradient's layout
+int read_span(ssdk_trainer* t, const ParamSpan& p, const float* src, float* out_dev, cudaStream_t s) {
+  if (p.taps) {
+    hwio_to_ohwi_kernel<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(src, p.taps, p.cin, p.cout, out_dev + p.off);
+    SSDK_COUNT_LAUNCH(t->m->ctx);
+  } else {
+    SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + p.off, src, (size_t)p.count * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  }
+  return SSDK_OK;
+}
+
 }  // namespace
 
 extern "C" int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float l2_reg, float grad_scale, void* stream_) {
   SSDK_REQUIRE(t, "ssdk_train_apply: NULL trainer");
-  ssdk_model* m = t->m;
-  ssdk_ctx* ctx = m->ctx;
   cudaStream_t s = (cudaStream_t)stream_;
-  int rc;
-  for (size_t i = 0; i < t->tl.size(); ++i) {
-    TLayer& T = t->tl[i];
-    LayerPlan& L = m->layers[i];
-    if (T.off_g >= 0) {
-      sgd_kernel_flat<<<(unsigned)((L.C + 255) / 256), 256, 0, s>>>(L.gamma, T.vgamma, t->grad + T.off_g, (size_t)L.C, lr, momentum, grad_scale);
-      SSDK_COUNT_LAUNCH(ctx);
-    }
-    if (T.off_w < 0) continue;
-    const size_t nw = (size_t)T.taps * T.cin * T.cout;
-    sgd_kernel_w<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(L.w_f32, T.vw, t->grad + T.off_w, T.taps, T.cin, T.cout, lr, momentum, l2_reg, grad_scale);
-    SSDK_COUNT_LAUNCH(ctx);
-    sgd_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bias, T.vb, t->grad + T.off_b, (size_t)T.cout, lr, momentum, grad_scale);
-    SSDK_COUNT_LAUNCH(ctx);
-    if (T.off_bng >= 0) {
-      sgd_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_gamma, T.m_bng, t->grad + T.off_bng, (size_t)T.cout, lr, momentum, grad_scale);
-      sgd_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_beta, T.m_bnb, t->grad + T.off_bnb, (size_t)T.cout, lr, momentum, grad_scale);
-      SSDK_COUNT_LAUNCH(ctx); SSDK_COUNT_LAUNCH(ctx);
-    }
-    rc = repack_layer(t, (int)i, s); if (rc) return rc;
+  for (size_t k = 0; k < t->params.size(); ++k) {
+    const ParamSpan& p = t->params[k];
+    const auto sgd = p.taps ? sgd_kernel<true> : sgd_kernel<false>;
+    sgd<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(p.value, t->state[0] + p.off, t->grad + p.off, (size_t)p.count, p.taps, p.cin, p.cout,
+                                                           lr, momentum, l2_reg, grad_scale);
+    SSDK_COUNT_LAUNCH(t->m->ctx);
+    if (ends_conv_layer(t, k)) { const int rc = repack_layer(t, p.layer, s); if (rc) return rc; }
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
-namespace {
-
-__global__ void adam_kernel_w(float* __restrict__ w, float* __restrict__ m1, float* __restrict__ m2, const float* __restrict__ g, int taps, int cin,
-                              int cout, float lr_t, float b1, float b2, float eps, float l2, float scale) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t total = (size_t)taps * cin * cout;
-  if (i >= total) return;
-  const int co = (int)(i % cout); const size_t r = i / cout; const int ci = (int)(r % cin); const int t = (int)(r / cin);
-  const float grad = g[((size_t)co * taps + t) * cin + ci] * scale + 2.f * l2 * w[i];
-  const float a = b1 * m1[i] + (1.f - b1) * grad;
-  const float b = b2 * m2[i] + (1.f - b2) * grad * grad;
-  m1[i] = a; m2[i] = b;
-  w[i] -= lr_t * a / (sqrtf(b) + eps);
-}
-__global__ void adam_kernel_flat(float* __restrict__ w, float* __restrict__ m1, float* __restrict__ m2, const float* __restrict__ g, size_t n,
-                                 float lr_t, float b1, float b2, float eps, float scale) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float grad = g[i] * scale;
-  const float a = b1 * m1[i] + (1.f - b1) * grad;
-  const float b = b2 * m2[i] + (1.f - b2) * grad * grad;
-  m1[i] = a; m2[i] = b;
-  w[i] -= lr_t * a / (sqrtf(b) + eps);
-}
-
-}  // namespace
-
 extern "C" int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, float beta2, float eps, float l2_reg, float grad_scale, int step,
                                      void* stream_) {
   SSDK_REQUIRE(t && step >= 1, "ssdk_train_apply_adam: bad argument");
-  ssdk_model* m = t->m;
-  ssdk_ctx* ctx = m->ctx;
   cudaStream_t s = (cudaStream_t)stream_;
   // Keras: lr_t = lr * sqrt(1 - beta_2^t) / (1 - beta_1^t)
   const float lr_t = lr * (float)(std::sqrt(1.0 - std::pow((double)beta2, (double)step)) / (1.0 - std::pow((double)beta1, (double)step)));
-  int rc;
-  for (size_t i = 0; i < t->tl.size(); ++i) {
-    TLayer& T = t->tl[i];
-    LayerPlan& L = m->layers[i];
-    if (T.off_g >= 0) {
-      if (!T.v2gamma) { rc = t_alloc(t, &T.v2gamma, (size_t)L.C, true); if (rc) return rc; }
-      adam_kernel_flat<<<(unsigned)((L.C + 255) / 256), 256, 0, s>>>(L.gamma, T.vgamma, T.v2gamma, t->grad + T.off_g, (size_t)L.C, lr_t, beta1, beta2, eps, grad_scale);
-      SSDK_COUNT_LAUNCH(ctx);
-    }
-    if (T.off_w < 0) continue;
-    const size_t nw = (size_t)T.taps * T.cin * T.cout;
-    if (!T.v2w) { rc = t_alloc(t, &T.v2w, nw, true); if (rc) return rc; rc = t_alloc(t, &T.v2b, (size_t)T.cout, true); if (rc) return rc; }
-    adam_kernel_w<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(L.w_f32, T.vw, T.v2w, t->grad + T.off_w, T.taps, T.cin, T.cout, lr_t, beta1, beta2, eps, l2_reg, grad_scale);
-    SSDK_COUNT_LAUNCH(ctx);
-    adam_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bias, T.vb, T.v2b, t->grad + T.off_b, (size_t)T.cout, lr_t, beta1, beta2, eps, grad_scale);
-    SSDK_COUNT_LAUNCH(ctx);
-    if (T.off_bng >= 0) {
-      adam_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_gamma, T.m_bng, T.v_bng, t->grad + T.off_bng, (size_t)T.cout, lr_t, beta1, beta2, eps, grad_scale);
-      adam_kernel_flat<<<(unsigned)((T.cout + 255) / 256), 256, 0, s>>>(L.bn_beta, T.m_bnb, T.v_bnb, t->grad + T.off_bnb, (size_t)T.cout, lr_t, beta1, beta2, eps, grad_scale);
-      SSDK_COUNT_LAUNCH(ctx); SSDK_COUNT_LAUNCH(ctx);
-    }
-    rc = repack_layer(t, (int)i, s); if (rc) return rc;
+  if (!t->state[1]) { const int rc = dev_alloc(t->allocs, &t->state[1], (size_t)t->n_params, true); if (rc) return rc; }
+  for (size_t k = 0; k < t->params.size(); ++k) {
+    const ParamSpan& p = t->params[k];
+    const auto adam = p.taps ? adam_kernel<true> : adam_kernel<false>;
+    adam<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(p.value, t->state[0] + p.off, t->state[1] + p.off, t->grad + p.off, (size_t)p.count,
+                                                            p.taps, p.cin, p.cout, lr_t, beta1, beta2, eps, l2_reg, grad_scale);
+    SSDK_COUNT_LAUNCH(t->m->ctx);
+    if (ends_conv_layer(t, k)) { const int rc = repack_layer(t, p.layer, s); if (rc) return rc; }
   }
-  t->adam = true;
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
 extern "C" int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out_dev, void* stream_) {
   SSDK_REQUIRE(t && out_dev, "ssdk_trainer_read_opt_state: NULL argument");
-  SSDK_REQUIRE(slot == 0 || (slot == 1 && t->adam),
+  SSDK_REQUIRE((slot == 0 || slot == 1) && t->state[slot],
                "ssdk_trainer_read_opt_state: slot %d does not exist (0: SGD velocity / Adam first moment, 1: Adam second moment, "
                "after an Adam update)", slot);
-  ssdk_model* m = t->m;
-  cudaStream_t s = (cudaStream_t)stream_;
-  for (size_t i = 0; i < t->tl.size(); ++i) {
-    TLayer& T = t->tl[i];
-    LayerPlan& L = m->layers[i];
-    if (T.off_g >= 0)
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_g, slot ? T.v2gamma : T.vgamma, (size_t)L.C * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if (T.off_w < 0) continue;
-    const size_t nw = (size_t)T.taps * T.cin * T.cout;
-    hwio_to_ohwi_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(slot ? T.v2w : T.vw, T.taps, T.cin, T.cout, out_dev + T.off_w);
-    SSDK_COUNT_LAUNCH(m->ctx);
-    SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_b, slot ? T.v2b : T.vb, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if (T.off_bng >= 0) {
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bng, slot ? T.v_bng : T.m_bng, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bnb, slot ? T.v_bnb : T.m_bnb, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    }
+  for (const ParamSpan& p : t->params) {
+    const int rc = read_span(t, p, t->state[slot] + p.off, out_dev, (cudaStream_t)stream_);
+    if (rc) return rc;
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
@@ -1042,21 +1029,9 @@ extern "C" int ssdk_trainer_read_bn_input(ssdk_trainer* t, int layer, float* out
 
 extern "C" int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream_) {
   SSDK_REQUIRE(t && out_dev, "ssdk_trainer_read_params: NULL argument");
-  ssdk_model* m = t->m;
-  cudaStream_t s = (cudaStream_t)stream_;
-  for (size_t i = 0; i < t->tl.size(); ++i) {
-    TLayer& T = t->tl[i];
-    LayerPlan& L = m->layers[i];
-    if (T.off_g >= 0) SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_g, L.gamma, (size_t)L.C * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if (T.off_w < 0) continue;
-    const size_t nw = (size_t)T.taps * T.cin * T.cout;
-    hwio_to_ohwi_kernel<<<(unsigned)((nw + 255) / 256), 256, 0, s>>>(L.w_f32, T.taps, T.cin, T.cout, out_dev + T.off_w);
-    SSDK_COUNT_LAUNCH(m->ctx);
-    SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_b, L.bias, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    if (T.off_bng >= 0) {
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bng, L.bn_gamma, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + T.off_bnb, L.bn_beta, (size_t)T.cout * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    }
+  for (const ParamSpan& p : t->params) {
+    const int rc = read_span(t, p, p.value, out_dev, (cudaStream_t)stream_);
+    if (rc) return rc;
   }
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

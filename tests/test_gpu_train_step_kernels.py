@@ -1,6 +1,6 @@
 """GPU tests of the launches a training step makes besides the convolutions and the backward pass, one launch at a time,
 against the operand-exact float64 references of oracle/opexact.py (sections 6 - 10 there):
-- the optimiser (sgd_kernel_w / _flat, adam_kernel_w / _flat) over several steps, each update judged on the parameters and the
+- the optimiser (sgd_kernel<true / false>, adam_kernel<true / false>) over several steps, each update judged on the parameters and the
   optimiser state read just before it (ssdk_trainer_read_params / ssdk_trainer_read_opt_state);
 - the re-pack after an update: the forward planes and the data-gradient planes must hold the new master;
 - the training-phase forward launches that are not convolutions: BatchNormalization (three consecutive passes, with the moving

@@ -502,7 +502,7 @@ def test_sgd_reference_loop_emulation_and_perturbations(contract, kernel):
                         want_w[i] = float(w[i]) + want_v[i]
         np.testing.assert_allclose(ref['v'], want_v, rtol=1e-13, atol=1e-300)
         np.testing.assert_allclose(ref['w'], want_w, rtol=1e-13, atol=1e-300)
-        # fp32 emulation of sgd_kernel_w / sgd_kernel_flat
+        # fp32 emulation of sgd_kernel<true> / sgd_kernel<false>
         gr = _grad32(w, g, l2, s, ks, contract) if kernel else (g * np.float32(s)).astype(np.float32)
         nv = _fma(np.float32(0.9), v, -(np.float32(lr) * gr).astype(np.float32), contract)
         got = {'w': (w + nv).astype(np.float32), 'v': nv}
@@ -534,7 +534,7 @@ def test_adam_reference_loop_emulation_and_perturbations(contract):
             assert abs(ref['m'][i] - mi) <= 1e-13 * abs(mi) and abs(ref['v'][i] - vi) <= 1e-13 * abs(vi)
             wi = float(w[i]) - lr_t * mi / (np.sqrt(vi) + float(eps))
             assert abs(ref['w'][i] - wi) <= 1e-13 * abs(wi)
-        # fp32 emulation of adam_kernel_w
+        # fp32 emulation of adam_kernel<true>
         lr_t32 = np.float32(np.float32(np.sqrt(1.0 - float(b2) ** t) / (1.0 - float(b1) ** t)) * np.float32(lr))
         gr = _grad32(w, g, l2, s, KSHAPE, contract)
         a = _fma(b1, m, ((np.float32(1) - b1) * gr).astype(np.float32), contract)
