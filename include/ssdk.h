@@ -284,6 +284,29 @@ int ssdk_ssd_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true_dev, const
                         const int* ties_all_dev /* [world], phase 4 */, int rank, const float* upstream_dev,
                         float* out_loss_dev, int* out_stats_dev, float* out_grad_dev, void* stream);
 
+/* Read-only views of the loss kernel, for tests and diagnostics.
+ *   ssdk_ssd_loss_plan  the launch a call with these arguments would make (want_grad: bwd / fwd_bwd / phase 4 with a gradient;
+ *                       cooperative: the fused entry points, 0 = ssdk_ssd_loss_phase), or the error that call would return.
+ *                       stages: shared-memory tile buffers (1 or 2); bulk_ok: tiles are loaded with cp.async.bulk (P*(C+12)
+ *                       a multiple of 4 and both inputs 16-byte aligned), else by plain loads.  Launches nothing and changes
+ *                       no state of the context (workspace, histogram parity).  Like a call of the same size, it may raise
+ *                       the kernels' process-wide cudaFuncAttributeMaxDynamicSharedMemorySize, which the occupancy query
+ *                       behind `grid` needs; that attribute only ever grows and changes no result.
+ *   ssdk_ssd_loss_read_box_losses  the per-box losses the last call's first phase stored, [B*P] float32 each: cls (the
+ *                       log-loss of the box, :93-95) and negl = cls * y_true[..., 0] (:151), the values the hard-negative
+ *                       selection ranks.  ws_dev NULL reads the context's own workspace (an error unless its last fused call
+ *                       had this (B, P)); otherwise a phase workspace (ssdk_ssd_loss_phase) after its phase 0.  Either output
+ *                       may be NULL. */
+typedef struct {
+  int stages;
+  int bulk_ok;
+  int grid;
+  long long smem_bytes;       /* dynamic shared memory per CTA */
+} ssdk_loss_plan;
+int ssdk_ssd_loss_plan(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
+                       int want_grad, int cooperative, ssdk_loss_plan* out);
+int ssdk_ssd_loss_read_box_losses(ssdk_ctx* ctx, const void* ws_dev, int B, int P, float* cls_dev, float* negl_dev, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Model graph.  Replaces ssd_300 (models/keras_ssd300.py:31-457), ssd_512 (models/keras_ssd512.py:31-477)
  * and build_model (models/keras_ssd7.py:30-430) + L2Normalization

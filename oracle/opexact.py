@@ -78,6 +78,26 @@ u = 2**-24 is the unit roundoff of fp32; a rounding of a value t loses at most u
    s = rsqrt(1e-12): max is continuous, so the reference uses the same formula in float64.
 10. Max-pooling and the input preprocessing move or compute values without an accumulation: ``pool_fwd_ref`` (the hi and lo
    planes of the first maximum of hi + lo) and ``preprocess_ref`` ((x - mean) / std in fp32, channel swap, split) are bit-exact.
+11. The SSD loss (ssd_loss_kernel, ssd_loss_phase_kernel; loss.cu builds with --fmad=false, so every product and every add is
+   one rounding).  ``loss_ref`` takes y_true, y_pred and the per-box losses the kernel stored (ssdk_ssd_loss_read_box_losses):
+   cls = -sum_c tv_c logf(max(p_c, 1e-15f)) and negl = cls * y_true[..., 0].
+   - negl must be fl(cls * yt0) bit for bit.  cls: logf is within 1 ulp (2 u relative), the product with tv one rounding, the
+     first add to 0 exact and the n - 1 others one each, every partial sum bounded by S = sum |tv log p| (1 + 3u):
+        |cls - cls_ref| <= (n + 2) u S (1 + 2**-20),   n = the non-zero tv of the box.
+   - The hard-negative selection is exact on the kernel's negl: k = min(max(ratio n_pos, n_neg_min), nnz) over the whole batch
+     (n_pos = int(fp32 sum of the positive flags), nnz = the non-zero negl), ordered by value descending, then flat index
+     ascending, -0 == +0 (tf.nn.top_k).  n_pos, nnz, k and `want` (the boxes equal to the k-th value that are kept) are exact.
+   - Smooth L1 is not stored: d = fl(yt - yp) is off by u |d|, and f(x) = 0.5 x^2 (|x| < 1) or |x| - 0.5 has |f'| <= min(|x|, 1)
+     (both branches give 0.5 at |d| = 1, so a d that rounds onto the other side moves f by the same amount); each f adds one
+     rounding, the three adds one each:  |l - l_ref| <= (u sum_j |d_j| min(1, |d_j|) + 4 u l_ref) (1 + 2**-20).
+   - The per-image loss (pc + ng + alpha loc) inv_norm global_B is summed in float64 from fp32 products: cls pmax and l pmax
+     one rounding each (u of the term; l carries its bound into the sum), the float64 sums (N + 8) 2**-53 of the absolute
+     sum, inv_norm = fp32(1 / max(1, n_pos)) is an operand, and the store one unit (2**-23) of the result.
+   - The gradient of a class entry is (-tv / q) w_cls, w_cls = (pmax + take) (up global_B inv_norm): up * global_B, * inv_norm,
+     pmax + take, * scale, the division and the last product are six roundings; a loc entry slope(fl(yp - yt)) (pmax scale alpha)
+     has six too (the difference, the two of scale, * pmax, * alpha, the product; slope = clip(d, -1, 1) is 1-Lipschitz and
+     exact at |d| = 1).  Each is a product of exactly rounded factors:  |g - g_ref| <= 6 u |g_ref| (1 + 2**-20).  q < 1e-15f
+     gives 0.  upstream is read as float32 operands (NULL: fp32(1 / global_B)).
 
 The module is CPU only: NumPy for the bit-level rounding, torch float64 for the convolutions.
 """
@@ -775,3 +795,155 @@ def preprocess_ref(img, mean=None, std=None, swap=None):
         t = (t / np.asarray(std, np.float32)).astype(np.float32)
     t = t[..., list(swap) if swap is not None else [0, 1, 2]]
     return split(t)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the SSD loss (section 11)
+# ------------------------------------------------------------------------------------------------------------------------------
+LOSS_PERTURBATIONS = ('drop_last', 'add_next', 'tie_reverse', 'per_image', 'signed_zero', 'no_max1', 'no_alpha', 'loc_by_yt0',
+                      'no_upstream', 'local_B', 'k_no_cap')
+_SLACK = 1.0 + 2.0 ** -20
+
+
+def okey(x):
+    """The selection's order key of float32 values (okey of csrc/loss.cu): a larger value has a larger key; -0 and +0 share
+    0x80000000."""
+    x = np.ascontiguousarray(x, np.float32)
+    b = x.view(np.uint32)
+    k = np.where(b & np.uint32(0x80000000), ~b, b | np.uint32(0x80000000)).astype(np.uint32)
+    return np.where(x == 0, np.uint32(0x80000000), k).astype(np.uint32)
+
+
+def loss_box_ref(y_true, y_pred):
+    """Per-box float64 references and bounds -> (cls, cls_bound, loc, loc_bound), each (B, P) (section 11)."""
+    yt, yp = _f64(y_true), _f64(y_pred)
+    C = yt.shape[-1] - 12
+    tv = yt[..., :C]
+    nz = tv != 0
+    terms = np.where(nz, tv * np.log(np.maximum(yp[..., :C], float(np.float32(1e-15)))), 0.0)
+    cls = -terms.sum(-1)
+    cls_b = (nz.sum(-1) + 2) * U32 * np.abs(terms).sum(-1) * _SLACK
+    d = yt[..., C:C + 4] - yp[..., C:C + 4]
+    ad = np.abs(d)
+    loc = np.where(ad < 1.0, 0.5 * d * d, ad - 0.5).sum(-1)
+    loc_b = (U32 * (ad * np.minimum(ad, 1.0)).sum(-1) + 4 * U32 * loc) * _SLACK
+    return cls, cls_b, loc, loc_b
+
+
+def _order(v, signed_zero=False):
+    """Flat indices by value descending, then index ascending (tf.nn.top_k); signed_zero orders -0 below +0."""
+    v = np.ascontiguousarray(v, np.float32).reshape(-1)
+    if signed_zero:
+        b = v.view(np.uint32)
+        key = np.where(b & np.uint32(0x80000000), ~b, b | np.uint32(0x80000000)).astype(np.int64)
+    else:
+        key = okey(v).astype(np.int64)
+    return np.lexsort((np.arange(v.size), -key))
+
+
+def loss_select(negl, n_pos, ratio, n_neg_min, perturb=None, img_pos=None):
+    """The hard-negative mask over the batch -> (mask (B, P) bool, stats [n_pos, nnz, k, want]).  perturb: one selection
+    perturbation of LOSS_PERTURBATIONS or None (the stats stay those of the exact selection, except k for 'k_no_cap');
+    img_pos: per-image n_pos for 'per_image'."""
+    negl = np.ascontiguousarray(negl, np.float32)
+    B, P = negl.shape
+    flat = negl.reshape(-1)
+    nnz = int(np.count_nonzero(flat))
+    k = min(max(int(ratio) * int(n_pos), int(n_neg_min)), nnz)
+    mask = np.zeros(flat.size, bool)
+    stats = [int(n_pos), nnz, 0, 0]
+    if k > 0:
+        order = _order(flat)
+        mask[order[:k]] = True
+        ties = np.flatnonzero(okey(flat) == okey(flat[order[k - 1]]))
+        stats[2:] = [k, int(mask[ties].sum())]
+    if perturb == 'drop_last' and k > 0:
+        mask[order[k - 1]] = False
+    elif perturb == 'add_next' and k < flat.size:
+        mask[_order(flat)[k]] = True
+    elif perturb == 'tie_reverse' and k > 0:
+        mask[ties] = False
+        mask[ties[ties.size - stats[3]:]] = True
+    elif perturb == 'signed_zero' and k > 0:
+        mask[:] = False
+        mask[_order(flat, signed_zero=True)[:k]] = True
+    elif perturb == 'k_no_cap':
+        kk = min(max(int(ratio) * int(n_pos), int(n_neg_min)), flat.size)
+        mask[:] = False
+        mask[_order(flat)[:kk]] = True
+        stats[2] = kk
+    elif perturb == 'per_image':
+        mask[:] = False
+        for b in range(B):
+            vb = flat[b * P:(b + 1) * P]
+            kb = min(max(int(ratio) * int(img_pos[b]), int(n_neg_min)), int(np.count_nonzero(vb)))
+            mask[b * P + _order(vb)[:kb]] = True
+    return mask.reshape(B, P), stats
+
+
+def loss_ref(y_true, y_pred, cls, negl, ratio=3, n_neg_min=0, alpha=1.0, upstream=None, global_B=None, local_B=None, perturb=()):
+    """The SSD loss of one fused call (or of the whole batch of a phase-wise run) from the kernel's own per-box losses
+    (section 11) -> (ref, bound, {perturbation: ref'}).
+
+    ref: {'mask': (B, P) bool, 'stats': [n_pos, nnz, k, want], 'loss': (B,), 'grad': (B, P, C+12), 'cls': (B, P)}, float64;
+    bound: {'cls', 'loss', 'grad'} of the same shapes.  cls, negl: the kernel's (B, P) float32 arrays (their consistency,
+    negl == fl(cls * yt0), is the caller's check).  upstream: (B,) float32 or None (fp32(1 / global_B)); global_B: the batch
+    size of the normalisation (default B); local_B: one rank's B, for the 'local_B' perturbation.  perturb: names of
+    LOSS_PERTURBATIONS: the mask without its last kept box / with the first unkept one, ties kept from the highest index, top-k
+    per image, -0 below +0, no max(1, n_pos), alpha = 1, the loc term weighted by yt0, upstream ignored, local_B for global_B,
+    k not capped at nnz."""
+    yt, yp = np.asarray(y_true, np.float32), np.asarray(y_pred, np.float32)
+    B, P, W = yt.shape
+    C = W - 12
+    gB = B if global_B is None else int(global_B)
+    cls_k = _f64(cls)
+    cls_ref, cls_b, loc, loc_b = loss_box_ref(yt, yp)
+    pmax = _f64(yt[..., 1:C].max(-1))
+    n_pos_f = float(np.float32(np.sum(pmax)))
+    img_pos = [int(np.float32(pmax[b].sum())) for b in range(B)]
+    a32 = float(np.float32(alpha))
+    tv, q = _f64(yt[..., :C]), _f64(yp[..., :C])
+    live = (tv != 0) & (q >= float(np.float32(1e-15)))
+    dlog = np.where(live, -tv / np.where(live, q, 1.0), 0.0)
+    d = _f64(yp[..., C:C + 4]) - _f64(yt[..., C:C + 4])
+    slope = np.clip(d, -1.0, 1.0)
+
+    def run(p=None):
+        sel = p if p in ('drop_last', 'add_next', 'tie_reverse', 'per_image', 'signed_zero', 'k_no_cap') else None
+        mask, stats = loss_select(negl, int(n_pos_f), ratio, n_neg_min, sel, img_pos)
+        den = n_pos_f if p == 'no_max1' else max(1.0, n_pos_f)
+        inv = float(np.float32(1.0) / np.float32(den)) if den else np.inf
+        nb = local_B if p == 'local_B' else gB
+        al = 1.0 if p == 'no_alpha' else a32
+        wl = _f64(yt[..., 0]) if p == 'loc_by_yt0' else pmax
+        if upstream is None or p == 'no_upstream':
+            up = np.full(B, float(np.float32(1) / np.float32(nb)))
+        else:
+            up = _f64(upstream)
+        with np.errstate(invalid='ignore'):
+            tot = ((cls_k * pmax).sum(-1) + (cls_k * mask).sum(-1) + al * (loc * wl).sum(-1)) * inv * nb
+            scale = (up * nb * inv)[:, None]
+            g = np.zeros((B, P, W))
+            g[..., :C] = dlog * ((pmax + mask) * scale)[..., None]
+            g[..., C:C + 4] = slope * (wl * scale * al)[..., None]
+        return {'mask': mask, 'stats': stats, 'loss': tot, 'grad': g, 'cls': cls_ref}
+    ref = run()
+    inv = float(np.float32(1.0) / np.float32(max(1.0, n_pos_f)))
+    cp = np.abs(cls_k * pmax)
+    lp = loc * pmax
+    s_abs = cp.sum(-1) + (np.abs(cls_k) * ref['mask']).sum(-1) + abs(a32) * lp.sum(-1)
+    e = U32 * cp.sum(-1) + abs(a32) * (pmax * (loc_b + U32 * (loc + loc_b))).sum(-1) + (P + 8) * 2.0 ** -53 * s_abs
+    bnd = {'cls': cls_b, 'loss': e * inv * gB * _SLACK + UNIT['f32'] * np.abs(ref['loss']),
+           'grad': 6 * U32 * _SLACK * np.abs(ref['grad'])}
+    return ref, bnd, {p: run(p) for p in perturb}
+
+
+def loss_ratio(got, ref, bnd):
+    """max |got - ref| / bound; equal values pass a zero bound, and a NaN or an infinite difference is an infinite ratio."""
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    assert got.shape == ref.shape == bnd.shape, (got.shape, ref.shape, bnd.shape)
+    with np.errstate(invalid='ignore', divide='ignore', over='ignore'):
+        d = np.abs(got - ref)
+        r = np.where(d == 0, 0.0, d / np.maximum(bnd, np.finfo(np.float64).tiny))
+    r = np.where(np.isnan(r), np.inf, r)
+    return float(r.max()) if r.size else 0.0

@@ -59,6 +59,31 @@ class LossWsLayout(C.Structure):
                 ('hist2_offset', C.c_longlong), ('hist_n', C.c_longlong), ('ties_offset', C.c_longlong)]
 
 
+class LossPlan(C.Structure):
+    _fields_ = [('stages', C.c_int), ('bulk_ok', C.c_int), ('grid', C.c_int), ('smem_bytes', C.c_longlong)]
+
+
+def loss_plan(y_true, y_pred, n_classes_total, want_grad, cooperative=True):
+    """The launch the loss would make for these (B, P, C+12) device tensors, as a dict (ssdk_ssd_loss_plan); raises what the
+    launch would raise."""
+    B, P = y_pred.shape[0], y_pred.shape[1]
+    p = LossPlan()
+    check(lib().ssdk_ssd_loss_plan(context(y_pred.device.index), dptr(y_true), dptr(y_pred), B, P, int(n_classes_total),
+                                   int(bool(want_grad)), int(bool(cooperative)), C.byref(p)))
+    return {n: getattr(p, n) for n, _ in LossPlan._fields_}
+
+
+def loss_box_losses(B, P, ws=None, device=None):
+    """(cls, negl), (B, P) float32 device tensors: the per-box losses the loss kernel's first phase stored, in the context's own
+    workspace (ws None) or in a phase workspace (ssdk_ssd_loss_read_box_losses)."""
+    import torch
+    dev = ws.device if ws is not None else torch.device('cuda', torch.cuda.current_device() if device is None else device)
+    cls = torch.empty((B, P), dtype=torch.float32, device=dev)
+    negl = torch.empty_like(cls)
+    check(lib().ssdk_ssd_loss_read_box_losses(context(dev.index), dptr(ws), int(B), int(P), dptr(cls), dptr(negl), stream_ptr()))
+    return cls, negl
+
+
 class LayerDesc(C.Structure):
     _fields_ = [('op', C.c_int), ('input', C.c_int), ('cout', C.c_int), ('kh', C.c_int), ('kw', C.c_int),
                 ('stride', C.c_int), ('dilation', C.c_int), ('pad_t', C.c_int), ('pad_l', C.c_int),
@@ -159,7 +184,10 @@ def lib():
         L.ssdk_ssd_loss_ws_layout.argtypes = [C.c_int, C.c_int, C.POINTER(LossWsLayout)]
         L.ssdk_ssd_loss_phase.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp,
                                           C.c_int, vp, vp, vp, vp, vp]
-        for name in ('ssdk_ssd_loss_fwd_bwd', 'ssdk_ssd_loss_ws_layout', 'ssdk_ssd_loss_phase'):
+        L.ssdk_ssd_loss_plan.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(LossPlan)]
+        L.ssdk_ssd_loss_read_box_losses.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp]
+        for name in ('ssdk_ssd_loss_fwd_bwd', 'ssdk_ssd_loss_ws_layout', 'ssdk_ssd_loss_phase', 'ssdk_ssd_loss_plan',
+                     'ssdk_ssd_loss_read_box_losses'):
             getattr(L, name).restype = C.c_int
         L.ssdk_eval_match.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int, vp, vp, vp]
         L.ssdk_eval_cumsum.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp]

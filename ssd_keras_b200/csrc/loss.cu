@@ -32,7 +32,10 @@ constexpr int kFine = 65536;           // fine bins:   key >> 16 (level 1), key 
 constexpr int kCache = 2048;           // per-CTA direct-mapped cache of level-1 fine bins (slot = bin & 2047, tag = bin >> 11)
 constexpr unsigned kZeroKey = 0x80000000u;
 
-__device__ __forceinline__ unsigned okey(float f) {       // order-preserving key: larger float -> larger unsigned
+// order-preserving key: larger float -> larger unsigned.  -0 and +0 share kZeroKey: the histograms count both as the zero bin,
+// and tf.nn.top_k, which the selection restates, does not tell them apart (the lower flat index wins between them).
+__device__ __forceinline__ unsigned okey(float f) {
+  if (f == 0.f) return kZeroKey;
   unsigned b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
@@ -580,11 +583,49 @@ int check_args(ssdk_ctx* ctx, const float* yt, const float* yp, int B, int P, in
   return SSDK_OK;
 }
 
-struct LossPlan { int grid; size_t smem; };
+struct LossPlan { int grid; size_t smem; int stages; int bulk_ok; };
+
+// The launch shape of one call (stages, bulk loads, dynamic shared memory, grid) and whether it can run at all.  The launches and
+// ssdk_ssd_loss_plan both come here, so a plan is refused exactly when the launch would be; nothing here touches a workspace or
+// the histogram parity.
+int plan_launch(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C, bool grad, bool cooperative,
+                LossPlan& plan) {
+  const int W = C + 12;
+  // cp.async.bulk needs 16-byte aligned tile starts: image stride P*W*4 and tile stride 128*W*4 (always a multiple of 16)
+  plan.bulk_ok = (((size_t)P * W) % 4 == 0) && ((reinterpret_cast<uintptr_t>(y_true) & 15) == 0) && ((reinterpret_cast<uintptr_t>(y_pred) & 15) == 0) ? 1 : 0;
+  plan.stages = loss_smem_bytes(W, 2, grad) > 100 * 1024 ? 1 : 2;
+  plan.smem = loss_smem_bytes(W, plan.stages, grad);
+  // the dynamic shared memory a CTA may opt into is what the device allows per block less the kernels' static arrays
+  static size_t static_smem = 0;
+  if (!static_smem) {
+    cudaFuncAttributes fa, fb;
+    SSDK_CHECK_CUDA(cudaFuncGetAttributes(&fa, ssd_loss_kernel));
+    SSDK_CHECK_CUDA(cudaFuncGetAttributes(&fb, ssd_loss_phase_kernel));
+    static_smem = std::max(fa.sharedSizeBytes, fb.sharedSizeBytes);
+  }
+  const size_t limit = ctx->prop.sharedMemPerBlockOptin - static_smem;
+  SSDK_REQUIRE(plan.smem <= limit, "ssd_loss: %d classes need %zu bytes of shared memory per CTA%s, at most %zu fit", C, plan.smem,
+               grad ? " with the gradient" : "", limit);
+  static size_t attr[2] = {0, 0};
+  if (plan.smem > 48 * 1024) {
+    if (plan.smem > attr[0]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[0] = plan.smem; }
+    if (plan.smem > attr[1]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_phase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[1] = plan.smem; }
+  }
+  int per_sm = 0;
+  if (cooperative) SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_kernel, kRows, plan.smem));
+  else SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_phase_kernel, kRows, plan.smem));
+  SSDK_REQUIRE(per_sm > 0, "ssd_loss: the kernel does not fit on an SM (%zu bytes of shared memory)", plan.smem);
+  if (per_sm > 4) per_sm = 4;
+  const int n_tiles = B * ((P + kRows - 1) / kRows);
+  plan.grid = std::max(1, std::min(n_tiles, per_sm * ctx->sm_count));
+  return SSDK_OK;
+}
 
 // fills everything of LossArgs that depends on the shapes and the workspace; hist parity chosen by the caller
 int fill_args(ssdk_ctx* ctx, LossArgs& a, const float* y_true, const float* y_pred, int B, int P, int C, int ratio, int n_neg_min,
               float alpha, unsigned char* ws, int parity, bool grad, LossPlan& plan, bool cooperative) {
+  const int rc = plan_launch(ctx, y_true, y_pred, B, P, C, grad, cooperative, plan);
+  if (rc) return rc;
   const WsLayout L = ws_layout(B, P);
   memset(&a, 0, sizeof(a));
   a.y_true = y_true; a.y_pred = y_pred; a.B = B; a.P = P; a.C = C;
@@ -600,41 +641,26 @@ int fill_args(ssdk_ctx* ctx, LossArgs& a, const float* y_true, const float* y_pr
   a.hist1 = cur; a.hist2 = cur + (kCoarse + kFine);
   a.hist_next = parity ? hA : hB;
   a.ticket = reinterpret_cast<int*>(ws + L.ticket);
-  const int W = C + 12;
-  // cp.async.bulk needs 16-byte aligned tile starts: image stride P*W*4 and tile stride 128*W*4 (always a multiple of 16)
-  a.bulk_ok = (((size_t)P * W) % 4 == 0) && ((reinterpret_cast<uintptr_t>(y_true) & 15) == 0) && ((reinterpret_cast<uintptr_t>(y_pred) & 15) == 0) ? 1 : 0;
-  a.stages = 2;
-  if (loss_smem_bytes(W, 2, grad) > 100 * 1024) a.stages = 1;
-  plan.smem = loss_smem_bytes(W, a.stages, grad);
-  SSDK_REQUIRE(plan.smem <= 227 * 1024, "ssd_loss: %d classes need %zu bytes of shared memory per CTA", C, plan.smem);
-  static size_t attr[2] = {0, 0};
-  if (plan.smem > 48 * 1024) {
-    if (plan.smem > attr[0]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[0] = plan.smem; }
-    if (plan.smem > attr[1]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_phase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[1] = plan.smem; }
-  }
-  int per_sm = 0;
-  if (cooperative) SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_kernel, kRows, plan.smem));
-  else SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_phase_kernel, kRows, plan.smem));
-  SSDK_REQUIRE(per_sm > 0, "ssd_loss: the kernel does not fit on an SM (%zu bytes of shared memory)", plan.smem);
-  if (per_sm > 4) per_sm = 4;
-  plan.grid = std::max(1, std::min(a.n_tiles, per_sm * ctx->sm_count));
+  a.bulk_ok = plan.bulk_ok; a.stages = plan.stages;
   return SSDK_OK;
 }
 
-// context-owned workspace: zeroed when (re)allocated; the histogram parity flips on every call
+long long ws_key(int B, int P) { return (long long)B << 32 | (unsigned)P; }
+
+// context-owned workspace: zeroed when (re)allocated; the caller flips the histogram parity once its launch is enqueued (a call
+// refused before the launch must not flip it: the set it would have cleared is the one the next call counts in)
 int own_ws(ssdk_ctx* ctx, int B, int P, unsigned char** ws, int* parity, cudaStream_t stream) {
   const WsLayout L = ws_layout(B, P);
   const size_t before = ctx->ws[2].bytes;
   int rc = ctx->ws[2].ensure(L.total);
   if (rc) return rc;
-  if (ctx->ws[2].bytes != before || ctx->loss_ws_shape != ((long long)B << 32 | (unsigned)P)) {
+  if (ctx->ws[2].bytes != before || ctx->loss_ws_shape != ws_key(B, P)) {
     SSDK_CHECK_CUDA(cudaMemsetAsync(ctx->ws[2].ptr, 0, ctx->ws[2].bytes, stream));   // layout moved: start from clean histograms
-    ctx->loss_ws_shape = ((long long)B << 32 | (unsigned)P);
+    ctx->loss_ws_shape = ws_key(B, P);
     ctx->loss_parity = 0;
   }
   *ws = reinterpret_cast<unsigned char*>(ctx->ws[2].ptr);
   *parity = ctx->loss_parity;
-  ctx->loss_parity ^= 1;
   return SSDK_OK;
 }
 
@@ -664,6 +690,7 @@ int loss_run(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int
     a.dbg_times = d_times;
   }
   rc = launch_fused(ctx, a, plan, stream);
+  if (rc == SSDK_OK) ctx->loss_parity ^= 1;                           // this launch clears the other set for the next call
   if (rc == SSDK_OK && a.dbg_times) {
     unsigned long long h[8] = {0};
     SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));
@@ -705,6 +732,35 @@ extern "C" int ssdk_ssd_loss_ws_layout(int B, int P, ssdk_loss_ws_layout* out) {
   out->hist1_offset = (long long)L.histA; out->hist_n = kCoarse + kFine;
   out->hist2_offset = (long long)(L.histA + (size_t)(kCoarse + kFine) * 4);
   out->ties_offset = (long long)(L.ties + (size_t)B * ((P + kRows - 1) / kRows) * 4);
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_ssd_loss_plan(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C, int want_grad,
+                                  int cooperative, ssdk_loss_plan* out) {
+  SSDK_REQUIRE(out != nullptr, "ssdk_ssd_loss_plan: out is NULL");
+  int rc = check_args(ctx, y_true, y_pred, B, P, C);
+  if (rc) return rc;
+  LossPlan plan;
+  rc = plan_launch(ctx, y_true, y_pred, B, P, C, want_grad != 0, cooperative != 0, plan);
+  if (rc) return rc;
+  out->stages = plan.stages; out->bulk_ok = plan.bulk_ok; out->grid = plan.grid; out->smem_bytes = (long long)plan.smem;
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_ssd_loss_read_box_losses(ssdk_ctx* ctx, const void* ws_dev, int B, int P, float* cls_dev, float* negl_dev,
+                                             void* stream_) {
+  SSDK_REQUIRE(ctx && B > 0 && P > 0 && (cls_dev || negl_dev), "ssdk_ssd_loss_read_box_losses: bad argument");
+  const unsigned char* ws = reinterpret_cast<const unsigned char*>(ws_dev);
+  if (!ws) {
+    SSDK_REQUIRE(ctx->ws[2].ptr && ctx->loss_ws_shape == ws_key(B, P),
+                 "ssdk_ssd_loss_read_box_losses: the context's loss workspace does not hold a (%d, %d) batch", B, P);
+    ws = reinterpret_cast<const unsigned char*>(ctx->ws[2].ptr);
+  }
+  const WsLayout L = ws_layout(B, P);
+  const size_t bytes = (size_t)B * P * 4;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (cls_dev) SSDK_CHECK_CUDA(cudaMemcpyAsync(cls_dev, ws + L.cls, bytes, cudaMemcpyDeviceToDevice, stream));
+  if (negl_dev) SSDK_CHECK_CUDA(cudaMemcpyAsync(negl_dev, ws + L.negl, bytes, cudaMemcpyDeviceToDevice, stream));
   return SSDK_OK;
 }
 

@@ -686,3 +686,242 @@ def test_train_step_case_tables_reach_every_variant():
     assert ts.bn_grid(1, 10, 10, 136) == (17, 2)
     # preprocessing: mean only, mean + std, and the BGR swap
     assert [(c['stddev'] is not None, c['swap'] is not None) for c in ts.PRE_CASES] == [(False, False), (True, False), (True, True)]
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the SSD loss (section 11 of oracle/opexact.py)
+# ------------------------------------------------------------------------------------------------------------------------------
+def _loss_kernel_f32(yt, yp, ratio, n_neg_min, alpha, up, log_ulp=0, global_B=None):
+    """float32 emulation of ssd_loss_kernel's arithmetic -> (cls, negl, loss, stats, grad); the selection is the exact one."""
+    import test_gpu_loss_kernel as tl
+    F, D = np.float32, np.float64
+    cls, negl, l = tl.box_losses_f32(yt, yp, log_ulp)
+    B, P, W = yt.shape
+    C = W - 12
+    gB = B if global_B is None else global_B
+    pmax = yt[..., 1:C].max(-1)
+    n_pos_f = F(np.sum(pmax, dtype=D))
+    mask, stats = opexact.loss_select(negl, int(n_pos_f), ratio, n_neg_min)
+    inv = F(1) / max(F(1), n_pos_f)
+    pc = (cls * pmax).astype(F).astype(D).sum(-1)
+    loc = (l * pmax).astype(F).astype(D).sum(-1)
+    ng = (cls.astype(D) * mask).sum(-1)
+    loss = ((pc + ng + float(F(alpha)) * loc) * float(inv) * gB).astype(F)
+    upf = np.full(B, F(1) / F(gB), F) if up is None else np.asarray(up, F)
+    scale = ((upf * F(gB)).astype(F) * inv).astype(F)[:, None]
+    w_cls = ((pmax + mask.astype(F)).astype(F) * scale).astype(F)
+    w_loc = ((pmax * scale).astype(F) * F(alpha)).astype(F)
+    tv, q = yt[..., :C], yp[..., :C]
+    live = (tv != 0) & (q >= F(1e-15))
+    g = np.zeros_like(yt)
+    g[..., :C] = np.where(live, ((-tv / np.where(live, q, F(1))).astype(F) * w_cls[..., None]).astype(F), F(0))
+    d = (yp[..., C:C + 4] - yt[..., C:C + 4]).astype(F)
+    g[..., C:C + 4] = (np.where(np.abs(d) < 1, d, np.sign(d)).astype(F) * w_loc[..., None]).astype(F)
+    return cls, negl, loss, stats, g
+
+
+def _fails(out, rp, bnd):
+    _, _, loss, stats, g = out
+    return stats != rp['stats'] or opexact.loss_ratio(loss, rp['loss'], bnd['loss']) > 1 or opexact.loss_ratio(g, rp['grad'], bnd['grad']) > 1
+
+
+LOSS_SCENARIOS = {   # (case, perturbations every bound must reject, global_B, local_B)
+    'ties_zeros_weights': (dict(B=4, P=300, C=6, seed=70, pos=0.06, neutral=0.1, levels=(0.5, 0.25), over1=0.1, p0_one=0.05,
+                                alpha=0.5, upstream=(0.5, 0.0, -1.25, 2.0), n_neg_min=0, ratio=3),
+                           ('drop_last', 'add_next', 'per_image', 'no_alpha', 'loc_by_yt0', 'no_upstream'), None, None),
+    'zero_bin': (dict(B=3, P=200, C=6, seed=71, pos=0.05, neutral=0.1, over1=0.15, p0_one=0.1, n_neg_min=10 ** 6, ratio=3),
+                 ('drop_last', 'add_next', 'signed_zero', 'tie_reverse'), None, None),
+    'partial_ties': (dict(B=3, P=300, C=5, seed=72, pos=0.0, levels=(0.5, 0.25, 0.125), cut=(1, 77), ratio=3),
+                     ('drop_last', 'add_next', 'tie_reverse', 'per_image'), None, None),
+    'no_positives': (dict(B=2, P=200, C=4, seed=73, pos=0.0, neutral=0.2, n_neg_min=10 ** 6, ratio=3),
+                     ('drop_last', 'no_max1', 'k_no_cap'), None, None),
+    'rank_of_four': (dict(B=2, P=200, C=4, seed=74, pos=0.05, ratio=3), ('drop_last', 'add_next', 'local_B'), 8, 2),
+}
+
+
+def _scenario(name):
+    import test_gpu_loss_kernel as tl
+    d, perts, gB, lB = LOSS_SCENARIOS[name]
+    d = dict(d)
+    kw = {k: d.pop(k) for k in ('alpha', 'upstream', 'n_neg_min', 'ratio') if k in d}
+    c = tl.case(name, d.pop('B'), d.pop('P'), d.pop('C'), d.pop('seed'), **kw, **d)
+    yt, yp, up, m = tl.make_case(c)
+    return c, yt, yp, up, m, perts, gB, lB
+
+
+@pytest.mark.parametrize('name', sorted(n for n, v in LOSS_SCENARIOS.items() if v[2] is None))   # the oracle has no global batch
+def test_loss_ref_reproduces_the_float32_oracle(name):
+    from oracle.loss import ssd_loss, ssd_loss_grad
+    c, yt, yp, up, m, _, _, _ = _scenario(name)
+    ref_l, parts = ssd_loss(yt, yp, c['ratio'], m, c['alpha'], return_parts=True)
+    cls = parts['cls']
+    negl = (cls * yt[..., 0]).astype(np.float32)
+    ref, bnd, _ = opexact.loss_ref(yt, yp, cls, negl, c['ratio'], m, c['alpha'], up)
+    assert np.array_equal(ref['mask'], parts['mask'].astype(bool))
+    assert ref['stats'][0] == parts['n_positive'] and ref['stats'][2] == parts['k']
+    assert opexact.loss_ratio(ref_l, ref['loss'], bnd['loss']) <= 1.0
+    g = ssd_loss_grad(yt, yp, c['ratio'], m, c['alpha'], upstream=up)
+    assert opexact.loss_ratio(g, ref['grad'], bnd['grad']) <= 1.0
+    assert opexact.loss_ratio(parts['cls'], ref['cls'], bnd['cls']) <= 1.0
+
+
+def test_loss_ref_matches_a_literal_loop():
+    import math
+    c, yt, yp, up, m, _, _, _ = _scenario('ties_zeros_weights')
+    yt, yp = yt[:, :60], yp[:, :60]
+    B, P, W = yt.shape
+    C = W - 12
+    cls32, negl, _ = __import__('test_gpu_loss_kernel').box_losses_f32(yt, yp)
+    ratio, alpha = c['ratio'], float(np.float32(c['alpha']))
+    ref, _, _ = opexact.loss_ref(yt, yp, cls32, negl, ratio, 2, c['alpha'], up)
+    pm = [[max(float(v) for v in yt[b, p, 1:C]) for p in range(P)] for b in range(B)]
+    n_pos = int(np.float32(sum(map(sum, pm))))
+    vals = [float(v) for v in negl.reshape(-1)]
+    nnz = sum(v != 0 for v in vals)
+    k = min(max(ratio * n_pos, 2), nnz)
+    order = sorted(range(len(vals)), key=lambda i: (-vals[i], i))            # Python floats: -0.0 == 0.0
+    take = set(order[:k])
+    inv = float(np.float32(1) / np.float32(max(1, n_pos)))
+    for b in range(B):
+        tot = 0.0
+        for p in range(P):
+            i = b * P + p
+            cl = -sum(float(yt[b, p, c_]) * math.log(max(float(yp[b, p, c_]), float(np.float32(1e-15)))) for c_ in range(C) if yt[b, p, c_] != 0)
+            assert abs(ref['cls'][b, p] - cl) <= 1e-12 * (1 + abs(cl))
+            lc = 0.0
+            for j in range(4):
+                dd = float(yt[b, p, C + j]) - float(yp[b, p, C + j])
+                lc += 0.5 * dd * dd if abs(dd) < 1 else abs(dd) - 0.5
+            tot += float(cls32[b, p]) * pm[b][p] + (float(cls32[b, p]) if i in take else 0.0) + alpha * lc * pm[b][p]
+            assert ref['mask'][b, p] == (i in take)
+            sc = float(up[b]) * B * inv
+            for c_ in range(C):
+                q, tv = float(yp[b, p, c_]), float(yt[b, p, c_])
+                want = -tv / q * (pm[b][p] + (i in take)) * sc if tv != 0 and q >= float(np.float32(1e-15)) else 0.0
+                assert abs(ref['grad'][b, p, c_] - want) <= 1e-13 * abs(want)
+            for j in range(4):
+                dd = float(yp[b, p, C + j]) - float(yt[b, p, C + j])
+                want = max(-1.0, min(1.0, dd)) * pm[b][p] * sc * alpha
+                assert abs(ref['grad'][b, p, C + j] - want) <= 1e-13 * abs(want)
+        assert abs(ref['loss'][b] - tot * inv * B) <= 1e-12 * abs(tot * inv * B)
+
+
+@pytest.mark.parametrize('log_ulp', [0, 1, -1])
+@pytest.mark.parametrize('name', sorted(LOSS_SCENARIOS))
+def test_loss_bounds_accept_the_float32_kernel_and_reject_perturbations(name, log_ulp):
+    c, yt, yp, up, m, perts, gB, lB = _scenario(name)
+    out = _loss_kernel_f32(yt, yp, c['ratio'], m, c['alpha'], up, log_ulp, gB)
+    cls, negl = out[0], out[1]
+    ref, bnd, pv = opexact.loss_ref(yt, yp, cls, negl, c['ratio'], m, c['alpha'], up, global_B=gB, local_B=lB, perturb=perts)
+    ref_n = opexact.loss_ref(yt, yp, cls, negl, c['ratio'], m, c['alpha'], up, global_B=gB)[0]
+    assert out[3] == ref['stats'] == ref_n['stats']
+    assert opexact.loss_ratio(cls, ref['cls'], bnd['cls']) <= 1.0
+    assert opexact.loss_ratio(out[2], ref['loss'], bnd['loss']) <= 1.0
+    assert opexact.loss_ratio(out[4], ref['grad'], bnd['grad']) <= 1.0
+    for p, rp in pv.items():
+        assert _fails(out, rp, bnd), (name, p)
+    if log_ulp:
+        assert not np.array_equal(cls, _loss_kernel_f32(yt, yp, c['ratio'], m, c['alpha'], up, 0, gB)[0])
+
+
+def test_loss_okey_orders_floats_and_merges_signed_zeros():
+    v = np.array([-np.inf, -3.0, -1e-30, -0.0, 0.0, 1e-45, 1e-30, 2.0 ** -16, 1.0, np.inf], np.float32)
+    k = opexact.okey(v).astype(np.int64)
+    assert np.all(np.diff(k[:3]) > 0) and k[3] == k[4] == 0x80000000 and np.all(np.diff(k[4:]) > 0) and k[2] < k[3]
+    assert opexact.okey(np.float32(1.0)) >> 16 == 0xbf80 and opexact.okey(np.float32(2.0 ** -16)) >> 16 == 0xb780
+
+
+def _collided_bins(negl, P):
+    """The fine bins of non-zero losses that share a cache slot (bin & 2047) with another fine bin in the same tile: one of
+    them takes the slot, the others count through the global-atomic fallback."""
+    out = set()
+    for b in range(negl.shape[0]):
+        for t0 in range(0, P, 128):
+            v = negl[b, t0:t0 + 128]
+            slots = {}
+            for x in np.unique(opexact.okey(v[v != 0]).astype(np.int64) >> 16):
+                slots.setdefault(x & 2047, set()).add(int(x))
+            out |= set().union(*[s for s in slots.values() if len(s) > 1])
+    return out
+
+
+def test_loss_case_table_reaches_every_path():
+    import test_gpu_loss_kernel as tl
+    assert (tl.largest_c(True), tl.largest_c(False)) == (tl.C_MAX_GRAD, tl.C_MAX_FWD) == (137, 188)
+    # the smem arithmetic of plan_launch: 1536 W + 128 bytes with the gradient, 1024 W + 24704 without, one stage from C = 26
+    assert tl.plan_of(128, 137, True) == (1, 1) and tl.plan_of(128, 138, True) is None and tl.plan_of(128, 188, False) == (1, 1)
+    assert tl.plan_of(128, 25, True)[0] == 2 and tl.plan_of(128, 26, True)[0] == 1 and tl.plan_of(128, 26, False)[0] == 1
+    seen = dict(stages=set(), bulk_odd=False, bulk_ptr=False, bulk=False, ragged=False, partial=False, collision=False,
+                ordered=False, unordered=False, zero_T=False, none=False, k_nnz=False, pos_at_zero=False, clamp=False,
+                cut_not_first=False, cut_mid_warp=False, cut_tile_edge=False, weights=False, grad_store_plain=False)
+    perts, t_collided = set(), set()
+    names = [c['name'] for c in tl.LOSS_CASES]
+    assert len(set(names)) == len(names)
+    for c in tl.LOSS_CASES:
+        B, P, C = c['B'], c['P'], c['C']
+        grad = 'bwd' in c['modes']
+        stages, bulk = tl.plan_of(P, C, grad, aligned=not c['offset'])
+        seen['stages'].add(stages)
+        seen['bulk'] |= bulk == 1
+        seen['bulk_odd'] |= bulk == 0 and P * (C + 12) % 4 != 0 and not c['offset']
+        seen['bulk_ptr'] |= bulk == 0 and P * (C + 12) % 4 == 0 and c['offset']
+        seen['grad_store_plain'] |= bulk == 1 and c['grad_offset'] and grad
+        seen['ragged'] |= P > 128 and P % 128 != 0
+        seen['partial'] |= P < 128
+        yt, yp, up, m = tl.make_case(c)
+        cls, negl, _ = tl.box_losses_f32(yt, yp)
+        pmax = yt[..., 1:C].max(-1)
+        mask, st = opexact.loss_select(negl, int(np.float32(pmax.sum())), c['ratio'], m)
+        hit = _collided_bins(negl, P)
+        seen['collision'] |= bool(hit)
+        seen['none'] |= st[2] == 0
+        seen['k_nnz'] |= 0 < st[2] == st[1]
+        seen['clamp'] |= bool(np.any((yt[..., :C] != 0) & (yp[..., :C] < np.float32(1e-15))))
+        seen['weights'] |= c['upstream'] is not None and 0.0 in c['upstream'] and min(c['upstream']) < 0 and c['alpha'] != 1
+        if st[2] > 0:
+            flat = negl.reshape(-1)
+            T = opexact.okey(flat[opexact._order(flat)[st[2] - 1]])[0]
+            ties = np.flatnonzero(opexact.okey(flat) == T)
+            seen['ordered'] |= st[3] < ties.size
+            seen['unordered'] |= st[3] == ties.size > 1
+            fine = opexact.okey(flat[flat != 0]).astype(np.int64) >> 16
+            tf = int(T) >> 16
+            if tf in hit and np.any((fine < tf) & (fine >> 5 == tf >> 5)):   # a populated fine bin below it, same coarse bin
+                t_collided.add(tf)
+            if T == 0x80000000:
+                sz = np.signbit(flat) & (flat == 0)
+                seen['zero_T'] |= bool(np.any(sz) and np.any(~np.signbit(flat) & (flat == 0)) and st[3] < ties.size)
+                seen['pos_at_zero'] |= bool(np.any(mask & (pmax > 0)))
+            if 'cut' in c['gen'] and st[3] < ties.size:
+                last = ties[st[3] - 1]
+                b, row = divmod(int(last), P)
+                seen['cut_not_first'] |= b > 0
+                seen['cut_mid_warp'] |= row % 32 not in (0, 31)
+                seen['cut_tile_edge'] |= row % 128 == 127
+        perts |= set(c['perturb'])
+    assert seen.pop('stages') == {1, 2}
+    # the threshold lands in both fine bins of a colliding pair, each above a populated fine bin of its coarse bin, so a lost
+    # fallback count moves it whichever bin took the slot
+    assert {0xbf81, 0xb781} <= t_collided, [hex(x) for x in t_collided]
+    # the phase-wise test compares each rank's histograms with np.bincount on data whose first tile collides, with the
+    # threshold in a collided bin
+    ph = []
+    for c in tl.PHASE_CASES:
+        yt, yp, _, m = tl.make_case(c)
+        negl = tl.box_losses_f32(yt, yp)[1]
+        pmax = yt[..., 1:c['C']].max(-1)
+        _, st = opexact.loss_select(negl, int(np.float32(pmax.sum())), c['ratio'], m)
+        flat = negl.reshape(-1)
+        T = int(opexact.okey(flat[opexact._order(flat)[st[2] - 1]])[0]) if st[2] else None
+        hit = _collided_bins(negl[: c['B'] // 4], c['P'])                  # rank 0 of 4
+        fine = opexact.okey(flat[flat != 0]).astype(np.int64) >> 16
+        ph.append(bool(hit) and T is not None and (T >> 16) in hit and bool(np.any((fine < T >> 16) & (fine >> 5 == T >> 21))))
+    assert any(ph), ph
+    assert all(seen.values()), {k: v for k, v in seen.items() if not v}
+    assert {1, 127, 128, 129} <= {c['P'] for c in tl.LOSS_CASES} and any(c['B'] == 1 for c in tl.LOSS_CASES)
+    assert {21, 81, 25, 26, tl.C_MAX_GRAD, tl.C_MAX_FWD} <= {c['C'] for c in tl.LOSS_CASES}
+    assert any(c['B'] == 32 and c['P'] == 8732 and c['C'] == 21 for c in tl.LOSS_CASES)
+    assert any(c['n_neg_min'] > 10 ** 5 and c['gen'].get('pos', 1) > 0 for c in tl.LOSS_CASES)
+    assert {c['n_neg_min'] > 0 for c in tl.LOSS_CASES if c['gen'].get('pos') == 0.0 and 'cut' not in c['gen']} == {False, True}
+    # every perturbation is rejected by some GPU case ('local_B' by the phase-wise test with more than one rank)
+    assert perts | {'local_B'} == set(opexact.LOSS_PERTURBATIONS)
