@@ -50,11 +50,19 @@ def greedy_nms(y_pred_decoded, iou_threshold=0.45, coords='corners', border_pixe
     return [_nms_rows(item, 1, 2, iou_threshold, coords, border_pixels) for item in y_pred_decoded]
 
 
-def _decode_boxes_inplace(dst, y_pred, input_coords, cols):
+def exp_cr(x):
+    """float32 ``exp`` rounded once from float64 -- what the CUDA decoder computes (``exp_cr`` in csrc/decode.cu).  NumPy's own
+    float32 ``np.exp`` may differ from it by an ulp or two; pass this as ``exp=`` to hold the kernels to the bit."""
+    x = np.asarray(x)
+    with np.errstate(over='ignore'):
+        return np.exp(x.astype(np.float64)).astype(x.dtype)
+
+
+def _decode_boxes_inplace(dst, y_pred, input_coords, cols, exp=np.exp):
     """Shared arithmetic of :174-190 / :296-312; ``cols`` = the four destination columns."""
     c0, c1, c2, c3 = cols
     if input_coords == 'centroids':
-        dst[:, :, [c2, c3]] = np.exp(dst[:, :, [c2, c3]] * y_pred[:, :, [-2, -1]])
+        dst[:, :, [c2, c3]] = exp(dst[:, :, [c2, c3]] * y_pred[:, :, [-2, -1]])
         dst[:, :, [c2, c3]] *= y_pred[:, :, [-6, -5]]
         dst[:, :, [c0, c1]] *= y_pred[:, :, [-4, -3]] * y_pred[:, :, [-6, -5]]
         dst[:, :, [c0, c1]] += y_pred[:, :, [-8, -7]]
@@ -76,8 +84,9 @@ def _decode_boxes_inplace(dst, y_pred, input_coords, cols):
 
 
 def decode_detections(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=200, input_coords='centroids',
-                      normalize_coords=True, img_height=None, img_width=None, border_pixels='half'):
-    """ssd_output_decoder.py:111-226."""
+                      normalize_coords=True, img_height=None, img_width=None, border_pixels='half', exp=np.exp,
+                      return_index=False):
+    """ssd_output_decoder.py:111-226.  ``return_index`` also returns, per image, the prior index of every row."""
     if normalize_coords and (img_height is None or img_width is None):
         raise ValueError("If relative box coordinates are supposed to be converted to absolute coordinates, the "
                          "decoder needs the image size in order to decode the predictions, but `img_height == {}` "
@@ -85,38 +94,43 @@ def decode_detections(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=
     y_pred = np.asarray(y_pred)
     raw = np.copy(y_pred[:, :, :-8])                                          # :172
     n_cols = raw.shape[2]
-    raw = _decode_boxes_inplace(raw, y_pred, input_coords, (n_cols - 4, n_cols - 3, n_cols - 2, n_cols - 1))
+    raw = _decode_boxes_inplace(raw, y_pred, input_coords, (n_cols - 4, n_cols - 3, n_cols - 2, n_cols - 1), exp)
     if normalize_coords:                                                      # :196-198
         raw[:, :, [-4, -2]] *= img_width
         raw[:, :, [-3, -1]] *= img_height
     n_classes = raw.shape[-1] - 4
-    out = []
+    out, out_idx = [], []
     for item in raw:                                                          # :205
-        per_class = []
+        per_class, per_idx = [], []
+        prior = np.arange(item.shape[0]).astype(item.dtype)[:, None]          # carried along in front of the score
         for cid in range(1, n_classes):                                       # :207
-            rows = item[:, [cid, -4, -3, -2, -1]]
-            rows = rows[rows[:, 0] > confidence_thresh]                       # :209 (strict)
+            rows = np.concatenate([prior, item[:, [cid, -4, -3, -2, -1]]], axis=1)
+            rows = rows[rows[:, 1] > confidence_thresh]                       # :209 (strict)
             if rows.shape[0] > 0:
-                kept = _nms_rows(rows, 0, 1, iou_threshold, 'corners', border_pixels)
+                kept = _nms_rows(rows, 1, 2, iou_threshold, 'corners', border_pixels)
                 block = np.zeros((kept.shape[0], 6))
                 block[:, 0] = cid
-                block[:, 1:] = kept
+                block[:, 1:] = kept[:, 1:]
                 per_class.append(block)
+                per_idx.append(kept[:, 0].astype(np.int64))
         if per_class:
             pred = np.concatenate(per_class, axis=0)
+            pidx = np.concatenate(per_idx)
             if top_k != 'all' and pred.shape[0] > top_k:                      # :219-221 (unordered)
                 sel = np.argpartition(pred[:, 1], kth=pred.shape[0] - top_k, axis=0)[pred.shape[0] - top_k:]
-                pred = pred[sel]
+                pred, pidx = pred[sel], pidx[sel]
         else:
             pred = np.array(per_class)                                        # :223 -> shape (0,)
+            pidx = np.zeros((0,), np.int64)
         out.append(pred)
-    return out
+        out_idx.append(pidx)
+    return (out, out_idx) if return_index else out
 
 
 def decode_detections_fast(y_pred, confidence_thresh=0.5, iou_threshold=0.45, top_k='all',
                            input_coords='centroids', normalize_coords=True, img_height=None, img_width=None,
-                           border_pixels='half'):
-    """ssd_output_decoder.py:228-333."""
+                           border_pixels='half', exp=np.exp, return_index=False):
+    """ssd_output_decoder.py:228-333.  ``return_index`` also returns, per image, the prior index of every row."""
     if normalize_coords and (img_height is None or img_width is None):
         raise ValueError("If relative box coordinates are supposed to be converted to absolute coordinates, the "
                          "decoder needs the image size in order to decode the predictions, but `img_height == {}` "
@@ -125,21 +139,32 @@ def decode_detections_fast(y_pred, confidence_thresh=0.5, iou_threshold=0.45, to
     conv = np.copy(y_pred[:, :, -14:-8])                                      # :291
     conv[:, :, 0] = np.argmax(y_pred[:, :, :-12], axis=-1)                    # :292
     conv[:, :, 1] = np.amax(y_pred[:, :, :-12], axis=-1)                      # :293
-    conv = _decode_boxes_inplace(conv, y_pred, input_coords, (2, 3, 4, 5))
+    conv = _decode_boxes_inplace(conv, y_pred, input_coords, (2, 3, 4, 5), exp)
     if normalize_coords:                                                      # :317-319
         conv[:, :, [2, 4]] *= img_width
         conv[:, :, [3, 5]] *= img_height
-    out = []
+    out, out_idx = [], []
     for item in conv:
-        boxes = item[np.nonzero(item[:, 0])]                                  # :324
-        boxes = boxes[boxes[:, 1] >= confidence_thresh]                       # :325 (non-strict)
+        prior = np.arange(item.shape[0])
+        keep = np.nonzero(item[:, 0])[0]                                      # :324
+        boxes, prior = item[keep], prior[keep]
+        keep = boxes[:, 1] >= confidence_thresh                               # :325 (non-strict)
+        boxes, prior = boxes[keep], prior[keep]
         if iou_threshold:                                                     # :326
-            boxes = _nms_rows(boxes, 1, 2, iou_threshold, 'corners', border_pixels)
+            # the prior index rides in the class column, which the NMS does not read (the class comes back below)
+            rows = np.concatenate([prior.astype(boxes.dtype)[:, None], boxes[:, 1:]], axis=1)
+            kept = _nms_rows(rows, 1, 2, iou_threshold, 'corners', border_pixels)
+            if kept.size:
+                prior = kept[:, 0].astype(np.int64)
+                boxes = item[prior]
+            else:
+                boxes, prior = kept, prior[:0]
         if top_k != 'all' and boxes.shape[0] > top_k:                         # :328-330
             sel = np.argpartition(boxes[:, 1], kth=boxes.shape[0] - top_k, axis=0)[boxes.shape[0] - top_k:]
-            boxes = boxes[sel]
+            boxes, prior = boxes[sel], prior[sel]
         out.append(boxes)
-    return out
+        out_idx.append(prior)
+    return (out, out_idx) if return_index else out
 
 
 # --------------------------------------------------------------------------------------
@@ -246,14 +271,14 @@ def tf_nms_c(boxes, scores, max_output_size, iou_threshold):
     return [int(v) for v in out[:k]]
 
 
-def _layer_boxes(y_pred, normalize_coords, img_height, img_width):
+def _layer_boxes(y_pred, normalize_coords, img_height, img_width, exp=np.exp):
     """keras_layer_DecodeDetections.py:124-146 in float32."""
     f = np.float32
     y = np.asarray(y_pred, dtype=f)
     cx = (y[..., -12] * y[..., -4] * y[..., -6] + y[..., -8]).astype(f)
     cy = (y[..., -11] * y[..., -3] * y[..., -5] + y[..., -7]).astype(f)
-    w = (np.exp(y[..., -10] * y[..., -2]).astype(f) * y[..., -6]).astype(f)
-    h = (np.exp(y[..., -9] * y[..., -1]).astype(f) * y[..., -5]).astype(f)
+    w = (exp(y[..., -10] * y[..., -2]).astype(f) * y[..., -6]).astype(f)
+    h = (exp(y[..., -9] * y[..., -1]).astype(f) * y[..., -5]).astype(f)
     xmin = (cx - f(0.5) * w).astype(f); ymin = (cy - f(0.5) * h).astype(f)
     xmax = (cx + f(0.5) * w).astype(f); ymax = (cy + f(0.5) * h).astype(f)
     if normalize_coords:
@@ -272,13 +297,13 @@ def _topk_pad(rows, top_k):
 
 
 def decode_layer(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=200, nms_max_output_size=400,
-                 normalize_coords=True, img_height=None, img_width=None, return_indices=False, nms=None):
+                 normalize_coords=True, img_height=None, img_width=None, return_indices=False, nms=None, exp=np.exp):
     """DecodeDetections.call, keras_layer_DecodeDetections.py:109-265 -> (B, top_k, 6) float32.
 
     ``return_indices`` also returns, per image, the prior index of every output row (-1 for padding)."""
     f = np.float32
     y = np.asarray(y_pred, dtype=f)
-    boxes = _layer_boxes(y, normalize_coords, img_height, img_width)
+    boxes = _layer_boxes(y, normalize_coords, img_height, img_width, exp)
     B, P = y.shape[0], y.shape[1]
     n_classes = y.shape[2] - 12
     out = np.zeros((B, top_k, 6), f)
@@ -308,11 +333,11 @@ def decode_layer(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=200, 
 
 
 def decode_layer_fast(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=200, nms_max_output_size=400,
-                      normalize_coords=True, img_height=None, img_width=None, return_indices=False):
+                      normalize_coords=True, img_height=None, img_width=None, return_indices=False, nms=None, exp=np.exp):
     """DecodeDetectionsFast.call, keras_layer_DecodeDetectionsFast.py:111-248 -> (B, top_k, 6) float32."""
     f = np.float32
     y = np.asarray(y_pred, dtype=f)
-    boxes = _layer_boxes(y, normalize_coords, img_height, img_width)
+    boxes = _layer_boxes(y, normalize_coords, img_height, img_width, exp)
     cls = np.argmax(y[..., :-12], axis=-1)                                     # :126 (first index on ties)
     conf = np.max(y[..., :-12], axis=-1)                                       # :128
     B = y.shape[0]
@@ -322,7 +347,7 @@ def decode_layer_fast(y_pred, confidence_thresh=0.01, iou_threshold=0.45, top_k=
         m = np.nonzero((cls[b] != 0) & (conf[b] > f(confidence_thresh)))[0]    # :174,:180 (strict)
         rows = np.zeros((0, 6), f); ridx = np.zeros((0,), np.int64)
         if m.size:
-            sel = tf_nms_fast(boxes[b, m], conf[b, m], nms_max_output_size, iou_threshold)
+            sel = (nms or tf_nms_fast)(boxes[b, m], conf[b, m], nms_max_output_size, iou_threshold)
             rows = np.zeros((len(sel), 6), f)
             rows[:, 0] = cls[b, m][sel]; rows[:, 1] = conf[b, m][sel]; rows[:, 2:] = boxes[b, m][sel]
             ridx = m[sel]

@@ -277,6 +277,7 @@ struct NmsParams {
   int strict, use64;
   float thr32; double thr64;
   double iou_thr; int d;
+  int no_nms;              // 1: nothing suppresses anything (decode_detections_fast with iou_threshold 0 / None)
   int band_cap;            // candidates per band (<= kNmsCap)
   int max_bands;           // > 0: stop after this many bands even if candidates remain (stage 1)
   uint32_t* cut_key;       // [B*S] out (stage 1): order key of the last candidate looked at when the scan was cut short, else 0
@@ -303,8 +304,37 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(NmsParams prm) {
   const T* boxes = reinterpret_cast<const T*>(prm.boxes) + (size_t)b * prm.n * 4;
   int* kept = prm.kept_idx + (size_t)seg * prm.kmax;
   const T thr = (T)prm.iou_thr;
+  const bool nms_on = !prm.no_nms;
   const T dd = (T)prm.d;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+  if (!nms_on) {
+    // decode_detections_fast without NMS keeps its rows in prior order (:324-326).  When every passing candidate fits under
+    // the cap, the kept list is exactly that: an ordered compaction, no scan.  Otherwise the scan below keeps the cap best.
+    int c = 0;
+    for (int i = threadIdx.x; i < sv.n; i += NT) c += seg_pass(sv, i, sv.scores[i]) ? 1 : 0;
+    const int R = block_sum_int<NT>(c, s_w);
+    if (R <= prm.cap) {
+      int base = 0;
+      for (int i0 = 0; i0 < sv.n; i0 += NT) {
+        const int i = i0 + threadIdx.x;
+        const bool take = i < sv.n && seg_pass(sv, i, sv.scores[i]);
+        const unsigned bal = __ballot_sync(0xffffffffu, take);
+        if (lane == 0) s_w[warp] = __popc(bal);
+        __syncthreads();
+        int wbase = 0, total = 0;
+        for (int w = 0; w < NW; ++w) { const int n_w = s_w[w]; if (w < warp) wbase += n_w; total += n_w; }
+        if (take) kept[base + wbase + __popc(bal & ((1u << lane) - 1))] = i;
+        base += total;
+        __syncthreads();
+      }
+      if (threadIdx.x == 0) {
+        prm.kept_cnt[seg] = R;
+        if (prm.cut_key) prm.cut_key[seg] = 0;
+      }
+      return;
+    }
+  }
 
   auto kept_box = [&](int t) {
     PBox<T> m;
@@ -340,7 +370,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(NmsParams prm) {
         for (int w = 0; w <= (j >> 5); ++w) {
           uint32_t bits = 0;
           const int i1 = min(j, w * 32 + 32);
-          for (int i = w * 32; i < i1; ++i) bits |= (suppressed<T, LAYER>(c, cb[i], thr) ? 1u : 0u) << (i & 31);
+          for (int i = w * 32; i < i1; ++i) bits |= ((nms_on && suppressed<T, LAYER>(c, cb[i], thr)) ? 1u : 0u) << (i & 31);
           msk[j * (kMaskN / 32) + w] = bits;
         }
       }
@@ -397,7 +427,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(NmsParams prm) {
         bool sup = false;
 #pragma unroll
         for (int u = 0; u < 4; ++u)
-          if (t + u < k_start) sup |= suppressed<T, LAYER>(bx, kept_box(t + u), thr);
+          if (t + u < k_start) sup |= nms_on && suppressed<T, LAYER>(bx, kept_box(t + u), thr);
         if (sup) alive = false;
       }
       __syncthreads();
@@ -406,7 +436,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(NmsParams prm) {
         if (warp == w) {
           const int k_cur = *((volatile int*)&s_K);
           for (int t = k_start; t < k_cur && alive; ++t)          // survivors added by earlier warps of this chunk
-            if (suppressed<T, LAYER>(bx, kept_box(t), thr)) alive = false;
+            if (nms_on && suppressed<T, LAYER>(bx, kept_box(t), thr)) alive = false;
           unsigned am = __ballot_sync(0xffffffffu, alive);
           int nk = 0, my_rank = -1;
           while (am) {
@@ -418,7 +448,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(NmsParams prm) {
             if (lane == i) my_rank = nk;
             ++nk;
             if (k_cur + nk >= prm.cap) break;                      // cap reached: later candidates are never looked at
-            if (alive && lane > i && suppressed<T, LAYER>(bx, m, thr)) alive = false;
+            if (alive && nms_on && lane > i && suppressed<T, LAYER>(bx, m, thr)) alive = false;
             am = __ballot_sync(0xffffffffu, alive && lane > i);
           }
           if (my_rank >= 0 && k_cur + my_rank < prm.cap) {
@@ -482,8 +512,9 @@ __global__ void __launch_bounds__(256) dec_prepare_kernel(PrepParams p) {
   if (p.mode == SSDK_DECODE_PER_CLASS) {
     for (int c = 1; c < C; ++c) p.scores[((size_t)b * (C - 1) + (c - 1)) * p.P + pi] = r[c];
   } else {
+    // np.argmax / np.amax: first index on ties, and the first NaN wins (its row then fails every threshold test)
     float best = r[0]; int bi = 0;
-    for (int c = 1; c < C; ++c) if (r[c] > best) { best = r[c]; bi = c; }   // first index on ties
+    for (int c = 1; c < C && best == best; ++c) if (!(r[c] <= best)) { best = r[c]; bi = c; }
     p.scores[(size_t)b * p.P + pi] = best;
     p.labels[(size_t)b * p.P + pi] = bi;
   }
@@ -660,7 +691,7 @@ int stage1_band(int S, int top_k) {
 }
 
 int run_nms_topk(ssdk_ctx* ctx, int B, int n, int S, int layer, int box_f64, int np_f32, const float* scores,
-                 const int* labels, const void* boxes, int strict, double conf_thr, double iou_thr, int d, int cap,
+                 const int* labels, const void* boxes, int strict, double conf_thr, double iou_thr, int d, int no_nms, int cap,
                  int top_k, int max_out, unsigned char* scratch, float* out, int* out_counts, int* out_index,
                  cudaStream_t stream) {
   // only top_k rows leave: no class needs more than top_k survivors (rows beyond the top_k-th of one class never reach
@@ -680,8 +711,9 @@ int run_nms_topk(ssdk_ctx* ctx, int B, int n, int S, int layer, int box_f64, int
   if (const char* e = getenv("SSDK_NMS_TWO_STAGE")) two_stage = two_stage && atoi(e) != 0;
   NmsParams np{};
   np.scores = scores; np.labels = labels; np.boxes = boxes; np.kept_idx = kept_idx; np.kept_cnt = kept_cnt;
-  np.n = n; np.S = S; np.kmax = kmax; np.cap = cap; np.strict = strict; np.use64 = layer ? 0 : 1;
-  np.thr32 = (float)conf_thr; np.thr64 = conf_thr; np.iou_thr = iou_thr; np.d = d;
+  np.n = n; np.S = S; np.kmax = kmax; np.cap = cap; np.strict = strict;
+  np.use64 = (layer || np_f32) ? 0 : 1;    // the NumPy API compares in the dtype of its score array: float32 in corners mode
+  np.thr32 = (float)conf_thr; np.thr64 = conf_thr; np.iou_thr = iou_thr; np.d = d; np.no_nms = no_nms;
   np.band_cap = two_stage ? band1 : kNmsCap; np.max_bands = two_stage ? 1 : 0; np.cut_key = two_stage ? cut_key : nullptr; np.redo = nullptr;
   auto nms = [&](const NmsParams& q) {
     if (layer) return launch_nms<float, true>(ctx, q, B, stream);
@@ -766,10 +798,10 @@ extern "C" int ssdk_decode(ssdk_ctx* ctx, const ssdk_decode_cfg* cfg, const floa
 
   int strict = 1;
   if (!layer && cfg->mode == SSDK_DECODE_FAST) strict = 0;      // decode_detections_fast uses >= (:325)
-  double iou_thr = cfg->iou_threshold;
-  if (!layer && cfg->mode == SSDK_DECODE_FAST && !(cfg->iou_threshold > 0.0)) iou_thr = INFINITY;   // "if iou_threshold:" (:326)
+  // "if iou_threshold:" (:326): without NMS every row that passes the threshold stays, NaN and infinite boxes included
+  const int no_nms = (!layer && cfg->mode == SSDK_DECODE_FAST && cfg->iou_threshold == 0.0) ? 1 : 0;
   return run_nms_topk(ctx, B, P, S, layer, box_f64, np_f32, scores, cfg->mode == SSDK_DECODE_FAST ? labels : nullptr, boxes,
-                      strict, cfg->confidence_thresh, iou_thr, cfg->border_d, cap, cfg->top_k, cfg->max_out, scratch,
+                      strict, cfg->confidence_thresh, cfg->iou_threshold, cfg->border_d, no_nms, cap, cfg->top_k, cfg->max_out, scratch,
                       out_dev, out_counts_dev, out_index_dev, stream);
 }
 
@@ -781,7 +813,7 @@ extern "C" int ssdk_nms(ssdk_ctx* ctx, const float* boxes_dev, const float* scor
   size_t total = nms_scratch_bytes(B, 1, nms_max_output);
   int rc = ctx->ws[1].ensure(total);
   if (rc) return rc;
-  return run_nms_topk(ctx, B, n, 1, 1, 0, 0, scores_dev, nullptr, boxes_dev, 1, confidence_thresh, iou_threshold, 0,
+  return run_nms_topk(ctx, B, n, 1, 1, 0, 0, scores_dev, nullptr, boxes_dev, 1, confidence_thresh, iou_threshold, 0, 0,
                       nms_max_output, top_k, top_k, reinterpret_cast<unsigned char*>(ctx->ws[1].ptr), out_dev,
                       out_counts_dev, out_index_dev, (cudaStream_t)stream_);
 }
