@@ -154,9 +154,22 @@ int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const double* boxes
  *   FILTER    flags bit0: drop degenerate boxes (xmax <= xmin or ymax <= ymin), bit1: drop boxes with area < a0
  *             (BoxFilter, object_detection_2d_image_boxes_validation_utils.py:155-165; also DataGenerator's
  *             degenerate_box_handling='remove')
+ *   TRANSLATE a0=dy_abs a1=dx_abs (integers, Translate's int(round(h*dy)) / int(round(w*dx))) a2=image height a3=image width;
+ *             boxes += dx_abs / dy_abs                                  (Translate.__call__, object_detection_2d_geometric_ops.py:276-317)
+ *   SCALE     a0=factor a1=image height a2=image width: both corners through M = getRotationMatrix2D((w/2, h/2), 0, factor)
+ *             as np.dot computes it, (m0*x + m1*y) + m2 with every step rounded, then np.round      (Scale.__call__, :487-532)
+ *   ROTATE    a0=angle (90, 180 or 270; other values leave the boxes alone) a1=image height a2=image width: Rotate's adjusted
+ *             matrix, the same corner arithmetic, then its ymin/ymax and xmin/xmax swaps             (Rotate.__call__, :681-737)
+ *   OVERLAP   BoxFilter's overlap test against an a2 x a3 (height x width) image, bounds (a0, a1] / [a0, a1]: flags bits 0-1
+ *             criterion 0 'center_point', 1 'area' (lower == 0 compares with >), 2 'iou' (the intersection ignores
+ *             border_pixels, as bounding_box_utils.iou does); bits 2-3 border_pixels 0 'half', 1 'include', 2 'exclude'
+ *             (object_detection_2d_image_boxes_validation_utils.py:186-230)
+ *   CLIP      a0=image height a1=image width: clip to [0, h-1] x [0, w-1] (the clip_boxes step of Translate / Scale / CropPad)
+ * Codes the kernel does not know are skipped.
  * ------------------------------------------------------------------------------------------ */
 typedef enum { SSDK_BOXOP_END = 0, SSDK_BOXOP_CROP_PAD = 1, SSDK_BOXOP_FLIP_H = 2, SSDK_BOXOP_FLIP_V = 3, SSDK_BOXOP_RESIZE = 4,
-               SSDK_BOXOP_FILTER = 5 } ssdk_box_op_kind;
+               SSDK_BOXOP_FILTER = 5, SSDK_BOXOP_TRANSLATE = 6, SSDK_BOXOP_SCALE = 7, SSDK_BOXOP_ROTATE = 8,
+               SSDK_BOXOP_OVERLAP = 9, SSDK_BOXOP_CLIP = 10 } ssdk_box_op_kind;
 typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
@@ -166,24 +179,33 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
                         const ssdk_box_op* ops_dev, int max_ops, float* gt_out_dev, int* offsets_out_dev, int* out_stats_dev,
                         void* stream);
 /* The image half of the same op lists: ConvertTo3Channels (object_detection_2d_photometric_ops.py:88-108; gray is replicated,
- * RGBA drops alpha, applied first), the image arithmetic of CropPad (:266-313) and Flip, and uint8 cv2.resize, into a float32
- * NHWC batch of [0,255] integers (what ssdk_model_forward takes).  The image fields live in flag bits the box kernel never reads:
+ * RGBA drops alpha, applied first), the image arithmetic of CropPad (:266-313) and Flip, uint8 cv2.resize, and uint8
+ * cv2.warpAffine (INTER_LINEAR, BORDER_CONSTANT) of Translate / Scale / Rotate, into a float32 NHWC batch of [0,255] integers
+ * (what ssdk_model_forward takes).  The image fields live in flag bits the box kernel never reads:
  *   CROP_PAD  flags bits 8-31: background R, G, B bytes (0 = black, as CropPad's default; SSDExpand uses 123,117,104)
  *   RESIZE    flags bits 8-15: cv2 interpolation code, INTER_NEAREST = 0 or INTER_LINEAR = 1 (an exact 2x linear downscale
  *             takes INTER_AREA's fast path, as cv2 does); any other code is an error
- *   FILTER    nothing to do for images
+ *   TRANSLATE flags bits 8-31: background; an integer shift, composed like a pad / crop
+ *   SCALE     flags bits 8-31: background; the bilinear warp, cv2's fixed-point scheme bit for bit
+ *   ROTATE    an exact signed axis permutation (cv2's fixed-point map is checked on the host to have fraction 0 everywhere),
+ *             black where the inverse map leaves the source
+ *   FILTER, OVERLAP, CLIP   nothing to do for images
  * src_dev: the B uint8 images packed back to back, image b at bytes src_offsets_host[b] .. src_offsets_host[b+1] (host, [B+1]),
  * of shape src_hwc_host[3b..3b+2] = h, w, c with c in {1, 3, 4}.  ops_host: [B*max_ops] on the HOST (a list ends at
  * SSDK_BOXOP_END or after max_ops entries).  out_dev: [B*out_h*out_w*3] float32.
  * Checked on the host before anything is enqueued (SSDK_ERR_INVALID, nothing written): sizes positive, B <= 65535, offsets
  * consistent with the shapes; each CROP_PAD integer with a positive size and overlapping its input (CropPad's own test, :270-271);
- * each flip's a0 equal to the canvas width / height at that point; at most one RESIZE, from the canvas size reached at that point,
- * and no crop / pad / flip after it; the final size out_h x out_w; a supported interpolation code; and all pads of one list that
- * reach past their input use one background colour (bands of different colours are not represented).
- * The crops, pads and flips before the resize are composed on the host into one integer map per image; one kernel launch
- * evaluates the whole list without an intermediate image.  The descriptors go to the device with one asynchronous copy from
- * pinned staging owned by the context (a ring of four buffers: the call waits only if the upload of the call four calls earlier
- * has not run yet); like the encoder, one context must not run this on two streams at the same time. */
+ * each flip's a0, and each TRANSLATE's, SCALE's and ROTATE's image height / width, equal to the canvas size at that point;
+ * TRANSLATE integer, ROTATE by 90 / 180 / 270, SCALE by a positive factor whose fixed-point coordinates fit cv2's int32 / int16
+ * ranges (canvas below 32767); at most one resampling step (RESIZE or SCALE); no crop / pad / flip / translate / rotate after
+ * a RESIZE (after a SCALE they are applied to its output); the final size out_h x out_w; a supported interpolation code; and one
+ * background colour per list: every pad or translate that brings in background, every SCALE, and a ROTATE whose map leaves
+ * the source (black) must agree (bands of different colours are not represented).
+ * The integer ops before the resampling step are composed on the host into one signed-permutation map per image, those after a
+ * SCALE into a second one; one kernel launch evaluates the whole list without an intermediate image.  The descriptors go to the
+ * device with one asynchronous copy from pinned staging owned by the context (a ring of four buffers: the call waits only if the
+ * upload of the call four calls earlier has not run yet); like the encoder, one context must not run this on two streams at the
+ * same time. */
 int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const long long* src_offsets_host, const int* src_hwc_host, int B,
                          const ssdk_box_op* ops_host, int max_ops, int out_h, int out_w, float* out_dev, void* stream);
 

@@ -51,6 +51,7 @@ class BoxOp(C.Structure):
 
 
 BOXOP_END, BOXOP_CROP_PAD, BOXOP_FLIP_H, BOXOP_FLIP_V, BOXOP_RESIZE, BOXOP_FILTER = range(6)
+BOXOP_TRANSLATE, BOXOP_SCALE, BOXOP_ROTATE, BOXOP_OVERLAP, BOXOP_CLIP = range(6, 11)
 INTER_NEAREST, INTER_LINEAR = 0, 1          # cv2's codes, in RESIZE's flag bits 8-15 (ssdk_assemble_images)
 
 

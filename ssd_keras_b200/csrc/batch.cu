@@ -13,12 +13,14 @@
 //   box_pack_kernel    one CTA per image: rows to their final place.
 // The image half of the same op lists (ssdk_assemble_images) is at the end of the file: ConvertTo3Channels
 // (object_detection_2d_photometric_ops.py:88-108), the image arithmetic of CropPad (:266-313) and Flip, and uint8 cv2.resize
-// (INTER_NEAREST / INTER_LINEAR) in one launch, restated in oracle/imageops.py.
+// (INTER_NEAREST / INTER_LINEAR) and uint8 cv2.warpAffine (Translate / Scale / Rotate, geometric_ops.py:233-737) in one launch,
+// restated in oracle/imageops.py and oracle/warpops.py; the box half of Translate / Scale / Rotate and BoxFilter's overlap test is in oracle/boxops.py.
 //   image_assemble_kernel  one CTA per (output row, image): every output pixel is traced back through the resize to at most
 //                          four canvas taps, and each tap through the composed crop / pad / flip map to a source pixel or to
 //                          the background colour.  No intermediate image exists.
 // The file is compiled with --fmad=false; the float64 resize coordinates also spell their roundings out (__dmul_rn / __dadd_rn).
 #include "common.cuh"
+#include <algorithm>
 #include <cmath>
 #include <vector>
 
@@ -27,6 +29,41 @@ using namespace ssdk;
 namespace {
 
 constexpr int kBoxThreads = 128;
+
+// cos / sin of angle * (CV_PI / 180) for the angles the ops use, as the C library computes them (cv2.getRotationMatrix2D).
+__host__ __device__ inline bool cv_cos_sin(double angle, double& c, double& s) {
+  if (angle == 0.0) { c = 1.0; s = 0.0; return true; }
+  if (angle == 90.0) { c = 0x1.1a62633145c07p-54; s = 1.0; return true; }
+  if (angle == 180.0) { c = -1.0; s = 0x1.1a62633145c07p-53; return true; }
+  if (angle == 270.0) { c = -0x1.a79394c9e8a0ap-53; s = -1.0; return true; }
+  return false;
+}
+
+// cv2.getRotationMatrix2D(center, angle, scale): the centre is a Point2f.  The file is compiled with --fmad=false, so every
+// product and sum below is rounded on its own, as in OpenCV's scalar code.
+__host__ __device__ inline void cv_rotation_matrix(double cx, double cy, double c, double s, double scale, double M[6]) {
+  cx = (double)(float)cx; cy = (double)(float)cy;
+  const double alpha = c * scale, beta = s * scale;
+  M[0] = alpha; M[1] = beta; M[2] = (1 - alpha) * cx - beta * cy;
+  M[3] = -beta; M[4] = alpha; M[5] = beta * cx + (1 - alpha) * cy;
+}
+
+// Rotate.__call__'s matrix and output size (object_detection_2d_geometric_ops.py:686-700).
+__host__ __device__ inline void rotate_geometry(double h, double w, double c, double s, double M[6], long long& h_new, long long& w_new) {
+  cv_rotation_matrix(w / 2, h / 2, c, s, 1.0, M);
+  const double cos_a = fabs(M[0]), sin_a = fabs(M[1]);
+  w_new = (long long)(h * sin_a + w * cos_a);
+  h_new = (long long)(h * cos_a + w * sin_a);
+  M[5] += (double)(h_new - (long long)h) / 2;
+  M[2] += (double)(w_new - (long long)w) / 2;
+}
+
+// Both corners through M as np.dot computes them ((m0*x + m1*y) + m2, each step rounded), then np.round.
+__device__ __forceinline__ void corners(const double M[6], double& x0, double& y0, double& x1, double& y1) {
+  const double nx0 = rint((M[0] * x0 + M[1] * y0) + M[2]), ny0 = rint((M[3] * x0 + M[4] * y0) + M[5]);
+  const double nx1 = rint((M[0] * x1 + M[1] * y1) + M[2]), ny1 = rint((M[3] * x1 + M[4] * y1) + M[5]);
+  x0 = nx0; y0 = ny0; x1 = nx1; y1 = ny1;
+}
 
 __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __restrict__ gt, int gt_f64, const int* __restrict__ offs, const ssdk_box_op* __restrict__ ops,
                                                               int max_ops, float* __restrict__ tmp, int* __restrict__ counts) {
@@ -69,6 +106,43 @@ __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __rest
         } else if (op.op == SSDK_BOXOP_FILTER) {             // BoxFilter: degenerate and / or minimum area
           if (op.flags & 1) valid = valid && (x1 > x0) && (y1 > y0);
           if (op.flags & 2) valid = valid && ((x1 - x0) * (y1 - y0) >= op.a0);
+        } else if (op.op == SSDK_BOXOP_TRANSLATE) {          // labels[:, [xmin, xmax]] += dx_abs; labels[:, [ymin, ymax]] += dy_abs
+          x0 += op.a1; x1 += op.a1; y0 += op.a0; y1 += op.a0;
+        } else if (op.op == SSDK_BOXOP_SCALE) {
+          double M[6];
+          cv_rotation_matrix(op.a2 / 2, op.a1 / 2, 1.0, 0.0, op.a0, M);
+          corners(M, x0, y0, x1, y1);
+        } else if (op.op == SSDK_BOXOP_ROTATE) {
+          double M[6], c, s;
+          long long hn, wn;
+          if (cv_cos_sin(op.a0, c, s) && op.a0 != 0.0) {
+            rotate_geometry(op.a1, op.a2, c, s, M, hn, wn);
+            corners(M, x0, y0, x1, y1);
+            if (op.a0 != 270.0) { const double t = y0; y0 = y1; y1 = t; }   // 90, 180: ymin and ymax were switched
+            if (op.a0 != 90.0) { const double t = x0; x0 = x1; x1 = t; }    // 180, 270: xmin and xmax were switched
+          }
+        } else if (op.op == SSDK_BOXOP_OVERLAP) {            // BoxFilter's overlap test against an a2 x a3 image
+          const int crit = op.flags & 3, bp = (op.flags >> 2) & 3;
+          const double d = bp == 1 ? 1.0 : bp == 2 ? -1.0 : 0.0, H = op.a2, W = op.a3, lower = op.a0, upper = op.a1;
+          if (crit == 0) {
+            const double cy = (y0 + y1) / 2, cx = (x0 + x1) / 2;
+            valid = valid && (cy >= 0.0) && (cy <= H - 1) && (cx >= 0.0) && (cx <= W - 1);
+          } else if (crit == 1) {
+            const double area = (x1 - x0 + d) * (y1 - y0 + d);
+            const double inter = (fmin(fmax(x1, 0.0), W - 1) - fmin(fmax(x0, 0.0), W - 1) + d) *
+                                 (fmin(fmax(y1, 0.0), H - 1) - fmin(fmax(y0, 0.0), H - 1) + d);
+            const bool lo = lower == 0.0 ? inter > lower * area : inter >= lower * area;
+            valid = valid && lo && (inter <= upper * area);
+          } else {                                           // iou(image, box): the intersection ignores border_pixels
+            const double iw = fmax(0.0, fmin(W, x1) - fmax(0.0, x0)), ih = fmax(0.0, fmin(H, y1) - fmax(0.0, y0));
+            const double inter = iw * ih;
+            const double ap = (W - 0.0 + d) * (H - 0.0 + d), aq = (x1 - x0 + d) * (y1 - y0 + d);
+            const double v = inter / ((ap + aq) - inter);
+            valid = valid && (v > lower) && (v <= upper);
+          }
+        } else if (op.op == SSDK_BOXOP_CLIP) {               // np.clip to [0, h-1] / [0, w-1]
+          y0 = fmin(fmax(y0, 0.0), op.a0 - 1); y1 = fmin(fmax(y1, 0.0), op.a0 - 1);
+          x0 = fmin(fmax(x0, 0.0), op.a1 - 1); x1 = fmin(fmax(x1, 0.0), op.a1 - 1);
         }
       }
     }
@@ -149,29 +223,43 @@ extern "C" int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_
 namespace {
 
 constexpr int kImgThreads = 128;
-enum { kImgCopy = 0, kImgNearest = 1, kImgLinear = 2, kImgArea2 = 3 };
+enum { kImgCopy = 0, kImgNearest = 1, kImgLinear = 2, kImgArea2 = 3, kImgWarp = 4 };
 
-// One image's op list, composed on the host.  Every crop, pad and flip before the resize is an integer translation and / or
-// reflection per axis, so the canvas the resize reads is described by its size, one affine map to the source and the rectangle
-// the source covers; canvas pixels outside that rectangle show the background colour.
+// An integer map from a canvas to the image it is drawn from: canvas (r, c) -> (o0 + m00 * r + m01 * c, o1 + m10 * r + m11 * c),
+// a translation and a signed axis permutation.  Canvas rows [v0, v1) x columns [v2, v3) come from that image; every other canvas
+// pixel shows the background colour.  Crops, pads, flips, translations and 90-degree rotations all compose into one.
+struct IntMap {
+  int o0, o1, m00, m01, m10, m11;
+  int v0, v1, v2, v3;
+};
+
+// One image's op list, composed on the host: the integer ops before the resampling step (RESIZE or SCALE) map the canvas it
+// reads to the source; the integer ops after a SCALE map the output to the SCALE's output.
 struct ImgDesc {
   long long src_off;           // byte offset of the image in the packed source buffer
   int h, w, c;                 // source geometry (c = 1, 3 or 4)
-  int ch, cw;                  // canvas size before the resize
-  int oy, sy, ox, sx;          // source row = oy + sy * canvas row, source column = ox + sx * canvas column (sy, sx = +-1)
-  int vy0, vy1, vx0, vx1;      // canvas rows [vy0, vy1) x columns [vx0, vx1) come from the source
+  int ch, cw;                  // canvas size before the resampling step
+  IntMap pre;                  // canvas -> source
+  IntMap post;                 // output -> SCALE output (kImgWarp only)
   int bg;                      // background R | G << 8 | B << 16
-  int mode;                    // kImgCopy / kImgNearest / kImgLinear / kImgArea2
-  double scale_y, scale_x;     // cv2's 1 / (out / in), float64
+  int mode;                    // kImgCopy / kImgNearest / kImgLinear / kImgArea2 / kImgWarp
+  double scale_y, scale_x;     // RESIZE: cv2's 1 / (out / in), float64
+  double m[6];                 // SCALE: cv2's inverted matrix, float64
 };
 
+__device__ __forceinline__ void bg_px(const ImgDesc& d, int v[3]) {
+  v[0] = d.bg & 255; v[1] = (d.bg >> 8) & 255; v[2] = (d.bg >> 16) & 255;
+}
+
 __device__ __forceinline__ void canvas_px(const uint8_t* __restrict__ src, const ImgDesc& d, int r, int c, int v[3]) {
-  if (r >= d.vy0 && r < d.vy1 && c >= d.vx0 && c < d.vx1) {
-    const uint8_t* p = src + d.src_off + ((long long)(d.oy + d.sy * r) * d.w + (d.ox + d.sx * c)) * d.c;
+  const IntMap& m = d.pre;
+  if (r >= m.v0 && r < m.v1 && c >= m.v2 && c < m.v3) {
+    const int sr = m.o0 + m.m00 * r + m.m01 * c, sc = m.o1 + m.m10 * r + m.m11 * c;
+    const uint8_t* p = src + d.src_off + ((long long)sr * d.w + sc) * d.c;
     if (d.c == 1) { v[0] = v[1] = v[2] = p[0]; }              // gray -> RGB by replication, RGBA -> RGB drops alpha
     else { v[0] = p[0]; v[1] = p[1]; v[2] = p[2]; }
   } else {
-    v[0] = d.bg & 255; v[1] = (d.bg >> 8) & 255; v[2] = (d.bg >> 16) & 255;
+    bg_px(d, v);
   }
 }
 
@@ -184,6 +272,30 @@ __device__ __forceinline__ void linear_coord(int dst, double scale, int& s, floa
 // saturate_cast<short>(w * 2048): round half to even; w is in [0, 1] so no saturation is needed.
 __device__ __forceinline__ int coef11(float w) { return __float2int_rn(__fmul_rn(w, 2048.f)); }
 
+// One pixel (row y, column x) of uint8 cv2.warpAffine, INTER_LINEAR, BORDER_CONSTANT (imgwarp.cpp's WarpAffineInvoker and
+// remapBilinear): X0 = rint((m1*y + m2)*1024) + 16, adelta = rint(m0*x*1024), X = (X0 + adelta) >> 5; source column X >> 5
+// (saturated to int16), fraction X & 31; likewise for rows with m4, m5, m3.  The bilinear weights (32-fy)(32-fx)*32, ... sum to
+// 2^15 exactly; a tap outside the canvas reads the border colour (the one background colour of the list).
+__device__ __forceinline__ void warp_px(const uint8_t* __restrict__ src, const ImgDesc& d, int y, int x, int v[3]) {
+  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(d.m[1], (double)y), d.m[2]), 1024.0)) + 16;
+  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(d.m[4], (double)y), d.m[5]), 1024.0)) + 16;
+  const int X = (X0 + __double2int_rn(__dmul_rn(__dmul_rn(d.m[0], (double)x), 1024.0))) >> 5;
+  const int Y = (Y0 + __double2int_rn(__dmul_rn(__dmul_rn(d.m[3], (double)x), 1024.0))) >> 5;
+  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767), fx = X & 31, fy = Y & 31;
+  if (sx >= d.cw || sx + 1 < 0 || sy >= d.ch || sy + 1 < 0) { bg_px(d, v); return; }   // all four taps outside
+  int p00[3], p01[3], p10[3], p11[3];
+  const bool r0 = sy >= 0, r1 = sy + 1 < d.ch, c0 = sx >= 0, c1 = sx + 1 < d.cw;
+  if (r0 && c0) canvas_px(src, d, sy, sx, p00); else bg_px(d, p00);
+  if (r0 && c1) canvas_px(src, d, sy, sx + 1, p01); else bg_px(d, p01);
+  if (r1 && c0) canvas_px(src, d, sy + 1, sx, p10); else bg_px(d, p10);
+  if (r1 && c1) canvas_px(src, d, sy + 1, sx + 1, p11); else bg_px(d, p11);
+  const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = (p00[k] * w00 + p01[k] * w01 + p10[k] * w10 + p11[k] * w11 + (1 << 14)) >> 15;
+}
+
+// kWarp: the batch has a SCALE; batches without one run an instantiation that carries no warp code (fewer registers).
+template <bool kWarp>
 __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8_t* __restrict__ src, const ImgDesc* __restrict__ descs,
                                                                      int out_h, int out_w, float* __restrict__ out) {
   const int b = blockIdx.y, dy = blockIdx.x;
@@ -205,6 +317,13 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8
     int v[3];
     if (d.mode == kImgCopy) {
       canvas_px(src, d, r0, dx, v);
+    } else if (kWarp && d.mode == kImgWarp) {
+      // the integer ops after the SCALE pick the pixel of its output, or the background
+      const IntMap& q = d.post;
+      if (dy >= q.v0 && dy < q.v1 && dx >= q.v2 && dx < q.v3)
+        warp_px(src, d, q.o0 + q.m00 * dy + q.m01 * dx, q.o1 + q.m10 * dy + q.m11 * dx, v);
+      else
+        bg_px(d, v);
     } else if (d.mode == kImgNearest) {
       canvas_px(src, d, r0, min((int)floor(__dmul_rn((double)dx, d.scale_x)), d.cw - 1), v);
     } else if (d.mode == kImgArea2) {                         // INTER_AREA's fast 2x path: rounded mean of a 2x2 block
@@ -237,6 +356,104 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8
 
 bool is_int(double a) { return a == std::floor(a) && std::fabs(a) <= (double)(1 << 24); }
 
+// Host form of IntMap while a list is composed: canvas h x w, canvas (r, c) -> o + m * (r, c), rows [v0, v1) x cols [v2, v3) valid.
+struct HostMap {
+  long long h, w, o0, o1, m00, m01, m10, m11, v0, v1, v2, v3;
+};
+// One integer op: the new canvas is nh x nw, and new (r, c) shows old (t0 + p00 * r + p01 * c, t1 + p10 * r + p11 * c), where
+// that lies in the old canvas, the op's background colour elsewhere.  p is a signed permutation.
+struct IntOp {
+  long long nh, nw, t0, t1;
+  int p00, p01, p10, p11;
+};
+
+HostMap identity_map(long long h, long long w) { return HostMap{h, w, 0, 0, 1, 0, 0, 1, 0, h, 0, w}; }
+
+// {u : lo <= t + s * u < hi} for s = +-1, as [a, b)
+void pre_interval(long long lo, long long hi, long long t, int s, long long& a, long long& b) {
+  if (s > 0) { a = lo - t; b = hi - t; } else { a = t - hi + 1; b = t - lo + 1; }
+}
+
+// The new-canvas rectangle whose pixels the op draws from the old rectangle rows [r0, r1) x cols [c0, c1).
+void preimage(const IntOp& op, long long r0, long long r1, long long c0, long long c1, long long v[4]) {
+  if (op.p00 != 0) { pre_interval(r0, r1, op.t0, op.p00, v[0], v[1]); pre_interval(c0, c1, op.t1, op.p11, v[2], v[3]); }
+  else { pre_interval(r0, r1, op.t0, op.p01, v[2], v[3]); pre_interval(c0, c1, op.t1, op.p10, v[0], v[1]); }
+  v[0] = std::max(v[0], 0LL); v[1] = std::min(v[1], op.nh); v[2] = std::max(v[2], 0LL); v[3] = std::min(v[3], op.nw);
+  if (v[1] <= v[0] || v[3] <= v[2]) v[0] = v[1] = v[2] = v[3] = 0;
+}
+
+// Compose op into map; returns whether the op brings background into its canvas.
+bool compose(HostMap& m, const IntOp& op) {
+  long long full[4], v[4];
+  preimage(op, 0, m.h, 0, m.w, full);
+  preimage(op, m.v0, m.v1, m.v2, m.v3, v);
+  HostMap n;
+  n.h = op.nh; n.w = op.nw;
+  n.o0 = m.o0 + m.m00 * op.t0 + m.m01 * op.t1; n.o1 = m.o1 + m.m10 * op.t0 + m.m11 * op.t1;
+  n.m00 = m.m00 * op.p00 + m.m01 * op.p10; n.m01 = m.m00 * op.p01 + m.m01 * op.p11;
+  n.m10 = m.m10 * op.p00 + m.m11 * op.p10; n.m11 = m.m10 * op.p01 + m.m11 * op.p11;
+  n.v0 = v[0]; n.v1 = v[1]; n.v2 = v[2]; n.v3 = v[3];
+  m = n;
+  return !(full[0] == 0 && full[1] == op.nh && full[2] == 0 && full[3] == op.nw);
+}
+
+IntMap device_map(const HostMap& m) {
+  return IntMap{(int)m.o0, (int)m.o1, (int)m.m00, (int)m.m01, (int)m.m10, (int)m.m11, (int)m.v0, (int)m.v1, (int)m.v2, (int)m.v3};
+}
+
+// warpAffine's inversion of a forward matrix (imgwarp.cpp; the same as cv2.invertAffineTransform).
+void cv_invert_affine(double M[6]) {
+  double D = M[0] * M[4] - M[1] * M[3];
+  D = D != 0 ? 1. / D : 0;
+  const double A11 = M[4] * D, A22 = M[0] * D;
+  M[0] = A11; M[1] *= -D;
+  M[3] *= -D; M[4] = A22;
+  const double b1 = -M[0] * M[2] - M[1] * M[5];
+  const double b2 = -M[3] * M[2] - M[4] * M[5];
+  M[2] = b1; M[5] = b2;
+}
+
+constexpr long long kShortMax = 32767;
+
+// cv2's fixed-point coordinates of a warp to nh x nw with inverse matrix m stay in int32 (the largest magnitude of
+// X0 + adelta, linear in the row and the column, is reached at a corner).
+bool fixed_point_fits(const double m[6], long long nh, long long nw) {
+  for (int k = 0; k < 2; ++k) {
+    const double* r = m + 3 * k;
+    double worst = 0;
+    for (long long y : {0LL, nh - 1})
+      for (long long x : {0LL, nw - 1})
+        worst = std::max(worst, std::fabs((r[1] * (double)y + r[2]) * 1024.0) + std::fabs(r[0] * (double)x * 1024.0));
+    if (!(worst < (double)(1 << 30))) return false;
+  }
+  return true;
+}
+
+// Rotate's warp as an integer op: cv2's fixed-point map (X0(y) + adelta(x), Y0(y) + bdelta(x)) is computed for every output row
+// and column and must be exactly 1024 * (a signed permutation of (y, x) plus an integer offset) + 16, so every sample has
+// fraction 0 and the warp is a pixel permutation with the border colour (black) where it leaves the source.
+bool rotate_op(long long h, long long w, double angle, IntOp& op) {
+  double c, s, M[6];
+  if (!cv_cos_sin(angle, c, s) || angle == 0.0) return false;
+  long long hn, wn;
+  rotate_geometry((double)h, (double)w, c, s, M, hn, wn);
+  cv_invert_affine(M);
+  op.nh = hn; op.nw = wn;
+  op.p11 = (int)std::rint(M[0]); op.p10 = (int)std::rint(M[1]); op.t1 = (long long)std::rint(M[2]);
+  op.p01 = (int)std::rint(M[3]); op.p00 = (int)std::rint(M[4]); op.t0 = (long long)std::rint(M[5]);
+  const bool perm = (op.p00 != 0 && op.p01 == 0 && op.p10 == 0 && op.p11 != 0) || (op.p00 == 0 && op.p01 != 0 && op.p10 != 0 && op.p11 == 0);
+  if (!perm || hn <= 0 || wn <= 0 || !fixed_point_fits(M, hn, wn)) return false;
+  for (long long x = 0; x < wn; ++x) {
+    if (std::nearbyint(M[0] * (double)x * 1024.0) != (double)(1024 * op.p11 * x)) return false;
+    if (std::nearbyint(M[3] * (double)x * 1024.0) != (double)(1024 * op.p01 * x)) return false;
+  }
+  for (long long y = 0; y < hn; ++y) {
+    if (std::nearbyint((M[1] * (double)y + M[2]) * 1024.0) != (double)(1024 * (op.t1 + op.p10 * y))) return false;
+    if (std::nearbyint((M[4] * (double)y + M[5]) * 1024.0) != (double)(1024 * (op.t0 + op.p00 * y))) return false;
+  }
+  return true;
+}
+
 // Compose image b's op list into its descriptor; every check the entry point documents.
 int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_op* ops, int max_ops, int out_h, int out_w, ImgDesc* out) {
   const int h = hwc[3 * b], w = hwc[3 * b + 1], c = hwc[3 * b + 2];
@@ -244,64 +461,104 @@ int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_o
   SSDK_REQUIRE(c == 1 || c == 3 || c == 4, "ssdk_assemble_images: image %d has %d channels (1, 3 or 4 are supported)", b, c);
   SSDK_REQUIRE(offs[b] >= 0 && offs[b + 1] - offs[b] == (long long)h * w * c,
                "ssdk_assemble_images: image %d: offsets %lld..%lld do not hold %dx%dx%d bytes", b, offs[b], offs[b + 1], h, w, c);
-  long long ch = h, cw = w, oy = 0, ox = 0, vy0 = 0, vy1 = h, vx0 = 0, vx1 = w;
-  int sy = 1, sx = 1, bg = 0, mode = kImgCopy;
-  bool has_bg = false, resized = false;
+  HostMap pre = identity_map(h, w), post = identity_map(0, 0);
+  HostMap* cur = &pre;                                            // the map the next integer op composes into
+  int bg = 0, mode = kImgCopy;
+  bool has_bg = false, resized = false, warped = false;
   long long rh = 0, rw = 0;
+  double minv[6] = {0, 0, 0, 0, 0, 0};
   for (int i = 0; i < max_ops; ++i) {
     const ssdk_box_op& op = ops[(size_t)b * max_ops + i];
     if (op.op == SSDK_BOXOP_END) break;
-    if (op.op == SSDK_BOXOP_FILTER) continue;                     // boxes only
-    SSDK_REQUIRE(op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_RESIZE, "ssdk_assemble_images: image %d, op %d: unknown op code %d", b, i, op.op);
+    if (op.op == SSDK_BOXOP_FILTER || op.op == SSDK_BOXOP_OVERLAP || op.op == SSDK_BOXOP_CLIP) continue;   // boxes only
+    SSDK_REQUIRE(op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE, "ssdk_assemble_images: image %d, op %d: unknown op code %d", b, i, op.op);
     SSDK_REQUIRE(!resized, "ssdk_assemble_images: image %d, op %d: the RESIZE must be the last op that changes the image", b, i);
+    const long long ch = cur->h, cw = cur->w;
+    const int col = (int)(((unsigned)op.flags >> 8) & 0xFFFFFFu);
+    IntOp io{ch, cw, 0, 0, 1, 0, 0, 1};
+    int io_bg = col;
     if (op.op == SSDK_BOXOP_CROP_PAD) {
       SSDK_REQUIRE(is_int(op.a0) && is_int(op.a1) && is_int(op.a2) && is_int(op.a3) && op.a2 > 0 && op.a3 > 0,
                    "ssdk_assemble_images: image %d, op %d: CROP_PAD needs an integer patch of positive size", b, i);
-      const long long py = (long long)op.a0, px = (long long)op.a1, ph = (long long)op.a2, pw = (long long)op.a3;
+      const long long py = (long long)op.a0, px = (long long)op.a1;
       SSDK_REQUIRE(!(py > ch || px > cw), "The given patch doesn't overlap with the input image. (image %d, op %d)", b, i);
-      if (py < 0 || px < 0 || py + ph > ch || px + pw > cw) {     // the patch reaches past its input: it adds background
-        const int col = (int)(((unsigned)op.flags >> 8) & 0xFFFFFFu);
-        SSDK_REQUIRE(!has_bg || col == bg, "ssdk_assemble_images: image %d, op %d: two pads with different background colours in "
-                     "one list are not supported", b, i);
-        has_bg = true; bg = col;
-      }
-      oy += sy * py; ox += sx * px;
-      vy0 = std::max(vy0 - py, 0LL); vy1 = std::min(vy1 - py, ph);
-      vx0 = std::max(vx0 - px, 0LL); vx1 = std::min(vx1 - px, pw);
-      if (vy1 <= vy0 || vx1 <= vx0) vy0 = vy1 = vx0 = vx1 = 0;      // nothing of the source is left
-      ch = ph; cw = pw;
+      io.nh = (long long)op.a2; io.nw = (long long)op.a3; io.t0 = py; io.t1 = px;
     } else if (op.op == SSDK_BOXOP_FLIP_H) {
       SSDK_REQUIRE(op.a0 == (double)cw, "ssdk_assemble_images: image %d, op %d: FLIP_H width %g is not the canvas width %lld", b, i, op.a0, cw);
-      ox += sx * (cw - 1); sx = -sx;
-      const long long t = vx0; vx0 = cw - vx1; vx1 = cw - t;
+      io.t1 = cw - 1; io.p11 = -1;
     } else if (op.op == SSDK_BOXOP_FLIP_V) {
       SSDK_REQUIRE(op.a0 == (double)ch, "ssdk_assemble_images: image %d, op %d: FLIP_V height %g is not the canvas height %lld", b, i, op.a0, ch);
-      oy += sy * (ch - 1); sy = -sy;
-      const long long t = vy0; vy0 = ch - vy1; vy1 = ch - t;
+      io.t0 = ch - 1; io.p00 = -1;
+    } else if (op.op == SSDK_BOXOP_TRANSLATE) {
+      SSDK_REQUIRE(op.a2 == (double)ch && op.a3 == (double)cw, "ssdk_assemble_images: image %d, op %d: TRANSLATE of a %gx%g image, but the "
+                   "canvas is %lldx%lld at that point", b, i, op.a2, op.a3, ch, cw);
+      SSDK_REQUIRE(is_int(op.a0) && is_int(op.a1) && std::fabs(op.a0) < (double)(1 << 20) && std::fabs(op.a1) < (double)(1 << 20),
+                   "ssdk_assemble_images: image %d, op %d: TRANSLATE needs integer shifts below 2^20 pixels", b, i);
+      io.t0 = -(long long)op.a0; io.t1 = -(long long)op.a1;       // warpAffine with an integer matrix: a shift, fraction 0
+    } else if (op.op == SSDK_BOXOP_ROTATE) {
+      SSDK_REQUIRE(op.a0 == 90.0 || op.a0 == 180.0 || op.a0 == 270.0, "ssdk_assemble_images: image %d, op %d: ROTATE angle %g is not "
+                   "90, 180 or 270", b, i, op.a0);
+      SSDK_REQUIRE(op.a1 == (double)ch && op.a2 == (double)cw, "ssdk_assemble_images: image %d, op %d: ROTATE of a %gx%g image, but the "
+                   "canvas is %lldx%lld at that point", b, i, op.a1, op.a2, ch, cw);
+      SSDK_REQUIRE(ch < kShortMax && cw < kShortMax, "ssdk_assemble_images: image %d, op %d: ROTATE of a %lldx%lld canvas (cv2's warp "
+                   "needs sides below 32767)", b, i, ch, cw);
+      SSDK_REQUIRE(rotate_op(ch, cw, op.a0, io), "ssdk_assemble_images: image %d, op %d: cv2's fixed-point map of this ROTATE is not an "
+                   "exact pixel permutation", b, i);
+      io_bg = 0;                                                  // Rotate's warpAffine keeps cv2's default border: black
     } else {
-      SSDK_REQUIRE(op.a0 == (double)ch && op.a1 == (double)cw, "ssdk_assemble_images: image %d, op %d: RESIZE from %gx%g, but the canvas "
-                   "is %lldx%lld at that point", b, i, op.a0, op.a1, ch, cw);
-      SSDK_REQUIRE(is_int(op.a2) && is_int(op.a3) && op.a2 > 0 && op.a3 > 0, "ssdk_assemble_images: image %d, op %d: RESIZE needs a "
-                   "positive integer output size", b, i);
-      const int interp = (op.flags >> 8) & 255;
-      SSDK_REQUIRE(interp == 0 || interp == 1, "ssdk_assemble_images: image %d, op %d: interpolation mode %d is not supported "
-                   "(INTER_NEAREST = 0 and INTER_LINEAR = 1 are)", b, i, interp);
-      resized = true; rh = (long long)op.a2; rw = (long long)op.a3;
-      mode = interp == 0 ? kImgNearest : kImgLinear;
+      const bool scale = op.op == SSDK_BOXOP_SCALE;
+      SSDK_REQUIRE(!warped, "ssdk_assemble_images: image %d, op %d: at most one resampling step (RESIZE or SCALE) per list", b, i);
+      if (!scale) {
+        SSDK_REQUIRE(op.a0 == (double)ch && op.a1 == (double)cw, "ssdk_assemble_images: image %d, op %d: RESIZE from %gx%g, but the canvas "
+                     "is %lldx%lld at that point", b, i, op.a0, op.a1, ch, cw);
+        SSDK_REQUIRE(is_int(op.a2) && is_int(op.a3) && op.a2 > 0 && op.a3 > 0, "ssdk_assemble_images: image %d, op %d: RESIZE needs a "
+                     "positive integer output size", b, i);
+        const int interp = (op.flags >> 8) & 255;
+        SSDK_REQUIRE(interp == 0 || interp == 1, "ssdk_assemble_images: image %d, op %d: interpolation mode %d is not supported "
+                     "(INTER_NEAREST = 0 and INTER_LINEAR = 1 are)", b, i, interp);
+        resized = true; rh = (long long)op.a2; rw = (long long)op.a3;
+        mode = interp == 0 ? kImgNearest : kImgLinear;
+        continue;
+      }
+      SSDK_REQUIRE(op.a1 == (double)ch && op.a2 == (double)cw, "ssdk_assemble_images: image %d, op %d: SCALE of a %gx%g image, but the "
+                   "canvas is %lldx%lld at that point", b, i, op.a1, op.a2, ch, cw);
+      SSDK_REQUIRE(op.a0 > 0 && std::isfinite(op.a0), "ssdk_assemble_images: image %d, op %d: SCALE factor %g is not positive", b, i, op.a0);
+      SSDK_REQUIRE(ch < kShortMax && cw < kShortMax, "ssdk_assemble_images: image %d, op %d: SCALE of a %lldx%lld canvas (cv2's warp "
+                   "needs sides below 32767)", b, i, ch, cw);
+      cv_rotation_matrix((double)cw / 2, (double)ch / 2, 1.0, 0.0, op.a0, minv);
+      cv_invert_affine(minv);
+      SSDK_REQUIRE(fixed_point_fits(minv, ch, cw), "ssdk_assemble_images: image %d, op %d: SCALE factor %g overflows cv2's fixed-point "
+                   "coordinates", b, i, op.a0);
+      SSDK_REQUIRE(!has_bg || col == bg, "ssdk_assemble_images: image %d, op %d: ops with different background colours in one list are "
+                   "not supported", b, i);
+      has_bg = true; bg = col;
+      warped = true; mode = kImgWarp;
+      post = identity_map(ch, cw);
+      cur = &post;
+      continue;
+    }
+    if (compose(*cur, io)) {                                      // the op brings in background
+      SSDK_REQUIRE(!has_bg || io_bg == bg, "ssdk_assemble_images: image %d, op %d: ops with different background colours in one list "
+                   "are not supported", b, i);
+      has_bg = true; bg = io_bg;
     }
   }
-  const long long fh = resized ? rh : ch, fw = resized ? rw : cw;
+  const long long ch = pre.h, cw = pre.w;
+  const long long fh = resized ? rh : warped ? post.h : ch, fw = resized ? rw : warped ? post.w : cw;
   SSDK_REQUIRE(fh == out_h && fw == out_w, "ssdk_assemble_images: image %d ends as %lldx%lld, the output is %dx%d", b, fh, fw, out_h, out_w);
-  SSDK_REQUIRE(std::llabs(oy) + ch < (1LL << 30) && std::llabs(ox) + cw < (1LL << 30), "ssdk_assemble_images: image %d: canvas too large", b);
-  if (!resized || (rh == ch && rw == cw)) mode = kImgCopy;           // cv2.resize to the same size is a copy
+  for (const HostMap* m : {&pre, &post})
+    SSDK_REQUIRE(std::llabs(m->o0) + m->h + m->w < (1LL << 30) && std::llabs(m->o1) + m->h + m->w < (1LL << 30),
+                 "ssdk_assemble_images: image %d: canvas too large", b);
+  if (resized && rh == ch && rw == cw) mode = kImgCopy;            // cv2.resize to the same size is a copy
   else if (mode == kImgLinear && ch == 2 * rh && cw == 2 * rw) mode = kImgArea2;
   ImgDesc& d = *out;
   d.src_off = offs[b]; d.h = h; d.w = w; d.c = c;
-  d.ch = (int)ch; d.cw = (int)cw; d.oy = (int)oy; d.sy = sy; d.ox = (int)ox; d.sx = sx;
-  d.vy0 = (int)vy0; d.vy1 = (int)vy1; d.vx0 = (int)vx0; d.vx1 = (int)vx1;
+  d.ch = (int)ch; d.cw = (int)cw;
+  d.pre = device_map(pre); d.post = device_map(post);
   d.bg = bg; d.mode = mode;
   d.scale_y = resized ? 1.0 / ((double)rh / (double)ch) : 1.0;
   d.scale_x = resized ? 1.0 / ((double)rw / (double)cw) : 1.0;
+  for (int k = 0; k < 6; ++k) d.m[k] = minv[k];
   return SSDK_OK;
 }
 
@@ -338,7 +595,11 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
   SSDK_CHECK_CUDA(cudaMemcpyAsync(ctx->ws[4].ptr, st.ptr, bytes, cudaMemcpyHostToDevice, stream));
   SSDK_CHECK_CUDA(cudaEventRecord(st.done, stream));
   ctx->img_stage_next = (ctx->img_stage_next + 1) % ssdk_ctx::kImgStages;
-  image_assemble_kernel<<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, reinterpret_cast<const ImgDesc*>(ctx->ws[4].ptr), out_h, out_w, out_dev);
+  const ImgDesc* d_dev = reinterpret_cast<const ImgDesc*>(ctx->ws[4].ptr);
+  if (std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; }))
+    image_assemble_kernel<true><<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, d_dev, out_h, out_w, out_dev);
+  else
+    image_assemble_kernel<false><<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, d_dev, out_h, out_w, out_dev);
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;

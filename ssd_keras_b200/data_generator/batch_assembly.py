@@ -18,13 +18,24 @@ one list moves the boxes and produces the image batch; ``assemble_training_batch
   pads with ``(123, 117, 104)``;
 - ``flip(width_or_height, dim)``: ``Flip``;
 - ``resize(..., interpolation_mode=1)``: uint8 ``cv2.resize`` with ``INTER_NEAREST`` (0) or ``INTER_LINEAR`` (1), bit-exact
-  to OpenCV 4.13 (``oracle/imageops.py`` restates it); at most one, as the last op that changes the image;
-- ``box_filter``: boxes only.
+  to OpenCV 4.13 (``oracle/imageops.py`` restates it); nothing that changes the image may follow it;
+- ``translate`` / ``scale`` / ``rotate``: ``Translate`` / ``Scale`` / ``Rotate`` (``geometric_ops.py:233-737``), uint8
+  ``cv2.warpAffine`` with ``INTER_LINEAR`` and ``BORDER_CONSTANT``, bit-exact to OpenCV 4.13.  ``translate`` and ``rotate``
+  (90 / 180 / 270) are exact integer maps; ``scale`` is a bilinear warp.  A list holds at most one resampling step
+  (``resize`` or ``scale``); crops, pads, flips, translations and rotations may come before it, and after a ``scale`` too.
+  One background colour per list: pads, translations and scales that bring in background must agree, and a rotation's
+  border is black;
+- ``box_filter``, ``overlap_filter``, ``clip``: boxes only.
+
+``translate_ops`` / ``scale_ops`` / ``rotate_ops`` / ``crop_pad_ops`` / ``resize_ops`` / ``box_filter_ops`` return the whole op
+sequence one call of the reference class runs, box filter and clipping included, so the geometric halves of
+``DataAugmentationConstantInputSize`` (SSD7: translate -> zoom in -> flip, or zoom out -> translate -> flip) and
+``DataAugmentationSatellite`` (flips -> rotate -> patch -> resize) are one op list per image.
 
 Not covered: photometric distortions, other interpolation modes (``INTER_CUBIC``, ``INTER_LANCZOS4``, ``INTER_AREA`` apart from
-cv2's own exact-2x linear path), ``Translate`` / ``Scale`` / ``Rotate`` (``cv2.warpAffine``), the random patch samplers, JPEG
-decoding.  The random decisions of a chain (which patch, flip or not, which interpolation) stay with the caller, as for the
-boxes."""
+cv2's own exact-2x linear path), a second resampling step, the random samplers (``RandomTranslate`` / ``RandomScale``'s draws,
+``ImageValidator`` retries, ``RandomPatch``), JPEG decoding.  The random decisions of a chain (which patch, flip or not, which
+factor) stay with the caller, as for the boxes."""
 import ctypes as C
 
 import numpy as np
@@ -67,6 +78,115 @@ def resize(in_height, in_width, out_height, out_width, drop_degenerate=True, int
 def box_filter(check_degenerate=True, min_area=None):
     """``BoxFilter`` without the overlap test (validation_utils.py:155-165); also ``degenerate_box_handling='remove'``."""
     return (_ffi.BOXOP_FILTER, (1 if check_degenerate else 0) | (2 if min_area is not None else 0), float(min_area or 0.0), 0.0, 0.0, 0.0)
+
+
+def _colour(background):
+    bg = tuple(int(v) for v in background)
+    if len(bg) != 3 or any(v < 0 or v > 255 for v in bg):
+        raise ValueError('`background` must be three integers in [0, 255]')
+    return (bg[0] << 8) | (bg[1] << 16) | (bg[2] << 24)
+
+
+def translate(img_height, img_width, dy, dx, background=(0, 0, 0)):
+    """``Translate`` (geometric_ops.py:276-304): ``dy`` / ``dx`` are fractions of the image height / width; the shifts are
+    ``int(round(h*dy))`` / ``int(round(w*dx))`` as there.  ``background`` (R, G, B) goes to flag bits 8-31."""
+    h, w = int(img_height), int(img_width)
+    return (_ffi.BOXOP_TRANSLATE, _int32(_colour(background)), float(int(round(h * dy))), float(int(round(w * dx))), float(h), float(w))
+
+
+def scale(img_height, img_width, factor, background=(0, 0, 0)):
+    """``Scale`` (geometric_ops.py:487-519): zoom by ``factor`` about the image centre, same output size."""
+    if not factor > 0:
+        raise ValueError('It must be `factor > 0`.')
+    return (_ffi.BOXOP_SCALE, _int32(_colour(background)), float(factor), float(img_height), float(img_width), 0.0)
+
+
+def rotate(img_height, img_width, angle):
+    """``Rotate`` (geometric_ops.py:681-737): counter-clockwise by 90, 180 or 270 degrees; the output is w x h for 90 / 270."""
+    if angle not in {90, 180, 270}:
+        raise ValueError('`angle` must be in the set {90, 180, 270}.')
+    return (_ffi.BOXOP_ROTATE, 0, float(angle), float(img_height), float(img_width), 0.0)
+
+
+_CRITERIA = {'center_point': 0, 'area': 1, 'iou': 2}
+_BORDERS = {'half': 0, 'include': 1, 'exclude': 2}
+
+
+def overlap_filter(img_height, img_width, overlap_criterion='center_point', overlap_bounds=(0.3, 1.0), border_pixels='half'):
+    """``BoxFilter``'s overlap test (validation_utils.py:186-230) against an ``img_height x img_width`` image."""
+    if overlap_criterion not in _CRITERIA:
+        raise ValueError("`overlap_criterion` must be one of 'iou', 'area', or 'center_point'.")
+    if border_pixels not in _BORDERS:
+        raise ValueError("`border_pixels` must be one of 'half', 'include', or 'exclude'.")
+    lower, upper = (float(v) for v in overlap_bounds)
+    if lower > upper:
+        raise ValueError('The lower bound must not be greater than the upper bound.')
+    return (_ffi.BOXOP_OVERLAP, _CRITERIA[overlap_criterion] | (_BORDERS[border_pixels] << 2), lower, upper, float(img_height),
+            float(img_width))
+
+
+def clip(img_height, img_width):
+    """``clip_boxes``: boxes clipped to ``[0, h-1] x [0, w-1]``."""
+    return (_ffi.BOXOP_CLIP, 0, float(img_height), float(img_width), 0.0, 0.0)
+
+
+_BOX_FILTER_DEFAULTS = dict(check_overlap=True, check_min_area=True, check_degenerate=True, overlap_criterion='center_point',
+                            overlap_bounds=(0.3, 1.0), min_area=16, border_pixels='half')
+
+
+def box_filter_ops(spec, img_height, img_width):
+    """The ops of one ``BoxFilter.__call__`` (validation_utils.py:147-232) against an ``img_height x img_width`` image: the
+    degenerate / minimum-area test, then the overlap test (all three are ANDed there, so the order does not matter).  ``spec``
+    is a dict of ``BoxFilter``'s keyword arguments (its defaults fill the rest) or any object with those attributes, a
+    reference ``BoxFilter`` included; ``None`` gives no ops.  Fixed bounds only (no ``BoundGenerator``)."""
+    if spec is None:
+        return []
+    if isinstance(spec, dict):
+        unknown = set(spec) - set(_BOX_FILTER_DEFAULTS) - {'labels_format'}
+        if unknown:
+            raise ValueError('unknown BoxFilter arguments %s' % sorted(unknown))
+        get = lambda k: spec.get(k, _BOX_FILTER_DEFAULTS[k])          # noqa: E731
+    else:
+        get = lambda k: getattr(spec, k, _BOX_FILTER_DEFAULTS[k])      # noqa: E731
+    if not isinstance(get('overlap_bounds'), (list, tuple)):
+        raise ValueError('only fixed `overlap_bounds` (a 2-tuple) are supported')
+    ops = []
+    if get('check_degenerate') or get('check_min_area'):
+        ops.append(box_filter(check_degenerate=bool(get('check_degenerate')), min_area=get('min_area') if get('check_min_area') else None))
+    if get('check_overlap'):
+        ops.append(overlap_filter(img_height, img_width, get('overlap_criterion'), get('overlap_bounds'), get('border_pixels')))
+    return ops
+
+
+def translate_ops(img_height, img_width, dy, dx, box_filter=None, clip_boxes=True, background=(0, 0, 0)):
+    """What ``Translate(dy, dx, clip_boxes, box_filter, background)(image, labels)`` runs: the shift, its box filter against
+    the image, then the clip."""
+    return ([translate(img_height, img_width, dy, dx, background)] + box_filter_ops(box_filter, img_height, img_width)
+            + ([clip(img_height, img_width)] if clip_boxes else []))
+
+
+def scale_ops(img_height, img_width, factor, box_filter=None, clip_boxes=True, background=(0, 0, 0)):
+    """What ``Scale(factor, clip_boxes, box_filter, background)(image, labels)`` runs."""
+    return ([scale(img_height, img_width, factor, background)] + box_filter_ops(box_filter, img_height, img_width)
+            + ([clip(img_height, img_width)] if clip_boxes else []))
+
+
+def rotate_ops(img_height, img_width, angle):
+    """What ``Rotate(angle)(image, labels)`` runs: the rotation alone (it neither filters nor clips)."""
+    return [rotate(img_height, img_width, angle)]
+
+
+def crop_pad_ops(patch_ymin, patch_xmin, patch_height, patch_width, box_filter=None, clip_boxes=True, background=(0, 0, 0)):
+    """What ``CropPad(..., clip_boxes, box_filter, background)(image, labels)`` runs, for any ``BoxFilter`` (``RandomPatch``
+    with the satellite chain's 'area' filter, for instance): the patch, its box filter against the patch, then the clip."""
+    return ([crop_pad(patch_ymin, patch_xmin, patch_height, patch_width, clip_boxes=False, background=background)]
+            + box_filter_ops(box_filter, patch_height, patch_width) + ([clip(patch_height, patch_width)] if clip_boxes else []))
+
+
+def resize_ops(in_height, in_width, out_height, out_width, box_filter=None, interpolation_mode=_ffi.INTER_LINEAR):
+    """What ``Resize(out_height, out_width, interpolation_mode, box_filter)(image, labels)`` runs."""
+    return ([resize(in_height, in_width, out_height, out_width, drop_degenerate=False, interpolation_mode=interpolation_mode)]
+            + box_filter_ops(box_filter, out_height, out_width))
 
 
 def _pack_ops(ops_per_image, B):
