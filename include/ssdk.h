@@ -227,6 +227,24 @@ int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets_dev, int n
 int ssdk_eval_cumsum(ssdk_ctx* ctx, const int* tp_dev, const int* fp_dev, const int* class_offsets_dev, int n_segments,
                      int* ctp_dev, int* cfp_dev, void* stream);
 
+/* ssdk_eval_collect: the per-box loop of Evaluator.predict_on_dataset (:374-419) and predict_all_to_json for one batch of
+ * decoded rows_dev (B, max_out, 6) float32.  A row is kept when its column 0 is not 0 (y_pred[i][y_pred[i,:,0] != 0]) and, if
+ * counts_dev is given, when it lies below counts_dev[b].  Each kept row goes through its image's inverters in the generator's
+ * (reversed) order: Resize's (geometric_ops.py:74-79), v = rint(v * ratio) on the y and x columns, then, when a pad offset is
+ * set (pad = 1, 'pad' mode), CropPad's (patch_sampling_ops.py:315-320), v += offset.  inv_dev holds four doubles per image:
+ * ratio_y = canvas_h / out_h, ratio_x = canvas_w / out_w, offset_y, offset_x.  Then the confidence is rounded to conf_decimals
+ * (0: not rounded) and the four box coordinates to one decimal, as round(numpy_scalar, n) does: rint(v * 10^n) / 10^n.
+ * f64 = 0: every step in float32 (the layer path: NumPy computes float32_array * python_float in float32, the ratio rounded to
+ * float32 first); f64 = 1: every step in float64 (the rows of decode_detections).
+ * cols[10] (host): the pred_format columns class, conf, xmin, ymin, xmax, ymax, then the inverter columns ymin, ymax, xmin, xmax
+ * (gt_format + 1).  The kept rows are appended in (image, row) order at *count_dev (device counter, not read by the host) to
+ * out_image (image_base + b), out_class (the class truncated to int), out_conf and out_box (4 per row), float64; rows past
+ * capacity are counted but not written, so that the caller can detect the overflow after the last batch.  One launch, no host
+ * synchronisation. */
+int ssdk_eval_collect(ssdk_ctx* ctx, const float* rows_dev, int B, int max_out, const int* counts_dev, const double* inv_dev,
+                      const int* cols_host, int f64, int pad, int conf_decimals, int image_base, int capacity, int* count_dev, int* out_image_dev,
+                      int* out_class_dev, double* out_conf_dev, double* out_box_dev, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Decoders.
  *   mode PER_CLASS + layer_semantics=1: DecodeDetections.call   (keras_layers/keras_layer_DecodeDetections.py:109-265)

@@ -194,6 +194,9 @@ def lib():
         L.ssdk_eval_cumsum.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp]
         L.ssdk_eval_match.restype = C.c_int
         L.ssdk_eval_cumsum.restype = C.c_int
+        L.ssdk_eval_collect.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, c_int_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp,
+                                        vp, vp, vp, vp]
+        L.ssdk_eval_collect.restype = C.c_int
         L.ssdk_assemble_batch.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp]
         L.ssdk_assemble_batch.restype = C.c_int
         L.ssdk_assemble_images.argtypes = [vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp]

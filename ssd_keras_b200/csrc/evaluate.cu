@@ -113,7 +113,113 @@ __global__ void __launch_bounds__(1024) eval_cumsum_kernel(const int* __restrict
   }
 }
 
+// eval_collect_kernel: ONE CTA per batch walks the rows in (image, row) order, 1024 at a time; a block-wide exclusive scan of
+// the keep flags gives every kept row its slot, so the output keeps the reference's order without atomics.
+struct CollectCols { int c[10]; };   // class, conf, xmin, ymin, xmax, ymax, inverter ymin, ymax, xmin, xmax
+
+template <typename T> __device__ __forceinline__ T mul_rn(T a, T b);
+template <> __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+template <> __device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+template <typename T> __device__ __forceinline__ T add_rn(T a, T b);
+template <> __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+template <> __device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+template <typename T> __device__ __forceinline__ T div_rn(T a, T b);
+template <> __device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
+template <> __device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
+__device__ __forceinline__ float rint_t(float v) { return rintf(v); }      // half to even, like np.round
+__device__ __forceinline__ double rint_t(double v) { return rint(v); }
+
+// round(numpy_scalar, n) for n > 0: multiply by 10^n in the scalar's type, rint, divide
+template <typename T> __device__ __forceinline__ T round_decimals(T v, T f) { return div_rn(rint_t(mul_rn(v, f)), f); }
+
+template <typename T>
+__device__ __forceinline__ void collect_row(const float* __restrict__ r, const double* __restrict__ inv, const CollectCols& cc, int pad, int decimals,
+                                            int& cls, double& conf, double* box) {
+  T v[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) v[k] = (T)r[k];
+  const T ry = (T)inv[0], rx = (T)inv[1];                      // the Python float ratio as NumPy rounds it for this path
+  v[cc.c[6]] = rint_t(mul_rn(v[cc.c[6]], ry)); v[cc.c[7]] = rint_t(mul_rn(v[cc.c[7]], ry));
+  v[cc.c[8]] = rint_t(mul_rn(v[cc.c[8]], rx)); v[cc.c[9]] = rint_t(mul_rn(v[cc.c[9]], rx));
+  if (pad) {                                                   // CropPad's inverter: even + 0 matters, it turns -0.0 into 0.0
+    const T oy = (T)inv[2], ox = (T)inv[3];
+    v[cc.c[6]] = add_rn(v[cc.c[6]], oy); v[cc.c[7]] = add_rn(v[cc.c[7]], oy);
+    v[cc.c[8]] = add_rn(v[cc.c[8]], ox); v[cc.c[9]] = add_rn(v[cc.c[9]], ox);
+  }
+  const T c = v[cc.c[0]];
+  cls = (sizeof(T) == 4) ? __float2int_rz((float)c) : __double2int_rz((double)c);
+  T p = v[cc.c[1]];
+  if (decimals > 0) {
+    T f = (T)1;
+    for (int i = 0; i < decimals; ++i) f = mul_rn(f, (T)10);   // 10^n is exact in both types for the n a caller uses
+    p = round_decimals(p, f);
+  }
+  conf = (double)p;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) box[k] = (double)round_decimals(v[cc.c[2 + k]], (T)10);
+}
+
+__global__ void __launch_bounds__(1024) eval_collect_kernel(const float* __restrict__ rows, int B, int max_out, const int* __restrict__ counts,
+                                                            const double* __restrict__ inv, CollectCols cc, int f64, int pad, int decimals, int image_base,
+                                                            int capacity, int* __restrict__ count, int* __restrict__ o_img,
+                                                            int* __restrict__ o_cls, double* __restrict__ o_conf, double* __restrict__ o_box) {
+  __shared__ int s_warp[32];
+  __shared__ int s_base;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_base = *count;
+  __syncthreads();
+  const long long total = (long long)B * max_out;
+  for (long long base = 0; base < total; base += 1024) {
+    const long long i = base + threadIdx.x;
+    int b = 0, j = 0, keep = 0;
+    if (i < total) {
+      b = (int)(i / max_out); j = (int)(i - (long long)b * max_out);
+      keep = rows[i * 6] != 0.0f && (counts == nullptr || j < counts[b]);
+    }
+    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) s_warp[warp] = __popc(ballot);
+    __syncthreads();
+    int before = s_base, chunk = 0;
+    for (int w = 0; w < 32; ++w) { const int n = s_warp[w]; if (w < warp) before += n; chunk += n; }
+    before += __popc(ballot & ((1u << lane) - 1u));
+    if (keep && before < capacity) {
+      int cls; double conf, box[4];
+      if (f64) collect_row<double>(rows + i * 6, inv + 4 * b, cc, pad, decimals, cls, conf, box);
+      else collect_row<float>(rows + i * 6, inv + 4 * b, cc, pad, decimals, cls, conf, box);
+      o_img[before] = image_base + b; o_cls[before] = cls; o_conf[before] = conf;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) o_box[(size_t)before * 4 + k] = box[k];
+    }
+    __syncthreads();                                           // every thread has read s_warp and s_base
+    if (threadIdx.x == 0) s_base += chunk;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *count = s_base;
+}
+
 }  // namespace
+
+extern "C" int ssdk_eval_collect(ssdk_ctx* ctx, const float* rows_dev, int B, int max_out, const int* counts_dev, const double* inv_dev,
+                                 const int* cols_host, int f64, int pad, int conf_decimals, int image_base, int capacity, int* count_dev,
+                                 int* out_image_dev, int* out_class_dev, double* out_conf_dev, double* out_box_dev, void* stream_) {
+  SSDK_REQUIRE(ctx && B >= 0 && max_out >= 0 && capacity >= 0 && image_base >= 0 && conf_decimals >= 0 && conf_decimals <= 15,
+               "ssdk_eval_collect: bad argument");
+  SSDK_REQUIRE(cols_host && count_dev, "ssdk_eval_collect: NULL argument");
+  CollectCols cc;
+  for (int k = 0; k < 10; ++k) {
+    SSDK_REQUIRE(cols_host[k] >= 0 && cols_host[k] < 6, "ssdk_eval_collect: column %d is %d, the decoded rows have 6 columns", k, cols_host[k]);
+    cc.c[k] = cols_host[k];
+  }
+  if (B == 0 || max_out == 0) return SSDK_OK;
+  SSDK_REQUIRE(rows_dev && inv_dev && (capacity == 0 || (out_image_dev && out_class_dev && out_conf_dev && out_box_dev)),
+               "ssdk_eval_collect: NULL argument");
+  eval_collect_kernel<<<1, 1024, 0, (cudaStream_t)stream_>>>(rows_dev, B, max_out, counts_dev, inv_dev, cc, f64 ? 1 : 0, pad ? 1 : 0, conf_decimals,
+                                                             image_base, capacity, count_dev, out_image_dev, out_class_dev, out_conf_dev,
+                                                             out_box_dev);
+  SSDK_COUNT_LAUNCH(ctx);
+  SSDK_CHECK_CUDA(cudaGetLastError());
+  return SSDK_OK;
+}
 
 extern "C" int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets_dev, int n_seg, const int* pred_image_dev,
                                const int* pred_class_dev, const float* pred_box_dev, const int* pred_rank_dev, const double* gt_rows_dev,

@@ -6,9 +6,16 @@ key sorts plus ``ssdk_eval_match`` (one warp per (class, image) pair, float64 Io
 ``ssdk_eval_cumsum``; precision / recall / AP (:738-905) are the reference's NumPy expressions on the cumulative counts.
 
 What the class needs from ``data_generator`` is what the reference reads from its ``DataGenerator``: ``labels`` (list of
-``(k_i, 5)`` arrays), ``image_ids`` and optionally ``eval_neutral``; for ``predict_on_dataset`` additionally ``images`` (a
-sequence of HxWx3 arrays already at the model's input size -- dataset parsing and resizing belong to the out-of-scope
-``data_generator`` package).
+``(k_i, 5)`` arrays), ``image_ids`` and optionally ``eval_neutral``; for ``predict_on_dataset`` additionally ``images`` (uint8
+arrays of any size and channel count) or, when that is None, ``filenames`` (decoded with PIL).
+
+``predict_on_dataset`` has two paths.  A dataset whose ``images`` all already have the model's input size is predicted as it
+is, with the coordinates rounded to one decimal (no inverse transform).  Any other dataset goes through ``dataset_predict``:
+the reference's ``ConvertTo3Channels`` / ``RandomPadFixedAR`` / ``Resize`` chain on the device and the detections mapped back
+to the original images with the reference's inverters (``ssdk_eval_collect``).  Its results stay on the device:
+``match_predictions`` reads them there, and ``prediction_results`` builds the reference's per-class tuple lists (NumPy
+float32 scalars for the layer path, float64 for ``decode_detections``) on first access.  Assigning ``prediction_results``
+replaces them.
 
 Note on a reference quirk: with ``verbose=False`` the reference iterates ``range(len(predictions.shape))`` (:641), i.e. it
 matches only the first prediction of every class.  This implementation always matches all of them (the ``verbose=True``
@@ -33,6 +40,7 @@ class Evaluator:
         self.model_mode = model_mode
         self.pred_format = pred_format
         self.gt_format = gt_format
+        self._detections = None                  # device results of dataset_predict, or None
         self.prediction_results = None
         self.num_gt_per_class = None
         self.true_positives = None
@@ -72,18 +80,42 @@ class Evaluator:
             return ret
         return mean_average_precision
 
+    @property
+    def prediction_results(self):
+        """Per class a list of ``(image_id, confidence, xmin, ymin, xmax, ymax)`` tuples (reference :83, :417-419)."""
+        if self._prediction_results is None and self._detections is not None:
+            self._prediction_results = self._detections.per_class(self.n_classes)
+        return self._prediction_results
+
+    @prediction_results.setter
+    def prediction_results(self, value):
+        self._prediction_results = value
+        self._detections = None
+
     # -- predictions ----------------------------------------------------------------------------
     def predict_on_dataset(self, img_height, img_width, batch_size, data_generator_mode='resize', decoding_confidence_thresh=0.01,
                            decoding_iou_threshold=0.45, decoding_top_k=200, decoding_pred_coords='centroids',
                            decoding_normalize_coords=True, decoding_border_pixels='include', round_confidences=False, verbose=True,
                            ret=False):
-        """Reference :258-448 for images that already have the model's input size (``data_generator.images``): forward pass,
-        decoding (the model's own decoder in 'inference' mode, ``decode_detections`` in 'training' mode), results per class as
-        ``(image_id, confidence, xmin, ymin, xmax, ymax)`` tuples."""
+        """Reference :258-424: forward pass, decoding (the model's own decoder in 'inference' mode, ``decode_detections`` in
+        'training' mode), results per class as ``(image_id, confidence, xmin, ymin, xmax, ymax)`` tuples.  Images that all
+        already have the input size are predicted as they are; any other dataset (or ``filenames``) goes through
+        ``dataset_predict`` with ``data_generator_mode`` 'resize' or 'pad' (seeded with ``np.random.seed``, 'pad' places every
+        image where the reference does) and keeps its results on the device."""
         from ..ssd_encoder_decoder.ssd_output_decoder import decode_detections
         images = getattr(self.data_generator, 'images', None)
-        if images is None:
-            raise ValueError("`data_generator.images` is needed to predict: a sequence of images at the model's input size.")
+        if images is None or any(tuple(np.shape(im)[:2]) != (img_height, img_width) for im in images):
+            from .dataset_predict import predict_dataset
+            self._detections = predict_dataset(
+                self.model, self.data_generator, img_height, img_width, batch_size, mode=data_generator_mode, model_mode=self.model_mode,
+                decode_kwargs=dict(confidence_thresh=decoding_confidence_thresh, iou_threshold=decoding_iou_threshold,
+                                   top_k=decoding_top_k, input_coords=decoding_pred_coords, normalize_coords=decoding_normalize_coords,
+                                   border_pixels=decoding_border_pixels),
+                round_confidences=round_confidences, pred_format=self.pred_format, gt_format=self.gt_format)
+            self._prediction_results = None
+            if ret:
+                return self.prediction_results
+            return
         ids = list(self.data_generator.image_ids)
         results = [list() for _ in range(self.n_classes + 1)]
         cid, conf = self.pred_format['class_id'], self.pred_format['conf']
@@ -139,7 +171,7 @@ class Evaluator:
         import torch
         if self.data_generator.labels is None:
             raise ValueError("Matching predictions to ground truth boxes not possible, no ground truth given.")
-        if self.prediction_results is None:
+        if self._prediction_results is None and self._detections is None:
             raise ValueError("There are no prediction results. You must run `predict_on_dataset()` before calling this method.")
         if border_pixels not in _ffi.BORDER_D:
             raise ValueError("`border_pixels` must be one of 'half', 'include', 'exclude'.")
@@ -156,23 +188,27 @@ class Evaluator:
         neutral = getattr(self.data_generator, 'eval_neutral', None)
         use_neutral = ignore_neutral_boxes and neutral is not None
         # predictions -> flat arrays, class-major, input order inside a class
-        counts = [len(self.prediction_results[c]) for c in range(nC + 1)]
-        counts[0] = 0
+        if self._detections is not None:
+            counts, t_img, t_cls, t_conf, t_box = self._flat_device_predictions(id_index)
+        else:
+            counts = [len(self.prediction_results[c]) for c in range(nC + 1)]
+            counts[0] = 0
         n = int(sum(counts))
         tp_all = [[]] + [np.zeros(counts[c], dtype=int) for c in range(1, nC + 1)]
         fp_all = [[]] + [np.zeros(counts[c], dtype=int) for c in range(1, nC + 1)]
         ctp_all = [[]] + [np.zeros(counts[c], dtype=int) for c in range(1, nC + 1)]
         cfp_all = [[]] + [np.zeros(counts[c], dtype=int) for c in range(1, nC + 1)]
         if n:
-            img = np.empty(n, np.int32); cls = np.empty(n, np.int32); conf = np.empty(n, np.float32); box = np.empty((n, 4), np.float32)
-            o = 0
-            for c in range(1, nC + 1):
-                for p in self.prediction_results[c]:
-                    img[o] = id_index[str(p[0])]; cls[o] = c; conf[o] = p[1]; box[o] = p[2:6]
-                    o += 1
             dev = 'cuda'
-            t_img, t_cls = torch.from_numpy(img).to(dev), torch.from_numpy(cls).to(dev)
-            t_conf, t_box = torch.from_numpy(conf).to(dev), torch.from_numpy(box).to(dev)
+            if self._detections is None:
+                img = np.empty(n, np.int32); cls = np.empty(n, np.int32); conf = np.empty(n, np.float32); box = np.empty((n, 4), np.float32)
+                o = 0
+                for c in range(1, nC + 1):
+                    for p in self.prediction_results[c]:
+                        img[o] = id_index[str(p[0])]; cls[o] = c; conf[o] = p[1]; box[o] = p[2:6]
+                        o += 1
+                t_img, t_cls = torch.from_numpy(img).to(dev), torch.from_numpy(cls).to(dev)
+                t_conf, t_box = torch.from_numpy(conf).to(dev), torch.from_numpy(box).to(dev)
             # order 1: (class, confidence desc), stable: two stable sorts, least significant key first
             ord_conf = torch.sort(-t_conf, stable=True).indices                 # by confidence desc (ties keep the input order)
             ord1 = ord_conf[torch.sort(t_cls[ord_conf].long(), stable=True).indices]     # then by class (stable): (class, conf desc)
@@ -216,6 +252,46 @@ class Evaluator:
         self.cumulative_true_positives, self.cumulative_false_positives = ctp_all, cfp_all
         if ret:
             return tp_all, fp_all, ctp_all, cfp_all
+
+    def _flat_device_predictions(self, id_index):
+        """The device results in the order the list path flattens ``prediction_results`` to: class-major (a stable sort by
+        class), collection order inside a class, values cast to float32 as that path does.  Returns the per-class counts (host)
+        and the image (``id_index`` of its id), class, confidence and box tensors."""
+        import torch
+        nC = self.n_classes
+        img, cls, conf, box = self._detections.device()
+        keep = (cls >= 1) & (cls <= nC)
+        img, cls, conf, box = img[keep], cls[keep], conf[keep], box[keep]
+        order = torch.sort(cls, stable=True).indices
+        remap = torch.from_numpy(np.asarray([id_index[str(i)] for i in self._detections.image_ids], dtype=np.int32)).to(img.device)
+        t_img = remap[img[order].long()].contiguous()
+        t_cls = cls[order].contiguous()
+        dt = torch.float32 if self._detections.dtype == np.float32 else torch.float64
+        t_conf = conf[order].to(dt).to(torch.float32).contiguous()
+        t_box = box[order].to(dt).to(torch.float32).contiguous()
+        counts = torch.bincount(cls.long(), minlength=nC + 1).cpu().numpy().tolist()
+        counts[0] = 0
+        return counts, t_img, t_cls, t_conf, t_box
+
+    def write_predictions_to_txt(self, classes=None, out_file_prefix='comp3_det_test_', verbose=True):
+        """Reference :426-475: one Pascal VOC results file per class, ``<image id as %06d> <confidence rounded to 4> <xmin> <ymin>
+        <xmax> <ymax>`` per line, written with ``str`` of the stored values."""
+        if self.prediction_results is None:
+            raise ValueError("There are no prediction results. You must run `predict_on_dataset()` before calling this method.")
+        for class_id in range(1, self.n_classes + 1):
+            if verbose:
+                print("Writing results file for class {}/{}.".format(class_id, self.n_classes))
+            class_suffix = '{:04d}'.format(class_id) if classes is None else classes[class_id]
+            lines = []
+            for prediction in self.prediction_results[class_id]:
+                prediction_list = list(prediction)
+                prediction_list[0] = '{:06d}'.format(int(prediction_list[0]))
+                prediction_list[1] = round(prediction_list[1], 4)
+                lines.append(' '.join(map(str, prediction_list)) + '\n')
+            with open('{}{}.txt'.format(out_file_prefix, class_suffix), 'w') as f:
+                f.write(''.join(lines))
+        if verbose:
+            print("All results files saved.")
 
     # -- precision / recall / AP: the reference's NumPy expressions (:738-905) -----------------------------
     def compute_precision_recall(self, verbose=True, ret=False):
