@@ -209,7 +209,7 @@ __device__ __forceinline__ void ld_f8(const float* p, float (&v)[8]) {
 enum { kSingle = 0, kSplitXS = 2 };
 static constexpr int kConvThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma consumers of rows [0, 64) / [64, 128)
 
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the two consumer warpgroups
+__device__ __forceinline__ void consumer_sync() { named_bar_sync<1, 256>(); }   // the two consumer warpgroups
 
 // The 8 accumulator columns [8j, 8j + 8) of a quad's rows, j = jp + (q & 1), row half h = q >> 1, gathered into lane q (= lane % 4)
 // of the quad: a 4 x 4 transpose of float2 pairs.  Lane p holds columns 8j + 2p + {0, 1} of rows r and r + 8 (d[4j + 2h + e]).
@@ -248,10 +248,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const uint32_t b_off = (uint32_t)kATile * (split ? 2u : 1u);            // stage: A_hi | A_lo | W_hi | W_lo
   const uint32_t stage = b_off + kBTile * (split ? 2u : 1u);
   const uint32_t ring = max(stage * (uint32_t)S, ((uint32_t)kBM * (BN + kAccPad) + 32u) * 4u);
-  const uint32_t bar_base = smem_base + ring;
-  auto full = [&](uint32_t s) { return bar_base + 8u * s; };
-  auto empty = [&](uint32_t s) { return bar_base + 8u * ((uint32_t)S + s); };
-  const uint32_t staged_free = bar_base + 16u * (uint32_t)S;              // staged epilogues: the tile over the ring has been read
+  const MbarRing bars{smem_base + ring, S};
+  const uint32_t staged_free = bars.end();                                 // staged epilogues: the tile over the ring has been read
   float* s_acc = reinterpret_cast<float*>(smem_al);                       // staged epilogues, after a tile's K loop: [128][BN + kAccPad]
   float* s_bias = reinterpret_cast<float*>(smem_al + ring + 256);
   float* s_scale = s_bias + BN;
@@ -263,9 +261,9 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   if (tid == 0) {
     prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_b_hi);
     if (split) { prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_lo); }
-    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }   // empty: one arrival per consumer warp
+    bars.init(1, 8);                                                       // empty: one arrival per consumer warp
     mbar_init(staged_free, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -283,7 +281,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 
   if (wg == 0) {
     // ===================== producer: one thread walks the tile schedule and keeps the ring full across tile boundaries =====
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    setmaxnreg_dec<40>();
     if (tid != 0) return;
     uint32_t g = 0;                                                        // ring uses so far (slot = g % S, phase = g / S)
     uint32_t lt = 0;                                                       // tiles of this CTA so far
@@ -294,18 +292,17 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       if (staged && lt > 0) mbar_wait(staged_free, (lt - 1) & 1u);
       // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +128) of the activation matrix
       for (int i = 0; i < nk; ++i) {
-        const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
-        mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
+        const uint32_t s = bars.wait_empty(g + (uint32_t)i);
         const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
         const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
         const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
         const uint32_t dst = smem_base + stage * s;
-        mbar_expect_tx(full(s), stage);
-        tma_load_2d(dst, &tm_a_hi, kb * kBK, row, full(s));
-        tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, full(s));
+        mbar_expect_tx(bars.full(s), stage);
+        tma_load_2d(dst, &tm_a_hi, kb * kBK, row, bars.full(s));
+        tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, bars.full(s));
         if (split) {
-          tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, full(s));
-          tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, full(s));
+          tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, bars.full(s));
+          tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, bars.full(s));
         }
       }
       g += (uint32_t)nk;
@@ -314,7 +311,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   }
 
   // ===================== consumers: warpgroup cw computes rows [64 cw, +64) of every tile =====================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  setmaxnreg_inc<232>();
   const int cw = wg - 1, ctid = tid - 128, cwarp = (tid >> 5) & 3;
   uint32_t g = 0;
   float acc[BN / 2], accx[split ? BN / 2 : 1];
@@ -331,7 +328,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     // k-iteration j's MMAs are done: its stage goes back to the producer
     auto release = [&](int j) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(empty((g + (uint32_t)j) % (uint32_t)S));
+      if (lane == 0) bars.release(g + (uint32_t)j);
     };
     // (the first k-step overwrites the accumulators; zeroing them here only ends their live range at the previous epilogue)
 #pragma unroll
@@ -344,8 +341,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     // the zeros of a padded operand), so the loop body has no data-dependent branch around the wgmma.  One group stays in flight:
     // the MMAs of iteration i are issued before the stage of iteration i-1 is released.
     for (int i = 0; i < nk; ++i) {
-      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
-      mbar_wait(full(s), (gi / (uint32_t)S) & 1u);
+      const uint32_t s = bars.wait_full(g + (uint32_t)i);
       const uint32_t a_hi = smem_base + stage * s + (uint32_t)cw * (kATile / 2), b_hi = smem_base + stage * s + b_off;
       constexpr uint64_t kDesc = wgmma_desc_hi(16);
       wgmma_fence();

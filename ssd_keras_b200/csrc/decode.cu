@@ -23,6 +23,7 @@
 // the full multi-band scan in a third launch whose other CTAs exit at once, and the image's top-k is recomputed.
 // Arithmetic follows the reference operation order with non-contracting intrinsics.
 #include "common.cuh"
+#include "rn.cuh"
 #include <cmath>
 
 using namespace ssdk;
@@ -211,15 +212,6 @@ __device__ void bitonic_sort(u64* keys, int count) {
 // IoU suppression rules on "prepared" boxes (coordinates + area computed once per box)
 // ---------------------------------------------------------------------------------------------
 template <typename T> struct PBox { T x0, y0, x1, y1, a; };
-
-__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-__device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
 
 // std::min / std::max exactly as the TF kernel uses them: NaN handling depends on the argument order.
 __device__ __forceinline__ float tf_min(float a, float b) { return (b < a) ? b : a; }

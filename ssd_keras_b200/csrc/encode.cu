@@ -29,6 +29,7 @@
 // Exactness: every decision is taken on float64 values computed with the reference's operation order; float32 is only
 // used for bounds that can skip work, never for a comparison the result depends on.
 #include "common.cuh"
+#include "tc.cuh"
 #include <climits>
 #include <cmath>
 #include <vector>
@@ -250,12 +251,6 @@ __device__ __forceinline__ void warp_argmax(double& val, int& idx) {
   }
 }
 
-__device__ __forceinline__ float rcp_approx(float x) {          // MUFU.RCP: at most 1 ulp off
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-
 // ------------------------------------------------------------------------------------------
 // tiles
 // ------------------------------------------------------------------------------------------
@@ -280,9 +275,7 @@ __device__ __forceinline__ float slice_iou_bound(const float4 k0, const float4 k
   const float oy = fmaxf(fminf(fminf(k1.y, __fsub_ru(gf.w, gf.y)), fminf(__fsub_ru(k0.w, gf.y), __fsub_ru(gf.w, k0.y))), 0.f);
   const float inter = __fmul_ru(ox, oy);
   const float un = fmaxf(__fsub_rd(__fadd_rd(k1.z, g_area), inter), 1e-30f);
-  float r;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(un));
-  return __fmul_ru(__fmul_ru(inter, r), 1.0f + 4.76837158203125e-7f);          // (1 + 2^-21): the reciprocal's ulp
+  return __fmul_ru(__fmul_ru(inter, rcp_approx(un)), 1.0f + 4.76837158203125e-7f);          // (1 + 2^-21): the reciprocal's ulp
 }
 
 // One warp: the exact best anchor of `gb` over ALL slices of all tiles, ignoring `removed`, starting from a known candidate
@@ -410,7 +403,7 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
   unsigned long long t_prev = 0;
   auto lap = [&](int slot) {                                  // SSDK_ENC_DEBUG=2: time since the previous lap -> prof[slot]
     if (sc.prof && tid == 0) {
-      unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+      const unsigned long long t = globaltimer();
       if (slot >= 0) atomicAdd(sc.prof + slot, t - t_prev);
       t_prev = t;
     }
@@ -806,7 +799,7 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
       if (lane == 0) { s_wV[w * Gs + g] = __hiloint2double((int)mh, (int)ml); s_wI[w * Gs + g] = (int)mi; }
     }
     // the previous tile's bulk store must have finished reading the staging rows before they are rewritten
-    if (store_pending && tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    if (store_pending && tid == 0) bulk_wait_read<0>();
     __syncthreads();
     if (tid == 0) *s_nitems = 0;                                  // (next appended after the barrier that follows the row stores)
     // ---- per (gt, tile) results -> global (consecutive threads write consecutive boxes) ----
@@ -846,7 +839,7 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
       }
       if (out_match) out_match[(size_t)b * p.P + a] = (dec.match_g >= 0) ? dec.match_g : (dec.neutral ? -2 : -1);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of the rows -> visible to the bulk copy engine
+    fence_proxy_async();                                          // generic-proxy writes of the rows -> visible to the bulk copy engine
     __syncthreads();
     // ---- 5. rows leave: one bulk store per contiguous run of priors ----
     // (runs whose byte ranges are not 16-byte aligned fall back to coalesced stores by all threads; whether a tile has any is
@@ -865,11 +858,10 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
           const int start = ts.linear ? tile * kTile : rn[1 + 2 * r];
           const int len = ts.linear ? lin_len : rn[2 + 2 * r];
           float* dst = out_y + ((size_t)b * p.P + start) * W;
-          asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                       ::"l"(dst), "r"((uint32_t)__cvta_generic_to_shared(rows + (size_t)slot0 * W)), "r"((uint32_t)((size_t)len * W * 4)) : "memory");
+          bulk_store(dst, smem_u32(rows + (size_t)slot0 * W), (uint32_t)((size_t)len * W * 4));
           slot0 += len;
         }
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        bulk_commit();
       }
       issued = true;
     } else {
@@ -889,10 +881,10 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
   }
   // ---- 6. last CTA of the image: bipartite matching ----
   if (sc.dbg & 1) {                                             // timing experiments only: no matching stage (wrong results)
-    if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    if (tid == 0) bulk_wait_read<0>();
     return;
   }
-  if (tid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (tid == 0) bulk_wait<0>();
   if (G <= 0) return;
   __syncthreads();                                              // every thread's global writes happen-before thread 0's fence
   if (tid == 0) {

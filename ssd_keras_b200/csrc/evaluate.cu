@@ -13,6 +13,7 @@
 // Sorting (two stable key sorts) is done by the caller; precision / recall / AP are a few vector operations on the cumulative
 // counts (host, same NumPy expressions as the reference).
 #include "common.cuh"
+#include "rn.cuh"
 #include <climits>
 #include <cmath>
 
@@ -117,20 +118,8 @@ __global__ void __launch_bounds__(1024) eval_cumsum_kernel(const int* __restrict
 // the keep flags gives every kept row its slot, so the output keeps the reference's order without atomics.
 struct CollectCols { int c[10]; };   // class, conf, xmin, ymin, xmax, ymax, inverter ymin, ymax, xmin, xmax
 
-template <typename T> __device__ __forceinline__ T mul_rn(T a, T b);
-template <> __device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-template <> __device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
-template <typename T> __device__ __forceinline__ T add_rn(T a, T b);
-template <> __device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-template <> __device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
-template <typename T> __device__ __forceinline__ T div_rn(T a, T b);
-template <> __device__ __forceinline__ float div_rn(float a, float b) { return __fdiv_rn(a, b); }
-template <> __device__ __forceinline__ double div_rn(double a, double b) { return __ddiv_rn(a, b); }
-__device__ __forceinline__ float rint_t(float v) { return rintf(v); }      // half to even, like np.round
-__device__ __forceinline__ double rint_t(double v) { return rint(v); }
-
 // round(numpy_scalar, n) for n > 0: multiply by 10^n in the scalar's type, rint, divide
-template <typename T> __device__ __forceinline__ T round_decimals(T v, T f) { return div_rn(rint_t(mul_rn(v, f)), f); }
+template <typename T> __device__ __forceinline__ T round_decimals(T v, T f) { return div_rn(rint_rn(mul_rn(v, f)), f); }
 
 template <typename T>
 __device__ __forceinline__ void collect_row(const float* __restrict__ r, const double* __restrict__ inv, const CollectCols& cc, int pad, int decimals,
@@ -139,8 +128,8 @@ __device__ __forceinline__ void collect_row(const float* __restrict__ r, const d
 #pragma unroll
   for (int k = 0; k < 6; ++k) v[k] = (T)r[k];
   const T ry = (T)inv[0], rx = (T)inv[1];                      // the Python float ratio as NumPy rounds it for this path
-  v[cc.c[6]] = rint_t(mul_rn(v[cc.c[6]], ry)); v[cc.c[7]] = rint_t(mul_rn(v[cc.c[7]], ry));
-  v[cc.c[8]] = rint_t(mul_rn(v[cc.c[8]], rx)); v[cc.c[9]] = rint_t(mul_rn(v[cc.c[9]], rx));
+  v[cc.c[6]] = rint_rn(mul_rn(v[cc.c[6]], ry)); v[cc.c[7]] = rint_rn(mul_rn(v[cc.c[7]], ry));
+  v[cc.c[8]] = rint_rn(mul_rn(v[cc.c[8]], rx)); v[cc.c[9]] = rint_rn(mul_rn(v[cc.c[9]], rx));
   if (pad) {                                                   // CropPad's inverter: even + 0 matters, it turns -0.0 into 0.0
     const T oy = (T)inv[2], ox = (T)inv[3];
     v[cc.c[6]] = add_rn(v[cc.c[6]], oy); v[cc.c[7]] = add_rn(v[cc.c[7]], oy);

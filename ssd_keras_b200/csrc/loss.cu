@@ -77,11 +77,6 @@ struct Sel {                           // what phases C / D know about the hard-
 };
 
 // ---- shared-memory tile loads ----------------------------------------------------------------------------------
-__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-
 // Loads rows [row0, row0+rows) of y_true and y_pred (W floats each) into the stage buffers.  Bulk path: one elected thread
 // issues two copies that complete on the stage's mbarrier; fallback: all threads copy and the caller's __syncthreads publishes.
 __device__ __forceinline__ void tile_load(const LossArgs& a, size_t flat_row0, int rows, float* s_t, float* s_p, uint32_t bar) {
@@ -392,7 +387,7 @@ __device__ void phase_d(const LossArgs& a, const Sel& s, bool ordered_ties, long
       if (tid == 0) a.negpart[t] = v;
     }
     if (a.out_grad) {
-      if (store_pending) { if (tid == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+      if (store_pending) { if (tid == 0) bulk_wait_read<0>(); }
       if (a.bulk_ok) mbar_wait(bar0, parity);
       __syncthreads();
       parity ^= 1u;
@@ -420,22 +415,19 @@ __device__ void phase_d(const LossArgs& a, const Sel& s, bool ordered_ties, long
 #pragma unroll
         for (int j = 4; j < 12; ++j) g[C + j] = 0.f;
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      fence_proxy_async();
       __syncthreads();
       float* dst = a.out_grad + flat0 * W;
       const size_t n_f = (size_t)rows * W;
       if (a.bulk_ok && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) && (((n_f * 4) & 15) == 0)) {
-        if (tid == 0) {
-          asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(s_g)), "r"((uint32_t)(n_f * 4)) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
+        if (tid == 0) { bulk_store(dst, smem_u32(s_g), (uint32_t)(n_f * 4)); bulk_commit(); }
         store_pending = true;
       } else {
         for (size_t i = tid; i < n_f; i += kRows) dst[i] = s_g[i];
       }
     }
   }
-  if (tid == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+  if (tid == 0) bulk_wait<0>();
   if (!a.out_loss) return;
   // last CTA: per-image totals in a fixed order
   __threadfence();
@@ -479,7 +471,7 @@ __device__ __forceinline__ uint32_t setup_barriers(uint64_t* bars) {
   const uint32_t bar0 = smem_u32(bars);
   if (threadIdx.x == 0) {
     mbar_init(bar0, 1); mbar_init(bar0 + 8, 1); mbar_init(bar0 + 16, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
   return bar0;
@@ -492,7 +484,7 @@ __global__ void __launch_bounds__(kRows) ssd_loss_kernel(const __grid_constant__
   __shared__ long long s_scan[kRows];
   cg::grid_group grid = cg::this_grid();
   auto stamp = [&](int i) {
-    if (a.dbg_times && blockIdx.x == 0 && threadIdx.x == 0) { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); a.dbg_times[i] = t; }
+    if (a.dbg_times && blockIdx.x == 0 && threadIdx.x == 0) a.dbg_times[i] = globaltimer();
   };
   const uint32_t bar0 = setup_barriers(s_bars);
   stamp(0);

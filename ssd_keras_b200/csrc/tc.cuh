@@ -1,5 +1,7 @@
-// PTX wrappers shared by the tensor-core kernels (conv.cu, wgrad.cu): mbarriers, TMA loads, Hopper wgmma descriptors / issue /
-// commit / wait.
+// The project's inline PTX, one __forceinline__ wrapper per instruction, and the asynchronous-copy pipeline built from it:
+// mbarriers and the MbarRing stage ring, TMA and cp.async.bulk copies, Hopper wgmma descriptors / issue / commit / wait, register
+// reallocation, named barriers, and a few single instructions.  Users: conv.cu and wgrad.cu (TMA ring feeding wgmma), loss.cu
+// (bulk tile loads on mbarriers, bulk stores), encode.cu (bulk stores, rcp.approx).  No other source file holds inline PTX.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -13,6 +15,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
+// after the inits, before the __syncthreads that publishes them: the barriers are visible to the async proxy (TMA, bulk copies)
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -33,6 +37,35 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (spins > 1024 && (spins & 1023) == 0 && clock64() - t0 > 4000000000ll) __trap();
   }
 }
+
+// S shared-memory stages, each guarded by a "full" mbarrier (the stage's data has landed) and an "empty" one (its consumers are
+// done with it): S full barriers at `base`, then S empty ones, 8 bytes each.  Use g = 0, 1, 2, ... of the ring takes slot g % S
+// in phase (g / S) & 1.  The producer waits on the empty barrier's previous phase, so the first round passes at once.
+struct MbarRing {
+  uint32_t base;
+  int S;                                                   // stages (the slot and phase arithmetic below is unsigned)
+  __device__ __forceinline__ uint32_t full(uint32_t s) const { return base + 8u * s; }
+  __device__ __forceinline__ uint32_t empty(uint32_t s) const { return base + 8u * (S + s); }
+  __device__ __forceinline__ uint32_t end() const { return base + 16u * S; }          // the first byte after the ring
+  __device__ __forceinline__ void init(uint32_t full_count, uint32_t empty_count) const {
+    for (int s = 0; s < S; ++s) { mbar_init(full(s), full_count); mbar_init(empty(s), empty_count); }
+  }
+  // consumer: wait until the data of use g has landed; returns its slot
+  __device__ __forceinline__ uint32_t wait_full(uint32_t g) const {
+    const uint32_t s = g % S;
+    mbar_wait(full(s), (g / S) & 1u);
+    return s;
+  }
+  // producer: wait until use g - S of the same slot has been released; returns the slot
+  __device__ __forceinline__ uint32_t wait_empty(uint32_t g) const {
+    const uint32_t s = g % S;
+    mbar_wait(empty(s), ((g / S) & 1u) ^ 1u);
+    return s;
+  }
+  // one consumer arrival: done with use g
+  __device__ __forceinline__ void release(uint32_t g) const { mbar_arrive(empty(g % S)); }
+};
+
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, int c0, int c1, uint32_t bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1) : "memory");
@@ -44,8 +77,49 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
-// generic-proxy accesses to shared memory -> ordered before later async-proxy ones (TMA writes, wgmma reads)
+// generic-proxy accesses to shared memory -> ordered before later async-proxy ones (TMA writes, wgmma reads, bulk stores)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// cp.async.bulk without a tensor map: one contiguous range, 16-byte aligned, a multiple of 16 bytes.
+// global -> shared, completing on mbarrier `bar` (armed with mbar_expect_tx for the bytes)
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// shared -> global, into this thread's open bulk group; bulk_commit closes the group
+__device__ __forceinline__ void bulk_store(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N committed bulk groups of this thread still in flight (bulk_wait) / still reading shared memory (bulk_wait_read)
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+
+// warpgroup register reallocation (every warp of the warpgroup executes it): lower / raise this warpgroup's registers to N
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// named barrier ID (1..15; 0 is __syncthreads) over the N threads (a multiple of 32) that use it
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_sync() { asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory"); }
+
+// p[0] += a, p[1] += b atomically in global memory, no return value (p 8-byte aligned)
+__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ float rcp_approx(float x) {          // MUFU.RCP: at most 1 ulp off
+  float r;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+  return r;
+}
+__device__ __forceinline__ unsigned long long globaltimer() {   // nanoseconds; for timing experiments
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
 
 // ------------------------------------------------------------------------------------------------
 // wgmma (sm_90a).  Shared-memory matrix descriptor, 128-byte swizzle: start address >> 4 at [0,14), leading byte offset >> 4 at

@@ -21,10 +21,6 @@ namespace {
 
 constexpr int kBoxA = 64 * 128;            // one {64 channels x 64 pixels} box: 8 KB
 
-__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
-}
-
 template <int BNc, bool SPLIT>
 __global__ void __launch_bounds__(256, 1)
 wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tm_g_hi, const __grid_constant__ CUtensorMap tm_g_lo,
@@ -41,14 +37,12 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tm_g_hi, const __grid_con
   const uint32_t a_plane = 2u * kBoxA, b_plane = (uint32_t)nB * kBoxA;
   const uint32_t b_off = a_plane * (split ? 2u : 1u);
   const uint32_t stage = (a_plane + b_plane) * (split ? 2u : 1u);
-  const uint32_t bar_base = smem_base + stage * S;
-  auto full = [&](uint32_t s) { return bar_base + 8u * s; };
-  auto empty = [&](uint32_t s) { return bar_base + 8u * ((uint32_t)S + s); };
+  const MbarRing bars{smem_base + stage * S, S};
 
   if (tid == 0) {
     prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_x_hi);
-    for (int s = 0; s < S; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    bars.init(1, 8);
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -68,34 +62,32 @@ wgrad_wgmma_kernel(const __grid_constant__ CUtensorMap tm_g_hi, const __grid_con
     const int p0 = ks * args.patches_per_split, p1 = min(args.total_patches, p0 + args.patches_per_split);
     const int nk = p1 - p0;
     auto issue = [&](int i) {
-      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
-      mbar_wait(empty(s), ((gi / (uint32_t)S) & 1u) ^ 1u);
+      const uint32_t s = bars.wait_empty(g + (uint32_t)i);
       const int p = p0 + i;
       const int n = p / patches_per_img; const int q = p - n * patches_per_img;
       const int py = q / args.px_tiles, px = q - py * args.px_tiles;
       const int x0 = px * args.bw, y0 = py * args.bh;
       const uint32_t dst = smem_base + stage * s;
-      mbar_expect_tx(full(s), args.tx_bytes);
+      mbar_expect_tx(bars.full(s), args.tx_bytes);
       for (int pl = 0; pl < (split ? 2 : 1); ++pl) {
         const CUtensorMap* tg = pl ? &tm_g_lo : &tm_g_hi;
         const CUtensorMap* tx = pl ? &tm_x_lo : &tm_x_hi;
         const uint32_t da = dst + pl * a_plane, db = dst + b_off + pl * b_plane;
-        for (int a = 0; a < nA; ++a) tma_load_4d(da + a * kBoxA, tg, co0 + 64 * a, x0 + args.g_pad, y0 + args.g_pad, n, full(s));
+        for (int a = 0; a < nA; ++a) tma_load_4d(da + a * kBoxA, tg, co0 + 64 * a, x0 + args.g_pad, y0 + args.g_pad, n, bars.full(s));
         for (int j = 0; j < nB; ++j)
-          tma_load_4d(db + j * kBoxA, tx, ci0 + 64 * j, x0 + kw * args.dil + args.x_off, y0 + kh * args.dil + args.y_off, n, full(s));
+          tma_load_4d(db + j * kBoxA, tx, ci0 + 64 * j, x0 + kw * args.dil + args.x_off, y0 + kh * args.dil + args.y_off, n, bars.full(s));
       }
     };
     auto release = [&](int j) {                                  // patch j's MMAs are done: refill its stage with patch j + S
       __syncwarp();
-      if (lane == 0) mbar_arrive(empty((g + (uint32_t)j) % (uint32_t)S));
+      if (lane == 0) bars.release(g + (uint32_t)j);
       if (tid == 0 && j + S < nk) issue(j + S);
     };
     if (tid == 0)
       for (int i = 0; i < min(S, nk); ++i) issue(i);
     wgmma_fence_acc(acc);
     for (int i = 0; i < nk; ++i) {                                 // one wgmma group stays in flight
-      const uint32_t gi = g + (uint32_t)i, s = gi % (uint32_t)S;
-      mbar_wait(full(s), (gi / (uint32_t)S) & 1u);
+      const uint32_t s = bars.wait_full(g + (uint32_t)i);
       constexpr uint64_t kDescA = wgmma_desc_hi(kBoxA), kDescB = wgmma_desc_hi(kBoxA);
       const uint32_t a_hi = smem_base + stage * s + a_box, b_hi = smem_base + stage * s + b_off;
       wgmma_fence();
