@@ -819,6 +819,9 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
     }
     // ---- 4. this anchor's row ----
     if (prev_one >= 0) { rows[prev_one] = 0.f; prev_one = -1; }   // (the previous tile's bulk store has finished reading: barrier above)
+    // spatial tiles of different shapes map threads to staging slots differently: this thread's previous slot may now be
+    // another thread's, whose 1 must not be cleared after it is set
+    if (!ts.linear && tile != tile0) __syncthreads();
     if (live) {
       RowDecision dec{-1, false};
       double val = best;
