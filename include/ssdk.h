@@ -169,7 +169,12 @@ int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const double* boxes
  * ------------------------------------------------------------------------------------------ */
 typedef enum { SSDK_BOXOP_END = 0, SSDK_BOXOP_CROP_PAD = 1, SSDK_BOXOP_FLIP_H = 2, SSDK_BOXOP_FLIP_V = 3, SSDK_BOXOP_RESIZE = 4,
                SSDK_BOXOP_FILTER = 5, SSDK_BOXOP_TRANSLATE = 6, SSDK_BOXOP_SCALE = 7, SSDK_BOXOP_ROTATE = 8,
-               SSDK_BOXOP_OVERLAP = 9, SSDK_BOXOP_CLIP = 10 } ssdk_box_op_kind;
+               SSDK_BOXOP_OVERLAP = 9, SSDK_BOXOP_CLIP = 10,
+               /* photometric ops, from 16 on (11-15 are unassigned: ssdk_assemble_images rejects them as unknown): images only; the
+                * box kernel skips them */
+               SSDK_BOXOP_TO_FLOAT32 = 16, SSDK_BOXOP_TO_UINT8 = 17, SSDK_BOXOP_BRIGHTNESS = 18, SSDK_BOXOP_CONTRAST = 19,
+               SSDK_BOXOP_SATURATION = 20, SSDK_BOXOP_HUE = 21, SSDK_BOXOP_RGB2HSV = 22, SSDK_BOXOP_HSV2RGB = 23,
+               SSDK_BOXOP_CHANNEL_SWAP = 24 } ssdk_box_op_kind;
 typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
@@ -190,6 +195,20 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
  *   ROTATE    an exact signed axis permutation (cv2's fixed-point map is checked on the host to have fraction 0 everywhere),
  *             black where the inverse map leaves the source
  *   FILTER, OVERLAP, CLIP   nothing to do for images
+ * The photometric ops (object_detection_2d_photometric_ops.py) form a prefix of the list, run by one launch of
+ * photometric_kernel in front of the assembly kernel, uint8 in and uint8 h x w x 3 out, bit for bit what NumPy and OpenCV 4.13
+ * compute (oracle/photoops.py):
+ *   TO_FLOAT32 / TO_UINT8    ConvertDataType: astype(float32) / np.round(x, 0).astype(uint8) (round half to even)
+ *   BRIGHTNESS a0=delta      np.clip(image + delta, 0, 255); a0 is rounded to float32, as NumPy does with a Python float
+ *   CONTRAST   a0=factor     np.clip(127.5 + factor * (image - 127.5), 0, 255), every step rounded to float32
+ *   SATURATION a0=factor     channel 1: np.clip(s * factor, 0, 255)
+ *   HUE        a0=delta      channel 0: (h + delta) % 180.0, NumPy's float32 remainder
+ *   RGB2HSV / HSV2RGB        uint8 cv2.cvtColor.  HSV2RGB is cv2's float32 code on a CPU with AVX2, which truncates in its
+ *                            32-pixel vector loop and rounds in the scalar loop that finishes each row: columns >= w / 32 * 32
+ *                            round, the others truncate
+ *   CHANNEL_SWAP a0..a2=order  image[:, :, order]
+ * Gamma, histogram equalisation and conversions to GRAY are not covered; the random draws stay with the caller (an op that a
+ * draw skipped is absent from the list).
  * src_dev: the B uint8 images packed back to back, image b at bytes src_offsets_host[b] .. src_offsets_host[b+1] (host, [B+1]),
  * of shape src_hwc_host[3b..3b+2] = h, w, c with c in {1, 3, 4}.  ops_host: [B*max_ops] on the HOST (a list ends at
  * SSDK_BOXOP_END or after max_ops entries).  out_dev: [B*out_h*out_w*3] float32.
@@ -200,7 +219,13 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
  * ranges (canvas below 32767); at most one resampling step (RESIZE or SCALE); no crop / pad / flip / translate / rotate after
  * a RESIZE (after a SCALE they are applied to its output); the final size out_h x out_w; a supported interpolation code; and one
  * background colour per list: every pad or translate that brings in background, every SCALE, and a ROTATE whose map leaves
- * the source (black) must agree (bands of different colours are not represented).
+ * the source (black) must agree (bands of different colours are not represented).  Photometric ops: all of them before the
+ * first op that changes the image geometry; at most 16; BRIGHTNESS / CONTRAST / SATURATION / HUE only between a TO_FLOAT32 and
+ * the next TO_UINT8, the colour conversions and the end of the prefix only in the uint8 state; factors > 0, -180 <= hue delta
+ * <= 180 (the reference's own ValueErrors), brightness delta finite, the swap order a permutation of (0, 1, 2).
+ * Images with photometric ops are written, converted to 3 channels, to a scratch buffer owned by the context (grown when needed,
+ * freed with the context) and assembled from there; the others are read from src_dev as before, and a call without photometric
+ * ops launches and allocates nothing more than it did.
  * The integer ops before the resampling step are composed on the host into one signed-permutation map per image, those after a
  * SCALE into a second one; one kernel launch evaluates the whole list without an intermediate image.  The descriptors go to the
  * device with one asynchronous copy from pinned staging owned by the context (a ring of four buffers: the call waits only if the

@@ -52,6 +52,8 @@ class BoxOp(C.Structure):
 
 BOXOP_END, BOXOP_CROP_PAD, BOXOP_FLIP_H, BOXOP_FLIP_V, BOXOP_RESIZE, BOXOP_FILTER = range(6)
 BOXOP_TRANSLATE, BOXOP_SCALE, BOXOP_ROTATE, BOXOP_OVERLAP, BOXOP_CLIP = range(6, 11)
+(BOXOP_TO_FLOAT32, BOXOP_TO_UINT8, BOXOP_BRIGHTNESS, BOXOP_CONTRAST, BOXOP_SATURATION, BOXOP_HUE, BOXOP_RGB2HSV, BOXOP_HSV2RGB,
+ BOXOP_CHANNEL_SWAP) = range(16, 25)         # photometric ops: images only (ssdk_assemble_images)
 INTER_NEAREST, INTER_LINEAR = 0, 1          # cv2's codes, in RESIZE's flag bits 8-15 (ssdk_assemble_images)
 
 

@@ -18,8 +18,12 @@
 //   image_assemble_kernel  one CTA per (output row, image): every output pixel is traced back through the resize to at most
 //                          four canvas taps, and each tap through the composed crop / pad / flip map to a source pixel or to
 //                          the background colour.  No intermediate image exists.
+//   photometric_kernel     the photometric prefix of the op lists (ConvertDataType, Brightness, Contrast, Saturation, Hue,
+//                          ConvertColor RGB <-> HSV, ChannelSwap; object_detection_2d_photometric_ops.py), one launch in front of
+//                          image_assemble_kernel: uint8 in, uint8 h x w x 3 out, restated in oracle/photoops.py.
 // The file is compiled with --fmad=false; the float64 resize coordinates also spell their roundings out (__dmul_rn / __dadd_rn).
 #include "common.cuh"
+#include "rn.cuh"
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -354,6 +358,237 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8
   }
 }
 
+// ---- the photometric prefix ----
+constexpr int kPhotoThreads = 256;
+constexpr int kPhotoMaxStages = 16;
+constexpr int kPhotoGroupsPerThread = 4;       // groups of 4 pixels a thread takes, when the grid is sized for the largest image
+
+struct PhotoStage { int op; float a; };        // CHANNEL_SWAP keeps its order in op bits 8-13
+struct PhotoDesc {
+  long long src_off;                           // the image in the packed source buffer
+  long long dst_off;                           // its 3-channel result in the scratch buffer, 16-byte aligned
+  int n_px, w, c, n_stages;
+  PhotoStage st[kPhotoMaxStages];
+};
+
+// The aligned 32-bit word at q, of which only the bytes inside the image [lo, hi) may be read (the packed images start and end
+// at arbitrary byte offsets); bytes outside read as 0.
+__device__ __forceinline__ uint32_t image_word(const uint8_t* q, const uint8_t* lo, const uint8_t* hi) {
+  if (q >= lo && q + 4 <= hi) return *reinterpret_cast<const uint32_t*>(q);
+  uint32_t v = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (q + k >= lo && q + k < hi) v |= (uint32_t)q[k] << (8 * k);
+  return v;
+}
+
+__device__ __forceinline__ float clip255(float x) { return fminf(fmaxf(x, 0.f), 255.f); }   // np.clip(x, 0, 255)
+__device__ __forceinline__ float pick3(int k, float x0, float x1, float x2) { return k == 0 ? x0 : k == 1 ? x1 : x2; }
+
+// uint8 cv2.cvtColor(COLOR_RGB2HSV): integer code; sdiv[i] = rint((255 << 12) / i), hdiv[i] = rint((180 << 12) / (6 i)).
+__device__ __forceinline__ void rgb2hsv_px(float p[3], const int* __restrict__ sdiv, const int* __restrict__ hdiv) {
+  const int r = (int)p[0], g = (int)p[1], b = (int)p[2];
+  const int v = max(max(r, g), b), d = v - min(min(r, g), b);
+  const int s = (d * sdiv[v] + (1 << 11)) >> 12;
+  int h = v == r ? g - b : v == g ? b - r + 2 * d : r - g + 4 * d;
+  h = (h * hdiv[d] + (1 << 11)) >> 12;
+  if (h < 0) h += 180;
+  p[0] = (float)h; p[1] = (float)s; p[2] = (float)v;
+}
+
+// uint8 cv2.cvtColor(COLOR_HSV2RGB) as OpenCV 4.13 computes it with AVX2: float32, the two inner 1 - s * x fused, every other
+// step rounded; the 32-pixel vector loop truncates the result, the scalar loop that finishes a row (`round`) rounds half to even.
+__device__ __forceinline__ void hsv2rgb_px(float p[3], bool round) {
+  const float s = mul_rn(p[1], 1.0f / 255.0f), v = mul_rn(p[2], 1.0f / 255.0f);
+  const float h = mul_rn(p[0], 6.0f / 180.0f);
+  const float ps = truncf(h), f = sub_rn(h, ps);
+  int sector = (int)ps;                                           // H <= 255, so h < 9
+  if (sector >= 6) sector -= 6;
+  const float t1 = mul_rn(v, sub_rn(1.f, s));
+  const float t2 = mul_rn(v, __fmaf_rn(-s, f, 1.f));
+  const float t3 = mul_rn(v, __fmaf_rn(-s, sub_rn(1.f, f), 1.f));
+  float r, g, b;
+  switch (sector) {
+    case 0: r = v; g = t3; b = t1; break;
+    case 1: r = t2; g = v; b = t1; break;
+    case 2: r = t1; g = v; b = t3; break;
+    case 3: r = t1; g = t2; b = v; break;
+    case 4: r = t3; g = t1; b = v; break;
+    default: r = v; g = t1; b = t2; break;
+  }
+  const float x[3] = {mul_rn(r, 255.f), mul_rn(g, 255.f), mul_rn(b, 255.f)};
+#pragma unroll
+  for (int k = 0; k < 3; ++k) p[k] = (float)min(max(round ? __float2int_rn(x[k]) : __float2int_rz(x[k]), 0), 255);
+}
+
+// One CTA column per image with photometric ops (blockIdx.y); a thread takes groups of 4 pixels: 4 * c source bytes from aligned
+// words (any source alignment), 12 result bytes as three aligned words.  A pixel is carried as three float32 values, which hold
+// the uint8 state exactly; the stage list is uniform across the CTA.
+__global__ void __launch_bounds__(kPhotoThreads) photometric_kernel(const uint8_t* __restrict__ src, const PhotoDesc* __restrict__ descs,
+                                                                    uint8_t* __restrict__ dst) {
+  __shared__ int s_sdiv[256], s_hdiv[256];
+  __shared__ PhotoDesc s_d;
+  if (threadIdx.x < sizeof(PhotoDesc) / 4)
+    reinterpret_cast<int*>(&s_d)[threadIdx.x] = reinterpret_cast<const int*>(descs + blockIdx.y)[threadIdx.x];
+  {
+    const int i = threadIdx.x;                                    // rint(N / i) = (2N + i) / (2i): neither quotient has a tie
+    s_sdiv[i] = i ? (2 * (255 << 12) + i) / (2 * i) : 0;
+    s_hdiv[i] = i ? (2 * ((180 << 12) / 6) + i) / (2 * i) : 0;
+  }
+  __syncthreads();
+  const int n_px = s_d.n_px, w = s_d.w, c = s_d.c, n_stages = s_d.n_stages;
+  const uint8_t* lo = src + s_d.src_off;
+  const uint8_t* hi = lo + (size_t)n_px * c;
+  uint8_t* out = dst + s_d.dst_off;
+  const int groups = (n_px + 3) >> 2;
+  const int tail_from = w & ~31;
+  for (int grp = blockIdx.x * kPhotoThreads + threadIdx.x; grp < groups; grp += gridDim.x * kPhotoThreads) {
+    // 4 * c bytes from lo + 4 * c * grp, through the aligned words that hold them
+    const uint8_t* at = lo + (size_t)grp * 4 * c;
+    const int sh = (int)(reinterpret_cast<uintptr_t>(at) & 3);
+    const uint8_t* q = at - sh;
+    uint32_t in[4] = {0, 0, 0, 0};
+    uint32_t prev = image_word(q, lo, hi);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (k < c) {
+        const uint32_t next = image_word(q + 4 * (k + 1), lo, hi);
+        in[k] = __funnelshift_r(prev, next, 8 * sh);
+        prev = next;
+      }
+    }
+    float p[4][3];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        // ConvertTo3Channels: gray is replicated, alpha is dropped
+        const uint32_t gray = (in[0] >> (8 * j)) & 255u, rgba = (in[j] >> (8 * k)) & 255u;
+        const uint32_t rgb = (in[(3 * j + k) >> 2] >> (8 * ((3 * j + k) & 3))) & 255u;
+        p[j][k] = (float)(c == 1 ? gray : c == 4 ? rgba : rgb);
+      }
+    }
+    for (int i = 0; i < n_stages; ++i) {
+      const int code = s_d.st[i].op;
+      const float a = s_d.st[i].a;
+      switch (code & 255) {
+        case SSDK_BOXOP_TO_UINT8:                                 // np.round(image, 0).astype(uint8); the values are in [0, 255]
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { p[j][0] = rint_rn(p[j][0]); p[j][1] = rint_rn(p[j][1]); p[j][2] = rint_rn(p[j][2]); }
+          break;
+        case SSDK_BOXOP_BRIGHTNESS:                               // np.clip(image + delta, 0, 255)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) p[j][k] = clip255(add_rn(p[j][k], a));
+          }
+          break;
+        case SSDK_BOXOP_CONTRAST:                                 // np.clip(127.5 + factor * (image - 127.5), 0, 255)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) p[j][k] = clip255(add_rn(127.5f, mul_rn(a, sub_rn(p[j][k], 127.5f))));
+          }
+          break;
+        case SSDK_BOXOP_SATURATION:                               // image[:, :, 1] = np.clip(image[:, :, 1] * factor, 0, 255)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) p[j][1] = clip255(mul_rn(p[j][1], a));
+          break;
+        case SSDK_BOXOP_HUE:                                      // image[:, :, 0] = (image[:, :, 0] + delta) % 180.0
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {                           // NumPy's remainder: fmod, then the sign of the divisor
+            float m = fmodf(add_rn(p[j][0], a), 180.f);
+            if (m < 0.f) m = add_rn(m, 180.f);
+            p[j][0] = m;
+          }
+          break;
+        case SSDK_BOXOP_RGB2HSV:
+#pragma unroll
+          for (int j = 0; j < 4; ++j) rgb2hsv_px(p[j], s_sdiv, s_hdiv);
+          break;
+        case SSDK_BOXOP_HSV2RGB: {
+          const int x0 = (int)(((long long)grp * 4) % w);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) hsv2rgb_px(p[j], (x0 + j) % w >= tail_from);
+          break;
+        }
+        case SSDK_BOXOP_CHANNEL_SWAP: {                           // image[:, :, order]
+          const int o0 = (code >> 8) & 3, o1 = (code >> 10) & 3, o2 = (code >> 12) & 3;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float x0 = p[j][0], x1 = p[j][1], x2 = p[j][2];
+            p[j][0] = pick3(o0, x0, x1, x2); p[j][1] = pick3(o1, x0, x1, x2); p[j][2] = pick3(o2, x0, x1, x2);
+          }
+          break;
+        }
+        default: break;                                           // TO_FLOAT32: the values are float32 already
+      }
+    }
+    uint32_t o[3] = {0, 0, 0};
+#pragma unroll
+    for (int m = 0; m < 12; ++m) o[m >> 2] |= (uint32_t)p[m / 3][m % 3] << (8 * (m & 3));
+    uint8_t* to = out + (size_t)grp * 12;
+    if (grp * 4 + 4 <= n_px) {
+      uint32_t* t32 = reinterpret_cast<uint32_t*>(to);
+      t32[0] = o[0]; t32[1] = o[1]; t32[2] = o[2];
+    } else {                                                      // the last, partial group
+      const int nb = (n_px - grp * 4) * 3;
+#pragma unroll
+      for (int m = 0; m < 9; ++m)
+        if (m < nb) to[m] = (uint8_t)(o[m >> 2] >> (8 * (m & 3)));
+    }
+  }
+}
+
+bool is_photo(int code) { return code >= SSDK_BOXOP_TO_FLOAT32 && code <= SSDK_BOXOP_CHANNEL_SWAP; }
+
+// The photometric prefix of image b's op list -> its stages; every check the entry point documents.
+int compose_photo(int b, const ssdk_box_op* ops, int max_ops, PhotoDesc* out) {
+  bool geometric = false, is_float = false;
+  int n = 0;
+  for (int i = 0; i < max_ops; ++i) {
+    const ssdk_box_op& op = ops[(size_t)b * max_ops + i];
+    if (op.op == SSDK_BOXOP_END) break;
+    if (!is_photo(op.op)) {
+      geometric = geometric || (op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE && op.op != SSDK_BOXOP_FILTER);
+      continue;
+    }
+    SSDK_REQUIRE(!geometric, "ssdk_assemble_images: image %d, op %d: photometric ops must come before every op that changes the "
+                 "image geometry", b, i);
+    SSDK_REQUIRE(n < kPhotoMaxStages, "ssdk_assemble_images: image %d: more than %d photometric ops", b, kPhotoMaxStages);
+    PhotoStage st{op.op, (float)op.a0};
+    switch (op.op) {
+      case SSDK_BOXOP_TO_FLOAT32: is_float = true; break;
+      case SSDK_BOXOP_TO_UINT8: is_float = false; break;
+      case SSDK_BOXOP_RGB2HSV: case SSDK_BOXOP_HSV2RGB:
+        SSDK_REQUIRE(!is_float, "ssdk_assemble_images: image %d, op %d: a colour conversion needs a uint8 image (TO_UINT8 first)", b, i);
+        break;
+      case SSDK_BOXOP_CHANNEL_SWAP: {
+        const double o[3] = {op.a0, op.a1, op.a2};
+        int seen = 0;
+        for (double v : o) seen |= (v == 0.0 || v == 1.0 || v == 2.0) ? 1 << (int)v : 8;
+        SSDK_REQUIRE(seen == 7, "ssdk_assemble_images: image %d, op %d: CHANNEL_SWAP order (%g, %g, %g) is not a permutation of "
+                     "(0, 1, 2)", b, i, op.a0, op.a1, op.a2);
+        st.op |= ((int)o[0] << 8) | ((int)o[1] << 10) | ((int)o[2] << 12);
+        break;
+      }
+      default:
+        SSDK_REQUIRE(is_float, "ssdk_assemble_images: image %d, op %d: BRIGHTNESS / CONTRAST / SATURATION / HUE need a float32 image "
+                     "(TO_FLOAT32 first)", b, i);
+        if (op.op == SSDK_BOXOP_BRIGHTNESS)
+          SSDK_REQUIRE(std::isfinite(op.a0), "ssdk_assemble_images: image %d, op %d: BRIGHTNESS delta %g is not finite", b, i, op.a0);
+        else if (op.op == SSDK_BOXOP_HUE)
+          SSDK_REQUIRE(op.a0 >= -180.0 && op.a0 <= 180.0, "`delta` must be in the closed interval `[-180, 180]`. (image %d, op %d: %g)", b, i, op.a0);
+        else
+          SSDK_REQUIRE(op.a0 > 0.0 && std::isfinite(op.a0), "It must be `factor > 0`. (image %d, op %d: %g)", b, i, op.a0);
+    }
+    out->st[n++] = st;
+  }
+  SSDK_REQUIRE(!is_float, "ssdk_assemble_images: image %d: the photometric ops leave a float32 image (TO_UINT8 is missing)", b);
+  out->n_stages = n;
+  return SSDK_OK;
+}
+
 bool is_int(double a) { return a == std::floor(a) && std::fabs(a) <= (double)(1 << 24); }
 
 // Host form of IntMap while a list is composed: canvas h x w, canvas (r, c) -> o + m * (r, c), rows [v0, v1) x cols [v2, v3) valid.
@@ -471,6 +706,7 @@ int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_o
     const ssdk_box_op& op = ops[(size_t)b * max_ops + i];
     if (op.op == SSDK_BOXOP_END) break;
     if (op.op == SSDK_BOXOP_FILTER || op.op == SSDK_BOXOP_OVERLAP || op.op == SSDK_BOXOP_CLIP) continue;   // boxes only
+    if (is_photo(op.op)) continue;                                  // run by photometric_kernel (compose_photo)
     SSDK_REQUIRE(op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE, "ssdk_assemble_images: image %d, op %d: unknown op code %d", b, i, op.op);
     SSDK_REQUIRE(!resized, "ssdk_assemble_images: image %d, op %d: the RESIZE must be the last op that changes the image", b, i);
     const long long ch = cur->h, cw = cur->w;
@@ -571,14 +807,41 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
   SSDK_REQUIRE(out_h > 0 && out_w > 0, "ssdk_assemble_images: output size %dx%d must be positive", out_h, out_w);
   SSDK_REQUIRE(max_ops >= 0 && (max_ops == 0 || ops_host), "ssdk_assemble_images: ops_host is NULL");
   std::vector<ImgDesc> descs(B);
+  std::vector<PhotoDesc> photo;                                   // the images with photometric ops
+  std::vector<int> photo_image;
+  long long photo_bytes = 0;
+  int photo_groups = 0;
   for (int b = 0; b < B; ++b) {
-    const int rc = compose_image(b, src_offsets_host, src_hwc_host, ops_host, max_ops, out_h, out_w, &descs[b]);
+    PhotoDesc p{};
+    int rc = compose_photo(b, ops_host, max_ops, &p);
     if (rc) return rc;
+    rc = compose_image(b, src_offsets_host, src_hwc_host, ops_host, max_ops, out_h, out_w, &descs[b]);
+    if (rc) return rc;
+    if (!p.n_stages) continue;
+    const long long n_px = (long long)descs[b].h * descs[b].w;
+    SSDK_REQUIRE(n_px < (1LL << 31) - 4, "ssdk_assemble_images: image %d is too large for the photometric ops", b);
+    p.src_off = descs[b].src_off; p.dst_off = photo_bytes;
+    p.n_px = (int)n_px; p.w = descs[b].w; p.c = descs[b].c;
+    photo_bytes += (n_px * 3 + 15) / 16 * 16;
+    photo_groups = std::max(photo_groups, (int)((n_px + 3) / 4));
+    photo.push_back(p); photo_image.push_back(b);
   }
   cudaStream_t stream = (cudaStream_t)stream_;
-  const size_t bytes = sizeof(ImgDesc) * (size_t)B;
+  const size_t img_bytes = sizeof(ImgDesc) * (size_t)B;
+  const size_t bytes = img_bytes + sizeof(PhotoDesc) * photo.size();
   int rc = ctx->ws[4].ensure(bytes);
   if (rc) return rc;
+  if (!photo.empty()) {
+    rc = ctx->ws[5].ensure((size_t)photo_bytes);
+    if (rc) return rc;
+    // image_assemble_kernel addresses every image as src_dev + src_off: the images in the scratch buffer get their distance
+    // from src_dev (both are device addresses of one flat address space)
+    for (size_t k = 0; k < photo.size(); ++k) {
+      ImgDesc& d = descs[photo_image[k]];
+      d.src_off = (long long)(reinterpret_cast<uintptr_t>(ctx->ws[5].ptr) + (uintptr_t)photo[k].dst_off) - (long long)reinterpret_cast<uintptr_t>(src_dev);
+      d.c = 3;
+    }
+  }
   // descriptors: pinned staging (one buffer of the ring) -> workspace, asynchronous; the host waits only if the upload of the
   // call kImgStages calls ago is still queued
   ssdk_ctx::HostStage& st = ctx->img_stage[ctx->img_stage_next];
@@ -591,11 +854,19 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
     SSDK_CHECK_CUDA(cudaHostAlloc(&st.ptr, want, cudaHostAllocDefault));
     st.bytes = want;
   }
-  std::memcpy(st.ptr, descs.data(), bytes);
+  std::memcpy(st.ptr, descs.data(), img_bytes);
+  if (!photo.empty()) std::memcpy(static_cast<unsigned char*>(st.ptr) + img_bytes, photo.data(), bytes - img_bytes);
   SSDK_CHECK_CUDA(cudaMemcpyAsync(ctx->ws[4].ptr, st.ptr, bytes, cudaMemcpyHostToDevice, stream));
   SSDK_CHECK_CUDA(cudaEventRecord(st.done, stream));
   ctx->img_stage_next = (ctx->img_stage_next + 1) % ssdk_ctx::kImgStages;
   const ImgDesc* d_dev = reinterpret_cast<const ImgDesc*>(ctx->ws[4].ptr);
+  if (!photo.empty()) {
+    const int gx = std::max(1, std::min(ceil_div(photo_groups, kPhotoThreads * kPhotoGroupsPerThread), 65535));
+    photometric_kernel<<<dim3(gx, (unsigned)photo.size()), kPhotoThreads, 0, stream>>>(
+        src_dev, reinterpret_cast<const PhotoDesc*>(static_cast<const unsigned char*>(ctx->ws[4].ptr) + img_bytes),
+        static_cast<uint8_t*>(ctx->ws[5].ptr));
+    SSDK_COUNT_LAUNCH(ctx);
+  }
   if (std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; }))
     image_assemble_kernel<true><<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, d_dev, out_h, out_w, out_dev);
   else

@@ -54,7 +54,7 @@ struct ssdk_ctx {
   int device = 0;
   int sm_count = 132;
   int64_t launches = 0;
-  ssdk::Scratch ws[5];          // decode / loss / nms / box assembly / image descriptor workspaces
+  ssdk::Scratch ws[6];          // decode / loss / nms / box assembly / image descriptor workspaces / photometric pre-pass images
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for
   int loss_parity = 0;          // which of its two histogram sets the next loss call uses (the other one is being cleared)
   cudaDeviceProp prop{};

@@ -25,17 +25,21 @@ one list moves the boxes and produces the image batch; ``assemble_training_batch
   (``resize`` or ``scale``); crops, pads, flips, translations and rotations may come before it, and after a ``scale`` too.
   One background colour per list: pads, translations and scales that bring in background must agree, and a rotation's
   border is black;
-- ``box_filter``, ``overlap_filter``, ``clip``: boxes only.
+- ``box_filter``, ``overlap_filter``, ``clip``: boxes only;
+- the photometric ops (``convert_dtype``, ``brightness``, ``contrast``, ``saturation``, ``hue``, ``convert_color``,
+  ``channel_swap``; ``object_detection_2d_photometric_ops.py``) come before every geometric op, as in all three training chains,
+  and run as a uint8 pre-pass on the device, bit-exact to NumPy and to OpenCV 4.13's uint8 ``cv2.cvtColor`` on a CPU with AVX2
+  (``oracle/photoops.py`` restates them).  ``photometric_ops`` returns ``SSDPhotometricDistortions``' two sequences.
 
 ``translate_ops`` / ``scale_ops`` / ``rotate_ops`` / ``crop_pad_ops`` / ``resize_ops`` / ``box_filter_ops`` return the whole op
 sequence one call of the reference class runs, box filter and clipping included, so the geometric halves of
 ``DataAugmentationConstantInputSize`` (SSD7: translate -> zoom in -> flip, or zoom out -> translate -> flip) and
 ``DataAugmentationSatellite`` (flips -> rotate -> patch -> resize) are one op list per image.
 
-Not covered: photometric distortions, other interpolation modes (``INTER_CUBIC``, ``INTER_LANCZOS4``, ``INTER_AREA`` apart from
+Not covered: ``Gamma`` (the reference's raises), histogram equalisation, conversion to GRAY, other interpolation modes (``INTER_CUBIC``, ``INTER_LANCZOS4``, ``INTER_AREA`` apart from
 cv2's own exact-2x linear path), a second resampling step, the random samplers (``RandomTranslate`` / ``RandomScale``'s draws,
 ``ImageValidator`` retries, ``RandomPatch``), JPEG decoding.  The random decisions of a chain (which patch, flip or not, which
-factor) stay with the caller, as for the boxes."""
+factor, which photometric op with which delta) stay with the caller, as for the boxes."""
 import ctypes as C
 
 import numpy as np
@@ -128,6 +132,73 @@ def overlap_filter(img_height, img_width, overlap_criterion='center_point', over
 def clip(img_height, img_width):
     """``clip_boxes``: boxes clipped to ``[0, h-1] x [0, w-1]``."""
     return (_ffi.BOXOP_CLIP, 0, float(img_height), float(img_width), 0.0, 0.0)
+
+
+def convert_dtype(to='uint8'):
+    """``ConvertDataType`` (photometric_ops.py:62-86): ``astype(float32)``, or ``np.round`` and ``astype(uint8)``."""
+    if to not in ('uint8', 'float32'):
+        raise ValueError("`to` can be either of 'uint8' or 'float32'.")
+    return (_ffi.BOXOP_TO_UINT8 if to == 'uint8' else _ffi.BOXOP_TO_FLOAT32, 0, 0.0, 0.0, 0.0, 0.0)
+
+
+def brightness(delta):
+    """``Brightness`` (:225-246) on a float32 image; ``delta`` is rounded to float32, as NumPy does with a Python float."""
+    return (_ffi.BOXOP_BRIGHTNESS, 0, float(delta), 0.0, 0.0, 0.0)
+
+
+def contrast(factor):
+    """``Contrast`` (:281-304) on a float32 image."""
+    if factor <= 0.0:
+        raise ValueError('It must be `factor > 0`.')
+    return (_ffi.BOXOP_CONTRAST, 0, float(factor), 0.0, 0.0, 0.0)
+
+
+def saturation(factor):
+    """``Saturation`` (:166-189) on a float32 HSV image."""
+    if factor <= 0.0:
+        raise ValueError('It must be `factor > 0`.')
+    return (_ffi.BOXOP_SATURATION, 0, float(factor), 0.0, 0.0, 0.0)
+
+
+def hue(delta):
+    """``Hue`` (:110-133) on a float32 HSV image (H in [0, 180])."""
+    if not (-180 <= delta <= 180):
+        raise ValueError('`delta` must be in the closed interval `[-180, 180]`.')
+    return (_ffi.BOXOP_HUE, 0, float(delta), 0.0, 0.0, 0.0)
+
+
+def convert_color(current='RGB', to='HSV'):
+    """``ConvertColor`` (:23-60) between RGB and HSV on a uint8 image; the GRAY targets are not supported."""
+    if not ((current == 'RGB' and to == 'HSV') or (current == 'HSV' and to == 'RGB')):
+        raise NotImplementedError
+    return (_ffi.BOXOP_RGB2HSV if to == 'HSV' else _ffi.BOXOP_HSV2RGB, 0, 0.0, 0.0, 0.0, 0.0)
+
+
+def channel_swap(order):
+    """``ChannelSwap`` (:438-455): ``image[:, :, order]``."""
+    order = tuple(int(v) for v in order)
+    if sorted(order) != [0, 1, 2]:
+        raise ValueError('`order` must be a permutation of (0, 1, 2)')
+    return (_ffi.BOXOP_CHANNEL_SWAP, 0, float(order[0]), float(order[1]), float(order[2]), 0.0)
+
+
+def photometric_ops(sequence, brightness=None, contrast=None, saturation=None, hue=None, channel_swap=None):
+    """The op list of ``SSDPhotometricDistortions.sequence1`` / ``sequence2`` (data_augmentation_chain_original_ssd.py:165-191;
+    also the photometric part of ``DataAugmentationConstantInputSize``'s sequences) for ``sequence`` 1 or 2, with the values the
+    caller drew; an op whose argument is ``None`` (its draw skipped it) is left out, the conversions stay as the reference
+    keeps them.  Prepend it to the geometric ops of the image."""
+    if sequence not in (1, 2):
+        raise ValueError('`sequence` must be 1 or 2')
+    g = globals()
+    f32, u8 = convert_dtype('float32'), convert_dtype('uint8')
+    b = [g['brightness'](brightness)] if brightness is not None else []
+    c = [g['contrast'](contrast)] if contrast is not None else []
+    hsv = ([convert_color('RGB', 'HSV'), f32] + ([g['saturation'](saturation)] if saturation is not None else [])
+           + ([g['hue'](hue)] if hue is not None else []) + [u8, convert_color('HSV', 'RGB')])
+    swap = [g['channel_swap'](channel_swap)] if channel_swap is not None else []
+    if sequence == 1:
+        return [f32] + b + c + [u8] + hsv + swap
+    return [f32] + b + [u8] + hsv + [f32] + c + [u8] + swap
 
 
 _BOX_FILTER_DEFAULTS = dict(check_overlap=True, check_min_area=True, check_degenerate=True, overlap_criterion='center_point',
