@@ -240,15 +240,24 @@ int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const long long*
  * The caller sorts the predictions twice (stable): by (class, confidence desc) -- the order of the outputs -- and by
  * (class, image, confidence desc) -- the order of the pred_* inputs, whose (class, image) runs are given by seg_offsets.
  *   pred_rank[i]   position of input prediction i in the (class, confidence desc) order
- *   gt_rows        float64 (class, xmin, ymin, xmax, ymax) rows of all images, gt_offsets [n_images+1]
+ *   gt_rows        float64 (class, xmin, ymin, xmax, ymax, area) rows of all images, gt_offsets [n_images+1]; area is the
+ *                  reference's (xmax - xmin + d) * (ymax - ymin + d) computed in the labels' own dtype (an int16 area wraps)
+ *   gt_f32         uint8 [n_images]: 1 when result_type(labels dtype, float32) is float32 (float32 / float16 / int16 / uint8
+ *                  labels), 0 when it is float64 (int32 / int64 / float64 labels)
  *   gt_neutral     optional uint8 flags (eval_neutral, :684), gt_matched uint8 scratch zeroed by the caller
  *   tp / fp        int32 [n_pred], zeroed by the caller, in (class, confidence desc) order
+ * The overlaps follow NumPy's types: the predicted area is float32 arithmetic (the reference's 'f4' structured array), the
+ * intersection, union and quotient run in the image's type, NaN-propagating minimum / maximum, and on the float32 path the
+ * threshold is rounded to float32.  Class ids are compared as float64 (a label class of 1.5 is no class).  The arg-max is
+ * np.argmax's: first maximum, the first NaN wins, and NaN < threshold is False.
+ * Two deliberate departures from the reference: every prediction is matched (its verbose=False loop matches only the first of
+ * each class), and a class without predictions has empty outputs (the reference's cumulative lists skip it).
  * ssdk_eval_cumsum: inclusive scans of tp / fp inside each of the n_segments ranges class_offsets[c] .. class_offsets[c+1].
  * ------------------------------------------------------------------------------------------ */
 int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets_dev, int n_seg, const int* pred_image_dev,
                     const int* pred_class_dev, const float* pred_box_dev, const int* pred_rank_dev, const double* gt_rows_dev,
-                    const int* gt_offsets_dev, const unsigned char* gt_neutral_dev, unsigned char* gt_matched_dev,
-                    double matching_iou_threshold, int border_d, int* tp_dev, int* fp_dev, void* stream);
+                    const int* gt_offsets_dev, const unsigned char* gt_f32_dev, const unsigned char* gt_neutral_dev,
+                    unsigned char* gt_matched_dev, double matching_iou_threshold, int border_d, int* tp_dev, int* fp_dev, void* stream);
 int ssdk_eval_cumsum(ssdk_ctx* ctx, const int* tp_dev, const int* fp_dev, const int* class_offsets_dev, int n_segments,
                      int* ctp_dev, int* cfp_dev, void* stream);
 

@@ -94,3 +94,167 @@ def json_text(img, cls, conf, box, image_ids, classes_to_cats):
         res.append({'image_id': image_ids[img[k]], 'category_id': classes_to_cats[int(cls[k])], 'score': float(round(conf[k], 3)),
                     'bbox': [xmin, ymin, xmax - xmin, ymax - ymin]})
     return json.dumps(res)
+
+
+# -- Evaluator.match_predictions and what follows it (reference :490-905) ---------------------------------------------------
+# Per prediction, the reference takes its box from a structured array with 'f4' fields (a float32 array) and the ground truth
+# as np.asarray(labels), in the labels' own dtype, so NumPy runs its element-wise iou in mixed types: the predicted area in
+# float32, the ground-truth area in the labels' dtype (an int16 area wraps), intersection, union and quotient in
+# result_type(labels, float32), and on a float32 overlap ``overlap < threshold`` rounds the threshold to float32 (NumPy >= 2).
+# The helpers below are the steps a kernel could get subtly wrong, one function each so that a test can swap one out.
+# Two deliberate departures from the reference, kept by the package: every prediction is matched (the reference's
+# verbose=False loop matches only the first of each class), and a class without predictions has empty cumulative arrays (the
+# reference's cumulative lists skip it, which shifts every later class).
+BORDER_D = {'half': 0, 'include': 1, 'exclude': -1}
+GT_FORMAT = {'class_id': 0, 'xmin': 1, 'ymin': 2, 'xmax': 3, 'ymax': 4}
+
+
+def class_mask(classes, class_id):
+    """``gt[:, class_id] == class_id`` in the labels' dtype: a class of 1.5 is no class."""
+    return classes == class_id
+
+
+def pred_area(b, d):
+    """The predicted box's area, ``b`` (1, 4) float32: float32 arithmetic."""
+    return (b[:, 2] - b[:, 0] + d) * (b[:, 3] - b[:, 1] + d)
+
+
+def gt_area(g, d):
+    """The ground-truth areas, ``g`` (k, 4) in the labels' dtype: that dtype's arithmetic."""
+    return (g[:, 2] - g[:, 0] + d) * (g[:, 3] - g[:, 1] + d)
+
+
+def best_index(overlaps):
+    """np.argmax: the first maximum, and the first NaN wins over every number."""
+    return int(np.argmax(overlaps))
+
+
+def below(overlap, threshold):
+    """``overlap < threshold`` with a NumPy scalar overlap and a Python float threshold (NaN < thr is False)."""
+    return bool(overlap < threshold)
+
+
+def cumulative(flags):
+    """np.cumsum: inclusive."""
+    return np.cumsum(flags)
+
+
+def overlaps(gt, pred_box, d):
+    """Element-wise iou (corners) of ``gt`` (k, 4) in the labels' dtype with one ``pred_box`` (4,) float32: intersection
+    without the border term (the reference's iou() calls intersection_area_ with its default), areas with it."""
+    b = pred_box[None, :]
+    with np.errstate(invalid='ignore', divide='ignore', over='ignore'):
+        return _iou(gt, b, d)
+
+
+def _iou(gt, b, d):
+    side = np.maximum(0, np.minimum(gt[:, [2, 3]], b[:, [2, 3]]) - np.maximum(gt[:, [0, 1]], b[:, [0, 1]]) + 0)
+    inter = side[:, 0] * side[:, 1]
+    return inter / (gt_area(gt, d) + pred_area(b, d) - inter)
+
+
+def match_predictions(labels, predictions, n_classes, image_ids, eval_neutral=None, ignore_neutral_boxes=True,
+                      matching_iou_threshold=0.5, border_pixels='include', gt_format=None):
+    """``labels``: per image an array in its own dtype; ``predictions``: per class (index 0 unused) a list of
+    ``(image_id, confidence, xmin, ymin, xmax, ymax)``.  Returns the true and false positive flags per class (index 0 empty),
+    in descending confidence, equal confidences in input order (the reference with 'mergesort')."""
+    f = GT_FORMAT if gt_format is None else gt_format
+    ci, cols = f['class_id'], [f['xmin'], f['ymin'], f['xmax'], f['ymax']]
+    d = BORDER_D[border_pixels]
+    index = {str(i): k for k, i in enumerate(image_ids)}
+    use_neutral = ignore_neutral_boxes and eval_neutral is not None
+    tps, fps = [np.zeros(0, np.int64)], [np.zeros(0, np.int64)]
+    for c in range(1, n_classes + 1):
+        preds = predictions[c]
+        tp, fp = np.zeros(len(preds), np.int64), np.zeros(len(preds), np.int64)
+        if len(preds):
+            conf = np.asarray([p[1] for p in preds], np.float32)
+            boxes = np.asarray([p[2:6] for p in preds], np.float64).astype(np.float32)
+            matched = {}                                    # per image of this class
+            for i, k in enumerate(np.argsort(-conf, kind='mergesort')):
+                img = index[str(preds[k][0])]
+                gt = np.asarray(labels[img])
+                mask = class_mask(gt[:, ci], c)
+                gt = gt[mask]
+                if gt.size == 0:
+                    fp[i] = 1
+                    continue
+                ov = overlaps(gt[:, cols], boxes[k], d)
+                j = best_index(ov)
+                if below(ov[j], matching_iou_threshold):
+                    fp[i] = 1
+                    continue
+                if use_neutral and not (np.asarray(eval_neutral[img])[mask][j] == False):     # noqa: E712 (the reference's test)
+                    continue                                # a neutral box: neither, and not marked matched
+                m = matched.setdefault(img, np.zeros(len(gt), bool))
+                if m[j]:
+                    fp[i] = 1
+                else:
+                    tp[i] = 1
+                    m[j] = True
+        tps.append(tp)
+        fps.append(fp)
+    return tps, fps
+
+
+def num_gt_per_class(labels, n_classes, eval_neutral=None, ignore_neutral_boxes=True, class_col=0):
+    """Evaluator.get_num_gt_per_class as the package counts: class ids cast to int (the reference indexes with the raw value
+    and so raises on float labels)."""
+    num = np.zeros(n_classes + 1, dtype=int)
+    for i, boxes in enumerate(labels):
+        boxes = np.asarray(boxes)
+        if boxes.size == 0:
+            continue
+        cls = boxes[:, class_col].astype(int)
+        if ignore_neutral_boxes and eval_neutral is not None:
+            cls = cls[~np.asarray(eval_neutral[i], dtype=bool)]
+        np.add.at(num, cls, 1)
+    return num
+
+
+def precision_recall(ctp, cfp, num_gt, n_classes):
+    """Cumulative precision (0 where nothing was predicted yet) and recall per class (index 0 empty)."""
+    prec, rec = [[]], [[]]
+    for c in range(1, n_classes + 1):
+        t, f = ctp[c], cfp[c]
+        with np.errstate(divide='ignore', invalid='ignore'):
+            prec.append(np.where(t + f > 0, t / (t + f), 0))
+            rec.append(t / num_gt[c])
+    return prec, rec
+
+
+def average_precisions(prec, rec, n_classes, mode='sample', num_recall_points=11):
+    """Per class (index 0 is 0.0): the maximum precision at recall >= t over ``num_recall_points`` t in [0, 1] averaged
+    ('sample'), or the sum over unique recalls of the recall step times the best precision from there on ('integrate')."""
+    aps = [0.0]
+    for c in range(1, n_classes + 1):
+        p, r = prec[c], rec[c]
+        ap = 0.0
+        if mode == 'sample':
+            for t in np.linspace(start=0, stop=1, num=num_recall_points, endpoint=True):
+                sel = p[r >= t]
+                ap += 0.0 if sel.size == 0 else np.amax(sel)
+            ap /= num_recall_points
+        else:
+            ur, ui = np.unique(r, return_index=True)
+            mp, dr = np.zeros_like(ur), np.zeros_like(ur)
+            for i in range(len(ur) - 2, -1, -1):
+                mp[i] = np.maximum(np.amax(p[ui[i]:ui[i + 1]]), mp[i + 1])
+                dr[i] = ur[i + 1] - ur[i]
+            ap = np.sum(mp * dr)
+        aps.append(ap)
+    return aps
+
+
+def evaluate(labels, predictions, n_classes, image_ids, eval_neutral=None, matching_iou_threshold=0.5, border_pixels='include',
+             gt_format=None):
+    """Everything the golden files hold: flags, cumulative counts, precisions, recalls, both AP modes and both mAPs."""
+    f = GT_FORMAT if gt_format is None else gt_format
+    tp, fp = match_predictions(labels, predictions, n_classes, image_ids, eval_neutral, True, matching_iou_threshold, border_pixels, f)
+    ctp, cfp = [tp[0]] + [cumulative(t) for t in tp[1:]], [fp[0]] + [cumulative(x) for x in fp[1:]]
+    num = num_gt_per_class(labels, n_classes, eval_neutral, True, f['class_id'])
+    prec, rec = precision_recall(ctp, cfp, num, n_classes)
+    ap_s = average_precisions(prec, rec, n_classes, 'sample')
+    ap_i = average_precisions(prec, rec, n_classes, 'integrate')
+    return dict(tp=tp, fp=fp, ctp=ctp, cfp=cfp, num_gt=num, prec=prec, rec=rec, ap_sample=ap_s, ap_integrate=ap_i,
+                map=np.asarray([np.average(ap_s[1:]), np.average(ap_i[1:])]))

@@ -192,7 +192,7 @@ def lib():
         for name in ('ssdk_ssd_loss_fwd_bwd', 'ssdk_ssd_loss_ws_layout', 'ssdk_ssd_loss_phase', 'ssdk_ssd_loss_plan',
                      'ssdk_ssd_loss_read_box_losses'):
             getattr(L, name).restype = C.c_int
-        L.ssdk_eval_match.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int, vp, vp, vp]
+        L.ssdk_eval_match.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int, vp, vp, vp]
         L.ssdk_eval_cumsum.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp]
         L.ssdk_eval_match.restype = C.c_int
         L.ssdk_eval_cumsum.restype = C.c_int

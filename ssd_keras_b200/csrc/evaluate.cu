@@ -6,12 +6,19 @@
 // threshold and that box is still free, else counted as a false positive (neutral boxes: neither).  The only sequential
 // dependency is the "still free" state of a ground-truth box, which is private to one (class, image) pair -- so:
 //   eval_match_kernel   one warp per (class, image) segment of the predictions (sorted by class, image, confidence desc):
-//                       lanes share the image's boxes of that class, float64 IoU with the reference's arithmetic (areas with
-//                       the border-pixel term, intersection without: the iou() quirk), warp arg-max with np.argmax's
-//                       first-index rule, flags written at the prediction's position in (class, confidence) order.
+//                       lanes share the image's boxes of that class, the IoU in the types NumPy uses (below), warp arg-max
+//                       with np.argmax's rules (first maximum; the first NaN wins), flags written at the prediction's position
+//                       in (class, confidence) order.
 //   eval_cumsum_kernel  one CTA per class: inclusive scans of the two flag arrays (np.cumsum, :726-727).
 // Sorting (two stable key sorts) is done by the caller; precision / recall / AP are a few vector operations on the cumulative
 // counts (host, same NumPy expressions as the reference).
+//
+// The reference's types: the predicted box is a float32 array (the structured array's 'f4' fields), the ground truth keeps the
+// labels' dtype.  So the predicted area is float32 arithmetic, the ground-truth area is the labels' dtype (the caller computes
+// it with the reference's expression, int16 wrap included, and passes it as column 5), and the intersection, union and quotient
+// run in result_type(labels, float32): float32 or float64, one flag per image.  On the float32 path the threshold is rounded to
+// float32 before the comparison (a Python float against a float32 scalar).  Minimum and maximum propagate NaN (np.minimum /
+// np.maximum), and NaN < thr is False, so a NaN overlap goes on to matching.
 #include "common.cuh"
 #include "rn.cuh"
 #include <climits>
@@ -27,39 +34,41 @@ struct EvalArgs {
   const int* pred_class;       // [n]
   const float* pred_box;       // [n*4] corners
   const int* pred_rank;        // [n] position in (class, confidence desc) order
-  const double* gt_rows;       // [sum G * 5] class, xmin, ymin, xmax, ymax
+  const double* gt_rows;       // [sum G * 6] class, xmin, ymin, xmax, ymax, area (in the labels' dtype, held exactly)
   const int* gt_offsets;       // [n_images+1]
+  const unsigned char* gt_f32; // [n_images] 1: the image's overlaps are float32 arithmetic, 0: float64
   const unsigned char* gt_neutral;   // [sum G] or NULL
   unsigned char* gt_matched;   // [sum G], zero on entry
   double thr; int d;
   int* tp; int* fp;            // [n], zero on entry
 };
 
-__global__ void __launch_bounds__(256) eval_match_kernel(EvalArgs a, int n_seg) {
-  const int seg = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (seg >= n_seg) return;
-  const int p0 = a.seg_offsets[seg], p1 = a.seg_offsets[seg + 1];
-  if (p1 <= p0) return;
-  const int img = a.pred_image[p0], cls = a.pred_class[p0];
-  const int g0 = a.gt_offsets[img], g1 = a.gt_offsets[img + 1];
+// np.maximum / np.minimum: a NaN in either operand is the result
+template <typename T> __device__ __forceinline__ T np_max(T a, T b) { return (a >= b || a != a) ? a : b; }
+template <typename T> __device__ __forceinline__ T np_min(T a, T b) { return (a <= b || a != a) ? a : b; }
+
+// One (class, image) segment, overlaps in T (float or double).  best / best_g start from "no candidate" (-inf, INT_MAX); a lane
+// takes its first candidate whatever its value, so an arg-max always names a box of the class.
+template <typename T>
+__device__ __forceinline__ void match_segment(const EvalArgs& a, int p0, int p1, int g0, int g1, int cls, int lane) {
+  const double thr = (double)(T)a.thr;
+  const float d = (float)a.d;
   for (int p = p0; p < p1; ++p) {                       // descending confidence inside the segment
-    const double px0 = a.pred_box[p * 4], py0 = a.pred_box[p * 4 + 1], px1 = a.pred_box[p * 4 + 2], py1 = a.pred_box[p * 4 + 3];
-    const double parea = __dmul_rn(__dadd_rn(__dsub_rn(px1, px0), (double)a.d), __dadd_rn(__dsub_rn(py1, py0), (double)a.d));
-    // best overlap among the boxes of this class (np.argmax: first maximum; a NaN counts as the maximum)
-    double best = -1.0; int best_g = INT_MAX; int best_nan = 0, any = 0;
+    const float fx0 = a.pred_box[p * 4], fy0 = a.pred_box[p * 4 + 1], fx1 = a.pred_box[p * 4 + 2], fy1 = a.pred_box[p * 4 + 3];
+    const T parea = (T)__fmul_rn(__fadd_rn(__fsub_rn(fx1, fx0), d), __fadd_rn(__fsub_rn(fy1, fy0), d));
+    const T px0 = (T)fx0, py0 = (T)fy0, px1 = (T)fx1, py1 = (T)fy1;
+    double best = -INFINITY; int best_g = INT_MAX; int best_nan = 0, any = 0;
     for (int g = g0 + lane; g < g1; g += 32) {
-      const double* r = a.gt_rows + (size_t)g * 5;
-      if ((int)r[0] != cls) continue;
+      const double* r = a.gt_rows + (size_t)g * 6;
+      if (r[0] != (double)cls) continue;                  // gt[:, class_id] == class_id
       any = 1;
-      const double iw = fmax(0.0, __dsub_rn(fmin(r[3], px1), fmax(r[1], px0)));
-      const double ih = fmax(0.0, __dsub_rn(fmin(r[4], py1), fmax(r[2], py0)));
-      const double inter = __dmul_rn(iw, ih);
-      const double garea = __dmul_rn(__dadd_rn(__dsub_rn(r[3], r[1]), (double)a.d), __dadd_rn(__dsub_rn(r[4], r[2]), (double)a.d));
-      const double v = __ddiv_rn(inter, __dsub_rn(__dadd_rn(garea, parea), inter));
-      const int is_nan = (v != v) ? 1 : 0;
+      const T iw = np_max((T)0, sub_rn(np_min((T)r[3], px1), np_max((T)r[1], px0)));
+      const T ih = np_max((T)0, sub_rn(np_min((T)r[4], py1), np_max((T)r[2], py0)));
+      const T inter = mul_rn(iw, ih);
+      const T v = div_rn(inter, sub_rn(add_rn((T)r[5], parea), inter));
       if (best_nan) continue;                             // an earlier NaN of this lane already wins
-      if (is_nan || v > best) { best = v; best_g = g; best_nan = is_nan; }
+      const int is_nan = (v != v) ? 1 : 0;
+      if (is_nan || best_g == INT_MAX || (double)v > best) { best = (double)v; best_g = g; best_nan = is_nan; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -70,13 +79,13 @@ __global__ void __launch_bounds__(256) eval_match_kernel(EvalArgs a, int n_seg) 
       bool take;
       if (on != best_nan) take = on > best_nan;           // NaN beats every number
       else if (on) take = og < best_g;                    // two NaNs: the first one
-      else take = (ov > best) || (ov == best && og < best_g);
+      else take = (ov > best) || (ov == best && og < best_g);   // equal values (or a lane without candidates): the first index
       if (take) { best = ov; best_g = og; best_nan = on; }
     }
     if (lane == 0) {
       const int r = a.pred_rank[p];
       if (!any) a.fp[r] = 1;                              // no box of this class in the image (:672-675)
-      else if (best < a.thr) a.fp[r] = 1;                 // (NaN < thr is False, as in the reference)
+      else if (best < thr) a.fp[r] = 1;                   // (NaN < thr is False, as in the reference)
       else if (!(a.gt_neutral && a.gt_neutral[best_g])) {
         if (!a.gt_matched[best_g]) { a.tp[r] = 1; a.gt_matched[best_g] = 1; }
         else a.fp[r] = 1;                                 // the box was matched by a more confident prediction
@@ -84,6 +93,18 @@ __global__ void __launch_bounds__(256) eval_match_kernel(EvalArgs a, int n_seg) 
     }
     __syncwarp();                                         // lane 0's gt_matched write is only ever read by lane 0
   }
+}
+
+__global__ void __launch_bounds__(256) eval_match_kernel(EvalArgs a, int n_seg) {
+  const int seg = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (seg >= n_seg) return;
+  const int p0 = a.seg_offsets[seg], p1 = a.seg_offsets[seg + 1];
+  if (p1 <= p0) return;
+  const int img = a.pred_image[p0], cls = a.pred_class[p0];
+  const int g0 = a.gt_offsets[img], g1 = a.gt_offsets[img + 1];
+  if (a.gt_f32[img]) match_segment<float>(a, p0, p1, g0, g1, cls, lane);
+  else match_segment<double>(a, p0, p1, g0, g1, cls, lane);
 }
 
 __global__ void __launch_bounds__(1024) eval_cumsum_kernel(const int* __restrict__ tp, const int* __restrict__ fp, const int* __restrict__ class_offsets,
@@ -212,14 +233,15 @@ extern "C" int ssdk_eval_collect(ssdk_ctx* ctx, const float* rows_dev, int B, in
 
 extern "C" int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets_dev, int n_seg, const int* pred_image_dev,
                                const int* pred_class_dev, const float* pred_box_dev, const int* pred_rank_dev, const double* gt_rows_dev,
-                               const int* gt_offsets_dev, const unsigned char* gt_neutral_dev, unsigned char* gt_matched_dev,
+                               const int* gt_offsets_dev, const unsigned char* gt_f32_dev, const unsigned char* gt_neutral_dev,
+                               unsigned char* gt_matched_dev,
                                double matching_iou_threshold, int border_d, int* tp_dev, int* fp_dev, void* stream_) {
   SSDK_REQUIRE(ctx && n_pred >= 0 && n_seg >= 0, "ssdk_eval_match: bad argument");
   if (n_pred == 0 || n_seg == 0) return SSDK_OK;
   SSDK_REQUIRE(seg_offsets_dev && pred_image_dev && pred_class_dev && pred_box_dev && pred_rank_dev && gt_rows_dev && gt_offsets_dev &&
-               gt_matched_dev && tp_dev && fp_dev, "ssdk_eval_match: NULL argument");
-  EvalArgs a{seg_offsets_dev, pred_image_dev, pred_class_dev, pred_box_dev, pred_rank_dev, gt_rows_dev, gt_offsets_dev, gt_neutral_dev,
-             gt_matched_dev, matching_iou_threshold, border_d, tp_dev, fp_dev};
+               gt_f32_dev && gt_matched_dev && tp_dev && fp_dev, "ssdk_eval_match: NULL argument");
+  EvalArgs a{seg_offsets_dev, pred_image_dev, pred_class_dev, pred_box_dev, pred_rank_dev, gt_rows_dev, gt_offsets_dev, gt_f32_dev,
+             gt_neutral_dev, gt_matched_dev, matching_iou_threshold, border_d, tp_dev, fp_dev};
   eval_match_kernel<<<ceil_div(n_seg, 8), 256, 0, (cudaStream_t)stream_>>>(a, n_seg);
   SSDK_COUNT_LAUNCH(ctx);
   SSDK_CHECK_CUDA(cudaGetLastError());

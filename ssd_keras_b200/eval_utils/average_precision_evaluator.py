@@ -2,8 +2,10 @@
 
 The expensive step of the reference is ``match_predictions`` (:538-736): for every class, a Python loop over all predictions in
 descending confidence with an element-wise ``iou`` against the ground truth of the prediction's image.  Here it is two stable
-key sorts plus ``ssdk_eval_match`` (one warp per (class, image) pair, float64 IoU with the reference's arithmetic) and
-``ssdk_eval_cumsum``; precision / recall / AP (:738-905) are the reference's NumPy expressions on the cumulative counts.
+key sorts plus ``ssdk_eval_match`` (one warp per (class, image) pair, the IoU in the types NumPy gives the reference's
+expression: a float32 predicted area, the ground-truth area in the labels' dtype, the rest in float32 or float64 by the labels'
+dtype) and ``ssdk_eval_cumsum``; precision / recall / AP (:738-905) are the reference's NumPy expressions on the cumulative
+counts.
 
 What the class needs from ``data_generator`` is what the reference reads from its ``DataGenerator``: ``labels`` (list of
 ``(k_i, 5)`` arrays), ``image_ids`` and optionally ``eval_neutral``; for ``predict_on_dataset`` additionally ``images`` (uint8
@@ -19,7 +21,7 @@ replaces them.
 
 Note on a reference quirk: with ``verbose=False`` the reference iterates ``range(len(predictions.shape))`` (:641), i.e. it
 matches only the first prediction of every class.  This implementation always matches all of them (the ``verbose=True``
-behaviour)."""
+behaviour), and a class without predictions gets empty arrays where the reference's cumulative lists skip it."""
 import ctypes as C
 
 import numpy as np
@@ -177,14 +179,28 @@ class Evaluator:
             raise ValueError("`border_pixels` must be one of 'half', 'include', 'exclude'.")
         nC = self.n_classes
         id_index = {str(i): k for k, i in enumerate(self.data_generator.image_ids)}
-        # ground truth -> packed float64 rows in the column order (class, xmin, ymin, xmax, ymax)
+        # ground truth -> float64 rows (class, xmin, ymin, xmax, ymax, area) and one arithmetic type per image, as NumPy types
+        # the reference's iou: the area is its expression in the labels' own dtype (an int16 area wraps, exactly held in
+        # float64), and intersection, union and quotient run in result_type(labels, float32), float32 or float64
+        d = _ffi.BORDER_D[border_pixels]
         cols = [self.gt_format[k] for k in ('class_id', 'xmin', 'ymin', 'xmax', 'ymax')]
-        rows, offs = [], [0]
+        labs, offs = [], [0]
         for lab in self.data_generator.labels:
-            lab = np.asarray(lab, dtype=np.float64)
-            lab = lab.reshape(-1, lab.shape[-1])[:, cols] if lab.size else np.zeros((0, 5))
-            rows.append(lab); offs.append(offs[-1] + lab.shape[0])
-        gt = np.concatenate(rows, axis=0) if offs[-1] else np.zeros((1, 5))
+            lab = np.asarray(lab)
+            lab = lab.reshape(-1, lab.shape[-1])[:, cols] if lab.size else np.zeros((0, 5), lab.dtype)
+            labs.append(lab); offs.append(offs[-1] + lab.shape[0])
+        dtypes = sorted({lab.dtype for lab in labs}, key=str)
+        code = np.asarray([dtypes.index(lab.dtype) for lab in labs], dtype=np.int64) if len(dtypes) > 1 else np.zeros(len(labs), np.int64)
+        f32 = np.asarray([np.result_type(dt, np.float32) == np.float32 for dt in dtypes], dtype=np.uint8)[code]
+        gt = np.zeros((max(offs[-1], 1), 6))
+        row_code = np.repeat(code, np.diff(offs))
+        for k, dt in enumerate(dtypes):                                  # one vectorised area per dtype, rows in image order
+            part = np.concatenate([lab for lab, c in zip(labs, code) if c == k]) if len(dtypes) > 1 else np.concatenate(labs)
+            if not part.shape[0]:
+                continue
+            rows = np.nonzero(row_code == k)[0]
+            gt[rows, :5] = part
+            gt[rows, 5] = (part[:, 3] - part[:, 1] + d) * (part[:, 4] - part[:, 2] + d)
         neutral = getattr(self.data_generator, 'eval_neutral', None)
         use_neutral = ignore_neutral_boxes and neutral is not None
         # predictions -> flat arrays, class-major, input order inside a class
@@ -226,6 +242,7 @@ class Evaluator:
             p_box, p_rank = t_box[ord2].contiguous(), rank[ord2].contiguous()
             d_gt = torch.from_numpy(np.ascontiguousarray(gt)).to(dev)
             d_off = torch.from_numpy(np.asarray(offs, dtype=np.int32)).to(dev)
+            d_f32 = torch.from_numpy(np.ascontiguousarray(f32) if len(f32) else np.zeros(1, np.uint8)).to(dev)
             d_neutral = None
             if use_neutral:
                 flat = np.concatenate([np.asarray(e, dtype=np.uint8).reshape(-1) for e in neutral]) if offs[-1] else np.zeros(1, np.uint8)
@@ -235,8 +252,8 @@ class Evaluator:
             ctp = torch.empty_like(tp); cfp = torch.empty_like(fp)
             ctx = _ffi.context()
             _ffi.check(_ffi.lib().ssdk_eval_match(ctx, n, _ffi.dptr(seg), n_seg, _ffi.dptr(p_img), _ffi.dptr(p_cls), _ffi.dptr(p_box),
-                                                  _ffi.dptr(p_rank), _ffi.dptr(d_gt), _ffi.dptr(d_off), _ffi.dptr(d_neutral), _ffi.dptr(matched),
-                                                  float(matching_iou_threshold), _ffi.BORDER_D[border_pixels], _ffi.dptr(tp), _ffi.dptr(fp),
+                                                  _ffi.dptr(p_rank), _ffi.dptr(d_gt), _ffi.dptr(d_off), _ffi.dptr(d_f32), _ffi.dptr(d_neutral),
+                                                  _ffi.dptr(matched), float(matching_iou_threshold), d, _ffi.dptr(tp), _ffi.dptr(fp),
                                                   _ffi.stream_ptr()))
             coff = torch.from_numpy(np.concatenate([[0], np.cumsum(counts[1:])]).astype(np.int32)).to(dev)
             _ffi.check(_ffi.lib().ssdk_eval_cumsum(ctx, _ffi.dptr(tp), _ffi.dptr(fp), _ffi.dptr(coff), nC, _ffi.dptr(ctp), _ffi.dptr(cfp),

@@ -1,15 +1,19 @@
 """Evaluator on the GPU (ssdk_eval_match / ssdk_eval_cumsum) against the REAL reference's match_predictions /
 compute_precision_recall / compute_average_precisions / compute_mean_average_precision on synthetic predictions
 (tests/golden/make_eval_golden.py): true / false positive flags and cumulative counts bit-exact per class, precisions,
-recalls, APs and mAP to float64 round-off."""
+recalls, APs and mAP to float64 round-off; and on the edge cases of tests/eval_cases.py (ref_eval_edges_golden.npz), all of
+it bit for bit."""
 import os
 import types
 
 import numpy as np
 import pytest
 
+import eval_cases as xc
+
 pytestmark = pytest.mark.gpu
 G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_eval_golden.npz'))
+E = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_eval_edges_golden.npz'))
 
 
 @pytest.fixture(scope='module', autouse=True)
@@ -56,6 +60,15 @@ def test_evaluator_vs_reference(name, use_neutral, bp):
     np.testing.assert_allclose(ev.compute_average_precisions(mode='integrate', ret=True), G[key + '/ap_integrate'], rtol=1e-14)
     m_i = ev.compute_mean_average_precision()
     np.testing.assert_allclose([m_s, m_i], G[key + '/map'], rtol=1e-14)
+
+
+@pytest.mark.parametrize('name', xc.EDGES)
+def test_evaluator_edges_vs_reference(name):
+    """The edge cases of tests/eval_cases.py (every label dtype, border mode and threshold, predictions on the threshold in
+    both arithmetic types, NaN and non-finite overlaps, ties and NaNs across lanes, neutral arg-maxes, an empty class,
+    integer ids, a permuted gt_format, a fractional class id) against the reference's own results, bit for bit."""
+    c = xc.edge(name)
+    xc.assert_same(xc.device(c), xc.golden(E, name, c['n_classes']), c['n_classes'], name)
 
 
 def test_evaluator_end_to_end_on_a_model():
