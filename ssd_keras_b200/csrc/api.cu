@@ -39,11 +39,8 @@ extern "C" int ssdk_ctx_create(int device, ssdk_ctx** out) {
 
 extern "C" int ssdk_ctx_destroy(ssdk_ctx* ctx) {
   if (!ctx) return SSDK_OK;
-  for (auto& w : ctx->ws) w.release();
-  for (auto& s : ctx->img_stage) {
-    if (s.done) { cudaEventSynchronize(s.done); cudaEventDestroy(s.done); }
-    if (s.ptr) cudaFreeHost(s.ptr);
-  }
+  for (Scratch* w : {&ctx->decode_ws, &ctx->nms_ws, &ctx->loss_ws, &ctx->box_ws, &ctx->img_desc_ws, &ctx->photo_ws}) w->release();
+  ctx->img_desc_ring.release();
   delete ctx;
   return SSDK_OK;
 }

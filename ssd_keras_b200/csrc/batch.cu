@@ -207,18 +207,15 @@ extern "C" int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_
   SSDK_REQUIRE(max_ops == 0 || ops_dev, "ssdk_assemble_batch: ops_dev is NULL");
   cudaStream_t stream = (cudaStream_t)stream_;
   const size_t need = (size_t)(total_in > 0 ? total_in : 1) * 5 * sizeof(float) + (size_t)B * sizeof(int) + 256;
-  int rc = ctx->ws[3].ensure(need);
+  int rc = ctx->box_ws.ensure(need);
   if (rc) return rc;
-  float* tmp = reinterpret_cast<float*>(ctx->ws[3].ptr);
-  int* counts = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(ctx->ws[3].ptr) + (((size_t)(total_in > 0 ? total_in : 1) * 5 * sizeof(float) + 255) / 256 * 256));
-  box_ops_kernel<<<B, kBoxThreads, 0, stream>>>(gt_in_dev, gt_in_f64, offsets_in_dev, ops_dev, max_ops, tmp, counts);
-  SSDK_COUNT_LAUNCH(ctx);
-  box_offsets_kernel<<<1, 1024, 0, stream>>>(counts, B, offsets_out_dev, out_stats_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  box_pack_kernel<<<B, kBoxThreads, 0, stream>>>(tmp, offsets_in_dev, offsets_out_dev, gt_out_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  float* tmp = reinterpret_cast<float*>(ctx->box_ws.ptr);
+  int* counts = reinterpret_cast<int*>(reinterpret_cast<unsigned char*>(ctx->box_ws.ptr) + (((size_t)(total_in > 0 ? total_in : 1) * 5 * sizeof(float) + 255) / 256 * 256));
+  rc = launch(ctx, box_ops_kernel, B, kBoxThreads, 0, stream, gt_in_dev, gt_in_f64, offsets_in_dev, ops_dev, max_ops, tmp, counts);
+  if (rc) return rc;
+  rc = launch(ctx, box_offsets_kernel, 1, 1024, 0, stream, counts, B, offsets_out_dev, out_stats_dev);
+  if (rc) return rc;
+  return launch(ctx, box_pack_kernel, B, kBoxThreads, 0, stream, tmp, offsets_in_dev, offsets_out_dev, gt_out_dev);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -829,49 +826,32 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
   cudaStream_t stream = (cudaStream_t)stream_;
   const size_t img_bytes = sizeof(ImgDesc) * (size_t)B;
   const size_t bytes = img_bytes + sizeof(PhotoDesc) * photo.size();
-  int rc = ctx->ws[4].ensure(bytes);
+  int rc = ctx->img_desc_ws.ensure(bytes);
   if (rc) return rc;
   if (!photo.empty()) {
-    rc = ctx->ws[5].ensure((size_t)photo_bytes);
+    rc = ctx->photo_ws.ensure((size_t)photo_bytes);
     if (rc) return rc;
     // image_assemble_kernel addresses every image as src_dev + src_off: the images in the scratch buffer get their distance
     // from src_dev (both are device addresses of one flat address space)
     for (size_t k = 0; k < photo.size(); ++k) {
       ImgDesc& d = descs[photo_image[k]];
-      d.src_off = (long long)(reinterpret_cast<uintptr_t>(ctx->ws[5].ptr) + (uintptr_t)photo[k].dst_off) - (long long)reinterpret_cast<uintptr_t>(src_dev);
+      d.src_off = (long long)(reinterpret_cast<uintptr_t>(ctx->photo_ws.ptr) + (uintptr_t)photo[k].dst_off) - (long long)reinterpret_cast<uintptr_t>(src_dev);
       d.c = 3;
     }
   }
-  // descriptors: pinned staging (one buffer of the ring) -> workspace, asynchronous; the host waits only if the upload of the
-  // call kImgStages calls ago is still queued
-  ssdk_ctx::HostStage& st = ctx->img_stage[ctx->img_stage_next];
-  if (!st.done) SSDK_CHECK_CUDA(cudaEventCreateWithFlags(&st.done, cudaEventDisableTiming));
-  else SSDK_CHECK_CUDA(cudaEventSynchronize(st.done));
-  if (st.bytes < bytes) {
-    if (st.ptr) cudaFreeHost(st.ptr);
-    st.ptr = nullptr; st.bytes = 0;
-    const size_t want = std::max(bytes, (size_t)16384);
-    SSDK_CHECK_CUDA(cudaHostAlloc(&st.ptr, want, cudaHostAllocDefault));
-    st.bytes = want;
-  }
-  std::memcpy(st.ptr, descs.data(), img_bytes);
-  if (!photo.empty()) std::memcpy(static_cast<unsigned char*>(st.ptr) + img_bytes, photo.data(), bytes - img_bytes);
-  SSDK_CHECK_CUDA(cudaMemcpyAsync(ctx->ws[4].ptr, st.ptr, bytes, cudaMemcpyHostToDevice, stream));
-  SSDK_CHECK_CUDA(cudaEventRecord(st.done, stream));
-  ctx->img_stage_next = (ctx->img_stage_next + 1) % ssdk_ctx::kImgStages;
-  const ImgDesc* d_dev = reinterpret_cast<const ImgDesc*>(ctx->ws[4].ptr);
+  // descriptors: pinned staging -> workspace, asynchronous; the host waits only if the upload from the same staging buffer,
+  // four calls ago, is still queued
+  rc = ctx->img_desc_ring.upload(ctx->img_desc_ws.ptr, stream, {{descs.data(), img_bytes}, {photo.data(), bytes - img_bytes}});
+  if (rc) return rc;
+  const ImgDesc* d_dev = reinterpret_cast<const ImgDesc*>(ctx->img_desc_ws.ptr);
   if (!photo.empty()) {
     const int gx = std::max(1, std::min(ceil_div(photo_groups, kPhotoThreads * kPhotoGroupsPerThread), 65535));
-    photometric_kernel<<<dim3(gx, (unsigned)photo.size()), kPhotoThreads, 0, stream>>>(
-        src_dev, reinterpret_cast<const PhotoDesc*>(static_cast<const unsigned char*>(ctx->ws[4].ptr) + img_bytes),
-        static_cast<uint8_t*>(ctx->ws[5].ptr));
-    SSDK_COUNT_LAUNCH(ctx);
+    rc = launch(ctx, photometric_kernel, dim3(gx, (unsigned)photo.size()), kPhotoThreads, 0, stream,
+                src_dev, reinterpret_cast<const PhotoDesc*>(static_cast<const unsigned char*>(ctx->img_desc_ws.ptr) + img_bytes),
+                static_cast<uint8_t*>(ctx->photo_ws.ptr));
+    if (rc) return rc;
   }
-  if (std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; }))
-    image_assemble_kernel<true><<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, d_dev, out_h, out_w, out_dev);
-  else
-    image_assemble_kernel<false><<<dim3(out_h, B), kImgThreads, 0, stream>>>(src_dev, d_dev, out_h, out_w, out_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  const bool warp = std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; });
+  return launch(ctx, warp ? image_assemble_kernel<true> : image_assemble_kernel<false>, dim3(out_h, B), kImgThreads, 0, stream,
+                src_dev, d_dev, out_h, out_w, out_dev);
 }

@@ -175,14 +175,10 @@ int launch_bn_forward(ssdk_ctx* ctx, LayerPlan& L, int act, cudaStream_t s) {
   const int groups = z.Cs / 8;
   const size_t total = (size_t)z.B * z.H * z.W * groups;
   const double N = (double)z.B * z.H * z.W;
-  bn_stats_kernel<<<bn_grid(z, ctx->sm_count), 256, (size_t)2 * z.Cs * sizeof(double), s>>>(z, L.bn_acc);
-  SSDK_COUNT_LAUNCH(ctx);
-  bn_finalize_kernel<<<(z.C + 127) / 128, 128, 0, s>>>(L.bn_acc, z.C, N, L.bn_eps, L.bn_momentum, L.bn_bmean, L.bn_brstd, L.bn_mmean, L.bn_mvar);
-  SSDK_COUNT_LAUNCH(ctx);
-  bn_apply_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(z, L.out, L.bn_gamma, L.bn_beta, L.bn_bmean, L.bn_brstd, act);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  if (int rc = launch(ctx, bn_stats_kernel, bn_grid(z, ctx->sm_count), 256, (size_t)2 * z.Cs * sizeof(double), s, z, L.bn_acc)) return rc;
+  if (int rc = launch(ctx, bn_finalize_kernel, (z.C + 127) / 128, 128, 0, s,
+                      L.bn_acc, z.C, N, L.bn_eps, L.bn_momentum, L.bn_bmean, L.bn_brstd, L.bn_mmean, L.bn_mvar)) return rc;
+  return launch(ctx, bn_apply_kernel, (unsigned)((total + 255) / 256), 256, 0, s, z, L.out, L.bn_gamma, L.bn_beta, L.bn_bmean, L.bn_brstd, act);
 }
 
 int launch_bn_backward(ssdk_ctx* ctx, LayerPlan& L, int act, const ActBuf& g, float* dgamma, float* dbeta, cudaStream_t s) {
@@ -190,15 +186,11 @@ int launch_bn_backward(ssdk_ctx* ctx, LayerPlan& L, int act, const ActBuf& g, fl
   const int groups = z.Cs / 8;
   const size_t total = (size_t)z.B * z.H * z.W * groups;
   const double N = (double)z.B * z.H * z.W;
-  bn_bwd_reduce_kernel<<<bn_grid(z, ctx->sm_count), 256, (size_t)2 * z.Cs * sizeof(double), s>>>(z, L.out, g, L.bn_bmean, L.bn_brstd, act, L.bn_acc);
-  SSDK_COUNT_LAUNCH(ctx);
-  bn_bwd_apply_kernel<<<(unsigned)((std::max(total, (size_t)z.C) + 255) / 256), 256, 0, s>>>(z, L.out, g, L.bn_gamma, L.bn_bmean, L.bn_brstd, act, L.bn_acc,
-                                                                                             N, dgamma, dbeta);
-  SSDK_COUNT_LAUNCH(ctx);
-  zero_acc_kernel<<<(2 * z.C + 127) / 128, 128, 0, s>>>(L.bn_acc, 2 * z.C);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  if (int rc = launch(ctx, bn_bwd_reduce_kernel, bn_grid(z, ctx->sm_count), 256, (size_t)2 * z.Cs * sizeof(double), s,
+                      z, L.out, g, L.bn_bmean, L.bn_brstd, act, L.bn_acc)) return rc;
+  if (int rc = launch(ctx, bn_bwd_apply_kernel, (unsigned)((std::max(total, (size_t)z.C) + 255) / 256), 256, 0, s,
+                      z, L.out, g, L.bn_gamma, L.bn_bmean, L.bn_brstd, act, L.bn_acc, N, dgamma, dbeta)) return rc;
+  return launch(ctx, zero_acc_kernel, (2 * z.C + 127) / 128, 128, 0, s, L.bn_acc, 2 * z.C);
 }
 
 }  // namespace ssdk

@@ -5,7 +5,12 @@
 #include <cstdio>
 #include <cstdarg>
 #include <cstring>
+#include <algorithm>
 #include <atomic>
+#include <initializer_list>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <vector>
 #include <string>
 #include "../../include/ssdk.h"
@@ -48,26 +53,111 @@ struct Scratch {
   void release() { if (ptr) cudaFree(ptr); ptr = nullptr; bytes = 0; }
 };
 
+// Pinned staging for host -> device uploads that must not wait for the stream: N buffers used in turn, each with an event
+// recorded after the copy issued from it, so the host runs up to N uploads ahead of the device before it waits for a buffer.
+template <int N>
+struct HostRing {
+  struct Slot { void* ptr = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; } slot[N];
+  int next = 0;
+
+  // Copies the concatenation of `parts` (host pointer, bytes) to dst_dev on `stream`.
+  int upload(void* dst_dev, cudaStream_t stream, std::initializer_list<std::pair<const void*, size_t>> parts) {
+    size_t bytes = 0;
+    for (const auto& p : parts) bytes += p.second;
+    Slot& s = slot[next];
+    if (!s.done) SSDK_CHECK_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+    else SSDK_CHECK_CUDA(cudaEventSynchronize(s.done));
+    if (s.bytes < bytes) {
+      if (s.ptr) cudaFreeHost(s.ptr);
+      s.ptr = nullptr; s.bytes = 0;
+      const size_t want = std::max(bytes, (size_t)16384);
+      SSDK_CHECK_CUDA(cudaHostAlloc(&s.ptr, want, cudaHostAllocDefault));
+      s.bytes = want;
+    }
+    unsigned char* h = static_cast<unsigned char*>(s.ptr);
+    for (const auto& p : parts) { if (p.second) std::memcpy(h, p.first, p.second); h += p.second; }
+    SSDK_CHECK_CUDA(cudaMemcpyAsync(dst_dev, s.ptr, bytes, cudaMemcpyHostToDevice, stream));
+    SSDK_CHECK_CUDA(cudaEventRecord(s.done, stream));
+    next = (next + 1) % N;
+    return SSDK_OK;
+  }
+
+  void release() {
+    for (Slot& s : slot) {
+      if (s.done) { cudaEventSynchronize(s.done); cudaEventDestroy(s.done); }
+      if (s.ptr) cudaFreeHost(s.ptr);
+      s = Slot{};
+    }
+  }
+};
+
 }  // namespace ssdk
 
 struct ssdk_ctx {
   int device = 0;
   int sm_count = 132;
-  int64_t launches = 0;
-  ssdk::Scratch ws[6];          // decode / loss / nms / box assembly / image descriptor workspaces / photometric pre-pass images
+  int64_t launches = 0;         // kernels launched through ssdk::launch
+  // grow-only device workspaces, one per user
+  ssdk::Scratch decode_ws;      // ssdk_decode: decoded boxes, scores, labels and its NMS scratch
+  ssdk::Scratch nms_ws;         // ssdk_nms
+  ssdk::Scratch loss_ws;        // the SSD loss
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for
   int loss_parity = 0;          // which of its two histogram sets the next loss call uses (the other one is being cleared)
+  ssdk::Scratch box_ws;         // ssdk_assemble_batch: transformed boxes and per-image counts
+  ssdk::Scratch img_desc_ws;    // ssdk_assemble_images: per-image and photometric descriptors
+  ssdk::Scratch photo_ws;       // ssdk_assemble_images: images after the photometric pre-pass
   cudaDeviceProp prop{};
-  // Pinned staging for the per-image descriptors of ssdk_assemble_images: a ring of buffers, each with an event recorded after
-  // its upload, so that the host can run up to kImgStages calls ahead of the device before a buffer has to be waited for.
-  static constexpr int kImgStages = 4;
-  struct HostStage { void* ptr = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; } img_stage[kImgStages];
-  int img_stage_next = 0;
+  ssdk::HostRing<4> img_desc_ring;   // pinned staging of img_desc_ws
 };
 
-#define SSDK_COUNT_LAUNCH(ctx) do { (ctx)->launches++; } while (0)
-
 namespace ssdk {
+
+// Raises `kernel`'s dynamic shared-memory limit on ctx->device to at least `bytes`; up to 48 KB every kernel may use without it.
+// The limit belongs to the kernel in one device's context, so the level set is kept per (kernel, device), behind a lock since
+// contexts are per (device, thread).
+inline int allow_smem(const ssdk_ctx* ctx, const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return SSDK_OK;
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> limit;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = limit[{kernel, ctx->device}];
+  if (bytes <= have) return SSDK_OK;
+  SSDK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  have = bytes;
+  return SSDK_OK;
+}
+
+// Counts a launch in ctx->launches and reports its error (`e`, else the thread's last CUDA error) by the kernel's name.
+inline int launched(ssdk_ctx* ctx, const void* kernel, cudaError_t e) {
+  const cudaError_t last = cudaGetLastError();   // also clears the error a failed launch leaves behind
+  if (e == cudaSuccess) e = last;
+  ctx->launches++;
+  if (e == cudaSuccess) return SSDK_OK;
+  const char* name = nullptr;
+  if (cudaFuncGetName(&name, kernel) != cudaSuccess || !name) name = "<unknown kernel>";
+  set_error("launch of %s failed: %s", name, cudaGetErrorString(e));
+  return SSDK_ERR_CUDA;
+}
+
+// Every kernel of the library is launched here: kernel<<<grid, block, smem, stream>>>(args...), with the shared-memory limit
+// raised as far as smem needs, the launch counted and its error returned as SSDK_ERR_CUDA.
+template <typename... Ps, typename... As>
+int launch(ssdk_ctx* ctx, void (*kernel)(Ps...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, As&&... args) {
+  if (int rc = allow_smem(ctx, (const void*)kernel, smem)) return rc;
+  kernel<<<grid, block, smem, stream>>>(std::forward<As>(args)...);
+  return launched(ctx, (const void*)kernel, cudaSuccess);
+}
+
+// The same as one cooperative grid: all blocks resident at once, so the kernel may synchronise the whole grid.
+template <typename... Ps, typename... As>
+int launch_cooperative(ssdk_ctx* ctx, void (*kernel)(Ps...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, As&&... args) {
+  if (int rc = allow_smem(ctx, (const void*)kernel, smem)) return rc;
+  cudaLaunchAttribute coop{};
+  coop.id = cudaLaunchAttributeCooperative;
+  coop.val.cooperative = 1;
+  const cudaLaunchConfig_t cfg = {grid, block, smem, stream, &coop, 1};
+  return launched(ctx, (const void*)kernel, cudaLaunchKernelEx(&cfg, kernel, std::forward<As>(args)...));
+}
 
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline long long ceil_div_ll(long long a, long long b) { return (a + b - 1) / b; }

@@ -464,38 +464,24 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   }
 }
 
-template <int BN, int MODE>
-static int launch_conv_bn(const ConvLaunch& L, int grid, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  conv_wgmma_kernel<BN, MODE><<<grid, kConvThreads, L.smem, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
-  return SSDK_OK;
-}
-
 int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int grid_cap) {
   // the kernel is persistent with a static stride over its work units: any grid size computes the same result
   const int grid = grid_cap > 0 ? std::max(1, std::min(L.grid, grid_cap)) : L.grid;
   const bool split = L.args.split != 0;
   SSDK_REQUIRE(!split || L.args.acc_split, "internal: bf16x3 conv plans carry the cross-term accumulator");
   SSDK_REQUIRE(split || L.args.BN != 160, "internal: 160-wide conv tiles are for bf16x3 predictor heads");
-  int rc;
+  decltype(&conv_wgmma_kernel<64, kSingle>) kernel;
   switch (L.args.BN) {
-    case 64: rc = split ? launch_conv_bn<64, kSplitXS>(L, grid, stream) : launch_conv_bn<64, kSingle>(L, grid, stream); break;
-    case 128: rc = split ? launch_conv_bn<128, kSplitXS>(L, grid, stream) : launch_conv_bn<128, kSingle>(L, grid, stream); break;
-    case 160: rc = launch_conv_bn<160, kSplitXS>(L, grid, stream); break;
+    case 64: kernel = split ? conv_wgmma_kernel<64, kSplitXS> : conv_wgmma_kernel<64, kSingle>; break;
+    case 128: kernel = split ? conv_wgmma_kernel<128, kSplitXS> : conv_wgmma_kernel<128, kSingle>; break;
+    case 160: kernel = conv_wgmma_kernel<160, kSplitXS>; break;
     case 256:
       SSDK_REQUIRE(!split, "internal: 256-wide conv tiles have no cross-term accumulator");
-      rc = launch_conv_bn<256, kSingle>(L, grid, stream);
+      kernel = conv_wgmma_kernel<256, kSingle>;
       break;
     default: set_error("internal: conv tile width %d", L.args.BN); return SSDK_ERR_INVALID;
   }
-  if (rc) return rc;
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, kernel, grid, kConvThreads, L.smem, stream, L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
 }
 
 // (x - mean) / std, channel swap (models/keras_ssd300.py:247-272) -> split bf16 planes
@@ -531,10 +517,7 @@ int launch_preprocess(ssdk_ctx* ctx, const float* images, int B, int H, int W, i
   float3 s = stddev ? make_float3(stddev[0], stddev[1], stddev[2]) : make_float3(1, 1, 1);
   int3 sw = swap ? make_int3(swap[0], swap[1], swap[2]) : make_int3(0, 1, 2);
   const size_t total = (size_t)B * H * W;
-  preprocess_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(images, B, H, W, Cimg, m, s, stddev ? 1 : 0, sw, out);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, preprocess_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, images, B, H, W, Cimg, m, s, stddev ? 1 : 0, sw, out);
 }
 
 // Explicit im2col for the few layers the descriptor trick does not cover (3-channel input, strided convs):
@@ -593,18 +576,9 @@ bool im2col_vec8_ok(const ActBuf& in, int Kpad, const void* out_hi, const void* 
 
 int launch_im2col(ssdk_ctx* ctx, const ActBuf& in, __nv_bfloat16* out_hi, __nv_bfloat16* out_lo, int Ho, int Wo, int kh, int kw,
                   int stride, int dil, int pad_t, int pad_l, int Kpad, bool vec8, cudaStream_t stream) {
-  if (vec8) {
-    const size_t total8 = (size_t)in.B * Ho * Wo * (Kpad / 8);
-    im2col8_kernel<<<(unsigned)((total8 + 255) / 256), 256, 0, stream>>>(in, out_hi, out_lo, Ho, Wo, kh, kw, stride, dil, pad_t, pad_l, Kpad);
-    SSDK_COUNT_LAUNCH(ctx);
-    SSDK_CHECK_CUDA(cudaGetLastError());
-    return SSDK_OK;
-  }
-  const size_t total = (size_t)in.B * Ho * Wo * Kpad;
-  im2col_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out_hi, out_lo, Ho, Wo, kh, kw, stride, dil, pad_t, pad_l, Kpad);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  const size_t total = (size_t)in.B * Ho * Wo * (vec8 ? Kpad / 8 : Kpad);
+  return launch(ctx, vec8 ? im2col8_kernel : im2col_kernel, (unsigned)((total + 255) / 256), 256, 0, stream,
+                in, out_hi, out_lo, Ho, Wo, kh, kw, stride, dil, pad_t, pad_l, Kpad);
 }
 
 // Direct fp32 convolution for the image-facing layer (Cin < 8, e.g. conv1_1 3x3x3 or SSD7's conv1 5x5x3): K = kh*kw*cin is
@@ -692,17 +666,9 @@ __global__ void __launch_bounds__(256) conv_direct_kernel(ActBuf in, ActBuf out,
 int launch_conv_direct(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const float* w, const float* bias, const float* bn_scale,
                        const float* bn_shift, int act, int kh, int kw, int dil, int pad_t, int pad_l, cudaStream_t stream) {
   const size_t smem = (size_t)kh * kw * in.C * out.C * sizeof(float);
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_direct_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    attr_set = true;
-  }
   const size_t total = (size_t)out.B * out.H * ((out.W + kDirectPx - 1) / kDirectPx) * (out.C / 16);
   const unsigned blocks = (unsigned)((total + 255) / 256);
-  conv_direct_kernel<0, 0><<<blocks, 256, smem, stream>>>(in, out, w, bias, bn_scale, bn_shift, act, kh, kw, dil, pad_t, pad_l);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, conv_direct_kernel<0, 0>, blocks, 256, smem, stream, in, out, w, bias, bn_scale, bn_shift, act, kh, kw, dil, pad_t, pad_l);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -869,20 +835,10 @@ bool first_border_ok(const ActBuf& in, int kh, int kw, int dil, int pad_t, int p
 }
 int first_tc_supported(int taps, int cin, int cout) { return cin <= 4 && taps * 4 <= 128 && cout % 8 == 0 && cout <= 128; }
 
-template <int BN, int KB, bool SPLIT>
-static int launch_first_bn(const FirstArgs& fa, int grid, size_t smem, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(conv_first_kernel<BN, KB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  conv_first_kernel<BN, KB, SPLIT><<<grid, 256, smem, stream>>>(fa);
-  return SSDK_OK;
-}
 template <int BN>
-static int launch_first_kb(const FirstArgs& fa, int grid, size_t smem, cudaStream_t stream) {
-  if (fa.kblocks == 1) return fa.split ? launch_first_bn<BN, 1, true>(fa, grid, smem, stream) : launch_first_bn<BN, 1, false>(fa, grid, smem, stream);
-  return fa.split ? launch_first_bn<BN, 2, true>(fa, grid, smem, stream) : launch_first_bn<BN, 2, false>(fa, grid, smem, stream);
+static auto first_kernel(const FirstArgs& fa) {
+  if (fa.kblocks == 1) return fa.split ? conv_first_kernel<BN, 1, true> : conv_first_kernel<BN, 1, false>;
+  return fa.split ? conv_first_kernel<BN, 2, true> : conv_first_kernel<BN, 2, false>;
 }
 
 int launch_conv_first(ssdk_ctx* ctx, const FirstPlan& fp, const ActBuf& in, const ActBuf& out, const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo,
@@ -907,12 +863,7 @@ int launch_conv_first(ssdk_ctx* ctx, const FirstPlan& fp, const ActBuf& in, cons
   fa.epi.out_hi = out.hi; fa.epi.out_lo = out.lo; fa.epi.out_Hp = out.Hp(); fa.epi.out_Wp = out.Wp(); fa.epi.out_pad = out.pad; fa.epi.out_Cs = out.Cs;
   const size_t smem = first_smem_bytes(fa.kblocks, BN, fa.split);
   SSDK_REQUIRE(smem <= 227 * 1024, "image-facing convolution: %zu bytes of shared memory", smem);
-  const int grid = fp.grid;
-  const int rc = BN == 64 ? launch_first_kb<64>(fa, grid, smem, stream) : launch_first_kb<128>(fa, grid, smem, stream);
-  if (rc) return rc;
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, BN == 64 ? first_kernel<64>(fa) : first_kernel<128>(fa), fp.grid, 256, smem, stream, fa);
 }
 
 // Max pooling; out-of-range window positions are ignored (TF 'same' pooling pads with -inf).
@@ -1004,16 +955,9 @@ __global__ void __launch_bounds__(256) maxpool2x2_kernel(ActBuf in, ActBuf out) 
 int launch_maxpool(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, int kh, int kw, int stride, int pad_t, int pad_l,
                    cudaStream_t stream) {
   const size_t total = (size_t)out.B * out.H * out.W * (in.Cs / 8);
-  if (kh == 2 && kw == 2 && stride == 2 && pad_t == 0 && pad_l == 0 && 2 * (out.H - 1) < in.H && 2 * (out.W - 1) < in.W) {
-    maxpool2x2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out);
-    SSDK_COUNT_LAUNCH(ctx);
-    SSDK_CHECK_CUDA(cudaGetLastError());
-    return SSDK_OK;
-  }
-  maxpool_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out, kh, kw, stride, pad_t, pad_l);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  if (kh == 2 && kw == 2 && stride == 2 && pad_t == 0 && pad_l == 0 && 2 * (out.H - 1) < in.H && 2 * (out.W - 1) < in.W)
+    return launch(ctx, maxpool2x2_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, in, out);
+  return launch(ctx, maxpool_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, in, out, kh, kw, stride, pad_t, pad_l);
 }
 
 // L2Normalization (keras_layer_L2Normalization.py:61-63): x * rsqrt(max(sum_c x^2, 1e-12)) * gamma_c, one warp per pixel.
@@ -1071,16 +1015,8 @@ __global__ void __launch_bounds__(256) l2norm8_kernel(ActBuf in, ActBuf out, con
 
 int launch_l2norm(ssdk_ctx* ctx, const ActBuf& in, const ActBuf& out, const float* gamma, cudaStream_t stream) {
   const size_t total = (size_t)in.B * in.H * in.W;
-  if (in.C % 8 == 0 && in.C <= 512 && in.Cs == in.C && out.Cs == out.C && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0) {
-    l2norm8_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(in, out, gamma);
-    SSDK_COUNT_LAUNCH(ctx);
-    SSDK_CHECK_CUDA(cudaGetLastError());
-    return SSDK_OK;
-  }
-  l2norm_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(in, out, gamma);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  const bool vec8 = in.C % 8 == 0 && in.C <= 512 && in.Cs == in.C && out.Cs == out.C && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0;
+  return launch(ctx, vec8 ? l2norm8_kernel : l2norm_kernel, (unsigned)((total + 7) / 8), 256, 0, stream, in, out, gamma);
 }
 
 // Reshape / softmax / Concat (models/keras_ssd300.py:363-419): one warp per prior.
@@ -1113,11 +1049,8 @@ __global__ void head_finalize_kernel(const float* __restrict__ head, int B, int 
 int launch_head_finalize(ssdk_ctx* ctx, const float* head, int B, int HW, int n_boxes, int C, int P, int prior_off,
                          const float* anchors, const float* variances, float* y_pred, cudaStream_t stream) {
   const size_t total = (size_t)B * HW * n_boxes;
-  head_finalize_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(head, B, HW, n_boxes, C, P, prior_off, anchors,
-                                                                        make_float4(variances[0], variances[1], variances[2], variances[3]), y_pred);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, head_finalize_kernel, (unsigned)((total + 7) / 8), 256, 0, stream, head, B, HW, n_boxes, C, P, prior_off, anchors,
+                make_float4(variances[0], variances[1], variances[2], variances[3]), y_pred);
 }
 
 __global__ void l2norm_f32_kernel(const float* __restrict__ x, long long rows, int C, const float* __restrict__ gamma,
@@ -1154,18 +1087,12 @@ __global__ void pack_kernel(const float* __restrict__ in, ActBuf out) {
 
 int launch_pack(ssdk_ctx* ctx, const float* in, const ActBuf& out, cudaStream_t stream) {
   const size_t total = (size_t)out.B * out.H * out.W * out.C;
-  pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, pack_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, in, out);
 }
 
 int launch_unpack(ssdk_ctx* ctx, const ActBuf& in, float* out, cudaStream_t stream) {
   const size_t total = (size_t)in.B * in.H * in.W * in.C;
-  unpack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(in, out);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, unpack_kernel, (unsigned)((total + 255) / 256), 256, 0, stream, in, out);
 }
 
 }  // namespace ssdk
@@ -1174,8 +1101,5 @@ extern "C" int ssdk_l2_normalize(ssdk_ctx* ctx, const float* x_dev, long long ro
                                  void* stream) {
   using namespace ssdk;
   SSDK_REQUIRE(ctx && x_dev && gamma_dev && out_dev && rows > 0 && C > 0, "ssdk_l2_normalize: bad argument");
-  l2norm_f32_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x_dev, rows, C, gamma_dev, out_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, l2norm_f32_kernel, (unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream, x_dev, rows, C, gamma_dev, out_dev);
 }

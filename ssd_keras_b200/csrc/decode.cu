@@ -669,11 +669,7 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 template <typename T, bool LAYER>
 int launch_nms(ssdk_ctx* ctx, const NmsParams& np, int B, cudaStream_t stream) {
-  dim3 grid(np.S, B);
-  nms_kernel<T, LAYER><<<grid, kNmsThreads, 0, stream>>>(np);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, nms_kernel<T, LAYER>, dim3(np.S, B), kNmsThreads, 0, stream, np);
 }
 
 int stage1_band(int S, int top_k) {
@@ -719,22 +715,15 @@ int run_nms_topk(ssdk_ctx* ctx, int B, int n, int S, int layer, int box_f64, int
   tp.n = n; tp.S = S; tp.kmax = kmax; tp.top_k = top_k; tp.max_out = max_out; tp.layer = layer;
   tp.cat_score = cat_score; tp.cat_src = cat_src; tp.out = out; tp.out_counts = out_counts; tp.out_index = out_index;
   if (two_stage) { tp.cut_key = cut_key; tp.redo = redo; tp.any_redo = any_redo; }
-  size_t sm = (size_t)kTopCap * sizeof(u64);
-  static bool attr_set = false;
-  if (!attr_set) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm)); attr_set = true; }
-  topk_kernel<<<B, kTopThreads, sm, stream>>>(tp);
-  SSDK_COUNT_LAUNCH(ctx);
-  if (two_stage) {
-    // classes that failed the check: full scan (the other CTAs exit at once), then the top-k of the affected images again
-    np.band_cap = kNmsCap; np.max_bands = 0; np.cut_key = nullptr; np.redo = redo;
-    rc = nms(np);
-    if (rc) return rc;
-    tp.cut_key = nullptr; tp.redo = nullptr; tp.any_redo = nullptr; tp.only_if = any_redo;
-    topk_kernel<<<B, kTopThreads, sm, stream>>>(tp);
-    SSDK_COUNT_LAUNCH(ctx);
-  }
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  const size_t sm = (size_t)kTopCap * sizeof(u64);
+  rc = launch(ctx, topk_kernel, B, kTopThreads, sm, stream, tp);
+  if (rc || !two_stage) return rc;
+  // classes that failed the check: full scan (the other CTAs exit at once), then the top-k of the affected images again
+  np.band_cap = kNmsCap; np.max_bands = 0; np.cut_key = nullptr; np.redo = redo;
+  rc = nms(np);
+  if (rc) return rc;
+  tp.cut_key = nullptr; tp.redo = nullptr; tp.any_redo = nullptr; tp.only_if = any_redo;
+  return launch(ctx, topk_kernel, B, kTopThreads, sm, stream, tp);
 }
 
 size_t nms_scratch_bytes(int B, int S, int kmax) {
@@ -768,9 +757,9 @@ extern "C" int ssdk_decode(ssdk_ctx* ctx, const ssdk_decode_cfg* cfg, const floa
   size_t b_scores = align_up((size_t)B * S * P * 4, 256);
   size_t b_labels = align_up((size_t)B * P * 4, 256);
   size_t total = b_boxes + b_scores + b_labels + nms_scratch_bytes(B, S, cap);
-  int rc = ctx->ws[0].ensure(total);
+  int rc = ctx->decode_ws.ensure(total);
   if (rc) return rc;
-  unsigned char* base = reinterpret_cast<unsigned char*>(ctx->ws[0].ptr);
+  unsigned char* base = reinterpret_cast<unsigned char*>(ctx->decode_ws.ptr);
   void* boxes = base;
   float* scores = reinterpret_cast<float*>(base + b_boxes);
   int* labels = reinterpret_cast<int*>(base + b_boxes + b_scores);
@@ -782,11 +771,8 @@ extern "C" int ssdk_decode(ssdk_ctx* ctx, const ssdk_decode_cfg* cfg, const floa
   pp.boxes = boxes; pp.scores = scores; pp.labels = labels; pp.box_f64 = box_f64;
   size_t sm = (size_t)256 * W * sizeof(float);
   SSDK_REQUIRE(sm <= 227 * 1024, "ssdk_decode: too many classes (%d) for the staging buffer", C);
-  if (sm > 48 * 1024) SSDK_CHECK_CUDA(cudaFuncSetAttribute(dec_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-  dim3 grid(ceil_div(P, 256), B);
-  dec_prepare_kernel<<<grid, 256, sm, stream>>>(pp);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
+  rc = launch(ctx, dec_prepare_kernel, dim3(ceil_div(P, 256), B), 256, sm, stream, pp);
+  if (rc) return rc;
 
   int strict = 1;
   if (!layer && cfg->mode == SSDK_DECODE_FAST) strict = 0;      // decode_detections_fast uses >= (:325)
@@ -803,9 +789,9 @@ extern "C" int ssdk_nms(ssdk_ctx* ctx, const float* boxes_dev, const float* scor
   SSDK_REQUIRE(ctx && boxes_dev && scores_dev && out_dev && out_counts_dev && B > 0 && n > 0, "ssdk_nms: bad argument");
   SSDK_REQUIRE(nms_max_output > 0 && top_k > 0 && top_k <= kTopCap, "ssdk_nms: bad nms_max_output / top_k");
   size_t total = nms_scratch_bytes(B, 1, nms_max_output);
-  int rc = ctx->ws[1].ensure(total);
+  int rc = ctx->nms_ws.ensure(total);
   if (rc) return rc;
   return run_nms_topk(ctx, B, n, 1, 1, 0, 0, scores_dev, nullptr, boxes_dev, 1, confidence_thresh, iou_threshold, 0, 0,
-                      nms_max_output, top_k, top_k, reinterpret_cast<unsigned char*>(ctx->ws[1].ptr), out_dev,
+                      nms_max_output, top_k, top_k, reinterpret_cast<unsigned char*>(ctx->nms_ws.ptr), out_dev,
                       out_counts_dev, out_index_dev, (cudaStream_t)stream_);
 }

@@ -1028,12 +1028,7 @@ struct ssdk_encoder {
   Scratch counters;                 // per-image tickets (self-resetting)
   size_t counters_n = 0;
   Scratch offsets;                  // device copy of the offsets for batches larger than kInlineB
-  // pinned staging ring for those offsets: a slot is reused only after the copy issued from it has completed (no stream sync)
-  static constexpr int kSlots = 8;
-  int* h_offsets = nullptr;   // kSlots * h_offsets_cap ints
-  int h_offsets_cap = 0;
-  cudaEvent_t slot_done[kSlots] = {};
-  int next_slot = 0;
+  HostRing<8> offsets_ring;         // pinned staging of those offsets
   OffsArg offs_arg{};               // ground-truth offsets passed by value with the launch (B <= kInlineB)
 };
 
@@ -1076,10 +1071,7 @@ int upload_tiles(ssdk_encoder* e, const TileSetHost* h, int n_linear_tiles, Tile
   }
   o.dev.bbox = o.d_bbox;
   o.dev.cls = o.d_cls;
-  tile_bbox_kernel<<<n_tiles, kTile>>>(e->p, o.dev, o.d_bbox, o.d_cls);
-  SSDK_COUNT_LAUNCH(e->ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(e->ctx, tile_bbox_kernel, n_tiles, kTile, 0, nullptr, e->p, o.dev, o.d_bbox, o.d_cls);
 }
 
 // every prior exactly once, every thread's staging slot inside its tile's runs exactly once
@@ -1109,8 +1101,6 @@ bool tiles_cover(const TileSetHost& h, int P) {
   for (char c : seen) if (!c) return false;
   return true;
 }
-
-size_t g_smem_attr[2] = {0, 0};
 
 }  // namespace
 
@@ -1169,19 +1159,14 @@ extern "C" int ssdk_encoder_destroy(ssdk_encoder* e) {
   cudaFree(e->d_anchors);
   e->linear.release(); e->spatial.release();
   e->tiles.release(); e->counters.release(); e->offsets.release();
-  if (e->h_offsets) cudaFreeHost(e->h_offsets);
-  for (int i = 0; i < ssdk_encoder::kSlots; ++i) if (e->slot_done[i]) cudaEventDestroy(e->slot_done[i]);
+  e->offsets_ring.release();
   delete e;
   return SSDK_OK;
 }
 
 extern "C" int ssdk_iou_matrix(ssdk_encoder* e, const float* gt_boxes_dev, int G, double* out_dev, void* stream) {
   SSDK_REQUIRE(e && gt_boxes_dev && out_dev && G > 0, "ssdk_iou_matrix: bad argument");
-  dim3 grid(ceil_div(e->p.P, 256), G);
-  iou_matrix_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(e->p, gt_boxes_dev, G, out_dev);
-  SSDK_COUNT_LAUNCH(e->ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(e->ctx, iou_matrix_kernel, dim3(ceil_div(e->p.P, 256), G), 256, 0, (cudaStream_t)stream, e->p, gt_boxes_dev, G, out_dev);
 }
 
 extern "C" int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const double* boxes2_dev, int n, int coords, int border_d,
@@ -1190,11 +1175,8 @@ extern "C" int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const do
   SSDK_REQUIRE(coords >= 0 && coords <= 2, "Unexpected value for `coords`. Supported values are 'minmax', 'corners' and 'centroids'.");
   SSDK_REQUIRE(!elementwise || m == n || m == 1 || n == 1, "ssdk_iou: element-wise mode needs broadcast-compatible box counts");
   long long total = elementwise ? (long long)(m > n ? m : n) : (long long)m * n;
-  iou_general_kernel<<<(unsigned)ceil_div_ll(total, 256), 256, 0, (cudaStream_t)stream>>>(boxes1_dev, m, boxes2_dev, n, coords,
-                                                                                          border_d, elementwise, out_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, iou_general_kernel, (unsigned)ceil_div_ll(total, 256), 256, 0, (cudaStream_t)stream, boxes1_dev, m, boxes2_dev, n,
+                coords, border_d, elementwise, out_dev);
 }
 
 namespace {
@@ -1245,54 +1227,30 @@ int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* of
   sc.counters = reinterpret_cast<int*>(e->counters.ptr);
   const EncSmem L = enc_smem_layout(W, max_g);
   SSDK_REQUIRE(L.total <= 227 * 1024, "ssdk_encode: n_classes (%d) / gt count (%d) need %zu bytes of shared memory", p.C, max_g, L.total);
+  // enc_tiles_kernel takes all of it as dynamic shared memory: if (L.total > 48 * 1024), ssdk::launch raises the kernel's limit first
   dim3 grid(ceil_div(ts.n_tiles, tpc), B);
   dim3 grid_lb(ceil_div(max_g, kTile / 32), B);
   const bool inline_offs = offs_host != nullptr && B <= kInlineB;
+  const int* d_offs = nullptr;
   if (inline_offs) {
-    if (L.total > 48 * 1024 && L.total > g_smem_attr[0]) {   // the attribute belongs to the kernel, not to an encoder: only ever raise it
-      SSDK_CHECK_CUDA(cudaFuncSetAttribute(enc_tiles_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-      g_smem_attr[0] = L.total;
-    }
-    OffsArg& arg = e->offs_arg;
-    memcpy(arg.v, offs_host, (size_t)(B + 1) * sizeof(int));
-    if (use_lb) {
-      enc_lb_kernel<true><<<grid_lb, kTile, 0, stream>>>(p, ts, arg, nullptr, gt_dev, gt_f64, lb);
-      SSDK_COUNT_LAUNCH(e->ctx);
-    }
-    enc_tiles_kernel<true><<<grid, kTile, L.total, stream>>>(p, ts, arg, nullptr, gt_dev, gt_f64, tpc, sc, out_y_dev, out_match_dev, status_dev);
-  } else {
-    const int* d_offs = offs_dev;
-    if (!d_offs) {                                         // large batch with host offsets: pinned ring + async copy
-      rc = e->offsets.ensure((size_t)(B + 1) * sizeof(int));
-      if (rc) return rc;
-      if (e->h_offsets_cap < B + 1) {
-        SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));
-        if (e->h_offsets) cudaFreeHost(e->h_offsets);
-        SSDK_CHECK_CUDA(cudaMallocHost(&e->h_offsets, (size_t)ssdk_encoder::kSlots * (B + 1) * sizeof(int)));
-        e->h_offsets_cap = B + 1;
-      }
-      const int slot = e->next_slot;
-      e->next_slot = (slot + 1) % ssdk_encoder::kSlots;
-      if (!e->slot_done[slot]) SSDK_CHECK_CUDA(cudaEventCreateWithFlags(&e->slot_done[slot], cudaEventDisableTiming));
-      else SSDK_CHECK_CUDA(cudaEventSynchronize(e->slot_done[slot]));
-      int* h_off = e->h_offsets + (size_t)slot * e->h_offsets_cap;
-      memcpy(h_off, offs_host, (size_t)(B + 1) * sizeof(int));
-      SSDK_CHECK_CUDA(cudaMemcpyAsync(e->offsets.ptr, h_off, (size_t)(B + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
-      SSDK_CHECK_CUDA(cudaEventRecord(e->slot_done[slot], stream));
-      d_offs = reinterpret_cast<const int*>(e->offsets.ptr);
-    }
-    if (L.total > 48 * 1024 && L.total > g_smem_attr[1]) {
-      SSDK_CHECK_CUDA(cudaFuncSetAttribute(enc_tiles_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-      g_smem_attr[1] = L.total;
-    }
-    if (use_lb) {
-      enc_lb_kernel<false><<<grid_lb, kTile, 0, stream>>>(p, ts, e->offs_arg, d_offs, gt_dev, gt_f64, lb);
-      SSDK_COUNT_LAUNCH(e->ctx);
-    }
-    enc_tiles_kernel<false><<<grid, kTile, L.total, stream>>>(p, ts, e->offs_arg, d_offs, gt_dev, gt_f64, tpc, sc, out_y_dev, out_match_dev, status_dev);
+    memcpy(e->offs_arg.v, offs_host, (size_t)(B + 1) * sizeof(int));
+  } else if (offs_dev) {
+    d_offs = offs_dev;
+  } else {                                                 // large batch with host offsets: pinned ring + async copy
+    rc = e->offsets.ensure((size_t)(B + 1) * sizeof(int));
+    if (rc) return rc;
+    rc = e->offsets_ring.upload(e->offsets.ptr, stream, {{offs_host, (size_t)(B + 1) * sizeof(int)}});
+    if (rc) return rc;
+    d_offs = reinterpret_cast<const int*>(e->offsets.ptr);
   }
-  SSDK_COUNT_LAUNCH(e->ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
+  if (use_lb) {
+    rc = launch(e->ctx, inline_offs ? enc_lb_kernel<true> : enc_lb_kernel<false>, grid_lb, kTile, 0, stream,
+                p, ts, e->offs_arg, d_offs, gt_dev, gt_f64, lb);
+    if (rc) return rc;
+  }
+  rc = launch(e->ctx, inline_offs ? enc_tiles_kernel<true> : enc_tiles_kernel<false>, grid, kTile, L.total, stream,
+              p, ts, e->offs_arg, d_offs, gt_dev, gt_f64, tpc, sc, out_y_dev, out_match_dev, status_dev);
+  if (rc) return rc;
   if (sc.prof) {                                                // experiments only: synchronises
     unsigned long long h[16];
     SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));

@@ -5,10 +5,10 @@
 // :679) with the ground-truth boxes of its image that have the same class, matched to the best one if the overlap reaches the
 // threshold and that box is still free, else counted as a false positive (neutral boxes: neither).  The only sequential
 // dependency is the "still free" state of a ground-truth box, which is private to one (class, image) pair -- so:
-//   eval_match_kernel   one warp per (class, image) segment of the predictions (sorted by class, image, confidence desc):
-//                       lanes share the image's boxes of that class, the IoU in the types NumPy uses (below), warp arg-max
-//                       with np.argmax's rules (first maximum; the first NaN wins), flags written at the prediction's position
-//                       in (class, confidence) order.
+//   eval_match_kernel   one warp per (class, image) segment of the predictions (sorted by class, image, confidence desc), eight
+//                       per CTA (eval_match_kernel<<<ceil_div(n_seg, 8), 256, 0, stream>>>): lanes share the image's boxes of
+//                       that class, the IoU in the types NumPy uses (below), warp arg-max with np.argmax's rules (first
+//                       maximum; the first NaN wins), flags written at the prediction's position in (class, confidence) order.
 //   eval_cumsum_kernel  one CTA per class: inclusive scans of the two flag arrays (np.cumsum, :726-727).
 // Sorting (two stable key sorts) is done by the caller; precision / recall / AP are a few vector operations on the cumulative
 // counts (host, same NumPy expressions as the reference).
@@ -223,12 +223,8 @@ extern "C" int ssdk_eval_collect(ssdk_ctx* ctx, const float* rows_dev, int B, in
   if (B == 0 || max_out == 0) return SSDK_OK;
   SSDK_REQUIRE(rows_dev && inv_dev && (capacity == 0 || (out_image_dev && out_class_dev && out_conf_dev && out_box_dev)),
                "ssdk_eval_collect: NULL argument");
-  eval_collect_kernel<<<1, 1024, 0, (cudaStream_t)stream_>>>(rows_dev, B, max_out, counts_dev, inv_dev, cc, f64 ? 1 : 0, pad ? 1 : 0, conf_decimals,
-                                                             image_base, capacity, count_dev, out_image_dev, out_class_dev, out_conf_dev,
-                                                             out_box_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, eval_collect_kernel, 1, 1024, 0, (cudaStream_t)stream_, rows_dev, B, max_out, counts_dev, inv_dev, cc, f64 ? 1 : 0,
+                pad ? 1 : 0, conf_decimals, image_base, capacity, count_dev, out_image_dev, out_class_dev, out_conf_dev, out_box_dev);
 }
 
 extern "C" int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets_dev, int n_seg, const int* pred_image_dev,
@@ -242,17 +238,11 @@ extern "C" int ssdk_eval_match(ssdk_ctx* ctx, int n_pred, const int* seg_offsets
                gt_f32_dev && gt_matched_dev && tp_dev && fp_dev, "ssdk_eval_match: NULL argument");
   EvalArgs a{seg_offsets_dev, pred_image_dev, pred_class_dev, pred_box_dev, pred_rank_dev, gt_rows_dev, gt_offsets_dev, gt_f32_dev,
              gt_neutral_dev, gt_matched_dev, matching_iou_threshold, border_d, tp_dev, fp_dev};
-  eval_match_kernel<<<ceil_div(n_seg, 8), 256, 0, (cudaStream_t)stream_>>>(a, n_seg);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, eval_match_kernel, ceil_div(n_seg, 8), 256, 0, (cudaStream_t)stream_, a, n_seg);
 }
 
 extern "C" int ssdk_eval_cumsum(ssdk_ctx* ctx, const int* tp_dev, const int* fp_dev, const int* class_offsets_dev, int n_segments,
                                 int* ctp_dev, int* cfp_dev, void* stream_) {
   SSDK_REQUIRE(ctx && tp_dev && fp_dev && class_offsets_dev && ctp_dev && cfp_dev && n_segments > 0, "ssdk_eval_cumsum: bad argument");
-  eval_cumsum_kernel<<<n_segments, 1024, 0, (cudaStream_t)stream_>>>(tp_dev, fp_dev, class_offsets_dev, ctp_dev, cfp_dev);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, eval_cumsum_kernel, n_segments, 1024, 0, (cudaStream_t)stream_, tp_dev, fp_dev, class_offsets_dev, ctp_dev, cfp_dev);
 }

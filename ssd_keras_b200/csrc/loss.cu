@@ -598,14 +598,11 @@ int plan_launch(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, 
   const size_t limit = ctx->prop.sharedMemPerBlockOptin - static_smem;
   SSDK_REQUIRE(plan.smem <= limit, "ssd_loss: %d classes need %zu bytes of shared memory per CTA%s, at most %zu fit", C, plan.smem,
                grad ? " with the gradient" : "", limit);
-  static size_t attr[2] = {0, 0};
-  if (plan.smem > 48 * 1024) {
-    if (plan.smem > attr[0]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[0] = plan.smem; }
-    if (plan.smem > attr[1]) { SSDK_CHECK_CUDA(cudaFuncSetAttribute(ssd_loss_phase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem)); attr[1] = plan.smem; }
-  }
+  const void* kernel = cooperative ? (const void*)ssd_loss_kernel : (const void*)ssd_loss_phase_kernel;
+  const int rc = allow_smem(ctx, kernel, plan.smem);             // the occupancy query needs the raised limit
+  if (rc) return rc;
   int per_sm = 0;
-  if (cooperative) SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_kernel, kRows, plan.smem));
-  else SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ssd_loss_phase_kernel, kRows, plan.smem));
+  SSDK_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kRows, plan.smem));
   SSDK_REQUIRE(per_sm > 0, "ssd_loss: the kernel does not fit on an SM (%zu bytes of shared memory)", plan.smem);
   if (per_sm > 4) per_sm = 4;
   const int n_tiles = B * ((P + kRows - 1) / kRows);
@@ -643,15 +640,15 @@ long long ws_key(int B, int P) { return (long long)B << 32 | (unsigned)P; }
 // refused before the launch must not flip it: the set it would have cleared is the one the next call counts in)
 int own_ws(ssdk_ctx* ctx, int B, int P, unsigned char** ws, int* parity, cudaStream_t stream) {
   const WsLayout L = ws_layout(B, P);
-  const size_t before = ctx->ws[2].bytes;
-  int rc = ctx->ws[2].ensure(L.total);
+  const size_t before = ctx->loss_ws.bytes;
+  int rc = ctx->loss_ws.ensure(L.total);
   if (rc) return rc;
-  if (ctx->ws[2].bytes != before || ctx->loss_ws_shape != ws_key(B, P)) {
-    SSDK_CHECK_CUDA(cudaMemsetAsync(ctx->ws[2].ptr, 0, ctx->ws[2].bytes, stream));   // layout moved: start from clean histograms
+  if (ctx->loss_ws.bytes != before || ctx->loss_ws_shape != ws_key(B, P)) {
+    SSDK_CHECK_CUDA(cudaMemsetAsync(ctx->loss_ws.ptr, 0, ctx->loss_ws.bytes, stream));   // layout moved: start from clean histograms
     ctx->loss_ws_shape = ws_key(B, P);
     ctx->loss_parity = 0;
   }
-  *ws = reinterpret_cast<unsigned char*>(ctx->ws[2].ptr);
+  *ws = reinterpret_cast<unsigned char*>(ctx->loss_ws.ptr);
   *parity = ctx->loss_parity;
   return SSDK_OK;
 }
@@ -659,10 +656,7 @@ int own_ws(ssdk_ctx* ctx, int B, int P, unsigned char** ws, int* parity, cudaStr
 int launch_fused(ssdk_ctx* ctx, LossArgs& a, const LossPlan& plan, cudaStream_t stream) {
   // the counts are cleared per call (16 bytes); histograms are self-cleaning (parity), the ticket resets itself
   SSDK_CHECK_CUDA(cudaMemsetAsync(a.counts, 0, 16, stream));
-  void* params[] = {(void*)&a};
-  SSDK_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)ssd_loss_kernel, dim3(plan.grid), dim3(kRows), params, plan.smem, stream));
-  SSDK_COUNT_LAUNCH(ctx);
-  return SSDK_OK;
+  return launch_cooperative(ctx, ssd_loss_kernel, plan.grid, kRows, plan.smem, stream, a);
 }
 
 int loss_run(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C, int ratio, int n_neg_min, float alpha,
@@ -744,9 +738,9 @@ extern "C" int ssdk_ssd_loss_read_box_losses(ssdk_ctx* ctx, const void* ws_dev, 
   SSDK_REQUIRE(ctx && B > 0 && P > 0 && (cls_dev || negl_dev), "ssdk_ssd_loss_read_box_losses: bad argument");
   const unsigned char* ws = reinterpret_cast<const unsigned char*>(ws_dev);
   if (!ws) {
-    SSDK_REQUIRE(ctx->ws[2].ptr && ctx->loss_ws_shape == ws_key(B, P),
+    SSDK_REQUIRE(ctx->loss_ws.ptr && ctx->loss_ws_shape == ws_key(B, P),
                  "ssdk_ssd_loss_read_box_losses: the context's loss workspace does not hold a (%d, %d) batch", B, P);
-    ws = reinterpret_cast<const unsigned char*>(ctx->ws[2].ptr);
+    ws = reinterpret_cast<const unsigned char*>(ctx->loss_ws.ptr);
   }
   const WsLayout L = ws_layout(B, P);
   const size_t bytes = (size_t)B * P * 4;
@@ -772,9 +766,5 @@ extern "C" int ssdk_ssd_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true
   a.global_B = global_B; a.n_total = (long long)global_B * P;
   a.ties_all = ties_all_dev; a.rank = rank;
   if (phase == 4) { a.out_loss = out_loss; a.out_stats = out_stats; a.upstream = upstream; a.out_grad = out_grad; }
-  const int grid = phase == 3 ? 1 : plan.grid;
-  ssd_loss_phase_kernel<<<grid, kRows, plan.smem, stream>>>(a, phase);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, ssd_loss_phase_kernel, phase == 3 ? 1 : plan.grid, kRows, plan.smem, stream, a, phase);
 }

@@ -252,10 +252,7 @@ int launch_repack(ssdk_ctx* ctx, const float* w, int taps, int cin, int cout, We
                   __nv_bfloat16* hi, __nv_bfloat16* lo, cudaStream_t s) {
   const int rows = layout == PACK_DGRAD ? cin : layout == PACK_DGRAD_COL ? taps * cin : cout;
   const size_t total = (size_t)rows * krow;
-  repack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(w, taps, cin, cout, layout, kblocks, krow, rows, hi, lo);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, repack_kernel, (unsigned)((total + 255) / 256), 256, 0, s, w, taps, cin, cout, layout, kblocks, krow, rows, hi, lo);
 }
 
 // Geometry, tile list, pipeline depths and TMA descriptors of one implicit-GEMM launch.  The caller fills the epilogue.

@@ -785,11 +785,8 @@ namespace {
 
 int do_transpose(ssdk_trainer* t, const __nv_bfloat16* hi, const __nv_bfloat16* lo, int src_ld, long long src_rows, const TMap& mp,
                  long long Kv, int C, __nv_bfloat16* dhi, __nv_bfloat16* dlo, long long ldT, cudaStream_t s, long long row_off = 0) {
-  dim3 grid((unsigned)((ldT + 63) / 64), (unsigned)((C + 63) / 64));
-  transpose_kernel<<<grid, 256, 0, s>>>(hi, lo, src_ld, src_rows, mp, row_off, Kv, C, dhi, dlo, ldT);
-  SSDK_COUNT_LAUNCH(t->m->ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(t->m->ctx, transpose_kernel, dim3((unsigned)((ldT + 63) / 64), (unsigned)((C + 63) / 64)), 256, 0, s,
+                hi, lo, src_ld, src_rows, mp, row_off, Kv, C, dhi, dlo, ldT);
 }
 
 }  // namespace
@@ -859,16 +856,17 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     const int relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
     if (d.op == SSDK_OP_HEAD) {
       const size_t total = (size_t)m->B * L.H * L.W * d.n_boxes;
-      head_bwd_kernel<<<(unsigned)((total + 7) / 8), 256, 0, s>>>(L.head_f32, dypred, m->B, L.H, L.W, d.n_boxes, m->Ctot, m->P, L.prior_off, T.g);
-      SSDK_COUNT_LAUNCH(ctx);
+      rc = launch(ctx, head_bwd_kernel, (unsigned)((total + 7) / 8), 256, 0, s, L.head_f32, dypred, m->B, L.H, L.W, d.n_boxes, m->Ctot, m->P,
+                  L.prior_off, T.g);
+      if (rc) return rc;
     }
     if (d.op == SSDK_OP_MAXPOOL) {
       if (prod_needs_grad) {
         if (PL.out.C % 8) { set_error("training: max-pool channels must be a multiple of 8"); return SSDK_ERR_UNSUPPORTED; }
         const size_t total = (size_t)PL.out.B * PL.out.H * PL.out.W * (PL.out.C / 8);
-        pool_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(PL.out, T.g, PT.g, L.H, L.W, d.kh, d.kw, d.stride, d.pad_t, d.pad_l,
-                                                                         relu_mask, written[pi] ? 1 : 0);
-        SSDK_COUNT_LAUNCH(ctx);
+        rc = launch(ctx, pool_bwd_kernel, (unsigned)((total + 255) / 256), 256, 0, s, PL.out, T.g, PT.g, L.H, L.W, d.kh, d.kw, d.stride,
+                    d.pad_t, d.pad_l, relu_mask, written[pi] ? 1 : 0);
+        if (rc) return rc;
         written[pi] = 1;
       }
       continue;
@@ -876,8 +874,9 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     if (d.op == SSDK_OP_L2NORM) {
       if (prod_needs_grad) {
         const size_t total = (size_t)PL.out.B * PL.out.H * PL.out.W;
-        l2norm_bwd_kernel<<<(unsigned)((total + 7) / 8), 256, 0, s>>>(PL.out, T.g, PT.g, L.gamma, span_grad(t, i, 2), relu_mask, written[pi] ? 1 : 0);
-        SSDK_COUNT_LAUNCH(ctx);
+        rc = launch(ctx, l2norm_bwd_kernel, (unsigned)((total + 7) / 8), 256, 0, s, PL.out, T.g, PT.g, L.gamma, span_grad(t, i, 2), relu_mask,
+                    written[pi] ? 1 : 0);
+        if (rc) return rc;
         written[pi] = 1;
       }
       continue;
@@ -890,18 +889,14 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       const int K = T.taps * T.cin;
       const size_t smem = (size_t)K * T.cout * sizeof(float);
       // the plan admits direct layers whose fp32 [K][Cout] accumulator needs up to 96 KB (model.cu, as conv_direct_kernel)
-      static bool attr_set = false;
-      if (!attr_set) {
-        SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct3x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr_set = true;
-      }
       const int total_rows = T.g.B * T.g.H;
       const int rpb = std::max(1, (total_rows + 8 * ctx->sm_count - 1) / (8 * ctx->sm_count));
-      const bool fast3 = direct_fast3(d, PL.out, T.cin, T.cout);
-      if (fast3) wgrad_direct3x3_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, span_grad(t, i, 0), d.pad_t, d.pad_l, rpb);
-      else wgrad_direct_kernel<<<(unsigned)((total_rows + rpb - 1) / rpb), 256, smem, s>>>(PL.out, T.g, span_grad(t, i, 0), d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
-      SSDK_COUNT_LAUNCH(ctx);
+      const unsigned grid = (unsigned)((total_rows + rpb - 1) / rpb);
+      if (direct_fast3(d, PL.out, T.cin, T.cout))
+        rc = launch(ctx, wgrad_direct3x3_kernel, grid, 256, smem, s, PL.out, T.g, span_grad(t, i, 0), d.pad_t, d.pad_l, rpb);
+      else
+        rc = launch(ctx, wgrad_direct_kernel, grid, 256, smem, s, PL.out, T.g, span_grad(t, i, 0), d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
+      if (rc) return rc;
       rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     } else if (T.wg_native) {
       rc = launch_wgrad(ctx, T.wg, s); if (rc) return rc;
@@ -923,17 +918,16 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
             if (T.wgrad_res[tp] == r) { rc = launch_conv(ctx, T.wgrad[tp], s); if (rc) return rc; }
         }
       }
-      dim3 gr(64, T.cout);
-      rowsum_kernel<<<gr, 256, 0, s>>>(t->dyT_hi, t->dyT_lo, T.ldT, T.Kv, span_grad(t, i, 1));
-      SSDK_COUNT_LAUNCH(ctx);
+      rc = launch(ctx, rowsum_kernel, dim3(64, T.cout), 256, 0, s, t->dyT_hi, t->dyT_lo, T.ldT, T.Kv, span_grad(t, i, 1));
+      if (rc) return rc;
     }
     // ---- data gradient
     if (T.has_dgrad && T.dgrad_strided) {
       rc = launch_conv(ctx, T.dgrad, s); if (rc) return rc;
       const size_t total = (size_t)PT.g.B * PT.g.H * PT.g.W * PT.g.C;
-      col2im_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(T.dcol, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t, d.pad_l, T.dcol_ld,
-                                                                     PL.out, PT.g, T.dgrad_relu_mask, written[pi] ? 1 : 0);
-      SSDK_COUNT_LAUNCH(ctx);
+      rc = launch(ctx, col2im_kernel, (unsigned)((total + 255) / 256), 256, 0, s, T.dcol, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t,
+                  d.pad_l, T.dcol_ld, PL.out, PT.g, T.dgrad_relu_mask, written[pi] ? 1 : 0);
+      if (rc) return rc;
       written[pi] = 1;
     } else if (T.has_dgrad) {
       T.dgrad.args.accumulate = written[pi] ? 1 : 0;
@@ -941,7 +935,6 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       written[pi] = 1;
     }
   }
-  SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
@@ -953,12 +946,8 @@ bool ends_conv_layer(const ssdk_trainer* t, size_t k) {
 
 // span p of `src` (its value, or its optimiser state) into out_dev, in the gradient's layout
 int read_span(ssdk_trainer* t, const ParamSpan& p, const float* src, float* out_dev, cudaStream_t s) {
-  if (p.taps) {
-    hwio_to_ohwi_kernel<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(src, p.taps, p.cin, p.cout, out_dev + p.off);
-    SSDK_COUNT_LAUNCH(t->m->ctx);
-  } else {
-    SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + p.off, src, (size_t)p.count * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  }
+  if (p.taps) return launch(t->m->ctx, hwio_to_ohwi_kernel, (unsigned)((p.count + 255) / 256), 256, 0, s, src, p.taps, p.cin, p.cout, out_dev + p.off);
+  SSDK_CHECK_CUDA(cudaMemcpyAsync(out_dev + p.off, src, (size_t)p.count * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return SSDK_OK;
 }
 
@@ -969,13 +958,11 @@ extern "C" int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float
   cudaStream_t s = (cudaStream_t)stream_;
   for (size_t k = 0; k < t->params.size(); ++k) {
     const ParamSpan& p = t->params[k];
-    const auto sgd = p.taps ? sgd_kernel<true> : sgd_kernel<false>;
-    sgd<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(p.value, t->state[0] + p.off, t->grad + p.off, (size_t)p.count, p.taps, p.cin, p.cout,
-                                                           lr, momentum, l2_reg, grad_scale);
-    SSDK_COUNT_LAUNCH(t->m->ctx);
-    if (ends_conv_layer(t, k)) { const int rc = repack_layer(t, p.layer, s); if (rc) return rc; }
+    int rc = launch(t->m->ctx, p.taps ? sgd_kernel<true> : sgd_kernel<false>, (unsigned)((p.count + 255) / 256), 256, 0, s, p.value,
+                    t->state[0] + p.off, t->grad + p.off, (size_t)p.count, p.taps, p.cin, p.cout, lr, momentum, l2_reg, grad_scale);
+    if (rc == SSDK_OK && ends_conv_layer(t, k)) rc = repack_layer(t, p.layer, s);
+    if (rc) return rc;
   }
-  SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
@@ -988,13 +975,12 @@ extern "C" int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, flo
   if (!t->state[1]) { const int rc = dev_alloc(t->allocs, &t->state[1], (size_t)t->n_params, true); if (rc) return rc; }
   for (size_t k = 0; k < t->params.size(); ++k) {
     const ParamSpan& p = t->params[k];
-    const auto adam = p.taps ? adam_kernel<true> : adam_kernel<false>;
-    adam<<<(unsigned)((p.count + 255) / 256), 256, 0, s>>>(p.value, t->state[0] + p.off, t->state[1] + p.off, t->grad + p.off, (size_t)p.count,
-                                                            p.taps, p.cin, p.cout, lr_t, beta1, beta2, eps, l2_reg, grad_scale);
-    SSDK_COUNT_LAUNCH(t->m->ctx);
-    if (ends_conv_layer(t, k)) { const int rc = repack_layer(t, p.layer, s); if (rc) return rc; }
+    int rc = launch(t->m->ctx, p.taps ? adam_kernel<true> : adam_kernel<false>, (unsigned)((p.count + 255) / 256), 256, 0, s, p.value,
+                    t->state[0] + p.off, t->state[1] + p.off, t->grad + p.off, (size_t)p.count, p.taps, p.cin, p.cout, lr_t, beta1, beta2, eps,
+                    l2_reg, grad_scale);
+    if (rc == SSDK_OK && ends_conv_layer(t, k)) rc = repack_layer(t, p.layer, s);
+    if (rc) return rc;
   }
-  SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
@@ -1007,7 +993,6 @@ extern "C" int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out
     const int rc = read_span(t, p, t->state[slot] + p.off, out_dev, (cudaStream_t)stream_);
     if (rc) return rc;
   }
-  SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }
 
@@ -1033,6 +1018,5 @@ extern "C" int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* s
     const int rc = read_span(t, p, p.value, out_dev, (cudaStream_t)stream_);
     if (rc) return rc;
   }
-  SSDK_CHECK_CUDA(cudaGetLastError());
   return SSDK_OK;
 }

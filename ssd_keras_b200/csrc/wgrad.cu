@@ -216,25 +216,11 @@ int plan_wgrad(ssdk_ctx* ctx, WgradLaunch& L, const ActBuf& X, const ActBuf& G, 
   return SSDK_OK;
 }
 
-template <int BNc, bool SPLIT>
-static int launch_wgrad_bn(const WgradLaunch& L, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SSDK_CHECK_CUDA(cudaFuncSetAttribute(wgrad_wgmma_kernel<BNc, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  wgrad_wgmma_kernel<BNc, SPLIT><<<L.grid, 256, L.smem, stream>>>(L.g_hi, L.g_lo, L.x_hi, L.x_lo, L.args);
-  return SSDK_OK;
-}
-
 int launch_wgrad(ssdk_ctx* ctx, const WgradLaunch& L, cudaStream_t stream) {
   const bool sp = L.args.split != 0;
-  const int rc = L.args.BNc == 128 ? (sp ? launch_wgrad_bn<128, true>(L, stream) : launch_wgrad_bn<128, false>(L, stream))
-                                   : (sp ? launch_wgrad_bn<64, true>(L, stream) : launch_wgrad_bn<64, false>(L, stream));
-  if (rc) return rc;
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  const auto kernel = L.args.BNc == 128 ? (sp ? wgrad_wgmma_kernel<128, true> : wgrad_wgmma_kernel<128, false>)
+                                        : (sp ? wgrad_wgmma_kernel<64, true> : wgrad_wgmma_kernel<64, false>);
+  return launch(ctx, kernel, L.grid, 256, L.smem, stream, L.g_hi, L.g_lo, L.x_hi, L.x_lo, L.args);
 }
 
 int launch_bias_grad(ssdk_ctx* ctx, const ActBuf& G, float* gb, cudaStream_t stream) {
@@ -243,10 +229,7 @@ int launch_bias_grad(ssdk_ctx* ctx, const ActBuf& G, float* gb, cudaStream_t str
   const int blocks = (int)std::min<long long>(4LL * ctx->sm_count, std::max<long long>(1, rows / 64));
   const long long rpb = (rows + blocks - 1) / blocks;
   const int RL = 256 / (G.Cs / 8);
-  bias_grad_kernel<<<blocks, 256, (size_t)std::max(1, RL) * G.Cs * sizeof(float), stream>>>(G.hi, G.lo, G.Cs, G.C, rows, rpb, gb);
-  SSDK_COUNT_LAUNCH(ctx);
-  SSDK_CHECK_CUDA(cudaGetLastError());
-  return SSDK_OK;
+  return launch(ctx, bias_grad_kernel, blocks, 256, (size_t)std::max(1, RL) * G.Cs * sizeof(float), stream, G.hi, G.lo, G.Cs, G.C, rows, rpb, gb);
 }
 
 }  // namespace ssdk

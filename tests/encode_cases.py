@@ -25,6 +25,7 @@ from oracle.encoder import OracleEncoder
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ENCODE_CU = os.path.join(ROOT, 'ssd_keras_b200', 'csrc', 'encode.cu')
+COMMON_CUH = os.path.join(ROOT, 'ssd_keras_b200', 'csrc', 'common.cuh')
 GOLDEN_DIR = os.path.join(ROOT, 'tests', 'golden')
 
 
@@ -37,8 +38,11 @@ def kernel_constants():
     k['spatial_min'], k['lb_min'] = int(m.group(1)), int(m.group(2))
     m = re.search(r'int tpc = max_g <= (\d+) \? 1 : \(max_g <= (\d+) \? 2 : \(max_g < (\d+) \? 4 : 8\)\);', src)
     k['tpc_ladder'] = tuple(int(v) for v in m.groups())
-    m = re.search(r'if \(L.total > 48 \* 1024', src)
-    assert m, 'dynamic shared-memory opt-in'
+    # enc_tiles_kernel gets L.total bytes of dynamic shared memory through ssdk::launch, which opts in above 48 KB
+    m = re.search(r'launch\(e->ctx, inline_offs \? enc_tiles_kernel<true> : enc_tiles_kernel<false>, grid, kTile, L\.total,', src)
+    assert m, 'dynamic shared memory of enc_tiles_kernel'
+    with open(COMMON_CUH) as f:
+        assert 'if (bytes <= 48 * 1024) return SSDK_OK;' in f.read(), 'dynamic shared-memory opt-in'
     m = re.search(r'SSDK_REQUIRE\(L.total <= (\d+) \* 1024', src)
     k['smem_max'] = int(m.group(1)) * 1024
     return k

@@ -30,7 +30,7 @@ def _constants():
     with open(EVALUATE_CU) as f:
         src = f.read()
     lanes = int(re.search(r'for \(int g = g0 \+ lane; g < g1; g \+= (\d+)\)', src).group(1))
-    warps = int(re.search(r'eval_match_kernel<<<ceil_div\(n_seg, (\d+)\), (\d+),', src).group(1))
+    warps = int(re.search(r'launch\(ctx, eval_match_kernel, ceil_div\(n_seg, (\d+)\), (\d+),', src).group(1))
     chunk = int(re.search(r'for \(int base = lo; base < hi; base \+= (\d+)\)', src).group(1))
     return lanes, warps, chunk
 

@@ -35,6 +35,8 @@ def test_kernel_constants_are_read_from_the_source():
     assert 'if (is_nan || best_g == INT_MAX || (double)v > best)' in src
     assert 'const double thr = (double)(T)a.thr;' in src
     assert 'if (a.gt_f32[img]) match_segment<float>' in src
+    # the launch shape the file's header documents is the one it launches
+    assert 'eval_match_kernel<<<ceil_div(n_seg, %d), %d, 0, stream>>>' % (xc.WARPS_PER_CTA, 32 * xc.WARPS_PER_CTA) in src
 
 
 @pytest.mark.parametrize('name', xc.EDGES)
