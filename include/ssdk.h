@@ -158,6 +158,8 @@ int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const double* boxes
  *             boxes += dx_abs / dy_abs                                  (Translate.__call__, object_detection_2d_geometric_ops.py:276-317)
  *   SCALE     a0=factor a1=image height a2=image width: both corners through M = getRotationMatrix2D((w/2, h/2), 0, factor)
  *             as np.dot computes it, (m0*x + m1*y) + m2 with every step rounded, then np.round      (Scale.__call__, :487-532)
+ *             stored as an integer (astype(int)): a corner that rounds to -0 is +0.  Both clips are np.clip: a NaN passes
+ *             through and a coordinate equal to a bound keeps its sign (-0.0 stays -0.0)
  *   ROTATE    a0=angle (90, 180 or 270; other values leave the boxes alone) a1=image height a2=image width: Rotate's adjusted
  *             matrix, the same corner arithmetic, then its ymin/ymax and xmin/xmax swaps             (Rotate.__call__, :681-737)
  *   OVERLAP   BoxFilter's overlap test against an a2 x a3 (height x width) image, bounds (a0, a1] / [a0, a1]: flags bits 0-1

@@ -28,13 +28,15 @@ BORDERS = ('half', 'include', 'exclude')
 
 
 def _corners(M, lab):
-    """Both corners of every box through M, as ``np.dot`` computes them, then ``np.round``."""
+    """Both corners of every box through M, as ``np.dot`` computes them, then ``np.round(...).astype(int)`` stored back into
+    the float64 labels: a corner that rounds to -0 becomes +0 (``+ 0.0``).  A NaN or infinite corner has no integer, so its
+    ``astype(int)`` is platform-defined; those keep the rounded float here."""
     x0, y0, x1, y1 = lab[:, 1], lab[:, 2], lab[:, 3], lab[:, 4]
     nx0 = (M[0, 0] * x0 + M[0, 1] * y0) + M[0, 2]
     ny0 = (M[1, 0] * x0 + M[1, 1] * y0) + M[1, 2]
     nx1 = (M[0, 0] * x1 + M[0, 1] * y1) + M[0, 2]
     ny1 = (M[1, 0] * x1 + M[1, 1] * y1) + M[1, 2]
-    return np.round(nx0), np.round(ny0), np.round(nx1), np.round(ny1)
+    return np.round(nx0) + 0.0, np.round(ny0) + 0.0, np.round(nx1) + 0.0, np.round(ny1) + 0.0
 
 
 def overlap_mask(lab, h, w, criterion, lower, upper, border_pixels='half'):
@@ -92,7 +94,7 @@ def apply_box_ops(labels, ops):
         elif op == _io.OP_SCALE:
             M = _io.rotation_matrix_2d((a2 / 2, a1 / 2), 0, a0)
             lab[:, 1], lab[:, 2], lab[:, 3], lab[:, 4] = _corners(M, lab)
-        elif op == _io.OP_ROTATE:
+        elif op == _io.OP_ROTATE and a0 in (90.0, 180.0, 270.0):    # other angles leave the boxes alone, as in ssdk.h
             angle = int(a0)
             M, _, _ = _io.rotate_geometry(int(a1), int(a2), angle)
             lab[:, 1], lab[:, 2], lab[:, 3], lab[:, 4] = _corners(M, lab)

@@ -62,11 +62,19 @@ __host__ __device__ inline void rotate_geometry(double h, double w, double c, do
   M[2] += (double)(w_new - (long long)w) / 2;
 }
 
-// Both corners through M as np.dot computes them ((m0*x + m1*y) + m2, each step rounded), then np.round.
+// Both corners through M as np.dot computes them ((m0*x + m1*y) + m2, each step rounded), then np.round(...).astype(int) stored
+// back into the float64 labels: a corner that rounds to -0 is stored as +0 (+ 0.0 does that and leaves every other value alone).
 __device__ __forceinline__ void corners(const double M[6], double& x0, double& y0, double& x1, double& y1) {
-  const double nx0 = rint((M[0] * x0 + M[1] * y0) + M[2]), ny0 = rint((M[3] * x0 + M[4] * y0) + M[5]);
-  const double nx1 = rint((M[0] * x1 + M[1] * y1) + M[2]), ny1 = rint((M[3] * x1 + M[4] * y1) + M[5]);
+  const double nx0 = rint((M[0] * x0 + M[1] * y0) + M[2]) + 0.0, ny0 = rint((M[3] * x0 + M[4] * y0) + M[5]) + 0.0;
+  const double nx1 = rint((M[0] * x1 + M[1] * y1) + M[2]) + 0.0, ny1 = rint((M[3] * x1 + M[4] * y1) + M[5]) + 0.0;
   x0 = nx0; y0 = ny0; x1 = nx1; y1 = ny1;
+}
+
+// np.clip(x, lo, hi) on float64 as NumPy computes it: a NaN passes through (fmin / fmax would return the bound), and x is kept
+// when it equals a bound, so np.clip(-0.0, 0, h) is -0.0.
+__device__ __forceinline__ double np_clip(double x, double lo, double hi) {
+  x = x < lo ? lo : x;
+  return x > hi ? hi : x;
 }
 
 __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __restrict__ gt, int gt_f64, const int* __restrict__ offs, const ssdk_box_op* __restrict__ ops,
@@ -96,8 +104,8 @@ __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __rest
             valid = valid && (cy >= 0.0) && (cy <= op.a2 - 1) && (cx >= 0.0) && (cx <= op.a3 - 1);
           }
           if (op.flags & 2) {
-            y0 = fmin(fmax(y0, 0.0), op.a2 - 1); y1 = fmin(fmax(y1, 0.0), op.a2 - 1);
-            x0 = fmin(fmax(x0, 0.0), op.a3 - 1); x1 = fmin(fmax(x1, 0.0), op.a3 - 1);
+            y0 = np_clip(y0, 0.0, op.a2 - 1); y1 = np_clip(y1, 0.0, op.a2 - 1);
+            x0 = np_clip(x0, 0.0, op.a3 - 1); x1 = np_clip(x1, 0.0, op.a3 - 1);
           }
         } else if (op.op == SSDK_BOXOP_FLIP_H) {             // labels[:, [xmin, xmax]] = img_width - labels[:, [xmax, xmin]]
           const double nx0 = op.a0 - x1, nx1 = op.a0 - x0; x0 = nx0; x1 = nx1;
@@ -133,8 +141,8 @@ __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __rest
             valid = valid && (cy >= 0.0) && (cy <= H - 1) && (cx >= 0.0) && (cx <= W - 1);
           } else if (crit == 1) {
             const double area = (x1 - x0 + d) * (y1 - y0 + d);
-            const double inter = (fmin(fmax(x1, 0.0), W - 1) - fmin(fmax(x0, 0.0), W - 1) + d) *
-                                 (fmin(fmax(y1, 0.0), H - 1) - fmin(fmax(y0, 0.0), H - 1) + d);
+            const double inter = (np_clip(x1, 0.0, W - 1) - np_clip(x0, 0.0, W - 1) + d) *
+                                 (np_clip(y1, 0.0, H - 1) - np_clip(y0, 0.0, H - 1) + d);
             const bool lo = lower == 0.0 ? inter > lower * area : inter >= lower * area;
             valid = valid && lo && (inter <= upper * area);
           } else {                                           // iou(image, box): the intersection ignores border_pixels
@@ -145,8 +153,8 @@ __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __rest
             valid = valid && (v > lower) && (v <= upper);
           }
         } else if (op.op == SSDK_BOXOP_CLIP) {               // np.clip to [0, h-1] / [0, w-1]
-          y0 = fmin(fmax(y0, 0.0), op.a0 - 1); y1 = fmin(fmax(y1, 0.0), op.a0 - 1);
-          x0 = fmin(fmax(x0, 0.0), op.a1 - 1); x1 = fmin(fmax(x1, 0.0), op.a1 - 1);
+          y0 = np_clip(y0, 0.0, op.a0 - 1); y1 = np_clip(y1, 0.0, op.a0 - 1);
+          x0 = np_clip(x0, 0.0, op.a1 - 1); x1 = np_clip(x1, 0.0, op.a1 - 1);
         }
       }
     }

@@ -7,6 +7,8 @@ import os
 import numpy as np
 import pytest
 
+import assembly_cases as ac
+
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 G = np.load(os.path.join(HERE, 'golden', 'ref_batch_golden.npz'))
@@ -43,14 +45,12 @@ def test_box_ops_match_reference_chain():
     assert offs[0] == 0 and total == sum(l.shape[0] for l in labels) and max_g == max(l.shape[0] for l in labels)
     for b in range(B):
         ref = G['out%d' % b]
-        got = gt[offs[b]:offs[b + 1]]
-        assert got.shape == ref.shape, (b, got.shape, ref.shape)
-        np.testing.assert_array_equal(got.astype(np.float64), ref.astype(np.float32).astype(np.float64))   # same boxes, same order
+        ac.assert_f32_bits(gt[offs[b]:offs[b + 1]], ref, 'image %d' % b)                  # same boxes, same order, same bits
     assert stats[0] == offs[-1] == sum(G['out%d' % b].shape[0] for b in range(B))
     assert stats[1] == max(G['out%d' % b].shape[0] for b in range(B))
     # pack only (no operations): the identity
     gt2, offs2, _, _, _ = assemble_batch_device(labels)
-    np.testing.assert_array_equal(gt2.cpu().numpy()[:total], np.concatenate(labels).astype(np.float32))
+    ac.assert_f32_bits(gt2.cpu().numpy()[:total], np.concatenate(labels), 'pack only')
     np.testing.assert_array_equal(offs2.cpu().numpy(), np.cumsum([0] + [l.shape[0] for l in labels]))
 
 

@@ -8,6 +8,7 @@ import os
 import numpy as np
 import pytest
 
+import assembly_cases as ac
 from oracle import boxops as bo
 from oracle import warpops as io
 
@@ -40,9 +41,7 @@ def _check_boxes(labels, ops, golden=None):
         ref = bo.apply_box_ops(labels[b], ops[b])
         if golden is not None:
             np.testing.assert_array_equal(ref, golden[b])
-        got = gt[offs[b]:offs[b + 1]]
-        assert got.shape == ref.shape, (b, got.shape, ref.shape, ops[b])
-        np.testing.assert_array_equal(got, ref.astype(np.float32), err_msg='image %d: %r' % (b, ops[b]))
+        ac.assert_f32_bits(gt[offs[b]:offs[b + 1]], ref, 'image %d: %r' % (b, ops[b]))
     assert stats[0] == offs[-1]
 
 
