@@ -1,9 +1,13 @@
 // Shared host/device helpers for libssdk.so (H100 / sm_90a).
 #pragma once
 #include <cuda_runtime.h>
+#include <cctype>
+#include <cerrno>
+#include <climits>
 #include <cstdint>
 #include <cstdio>
 #include <cstdarg>
+#include <cstdlib>
 #include <cstring>
 #include <algorithm>
 #include <atomic>
@@ -124,6 +128,41 @@ inline int allow_smem(const ssdk_ctx* ctx, const void* kernel, size_t bytes) {
   if (bytes <= have) return SSDK_OK;
   SSDK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
   have = bytes;
+  return SSDK_OK;
+}
+
+// Environment switches.  These are the only environment variables the library reads, and env_int is the only place that reads
+// them.  They let the tests reach on small inputs the paths the defaults take only on large ones (each selects between paths
+// that the tests hold to the same reference), or report what the encoder's matching stage did; none is needed in normal use.
+//
+//   switch                 default             read at                 selects
+//   SSDK_ENC_SPATIAL_MIN   24                  each ssdk_encode*       the spatial tile set once the batch's largest image has
+//                                                                      this many boxes
+//   SSDK_ENC_LB_MIN        17                  each ssdk_encode*       enc_lb_kernel's lower bounds from the same count on
+//   SSDK_ENC_TPC           1 ... 8 by boxes    each ssdk_encode*       tiles per CTA (at least 1; halved while the grid has
+//                                                                      fewer than 8 CTAs per SM)
+//   SSDK_ENC_COUNTERS      0                   each ssdk_encode*       1: print the conflict loop's event counts to stderr
+//                                                                      (synchronises the stream)
+//   SSDK_NMS_TWO_STAGE     1                   each ssdk_decode / nms  0: always the full multi-band NMS scan
+//   SSDK_SHARED_BORDER     1                   model plan creation     0: inference activations keep one border per image
+//   SSDK_NO_HEAD_FUSION    0                   model plan creation     1: inference heads write fp32 logits, head_finalize_kernel
+//                                                                      finishes them
+//   SSDK_OVERLAP           1                   model plan creation     0: inference plans run on one stream
+//   SSDK_OVERLAP_R         sm_count / 3 + 1    model plan creation     the grid up to which a launch counts as narrow
+//   SSDK_WGRAD_TRANSPOSED  0                   trainer creation        1: weight gradients on transposed copies, never in place
+//
+// *out = the switch's value: `def` when it is unset or empty, the value of a whole decimal integer, and anything else is refused
+// as SSDK_ERR_INVALID under the variable's name.
+inline int env_int(const char* name, int def, int* out) {
+  const char* s = getenv(name);
+  *out = def;
+  if (!s || !*s) return SSDK_OK;
+  char* end = nullptr;
+  errno = 0;
+  const long v = strtol(s, &end, 10);
+  SSDK_REQUIRE((isdigit((unsigned char)s[0]) || s[0] == '-' || s[0] == '+') && *end == '\0' && errno == 0 && v >= INT_MIN &&
+               v <= INT_MAX, "%s=\"%s\" is not an integer", name, s);
+  *out = (int)v;
   return SSDK_OK;
 }
 

@@ -696,7 +696,9 @@ int run_nms_topk(ssdk_ctx* ctx, int B, int n, int S, int layer, int box_f64, int
   int* any_redo = reinterpret_cast<int*>(scratch + o); o += align_up((size_t)B * 4, 256);
   const int band1 = stage1_band(S, top_k);
   bool two_stage = top_k > 0 && n > band1 && band1 < kNmsCap;
-  if (const char* e = getenv("SSDK_NMS_TWO_STAGE")) two_stage = two_stage && atoi(e) != 0;
+  int allow_two_stage;
+  if (int rc = env_int("SSDK_NMS_TWO_STAGE", 1, &allow_two_stage)) return rc;
+  two_stage = two_stage && allow_two_stage;
   NmsParams np{};
   np.scores = scores; np.labels = labels; np.boxes = boxes; np.kept_idx = kept_idx; np.kept_cnt = kept_cnt;
   np.n = n; np.S = S; np.kmax = kmax; np.cap = cap; np.strict = strict;

@@ -42,6 +42,8 @@ constexpr int kTile = 256;      // anchor slots per tile == threads per CTA
 constexpr int kMaxRuns = 16;    // contiguous prior runs per tile
 constexpr int kRunRec = 1 + 2 * kMaxRuns;
 constexpr int kInlineB = 1024;  // batch sizes up to this pass the ground-truth offsets as a kernel argument (no H2D copy)
+// the matching stage's event counters (SSDK_ENC_COUNTERS): conflict-loop iterations, victims, below-bound searches, images
+enum { EV_ITERATIONS, EV_VICTIMS, EV_BELOW_BOUND, EV_IMAGES, kEvents };
 
 struct EncParams {
   const double* anchors;        // [P*4] template coords (format = coords)
@@ -57,8 +59,7 @@ struct EncScratch {             // per call, global memory; TG = total number of
   const float* lb;              // [TG] lower bound of each box's row maximum, or NULL (= 0)
   int* counters;                // [B] tickets
   int TG;
-  int dbg;                      // experiment knobs (SSDK_ENC_DEBUG), 0 in production
-  unsigned long long* prof;     // SSDK_ENC_DEBUG=2: [16] nanoseconds / event counts of the matching stage, summed over images
+  unsigned long long* events;   // SSDK_ENC_COUNTERS=1: [kEvents] counts of the matching stage, summed over images, else NULL
 };
 
 struct TileSetDev {
@@ -400,16 +401,7 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
   int* matches = removed + G;                                 // [G]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int W = p.C + 12, TG = sc.TG;
-  unsigned long long t_prev = 0;
-  auto lap = [&](int slot) {                                  // SSDK_ENC_DEBUG=2: time since the previous lap -> prof[slot]
-    if (sc.prof && tid == 0) {
-      const unsigned long long t = globaltimer();
-      if (slot >= 0) atomicAdd(sc.prof + slot, t - t_prev);
-      t_prev = t;
-    }
-  };
-  auto count = [&](int slot, int n) { if (sc.prof && tid == 0 && n) atomicAdd(sc.prof + slot, (unsigned long long)n); };
-  lap(-1);
+  auto count = [&](int slot, int n) { if (sc.events && tid == 0 && n) atomicAdd(sc.events + slot, (unsigned long long)n); };
   auto gbox = [&](int g) {
     Box q; q.x0 = s_gbox[g * 5]; q.y0 = s_gbox[g * 5 + 1]; q.x1 = s_gbox[g * 5 + 2]; q.y1 = s_gbox[g * 5 + 3]; q.area = s_gbox[g * 5 + 4];
     return q;
@@ -442,7 +434,6 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
       __syncthreads();
     }
   }
-  lap(0);
   if (tid == 0) { s_flag[0] = 0; s_flag[1] = 0; }
   __syncthreads();
   for (int g = tid; g < G; g += kTile) {
@@ -471,9 +462,8 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
     for (int g = tid; g < G; g += kTile) matches[g] = 0;
     if (tid == 0) s_nrem = 0;
     __syncthreads();
-    lap(1);
     for (;;) {
-      count(8, 1);
+      count(EV_ITERATIONS, 1);
       // A. the first row with a later duplicate
       double cv = -1.0; int ci = INT_MAX;
       for (int g = tid; g < G; g += kTile) {
@@ -513,7 +503,6 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
         }
       }
       __syncthreads();
-      lap(2);
       if (f < 0) break;
       // C. the rows that pointed at f's prior recompute their maximum (one warp per row)
       const int n_removed = s_nrem;
@@ -523,7 +512,7 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
         if (rv[g] > 0.0 && ra[g] == a_star) victims[atomicAdd(&s_nvict, 1)] = g;
       __syncthreads();
       const int n_vict = s_nvict;
-      count(9, n_vict);
+      count(EV_VICTIMS, n_vict);
       // C1. per row, all eight warps together: re-evaluate the tile of the lost prior without the taken priors (one 32-anchor
       // slice per warp) while every thread looks at one or two of the other tiles' recorded bests; repeat while the new best is
       // itself a taken prior recorded by another tile
@@ -582,7 +571,6 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
         }
       }
       __syncthreads();
-      lap(3);
       // C2. pairs below a row's lower bound were never evaluated by the tile pass: a row whose best that is left fell below it is
       // searched over all slices, by all warps together
       for (int vi = 0; vi < n_vict; ++vi) {
@@ -590,7 +578,7 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
         const float lbg = sc.lb ? __ldg(sc.lb + g0 + gg) : 0.f;
         double nv = pv[vi]; int ni = pi[vi];
         if (!(nv < (double)lbg)) continue;                       // uniform over the CTA
-        count(10, 1);
+        count(EV_BELOW_BOUND, 1);
         warp_row_best(p, ts, gbox(gg), removed, n_removed, nv, ni, warp, kTile / 32);
         if (lane == 0) { s_cv[warp] = nv; s_ci[warp] = ni; }
         __syncthreads();
@@ -608,7 +596,6 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
         rv[gg] = nv; ra[gg] = (nv > 0.0) ? pi[vi] : 0;
       }
       __syncthreads();
-      lap(4);
     }
     if (tid == 0 && s_nrem < G) matches[0] = 0;                  // rounds with nothing left to match select (box 0, prior 0)
   }
@@ -626,8 +613,7 @@ __device__ void finish_image(const EncParams& p, const TileSetDev& ts, const Enc
     if (out_match) out_match[(size_t)b * p.P + a] = g;
   }
   __syncthreads();
-  lap(5);
-  count(11, 1);
+  count(EV_IMAGES, 1);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -883,10 +869,6 @@ __global__ void __launch_bounds__(kTile, 3) enc_tiles_kernel(const __grid_consta
     store_pending = issued;
   }
   // ---- 6. last CTA of the image: bipartite matching ----
-  if (sc.dbg & 1) {                                             // timing experiments only: no matching stage (wrong results)
-    if (tid == 0) bulk_wait_read<0>();
-    return;
-  }
   if (tid == 0) bulk_wait<0>();
   if (G <= 0) return;
   __syncthreads();                                              // every thread's global writes happen-before thread 0's fence
@@ -1027,6 +1009,7 @@ struct ssdk_encoder {
   Scratch tiles;                    // per-(gt, tile) bounds and exact bests, per-gt lower bounds
   Scratch counters;                 // per-image tickets (self-resetting)
   size_t counters_n = 0;
+  Scratch events;                   // the matching stage's event counts, allocated by the first call with SSDK_ENC_COUNTERS=1
   Scratch offsets;                  // device copy of the offsets for batches larger than kInlineB
   HostRing<8> offsets_ring;         // pinned staging of those offsets
   OffsArg offs_arg{};               // ground-truth offsets passed by value with the launch (B <= kInlineB)
@@ -1158,7 +1141,7 @@ extern "C" int ssdk_encoder_destroy(ssdk_encoder* e) {
   if (!e) return SSDK_OK;
   cudaFree(e->d_anchors);
   e->linear.release(); e->spatial.release();
-  e->tiles.release(); e->counters.release(); e->offsets.release();
+  e->tiles.release(); e->counters.release(); e->events.release(); e->offsets.release();
   e->offsets_ring.release();
   delete e;
   return SSDK_OK;
@@ -1191,13 +1174,16 @@ int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* of
   // tile set: compact cell blocks pay off once many boxes compete per tile; consecutive priors give full tiles, one aligned
   // run each and nothing to look up, which is what matters when the kernel is purely store / latency bound
   int spatial_min = 24, lb_min = 17;
-  if (const char* s = getenv("SSDK_ENC_SPATIAL_MIN")) spatial_min = atoi(s);
-  if (const char* s = getenv("SSDK_ENC_LB_MIN")) lb_min = atoi(s);
+  if (int rc = env_int("SSDK_ENC_SPATIAL_MIN", spatial_min, &spatial_min)) return rc;
+  if (int rc = env_int("SSDK_ENC_LB_MIN", lb_min, &lb_min)) return rc;
   const bool use_spatial = e->spatial.dev.n_tiles > 0 && max_g >= spatial_min;
   const TileSetDev& ts = use_spatial ? e->spatial.dev : e->linear.dev;
   const bool use_lb = max_g >= lb_min && total_g > 0;
   int tpc = max_g <= 16 ? 1 : (max_g <= 48 ? 2 : (max_g < 96 ? 4 : 8));   // tiles per CTA: amortises the per-CTA box set-up (measured)
-  if (const char* s = getenv("SSDK_ENC_TPC")) tpc = std::max(1, atoi(s));
+  if (int rc = env_int("SSDK_ENC_TPC", tpc, &tpc)) return rc;
+  tpc = std::max(1, tpc);
+  int counters;
+  if (int rc = env_int("SSDK_ENC_COUNTERS", 0, &counters)) return rc;
   while (tpc > 1 && (long long)ceil_div(ts.n_tiles, tpc) * B < 8ll * e->ctx->sm_count) tpc >>= 1;
   // scratch: tV (f64) | tI (i32) each [n_tiles * TG], lb [TG]
   const size_t TG = (size_t)(total_g > 0 ? total_g : 1);
@@ -1210,12 +1196,11 @@ int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* of
   float* lb = reinterpret_cast<float*>(sc.tI + nt);
   sc.lb = use_lb ? lb : nullptr;
   sc.TG = (int)TG;
-  if (const char* s = getenv("SSDK_ENC_DEBUG")) sc.dbg = atoi(s);
-  static unsigned long long* d_prof = nullptr;
-  if (sc.dbg & 2) {
-    if (!d_prof) SSDK_CHECK_CUDA(cudaMalloc(&d_prof, 16 * sizeof(unsigned long long)));
-    SSDK_CHECK_CUDA(cudaMemsetAsync(d_prof, 0, 16 * sizeof(unsigned long long), stream));
-    sc.prof = d_prof;
+  if (counters) {
+    rc = e->events.ensure(kEvents * sizeof(unsigned long long));
+    if (rc) return rc;
+    sc.events = reinterpret_cast<unsigned long long*>(e->events.ptr);
+    SSDK_CHECK_CUDA(cudaMemsetAsync(sc.events, 0, kEvents * sizeof(unsigned long long), stream));
   }
   if (e->counters_n < (size_t)B) {
     SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));
@@ -1251,14 +1236,13 @@ int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* of
   rc = launch(e->ctx, inline_offs ? enc_tiles_kernel<true> : enc_tiles_kernel<false>, grid, kTile, L.total, stream,
               p, ts, e->offs_arg, d_offs, gt_dev, gt_f64, tpc, sc, out_y_dev, out_match_dev, status_dev);
   if (rc) return rc;
-  if (sc.prof) {                                                // experiments only: synchronises
-    unsigned long long h[16];
+  if (sc.events) {                                              // synchronises
+    unsigned long long h[kEvents];
+    SSDK_CHECK_CUDA(cudaMemcpyAsync(h, sc.events, sizeof(h), cudaMemcpyDeviceToHost, stream));
     SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));
-    SSDK_CHECK_CUDA(cudaMemcpy(h, sc.prof, sizeof(h), cudaMemcpyDeviceToHost));
-    const double n = h[11] ? (double)h[11] : 1.0;
-    fprintf(stderr, "enc matching stage, per image (us): row maxima %.1f | duplicates? %.1f | A+B %.1f | C1 %.1f | C2+write %.1f | tail %.1f"
-                    " || iterations %.1f victims %.1f below-bound searches %.1f (images %llu)\n",
-            h[0] / n / 1e3, h[1] / n / 1e3, h[2] / n / 1e3, h[3] / n / 1e3, h[4] / n / 1e3, h[5] / n / 1e3, h[8] / n, h[9] / n, h[10] / n, h[11]);
+    const double n = h[EV_IMAGES] ? (double)h[EV_IMAGES] : 1.0;
+    fprintf(stderr, "enc matching stage, per image: iterations %.1f victims %.1f below-bound searches %.1f (images %llu)\n",
+            h[EV_ITERATIONS] / n, h[EV_VICTIMS] / n, h[EV_BELOW_BOUND] / n, h[EV_IMAGES]);
   }
   return SSDK_OK;
 }

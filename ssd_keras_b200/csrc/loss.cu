@@ -62,7 +62,6 @@ struct LossArgs {
   int* ties_local;                     // multi-GPU: out, boxes equal to T on this rank
   // outputs
   float* out_loss; int* out_stats; const float* upstream; float* out_grad;
-  unsigned long long* dbg_times;       // optional [8]: globaltimer of CTA 0 at the phase boundaries (SSDK_LOSS_TIMES)
   int stages;                          // shared-memory stages of phase A / D tile loads (1 or 2)
   int bulk_ok;                         // rows of a tile start 16-byte aligned: cp.async.bulk is usable
 };
@@ -483,25 +482,16 @@ __global__ void __launch_bounds__(kRows) ssd_loss_kernel(const __grid_constant__
   __shared__ uint64_t s_bars[3];
   __shared__ long long s_scan[kRows];
   cg::grid_group grid = cg::this_grid();
-  auto stamp = [&](int i) {
-    if (a.dbg_times && blockIdx.x == 0 && threadIdx.x == 0) a.dbg_times[i] = globaltimer();
-  };
   const uint32_t bar0 = setup_barriers(s_bars);
-  stamp(0);
   phase_a(a, smem, bar0);
-  stamp(1);
   grid.sync();
-  stamp(2);
   Sel s;
   read_counts(a, s);
   int b1 = 0; long long want1 = 0;
   if (!s.none) level1(a, s, b1, want1, s_scan);
-  stamp(3);
   phase_b(a, s, b1);
   grid.sync();
-  stamp(4);
   finish_select(a, s, b1, want1, s_scan);
-  stamp(5);
   const bool ordered = !s.none && s.want < s.ties_total;                 // uniform over the grid
   if (ordered) {
     phase_ties(a, s);
@@ -512,7 +502,6 @@ __global__ void __launch_bounds__(kRows) ssd_loss_kernel(const __grid_constant__
     s.want = s.ties_total;                                               // every box equal to T is kept: no order needed
   }
   phase_d(a, s, ordered, 0, smem, bar0 + 16);
-  stamp(6);
 }
 
 // The same phases as separate launches (multi-GPU, global-batch-exact): 0 = A, 1 = B, 2 = threshold + local ties, 3 = scan, 4 = D
@@ -670,21 +659,8 @@ int loss_run(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int
   rc = fill_args(ctx, a, y_true, y_pred, B, P, C, ratio, n_neg_min, alpha, ws, parity, out_grad != nullptr, plan, true);
   if (rc) return rc;
   a.out_loss = out_loss; a.out_stats = out_stats; a.upstream = upstream; a.out_grad = out_grad;
-  static unsigned long long* d_times = nullptr;
-  if (getenv("SSDK_LOSS_TIMES")) {                                     // experiment: phase boundaries of CTA 0
-    if (!d_times) SSDK_CHECK_CUDA(cudaMalloc(&d_times, 64));
-    a.dbg_times = d_times;
-  }
   rc = launch_fused(ctx, a, plan, stream);
   if (rc == SSDK_OK) ctx->loss_parity ^= 1;                           // this launch clears the other set for the next call
-  if (rc == SSDK_OK && a.dbg_times) {
-    unsigned long long h[8] = {0};
-    SSDK_CHECK_CUDA(cudaStreamSynchronize(stream));
-    SSDK_CHECK_CUDA(cudaMemcpy(h, d_times, 56, cudaMemcpyDeviceToHost));
-    fprintf(stderr, "ssd_loss phases (CTA 0, us): A %.1f | sync %.1f | level1 %.1f | B+sync %.1f | select2 %.1f | D %.1f | total %.1f (grid %d, smem %zu)\n",
-            (h[1] - h[0]) / 1e3, (h[2] - h[1]) / 1e3, (h[3] - h[2]) / 1e3, (h[4] - h[3]) / 1e3, (h[5] - h[4]) / 1e3, (h[6] - h[5]) / 1e3,
-            (h[6] - h[0]) / 1e3, plan.grid, plan.smem);
-  }
   return rc;
 }
 

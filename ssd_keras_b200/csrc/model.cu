@@ -58,8 +58,6 @@ int build_conv(ssdk_model* m, int li) {
     L.bn_eps = d.bn_eps > 0.f ? d.bn_eps : 1e-3f;
     L.bn_momentum = (d.bn_momentum > 0.f && d.bn_momentum < 1.f) ? d.bn_momentum : 0.99f;
   }
-  // experiment knob (inference plans only): route the image-facing layer through im2col (K = 27 -> 32) + the implicit GEMM instead
-  if (L.direct && !m->training && getenv("SSDK_NO_DIRECT")) L.direct = false;
   if (L.direct) {
     int rc = upload_f32(m, &L.w_f32, master.data(), master.size()); if (rc) return rc;
     rc = upload_f32(m, &L.bias, bias.data(), bias.size()); if (rc) return rc;
@@ -71,8 +69,7 @@ int build_conv(ssdk_model* m, int li) {
     m->flops_algo += fl;                 // counted as algorithmic FLOPs only (the timed conv launches exclude this layer)
     // inference plans: the layer runs on the tensor cores with a gathered A tile (conv_first_kernel); training plans keep the fp32
     // direct kernel, whose weights are the optimizer's master copy
-    if (!m->training && first_tc_supported(taps, cin, cout) && d.dilation >= 1 && first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l) &&
-        !getenv("SSDK_NO_FIRST_TC")) {
+    if (!m->training && first_tc_supported(taps, cin, cout) && d.dilation >= 1 && first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l)) {
       std::vector<uint16_t> whi, wlo;
       L.first = first_plan(L.out, d.kh, d.kw, m->ctx->sm_count);
       first_weight_image(master.data(), taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
@@ -136,8 +133,9 @@ int build_conv(ssdk_model* m, int li) {
   if (head) {
     // inference plans: softmax / concat / anchors in the epilogue, straight into y_pred (one n-tile holds all boxes of a pixel);
     // training plans keep the raw logits (the backward pass needs them) and finish with head_finalize_kernel
-    const bool fuse = !m->training && a.n_tiles_n == 1 && !getenv("SSDK_NO_HEAD_FUSION");
-    if (fuse) {
+    int no_fusion;
+    rc = env_int("SSDK_NO_HEAD_FUSION", 0, &no_fusion); if (rc) return rc;
+    if (!m->training && a.n_tiles_n == 1 && !no_fusion) {
       a.epi = EPI_HEAD;
       a.head_nb = d.n_boxes; a.head_C = m->Ctot; a.head_prior_off = 0;          // prior offset, P, anchors: set once they are known
       L.head_fused = true;
@@ -201,9 +199,10 @@ int plan_overlap(ssdk_model* m) {
   m->on_side.assign(n, 0);
   m->overlap_from = -1; m->grid_cap = 0;
   if (m->training) return SSDK_OK;
-  if (const char* e = getenv("SSDK_OVERLAP")) { if (!atoi(e)) return SSDK_OK; }
-  int R = m->ctx->sm_count / 3 + 1;
-  if (const char* e = getenv("SSDK_OVERLAP_R")) R = atoi(e);
+  int overlap, R;
+  if (int rc = env_int("SSDK_OVERLAP", 1, &overlap)) return rc;
+  if (int rc = env_int("SSDK_OVERLAP_R", m->ctx->sm_count / 3 + 1, &R)) return rc;
+  if (!overlap) return SSDK_OK;
   std::vector<int> kind(n, 0), grid(n, 0), input(n, -1);
   for (int i = 0; i < n; ++i) {
     const LayerPlan& L = m->layers[i];

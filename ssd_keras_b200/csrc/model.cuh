@@ -4,7 +4,6 @@
 #include <vector>
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 namespace ssdk {
 
@@ -90,8 +89,9 @@ inline int upload_f32(ssdk_model* m, float** out, const float* host, size_t n) {
 
 inline int alloc_act(ssdk_model* m, ActBuf& a, int B, int H, int W, int C, int pad) {
   a.B = B; a.H = H; a.W = W; a.C = C; a.Cs = (C + 7) / 8 * 8; a.pad = pad;
-  a.shared = 0;
-  if (!m->training && pad > 0) { const char* e = getenv("SSDK_SHARED_BORDER"); a.shared = e ? (atoi(e) ? 1 : 0) : 1; }
+  int shared;
+  if (int rc = env_int("SSDK_SHARED_BORDER", 1, &shared)) return rc;
+  a.shared = !m->training && pad > 0 && shared ? 1 : 0;
   // slack: TMA boxes may start on the last rows; with a shared border the last row's right border lies behind the last image
   size_t n = a.elems() + std::max<size_t>(64 * 8, (size_t)(pad + 1) * a.Cs);
   int rc = dev_alloc(m->allocs, &a.hi, n, true);

@@ -115,11 +115,6 @@ __device__ __forceinline__ float rcp_approx(float x) {          // MUFU.RCP: at 
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
 }
-__device__ __forceinline__ unsigned long long globaltimer() {   // nanoseconds; for timing experiments
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
 
 // ------------------------------------------------------------------------------------------------
 // wgmma (sm_90a).  Shared-memory matrix descriptor, 128-byte swizzle: start address >> 4 at [0,14), leading byte offset >> 4 at

@@ -585,7 +585,9 @@ int plan_wgrad_layer(ssdk_trainer* t, int i, long long& max_xT, long long& max_d
   const ssdk_layer_desc& d = L.d;
   if (L.direct) return SSDK_OK;               // handled by wgrad_direct_kernel
   const ActBuf& X = m->layers[d.input].out;
-  if (!L.im2col && !getenv("SSDK_WGRAD_TRANSPOSED") && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
+  int transposed;
+  if (int rc = env_int("SSDK_WGRAD_TRANSPOSED", 0, &transposed)) return rc;
+  if (!L.im2col && !transposed && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
     T.wg_native = true;
     return plan_wgrad(m->ctx, T.wg, X, T.g, L.H, L.W, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, m->split, span_grad(t, i, 0));
   }

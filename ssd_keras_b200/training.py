@@ -153,8 +153,7 @@ class SSDTrainer:
         soon as its layers have been differentiated (NCCL on its own stream under the weight / data gradient kernels of the lower
         layers), or in one call after the backward pass.  ``overlap=None`` picks: at 2 ranks the whole exchange is short while
         NCCL's kernels share the SMs with the persistent (one CTA per SM) conv launches when they run side by side, so the
-        bucketed exchange is used from 4 ranks on (SSDK_GRAD_OVERLAP=0/1 overrides; SSDK_OVERLAP is the two-stream schedule of inference plans)."""
-        import os
+        bucketed exchange is used from 4 ranks on."""
         import torch.distributed as dist
         on = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
         loss, _, dy = self._loss_and_dy(images, y_true)
@@ -163,8 +162,7 @@ class SSDTrainer:
             self.apply(1.0)
             return loss
         if overlap is None:
-            env = os.environ.get('SSDK_GRAD_OVERLAP')
-            overlap = (env == '1') if env in ('0', '1') else dist.get_world_size(group) > 2
+            overlap = dist.get_world_size(group) > 2
         from .distributed import all_reduce_buckets_
         if overlap:
             all_reduce_buckets_(self.grad, self.buckets(), lambda hi, lo: self._backward_layers(dy, hi, lo), group=group)

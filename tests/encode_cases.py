@@ -38,6 +38,10 @@ def kernel_constants():
     k['spatial_min'], k['lb_min'] = int(m.group(1)), int(m.group(2))
     m = re.search(r'int tpc = max_g <= (\d+) \? 1 : \(max_g <= (\d+) \? 2 : \(max_g < (\d+) \? 4 : 8\)\);', src)
     k['tpc_ladder'] = tuple(int(v) for v in m.groups())
+    # each default is what its switch (ssdk::env_int) falls back to; SSDK_ENC_TPC is clamped to >= 1 as in paths() below
+    for name, var in (('SSDK_ENC_SPATIAL_MIN', 'spatial_min'), ('SSDK_ENC_LB_MIN', 'lb_min'), ('SSDK_ENC_TPC', 'tpc')):
+        assert 'env_int("%s", %s, &%s)' % (name, var, var) in src, name
+    assert 'tpc = std::max(1, tpc);' in src, 'tiles per CTA clamped to >= 1'
     # enc_tiles_kernel gets L.total bytes of dynamic shared memory through ssdk::launch, which opts in above 48 KB
     m = re.search(r'launch\(e->ctx, inline_offs \? enc_tiles_kernel<true> : enc_tiles_kernel<false>, grid, kTile, L\.total,', src)
     assert m, 'dynamic shared memory of enc_tiles_kernel'

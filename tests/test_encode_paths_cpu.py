@@ -45,7 +45,7 @@ def test_case_table_reaches_path(reached, path):
 
 
 def test_conflict_cases_model():
-    """The numbers the kernel's SSDK_ENC_DEBUG=2 counters are held to, and the C1 claim that does not rest on a float32 bound."""
+    """The numbers the kernel's SSDK_ENC_COUNTERS=1 counters are held to, and the C1 claim that does not rest on a float32 bound."""
     ev = ec.paths(ec.BY_NAME['chain4'], ec.inputs('chain4'))[2][0]
     assert (ev['iterations'], ev['victims'], ev['c2']) == (4, [3, 2, 1], 0)
     ev = ec.paths(ec.BY_NAME['chain4_lb'], ec.inputs('chain4_lb'))[2][0]

@@ -14,7 +14,7 @@ import encode_cases as ec
 
 pytestmark = pytest.mark.gpu
 
-ENV_KEYS = ('SSDK_ENC_SPATIAL_MIN', 'SSDK_ENC_LB_MIN', 'SSDK_ENC_TPC', 'SSDK_ENC_DEBUG')
+ENV_KEYS = ('SSDK_ENC_SPATIAL_MIN', 'SSDK_ENC_LB_MIN', 'SSDK_ENC_TPC', 'SSDK_ENC_COUNTERS')
 
 
 @pytest.fixture(scope='module', autouse=True)
@@ -114,12 +114,12 @@ _COUNTERS = re.compile(r'iterations ([\d.]+) victims ([\d.]+) below-bound search
 
 
 @pytest.mark.parametrize('name', [c['name'] for c in ec.CASES if c['counters']])
-def test_conflict_loop_counters(name, env, capfd):
-    """SSDK_ENC_DEBUG=2 prints the matching stage's event counts; one image per launch, so they are integers."""
+def test_conflict_loop_counters_enc_counters(name, env, capfd):
+    """SSDK_ENC_COUNTERS=1 prints the matching stage's event counts; one image per launch, so they are integers."""
     c = ec.BY_NAME[name]
     for k, v in c['env'].items():
         env.setenv(k, v)
-    env.setenv('SSDK_ENC_DEBUG', '2')
+    env.setenv('SSDK_ENC_COUNTERS', '1')
     for b, g in enumerate(ec.inputs(name)):
         _, _, events = ec.paths(c, [g])
         ev = events[0]

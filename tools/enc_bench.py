@@ -20,7 +20,7 @@ hbm = peaks['hbm_gbs']
 
 
 def run(tag, enc, gdev, offs, ybuf, bytes_, inner, env):
-    for k in ('SSDK_ENC_SPATIAL_MIN', 'SSDK_ENC_TPC', 'SSDK_ENC_DEBUG', 'SSDK_ENC_LB_MIN'):
+    for k in ('SSDK_ENC_SPATIAL_MIN', 'SSDK_ENC_TPC', 'SSDK_ENC_LB_MIN'):
         os.environ.pop(k, None)
     os.environ.update(env)
     ms = bench._time_cuda(lambda: enc.encode_device(gdev, offs, out=ybuf), iters=7, warm=3, inner=inner)
@@ -37,7 +37,7 @@ def main():
     ybuf = torch.empty((Bm, 100000, 33), dtype=torch.float32, device='cuda')
     bytes_ = Bm * (100000 * 16 + 128 * 20 + 100000 * 4 * 33)
     for env in ({}, {'SSDK_ENC_SPATIAL_MIN': '1000000'}, {'SSDK_ENC_TPC': '1'}, {'SSDK_ENC_TPC': '2'}, {'SSDK_ENC_TPC': '8'},
-                {'SSDK_ENC_SPATIAL_MIN': '1000000', 'SSDK_ENC_TPC': '1'}, {'SSDK_ENC_DEBUG': '1'}):
+                {'SSDK_ENC_SPATIAL_MIN': '1000000', 'SSDK_ENC_TPC': '1'}):
         run('micro_b%d' % Bm, encm, gm, offm, ybuf, bytes_, 1, env)
     # memory-bound floor of the same output: a plain fill of the target tensor
     ms = bench._time_cuda(lambda: ybuf.fill_(1.0), iters=7, warm=2)
@@ -51,7 +51,7 @@ def main():
     gdev = torch.from_numpy(np.concatenate(gt)).cuda()
     y300 = torch.empty((32, 8732, 33), dtype=torch.float32, device='cuda')
     b300 = 32 * (8732 * 16 + 8 * 20 + 8732 * 4 * 33)
-    for env in ({}, {'SSDK_ENC_SPATIAL_MIN': '0'}, {'SSDK_ENC_TPC': '2'}, {'SSDK_ENC_DEBUG': '1'}):
+    for env in ({}, {'SSDK_ENC_SPATIAL_MIN': '0'}, {'SSDK_ENC_TPC': '2'}):
         run('ssd300_b32', enc, gdev, offs, y300, b300, 50, env)
     ms = bench._time_cuda(lambda: y300.fill_(1.0), iters=7, warm=2, inner=50)
     print(json.dumps({'case': 'fill_same_bytes_ssd300', 'ms': round(ms, 5), 'GBps': round(y300.numel() * 4 / ms / 1e6, 1)}), flush=True)
