@@ -37,7 +37,7 @@ returns (ref, A, {perturbation: ref'}) and is judged with the same form |g - ref
    puts all three products of a k-step on one accumulator (wgrad_wgmma_kernel: ``4 * patches per split * products`` k-steps)
    or runs the pixel axis through conv_wgmma_kernel (cross terms apart: ``4 * K blocks per split``); the ``k_split`` partial
    sums meet in fp32 atomics (``n_steps_wgrad``).  The X operand is the stored planes themselves, not a re-split of hi + lo.
-4. fp32 sums (wgrad_direct, bias_grad_kernel, rowsum_kernel, col2im, pool routing, the gamma gradient).  Adding N terms in
+4. fp32 sums (wgrad_direct, bias_grad_kernel, col2im, pool routing, the gamma gradient).  Adding N terms in
    any order loses at most (N - 1) * 2**-24 * sum |term| (every partial sum is bounded by the sum of absolute terms); a
    rounded product adds 2**-24 * |term|.  So n_steps = N + 1 in kappa = 2**-22 * (n_steps + 1) is a bound, whatever order
    the atomics take.
@@ -418,7 +418,7 @@ def wgrad_ref(x, dz, KH, KW, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', 
 
 
 def bias_grad_ref(dz, perturb=()):
-    """Bias gradient (bias_grad_kernel, rowsum_kernel): fp32 sum of hi and lo over all pixels -> (ref, A, n_steps, {...}).
+    """Bias gradient (bias_grad_kernel): fp32 sum of hi and lo over all pixels -> (ref, A, n_steps, {...}).
     perturb: ('lo',) leaves the lo plane out; ('row', n, y) leaves pixel row y of image n out."""
     g = _planes(dz)
     ref = g[0].astype(np.float64).sum(axis=(0, 1, 2)) + g[1].astype(np.float64).sum(axis=(0, 1, 2))

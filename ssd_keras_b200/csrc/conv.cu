@@ -201,12 +201,11 @@ __device__ __forceinline__ void ld_f8(const float* p, float (&v)[8]) {
 // ------------------------------------------------------------------------------------------------
 // The convolution kernel
 // ------------------------------------------------------------------------------------------------
-// MODE (ConvArgs::split / acc_split as a compile-time constant, so that every wgmma of the K loop is issued on a uniform path):
-//   kSingle  one bf16 product per k-step;
-//   kSplitXS bf16x3, the cross terms (hi*lo, lo*hi) accumulate in their own registers and are added to the hi*hi sum after the
-//            K loop: the large accumulator takes one rounding add per k-step instead of three (deep-K layers: fc6, fc7,
-//            conv6_2 ... stay within 1e-4 of an fp32 convolution).
-enum { kSingle = 0, kSplitXS = 2 };
+// SPLIT (ConvArgs::split as a compile-time constant, so that every wgmma of the K loop is issued on a uniform path):
+//   false  single-pass bf16: one hi*hi product per k-step;
+//   true   bf16x3: the cross terms (hi*lo, lo*hi) accumulate in their own registers and are added to the hi*hi sum after the
+//          K loop: the large accumulator takes one rounding add per k-step instead of three (deep-K layers: fc6, fc7,
+//          conv6_2 ... stay within 1e-4 of an fp32 convolution).
 static constexpr int kConvThreads = 384;   // warpgroup 0: TMA producer; warpgroups 1, 2: wgmma consumers of rows [0, 64) / [64, 128)
 
 __device__ __forceinline__ void consumer_sync() { named_bar_sync<1, 256>(); }   // the two consumer warpgroups
@@ -233,7 +232,22 @@ __device__ __forceinline__ void quad_gather8(const float (&acc)[N], int jp, int 
   }
 }
 
-template <int BN, int MODE>
+// Virtual row v -> image n and position (y, x) of the virtual grid; true when v is a real output pixel (y < Ho, x < Wo).  Past the
+// last row: false, with n = y = x = 0.
+__device__ __forceinline__ bool decode_vrow(const ConvArgs& args, int v, int& n, int& y, int& x) {
+  bool valid = v < args.M_total;
+  n = 0; y = 0; x = 0;
+  if (valid) {
+    n = v / args.rows_per_img;
+    const int rr = v - n * args.rows_per_img;
+    y = rr / args.in_Wp;
+    x = rr - y * args.in_Wp;
+    valid = (y < args.Ho) && (x < args.Wo);
+  }
+  return valid;
+}
+
+template <int BN, bool SPLIT>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                   const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
@@ -242,7 +256,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
   const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-  constexpr bool split = MODE == kSplitXS;
+  constexpr bool split = SPLIT;
   const int S = args.stages;
   constexpr uint32_t kBTile = (uint32_t)BN * kBK * 2;
   const uint32_t b_off = (uint32_t)kATile * (split ? 2u : 1u);            // stage: A_hi | A_lo | W_hi | W_lo
@@ -374,15 +388,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
       // ===================== EPI_SPLIT from the registers: a quad exchange gives each lane 8 consecutive columns of one row ====
       const int q = lane & 3;
       const int v = m0 + cw * 64 + cwarp * 16 + (lane >> 2) + 8 * (q >> 1);   // virtual row of this lane's stores
-      bool valid = v < args.M_total;
-      int n = 0, y = 0, x = 0;
-      if (valid) {
-        n = v / args.rows_per_img;
-        const int rr = v - n * args.rows_per_img;
-        y = rr / args.in_Wp;
-        x = rr - y * args.in_Wp;
-        valid = (y < args.Ho) && (x < args.Wo);
-      }
+      int n, y, x;
+      const bool valid = decode_vrow(args, v, n, y, x);
       const size_t o_row = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + n0;
       const bool bwd = args.mask_hi || args.accumulate;
 #pragma unroll
@@ -413,15 +420,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
     consumer_sync();
     const int r = ctid & (kBM - 1), half = ctid >> 7;
     const int v = m0 + r;                                                  // virtual row of this thread
-    bool valid = v < args.M_total;
-    int n = 0, y = 0, x = 0;
-    if (valid) {
-      n = v / args.rows_per_img;
-      const int rr = v - n * args.rows_per_img;
-      y = rr / args.in_Wp;
-      x = rr - y * args.in_Wp;
-      valid = (y < args.Ho) && (x < args.Wo);
-    }
+    int n, y, x;
+    const bool valid = decode_vrow(args, v, n, y, x);
     const float* arow = s_acc + (size_t)r * (BN + kAccPad);
     const int h0 = half * (BN / 2), nh = min(BN / 2, ncols - h0);       // this thread's columns: [h0, h0 + nh)
     if (valid && args.epi == EPI_HEAD) {
@@ -468,16 +468,15 @@ int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int gri
   // the kernel is persistent with a static stride over its work units: any grid size computes the same result
   const int grid = grid_cap > 0 ? std::max(1, std::min(L.grid, grid_cap)) : L.grid;
   const bool split = L.args.split != 0;
-  SSDK_REQUIRE(!split || L.args.acc_split, "internal: bf16x3 conv plans carry the cross-term accumulator");
   SSDK_REQUIRE(split || L.args.BN != 160, "internal: 160-wide conv tiles are for bf16x3 predictor heads");
-  decltype(&conv_wgmma_kernel<64, kSingle>) kernel;
+  decltype(&conv_wgmma_kernel<64, false>) kernel;
   switch (L.args.BN) {
-    case 64: kernel = split ? conv_wgmma_kernel<64, kSplitXS> : conv_wgmma_kernel<64, kSingle>; break;
-    case 128: kernel = split ? conv_wgmma_kernel<128, kSplitXS> : conv_wgmma_kernel<128, kSingle>; break;
-    case 160: kernel = conv_wgmma_kernel<160, kSplitXS>; break;
+    case 64: kernel = split ? conv_wgmma_kernel<64, true> : conv_wgmma_kernel<64, false>; break;
+    case 128: kernel = split ? conv_wgmma_kernel<128, true> : conv_wgmma_kernel<128, false>; break;
+    case 160: kernel = conv_wgmma_kernel<160, true>; break;
     case 256:
       SSDK_REQUIRE(!split, "internal: 256-wide conv tiles have no cross-term accumulator");
-      kernel = conv_wgmma_kernel<256, kSingle>;
+      kernel = conv_wgmma_kernel<256, false>;
       break;
     default: set_error("internal: conv tile width %d", L.args.BN); return SSDK_ERR_INVALID;
   }

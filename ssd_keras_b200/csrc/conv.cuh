@@ -125,7 +125,6 @@ struct ConvArgs {
   int BN;               // accumulator tile width (64/128/160/256: the wgmma N); TMA box rows of the weight tile
   int cout;
   int split;            // 1: bf16x3 (hi*hi + hi*lo + lo*hi), 0: single bf16 pass
-  int acc_split;        // 1 (always with split): the cross terms accumulate apart from hi*hi and are added after the K loop
   // epilogue
   int epi;
   const float* bias; const float* bn_scale; const float* bn_shift;

@@ -281,42 +281,9 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   a.kblocks = kblocks;
   a.Ho = g.Ho; a.Wo = g.Wo; a.B = g.B;
   a.cout = g.cout;
-  a.BN = g.cout <= 64 ? 64 : (g.cout <= 128 ? 128 : 256);
-  a.split = m->split;
-  a.k_split = 1;
-  if (a.split && a.BN == 256) {
-    // bf16x3 tiles carry the cross-term accumulator (acc_split), which fits in registers up to 160 columns: 160-wide tiles for
-    // the predictor heads of <= 160 columns (6 boxes x 25 for VOC: the fused head epilogue needs all boxes of a pixel in one
-    // tile), 128-wide tiles otherwise
-    a.BN = g.cout <= 160 ? 160 : 128;
-  } else if (a.BN == 256 && g.cout % 128 == 0) {                // (not the predictor heads: their epilogue needs all boxes in one tile)
-    // 256-wide tiles on few m-tiles leave the last wave of the persistent grid mostly empty; 128-wide tiles double the units.
-    // Pick the width with fewer tile-columns per SM over all waves (a partial last wave costs a whole one).
-    long long n_valid = 0;
-    for (long long t = 0; t < (a.M_total + 127) / 128; ++t) {
-      bool any = false;
-      for (int r = 0; r < 128 && !any; ++r) {
-        const long long v = t * 128 + r;
-        if (v >= a.M_total) break;
-        const int rr = (int)(v % a.rows_per_img);
-        any = (rr / a.in_Wp < g.Ho) && (rr % a.in_Wp < g.Wo);
-      }
-      n_valid += any;
-    }
-    const int sms = m->ctx->sm_count;
-    const long long u256 = n_valid * ((g.cout + 255) / 256), u128 = n_valid * ((g.cout + 127) / 128);
-    const double t256 = (double)((u256 + sms - 1) / sms) * 256.0;
-    const double t128 = (double)((u128 + sms - 1) / sms) * 128.0;
-    const bool use128 = t128 < t256;
-    if (use128) a.BN = 128;
-  }
-  a.acc_split = a.split;
-  a.n_tiles_n = (g.cout + a.BN - 1) / a.BN;
-  const int n_m = (a.M_total + 127) / 128;
-  conv_pick_stages(a);
   // m-tiles that hold at least one valid output row
   std::vector<int> tiles;
-  for (int t = 0; t < n_m; ++t) {
+  for (int t = 0; t < (a.M_total + 127) / 128; ++t) {
     bool any = false;
     for (int r = 0; r < 128 && !any; ++r) {
       long long v = (long long)t * 128 + r;
@@ -326,6 +293,27 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
     }
     if (any) tiles.push_back(t);
   }
+  a.BN = g.cout <= 64 ? 64 : (g.cout <= 128 ? 128 : 256);
+  a.split = m->split;
+  a.k_split = 1;
+  if (a.split && a.BN == 256) {
+    // bf16x3 tiles carry the cross-term accumulator, which fits in registers up to 160 columns: 160-wide tiles for
+    // the predictor heads of <= 160 columns (6 boxes x 25 for VOC: the fused head epilogue needs all boxes of a pixel in one
+    // tile), 128-wide tiles otherwise
+    a.BN = g.cout <= 160 ? 160 : 128;
+  } else if (a.BN == 256 && g.cout % 128 == 0) {                // (not the predictor heads: their epilogue needs all boxes in one tile)
+    // 256-wide tiles on few m-tiles leave the last wave of the persistent grid mostly empty; 128-wide tiles double the units.
+    // Pick the width with fewer tile-columns per SM over all waves (a partial last wave costs a whole one).
+    const long long n_valid = (long long)tiles.size();
+    const int sms = m->ctx->sm_count;
+    const long long u256 = n_valid * ((g.cout + 255) / 256), u128 = n_valid * ((g.cout + 127) / 128);
+    const double t256 = (double)((u256 + sms - 1) / sms) * 256.0;
+    const double t128 = (double)((u128 + sms - 1) / sms) * 128.0;
+    const bool use128 = t128 < t256;
+    if (use128) a.BN = 128;
+  }
+  a.n_tiles_n = (g.cout + a.BN - 1) / a.BN;
+  conv_pick_stages(a);
   a.n_tiles_m = (int)tiles.size();
   int* tl = nullptr;
   int rc = dev_alloc(m->allocs, &tl, tiles.size(), false); if (rc) return rc;

@@ -71,28 +71,6 @@ __global__ void __launch_bounds__(256) transpose_kernel(const __nv_bfloat16* __r
   }
 }
 
-// bias gradient: gb[c] += sum_v dZT[c][v]
-__global__ void __launch_bounds__(256) rowsum_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo, long long ldT,
-                                                     long long Kv, float* __restrict__ gb) {
-  __shared__ float s[8];
-  const int c = blockIdx.y;
-  const long long chunk = (Kv + gridDim.x - 1) / gridDim.x;
-  const long long v0 = (long long)blockIdx.x * chunk, v1 = min(Kv, v0 + chunk);
-  float acc = 0.f;
-  for (long long v = v0 + threadIdx.x; v < v1; v += 256) {
-    acc += __bfloat162float(hi[(long long)c * ldT + v]);
-    if (lo) acc += __bfloat162float(lo[(long long)c * ldT + v]);
-  }
-  acc = warp_sum(acc);
-  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t = 0.f;
-    for (int w = 0; w < 8; ++w) t += s[w];
-    atomicAdd(gb + c, t);
-  }
-}
-
 // Backward of Reshape/softmax/Concat (models/keras_ssd300.py:363-419): dY_pred rows -> gradient of the fused head conv output.
 __global__ void head_bwd_kernel(const float* __restrict__ head, const float* __restrict__ dy, int B, int H, int W, int n_boxes, int C,
                                 int P, int prior_off, ActBuf g) {
@@ -899,10 +877,8 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       else
         rc = launch(ctx, wgrad_direct_kernel, grid, 256, smem, s, PL.out, T.g, span_grad(t, i, 0), d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
       if (rc) return rc;
-      rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     } else if (T.wg_native) {
       rc = launch_wgrad(ctx, T.wg, s); if (rc) return rc;
-      rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     } else {
       // transposed operands
       rc = do_transpose(t, T.g.hi, T.g.lo, T.g.Cs, (long long)T.g.rows(), T.dy_map, T.Kv, T.cout, t->dyT_hi, t->dyT_lo, T.ldT, s); if (rc) return rc;
@@ -920,9 +896,8 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
             if (T.wgrad_res[tp] == r) { rc = launch_conv(ctx, T.wgrad[tp], s); if (rc) return rc; }
         }
       }
-      rc = launch(ctx, rowsum_kernel, dim3(64, T.cout), 256, 0, s, t->dyT_hi, t->dyT_lo, T.ldT, T.Kv, span_grad(t, i, 1));
-      if (rc) return rc;
     }
+    rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     // ---- data gradient
     if (T.has_dgrad && T.dgrad_strided) {
       rc = launch_conv(ctx, T.dgrad, s); if (rc) return rc;
