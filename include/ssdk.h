@@ -118,21 +118,18 @@ typedef struct {
 int ssdk_encoder_create(ssdk_ctx* ctx, const ssdk_encode_cfg* cfg, const double* anchors_host /* [P*4], in cfg->coords */,
                         ssdk_encoder** out);
 int ssdk_encoder_destroy(ssdk_encoder* enc);
-/* gt_boxes_dev: [sum(G_i) * 5] float32 rows (class_id, xmin, ymin, xmax, ymax) in pixels, images concatenated;
- * gt_offsets_host: [B+1] row offsets (host; the ragged shape is host knowledge in the reference too);
+/* gt_boxes_dev: [sum(G_i) * 5] rows (class_id, xmin, ymin, xmax, ymax) in pixels, images concatenated, float32 (gt_f64 = 0)
+ * or float64 (1): the reference converts whatever it is given to float64 (:330), so labels that are not representable in
+ * float32 (sub-pixel coordinates after augmentation) need float64 rows to stay bit-exact.
+ * Row offsets [B+1], exactly one of: gt_offsets_host (the ragged shape is host knowledge in the reference too; total_g and
+ * max_g are derived from it and the arguments ignored), or gt_offsets_dev (the batch was assembled on the device, see
+ * ssdk_assemble_batch: nothing is read from the host; total_g = gt_offsets[B] and max_g = the largest per-image box count, or
+ * an upper bound of it; float32 rows only).
  * out_y_dev: [B * P * (C+12)] float32;  out_match_dev (optional): [B * P] int32, matched gt index within the
  * image, -1 = background, -2 = neutral.  status_dev (optional): one int32 that is set to the 1-based index of
  * a batch item with a degenerate box (xmax<=xmin or ymax<=ymin), else left 0 (reference raises :333-336). */
-int ssdk_encode(ssdk_encoder* enc, const float* gt_boxes_dev, const int* gt_offsets_host, int B,
-                float* out_y_dev, int* out_match_dev, int* status_dev, void* stream);
-/* Same with float64 ground-truth rows: the reference converts whatever it is given to float64 (:330), so labels that are
- * not representable in float32 (sub-pixel coordinates after augmentation) need this entry to stay bit-exact. */
-int ssdk_encode_f64(ssdk_encoder* enc, const double* gt_boxes_dev, const int* gt_offsets_host, int B,
-                    float* out_y_dev, int* out_match_dev, int* status_dev, void* stream);
-/* Same with the row offsets already on the device (the batch was assembled there, see ssdk_assemble_batch): nothing
- * is read from the host; total_g = gt_offsets[B] and max_g = the largest per-image box count (or an upper bound of it). */
-int ssdk_encode_dev(ssdk_encoder* enc, const float* gt_boxes_dev, const int* gt_offsets_dev, int B, int total_g, int max_g,
-                    float* out_y_dev, int* out_match_dev, int* status_dev, void* stream);
+int ssdk_encode(ssdk_encoder* enc, const void* gt_boxes_dev, int gt_f64, const int* gt_offsets_host, const int* gt_offsets_dev,
+                int B, int total_g, int max_g, float* out_y_dev, int* out_match_dev, int* status_dev, void* stream);
 /* Standalone pieces, used by tests and the micro-benchmark: IoU matrix (G x P, float64, row-major). */
 int ssdk_iou_matrix(ssdk_encoder* enc, const float* gt_boxes_dev, int G, double* out_dev, void* stream);
 /* General IoU, replaces iou() (bounding_box_utils/bounding_box_utils.py:283-383): boxes1 [m*4], boxes2 [n*4] float64 in
@@ -181,7 +178,7 @@ typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
  * out_stats_dev (optional) [2] = total number of boxes left, largest per-image count.  Everything stays on the device: feed
- * the result to ssdk_encode_dev with total_in / the input's largest count as upper bounds. */
+ * the result to ssdk_encode with device offsets and total_in / the input's largest count as upper bounds. */
 int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, const int* offsets_in_dev, int B, int total_in,
                         const ssdk_box_op* ops_dev, int max_ops, float* gt_out_dev, int* offsets_out_dev, int* out_stats_dev,
                         void* stream);
@@ -322,20 +319,15 @@ int ssdk_nms(ssdk_ctx* ctx, const float* boxes_dev, const float* scores_dev, int
 
 /* ------------------------------------------------------------------------------------------
  * SSD loss.  Replaces SSDLoss.compute_loss (keras_loss_function/keras_ssd_loss.py:98-211).
- * out_loss_dev [B] float32.  bwd writes d(sum_b upstream[b]*loss[b])/d y_pred with the hard-negative
- * mask held constant (upstream_dev NULL = 1/B each, the Keras batch mean).  One cooperative kernel launch per call
- * (csrc/loss.cu): per-box losses, batch-global top-k by a two-level histogram select, masked sums / gradient.
+ * out_loss_dev [B] float32; out_stats_dev (optional) [4]: n_positive, n_neg_losses, k, ties_taken; out_grad_dev
+ * [B*P*(C+12)]: d(sum_b upstream[b]*loss[b])/d y_pred with the hard-negative mask held constant (upstream_dev NULL = 1/B
+ * each, the Keras batch mean).  The gradient is computed exactly when out_grad_dev is given; out_loss_dev and out_grad_dev
+ * must not both be NULL.  One cooperative kernel launch per call (csrc/loss.cu): per-box losses, batch-global top-k by a
+ * two-level histogram select, masked sums / gradient.
  * ------------------------------------------------------------------------------------------ */
-int ssdk_ssd_loss_fwd(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
-                      int neg_pos_ratio, int n_neg_min, float alpha, float* out_loss_dev,
-                      int* out_stats_dev /* optional [4]: n_positive, n_neg_losses, k, ties_taken */, void* stream);
-int ssdk_ssd_loss_bwd(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
-                      int neg_pos_ratio, int n_neg_min, float alpha, const float* upstream_dev,
-                      float* out_grad_dev /* [B*P*(C+12)] */, void* stream);
-/* Loss and gradient from ONE launch of the same kernel (what a training step needs). */
-int ssdk_ssd_loss_fwd_bwd(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
-                          int neg_pos_ratio, int n_neg_min, float alpha, const float* upstream_dev, float* out_loss_dev,
-                          int* out_stats_dev, float* out_grad_dev, void* stream);
+int ssdk_ssd_loss(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
+                  int neg_pos_ratio, int n_neg_min, float alpha, const float* upstream_dev, float* out_loss_dev,
+                  int* out_stats_dev, float* out_grad_dev, void* stream);
 
 /* Multi-GPU, global-batch-exact loss.  The reference's n_positive (:143) and hard-negative top-k (:179-183) run over the
  * WHOLE batch; when the batch is sharded over ranks the kernel's phases are launched one by one on a caller-provided
@@ -361,8 +353,9 @@ int ssdk_ssd_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true_dev, const
                         float* out_loss_dev, int* out_stats_dev, float* out_grad_dev, void* stream);
 
 /* Read-only views of the loss kernel, for tests and diagnostics.
- *   ssdk_ssd_loss_plan  the launch a call with these arguments would make (want_grad: bwd / fwd_bwd / phase 4 with a gradient;
- *                       cooperative: the fused entry points, 0 = ssdk_ssd_loss_phase), or the error that call would return.
+ *   ssdk_ssd_loss_plan  the launch a call with these arguments would make (want_grad: ssdk_ssd_loss with out_grad_dev, or
+ *                       phase 4 with a gradient; cooperative: ssdk_ssd_loss, 0 = ssdk_ssd_loss_phase), or the error that
+ *                       call would return.
  *                       stages: shared-memory tile buffers (1 or 2); bulk_ok: tiles are loaded with cp.async.bulk (P*(C+12)
  *                       a multiple of 4 and both inputs 16-byte aligned), else by plain loads.  Launches nothing and changes
  *                       no state of the context (workspace, histogram parity).  Like a call of the same size, it may raise
@@ -511,8 +504,8 @@ int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_plan* out);
  * Training step (BASELINE config 3).  Replaces what Keras/TensorFlow do for the reference in model.fit_generator:
  * autodiff of the graph (models/keras_ssd300.py:263-419) and of SSDLoss (keras_ssd_loss.py:98-211), the kernel_regularizer
  * l2(l2_reg) (models/keras_ssd300.py:274), SGD(lr, momentum) (ssd300_training.ipynb:169) and Adam (ssd7_training.ipynb:153).
- *   ssdk_train_backward  after ssdk_model_forward on the same images: loss + gradients of every kernel / bias / gamma into one
- *                        flat float32 buffer (so that a single NCCL all-reduce covers it).
+ *   ssdk_train_backward_begin / _layers  after ssdk_model_forward on the same images: loss + gradients of every kernel /
+ *                        bias / gamma into one flat float32 buffer (so that a single NCCL all-reduce covers it).
  *   ssdk_train_apply     g = grad*grad_scale + 2*l2*w (kernels only); v = momentum*v - lr*g; w += v; re-pack the bf16 planes.
  * Parameter order in the flat buffer: layers in graph order, for each conv [kernel as (cout, kh, kw, cin) | bias | BatchNorm
  * gamma | BatchNorm beta], for each head [fused kernel (n_boxes*(C+4), 3, 3, cin) | fused bias], for L2Normalization [gamma].
@@ -525,7 +518,6 @@ int ssdk_trainer_num_params(const ssdk_trainer* t, long long* out_n);
 /* offset (in floats) and element count of a layer's kernel (which=0), bias (1), L2Normalization gamma (2), BatchNormalization
  * gamma (3) or beta (4) inside the flat buffers */
 int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int which, long long* out_offset, long long* out_count);
-float* ssdk_trainer_grad_buffer(ssdk_trainer* t);
 /* Read-only views of a layer's output gradient (the planes the backward pass writes and the next launches read).
  *   ssdk_trainer_grad_shape        stored geometry of the planes: padded rows Hp, padded row pitch Wp, stored channels Cs
  *                                  (multiple of 8), zero border pad; a plane holds B*Hp*Wp*Cs bf16 values.
@@ -535,20 +527,19 @@ float* ssdk_trainer_grad_buffer(ssdk_trainer* t);
 int ssdk_trainer_grad_shape(const ssdk_trainer* t, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad);
 int ssdk_trainer_read_grad(ssdk_trainer* t, int layer, float* out_dev, void* stream);
 int ssdk_trainer_read_grad_planes(ssdk_trainer* t, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream);
-int ssdk_train_backward(ssdk_trainer* t, const float* y_true_dev, const float* y_pred_dev, int neg_pos_ratio, int n_neg_min,
-                        float alpha, float* out_loss_dev /* [B] */, void* stream);
-/* The step in pieces, for overlapping the gradient exchange with the backward pass:
- *   ssdk_train_backward_begin   loss + d loss / d y_pred (kept inside the trainer), gradient buffer cleared;
+/* The backward pass in pieces, so that the gradient exchange can overlap it:
+ *   ssdk_train_backward_begin   loss (out_loss_dev [B], optional) + d loss / d y_pred (kept inside the trainer), gradient
+ *                               buffer cleared;
  *   ssdk_train_backward_layers  layers hi .. lo (graph indices, top down, consecutive calls cover n_layers-1 .. 0).  In stream
  *                               order after the call the parameter gradients of exactly these layers are final, so their
  *                               span of the flat buffer (ssdk_trainer_param_span) can be all-reduced on another stream while the
- *                               lower layers are still being differentiated.  dypred_dev NULL = the trainer's own. */
+ *                               lower layers are still being differentiated.  dypred_dev NULL = the trainer's own; otherwise
+ *                               d loss / d y_pred, (B,P,C+12) float32, that the caller computed (the multi-GPU
+ *                               global-batch-exact loss, whose phases run between NCCL collectives, see ssdk_ssd_loss_phase),
+ *                               and a pass that starts at the top layer clears the gradient buffer first. */
 int ssdk_train_backward_begin(ssdk_trainer* t, const float* y_true_dev, const float* y_pred_dev, int neg_pos_ratio, int n_neg_min,
                               float alpha, float* out_loss_dev, void* stream);
 int ssdk_train_backward_layers(ssdk_trainer* t, const float* dypred_dev, int hi, int lo, void* stream);
-/* The same backward pass from a gradient the caller computed: dypred_dev = d loss / d y_pred, (B,P,C+12) float32 (used with the
- * multi-GPU global-batch-exact loss, whose phases run between NCCL collectives, see ssdk_ssd_loss_phase). */
-int ssdk_train_backward_dy(ssdk_trainer* t, const float* dypred_dev, void* stream);
 int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float l2_reg, float grad_scale, void* stream);
 /* Adam as Keras applies it (ssd7_training.ipynb:153: Adam(lr=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-08, decay=0.0)):
  * g = grad*grad_scale + 2*l2*w (kernels); lr_t = lr*sqrt(1-beta2^t)/(1-beta1^t); m = b1*m + (1-b1)*g; v = b2*v + (1-b2)*g^2;

@@ -23,6 +23,7 @@ c_float_p = C.POINTER(C.c_float)
 c_double_p = C.POINTER(C.c_double)
 
 
+# The structs of include/ssdk.h, each named after the C struct without its ssdk_ prefix (BoxOp = ssdk_box_op).
 class AnchorCfg(C.Structure):
     _fields_ = [('img_height', C.c_int), ('img_width', C.c_int), ('n_layers', C.c_int),
                 ('fm_height', c_int_p), ('fm_width', c_int_p), ('scales', c_double_p),
@@ -108,7 +109,7 @@ class LayerPlan(C.Structure):
                                        'epilogue', 'head_fused', 'im2col_vec8')]
 
 
-class TrainerLayerPlan(C.Structure):
+class BackwardPlan(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('dgrad', 'dgrad_bn', 'dgrad_mask', 'dgrad_accumulate', 'dgrad_n_tiles_m', 'dgrad_n_tiles_n',
                                        'dgrad_grid', 'wgrad', 'wgrad_bn', 'a_boxes', 'bw', 'bh', 'co_tiles', 'ci_tiles', 'k_split',
                                        'n_gemms', 'stages', 'grid', 'kv', 'direct_fast')]
@@ -132,9 +133,9 @@ def model_layer_plan(handle, layer):
 
 def trainer_layer_plan(handle, layer):
     """The backward launches of one layer of a trainer, as a dict (ssdk_trainer_layer_plan)."""
-    p = TrainerLayerPlan()
+    p = BackwardPlan()
     check(lib().ssdk_trainer_layer_plan(handle, int(layer), C.byref(p)))
-    out = {n: getattr(p, n) for n, _ in TrainerLayerPlan._fields_}
+    out = {n: getattr(p, n) for n, _ in BackwardPlan._fields_}
     out['dgrad'] = DGRAD_PATHS[p.dgrad]
     out['wgrad'] = WGRAD_PATHS[p.wgrad]
     return out
@@ -142,6 +143,68 @@ def trainer_layer_plan(handle, layer):
 
 OP_INPUT, OP_CONV, OP_MAXPOOL, OP_L2NORM, OP_HEAD, OP_TENSOR = range(6)
 ACT_NONE, ACT_RELU, ACT_ELU = range(3)
+
+# Every function of include/ssdk.h, in its order: name -> (restype, argtypes).  tests/test_abi_cpu.py holds it to the header.
+_p, _i, _ll, _f, _d = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
+SIGNATURES = {
+    'ssdk_version': (_i, []),
+    'ssdk_last_error': (C.c_char_p, []),
+    'ssdk_ctx_create': (_i, [_i, C.POINTER(_p)]),
+    'ssdk_ctx_destroy': (_i, [_p]),
+    'ssdk_ctx_launch_count': (C.c_int64, [_p]),
+    'ssdk_anchors_count': (_i, [C.POINTER(AnchorCfg), c_int_p, c_int_p]),
+    'ssdk_anchors_generate': (_i, [C.POINTER(AnchorCfg), c_double_p, c_float_p]),
+    'ssdk_encoder_create': (_i, [_p, C.POINTER(EncodeCfg), c_double_p, C.POINTER(_p)]),
+    'ssdk_encoder_destroy': (_i, [_p]),
+    'ssdk_encode': (_i, [_p, _p, _i, c_int_p, _p, _i, _i, _i, _p, _p, _p, _p]),
+    'ssdk_iou_matrix': (_i, [_p, _p, _i, _p, _p]),
+    'ssdk_iou': (_i, [_p, _p, _i, _p, _i, _i, _i, _i, _p, _p]),
+    'ssdk_assemble_batch': (_i, [_p, _p, _i, _p, _i, _i, _p, _i, _p, _p, _p, _p]),
+    'ssdk_assemble_images': (_i, [_p, _p, _p, _p, _i, _p, _i, _i, _i, _p, _p]),
+    'ssdk_eval_match': (_i, [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _d, _i, _p, _p, _p]),
+    'ssdk_eval_cumsum': (_i, [_p, _p, _p, _p, _i, _p, _p, _p]),
+    'ssdk_eval_collect': (_i, [_p, _p, _i, _i, _p, _p, c_int_p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
+    'ssdk_decode': (_i, [_p, C.POINTER(DecodeCfg), _p, _i, _p, _p, _p, _p]),
+    'ssdk_nms': (_i, [_p, _p, _p, _i, _i, _d, _d, _i, _i, _p, _p, _p, _p]),
+    'ssdk_ssd_loss': (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _f, _p, _p, _p, _p, _p]),
+    'ssdk_ssd_loss_ws_layout': (_i, [_i, _i, C.POINTER(LossWsLayout)]),
+    'ssdk_ssd_loss_phase': (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _f, _p, _i, _p, _i, _p, _p, _p, _p, _p]),
+    'ssdk_ssd_loss_plan': (_i, [_p, _p, _p, _i, _i, _i, _i, _i, C.POINTER(LossPlan)]),
+    'ssdk_ssd_loss_read_box_losses': (_i, [_p, _p, _i, _i, _p, _p, _p]),
+    'ssdk_l2_normalize': (_i, [_p, _p, _ll, _i, _p, _p, _p]),
+    'ssdk_conv2d_fwd': (_i, [_p, _p] + [_i] * 4 + [_p, _p] + [_i] * 11 + [_p, _p]),
+    'ssdk_maxpool': (_i, [_p, _p] + [_i] * 11 + [_p, _p]),
+    'ssdk_schedule_preview': (_i, [_i, c_int_p, c_int_p, c_int_p, _i, _i, C.POINTER(C.c_ubyte), c_int_p, c_int_p]),
+    'ssdk_model_create': (_i, [_p, C.POINTER(ModelDesc), C.POINTER(_p)]),
+    'ssdk_model_destroy': (_i, [_p]),
+    'ssdk_model_num_priors': (_i, [_p, c_int_p]),
+    'ssdk_model_layer_shape': (_i, [_p, _i, c_int_p, c_int_p, c_int_p]),
+    'ssdk_model_forward': (_i, [_p, _p, _p, _p]),
+    'ssdk_model_read_layer': (_i, [_p, _i, _p, _p]),
+    'ssdk_model_layer_planes_shape': (_i, [_p, _i, c_int_p, c_int_p, c_int_p, c_int_p]),
+    'ssdk_model_read_layer_planes': (_i, [_p, _i, _p, _p, _p]),
+    'ssdk_model_flops': (_i, [_p, c_double_p, c_double_p]),
+    'ssdk_model_set_timing': (_i, [_p, _i]),
+    'ssdk_model_last_conv_ms': (_i, [_p, c_float_p]),
+    'ssdk_model_layer_ms': (_i, [_p, _i, c_float_p]),
+    'ssdk_model_layer_plan': (_i, [_p, _i, C.POINTER(LayerPlan)]),
+    'ssdk_trainer_create': (_i, [_p, _p, C.POINTER(_p)]),
+    'ssdk_trainer_destroy': (_i, [_p]),
+    'ssdk_trainer_num_params': (_i, [_p, C.POINTER(_ll)]),
+    'ssdk_trainer_param_span': (_i, [_p, _i, _i, C.POINTER(_ll), C.POINTER(_ll)]),
+    'ssdk_trainer_grad_shape': (_i, [_p, _i, c_int_p, c_int_p, c_int_p, c_int_p]),
+    'ssdk_trainer_read_grad': (_i, [_p, _i, _p, _p]),
+    'ssdk_trainer_read_grad_planes': (_i, [_p, _i, _p, _p, _p]),
+    'ssdk_train_backward_begin': (_i, [_p, _p, _p, _i, _i, _f, _p, _p]),
+    'ssdk_train_backward_layers': (_i, [_p, _p, _i, _i, _p]),
+    'ssdk_train_apply': (_i, [_p, _f, _f, _f, _f, _p]),
+    'ssdk_train_apply_adam': (_i, [_p, _f, _f, _f, _f, _f, _f, _i, _p]),
+    'ssdk_trainer_read_bn_stats': (_i, [_p, _i, _p, _p, _p]),
+    'ssdk_trainer_read_bn_input': (_i, [_p, _i, _p, _p]),
+    'ssdk_trainer_read_params': (_i, [_p, _p, _p]),
+    'ssdk_trainer_read_opt_state': (_i, [_p, _i, _p, _p]),
+    'ssdk_trainer_layer_plan': (_i, [_p, _i, C.POINTER(BackwardPlan)]),
+}
 
 _lib = None
 _lock = threading.Lock()
@@ -163,106 +226,9 @@ def lib():
             raise SSDKError("libssdk.so is not built (%s). Run `python -m ssd_keras_b200.build` "
                             "(or __graft_entry__.build()); there is no CPU/PyTorch fallback." % _LIB_PATH)
         L = C.CDLL(_LIB_PATH)
-        vp = C.c_void_p
-        L.ssdk_version.restype = C.c_int
-        L.ssdk_last_error.restype = C.c_char_p
-        L.ssdk_ctx_create.argtypes = [C.c_int, C.POINTER(vp)]
-        L.ssdk_ctx_destroy.argtypes = [vp]
-        L.ssdk_ctx_launch_count.argtypes = [vp]
-        L.ssdk_ctx_launch_count.restype = C.c_int64
-        L.ssdk_anchors_count.argtypes = [C.POINTER(AnchorCfg), c_int_p, c_int_p]
-        L.ssdk_anchors_generate.argtypes = [C.POINTER(AnchorCfg), c_double_p, c_float_p]
-        L.ssdk_encoder_create.argtypes = [vp, C.POINTER(EncodeCfg), c_double_p, C.POINTER(vp)]
-        L.ssdk_encoder_destroy.argtypes = [vp]
-        L.ssdk_encode.argtypes = [vp, vp, c_int_p, C.c_int, vp, vp, vp, vp]
-        L.ssdk_encode_f64.argtypes = [vp, vp, c_int_p, C.c_int, vp, vp, vp, vp]
-        L.ssdk_encode_dev.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
-        L.ssdk_iou_matrix.argtypes = [vp, vp, C.c_int, vp, vp]
-        L.ssdk_iou.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
-        L.ssdk_decode.argtypes = [vp, C.POINTER(DecodeCfg), vp, C.c_int, vp, vp, vp, vp]
-        L.ssdk_nms.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_int, vp, vp, vp, vp]
-        L.ssdk_ssd_loss_fwd.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, vp, vp]
-        L.ssdk_ssd_loss_bwd.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, vp, vp]
-        L.ssdk_ssd_loss_fwd_bwd.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, vp, vp, vp, vp]
-        L.ssdk_ssd_loss_ws_layout.argtypes = [C.c_int, C.c_int, C.POINTER(LossWsLayout)]
-        L.ssdk_ssd_loss_phase.argtypes = [vp, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp,
-                                          C.c_int, vp, vp, vp, vp, vp]
-        L.ssdk_ssd_loss_plan.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(LossPlan)]
-        L.ssdk_ssd_loss_read_box_losses.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp]
-        for name in ('ssdk_ssd_loss_fwd_bwd', 'ssdk_ssd_loss_ws_layout', 'ssdk_ssd_loss_phase', 'ssdk_ssd_loss_plan',
-                     'ssdk_ssd_loss_read_box_losses'):
-            getattr(L, name).restype = C.c_int
-        L.ssdk_eval_match.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_double, C.c_int, vp, vp, vp]
-        L.ssdk_eval_cumsum.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp]
-        L.ssdk_eval_match.restype = C.c_int
-        L.ssdk_eval_cumsum.restype = C.c_int
-        L.ssdk_eval_collect.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, c_int_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp,
-                                        vp, vp, vp, vp]
-        L.ssdk_eval_collect.restype = C.c_int
-        L.ssdk_assemble_batch.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp]
-        L.ssdk_assemble_batch.restype = C.c_int
-        L.ssdk_assemble_images.argtypes = [vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp]
-        L.ssdk_assemble_images.restype = C.c_int
-        L.ssdk_l2_normalize.argtypes = [vp, vp, C.c_longlong, C.c_int, vp, vp, vp]
-        L.ssdk_l2_normalize.restype = C.c_int
-        L.ssdk_conv2d_fwd.argtypes = [vp, vp] + [C.c_int] * 4 + [vp, vp] + [C.c_int] * 11 + [vp, vp]
-        L.ssdk_conv2d_fwd.restype = C.c_int
-        L.ssdk_maxpool.argtypes = [vp, vp] + [C.c_int] * 11 + [vp, vp]
-        L.ssdk_maxpool.restype = C.c_int
-        if hasattr(L, 'ssdk_model_create'):
-            L.ssdk_model_create.argtypes = [vp, C.POINTER(ModelDesc), C.POINTER(vp)]
-            L.ssdk_model_destroy.argtypes = [vp]
-            L.ssdk_model_num_priors.argtypes = [vp, c_int_p]
-            L.ssdk_model_layer_shape.argtypes = [vp, C.c_int, c_int_p, c_int_p, c_int_p]
-            L.ssdk_model_forward.argtypes = [vp, vp, vp, vp]
-            L.ssdk_model_read_layer.argtypes = [vp, C.c_int, vp, vp]
-            L.ssdk_model_flops.argtypes = [vp, c_double_p, c_double_p]
-            L.ssdk_model_set_timing.argtypes = [vp, C.c_int]
-            L.ssdk_model_last_conv_ms.argtypes = [vp, c_float_p]
-            L.ssdk_model_layer_ms.argtypes = [vp, C.c_int, c_float_p]
-            L.ssdk_model_layer_plan.argtypes = [vp, C.c_int, C.POINTER(LayerPlan)]
-            L.ssdk_model_layer_plan.restype = C.c_int
-            L.ssdk_model_layer_planes_shape.argtypes = [vp, C.c_int, c_int_p, c_int_p, c_int_p, c_int_p]
-            L.ssdk_model_read_layer_planes.argtypes = [vp, C.c_int, vp, vp, vp]
-            L.ssdk_model_layer_planes_shape.restype = C.c_int
-            L.ssdk_model_read_layer_planes.restype = C.c_int
-        if hasattr(L, 'ssdk_trainer_create'):
-            L.ssdk_trainer_create.argtypes = [vp, vp, C.POINTER(vp)]
-            L.ssdk_trainer_destroy.argtypes = [vp]
-            L.ssdk_trainer_num_params.argtypes = [vp, C.POINTER(C.c_longlong)]
-            L.ssdk_trainer_param_span.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
-            L.ssdk_trainer_grad_buffer.argtypes = [vp]
-            L.ssdk_trainer_grad_buffer.restype = vp
-            L.ssdk_train_backward.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, vp]
-            L.ssdk_train_apply_adam.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, vp]
-            L.ssdk_train_apply_adam.restype = C.c_int
-            L.ssdk_trainer_read_bn_stats.argtypes = [vp, C.c_int, vp, vp, vp]
-            L.ssdk_trainer_read_bn_stats.restype = C.c_int
-            L.ssdk_train_backward_dy.argtypes = [vp, vp, vp]
-            L.ssdk_train_backward_dy.restype = C.c_int
-            L.ssdk_train_backward_begin.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, vp]
-            L.ssdk_train_backward_begin.restype = C.c_int
-            L.ssdk_train_backward_layers.argtypes = [vp, vp, C.c_int, C.c_int, vp]
-            L.ssdk_train_backward_layers.restype = C.c_int
-            L.ssdk_train_apply.argtypes = [vp, C.c_float, C.c_float, C.c_float, C.c_float, vp]
-            L.ssdk_trainer_read_params.argtypes = [vp, vp, vp]
-            L.ssdk_trainer_layer_plan.argtypes = [vp, C.c_int, C.POINTER(TrainerLayerPlan)]
-            L.ssdk_trainer_layer_plan.restype = C.c_int
-            L.ssdk_trainer_grad_shape.argtypes = [vp, C.c_int, c_int_p, c_int_p, c_int_p, c_int_p]
-            L.ssdk_trainer_read_grad.argtypes = [vp, C.c_int, vp, vp]
-            L.ssdk_trainer_read_grad_planes.argtypes = [vp, C.c_int, vp, vp, vp]
-            L.ssdk_trainer_read_bn_input.argtypes = [vp, C.c_int, vp, vp]
-            L.ssdk_trainer_read_opt_state.argtypes = [vp, C.c_int, vp, vp]
-            for name in ('ssdk_trainer_grad_shape', 'ssdk_trainer_read_grad', 'ssdk_trainer_read_grad_planes', 'ssdk_trainer_read_bn_input',
-                         'ssdk_trainer_read_opt_state'):
-                getattr(L, name).restype = C.c_int
-            for name in ('ssdk_trainer_create', 'ssdk_trainer_destroy', 'ssdk_trainer_num_params', 'ssdk_trainer_param_span',
-                         'ssdk_train_backward', 'ssdk_train_apply', 'ssdk_trainer_read_params'):
-                getattr(L, name).restype = C.c_int
-        for name in ('ssdk_ctx_create', 'ssdk_ctx_destroy', 'ssdk_anchors_count', 'ssdk_anchors_generate',
-                     'ssdk_encoder_create', 'ssdk_encoder_destroy', 'ssdk_encode', 'ssdk_encode_f64', 'ssdk_encode_dev', 'ssdk_iou_matrix', 'ssdk_iou', 'ssdk_decode',
-                     'ssdk_nms', 'ssdk_ssd_loss_fwd', 'ssdk_ssd_loss_bwd'):
-            getattr(L, name).restype = C.c_int
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
 

@@ -136,12 +136,12 @@ inline int allow_smem(const ssdk_ctx* ctx, const void* kernel, size_t bytes) {
 // that the tests hold to the same reference), or report what the encoder's matching stage did; none is needed in normal use.
 //
 //   switch                 default             read at                 selects
-//   SSDK_ENC_SPATIAL_MIN   24                  each ssdk_encode*       the spatial tile set once the batch's largest image has
+//   SSDK_ENC_SPATIAL_MIN   24                  each ssdk_encode        the spatial tile set once the batch's largest image has
 //                                                                      this many boxes
-//   SSDK_ENC_LB_MIN        17                  each ssdk_encode*       enc_lb_kernel's lower bounds from the same count on
-//   SSDK_ENC_TPC           1 ... 8 by boxes    each ssdk_encode*       tiles per CTA (at least 1; halved while the grid has
+//   SSDK_ENC_LB_MIN        17                  each ssdk_encode        enc_lb_kernel's lower bounds from the same count on
+//   SSDK_ENC_TPC           1 ... 8 by boxes    each ssdk_encode        tiles per CTA (at least 1; halved while the grid has
 //                                                                      fewer than 8 CTAs per SM)
-//   SSDK_ENC_COUNTERS      0                   each ssdk_encode*       1: print the conflict loop's event counts to stderr
+//   SSDK_ENC_COUNTERS      0                   each ssdk_encode        1: print the conflict loop's event counts to stderr
 //                                                                      (synchronises the stream)
 //   SSDK_NMS_TWO_STAGE     1                   each ssdk_decode / nms  0: always the full multi-band NMS scan
 //   SSDK_SHARED_BORDER     1                   model plan creation     0: inference activations keep one border per image

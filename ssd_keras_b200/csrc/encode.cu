@@ -1164,9 +1164,33 @@ extern "C" int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const do
 
 namespace {
 
-// Common launch path.  offs_host (B+1 ints) may be NULL when offs_dev is given together with total_g / max_g.
-int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* offs_host, const int* offs_dev, int B, int total_g,
-                  int max_g, float* out_y_dev, int* out_match_dev, int* status_dev, cudaStream_t stream) {
+int scan_offsets(const int* offs, int B, int* total_g, int* max_g) {
+  SSDK_REQUIRE(offs[0] == 0 && offs[B] >= 0, "ssdk_encode: gt_offsets must start at 0 and be non-decreasing");
+  int mg = 0;
+  for (int b = 0; b < B; ++b) {
+    const int g = offs[b + 1] - offs[b];
+    SSDK_REQUIRE(g >= 0, "ssdk_encode: gt_offsets must be non-decreasing");
+    mg = g > mg ? g : mg;
+  }
+  *total_g = offs[B]; *max_g = mg;
+  return SSDK_OK;
+}
+
+}  // namespace
+
+// Exactly one of offs_host / offs_dev (B+1 ints).  Host offsets are scanned for total_g / max_g; with device offsets the caller
+// gives them, and the rows must be float32 (float64 rows with device offsets have no caller).
+extern "C" int ssdk_encode(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* offs_host, const int* offs_dev, int B,
+                           int total_g, int max_g, float* out_y_dev, int* out_match_dev, int* status_dev, void* stream_) {
+  SSDK_REQUIRE(e && (offs_host != nullptr) != (offs_dev != nullptr) && out_y_dev && B > 0, "ssdk_encode: bad argument");
+  if (offs_host) {
+    const int rc = scan_offsets(offs_host, B, &total_g, &max_g);
+    if (rc) return rc;
+  } else {
+    SSDK_REQUIRE(total_g >= 0 && max_g >= 0, "ssdk_encode: bad argument");
+    SSDK_REQUIRE(!gt_f64, "ssdk_encode: float64 rows need host offsets");
+  }
+  cudaStream_t stream = (cudaStream_t)stream_;
   const EncParams& p = e->p;
   const int W = p.C + 12;
   SSDK_REQUIRE(total_g == 0 || gt_dev, "ssdk_encode: gt_boxes_dev is NULL");
@@ -1245,45 +1269,4 @@ int encode_launch(ssdk_encoder* e, const void* gt_dev, int gt_f64, const int* of
             h[EV_ITERATIONS] / n, h[EV_VICTIMS] / n, h[EV_BELOW_BOUND] / n, h[EV_IMAGES]);
   }
   return SSDK_OK;
-}
-
-int scan_offsets(const int* offs, int B, int* total_g, int* max_g) {
-  SSDK_REQUIRE(offs[0] == 0 && offs[B] >= 0, "ssdk_encode: gt_offsets must start at 0 and be non-decreasing");
-  int mg = 0;
-  for (int b = 0; b < B; ++b) {
-    const int g = offs[b + 1] - offs[b];
-    SSDK_REQUIRE(g >= 0, "ssdk_encode: gt_offsets must be non-decreasing");
-    mg = g > mg ? g : mg;
-  }
-  *total_g = offs[B]; *max_g = mg;
-  return SSDK_OK;
-}
-
-}  // namespace
-
-extern "C" int ssdk_encode(ssdk_encoder* e, const float* gt_boxes_dev, const int* gt_offsets_host, int B,
-                           float* out_y_dev, int* out_match_dev, int* status_dev, void* stream_) {
-  SSDK_REQUIRE(e && gt_offsets_host && out_y_dev && B > 0, "ssdk_encode: bad argument");
-  int total_g, max_g;
-  int rc = scan_offsets(gt_offsets_host, B, &total_g, &max_g);
-  if (rc) return rc;
-  return encode_launch(e, gt_boxes_dev, 0, gt_offsets_host, nullptr, B, total_g, max_g, out_y_dev, out_match_dev, status_dev,
-                       (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_encode_f64(ssdk_encoder* e, const double* gt_boxes_dev, const int* gt_offsets_host, int B,
-                               float* out_y_dev, int* out_match_dev, int* status_dev, void* stream_) {
-  SSDK_REQUIRE(e && gt_offsets_host && out_y_dev && B > 0, "ssdk_encode_f64: bad argument");
-  int total_g, max_g;
-  int rc = scan_offsets(gt_offsets_host, B, &total_g, &max_g);
-  if (rc) return rc;
-  return encode_launch(e, gt_boxes_dev, 1, gt_offsets_host, nullptr, B, total_g, max_g, out_y_dev, out_match_dev, status_dev,
-                       (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_encode_dev(ssdk_encoder* e, const float* gt_boxes_dev, const int* gt_offsets_dev, int B, int total_g, int max_g,
-                               float* out_y_dev, int* out_match_dev, int* status_dev, void* stream_) {
-  SSDK_REQUIRE(e && gt_offsets_dev && out_y_dev && B > 0 && total_g >= 0 && max_g >= 0, "ssdk_encode_dev: bad argument");
-  return encode_launch(e, gt_boxes_dev, 0, nullptr, gt_offsets_dev, B, total_g, max_g, out_y_dev, out_match_dev, status_dev,
-                       (cudaStream_t)stream_);
 }

@@ -648,42 +648,25 @@ int launch_fused(ssdk_ctx* ctx, LossArgs& a, const LossPlan& plan, cudaStream_t 
   return launch_cooperative(ctx, ssd_loss_kernel, plan.grid, kRows, plan.smem, stream, a);
 }
 
-int loss_run(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C, int ratio, int n_neg_min, float alpha,
-             const float* upstream, float* out_loss, int* out_stats, float* out_grad, cudaStream_t stream) {
+}  // namespace
+
+extern "C" int ssdk_ssd_loss(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C, int neg_pos_ratio,
+                             int n_neg_min, float alpha, const float* upstream, float* out_loss, int* out_stats, float* out_grad,
+                             void* stream_) {
+  SSDK_REQUIRE(out_loss != nullptr || out_grad != nullptr, "ssdk_ssd_loss: out_loss and out_grad are both NULL");
   int rc = check_args(ctx, y_true, y_pred, B, P, C);
   if (rc) return rc;
+  cudaStream_t stream = (cudaStream_t)stream_;
   unsigned char* ws; int parity;
   rc = own_ws(ctx, B, P, &ws, &parity, stream);
   if (rc) return rc;
   LossArgs a; LossPlan plan;
-  rc = fill_args(ctx, a, y_true, y_pred, B, P, C, ratio, n_neg_min, alpha, ws, parity, out_grad != nullptr, plan, true);
+  rc = fill_args(ctx, a, y_true, y_pred, B, P, C, neg_pos_ratio, n_neg_min, alpha, ws, parity, out_grad != nullptr, plan, true);
   if (rc) return rc;
   a.out_loss = out_loss; a.out_stats = out_stats; a.upstream = upstream; a.out_grad = out_grad;
   rc = launch_fused(ctx, a, plan, stream);
   if (rc == SSDK_OK) ctx->loss_parity ^= 1;                           // this launch clears the other set for the next call
   return rc;
-}
-
-}  // namespace
-
-extern "C" int ssdk_ssd_loss_fwd(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C,
-                                 int neg_pos_ratio, int n_neg_min, float alpha, float* out_loss, int* out_stats, void* stream_) {
-  SSDK_REQUIRE(out_loss != nullptr, "ssd_loss: out_loss is NULL");
-  return loss_run(ctx, y_true, y_pred, B, P, C, neg_pos_ratio, n_neg_min, alpha, nullptr, out_loss, out_stats, nullptr, (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_ssd_loss_bwd(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C,
-                                 int neg_pos_ratio, int n_neg_min, float alpha, const float* upstream, float* out_grad,
-                                 void* stream_) {
-  SSDK_REQUIRE(out_grad != nullptr, "ssd_loss_bwd: out_grad is NULL");
-  return loss_run(ctx, y_true, y_pred, B, P, C, neg_pos_ratio, n_neg_min, alpha, upstream, nullptr, nullptr, out_grad, (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_ssd_loss_fwd_bwd(ssdk_ctx* ctx, const float* y_true, const float* y_pred, int B, int P, int C,
-                                     int neg_pos_ratio, int n_neg_min, float alpha, const float* upstream, float* out_loss,
-                                     int* out_stats, float* out_grad, void* stream_) {
-  SSDK_REQUIRE(out_loss != nullptr && out_grad != nullptr, "ssdk_ssd_loss_fwd_bwd: out_loss / out_grad is NULL");
-  return loss_run(ctx, y_true, y_pred, B, P, C, neg_pos_ratio, n_neg_min, alpha, upstream, out_loss, out_stats, out_grad, (cudaStream_t)stream_);
 }
 
 extern "C" int ssdk_ssd_loss_ws_layout(int B, int P, ssdk_loss_ws_layout* out) {

@@ -698,8 +698,6 @@ extern "C" int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int whi
   return SSDK_OK;
 }
 
-extern "C" float* ssdk_trainer_grad_buffer(ssdk_trainer* t) { return t ? t->grad : nullptr; }
-
 extern "C" int ssdk_trainer_grad_shape(const ssdk_trainer* t, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad) {
   SSDK_REQUIRE(t && out_hp && out_wp && out_cs && out_pad && layer >= 0 && layer < (int)t->tl.size(), "ssdk_trainer_grad_shape: bad argument");
   const TLayer& T = t->tl[layer];
@@ -769,11 +767,9 @@ int do_transpose(ssdk_trainer* t, const __nv_bfloat16* hi, const __nv_bfloat16* 
                 hi, lo, src_ld, src_rows, mp, row_off, Kv, C, dhi, dlo, ldT);
 }
 
-}  // namespace
-
-namespace {
 int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaStream_t s);
-}
+
+}  // namespace
 
 // Loss (optional) and d loss / d y_pred from one launch of the fused loss kernel; clears the gradient buffer.
 extern "C" int ssdk_train_backward_begin(ssdk_trainer* t, const float* y_true, const float* y_pred, int neg_pos_ratio, int n_neg_min,
@@ -781,11 +777,8 @@ extern "C" int ssdk_train_backward_begin(ssdk_trainer* t, const float* y_true, c
   SSDK_REQUIRE(t && y_true && y_pred, "ssdk_train_backward_begin: NULL argument");
   ssdk_model* m = t->m;
   ssdk_ctx* ctx = m->ctx;
-  int rc;
   SSDK_CHECK_CUDA(cudaMemsetAsync(t->grad, 0, (size_t)t->n_params * sizeof(float), (cudaStream_t)stream_));
-  if (out_loss) rc = ssdk_ssd_loss_fwd_bwd(ctx, y_true, y_pred, m->B, m->P, m->Ctot, neg_pos_ratio, n_neg_min, alpha, nullptr, out_loss, nullptr, t->dypred, stream_);
-  else rc = ssdk_ssd_loss_bwd(ctx, y_true, y_pred, m->B, m->P, m->Ctot, neg_pos_ratio, n_neg_min, alpha, nullptr, t->dypred, stream_);
-  return rc;
+  return ssdk_ssd_loss(ctx, y_true, y_pred, m->B, m->P, m->Ctot, neg_pos_ratio, n_neg_min, alpha, nullptr, out_loss, nullptr, t->dypred, stream_);
 }
 
 // The backward pass of layers hi, hi-1, ..., lo (graph indices; a full pass is n_layers-1 .. 0 in one or several calls, top
@@ -799,18 +792,6 @@ extern "C" int ssdk_train_backward_layers(ssdk_trainer* t, const float* dypred_d
   SSDK_REQUIRE(hi < n && lo >= 0 && lo <= hi, "ssdk_train_backward_layers: bad layer range [%d, %d] of %d layers", lo, hi, n);
   if (dypred_dev && hi == n - 1) SSDK_CHECK_CUDA(cudaMemsetAsync(t->grad, 0, (size_t)t->n_params * sizeof(float), (cudaStream_t)stream_));
   return backward_layers(t, dypred_dev ? dypred_dev : t->dypred, hi, lo, (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_train_backward(ssdk_trainer* t, const float* y_true, const float* y_pred, int neg_pos_ratio, int n_neg_min,
-                                   float alpha, float* out_loss, void* stream_) {
-  int rc = ssdk_train_backward_begin(t, y_true, y_pred, neg_pos_ratio, n_neg_min, alpha, out_loss, stream_);
-  if (rc) return rc;
-  return backward_layers(t, t->dypred, (int)t->m->layers.size() - 1, 0, (cudaStream_t)stream_);
-}
-
-extern "C" int ssdk_train_backward_dy(ssdk_trainer* t, const float* dypred_dev, void* stream_) {
-  SSDK_REQUIRE(t && dypred_dev, "ssdk_train_backward_dy: NULL argument");
-  return ssdk_train_backward_layers(t, dypred_dev, (int)t->m->layers.size() - 1, 0, stream_);
 }
 
 namespace {

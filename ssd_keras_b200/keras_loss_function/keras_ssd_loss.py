@@ -1,7 +1,7 @@
 """``SSDLoss`` on H100 (reference ``keras_loss_function/keras_ssd_loss.py:22-211``), computed by
 ``csrc/loss.cu``.  ``compute_loss`` takes / returns torch CUDA tensors (NumPy arrays are accepted and
 copied) and is differentiable with respect to ``y_pred`` through a ``torch.autograd.Function`` whose
-backward is the hand-written ``ssdk_ssd_loss_bwd`` kernel.
+backward is the same hand-written kernel (``ssdk_ssd_loss`` with a gradient output).
 """
 import numpy as np
 
@@ -26,9 +26,9 @@ def _make_fn():
             B, P, W = y_pred.shape
             out = torch.empty((B,), dtype=torch.float32, device=y_pred.device)
             stats = torch.zeros((4,), dtype=torch.int32, device=y_pred.device)
-            _ffi.check(_ffi.lib().ssdk_ssd_loss_fwd(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
-                                                    W - 12, int(neg_pos_ratio), int(n_neg_min), float(alpha), _ffi.dptr(out),
-                                                    _ffi.dptr(stats), _ffi.stream_ptr()))
+            _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
+                                                W - 12, int(neg_pos_ratio), int(n_neg_min), float(alpha), _ffi.dptr(None),
+                                                _ffi.dptr(out), _ffi.dptr(stats), _ffi.dptr(None), _ffi.stream_ptr()))
             ctx.save_for_backward(y_true, y_pred)
             ctx.cfg = (int(neg_pos_ratio), int(n_neg_min), float(alpha))
             ctx.stats = stats
@@ -41,8 +41,9 @@ def _make_fn():
             r, m, a = ctx.cfg
             g = torch.empty_like(y_pred)
             up = grad_out.to(dtype=torch.float32).contiguous()
-            _ffi.check(_ffi.lib().ssdk_ssd_loss_bwd(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
-                                                    W - 12, r, m, a, _ffi.dptr(up), _ffi.dptr(g), _ffi.stream_ptr()))
+            _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
+                                                W - 12, r, m, a, _ffi.dptr(up), _ffi.dptr(None), _ffi.dptr(None), _ffi.dptr(g),
+                                                _ffi.stream_ptr()))
             return None, g, None, None, None
 
     return _SSDLossFn
@@ -73,7 +74,7 @@ class SSDLoss:
 
     def smooth_L1_loss(self, y_true, y_pred):
         """Reference :53-75, (B,P,4) x2 -> (B,P) float32 CUDA tensor.  Stand-alone helper (a few tensor operations on the
-        device); ``compute_loss`` computes the same quantity inside ``ssdk_ssd_loss_fwd``."""
+        device); ``compute_loss`` computes the same quantity inside ``ssdk_ssd_loss``."""
         return self._smooth_l1_t(_as_cuda(y_true), _as_cuda(y_pred))
 
     def log_loss(self, y_true, y_pred):
@@ -100,7 +101,7 @@ class SSDLoss:
         B, P, W = yp.shape
         out = torch.empty((B,), dtype=torch.float32, device=yp.device)
         stats = torch.zeros((4,), dtype=torch.int32, device=yp.device)
-        _ffi.check(_ffi.lib().ssdk_ssd_loss_fwd(_ffi.context(yp.device.index), _ffi.dptr(yt), _ffi.dptr(yp), B, P, W - 12,
-                                                int(self.neg_pos_ratio), int(self.n_neg_min), float(self.alpha), _ffi.dptr(out),
-                                                _ffi.dptr(stats), _ffi.stream_ptr()))
+        _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(yp.device.index), _ffi.dptr(yt), _ffi.dptr(yp), B, P, W - 12,
+                                            int(self.neg_pos_ratio), int(self.n_neg_min), float(self.alpha), _ffi.dptr(None),
+                                            _ffi.dptr(out), _ffi.dptr(stats), _ffi.dptr(None), _ffi.stream_ptr()))
         return out, stats

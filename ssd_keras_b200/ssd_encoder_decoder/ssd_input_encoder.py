@@ -210,22 +210,23 @@ class SSDInputEncoder:
         if self._status is None:
             self._status = torch.zeros((1,), dtype=torch.int32, device=dev)
         f64 = gt_boxes_dev is not None and gt_boxes_dev.dtype == torch.float64
-        fn = _ffi.lib().ssdk_encode_f64 if f64 else _ffi.lib().ssdk_encode
-        _ffi.check(fn(self._encoder(), _ffi.dptr(gt_boxes_dev), _ffi.np_ptr(offs, C.c_int), B,
-                      _ffi.dptr(y), _ffi.dptr(match), _ffi.dptr(self._status), _ffi.stream_ptr()))
+        _ffi.check(_ffi.lib().ssdk_encode(self._encoder(), _ffi.dptr(gt_boxes_dev), int(f64), _ffi.np_ptr(offs, C.c_int), None,
+                                          B, 0, 0, _ffi.dptr(y), _ffi.dptr(match), _ffi.dptr(self._status), _ffi.stream_ptr()))
         return (y, match) if return_matches else y
 
     def encode_device_offsets(self, gt_boxes_dev, gt_offsets_dev, total_g, max_g, out=None):
         """Like ``encode_device`` for a batch that was assembled on the device (``data_generator.assemble_batch_device``):
-        the row offsets are an int32 CUDA tensor (B+1,), nothing is read from the host."""
+        the row offsets are an int32 CUDA tensor (B+1,), nothing is read from the host.  The rows must be float32."""
         import torch
         B = gt_offsets_dev.shape[0] - 1
         P, W = self.anchors.shape[0], self.n_classes + 12
         y = out if out is not None else torch.empty((B, P, W), dtype=torch.float32, device=gt_offsets_dev.device)
         if self._status is None:
             self._status = torch.zeros((1,), dtype=torch.int32, device=gt_offsets_dev.device)
-        _ffi.check(_ffi.lib().ssdk_encode_dev(self._encoder(), _ffi.dptr(gt_boxes_dev), _ffi.dptr(gt_offsets_dev), B, int(total_g),
-                                              int(max_g), _ffi.dptr(y), _ffi.dptr(None), _ffi.dptr(self._status), _ffi.stream_ptr()))
+        f64 = gt_boxes_dev is not None and gt_boxes_dev.dtype == torch.float64
+        _ffi.check(_ffi.lib().ssdk_encode(self._encoder(), _ffi.dptr(gt_boxes_dev), int(f64), None, _ffi.dptr(gt_offsets_dev), B,
+                                          int(total_g), int(max_g), _ffi.dptr(y), _ffi.dptr(None), _ffi.dptr(self._status),
+                                          _ffi.stream_ptr()))
         return y
 
     def __call__(self, ground_truth_labels, diagnostics=False):

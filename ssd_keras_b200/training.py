@@ -1,7 +1,8 @@
 """Training step on H100: what ``model.compile(optimizer=SGD(lr, momentum), loss=SSDLoss().compute_loss)`` +
-``train_on_batch`` do in the reference (``ssd300_training.ipynb:169-173``), through ``ssdk_train_backward`` /
-``ssdk_train_apply`` (``csrc/train.cu``).  Data-parallel: every rank runs the same step on its shard and the flat
-gradient buffer is summed with ONE NCCL all-reduce before the update (replica-local loss, SURVEY.md section 8e(i)).
+``train_on_batch`` do in the reference (``ssd300_training.ipynb:169-173``), through ``ssdk_train_backward_begin`` /
+``ssdk_train_backward_layers`` / ``ssdk_train_apply`` (``csrc/train.cu``).  Data-parallel: every rank runs the same step on
+its shard and the flat gradient buffer is summed with ONE NCCL all-reduce before the update (replica-local loss, SURVEY.md
+section 8e(i)).
 """
 import ctypes as C
 import weakref

@@ -20,13 +20,59 @@ def lib():
     return _ffi.lib()
 
 
-def test_library_exports_every_declared_symbol(lib):
-    header = open(os.path.join(ROOT, 'include', 'ssdk.h')).read()
-    names = sorted(set(re.findall(r'\b(ssdk_[a-z0-9_]+)\s*\(', header)))
-    assert len(names) >= 25
-    for n in names:
-        assert hasattr(lib, n), 'libssdk.so does not export ' + n
+HEADER_KINDS = {'int': 'i32', 'long long': 'i64', 'int64_t': 'i64', 'float': 'f32', 'double': 'f64', 'void': 'void'}
+
+
+def _header():
+    """include/ssdk.h without its comments."""
+    src = open(os.path.join(ROOT, 'include', 'ssdk.h')).read()
+    return re.sub(r'//[^\n]*', '', re.sub(r'/\*.*?\*/', ' ', src, flags=re.S))
+
+
+def _declarators(decl):
+    """'const int* a, b[4]' -> [(name, kind, array length or None)]; a pointer is 'ptr', a scalar its HEADER_KINDS kind."""
+    first, *more = re.sub(r'\bconst\b', ' ', decl).split(',')
+    base, d0 = re.fullmatch(r'\s*([\w\s]*?\w)((?:\s|\*)*\w*\s*(?:\[\d+\])?)\s*', first).groups()
+    out = []
+    for d in [d0] + more:
+        stars, name, n = re.fullmatch(r'\s*(\**)\s*(\w*)\s*(?:\[(\d+)\])?\s*', d).groups()
+        out.append((name, 'ptr' if stars else HEADER_KINDS[base], int(n) if n else None))
+    return out
+
+
+def _ctypes_kind(t):
+    if t is None:
+        return 'void'
+    if issubclass(t, (ctypes._Pointer, ctypes.c_void_p, ctypes.c_char_p)):
+        return 'ptr'
+    return {'f': 'f32', 'd': 'f64'}.get(t._type_, 'i%d' % (8 * ctypes.sizeof(t)))
+
+
+def test_binding_table_matches_the_header(lib):
+    """_ffi.SIGNATURES declares exactly the functions of ssdk.h, each exported, with the header's arity and the kind (pointer,
+    32- / 64-bit int, float, double) of every argument and return value; each ctypes Structure of _ffi (named after its C
+    struct: BoxOp mirrors ssdk_box_op) has the header's fields in order, with the same kinds and array lengths."""
+    from ssd_keras_b200 import _ffi
+    header = _header()
+    decls = {name: (ret, params) for ret, name, params in
+             re.findall(r'((?:const\s+)?\w+\s*\**)\s*\b(ssdk_\w+)\s*\(([^()]*)\)\s*;', header)}
+    assert sorted(decls) == sorted(_ffi.SIGNATURES)
+    for name, (ret, params) in decls.items():
+        assert hasattr(lib, name), 'libssdk.so does not export ' + name
+        restype, argtypes = _ffi.SIGNATURES[name]
+        want = [k for p in params.split(',') if p.strip() != 'void' for _, k, _ in _declarators(p)]
+        assert (_declarators(ret + ' r')[0][1], want) == (_ctypes_kind(restype), [_ctypes_kind(t) for t in argtypes]), name
     assert lib.ssdk_version() == 100
+    structs = {name: body for body, name in re.findall(r'typedef\s+struct\s*\w*\s*\{([^{}]*)\}\s*(\w+)\s*;', header)}
+    mirrors = [c for c in vars(_ffi).values() if isinstance(c, type) and issubclass(c, ctypes.Structure)]
+    assert mirrors
+    for cls in mirrors:
+        c_name = 'ssdk_' + re.sub(r'(?<!^)([A-Z])', r'_\1', cls.__name__).lower()
+        assert c_name in structs, (cls.__name__, c_name)
+        want = [f for decl in structs[c_name].split(';') if decl.strip() for f in _declarators(decl)]
+        have = [(n, _ctypes_kind(t._type_ if issubclass(t, ctypes.Array) else t), t._length_ if issubclass(t, ctypes.Array) else None)
+                for n, t in cls._fields_]
+        assert have == want, cls.__name__
 
 
 def test_no_cpu_fallback(lib):

@@ -151,7 +151,7 @@ def test_encode_integer_pixel_labels_ties(configs):
 
 
 def test_encode_float64_labels(configs):
-    """Labels that float32 cannot hold: the reference computes on float64 copies (:330) and so does ssdk_encode_f64."""
+    """Labels that float32 cannot hold: the reference computes on float64 copies (:330) and so does ssdk_encode with gt_f64 = 1."""
     rng = np.random.default_rng(3)
     gts = []
     for _ in range(3):
@@ -185,6 +185,8 @@ def test_encode_large_batch_and_device_offsets(configs):
     gd = torch.from_numpy(np.concatenate(gts)).cuda()
     yd = enc.encode_device_offsets(gd, torch.from_numpy(offs).cuda(), int(offs[-1]), 7).cpu().numpy()
     np.testing.assert_array_equal(yd, enc.encode_device(gd, offs).cpu().numpy())
+    with pytest.raises(ValueError, match='float64 rows need host offsets'):
+        enc.encode_device_offsets(gd.double(), torch.from_numpy(offs).cuda(), int(offs[-1]), 7)
     out = torch.empty((5, enc.anchors.shape[0], enc.n_classes + 12), dtype=torch.float32, device='cuda')
     assert enc.encode_device(gd, offs, out=out) is out
     np.testing.assert_array_equal(out.cpu().numpy(), yd)
@@ -481,8 +483,9 @@ def test_loss_global_batch_exact_phases(configs, shards):
     np.testing.assert_allclose(loss, ssd_loss(yt0, yp, n_neg_min=10), rtol=1e-5)
 
 
-def test_loss_forward_backward_one_launch(configs):
-    """ssdk_ssd_loss_fwd_bwd (what the training step calls): same loss and gradient as the separate entry points."""
+def test_ssd_loss_with_loss_and_gradient_is_one_launch(configs):
+    """ssdk_ssd_loss with the loss and the gradient (what the training step calls): one launch, the loss and gradient of the
+    reference."""
     import ctypes as C
     import torch
     from ssd_keras_b200 import _ffi
@@ -491,8 +494,8 @@ def test_loss_forward_backward_one_launch(configs):
     yt, yp = torch.from_numpy(y_true).cuda(), torch.from_numpy(y_pred).cuda()
     loss = torch.empty((4,), dtype=torch.float32, device='cuda'); grad = torch.empty_like(yp)
     n0 = _ffi.launch_count()
-    _ffi.check(_ffi.lib().ssdk_ssd_loss_fwd_bwd(_ffi.context(), _ffi.dptr(yt), _ffi.dptr(yp), 4, yp.shape[1], 21, 3, 0, 1.0, _ffi.dptr(None),
-                                                _ffi.dptr(loss), _ffi.dptr(None), _ffi.dptr(grad), _ffi.stream_ptr()))
+    _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(), _ffi.dptr(yt), _ffi.dptr(yp), 4, yp.shape[1], 21, 3, 0, 1.0, _ffi.dptr(None),
+                                        _ffi.dptr(loss), _ffi.dptr(None), _ffi.dptr(grad), _ffi.stream_ptr()))
     assert _ffi.launch_count() - n0 == 1
     np.testing.assert_allclose(loss.cpu().numpy(), ssd_loss(y_true, y_pred), rtol=1e-5)
     np.testing.assert_allclose(grad.cpu().numpy(), ssd_loss_grad(y_true, y_pred), rtol=1e-4, atol=1e-7)

@@ -102,7 +102,7 @@ def test_encode_path_exact(name, env):
 
 
 def test_encode_call_api_exact(env):
-    """SSDInputEncoder.__call__ (float64 labels, ssdk_encode_f64) on the threshold and thr_adj = 0 cases."""
+    """SSDInputEncoder.__call__ (float64 labels, ssdk_encode with gt_f64 = 1) on the threshold and thr_adj = 0 cases."""
     for name in ('thr_at_centroids', 'thr_below_minmax', 'thr0_neg0', 'thr0_negative', 'tozero', 'c1_other_tile'):
         c = ec.BY_NAME[name]
         gts = ec.inputs(name)

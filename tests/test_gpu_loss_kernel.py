@@ -1,8 +1,9 @@
 """GPU tests of the SSD loss kernel (ssd_loss_kernel, ssd_loss_phase_kernel in csrc/loss.cu) against the operand-exact float64
 reference of oracle/opexact.py (section 11), launch by launch:
-- every case asserts its launch plan (ssdk_ssd_loss_plan), runs fwd, bwd and fwd_bwd, reads the per-box losses back after each
-  (ssdk_ssd_loss_read_box_losses; they must be identical), holds n_pos / nnz / k / want exactly and the per-box losses, the loss
-  and the gradient to their bounds, and requires every listed perturbation of the reference to fail;
+- every case asserts its launch plan (ssdk_ssd_loss_plan), runs ssdk_ssd_loss with the loss outputs (fwd), the gradient (bwd)
+  and both (fwd_bwd), reads the per-box losses back after each (ssdk_ssd_loss_read_box_losses; they must be identical), holds
+  n_pos / nnz / k / want exactly and the per-box losses, the loss and the gradient to their bounds, and requires every listed
+  perturbation of the reference to fail;
 - the hard-negative mask is checked through the gradient: a kept negative has w_cls = scale, an unkept one 0, a kept positive
   2 scale;
 - a sweep of k over every rank of a small batch, refused calls between exact ones, and the phase-wise (multi-GPU) launches with
@@ -227,13 +228,8 @@ def run_loss(mode, yt_d, yp_d, C, ratio, n_neg_min, alpha, up_d=None, grad_offse
     loss = torch.full((B,), np.nan, dtype=torch.float32, device='cuda') if mode != 'bwd' else None
     stats = torch.full((4,), -7, dtype=torch.int32, device='cuda') if mode != 'bwd' else None
     grad = _dev(np.full(yp_d.shape, np.nan, np.float32), grad_offset) if mode != 'fwd' else None
-    if mode == 'fwd':
-        rc = lib.ssdk_ssd_loss_fwd(ctx, d(yt_d), d(yp_d), B, P, C, ratio, n_neg_min, alpha, d(loss), d(stats), st)
-    elif mode == 'bwd':
-        rc = lib.ssdk_ssd_loss_bwd(ctx, d(yt_d), d(yp_d), B, P, C, ratio, n_neg_min, alpha, d(up_d), d(grad), st)
-    else:
-        rc = lib.ssdk_ssd_loss_fwd_bwd(ctx, d(yt_d), d(yp_d), B, P, C, ratio, n_neg_min, alpha, d(up_d), d(loss), d(stats), d(grad), st)
-    _ffi.check(rc)
+    up = up_d if mode != 'fwd' else None
+    _ffi.check(lib.ssdk_ssd_loss(ctx, d(yt_d), d(yp_d), B, P, C, ratio, n_neg_min, alpha, d(up), d(loss), d(stats), d(grad), st))
     cls, negl = _ffi.loss_box_losses(B, P)
     torch.cuda.synchronize()
     f = lambda t: None if t is None else t.cpu().numpy()
@@ -280,7 +276,7 @@ def judge(name, yt, yp, outs, ratio, n_neg_min, alpha, up, perturb, log=True, **
 # tests
 # ------------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize('c', LOSS_CASES, ids=[c['name'] for c in LOSS_CASES])
-def test_loss_case(c):
+def test_ssd_loss_case(c):
     from ssd_keras_b200 import _ffi
     yt, yp, up, n_neg_min = make_case(c)
     B, P, C = c['B'], c['P'], c['C']
@@ -305,7 +301,7 @@ def _sm_count():
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
-def test_largest_classes_and_one_more():
+def test_ssd_loss_largest_classes_and_one_more():
     """C_MAX_GRAD / C_MAX_FWD launch; one class more is refused with ValueError before any launch, by the plan and by the call."""
     import torch
     from ssd_keras_b200 import _ffi
@@ -329,7 +325,7 @@ def test_largest_classes_and_one_more():
         torch.cuda.synchronize()
 
 
-def test_k_sweep_every_rank():
+def test_ssd_loss_k_sweep_every_rank():
     """No positives: k = min(n_neg_min, nnz).  n_neg_min from 0 to nnz + 1 puts the threshold at every rank of the batch, so at
     every coarse and fine bin boundary it has; then neg_pos_ratio from 0 to 12 with positives."""
     rng = np.random.default_rng(SWEEP['seed'])
@@ -357,9 +353,10 @@ def test_k_sweep_every_rank():
         judge('sweep_ratio', yt, yp, [out], ratio, 0, 1.0, None, ('drop_last', 'add_next') if ratio else ())
 
 
-def test_refused_call_leaves_the_next_call_exact():
-    """A bwd refused at the same (B, P) (too many classes for the gradient's shared memory) between two identical calls; three
-    consecutive same-shape calls on different data; two shapes alternating.  Every call must be exact."""
+def test_refused_ssd_loss_call_leaves_the_next_call_exact():
+    """A bwd refused at the same (B, P) (too many classes for the gradient's shared memory) between two identical calls; a call
+    that asks for neither the loss nor the gradient, refused; three consecutive same-shape calls on different data; two shapes
+    alternating.  Every call must be exact."""
     import torch
     from ssd_keras_b200 import _ffi
     B, P = 2, 300
@@ -381,6 +378,11 @@ def test_refused_call_leaves_the_next_call_exact():
         assert _ffi.launch_count() == n0
         again = exact(data[0])
         assert np.array_equal(_bits(first[0]), _bits(again[0])) and np.array_equal(first[1], again[1])
+    n0 = _ffi.launch_count()
+    with pytest.raises(ValueError, match='out_loss and out_grad are both NULL'):
+        _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(), _ffi.dptr(yt_big), _ffi.dptr(yp_big), B, P, big, 3, 0, 1.0, None, None,
+                                            None, None, _ffi.stream_ptr()))
+    assert _ffi.launch_count() == n0
     for d in data:
         exact(d, 'fwd_bwd')
     for _ in range(2):
@@ -427,7 +429,7 @@ def _phase_run(yt, yp, shards, ratio, n_neg_min, alpha):
 
 @pytest.mark.parametrize('shards', [1, 2, 4])
 @pytest.mark.parametrize('c', PHASE_CASES, ids=[c['name'] for c in PHASE_CASES])
-def test_phases_match_the_fused_launch_bit_for_bit(c, shards):
+def test_phases_match_ssd_loss_bit_for_bit(c, shards):
     import torch
     yt, yp, _, n_neg_min = make_case(c)
     B, P, C = c['B'], c['P'], c['C']

@@ -31,11 +31,7 @@ def preview(layers, R, sms=148):
     inp = (C.c_int * n)(*[-1 if l[3] is None else names.index(l[3]) for l in layers])
     side = (C.c_ubyte * n)()
     frm, cap = C.c_int(), C.c_int()
-    lib = _ffi.lib()
-    lib.ssdk_schedule_preview.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int,
-                                          C.POINTER(C.c_ubyte), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    lib.ssdk_schedule_preview.restype = C.c_int
-    _ffi.check(lib.ssdk_schedule_preview(n, kind, grid, inp, R, sms, side, C.byref(frm), C.byref(cap)))
+    _ffi.check(_ffi.lib().ssdk_schedule_preview(n, kind, grid, inp, R, sms, side, C.byref(frm), C.byref(cap)))
     return {names[i] for i in range(n) if side[i]}, (names[frm.value] if frm.value >= 0 else None), cap.value
 
 
