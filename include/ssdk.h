@@ -279,6 +279,81 @@ int ssdk_eval_collect(ssdk_ctx* ctx, const float* rows_dev, int B, int max_out, 
                       int* out_class_dev, double* out_conf_dev, double* out_box_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * MS COCO evaluation.  Replaces COCOeval.evaluate / accumulate of pycocotools for iouType 'bbox' (cocoapi
+ * PythonAPI/pycocotools/cocoeval.py evaluateImg and accumulate, the IoU of common/maskApi.c bbIou), bit for bit.  All arrays
+ * are device arrays.  The caller segments the ground truths and detections by (image position, category position): a
+ * segment is a pair that has either; its ground truths are in annotation-file order, its detections in -score order (stable,
+ * -0.0 equal to 0.0, NaN last), cut to the largest maxDet.
+ *
+ * ssdk_cocoeval_match: evaluateImg for every segment and area range, one launch.
+ *   boxes        [x, y, w, h] float64; the ground truth's IoU uses its box area, the area-range test its gt_area ('area')
+ *   gt_flags     bit 0: crowd ('iscrowd', which also makes it ignored), bit 1: its id is 0 (then a match reads as unmatched)
+ *   det_area     w * h in float64 (loadRes), for the test of unmatched detections against the range
+ *   area_rng     [n_area][2] inclusive bounds; iou_thrs [n_thr], each capped at 1 - 1e-10
+ *   gt_matched   uint8 [n_area * n_thr * n_gt] scratch, zeroed by the caller
+ *   det_flags    uint8 [n_area * n_thr][n_det], row area * n_thr + thr: bit 0 dtm != 0, bit 1 dtIgnore
+ *   det_match    int32, same layout: the matched ground truth's index, or -1
+ *   seg_npig     int32 [n_seg][n_area]: non-ignored ground truths of the segment
+ *   npig         int32 [categories][n_area], zeroed by the caller: the same summed over the category's segments
+ * Greedy matching as evaluateImg: detections in order, ground truths with the ignored ones last; a matched non-crowd box is
+ * skipped, an ignored one is not taken after a non-ignored match, an IoU below the best so far is skipped (so the last of
+ * equal IoUs wins).  The IoU is bbIou's float64 expression with C's fmin / fmax and no contraction.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct {
+  int n_seg, n_gt, n_det, n_area, n_thr;
+  const int* seg_gt;             /* [n_seg + 1] ground-truth range of each segment */
+  const int* seg_det;            /* [n_seg + 1] detection range of each segment */
+  const int* seg_cat;            /* [n_seg] category position */
+  const double* gt_box;          /* [n_gt * 4] */
+  const double* gt_area;         /* [n_gt] */
+  const unsigned char* gt_flags; /* [n_gt] */
+  const double* det_box;         /* [n_det * 4] */
+  const double* det_area;        /* [n_det] */
+  const double* area_rng;        /* [n_area * 2] */
+  const double* iou_thrs;        /* [n_thr] */
+  unsigned char* gt_matched;
+  unsigned char* det_flags;
+  int* det_match;
+  int* seg_npig;
+  int* npig;
+} ssdk_coco_match;
+
+/* ssdk_cocoeval_accumulate: accumulate's precision [T, R, out_k, out_a, out_m], scores (same) and recall [T, out_k, out_a, out_m],
+ * float64, filled with -1 by the caller; one launch, one CTA per (threshold, selected category, area, maxDet).
+ *   ord_det / ord_rank / ord_score   every detection of the match, category by category (cat_off [categories + 1]) in
+ *                                    accumulate's order: score desc (stable, -0.0 equal to 0.0, NaN last), image position,
+ *                                    rank in its segment; ord_det is its index in the match's arrays
+ *   det_flags / npig                 the match's outputs (n_thr, n_area, n_det as there)
+ *   rec_thrs [n_rec]                 as given; rec_sorted the same sorted ascending (NaN last), rec_perm the original positions
+ *   sel_cat / sel_area / sel_max_det accumulate's k_list / a_list / m_list: the match's category and area positions and the
+ *                                    maxDet values behind output positions 0 .. n_k / n_a / n_m - 1
+ * Per row, with npig non-ignored ground truths (npig 0: the row keeps -1): the detections of rank < maxDet, tp / fp cumulative
+ * counts over the non-ignored ones, rc = tp / npig, pr = tp / (fp + tp + 2^-52) made non-increasing from the right, and
+ * precision / scores at searchsorted(rc, recThrs, 'left'), zero from the first threshold past the end; recall rc[-1], 0 without
+ * detections. */
+typedef struct {
+  int n_thr, n_area, n_det, n_rec, n_k, n_a, n_m, out_k, out_a, out_m;
+  const int* cat_off;
+  const int* ord_det;
+  const int* ord_rank;
+  const double* ord_score;
+  const unsigned char* det_flags;
+  const int* npig;
+  const double* rec_thrs;
+  const double* rec_sorted;
+  const int* rec_perm;
+  const int* sel_cat;
+  const int* sel_area;
+  const int* sel_max_det;
+  double* precision;
+  double* scores;
+  double* recall;
+} ssdk_coco_accumulate;
+
+int ssdk_cocoeval_match(ssdk_ctx* ctx, const ssdk_coco_match* args, void* stream);
+int ssdk_cocoeval_accumulate(ssdk_ctx* ctx, const ssdk_coco_accumulate* args, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Decoders.
  *   mode PER_CLASS + layer_semantics=1: DecodeDetections.call   (keras_layers/keras_layer_DecodeDetections.py:109-265)
  *   mode FAST      + layer_semantics=1: DecodeDetectionsFast.call (keras_layers/keras_layer_DecodeDetectionsFast.py:111-248)

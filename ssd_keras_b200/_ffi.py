@@ -141,6 +141,18 @@ def trainer_layer_plan(handle, layer):
     return out
 
 
+class CocoMatch(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ('n_seg', 'n_gt', 'n_det', 'n_area', 'n_thr')] + \
+               [(n, C.c_void_p) for n in ('seg_gt', 'seg_det', 'seg_cat', 'gt_box', 'gt_area', 'gt_flags', 'det_box', 'det_area',
+                                          'area_rng', 'iou_thrs', 'gt_matched', 'det_flags', 'det_match', 'seg_npig', 'npig')]
+
+
+class CocoAccumulate(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ('n_thr', 'n_area', 'n_det', 'n_rec', 'n_k', 'n_a', 'n_m', 'out_k', 'out_a', 'out_m')] + \
+               [(n, C.c_void_p) for n in ('cat_off', 'ord_det', 'ord_rank', 'ord_score', 'det_flags', 'npig', 'rec_thrs', 'rec_sorted',
+                                          'rec_perm', 'sel_cat', 'sel_area', 'sel_max_det', 'precision', 'scores', 'recall')]
+
+
 OP_INPUT, OP_CONV, OP_MAXPOOL, OP_L2NORM, OP_HEAD, OP_TENSOR = range(6)
 ACT_NONE, ACT_RELU, ACT_ELU = range(3)
 
@@ -164,6 +176,8 @@ SIGNATURES = {
     'ssdk_eval_match': (_i, [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _d, _i, _p, _p, _p]),
     'ssdk_eval_cumsum': (_i, [_p, _p, _p, _p, _i, _p, _p, _p]),
     'ssdk_eval_collect': (_i, [_p, _p, _i, _i, _p, _p, c_int_p, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p]),
+    'ssdk_cocoeval_match': (_i, [_p, C.POINTER(CocoMatch), _p]),
+    'ssdk_cocoeval_accumulate': (_i, [_p, C.POINTER(CocoAccumulate), _p]),
     'ssdk_decode': (_i, [_p, C.POINTER(DecodeCfg), _p, _i, _p, _p, _p, _p]),
     'ssdk_nms': (_i, [_p, _p, _p, _i, _i, _d, _d, _i, _i, _p, _p, _p, _p]),
     'ssdk_ssd_loss': (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _f, _p, _p, _p, _p, _p]),

@@ -27,6 +27,7 @@ SOURCES = {
     'loss.cu': ['--fmad=false'],
     'batch.cu': ['--fmad=false'],
     'evaluate.cu': ['--fmad=false'],
+    'cocoeval.cu': ['--fmad=false'],
     'conv.cu': [],
     'model.cu': [],
     'train.cu': [],
