@@ -30,6 +30,21 @@ void fused_master(const ssdk_layer_desc& d, int cin, int cout, int Ctot, std::ve
 
 struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
 
+// The forward kernel of a convolution or head: every reader of the plan switches on it, and pass 2 sizes the borders from it.
+ssdk_plan_kernel conv_kernel(const ssdk_layer_desc& d, int cin, int cout, bool training) {
+  const int taps = d.kh * d.kw;
+  // the image-facing layer: 1 ... 4 input channels (one stored 8-channel group), an fp32 [K][Cout] kernel within 96 KB
+  const bool direct = d.op != SSDK_OP_HEAD && cin >= 1 && cin <= 4 && d.stride == 1 && cout % 16 == 0 && (size_t)taps * cin * cout * 4 <= 96 * 1024;
+  if (direct) {
+    // inference plans run it on the tensor cores with a gathered A tile; training plans keep the fp32 direct kernel, whose
+    // weights are the optimizer's master copy
+    if (!training && first_tc_supported(taps, cin, cout) && d.dilation >= 1) return SSDK_PLAN_FIRST_TC;
+    return SSDK_PLAN_DIRECT;
+  }
+  if (d.stride != 1 || cin < 8) return SSDK_PLAN_IM2COL_GEMM;
+  return SSDK_PLAN_GEMM;
+}
+
 int build_conv(ssdk_model* m, int li) {
   LayerPlan& L = m->layers[li];
   const ssdk_layer_desc& d = L.d;
@@ -37,11 +52,10 @@ int build_conv(ssdk_model* m, int li) {
   const ActBuf& ia = in.out;
   const int cin = in.C;
   const bool head = d.op == SSDK_OP_HEAD;
-  const int cout = head ? d.n_boxes * (m->Ctot + 4) : d.cout;
+  const int cout = L.C;
   const int taps = d.kh * d.kw;
   SSDK_REQUIRE(taps <= kMaxTaps, "conv kernel %dx%d is larger than the supported %d taps", d.kh, d.kw, kMaxTaps);
   SSDK_REQUIRE(head || cout % 8 == 0, "conv output channels must be a multiple of 8 (got %d)", cout);
-  L.direct = !head && cin <= 4 && d.stride == 1 && cout % 16 == 0 && (size_t)taps * cin * cout * 4 <= 96 * 1024 && ia.Cs == 8;
   std::vector<float> master, bias;
   fused_master(d, cin, cout, m->Ctot, master, bias);
   // conv + BatchNormalization in a training plan: the conv writes its raw output z, batch statistics follow (bn.cu)
@@ -58,7 +72,7 @@ int build_conv(ssdk_model* m, int li) {
     L.bn_eps = d.bn_eps > 0.f ? d.bn_eps : 1e-3f;
     L.bn_momentum = (d.bn_momentum > 0.f && d.bn_momentum < 1.f) ? d.bn_momentum : 0.99f;
   }
-  if (L.direct) {
+  if (L.kernel == SSDK_PLAN_DIRECT || L.kernel == SSDK_PLAN_FIRST_TC) {
     int rc = upload_f32(m, &L.w_f32, master.data(), master.size()); if (rc) return rc;
     rc = upload_f32(m, &L.bias, bias.data(), bias.size()); if (rc) return rc;
     if (d.bn_scale && d.bn_shift && !L.bn_train) {
@@ -67,9 +81,8 @@ int build_conv(ssdk_model* m, int li) {
     }
     const double fl = 2.0 * m->B * L.H * L.W * (double)taps * cin * cout;
     m->flops_algo += fl;                 // counted as algorithmic FLOPs only (the timed conv launches exclude this layer)
-    // inference plans: the layer runs on the tensor cores with a gathered A tile (conv_first_kernel); training plans keep the fp32
-    // direct kernel, whose weights are the optimizer's master copy
-    if (!m->training && first_tc_supported(taps, cin, cout) && d.dilation >= 1 && first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l)) {
+    if (L.kernel == SSDK_PLAN_FIRST_TC) {
+      SSDK_REQUIRE(first_border_ok(ia, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l), "internal: activation border too small for the gathered A tile");
       std::vector<uint16_t> whi, wlo;
       L.first = first_plan(L.out, d.kh, d.kw, m->ctx->sm_count);
       first_weight_image(master.data(), taps, cin, cout, L.first.BN, L.first.kblocks, whi, wlo);
@@ -79,18 +92,17 @@ int build_conv(ssdk_model* m, int li) {
         rc = dev_alloc(m->allocs, &L.w_lo, wlo.size(), false); if (rc) return rc;
         SSDK_CHECK_CUDA(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
       }
-      L.first_tc = true;
     }
     return SSDK_OK;
   }
-  L.im2col = (d.stride != 1) || (cin < 8);
+  const bool im2col = L.kernel == SSDK_PLAN_IM2COL_GEMM;
   ConvLaunch& cl = L.launch;
   ConvArgs& a = cl.args;
   const int Ho = L.H, Wo = L.W;
   ConvGeom g;
   g.Ho = Ho; g.Wo = Wo; g.B = m->B; g.cout = cout;
   int kblocks;
-  if (L.im2col) {
+  if (im2col) {
     L.Kpad = (taps * cin + 7) / 8 * 8;
     kblocks = (L.Kpad + 63) / 64;
     size_t n = (size_t)m->B * Ho * Wo * L.Kpad + 64 * 8;
@@ -105,7 +117,7 @@ int build_conv(ssdk_model* m, int li) {
   }
   L.kblocks = kblocks;
   // weights: forward planes packed on the device from the master, which training plans keep for the optimiser
-  L.w_krow = L.im2col ? (size_t)kblocks * 64 : (size_t)taps * kblocks * 64;
+  L.w_krow = im2col ? (size_t)kblocks * 64 : (size_t)taps * kblocks * 64;
   int rc = dev_alloc(m->allocs, &L.w_hi, (size_t)cout * L.w_krow, false); if (rc) return rc;
   if (m->split) { rc = dev_alloc(m->allocs, &L.w_lo, (size_t)cout * L.w_krow, false); if (rc) return rc; }
   std::unique_ptr<float, CudaFree> scratch;         // the master of an inference plan, freed once the planes are packed
@@ -118,7 +130,7 @@ int build_conv(ssdk_model* m, int li) {
     scratch.reset(w_dev);
     SSDK_CHECK_CUDA(cudaMemcpy(w_dev, master.data(), master.size() * sizeof(float), cudaMemcpyHostToDevice));
   }
-  rc = launch_repack(m->ctx, w_dev, taps, cin, cout, L.im2col ? PACK_FWD_IM2COL : PACK_FWD, kblocks, L.w_krow, L.w_hi, L.w_lo, 0);
+  rc = launch_repack(m->ctx, w_dev, taps, cin, cout, im2col ? PACK_FWD_IM2COL : PACK_FWD, kblocks, L.w_krow, L.w_hi, L.w_lo, 0);
   if (rc) return rc;
   rc = plan_conv_gemm(m, cl, g, L.w_hi, L.w_lo, L.w_krow, kblocks, &L.tile_list);
   if (rc) return rc;
@@ -206,10 +218,9 @@ int plan_overlap(ssdk_model* m) {
   std::vector<int> kind(n, 0), grid(n, 0), input(n, -1);
   for (int i = 0; i < n; ++i) {
     const LayerPlan& L = m->layers[i];
-    const bool gemm = (L.d.op == SSDK_OP_CONV || L.d.op == SSDK_OP_HEAD) && !L.direct;
-    // an image-facing (direct) convolution in the trunk ends the narrow suffix like a wide one: give it a grid no R admits
-    if (L.d.op == SSDK_OP_CONV && L.direct) { kind[i] = 1; grid[i] = 1 << 30; }
-    else if (gemm) { kind[i] = L.d.op == SSDK_OP_HEAD ? 2 : 1; grid[i] = L.launch.grid; }
+    // an image-facing convolution in the trunk ends the narrow suffix like a wide one: give it a grid no R admits
+    if (L.kernel == SSDK_PLAN_FIRST_TC || L.kernel == SSDK_PLAN_DIRECT) { kind[i] = 1; grid[i] = 1 << 30; }
+    else if (L.kernel != SSDK_PLAN_NONE) { kind[i] = L.d.op == SSDK_OP_HEAD ? 2 : 1; grid[i] = L.launch.grid; }
     input[i] = (L.d.op == SSDK_OP_INPUT || L.d.op == SSDK_OP_TENSOR) ? -1 : L.d.input;
   }
   m->overlap_from = overlap_assign(n, kind.data(), grid.data(), input.data(), R, m->ctx->sm_count, m->on_side.data(), &m->grid_cap);
@@ -389,27 +400,27 @@ extern "C" int ssdk_model_create(ssdk_ctx* ctx, const ssdk_model_desc* desc, ssd
       L.H = in.H; L.W = in.W; L.C = in.C;
     } else { set_error("layer %d: unknown op %d", i, d.op); return fail(SSDK_ERR_INVALID); }
   }
-  // pass 2: border each producer must provide (max over its virtual-path conv consumers)
+  // pass 2: each convolution's kernel, and the borders its kernels read (im2col and conv_direct_kernel check bounds instead)
   for (int i = 0; i < n; ++i) {
-    const ssdk_layer_desc& d = m->layers[i].d;
+    LayerPlan& L = m->layers[i];
+    const ssdk_layer_desc& d = L.d;
     if (d.op != SSDK_OP_CONV && d.op != SSDK_OP_HEAD) continue;
     LayerPlan& in = m->layers[d.input];
-    const bool im2col = (d.stride != 1) || (in.C < 8);
-    if (!im2col) in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)));
-    // the image-facing layer's gathered A tile (conv_first_kernel) reads its taps from the input planes' zero border
-    if (!desc->training && in.C < 8 && d.stride == 1)
+    L.kernel = conv_kernel(d, in.C, L.C, m->training);
+    // the implicit GEMM and the gathered A tile (conv_first_kernel) read their taps from the input planes' zero border
+    if (L.kernel == SSDK_PLAN_GEMM) in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)));
+    if (L.kernel == SSDK_PLAN_FIRST_TC)
       in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_l),
                                                    std::max((d.kh - 1) * d.dilation - d.pad_t, (d.kw - 1) * d.dilation - d.pad_l)));
     // training: the image-facing weight-gradient kernel reads its 3x3 window without bounds checks
-    if (desc->training && in.C < 8 && d.stride == 1)
+    if (m->training && L.kernel == SSDK_PLAN_DIRECT)
       in.need_pad = std::max(in.need_pad, d.dilation * std::max(d.kh - 1, d.kw - 1));
-    if (desc->training && !im2col) {
+    if (m->training && L.kernel == SSDK_PLAN_GEMM) {
       // the gradient of this layer's output shares the geometry of the output itself and is the input of the
       // data-gradient convolution, whose padding is dilation*(k-1) - pad
-      LayerPlan& self = m->layers[i];
       const int pt = d.dilation * (d.kh - 1) - d.pad_t, pb = d.dilation * (d.kh - 1) - d.pad_b;
       const int pl = d.dilation * (d.kw - 1) - d.pad_l, pr = d.dilation * (d.kw - 1) - d.pad_r;
-      self.need_pad = std::max(self.need_pad, std::max(std::max(pt, pb), std::max(pl, pr)));
+      L.need_pad = std::max(L.need_pad, std::max(std::max(pt, pb), std::max(pl, pr)));
     }
   }
   // pass 3: buffers, weights, launches
@@ -474,22 +485,19 @@ extern "C" int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_
   SSDK_REQUIRE(m && out && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_plan: bad argument");
   memset(out, 0, sizeof(*out));
   const LayerPlan& L = m->layers[layer];
-  if (L.d.op != SSDK_OP_CONV && L.d.op != SSDK_OP_HEAD) return SSDK_OK;
-  out->split = m->split;
-  if (L.direct && L.first_tc) {
-    out->kernel = SSDK_PLAN_FIRST_TC;
-    out->bn = L.first.BN; out->kblocks = L.first.kblocks;
+  out->kernel = L.kernel;
+  if (L.kernel == SSDK_PLAN_NONE || L.kernel == SSDK_PLAN_DIRECT) return SSDK_OK;
+  if (L.kernel == SSDK_PLAN_FIRST_TC) {
+    out->bn = L.first.BN; out->split = m->split; out->kblocks = L.first.kblocks;
     out->n_tiles_m = L.first.n_tiles; out->n_tiles_n = 1;
     out->grid = L.first.grid; out->k_split = 1;
     return SSDK_OK;
   }
-  if (L.direct) { out->kernel = SSDK_PLAN_DIRECT; out->split = 0; return SSDK_OK; }
   const ConvArgs& a = L.launch.args;
-  out->kernel = L.im2col ? SSDK_PLAN_IM2COL_GEMM : SSDK_PLAN_GEMM;
   out->bn = a.BN; out->split = a.split; out->stages = a.stages; out->kblocks = a.kblocks;
   out->n_tiles_m = a.n_tiles_m; out->n_tiles_n = a.n_tiles_n; out->grid = L.launch.grid; out->k_split = a.k_split > 1 ? a.k_split : 1;
   out->epilogue = a.epi; out->head_fused = L.head_fused ? 1 : 0;
-  out->im2col_vec8 = L.im2col && L.im2col_vec8 ? 1 : 0;
+  out->im2col_vec8 = L.im2col_vec8 ? 1 : 0;
   return SSDK_OK;
 }
 
@@ -509,11 +517,9 @@ extern "C" int ssdk_model_set_timing(ssdk_model* m, int enable) {
 extern "C" int ssdk_model_last_conv_ms(ssdk_model* m, float* out_ms) {
   SSDK_REQUIRE(m && out_ms, "ssdk_model_last_conv_ms: NULL argument");
   float total = 0.f;
-  for (auto& L : m->layers) {
-    if (!L.ev0 || L.direct) continue;
-    SSDK_CHECK_CUDA(cudaEventSynchronize(L.ev1));
-    float ms = 0.f;
-    SSDK_CHECK_CUDA(cudaEventElapsedTime(&ms, L.ev0, L.ev1));
+  for (int i = 0; i < (int)m->layers.size(); ++i) {
+    float ms;
+    if (int rc = ssdk_model_layer_ms(m, i, &ms)) return rc;
     total += ms;
   }
   *out_ms = total;
@@ -524,7 +530,7 @@ extern "C" int ssdk_model_layer_ms(const ssdk_model* m, int layer, float* out_ms
   SSDK_REQUIRE(m && out_ms && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_ms: bad argument");
   const LayerPlan& L = m->layers[layer];
   *out_ms = 0.f;
-  if (!L.ev0 || L.direct) return SSDK_OK;
+  if (L.kernel != SSDK_PLAN_GEMM && L.kernel != SSDK_PLAN_IM2COL_GEMM) return SSDK_OK;
   SSDK_CHECK_CUDA(cudaEventSynchronize(L.ev1));
   SSDK_CHECK_CUDA(cudaEventElapsedTime(out_ms, L.ev0, L.ev1));
   return SSDK_OK;
@@ -577,18 +583,18 @@ extern "C" int ssdk_model_forward(ssdk_model* m, const float* images_dev, float*
       case SSDK_OP_CONV:
       case SSDK_OP_HEAD: {
         const LayerPlan& in = m->layers[d.input];
-        if (L.direct) {
-          if (L.first_tc)
+        if (L.kernel == SSDK_PLAN_FIRST_TC || L.kernel == SSDK_PLAN_DIRECT) {
+          if (L.kernel == SSDK_PLAN_FIRST_TC)
             rc = launch_conv_first(ctx, L.first, in.out, L.out, L.w_hi, L.w_lo, L.bias, L.bn_scale, L.bn_shift, d.act, d.kh, d.kw, d.dilation, d.pad_t,
                                    d.pad_l, stream);
           else
-          rc = launch_conv_direct(ctx, in.out, L.bn_train ? L.z : L.out, L.w_f32, L.bias, L.bn_scale, L.bn_shift, L.bn_train ? (int)SSDK_ACT_NONE : d.act,
-                                  d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, stream);
+            rc = launch_conv_direct(ctx, in.out, L.bn_train ? L.z : L.out, L.w_f32, L.bias, L.bn_scale, L.bn_shift, L.bn_train ? (int)SSDK_ACT_NONE : d.act,
+                                    d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, stream);
           if (rc) return rc;
           if (L.bn_train) { rc = launch_bn_forward(ctx, L, d.act, stream); if (rc) return rc; }
           break;
         }
-        if (L.im2col) {
+        if (L.kernel == SSDK_PLAN_IM2COL_GEMM) {
           rc = launch_im2col(ctx, in.out, L.col_hi, L.col_lo, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t, d.pad_l, L.Kpad, L.im2col_vec8, stream);
           if (rc) return rc;
         }

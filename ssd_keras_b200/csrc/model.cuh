@@ -12,11 +12,9 @@ struct LayerPlan {
   int H = 0, W = 0, C = 0;            // logical output shape
   int in_H = 0, in_W = 0, in_C = 0;
   ActBuf out;                         // INPUT / CONV / MAXPOOL / L2NORM
-  bool im2col = false;
-  bool direct = false;                // fp32 SIMT path for the image-facing conv (Cin < 8)
-  bool first_tc = false;           // direct layer of an inference plan on the tensor cores (conv_first_kernel)
-  FirstPlan first;                    // its launch shape (first_tc)
-  bool im2col_vec8 = false;           // im2col path: im2col8_kernel rather than im2col_kernel
+  ssdk_plan_kernel kernel = SSDK_PLAN_NONE;   // CONV / HEAD: the forward kernel (model.cu, conv_kernel)
+  FirstPlan first;                    // FIRST_TC: its launch shape
+  bool im2col_vec8 = false;           // IM2COL_GEMM: im2col8_kernel rather than im2col_kernel
   float* w_f32 = nullptr;
   int Kpad = 0;
   __nv_bfloat16* col_hi = nullptr; __nv_bfloat16* col_lo = nullptr;

@@ -368,18 +368,17 @@ struct TLayer {
   ActBuf g;                                 // gradient of this layer's output (pre-activation); same geometry as the output
   bool has_g = false;
   // data gradient
-  bool has_dgrad = false;
+  ssdk_dgrad_path dgrad_path = SSDK_DGRAD_NONE;   // plan_dgrad
   ConvLaunch dgrad{};
   __nv_bfloat16 *w2_hi = nullptr, *w2_lo = nullptr; size_t w2_krow = 0; int w2_kblocks = 0;
   int* dgrad_tiles = nullptr;
-  bool dgrad_strided = false;               // stride != 1: col-gradient GEMM (dZ * W^T) + col2im
-  int dgrad_relu_mask = 0;                  // col2im zeroes the gradient where the ReLU producer's output is <= 0
-  int dgrad_col2im_accumulate = 0;          // col2im adds to a gradient another consumer of the producer already wrote
+  int dgrad_relu_mask = 0;                  // STRIDED: col2im zeroes the gradient where the ReLU producer's output is <= 0
+  int dgrad_col2im_accumulate = 0;          // STRIDED: col2im adds to a gradient another consumer of the producer already wrote
   float* dcol = nullptr; int dcol_ld = 0;
   // weight gradient
-  bool wg_native = false;                   // stride-1 layers: wgrad.cu reads dZ / X in place (no transposed copies)
-  WgradLaunch wg;
-  std::vector<ConvLaunch> wgrad;            // fallback: one GEMM per tap (or one for the im2col path) on transposed operands
+  ssdk_wgrad_path wgrad_path = SSDK_WGRAD_NONE;   // plan_wgrad_layer
+  WgradLaunch wg;                           // NATIVE
+  std::vector<ConvLaunch> wgrad;            // TRANSPOSED / IM2COL: one GEMM per tap, or one on the im2col matrix
   int Wq = 0;                               // row pitch of the transposed operands' pixel grid
   std::vector<int> wgrad_res;               // tap shift mod 8: TMA needs 16-byte aligned K offsets, so XT is built once per residue
   long long Kv = 0, ldT = 0;
@@ -441,13 +440,14 @@ int repack_layer(ssdk_trainer* t, int i, cudaStream_t s) {
   const TLayer& T = t->tl[i];
   const LayerPlan& L = m->layers[i];
   int rc;
-  if (!L.direct) {
-    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, L.im2col ? PACK_FWD_IM2COL : PACK_FWD, L.kblocks, L.w_krow, L.w_hi, L.w_lo, s);
+  if (L.kernel == SSDK_PLAN_GEMM || L.kernel == SSDK_PLAN_IM2COL_GEMM) {
+    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, L.kernel == SSDK_PLAN_GEMM ? PACK_FWD : PACK_FWD_IM2COL, L.kblocks, L.w_krow,
+                       L.w_hi, L.w_lo, s);
     if (rc) return rc;
   }
-  if (T.has_dgrad) {
-    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, T.dgrad_strided ? PACK_DGRAD_COL : PACK_DGRAD, T.w2_kblocks, T.w2_krow, T.w2_hi,
-                       T.w2_lo, s);
+  if (T.dgrad_path != SSDK_DGRAD_NONE) {
+    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, T.dgrad_path == SSDK_DGRAD_GEMM ? PACK_DGRAD : PACK_DGRAD_COL, T.w2_kblocks, T.w2_krow,
+                       T.w2_hi, T.w2_lo, s);
     if (rc) return rc;
   }
   return SSDK_OK;
@@ -515,13 +515,12 @@ int plan_dgrad(ssdk_trainer* t, int i, std::vector<char>& written) {
   if (is_source(PL.d.op)) return SSDK_OK;
   if (T.cin % 8 != 0) { set_error("training: input channels must be a multiple of 8 (layer %d)", i); return SSDK_ERR_UNSUPPORTED; }
   const int relu_mask = (PL.d.op == SSDK_OP_CONV && PL.d.act == SSDK_ACT_RELU) ? 1 : 0;
-  T.has_dgrad = true;
-  T.dgrad_strided = d.stride != 1;
+  T.dgrad_path = d.stride != 1 ? SSDK_DGRAD_STRIDED : SSDK_DGRAD_GEMM;
   T.w2_kblocks = (T.g.Cs + 63) / 64;
   ConvGeom gg;
   gg.in = &T.g; gg.B = m->B;
   int rows, rc;                               // rows of the packed planes
-  if (T.dgrad_strided) {
+  if (T.dgrad_path == SSDK_DGRAD_STRIDED) {
     // dCol[M][taps*cin] = dZ[M][cout] * W^T, then col2im
     rows = T.dcol_ld = T.taps * T.cin;
     T.w2_krow = (size_t)T.w2_kblocks * 64;
@@ -540,7 +539,7 @@ int plan_dgrad(ssdk_trainer* t, int i, std::vector<char>& written) {
   if (rc) return rc;
   ConvArgs& a = T.dgrad.args;
   a.bias = nullptr; a.act = SSDK_ACT_NONE;
-  if (T.dgrad_strided) {
+  if (T.dgrad_path == SSDK_DGRAD_STRIDED) {
     a.epi = EPI_F32; a.out_f32 = T.dcol;
     T.dgrad_relu_mask = relu_mask;
     T.dgrad_col2im_accumulate = written[pi];
@@ -554,22 +553,23 @@ int plan_dgrad(ssdk_trainer* t, int i, std::vector<char>& written) {
   return SSDK_OK;
 }
 
-// Weight-gradient plan of conv layer i: wgrad.cu's GEMM on dZ / X in place, or the geometry of the transposed operands (their
-// GEMMs are planned by plan_transposed_gemms once the shared scratch is sized).  Direct layers need none.
+// Weight-gradient path of conv layer i and its plan: wgrad.cu's GEMM on dZ / X in place, or the geometry of the transposed
+// operands (their GEMMs are planned by plan_transposed_gemms once the shared scratch is sized).  DIRECT needs none.
 int plan_wgrad_layer(ssdk_trainer* t, int i, long long& max_xT, long long& max_dyT) {
   ssdk_model* m = t->m;
   const LayerPlan& L = m->layers[i];
   TLayer& T = t->tl[i];
   const ssdk_layer_desc& d = L.d;
-  if (L.direct) return SSDK_OK;               // handled by wgrad_direct_kernel
+  if (L.kernel == SSDK_PLAN_DIRECT) { T.wgrad_path = SSDK_WGRAD_DIRECT; return SSDK_OK; }
   const ActBuf& X = m->layers[d.input].out;
   int transposed;
   if (int rc = env_int("SSDK_WGRAD_TRANSPOSED", 0, &transposed)) return rc;
-  if (!L.im2col && !transposed && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
-    T.wg_native = true;
+  if (L.kernel == SSDK_PLAN_GEMM && !transposed && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
+    T.wgrad_path = SSDK_WGRAD_NATIVE;
     return plan_wgrad(m->ctx, T.wg, X, T.g, L.H, L.W, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, m->split, span_grad(t, i, 0));
   }
-  if (L.im2col) {
+  T.wgrad_path = L.kernel == SSDK_PLAN_IM2COL_GEMM ? SSDK_WGRAD_IM2COL : SSDK_WGRAD_TRANSPOSED;
+  if (T.wgrad_path == SSDK_WGRAD_IM2COL) {
     T.Kv = (long long)m->B * L.H * L.W;
     T.ldT = (T.Kv + 7) / 8 * 8 + 64;
     T.dy_map = TMap{0, L.H * L.W, L.W, L.H, L.W, T.g.Hp(), T.g.Wp(), T.g.pad};
@@ -596,11 +596,12 @@ int plan_transposed_gemms(ssdk_trainer* t) {
   for (int i = 0; i < (int)m->layers.size(); ++i) {
     const LayerPlan& L = m->layers[i];
     TLayer& T = t->tl[i];
-    if (!is_conv(L.d.op) || L.direct || T.wg_native) continue;
+    if (T.wgrad_path != SSDK_WGRAD_TRANSPOSED && T.wgrad_path != SSDK_WGRAD_IM2COL) continue;
+    const bool im2col = T.wgrad_path == SSDK_WGRAD_IM2COL;
     const ssdk_layer_desc& d = L.d;
     const ActBuf& X = m->layers[d.input].out;
-    const int n_gemm = L.im2col ? 1 : T.taps;
-    const int ncols = L.im2col ? L.Kpad : T.cin;            // N of the GEMM
+    const int n_gemm = im2col ? 1 : T.taps;
+    const int ncols = im2col ? L.Kpad : T.cin;              // N of the GEMM
     const int kblocks = (int)((T.Kv + 63) / 64);
     T.wgrad.resize(n_gemm); T.wgrad_res.assign(n_gemm, 0);
     for (int tp = 0; tp < n_gemm; ++tp) {
@@ -614,7 +615,7 @@ int plan_transposed_gemms(ssdk_trainer* t) {
       ConvArgs& a = cl.args;
       a.epi = EPI_ATOMIC; a.bias = nullptr; a.act = SSDK_ACT_NONE;
       a.out_f32 = span_grad(t, i, 0);
-      if (L.im2col) { a.out_ld = T.taps * T.cin; a.out_col_off = 0; a.b_k_offset = 0; a.cout = T.taps * T.cin; a.n_tiles_n = (a.cout + a.BN - 1) / a.BN; }
+      if (im2col) { a.out_ld = T.taps * T.cin; a.out_col_off = 0; a.b_k_offset = 0; a.cout = T.taps * T.cin; a.n_tiles_n = (a.cout + a.BN - 1) / a.BN; }
       else {
         const int kh = tp / d.kw, kw = tp % d.kw;
         a.out_ld = T.taps * T.cin; a.out_col_off = tp * T.cin;
@@ -729,33 +730,27 @@ extern "C" int ssdk_trainer_layer_plan(const ssdk_trainer* t, int layer, ssdk_ba
   memset(out, 0, sizeof(*out));
   const TLayer& T = t->tl[layer];
   const LayerPlan& L = t->m->layers[layer];
-  if (!is_conv(L.d.op)) return SSDK_OK;
-  if (T.has_dgrad) {
+  out->dgrad = T.dgrad_path;
+  if (T.dgrad_path != SSDK_DGRAD_NONE) {
     const ConvArgs& a = T.dgrad.args;
-    out->dgrad = T.dgrad_strided ? SSDK_DGRAD_STRIDED : SSDK_DGRAD_GEMM;
     out->dgrad_bn = a.BN;
-    out->dgrad_mask = T.dgrad_strided ? T.dgrad_relu_mask : (a.mask_hi != nullptr);
-    out->dgrad_accumulate = T.dgrad_strided ? T.dgrad_col2im_accumulate : a.accumulate;
+    out->dgrad_mask = T.dgrad_path == SSDK_DGRAD_STRIDED ? T.dgrad_relu_mask : (a.mask_hi != nullptr);
+    out->dgrad_accumulate = T.dgrad_path == SSDK_DGRAD_STRIDED ? T.dgrad_col2im_accumulate : a.accumulate;
     out->dgrad_n_tiles_m = a.n_tiles_m; out->dgrad_n_tiles_n = a.n_tiles_n; out->dgrad_grid = T.dgrad.grid;
   }
-  if (L.direct) {
-    out->wgrad = SSDK_WGRAD_DIRECT;
+  out->wgrad = T.wgrad_path;
+  if (T.wgrad_path == SSDK_WGRAD_DIRECT) {
     out->direct_fast = direct_fast3(L.d, t->m->layers[L.d.input].out, T.cin, T.cout) ? 1 : 0;
-    return SSDK_OK;
-  }
-  if (T.wg_native) {
+  } else if (T.wgrad_path == SSDK_WGRAD_NATIVE) {
     const WgradArgs& w = T.wg.args;
-    out->wgrad = SSDK_WGRAD_NATIVE;
     out->wgrad_bn = w.BNc; out->a_boxes = w.a_boxes; out->bw = w.bw; out->bh = w.bh;
     out->co_tiles = w.co_tiles; out->ci_tiles = w.ci_tiles; out->k_split = w.k_split > 1 ? w.k_split : 1;
     out->stages = w.stages; out->grid = T.wg.grid; out->kv = w.total_patches;
-    return SSDK_OK;
+  } else if (T.wgrad_path != SSDK_WGRAD_NONE) {
+    const ConvLaunch& c = T.wgrad[0];
+    out->wgrad_bn = c.args.BN; out->k_split = c.args.k_split > 1 ? c.args.k_split : 1;
+    out->n_gemms = (int)T.wgrad.size(); out->stages = c.args.stages; out->grid = c.grid; out->kv = (int)T.Kv;
   }
-  if (T.wgrad.empty()) return SSDK_OK;
-  const ConvLaunch& c = T.wgrad[0];
-  out->wgrad = L.im2col ? SSDK_WGRAD_IM2COL : SSDK_WGRAD_TRANSPOSED;
-  out->wgrad_bn = c.args.BN; out->k_split = c.args.k_split > 1 ? c.args.k_split : 1;
-  out->n_gemms = (int)T.wgrad.size(); out->stages = c.args.stages; out->grid = c.grid; out->kv = (int)T.Kv;
   return SSDK_OK;
 }
 
@@ -846,10 +841,10 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     //      the raw conv output (and produce dgamma / dbeta) before the conv's own gradients are formed
     if (L.bn_train) { rc = launch_bn_backward(ctx, L, d.act, T.g, span_grad(t, i, 3), span_grad(t, i, 4), s); if (rc) return rc; }
     // ---- convolution / head: weight + bias gradients
-    if (L.direct) {
+    if (T.wgrad_path == SSDK_WGRAD_DIRECT) {
       const int K = T.taps * T.cin;
       const size_t smem = (size_t)K * T.cout * sizeof(float);
-      // the plan admits direct layers whose fp32 [K][Cout] accumulator needs up to 96 KB (model.cu, as conv_direct_kernel)
+      // the plan admits direct layers whose fp32 [K][Cout] accumulator needs up to 96 KB (model.cu, conv_kernel)
       const int total_rows = T.g.B * T.g.H;
       const int rpb = std::max(1, (total_rows + 8 * ctx->sm_count - 1) / (8 * ctx->sm_count));
       const unsigned grid = (unsigned)((total_rows + rpb - 1) / rpb);
@@ -858,12 +853,12 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
       else
         rc = launch(ctx, wgrad_direct_kernel, grid, 256, smem, s, PL.out, T.g, span_grad(t, i, 0), d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, rpb);
       if (rc) return rc;
-    } else if (T.wg_native) {
+    } else if (T.wgrad_path == SSDK_WGRAD_NATIVE) {
       rc = launch_wgrad(ctx, T.wg, s); if (rc) return rc;
     } else {
       // transposed operands
       rc = do_transpose(t, T.g.hi, T.g.lo, T.g.Cs, (long long)T.g.rows(), T.dy_map, T.Kv, T.cout, t->dyT_hi, t->dyT_lo, T.ldT, s); if (rc) return rc;
-      if (L.im2col) {
+      if (T.wgrad_path == SSDK_WGRAD_IM2COL) {
         rc = do_transpose(t, L.col_hi, L.col_lo, L.Kpad, T.Kv, T.x_map, T.Kv, L.Kpad, t->xT_hi, t->xT_lo, T.ldT, s); if (rc) return rc;
         rc = launch_conv(ctx, T.wgrad[0], s); if (rc) return rc;
       } else {
@@ -880,14 +875,14 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
     }
     rc = launch_bias_grad(ctx, T.g, span_grad(t, i, 1), s); if (rc) return rc;
     // ---- data gradient
-    if (T.has_dgrad && T.dgrad_strided) {
+    if (T.dgrad_path == SSDK_DGRAD_STRIDED) {
       rc = launch_conv(ctx, T.dgrad, s); if (rc) return rc;
       const size_t total = (size_t)PT.g.B * PT.g.H * PT.g.W * PT.g.C;
       rc = launch(ctx, col2im_kernel, (unsigned)((total + 255) / 256), 256, 0, s, T.dcol, L.H, L.W, d.kh, d.kw, d.stride, d.dilation, d.pad_t,
                   d.pad_l, T.dcol_ld, PL.out, PT.g, T.dgrad_relu_mask, written[pi] ? 1 : 0);
       if (rc) return rc;
       written[pi] = 1;
-    } else if (T.has_dgrad) {
+    } else if (T.dgrad_path == SSDK_DGRAD_GEMM) {
       T.dgrad.args.accumulate = written[pi] ? 1 : 0;
       rc = launch_conv(ctx, T.dgrad, s); if (rc) return rc;
       written[pi] = 1;
