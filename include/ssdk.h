@@ -632,6 +632,10 @@ int ssdk_trainer_read_params(ssdk_trainer* t, float* out_dev, void* stream);
  * slot 0 = the SGD velocity or the Adam first moment m, slot 1 = the Adam second moment v (an error before the first Adam
  * update, and for any other slot). */
 int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out_dev, void* stream);
+/* The inverse of ssdk_trainer_read_opt_state: overwrite one slot of the optimiser state from src_dev, in the gradient's layout
+ * (kernels OHWI), bit for bit, so that a run resumes with the state it was saved with.  Slot 1 (Adam's v) is made by its first
+ * write if no Adam update has made it yet; any other slot is an error. */
+int ssdk_trainer_write_opt_state(ssdk_trainer* t, int slot, const float* src_dev, void* stream);
 
 /* Read-only view of the backward launches ssdk_trainer_create planned for one convolution or head (host only). */
 enum ssdk_dgrad_path { SSDK_DGRAD_NONE = 0, SSDK_DGRAD_GEMM = 1 /* implicit GEMM into the producer's gradient planes */,

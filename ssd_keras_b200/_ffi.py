@@ -217,6 +217,7 @@ SIGNATURES = {
     'ssdk_trainer_read_bn_input': (_i, [_p, _i, _p, _p]),
     'ssdk_trainer_read_params': (_i, [_p, _p, _p]),
     'ssdk_trainer_read_opt_state': (_i, [_p, _i, _p, _p]),
+    'ssdk_trainer_write_opt_state': (_i, [_p, _i, _p, _p]),
     'ssdk_trainer_layer_plan': (_i, [_p, _i, C.POINTER(BackwardPlan)]),
 }
 

@@ -360,6 +360,15 @@ __global__ void hwio_to_ohwi_kernel(const float* __restrict__ w, int taps, int c
   out[i] = w[((size_t)t * cin + ci) * cout + co];
 }
 
+// the inverse of hwio_to_ohwi_kernel: `in` in the gradient's OHWI layout -> the master's HWIO
+__global__ void ohwi_to_hwio_kernel(const float* __restrict__ in, int taps, int cin, int cout, float* __restrict__ w) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t total = (size_t)taps * cin * cout;
+  if (i >= total) return;
+  const int ci = (int)(i % cin); const size_t r = i / cin; const int t = (int)(r % taps); const int co = (int)(r / taps);
+  w[((size_t)t * cin + ci) * cout + co] = in[i];
+}
+
 // ---------------------------------------------------------------------------------------------
 // plan
 // ---------------------------------------------------------------------------------------------
@@ -904,6 +913,18 @@ int read_span(ssdk_trainer* t, const ParamSpan& p, const float* src, float* out_
   return SSDK_OK;
 }
 
+// the inverse of read_span: span p of src_dev, in the gradient's layout, into `dst` (its value's layout)
+int write_span(ssdk_trainer* t, const ParamSpan& p, const float* src_dev, float* dst, cudaStream_t s) {
+  if (p.taps) return launch(t->m->ctx, ohwi_to_hwio_kernel, (unsigned)((p.count + 255) / 256), 256, 0, s, src_dev + p.off, p.taps, p.cin, p.cout, dst);
+  SSDK_CHECK_CUDA(cudaMemcpyAsync(dst, src_dev + p.off, (size_t)p.count * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return SSDK_OK;
+}
+
+// slot 1 of the optimiser state (Adam's second moment) is made, zeroed, by the first Adam update or the first write into it
+int ensure_state(ssdk_trainer* t, int slot) {
+  return t->state[slot] ? SSDK_OK : dev_alloc(t->allocs, &t->state[slot], (size_t)t->n_params, true);
+}
+
 }  // namespace
 
 extern "C" int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float l2_reg, float grad_scale, void* stream_) {
@@ -925,7 +946,7 @@ extern "C" int ssdk_train_apply_adam(ssdk_trainer* t, float lr, float beta1, flo
   cudaStream_t s = (cudaStream_t)stream_;
   // Keras: lr_t = lr * sqrt(1 - beta_2^t) / (1 - beta_1^t)
   const float lr_t = lr * (float)(std::sqrt(1.0 - std::pow((double)beta2, (double)step)) / (1.0 - std::pow((double)beta1, (double)step)));
-  if (!t->state[1]) { const int rc = dev_alloc(t->allocs, &t->state[1], (size_t)t->n_params, true); if (rc) return rc; }
+  if (const int rc = ensure_state(t, 1)) return rc;
   for (size_t k = 0; k < t->params.size(); ++k) {
     const ParamSpan& p = t->params[k];
     int rc = launch(t->m->ctx, p.taps ? adam_kernel<true> : adam_kernel<false>, (unsigned)((p.count + 255) / 256), 256, 0, s, p.value,
@@ -944,6 +965,18 @@ extern "C" int ssdk_trainer_read_opt_state(ssdk_trainer* t, int slot, float* out
                "after an Adam update)", slot);
   for (const ParamSpan& p : t->params) {
     const int rc = read_span(t, p, t->state[slot] + p.off, out_dev, (cudaStream_t)stream_);
+    if (rc) return rc;
+  }
+  return SSDK_OK;
+}
+
+extern "C" int ssdk_trainer_write_opt_state(ssdk_trainer* t, int slot, const float* src_dev, void* stream_) {
+  SSDK_REQUIRE(t && src_dev, "ssdk_trainer_write_opt_state: NULL argument");
+  SSDK_REQUIRE(slot == 0 || slot == 1,
+               "ssdk_trainer_write_opt_state: slot %d does not exist (0: SGD velocity / Adam first moment, 1: Adam second moment)", slot);
+  if (const int rc = ensure_state(t, slot)) return rc;
+  for (const ParamSpan& p : t->params) {
+    const int rc = write_span(t, p, src_dev, t->state[slot] + p.off, (cudaStream_t)stream_);
     if (rc) return rc;
   }
   return SSDK_OK;

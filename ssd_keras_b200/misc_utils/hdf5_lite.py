@@ -11,8 +11,9 @@ Anything outside the subset (new-style groups, superblock >= 2, variable-length 
 name of the feature, never a silent misread.
 
 ``read_datasets(path)`` -> ``{'/group/sub/name': ndarray}``;  ``read_attributes(path, '/')`` -> ``{name: value}`` (fixed-length
-strings / numeric arrays only).  ``write_keras_weights(path, layers)`` writes a file with the same structures (used by the tests
-to produce Keras-layout files; files from real h5py use the same structures with different block placement)."""
+strings / numeric arrays only);  ``read_optimizer_weights(path)`` -> ``[(name, array)]`` of ``/optimizer_weights``.
+``write_keras_weights(path, layers)`` writes a file with the same structures (``model.save`` / ``save_weights`` and the tests use
+it; files from real h5py use the same structures with different block placement)."""
 import struct
 import zlib
 
@@ -443,7 +444,7 @@ class _Writer:
         return self._header(msgs)
 
     def dataset(self, arr):
-        arr = np.ascontiguousarray(arr)
+        arr = np.ascontiguousarray(arr).reshape(np.shape(arr))     # a scalar stays a scalar (Keras' iterations:0)
         data = self._alloc(max(arr.nbytes, 1))
         self.buf[data:data + arr.nbytes] = arr.tobytes()
         layout = struct.pack('<BBQQ', 3, 1, data, arr.nbytes)
@@ -496,12 +497,42 @@ class _Writer:
             f.write(bytes(b))
 
 
-def write_keras_weights(path, weights, full_model=False, chunked=(), root_attrs=None):
+def read_optimizer_weights(path):
+    """The ``/optimizer_weights`` group of a full-model file as ``[(name, array), ...]`` in the order of its ``weight_names``
+    attribute (Keras' ``optimizer.get_weights()`` order); ``[]`` when the file has none."""
+    with open(path, 'rb') as f:
+        datasets, attrs = _Reader(f.read()).walk()
+    names = attrs.get('/optimizer_weights', {}).get('weight_names')
+    if names is None:
+        return []
+    out = []
+    for n in np.atleast_1d(names):
+        n = bytes(n).decode('utf-8')
+        if '/optimizer_weights/' + n not in datasets:
+            raise ValueError('%s: optimizer weight %s is listed in weight_names but not stored' % (path, n))
+        out.append((n, datasets['/optimizer_weights/' + n]))
+    return out
+
+
+def _tree(w, items):
+    """[('a/b/name', array), ...] -> the links of one group: datasets for plain names, nested groups for 'a/...' prefixes."""
+    links, sub = [], {}
+    for name, arr in items:
+        head, _, rest = name.partition('/')
+        if rest:
+            sub.setdefault(head, []).append((rest, arr))
+        else:
+            links.append((head, w.dataset(np.asarray(arr))))
+    return links + [(head, w.group(_tree(w, part))[0]) for head, part in sub.items()]
+
+
+def write_keras_weights(path, weights, full_model=False, chunked=(), root_attrs=None, optimizer_weights=()):
     """``weights``: ``{'conv1_1/kernel': array, 'conv1_1/bias': array, ...}`` -> an HDF5 file with the layout of
     ``model.save_weights`` (``/<layer>/<layer>/kernel:0`` datasets, ``layer_names`` / ``weight_names`` attributes); with
     ``full_model`` everything sits below ``/model_weights`` like in ``model.save``; the weights named in ``chunked`` are stored
     chunked with shuffle + gzip filters; ``root_attrs`` (name -> bytes / array) become attributes of the root group, where
-    ``model.save`` keeps ``model_config``."""
+    ``model.save`` keeps ``model_config``.  ``optimizer_weights`` (full model only): ``[(name, array), ...]`` stored below
+    ``/optimizer_weights`` -- a name's '/' parts become nested groups -- with their order in its ``weight_names`` attribute."""
     w = _Writer()
     layers = {}
     for k, v in weights.items():
@@ -519,8 +550,14 @@ def write_keras_weights(path, weights, full_model=False, chunked=(), root_attrs=
     if full_model:
         mw, _, _ = w.group(top, attrs=attrs)
         ra = {k: (np.array(v) if isinstance(v, (bytes, str)) else np.asarray(v)) for k, v in (root_attrs or {}).items()}
-        root, bt, heap = w.group([('model_weights', mw)], attrs=ra or None)
+        links = [('model_weights', mw)]
+        if optimizer_weights:
+            names = np.array([n.encode() for n, _ in optimizer_weights])
+            links.append(('optimizer_weights', w.group(_tree(w, optimizer_weights), attrs={'weight_names': names})[0]))
+        root, bt, heap = w.group(links, attrs=ra or None)
     else:
+        if optimizer_weights:
+            raise ValueError('optimizer weights belong to a full-model file')
         if root_attrs:
             attrs.update({k: (np.array(v) if isinstance(v, (bytes, str)) else np.asarray(v)) for k, v in root_attrs.items()})
         root, bt, heap = w.group(top, attrs=attrs)

@@ -226,6 +226,7 @@ class SSDModel(KerasTrainingMixin):
             if tuple(v.shape) != tuple(shapes[k]):
                 raise ValueError('Weight %s has shape %s, expected %s' % (k, v.shape, shapes[k]))
             self.weights[k] = np.ascontiguousarray(v)
+        self._pending_opt_state = None             # new weights start a fresh optimiser state, as they do for a live trainer
         self._release()
 
     def get_weights(self):
@@ -285,20 +286,27 @@ class SSDModel(KerasTrainingMixin):
         else:
             np.savez(p, **self.weights)
 
-    def save(self, filepath):
+    def save(self, filepath, include_optimizer=True):
         """``model.save(filepath)`` (reference ``ssd300_training.ipynb:409-413`` via ``ModelCheckpoint``): one HDF5 file with the
         weights below ``/model_weights`` (Keras' layout: ``load_weights(filepath, by_name=True)`` of either library reads it) and,
         as the root attribute ``model_config``, the builder call that made this model -- what ``models.load_model`` rebuilds it
-        from.  Optimizer state is not stored."""
+        from.  With ``include_optimizer`` a compiled model also stores Keras' ``training_config`` (optimizer, current learning
+        rate, loss) and, once it has trained, the optimizer state below ``/optimizer_weights`` (Keras' order: ``iterations:0``,
+        then the SGD velocities ``moments/...`` or Adam's ``ms/...`` and ``vs/...``), so that a run resumed from the file picks
+        up where it left off."""
         import json
         self._sync_trained()
         if getattr(self, '_build_config', None) is None:
             raise ValueError('this model was not made by ssd_300 / ssd_512 / build_model: save_weights() it instead')
         name, kwargs = self._build_config
         cfg = json.dumps({'class_name': 'SSDModel', 'config': {'builder': name, 'kwargs': kwargs}}).encode()
+        attrs = {'model_config': cfg, 'keras_version': b'2.1.4', 'backend': b'ssd_keras_b200'}
+        opt_weights = []
+        if include_optimizer and self._compiled is not None:
+            attrs['training_config'] = json.dumps(self._training_config()).encode()
+            opt_weights = self._optimizer_weights()
         from ..misc_utils.hdf5_lite import write_keras_weights
-        write_keras_weights(str(filepath), self.weights, full_model=True,
-                            root_attrs={'model_config': cfg, 'keras_version': b'2.1.4', 'backend': b'ssd_keras_b200'})
+        write_keras_weights(str(filepath), self.weights, full_model=True, root_attrs=attrs, optimizer_weights=opt_weights)
 
     # -- execution ---------------------------------------------------------------------------
     def _release(self):

@@ -20,10 +20,16 @@ def _call(callbacks, name, *args):
             fn(*args)
 
 
+# the dataset-name prefix of each optimiser slot below /optimizer_weights: Keras' SGD keeps [iterations] + moments, Adam
+# [iterations] + ms + vs
+SLOT_PREFIXES = {'sgd': ('moments',), 'adam': ('ms', 'vs')}
+
+
 class KerasTrainingMixin:
     optimizer = None
     _compiled = None
     _fit_trainer = None
+    _pending_opt_state = None          # optimiser state loaded by load_model, applied to the next trainer _trainer_for makes
     stop_training = False
 
     def compile(self, optimizer, loss=None, **kwargs):
@@ -46,6 +52,71 @@ class KerasTrainingMixin:
                              'computes that loss and its gradient on the device')
         self.optimizer, self._compiled = optimizer, (kind, owner)
         self._fit_trainer = None
+        self._pending_opt_state = None
+
+    # -- the training half of a full-model file (Keras' training_config and /optimizer_weights) --------------------------------
+    def _training_config(self):
+        """Keras' ``training_config`` root attribute of ``model.save``, with the ``SSDLoss`` parameters load_model rebuilds the
+        loss from when ``custom_objects`` does not bring it."""
+        kind, lossobj = self._compiled
+        o = self.optimizer
+        if kind == 'sgd':
+            opt = {'class_name': 'SGD', 'config': {'lr': float(o.lr), 'momentum': float(getattr(o, 'momentum', 0.0)), 'decay': 0.0,
+                                                   'nesterov': False}}
+        else:
+            opt = {'class_name': 'Adam', 'config': {'lr': float(o.lr), 'beta_1': float(getattr(o, 'beta_1', 0.9)),
+                                                    'beta_2': float(getattr(o, 'beta_2', 0.999)), 'decay': 0.0,
+                                                    'epsilon': float(getattr(o, 'epsilon', 1e-8)), 'amsgrad': False}}
+        return {'optimizer_config': opt, 'loss': 'compute_loss', 'metrics': [], 'sample_weight_mode': None, 'loss_weights': None,
+                'ssd_loss': {'neg_pos_ratio': lossobj.neg_pos_ratio, 'n_neg_min': lossobj.n_neg_min, 'alpha': lossobj.alpha}}
+
+    def _optimizer_weights(self):
+        """``[(name, array), ...]`` for ``/optimizer_weights`` in Keras' order -- ``iterations:0``, then each slot in the trainer's
+        parameter order -- from the trainer that has been training, or the loaded state still waiting for one; ``[]`` when the
+        model has not trained."""
+        t = self._fit_trainer
+        state = t.get_optimizer_state() if t is not None and t.iterations > 0 else self._pending_opt_state
+        if state is None:
+            return []
+        out = [('iterations:0', np.array(state['iterations'], np.int64))]
+        for prefix, named in zip(SLOT_PREFIXES[self._compiled[0]], state['slots']):
+            out += [('%s/%s:0' % (prefix, k), v) for k, v in named.items()]
+        return out
+
+    def _restore_training(self, config, opt_weights, custom_objects):
+        """``load_model``'s ``compile=True``: compile with the stored optimizer and learning rate, and keep the stored optimizer
+        state (checked against this model) for the trainer of the next step."""
+        from .. import optimizers
+        from ..keras_loss_function.keras_ssd_loss import SSDLoss
+        from ..training import check_optimizer_state
+        oc = config['optimizer_config']
+        c = oc['config']
+        if oc['class_name'] == 'SGD':
+            opt = optimizers.SGD(lr=c['lr'], momentum=c.get('momentum', 0.0))
+        elif oc['class_name'] == 'Adam':
+            opt = optimizers.Adam(lr=c['lr'], beta_1=c.get('beta_1', 0.9), beta_2=c.get('beta_2', 0.999), epsilon=c.get('epsilon', 1e-8))
+        else:
+            raise ValueError('training_config names the optimizer %r: SGD and Adam are implemented' % (oc['class_name'],))
+        loss = (custom_objects or {}).get('compute_loss')
+        if not isinstance(getattr(loss, '__self__', None), SSDLoss):
+            loss = SSDLoss(**config['ssd_loss']).compute_loss
+        self.compile(optimizer=opt, loss=loss)
+        if not opt_weights:
+            return
+        if opt_weights[0][0] != 'iterations:0':
+            raise ValueError('optimizer weights must start with iterations:0, got %s' % opt_weights[0][0])
+        prefixes = SLOT_PREFIXES[opt.kind]
+        slots = {}
+        for name, arr in opt_weights[1:]:
+            prefix, _, key = name.partition('/')
+            if prefix not in prefixes or not key.endswith(':0'):
+                raise ValueError('optimizer weight %s does not belong to %s' % (name, oc['class_name']))
+            slots.setdefault(prefixes.index(prefix), {})[key[:-2]] = arr
+        if sorted(slots) != list(range(len(slots))):
+            raise ValueError('optimizer weights: %s has no %s slot' % (oc['class_name'], prefixes[0]))
+        state = {'iterations': int(opt_weights[0][1]), 'slots': [slots[i] for i in range(len(slots))]}
+        check_optimizer_state(self, opt.kind, state)
+        self._pending_opt_state = state
 
     def _trainer_for(self, batch):
         from ..training import SSDTrainer
@@ -61,6 +132,9 @@ class KerasTrainingMixin:
             t = SSDTrainer(self, batch, lr=o.lr, momentum=getattr(o, 'momentum', 0.0), neg_pos_ratio=lossobj.neg_pos_ratio,
                            n_neg_min=lossobj.n_neg_min, alpha=lossobj.alpha, optimizer=kind, beta_1=getattr(o, 'beta_1', 0.9),
                            beta_2=getattr(o, 'beta_2', 0.999), epsilon=getattr(o, 'epsilon', 1e-8))
+            if self._pending_opt_state is not None:
+                t.set_optimizer_state(self._pending_opt_state)
+                self._pending_opt_state = None
             self._fit_trainer = t
         t.lr = float(self.optimizer.lr)                  # a callback (or the caller) may have changed the learning rate
         return t

@@ -12,6 +12,29 @@ import numpy as np
 from . import _ffi
 
 
+def check_optimizer_state(model, optimizer, state):
+    """Raise ``ValueError`` unless ``state`` (``{'iterations': int, 'slots': [dict, ...]}``, see
+    ``SSDTrainer.get_optimizer_state``) fits ``model`` and ``optimizer`` ('sgd' / 'adam'): SGD has one slot, Adam two once it
+    has taken a step (one before), and every slot holds exactly the model's trainable weights with their shapes."""
+    it = state.get('iterations') if isinstance(state, dict) else None
+    if not isinstance(it, (int, np.integer)) or isinstance(it, bool) or it < 0:
+        raise ValueError('optimizer state: iterations must be a non-negative integer, got %r' % (it,))
+    slots = state['slots']
+    want = (1,) if optimizer == 'sgd' else (2,) if it > 0 else (1, 2)
+    if len(slots) not in want:
+        raise ValueError('optimizer state: %d slot(s) after %d iterations, but %s keeps %s' % (len(slots), it, optimizer, ' or '.join(map(str, want))))
+    shapes = {k: tuple(v) for k, v in model.weight_shapes().items() if not k.endswith(('/moving_mean', '/moving_variance'))}
+    for i, named in enumerate(slots):
+        for k, shp in shapes.items():
+            if k not in named:
+                raise ValueError('optimizer state: slot %d has no entry for weight %s' % (i, k))
+            if tuple(np.shape(named[k])) != shp:
+                raise ValueError('optimizer state: slot %d, weight %s has shape %s, expected %s' % (i, k, tuple(np.shape(named[k])), shp))
+        for k in named:
+            if k not in shapes:
+                raise ValueError('optimizer state: slot %d has an entry for %s, which is not a trainable weight of this model' % (i, k))
+
+
 class SSDTrainer:
     def __init__(self, model, batch_size, lr=1e-3, momentum=0.9, l2_regularization=None, neg_pos_ratio=3, n_neg_min=0,
                  alpha=1.0, loss_mode='replica', optimizer='sgd', beta_1=0.9, beta_2=0.999, epsilon=1e-8):
@@ -25,6 +48,7 @@ class SSDTrainer:
         self.loss_mode = loss_mode
         self.optimizer, self.beta_1, self.beta_2, self.epsilon = optimizer, float(beta_1), float(beta_2), float(epsilon)
         self.iterations = 0                      # optimiser steps taken (Adam's bias correction)
+        self._n_slots = 1                        # optimiser state slots on the device: Adam's v is made by its first update
         import torch
         self.model = model
         self.batch = int(batch_size)
@@ -75,6 +99,7 @@ class SSDTrainer:
         self.plan = None
         self._dirty = False
         self.iterations = 0
+        self._n_slots = 1
 
     def __del__(self):
         try:
@@ -125,6 +150,7 @@ class SSDTrainer:
         if self.optimizer == 'adam':
             _ffi.check(_ffi.lib().ssdk_train_apply_adam(self.handle, self.lr, self.beta_1, self.beta_2, self.epsilon, self.l2, float(grad_scale),
                                                         int(self.iterations), _ffi.stream_ptr()))
+            self._n_slots = 2
         else:
             _ffi.check(_ffi.lib().ssdk_train_apply(self.handle, self.lr, self.momentum, self.l2, float(grad_scale), _ffi.stream_ptr()))
 
@@ -219,6 +245,63 @@ class SSDTrainer:
                 o, c = self.spans()[(s.name, 'gamma')]
                 res[s.name + '/gamma'] = flat[o:o + c].copy()
         return res
+
+    def _flatten(self, named):
+        """The inverse of ``_unflatten``: dict with Keras names / layouts -> flat float32 ndarray in the gradient's layout."""
+        m = self.model
+        flat = np.empty((self.n_params,), np.float32)
+        sp = self.spans()
+
+        def put(key, a):
+            o, c = sp[key]
+            flat[o:o + c] = np.asarray(a, np.float32).reshape(-1)
+
+        def ohwi(k):
+            return np.asarray(k, np.float32).transpose(3, 0, 1, 2)
+        for s in m.specs:
+            if s.op == _ffi.OP_CONV:
+                put((s.name, 'kernel'), ohwi(named[s.name + '/kernel']))
+                put((s.name, 'bias'), named[s.name + '/bias'])
+                if s.bn and (s.name, 'bn_gamma') in sp:
+                    put((s.name, 'bn_gamma'), named[s.bn + '/gamma'])
+                    put((s.name, 'bn_beta'), named[s.bn + '/beta'])
+            elif s.op == _ffi.OP_HEAD:
+                nb, cn, ln = s.n_boxes, s.params['conf_name'], s.params['loc_name']
+                conf, loc = ohwi(named[cn + '/kernel']), ohwi(named[ln + '/kernel'])
+                put((s.name, 'kernel'), np.concatenate([conf.reshape(nb, -1), loc.reshape(nb, -1)], axis=1))
+                put((s.name, 'bias'), np.concatenate([np.reshape(named[cn + '/bias'], (nb, -1)), np.reshape(named[ln + '/bias'], (nb, -1))], axis=1))
+            elif s.op == _ffi.OP_L2NORM:
+                put((s.name, 'gamma'), named[s.name + '/gamma'])
+        return flat
+
+    # -- optimiser state (resuming a run from a full-model checkpoint) ---------------------------------
+    def get_optimizer_state(self):
+        """``{'iterations': int, 'slots': [dict, ...]}``: the step count and every optimiser slot that exists (SGD: the velocity;
+        Adam: m, then v once an update has made it), each with Keras' weight names and layouts like :meth:`get_weights`."""
+        import torch
+        self._attach()
+        out = torch.empty_like(self.grad)
+        slots = []
+        for slot in range(self._n_slots):
+            _ffi.check(_ffi.lib().ssdk_trainer_read_opt_state(self.handle, slot, _ffi.dptr(out), _ffi.stream_ptr()))
+            slots.append(self._unflatten(out.cpu().numpy()))
+        return {'iterations': int(self.iterations), 'slots': slots}
+
+    def set_optimizer_state(self, state):
+        """Overwrite the optimiser state with ``state`` as :meth:`get_optimizer_state` returns it (checked first by
+        :func:`check_optimizer_state`); the next update continues from it, bit for bit.  The state does not depend on the batch
+        size, so it may come from a trainer built for another one."""
+        import torch
+        check_optimizer_state(self.model, self.optimizer, state)
+        self._attach()
+        slots = list(state['slots'])
+        if len(slots) < self._n_slots:               # an Adam state from before its first update: v is zero again
+            slots.append({k: np.zeros_like(v) for k, v in slots[0].items()})
+        for slot, named in enumerate(slots):
+            src = torch.from_numpy(self._flatten(named)).cuda()
+            _ffi.check(_ffi.lib().ssdk_trainer_write_opt_state(self.handle, slot, _ffi.dptr(src), _ffi.stream_ptr()))
+        self._n_slots = len(slots)
+        self.iterations = int(state['iterations'])
 
     def gradients(self):
         return self._unflatten(self.grad.cpu().numpy())
