@@ -557,7 +557,9 @@ enum ssdk_plan_kernel {
   SSDK_PLAN_GEMM = 1,          /* conv_wgmma_kernel on the zero-bordered activation (implicit GEMM) */
   SSDK_PLAN_IM2COL_GEMM = 2,   /* im2col_kernel / im2col8_kernel, then conv_wgmma_kernel on the column matrix */
   SSDK_PLAN_FIRST_TC = 3,      /* conv_first_kernel: image-facing layer, gathered A tile, tensor cores */
-  SSDK_PLAN_DIRECT = 4         /* conv_direct_kernel: fp32 FMAs on the float32 master kernel */
+  SSDK_PLAN_DIRECT = 4,        /* conv_direct_kernel: fp32 FMAs on the float32 master kernel */
+  SSDK_PLAN_GEMM_SWAP = 5      /* conv_swap_kernel: implicit GEMM of a forward conv with <= 64 output channels on a large map,
+                                  weights on the wgmma M side, 192-pixel tiles */
 };
 enum ssdk_plan_epilogue { SSDK_PLAN_EPI_SPLIT = 0, SSDK_PLAN_EPI_F32 = 1, SSDK_PLAN_EPI_ATOMIC = 2, SSDK_PLAN_EPI_HEAD = 3 };
 typedef struct ssdk_layer_plan {
@@ -566,12 +568,13 @@ typedef struct ssdk_layer_plan {
   int split;                   /* 1: bf16x3 (hi*hi + hi*lo + lo*hi), 0: one bf16 product */
   int stages;                  /* TMA ring depth (GEMM) */
   int kblocks;                 /* 64-wide K blocks per tap (GEMM: of the input channels or of the im2col row; FIRST_TC: of taps*4) */
-  int n_tiles_m, n_tiles_n;    /* scheduled 128-row m-tiles and BN-wide n-tiles */
+  int n_tiles_m, n_tiles_n;    /* scheduled bm-row m-tiles and BN-wide n-tiles */
   int grid;                    /* CTAs of the (persistent) launch */
   int k_split;                 /* work units per tile along K */
   int epilogue;                /* ssdk_plan_epilogue, of GEMM launches */
   int head_fused;              /* 1: softmax / anchors / variances in the GEMM epilogue, straight into y_pred */
   int im2col_vec8;             /* IM2COL_GEMM: 1 = im2col8_kernel (8 channels per thread), 0 = im2col_kernel */
+  int bm;                      /* output rows (pixels) per tile: 192 (GEMM_SWAP) or 128 (the other tensor-core kernels) */
 } ssdk_layer_plan;
 int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_plan* out);
 

@@ -106,7 +106,7 @@ class ModelDesc(C.Structure):
 
 class LayerPlan(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('kernel', 'bn', 'split', 'stages', 'kblocks', 'n_tiles_m', 'n_tiles_n', 'grid', 'k_split',
-                                       'epilogue', 'head_fused', 'im2col_vec8')]
+                                       'epilogue', 'head_fused', 'im2col_vec8', 'bm')]
 
 
 class BackwardPlan(C.Structure):
@@ -115,7 +115,7 @@ class BackwardPlan(C.Structure):
                                        'n_gemms', 'stages', 'grid', 'kv', 'direct_fast')]
 
 
-PLAN_KERNELS = {0: None, 1: 'gemm', 2: 'im2col_gemm', 3: 'first_tc', 4: 'direct'}
+PLAN_KERNELS = {0: None, 1: 'gemm', 2: 'im2col_gemm', 3: 'first_tc', 4: 'direct', 5: 'gemm_swap'}
 PLAN_EPILOGUES = {0: 'split', 1: 'f32', 2: 'atomic', 3: 'head'}
 DGRAD_PATHS = {0: None, 1: 'gemm', 2: 'strided'}
 WGRAD_PATHS = {0: None, 1: 'native', 2: 'transposed', 3: 'im2col', 4: 'direct'}

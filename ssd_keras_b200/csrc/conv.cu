@@ -85,17 +85,29 @@ static constexpr int kATile = kBM * kBK * 2;   // 16 KB
 static constexpr int kAccPad = 4;        // the fp32 accumulator tile in shared memory has rows of BN + 4 floats (conflict-free reads)
 static constexpr int kParBytes = 3 * 256 * (int)sizeof(float);   // bias | bn scale | bn shift of one n-tile
 
-static size_t stage_bytes(const ConvArgs& a) { return ((size_t)kATile + (size_t)a.BN * kBK * 2) * (a.split ? 2 : 1); }
+// conv_swap_kernel: 192 pixels (96 per consumer warpgroup) x 64 output channels per tile, and its own epilogue staging tile after
+// the ring: per consumer warpgroup [48 pixels][64 + kAccPad channels] of fp32 (its 96 pixels in two passes)
+static constexpr int kSwapN = 96;
+static constexpr int kSwapNP = 48;
+static constexpr int kSwapBM = 2 * kSwapN;
+static constexpr int kSwapPitch = 64 + kAccPad;
+static constexpr int kSwapStaging = 2 * kSwapNP * kSwapPitch * (int)sizeof(float);
+
+int conv_swap_bm() { return kSwapBM; }
+static size_t stage_bytes(const ConvArgs& a, int bm) { return ((size_t)bm * kBK * 2 + (size_t)a.BN * kBK * 2) * (a.split ? 2 : 1); }
 // (+32 floats: the 32-column chunk reads of the epilogue may run past the end of a row whose width is not a multiple of 64)
 static size_t acc_tile_bytes(int BN) { return ((size_t)kBM * (BN + kAccPad) + 32) * sizeof(float); }
-static size_t ring_bytes(const ConvArgs& a) { return std::max(stage_bytes(a) * a.stages, acc_tile_bytes(a.BN)); }
-size_t conv_smem_bytes(const ConvArgs& a) { return 1024 + ring_bytes(a) + 256 + kParBytes; }
+static size_t ring_bytes(const ConvArgs& a) { return std::max(stage_bytes(a, kBM) * a.stages, acc_tile_bytes(a.BN)); }
+size_t conv_smem_bytes(const ConvArgs& a, int bm) {
+  if (bm == kSwapBM) return 1024 + stage_bytes(a, bm) * a.stages + kSwapStaging + 256;
+  return 1024 + ring_bytes(a) + 256 + kParBytes;
+}
 // As many ring stages ({A_hi, A_lo, W_hi, W_lo} per k-iteration) as shared memory holds, 2 ... 6.
-void conv_pick_stages(ConvArgs& a) {
+void conv_pick_stages(ConvArgs& a, int bm) {
   a.stages = 2;
   while (a.stages < 6) {
     ++a.stages;
-    if (conv_smem_bytes(a) > 227 * 1024) { --a.stages; break; }
+    if (conv_smem_bytes(a, bm) > 227 * 1024) { --a.stages; break; }
   }
 }
 
@@ -247,6 +259,53 @@ __device__ __forceinline__ bool decode_vrow(const ConvArgs& args, int v, int& n,
   return valid;
 }
 
+// work unit t -> output rows [m0, m0 + BM), columns [n0, n0 + BN), k-blocks [kb0, kb0 + nkb), nk = taps * nkb k-iterations
+template <int BM, int BN>
+__device__ __forceinline__ void conv_unit(const ConvArgs& args, int KS, int t, int& m0, int& n0, int& kb0, int& nkb) {
+  const int tt = t / KS, ks = t - tt * KS;
+  m0 = args.tile_list[tt / args.n_tiles_n] * BM;
+  n0 = (tt % args.n_tiles_n) * BN;
+  kb0 = KS > 1 ? ks * args.kb_per : 0;
+  const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
+  nkb = kb1 - kb0;
+}
+
+// The TMA producer thread: walks the tile schedule and keeps the ring full across tile boundaries.  A stage is
+// A_hi | A_lo | W_hi | W_lo (BM activation rows, BN weight rows, 64 channels each); `staged`: before each tile after the first,
+// wait until the consumers have read the previous tile's epilogue staged over the ring.
+template <int BM, int BN, bool SPLIT>
+__device__ __forceinline__ void conv_produce(const CUtensorMap* tm_a_hi, const CUtensorMap* tm_a_lo, const CUtensorMap* tm_b_hi,
+                                             const CUtensorMap* tm_b_lo, const ConvArgs& args, const MbarRing& bars, uint32_t smem_base,
+                                             int KS, int total_tiles, bool staged, uint32_t staged_free) {
+  constexpr uint32_t kATileB = (uint32_t)BM * kBK * 2, kBTile = (uint32_t)BN * kBK * 2;
+  constexpr uint32_t b_off = kATileB * (SPLIT ? 2u : 1u);
+  constexpr uint32_t stage = b_off + kBTile * (SPLIT ? 2u : 1u);
+  uint32_t g = 0;                                                          // ring uses so far (slot = g % S, phase = g / S)
+  uint32_t lt = 0;                                                         // tiles of this CTA so far
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
+    int m0, n0, kb0, nkb;
+    conv_unit<BM, BN>(args, KS, t, m0, n0, kb0, nkb);
+    const int nk = args.KH * args.KW * nkb;
+    if (staged && lt > 0) mbar_wait(staged_free, (lt - 1) & 1u);
+    // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +BM) of the activation matrix
+    for (int i = 0; i < nk; ++i) {
+      const uint32_t s = bars.wait_empty(g + (uint32_t)i);
+      const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
+      const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
+      const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
+      const uint32_t dst = smem_base + stage * s;
+      mbar_expect_tx(bars.full(s), stage);
+      tma_load_2d(dst, tm_a_hi, kb * kBK, row, bars.full(s));
+      tma_load_2d(dst + b_off, tm_b_hi, kcol, n0, bars.full(s));
+      if (SPLIT) {
+        tma_load_2d(dst + kATileB, tm_a_lo, kb * kBK, row, bars.full(s));
+        tma_load_2d(dst + b_off + kBTile, tm_b_lo, kcol, n0, bars.full(s));
+      }
+    }
+    g += (uint32_t)nk;
+  }
+}
+
 template <int BN, bool SPLIT>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -283,44 +342,11 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
 
   const int KS = args.k_split > 1 ? args.k_split : 1;
   const int total_tiles = args.n_tiles_m * args.n_tiles_n * KS;
-  // work unit t -> output rows [m0, m0 + 128), columns [n0, n0 + BN), k-blocks [kb0, kb0 + nkb), nk = taps * nkb k-iterations
-  auto unit = [&](int t, int& m0, int& n0, int& kb0, int& nkb) {
-    const int tt = t / KS, ks = t - tt * KS;
-    m0 = args.tile_list[tt / args.n_tiles_n] * kBM;
-    n0 = (tt % args.n_tiles_n) * BN;
-    kb0 = KS > 1 ? ks * args.kb_per : 0;
-    const int kb1 = KS > 1 ? min(args.kblocks, kb0 + args.kb_per) : args.kblocks;
-    nkb = kb1 - kb0;
-  };
 
   if (wg == 0) {
-    // ===================== producer: one thread walks the tile schedule and keeps the ring full across tile boundaries =====
     setmaxnreg_dec<40>();
     if (tid != 0) return;
-    uint32_t g = 0;                                                        // ring uses so far (slot = g % S, phase = g / S)
-    uint32_t lt = 0;                                                       // tiles of this CTA so far
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++lt) {
-      int m0, n0, kb0, nkb;
-      unit(t, m0, n0, kb0, nkb);
-      const int nk = args.KH * args.KW * nkb;
-      if (staged && lt > 0) mbar_wait(staged_free, (lt - 1) & 1u);
-      // k-iteration i = (tap, k-block): the A tile of tap (kh, kw) is rows [m0 + shift(kh, kw), +128) of the activation matrix
-      for (int i = 0; i < nk; ++i) {
-        const uint32_t s = bars.wait_empty(g + (uint32_t)i);
-        const int tap = i / nkb, kb = kb0 + (i - tap * nkb), kh = tap / args.KW, kw = tap - kh * args.KW;
-        const int row = m0 + args.row_shift[kh] + kw * args.kw_rows;
-        const int kcol = (tap * args.kblocks + kb) * kBK + args.b_k_offset;
-        const uint32_t dst = smem_base + stage * s;
-        mbar_expect_tx(bars.full(s), stage);
-        tma_load_2d(dst, &tm_a_hi, kb * kBK, row, bars.full(s));
-        tma_load_2d(dst + b_off, &tm_b_hi, kcol, n0, bars.full(s));
-        if (split) {
-          tma_load_2d(dst + kATile, &tm_a_lo, kb * kBK, row, bars.full(s));
-          tma_load_2d(dst + b_off + kBTile, &tm_b_lo, kcol, n0, bars.full(s));
-        }
-      }
-      g += (uint32_t)nk;
-    }
+    conv_produce<kBM, BN, SPLIT>(&tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, args, bars, smem_base, KS, total_tiles, staged, staged_free);
     return;
   }
 
@@ -331,7 +357,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   float acc[BN / 2], accx[split ? BN / 2 : 1];
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     int m0, n0, kb0, nkb;
-    unit(t, m0, n0, kb0, nkb);
+    conv_unit<kBM, BN>(args, KS, t, m0, n0, kb0, nkb);
     const int nk = args.KH * args.KW * nkb;
     if (staged)
       for (int i = ctid; i < BN; i += 256) {
@@ -464,12 +490,155 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_cons
   }
 }
 
+// conv_swap_kernel -- the forward convolutions with at most 64 output channels on large maps (conv1_2 of the VGG trunk), with the
+// wgmma operands swapped:  D^T[M = 64 output channels, N = 96 pixels] per consumer warpgroup.  The weight tile is the A operand,
+// the warpgroup's half of a 192-row activation tile the B operand; both are the same K-major 128B-swizzled tiles the TMA loads
+// for conv_wgmma_kernel, only their descriptors change roles.  Same producer, ring, k-iteration schedule and products (in the
+// same order) as conv_wgmma_kernel.  Why 192 pixels: with 9 short k-iterations per tile these layers are bound by the bytes the
+// TMA ring has in flight from L2, and 64 KB stages (3 in 227 KB, next to the staging tile) keep 128 KB in flight where 256-pixel
+// stages of 80 KB fit only twice (80 KB); the tile still shares each weight tile between both warpgroups.
+// Epilogue (EPI_SPLIT only, no ReLU' mask or accumulation): each warpgroup stages its accumulators transposed into its own
+// shared-memory tile, 64 pixels at a time, and finishes 8 channels of one pixel per thread with epi_split8.  The staging tile is
+// not part of the ring, so the producer fills the next tile's stages while the consumers store.
+template <bool SPLIT>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_swap_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
+                 const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
+                 const __grid_constant__ ConvArgs args) {
+  extern __shared__ unsigned char smem_dyn[];
+  const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
+  unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
+  const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+  constexpr bool split = SPLIT;
+  const int S = args.stages;
+  constexpr uint32_t kPTile = (uint32_t)kSwapBM * kBK * 2, kWTile = 64u * kBK * 2;
+  constexpr int NP = kSwapNP, JP = NP / 8;                                // pixels and 8-pixel column blocks per epilogue pass
+  static_assert(kSwapN % NP == 0 && NP % 8 == 0, "the epilogue passes cover the warpgroup's pixels in 8-pixel blocks");
+  constexpr uint32_t w_off = kPTile * (split ? 2u : 1u);                   // stage: P_hi | P_lo | W_hi | W_lo
+  constexpr uint32_t stage = w_off + kWTile * (split ? 2u : 1u);
+  const uint32_t ring = stage * (uint32_t)S;
+  const MbarRing bars{smem_base + ring + (uint32_t)kSwapStaging, S};
+  const int total_tiles = args.n_tiles_m;
+
+  if (tid == 0) {
+    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_b_hi);
+    if (split) { prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_lo); }
+    bars.init(1, 8);                                                       // empty: one arrival per consumer warp
+    mbar_init_fence();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (tid != 0) return;
+    conv_produce<kSwapBM, 64, SPLIT>(&tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, args, bars, smem_base, 1, total_tiles, false, 0u);
+    return;
+  }
+
+  // ===================== consumers: warpgroup cw computes pixels [kSwapN cw, +kSwapN) of every tile =====================
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1, wtid = tid & 127, cwarp = (tid >> 5) & 3;
+  float* s_t = reinterpret_cast<float*>(smem_al + ring) + cw * NP * kSwapPitch;   // [NP pixels][kSwapPitch]
+  auto wg_sync = [&]() { if (cw == 0) named_bar_sync<2, 128>(); else named_bar_sync<3, 128>(); };
+  // epilogue: this thread's channel group [8 cg, +8), and its parameters
+  const int cg = wtid & 7;
+  const bool store_group = 8 * cg < args.cout;
+  float sb[8], ss[8], sh[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int col = 8 * cg + e;
+    const bool in = col < args.cout;
+    sb[e] = (args.bias && in) ? __ldg(args.bias + col) : 0.f;
+    ss[e] = (args.bn_scale && in) ? __ldg(args.bn_scale + col) : 0.f;
+    sh[e] = (args.bn_scale && in) ? __ldg(args.bn_shift + col) : 0.f;
+  }
+  uint32_t g = 0;
+  float acc[kSwapN / 2], accx[split ? kSwapN / 2 : 1];
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    int m0, n0, kb0, nkb;
+    conv_unit<kSwapBM, 64>(args, 1, t, m0, n0, kb0, nkb);
+    const int nk = args.KH * args.KW * nkb;
+    auto release = [&](int j) {
+      __syncwarp();
+      if (lane == 0) bars.release(g + (uint32_t)j);
+    };
+#pragma unroll
+    for (int j = 0; j < kSwapN / 2; ++j) acc[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (split ? kSwapN / 2 : 1); ++j) accx[j] = 0.f;
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(accx);
+    for (int i = 0; i < nk; ++i) {
+      const uint32_t s = bars.wait_full(g + (uint32_t)i);
+      const uint32_t p_hi = smem_base + stage * s + (uint32_t)cw * (kPTile / 2), w_hi = smem_base + stage * s + w_off;
+      constexpr uint64_t kDesc = wgmma_desc_hi(16);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t sc = (i | k) ? 1u : 0u;
+        const uint64_t dw = wgmma_desc(kDesc, w_hi + 32u * k), dp = wgmma_desc(kDesc, p_hi + 32u * k);
+        Wgmma<kSwapN, 0, 0>::mma(acc, dw, dp, sc);
+        if constexpr (split) {
+          Wgmma<kSwapN, 0, 0>::mma(accx, wgmma_desc(kDesc, w_hi + kWTile + 32u * k), dp, sc);           // hi * lo
+          Wgmma<kSwapN, 0, 0>::mma(accx, dw, wgmma_desc(kDesc, p_hi + kPTile + 32u * k), 1u);          // lo * hi
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (i > 0) release(i - 1);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    wgmma_fence_acc(accx);
+    if (nk > 0) release(nk - 1);
+    g += (uint32_t)nk;
+    if constexpr (split) {
+#pragma unroll
+      for (int j = 0; j < kSwapN / 2; ++j) acc[j] += accx[j];
+    }
+
+    // ===================== epilogue: NP pixels per pass through the staging tile =====================
+    // acc[4j + 2h + e] is channel 16 cwarp + lane / 4 + 8h of pixel 8j + 2 (lane % 4) + e
+    const int ch = cwarp * 16 + (lane >> 2), pc = 2 * (lane & 3);
+#pragma unroll
+    for (int ph = 0; ph < kSwapN / NP; ++ph) {
+#pragma unroll
+      for (int j = 0; j < JP; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) s_t[(8 * j + pc + e) * kSwapPitch + ch + 8 * h] = acc[4 * (JP * ph + j) + 2 * h + e];
+      wg_sync();
+#pragma unroll
+      for (int r = 0; r < (NP + 15) / 16; ++r) {
+        const int p = (wtid >> 3) + 16 * r;
+        if (NP % 16 != 0 && p >= NP) break;
+        int n, y, x;
+        const bool valid = decode_vrow(args, m0 + cw * kSwapN + ph * NP + p, n, y, x);
+        float vr[8];
+        ld_f8(s_t + p * kSwapPitch + 8 * cg, vr);
+        if (valid && store_group) {
+          const size_t o = (((size_t)n * args.out_Hp + (y + args.out_pad)) * args.out_Wp + (x + args.out_pad)) * args.out_Cs + 8 * cg;
+          epi_split8<false>(args, vr, o, sb, ss, sh);
+        }
+      }
+      wg_sync();
+    }
+  }
+}
+
 int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int grid_cap) {
   // the kernel is persistent with a static stride over its work units: any grid size computes the same result
   const int grid = grid_cap > 0 ? std::max(1, std::min(L.grid, grid_cap)) : L.grid;
   const bool split = L.args.split != 0;
   SSDK_REQUIRE(split || L.args.BN != 160, "internal: 160-wide conv tiles are for bf16x3 predictor heads");
   decltype(&conv_wgmma_kernel<64, false>) kernel;
+  if (L.bm == kSwapBM) {
+    SSDK_REQUIRE(L.args.BN == 64 && L.args.epi == EPI_SPLIT && !L.args.mask_hi && !L.args.accumulate && L.args.k_split <= 1,
+                 "internal: %d-pixel conv tiles are for 64-channel forward convolutions", kSwapBM);
+    kernel = split ? conv_swap_kernel<true> : conv_swap_kernel<false>;
+    return launch(ctx, kernel, grid, kConvThreads, L.smem, stream, L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.args);
+  }
   switch (L.args.BN) {
     case 64: kernel = split ? conv_wgmma_kernel<64, true> : conv_wgmma_kernel<64, false>; break;
     case 128: kernel = split ? conv_wgmma_kernel<128, true> : conv_wgmma_kernel<128, false>; break;

@@ -150,6 +150,7 @@ struct ConvArgs {
 struct ConvLaunch {
   CUtensorMap a_hi, a_lo, b_hi, b_lo;
   ConvArgs args;
+  int bm;               // output rows (pixels) per tile: 128 (conv_wgmma_kernel) or conv_swap_bm() (conv_swap_kernel)
   int grid;
   size_t smem;
   double flops_algo, flops_issued;
@@ -160,8 +161,9 @@ int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t inner, uint64_t ro
                  uint32_t box_inner, uint32_t box_rows);
 // 4-D map over a bf16 NHWC tensor, dims / box innermost first (channels, x, y, image); 128B swizzle, zero fill
 int make_tmap_4d(CUtensorMap* out, const void* base, const uint64_t dims[4], const uint32_t box[4]);
-size_t conv_smem_bytes(const ConvArgs& a);
-void conv_pick_stages(ConvArgs& a);
+int conv_swap_bm();    // pixels per tile of conv_swap_kernel (the weights on the wgmma M side, SSDK_PLAN_GEMM_SWAP)
+size_t conv_smem_bytes(const ConvArgs& a, int bm);    // bm: output rows per tile (ConvLaunch::bm)
+void conv_pick_stages(ConvArgs& a, int bm);
 int launch_conv(ssdk_ctx* ctx, const ConvLaunch& L, cudaStream_t stream, int grid_cap = 0);   // grid_cap > 0: at most that many CTAs
 
 // elementwise / data movement kernels

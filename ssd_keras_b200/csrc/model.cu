@@ -31,7 +31,8 @@ void fused_master(const ssdk_layer_desc& d, int cin, int cout, int Ctot, std::ve
 struct CudaFree { void operator()(void* p) const { cudaFree(p); } };
 
 // The forward kernel of a convolution or head: every reader of the plan switches on it, and pass 2 sizes the borders from it.
-ssdk_plan_kernel conv_kernel(const ssdk_layer_desc& d, int cin, int cout, bool training) {
+// `pixels`: B * Ho * Wo output pixels.
+ssdk_plan_kernel conv_kernel(const ssdk_layer_desc& d, int cin, int cout, bool training, long long pixels, int sm_count) {
   const int taps = d.kh * d.kw;
   // the image-facing layer: 1 ... 4 input channels (one stored 8-channel group), an fp32 [K][Cout] kernel within 96 KB
   const bool direct = d.op != SSDK_OP_HEAD && cin >= 1 && cin <= 4 && d.stride == 1 && cout % 16 == 0 && (size_t)taps * cin * cout * 4 <= 96 * 1024;
@@ -42,6 +43,11 @@ ssdk_plan_kernel conv_kernel(const ssdk_layer_desc& d, int cin, int cout, bool t
     return SSDK_PLAN_DIRECT;
   }
   if (d.stride != 1 || cin < 8) return SSDK_PLAN_IM2COL_GEMM;
+  // at most 64 output channels from at least 64 input channels on a large map (conv1_2 of the VGG trunk): 64-wide tiles run at
+  // a fraction of the tensor rate of the wider ones, so the 64 channels go on the wgmma M side and conv_swap_bm() pixels on N
+  // (conv_swap_kernel).  Only where every SM gets at least two such tiles: a tile with a valid pixel holds at most
+  // conv_swap_bm() of them, so `pixels` >= 2 * sm_count * conv_swap_bm() guarantees that many tiles.
+  if (d.op == SSDK_OP_CONV && cout <= 64 && cin >= 64 && pixels >= 2ll * sm_count * conv_swap_bm()) return SSDK_PLAN_GEMM_SWAP;
   return SSDK_PLAN_GEMM;
 }
 
@@ -113,6 +119,7 @@ int build_conv(ssdk_model* m, int li) {
   } else {
     kblocks = (ia.Cs + 63) / 64;
     g.in = &ia; g.kh = d.kh; g.kw = d.kw; g.dilation = d.dilation; g.pad_t = d.pad_t; g.pad_l = d.pad_l;
+    g.swap = L.kernel == SSDK_PLAN_GEMM_SWAP;
     SSDK_REQUIRE(ia.pad >= std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)), "internal: activation border too small");
   }
   L.kblocks = kblocks;
@@ -292,12 +299,14 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   a.kblocks = kblocks;
   a.Ho = g.Ho; a.Wo = g.Wo; a.B = g.B;
   a.cout = g.cout;
+  const int BM = g.swap ? conv_swap_bm() : 128;
+  cl.bm = BM;
   // m-tiles that hold at least one valid output row
   std::vector<int> tiles;
-  for (int t = 0; t < (a.M_total + 127) / 128; ++t) {
+  for (int t = 0; t < (a.M_total + BM - 1) / BM; ++t) {
     bool any = false;
-    for (int r = 0; r < 128 && !any; ++r) {
-      long long v = (long long)t * 128 + r;
+    for (int r = 0; r < BM && !any; ++r) {
+      long long v = (long long)t * BM + r;
       if (v >= a.M_total) break;
       int rr = (int)(v % a.rows_per_img);
       any = (rr / a.in_Wp < g.Ho) && (rr % a.in_Wp < g.Wo);
@@ -324,7 +333,7 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
     if (use128) a.BN = 128;
   }
   a.n_tiles_n = (g.cout + a.BN - 1) / a.BN;
-  conv_pick_stages(a);
+  conv_pick_stages(a, BM);
   a.n_tiles_m = (int)tiles.size();
   int* tl = nullptr;
   int rc = dev_alloc(m->allocs, &tl, tiles.size(), false); if (rc) return rc;
@@ -332,21 +341,21 @@ int plan_conv_gemm(ssdk_model* m, ConvLaunch& cl, const ConvGeom& g, const __nv_
   a.tile_list = tl;
   if (tile_list_out) *tile_list_out = tl;
   const uint64_t a_ld = (!g.in && g.a_ld) ? g.a_ld : a_inner;
-  rc = make_tmap_2d(&cl.a_hi, a_hi, a_inner, a_rows, a_ld * 2, 64, 128); if (rc) return rc;
+  rc = make_tmap_2d(&cl.a_hi, a_hi, a_inner, a_rows, a_ld * 2, 64, (uint32_t)BM); if (rc) return rc;
   rc = make_tmap_2d(&cl.b_hi, w_hi, krow, (uint64_t)g.cout, krow * 2, 64, (uint32_t)a.BN); if (rc) return rc;
   if (m->split) {
-    rc = make_tmap_2d(&cl.a_lo, a_lo, a_inner, a_rows, a_ld * 2, 64, 128); if (rc) return rc;
+    rc = make_tmap_2d(&cl.a_lo, a_lo, a_inner, a_rows, a_ld * 2, 64, (uint32_t)BM); if (rc) return rc;
     rc = make_tmap_2d(&cl.b_lo, w_lo, krow, (uint64_t)g.cout, krow * 2, 64, (uint32_t)a.BN); if (rc) return rc;
   } else { cl.a_lo = cl.a_hi; cl.b_lo = cl.b_hi; }
   const int total_tiles = a.n_tiles_m * a.n_tiles_n;
   cl.grid = std::max(1, std::min(total_tiles, m->ctx->sm_count));
-  cl.smem = conv_smem_bytes(a);
+  cl.smem = conv_smem_bytes(a, BM);
   SSDK_REQUIRE(cl.smem <= 227 * 1024, "internal: conv plan needs %zu bytes of shared memory", cl.smem);
   double issued = 0;
   for (int nt = 0; nt < a.n_tiles_n; ++nt) {
     // every tile issues the full BN columns (the weight rows past cout are TMA zero fill) and all 64 channels of every k-block,
     // 3 products with split planes
-    issued += 2.0 * a.n_tiles_m * 128.0 * a.BN * (m->split ? 3.0 : 1.0) * (double)(a.KH * a.KW) * (kblocks * 64);
+    issued += 2.0 * a.n_tiles_m * (double)BM * a.BN * (m->split ? 3.0 : 1.0) * (double)(a.KH * a.KW) * (kblocks * 64);
   }
   cl.flops_issued = issued;
   return SSDK_OK;
@@ -406,16 +415,16 @@ extern "C" int ssdk_model_create(ssdk_ctx* ctx, const ssdk_model_desc* desc, ssd
     const ssdk_layer_desc& d = L.d;
     if (d.op != SSDK_OP_CONV && d.op != SSDK_OP_HEAD) continue;
     LayerPlan& in = m->layers[d.input];
-    L.kernel = conv_kernel(d, in.C, L.C, m->training);
+    L.kernel = conv_kernel(d, in.C, L.C, m->training, (long long)m->B * L.H * L.W, m->ctx->sm_count);
     // the implicit GEMM and the gathered A tile (conv_first_kernel) read their taps from the input planes' zero border
-    if (L.kernel == SSDK_PLAN_GEMM) in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)));
+    if (implicit_gemm(L.kernel)) in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_b), std::max(d.pad_l, d.pad_r)));
     if (L.kernel == SSDK_PLAN_FIRST_TC)
       in.need_pad = std::max(in.need_pad, std::max(std::max(d.pad_t, d.pad_l),
                                                    std::max((d.kh - 1) * d.dilation - d.pad_t, (d.kw - 1) * d.dilation - d.pad_l)));
     // training: the image-facing weight-gradient kernel reads its 3x3 window without bounds checks
     if (m->training && L.kernel == SSDK_PLAN_DIRECT)
       in.need_pad = std::max(in.need_pad, d.dilation * std::max(d.kh - 1, d.kw - 1));
-    if (m->training && L.kernel == SSDK_PLAN_GEMM) {
+    if (m->training && implicit_gemm(L.kernel)) {
       // the gradient of this layer's output shares the geometry of the output itself and is the input of the
       // data-gradient convolution, whose padding is dilation*(k-1) - pad
       const int pt = d.dilation * (d.kh - 1) - d.pad_t, pb = d.dilation * (d.kh - 1) - d.pad_b;
@@ -491,6 +500,7 @@ extern "C" int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_
     out->bn = L.first.BN; out->split = m->split; out->kblocks = L.first.kblocks;
     out->n_tiles_m = L.first.n_tiles; out->n_tiles_n = 1;
     out->grid = L.first.grid; out->k_split = 1;
+    out->bm = 128;
     return SSDK_OK;
   }
   const ConvArgs& a = L.launch.args;
@@ -498,6 +508,7 @@ extern "C" int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_
   out->n_tiles_m = a.n_tiles_m; out->n_tiles_n = a.n_tiles_n; out->grid = L.launch.grid; out->k_split = a.k_split > 1 ? a.k_split : 1;
   out->epilogue = a.epi; out->head_fused = L.head_fused ? 1 : 0;
   out->im2col_vec8 = L.im2col_vec8 ? 1 : 0;
+  out->bm = L.launch.bm;
   return SSDK_OK;
 }
 
@@ -530,7 +541,7 @@ extern "C" int ssdk_model_layer_ms(const ssdk_model* m, int layer, float* out_ms
   SSDK_REQUIRE(m && out_ms && layer >= 0 && layer < (int)m->layers.size(), "ssdk_model_layer_ms: bad argument");
   const LayerPlan& L = m->layers[layer];
   *out_ms = 0.f;
-  if (L.kernel != SSDK_PLAN_GEMM && L.kernel != SSDK_PLAN_IM2COL_GEMM) return SSDK_OK;
+  if (!implicit_gemm(L.kernel) && L.kernel != SSDK_PLAN_IM2COL_GEMM) return SSDK_OK;
   SSDK_CHECK_CUDA(cudaEventSynchronize(L.ev1));
   SSDK_CHECK_CUDA(cudaEventElapsedTime(out_ms, L.ev0, L.ev1));
   return SSDK_OK;

@@ -40,6 +40,9 @@ struct LayerPlan {
   float bn_eps = 1e-3f, bn_momentum = 0.99f;
 };
 
+// the forward kernels that run the implicit GEMM on the zero-bordered input (conv_wgmma_kernel, conv_swap_kernel)
+inline bool implicit_gemm(ssdk_plan_kernel k) { return k == SSDK_PLAN_GEMM || k == SSDK_PLAN_GEMM_SWAP; }
+
 }  // namespace ssdk
 
 struct ssdk_model {
@@ -108,6 +111,7 @@ struct ConvGeom {
   int kh = 1, kw = 1, dilation = 1, pad_t = 0, pad_l = 0;
   int Ho = 0, Wo = 0, B = 0;
   int cout = 0;
+  bool swap = false;                    // conv_swap_kernel: 256-pixel tiles, weights on the wgmma M side (SSDK_PLAN_GEMM_SWAP)
 };
 // BatchNormalization (training phase) + activation: z -> out with batch statistics; and its backward on the gradient planes
 int launch_bn_forward(ssdk_ctx* ctx, LayerPlan& L, int act, cudaStream_t s);

@@ -449,8 +449,8 @@ int repack_layer(ssdk_trainer* t, int i, cudaStream_t s) {
   const TLayer& T = t->tl[i];
   const LayerPlan& L = m->layers[i];
   int rc;
-  if (L.kernel == SSDK_PLAN_GEMM || L.kernel == SSDK_PLAN_IM2COL_GEMM) {
-    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, L.kernel == SSDK_PLAN_GEMM ? PACK_FWD : PACK_FWD_IM2COL, L.kblocks, L.w_krow,
+  if (implicit_gemm(L.kernel) || L.kernel == SSDK_PLAN_IM2COL_GEMM) {
+    rc = launch_repack(m->ctx, L.w_f32, T.taps, T.cin, T.cout, implicit_gemm(L.kernel) ? PACK_FWD : PACK_FWD_IM2COL, L.kblocks, L.w_krow,
                        L.w_hi, L.w_lo, s);
     if (rc) return rc;
   }
@@ -573,7 +573,7 @@ int plan_wgrad_layer(ssdk_trainer* t, int i, long long& max_xT, long long& max_d
   const ActBuf& X = m->layers[d.input].out;
   int transposed;
   if (int rc = env_int("SSDK_WGRAD_TRANSPOSED", 0, &transposed)) return rc;
-  if (L.kernel == SSDK_PLAN_GEMM && !transposed && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
+  if (implicit_gemm(L.kernel) && !transposed && wgrad_supported(X, T.g, d.kh, d.kw, d.stride, d.dilation)) {
     T.wgrad_path = SSDK_WGRAD_NATIVE;
     return plan_wgrad(m->ctx, T.wg, X, T.g, L.H, L.W, d.kh, d.kw, d.dilation, d.pad_t, d.pad_l, m->split, span_grad(t, i, 0));
   }

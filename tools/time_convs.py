@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Per-layer timing of the conv_wgmma_kernel launches of the benchmark's model: SSD300, batch 32, mode='inference',
 divide_by_stddev, bf16x3 (or bf16 with `fast`).  CUDA events around every launch, on one stream (the instrumented forward does
-not use the two-stream schedule).  Per layer: the plan (BN, k-iterations per tile, tiles, grid, cluster size), the median time of
+not use the two-stream schedule).  Per layer: the plan (pixels x channels of the tile, k-iterations per tile, tiles, grid, cluster
+size), the median time of
 `reps` timed forwards, the issued MMA rate and the bytes the TMA ring moves from L2 into shared memory, computed from the plan.
 
     python tools/time_convs.py [fast] [json=PATH]
@@ -44,29 +45,29 @@ def main():
     rows, tot_ms, tot_bytes, tot_fl = [], 0.0, 0.0, 0.0
     for s in convs:
         p = model.layer_plan(BATCH, s.name)
-        if p['kernel'] not in ('gemm', 'im2col_gemm'):
+        if p['kernel'] not in ('gemm', 'gemm_swap', 'im2col_gemm'):
             continue
         taps = 1 if p['kernel'] == 'im2col_gemm' else s.kh * s.kw
         kiter = taps * p['kblocks']
         tiles = p['n_tiles_m'] * p['n_tiles_n']
         planes = 2 if p['split'] else 1
-        stage = (128 * 64 * 2 + p['bn'] * 64 * 2) * planes
+        stage = (p['bm'] * 64 * 2 + p['bn'] * 64 * 2) * planes           # activation rows + weight rows of one k-iteration
         l2_bytes = float(tiles) * kiter * stage
-        issued = 2.0 * tiles * 128 * p['bn'] * (3 if p['split'] else 1) * kiter * 64
+        issued = 2.0 * tiles * p['bm'] * p['bn'] * (3 if p['split'] else 1) * kiter * 64
         t = float(np.median(ms[s.name]))
-        rows.append({'layer': s.name, 'bn': p['bn'], 'stages': p['stages'], 'kiter': kiter, 'tiles': tiles, 'grid': p['grid'],
+        rows.append({'layer': s.name, 'kernel': p['kernel'], 'bm': p['bm'], 'bn': p['bn'], 'stages': p['stages'], 'kiter': kiter, 'tiles': tiles, 'grid': p['grid'],
                      'cluster': p.get('cluster', 1), 'epilogue': p['epilogue'], 'ms': t, 'issued_tflops': issued / t / 1e9,
                      'l2_smem_gb': l2_bytes / 1e9, 'l2_smem_tbps': l2_bytes / t / 1e9})
         tot_ms += t; tot_bytes += l2_bytes; tot_fl += issued
-    hdr = '%-12s %4s %3s %5s %6s %4s %3s %-6s %8s %8s %8s %8s' % ('layer', 'BN', 'stg', 'kiter', 'tiles', 'grid', 'cl', 'epi', 'ms',
+    hdr = '%-12s %4s %4s %3s %5s %6s %4s %3s %-6s %8s %8s %8s %8s' % ('layer', 'BM', 'BN', 'stg', 'kiter', 'tiles', 'grid', 'cl', 'epi', 'ms',
                                                                   'TFLOP/s', 'L2->S GB', 'TB/s')
     print('%s, %d SMs, %s, batch %d, median of %d timed forwards (measured)' % (props.name, props.multi_processor_count, prec, BATCH, reps))
     print(hdr)
     for r in rows:
-        print('%-12s %4d %3d %5d %6d %4d %3d %-6s %8.3f %8.1f %8.2f %8.2f' % (
-            r['layer'], r['bn'], r['stages'], r['kiter'], r['tiles'], r['grid'], r['cluster'], r['epilogue'], r['ms'],
+        print('%-12s %4d %4d %3d %5d %6d %4d %3d %-6s %8.3f %8.1f %8.2f %8.2f' % (
+            r['layer'], r['bm'], r['bn'], r['stages'], r['kiter'], r['tiles'], r['grid'], r['cluster'], r['epilogue'], r['ms'],
             r['issued_tflops'], r['l2_smem_gb'], r['l2_smem_tbps']))
-    print('%-12s %50s %8.3f %8.1f %8.2f %8.2f' % ('total', '', tot_ms, tot_fl / tot_ms / 1e9, tot_bytes / 1e9, tot_bytes / tot_ms / 1e9))
+    print('%-12s %55s %8.3f %8.1f %8.2f %8.2f' % ('total', '', tot_ms, tot_fl / tot_ms / 1e9, tot_bytes / 1e9, tot_bytes / tot_ms / 1e9))
     if out_json:
         with open(out_json, 'w') as f:
             json.dump({'gpu': props.name, 'precision': prec, 'layers': rows, 'total_ms': tot_ms}, f, indent=1)
