@@ -36,6 +36,17 @@ def load_image(filename):
         return np.array(image, dtype=np.uint8)
 
 
+def _random_patch(img_h, img_w, ph, pw, random):
+    """``RandomPatch``'s draws for a ``ph x pw`` patch (patch_sampling_ops.py:506, :180-193): one ``uniform(0, 1)``, then the
+    ``randint`` for y and for x, all three also when a range is 0.  Returns ``(patch_ymin, patch_xmin, ph, pw)``."""
+    random.uniform(0, 1)
+    y_range = img_h - ph
+    py = random.randint(0, y_range + 1) if y_range >= 0 else random.randint(y_range, 1)
+    x_range = img_w - pw
+    px = random.randint(0, x_range + 1) if x_range >= 0 else random.randint(x_range, 1)
+    return py, px, ph, pw
+
+
 def pad_patch(img_h, img_w, img_height, img_width, random=np.random):
     """``RandomPadFixedAR(patch_aspect_ratio=img_width/img_height)`` on an ``img_h x img_w`` image (patch_sampling_ops.py:859-881,
     :180-193, :508): the patch size, then one ``uniform(0, 1)`` and the ``randint`` draws for y and x, all three also when a range
@@ -48,12 +59,34 @@ def pad_patch(img_h, img_w, img_height, img_width, random=np.random):
     else:
         pw = img_w
         ph = int(round(pw / ar))
-    random.uniform(0, 1)
-    y_range = img_h - ph
-    py = random.randint(0, y_range + 1) if y_range >= 0 else random.randint(y_range, 1)
-    x_range = img_w - pw
-    px = random.randint(0, x_range + 1) if x_range >= 0 else random.randint(x_range, 1)
-    return py, px, ph, pw
+    return _random_patch(img_h, img_w, ph, pw, random)
+
+
+def max_crop_patch(img_h, img_w, patch_aspect_ratio, random=np.random):
+    """``RandomMaxCropFixedAR(patch_aspect_ratio)`` on an ``img_h x img_w`` image (patch_sampling_ops.py:796-821, :117-193,
+    :506), the patch of ``weight_sampling_tutorial.ipynb``'s sample chain: the largest patch of that aspect ratio, then
+    ``RandomPatch``'s ``uniform(0, 1)`` and the ``randint`` draws for y and x, all three also when a range is 0.  Returns
+    ``(patch_ymin, patch_xmin, patch_height, patch_width)``."""
+    if img_w / img_h < patch_aspect_ratio:
+        pw = img_w
+        ph = int(round(pw / patch_aspect_ratio))
+    else:
+        ph = img_h
+        pw = int(round(ph * patch_aspect_ratio))
+    return _random_patch(img_h, img_w, ph, pw, random)
+
+
+def max_crop_ops(img_h, img_w, patch_aspect_ratio, box_filter=None, image_validator=None, clip_boxes=True, random=np.random):
+    """The op list of one ``RandomMaxCropFixedAR(patch_aspect_ratio, clip_boxes=clip_boxes)`` call with ``max_crop_patch``'s
+    draw: the ``crop_pad`` of the patch and, with ``clip_boxes``, the clip to it.  Follow it with ``batch_assembly.resize_ops``
+    and give the lists to ``assemble_images_device`` / ``assemble_training_batch``: the tutorial's ``ConvertTo3Channels ->
+    RandomMaxCropFixedAR -> Resize``.  Without a ``box_filter`` or ``image_validator`` the first patch is the one the reference
+    keeps; with one of them it may retry, and those draws stay with the caller (``NotImplementedError``)."""
+    if box_filter is not None or image_validator is not None:
+        raise NotImplementedError('RandomMaxCropFixedAR with a box_filter or image_validator: draw the patches and build the '
+                                  'ops with batch_assembly.crop_pad_ops')
+    py, px, ph, pw = max_crop_patch(img_h, img_w, patch_aspect_ratio, random)
+    return ba.crop_pad_ops(py, px, ph, pw, clip_boxes=clip_boxes)
 
 
 def image_plan(img_h, img_w, img_height, img_width, mode, random=np.random):

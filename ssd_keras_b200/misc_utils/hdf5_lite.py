@@ -11,9 +11,12 @@ Anything outside the subset (new-style groups, superblock >= 2, variable-length 
 name of the feature, never a silent misread.
 
 ``read_datasets(path)`` -> ``{'/group/sub/name': ndarray}``;  ``read_attributes(path, '/')`` -> ``{name: value}`` (fixed-length
-strings / numeric arrays only);  ``read_optimizer_weights(path)`` -> ``[(name, array)]`` of ``/optimizer_weights``.
+strings / numeric arrays only);  ``read_optimizer_weights(path)`` -> ``[(name, array)]`` of ``/optimizer_weights``;
+``read_keras_weights(path)`` -> ``{'conv1_1/kernel': ndarray}`` in the file's layer order; ``read_keras_file(path)`` -> the
+layers, weights and attributes in the file's order (``KerasFile``).
 ``write_keras_weights(path, layers)`` writes a file with the same structures (``model.save`` / ``save_weights`` and the tests use
-it; files from real h5py use the same structures with different block placement)."""
+it; files from real h5py use the same structures with different block placement); ``write_keras_file(path, keras_file,
+replace=...)`` writes a ``KerasFile`` back with chosen weights replaced (the weight-sampling tutorial's edit)."""
 import struct
 import zlib
 
@@ -323,38 +326,99 @@ def read_attributes(path, group='/'):
     return _Reader(buf).walk()[1].get(group, {})
 
 
-def read_keras_weights(path):
-    """Keras weight names -> arrays: ``{'conv1_1/kernel': ..., 'conv1_1/bias': ..., 'conv4_3_norm/gamma': ...}``.
-
-    Handles both layouts Keras writes: a weights file (``/<layer>/<layer>/kernel:0``, ``model.save_weights``) and a full model
-    file (``/model_weights/<layer>/<layer>/kernel:0``, ``model.save``).  The weight name is the dataset's own path below the
-    layer group with the ``:0`` suffix removed; Keras-1-style names (``<layer>_W:0`` / ``<layer>_b:0``) are mapped to
+def keras_weight_key(layer, stored_name):
+    """The package's name of a weight (``'conv1_1/kernel'``) from its layer and its name in ``weight_names``
+    (``'conv1_1/kernel:0'``).  The ``:0`` suffix is removed; Keras-1-style names (``<layer>_W:0`` / ``<layer>_b:0``) are mapped to
     ``kernel`` / ``bias``."""
-    out = {}
-    for p, arr in read_datasets(path).items():
-        parts = [q for q in p.split('/') if q]
-        if parts and parts[0] == 'model_weights':
-            parts = parts[1:]
-        if parts and parts[0] == 'optimizer_weights':
-            continue
-        if len(parts) < 2:
-            continue
-        layer = parts[0]
-        name = '/'.join(parts[1:])                      # '<layer>/kernel:0'  (or 'kernel:0' in some writers)
-        name = name.split(':')[0]
-        if not name.startswith(layer + '/'):
-            leaf = name.split('/')[-1]
-            if leaf.startswith(layer + '_'):
-                leaf = {'W': 'kernel', 'b': 'bias'}.get(leaf[len(layer) + 1:], leaf[len(layer) + 1:])
-            name = layer + '/' + leaf
-        out[name] = np.ascontiguousarray(arr)
+    name = stored_name.split(':')[0]
+    if not name.startswith(layer + '/'):
+        leaf = name.split('/')[-1]
+        if leaf.startswith(layer + '_'):
+            leaf = {'W': 'kernel', 'b': 'bias'}.get(leaf[len(layer) + 1:], leaf[len(layer) + 1:])
+        name = layer + '/' + leaf
+    return name
+
+
+def _names(value):
+    return [bytes(n).decode('utf-8') for n in np.atleast_1d(value)] if value is not None else []
+
+
+def _in_listed_order(listed, present):
+    """The members of ``present`` (in its order) with those in ``listed`` first, in that order."""
+    first = [n for n in listed if n in present]
+    seen = set(first)
+    return first + [n for n in present if n not in seen]
+
+
+def _optimizer_weights(datasets, attrs, path):
+    names = attrs.get('/optimizer_weights', {}).get('weight_names')
+    if names is None:
+        return []
+    out = []
+    for n in _names(names):
+        if '/optimizer_weights/' + n not in datasets:
+            raise ValueError('%s: optimizer weight %s is listed in weight_names but not stored' % (path, n))
+        out.append((n, datasets['/optimizer_weights/' + n]))
     return out
 
 
+class KerasFile:
+    """The contents of a Keras HDF5 weights file or of a full-model file's ``/model_weights``, in the file's own order.
+
+    ``layers``: ``[(layer, attributes, [(stored name, array), ...]), ...]`` in ``layer_names`` order, each layer's weights in
+    its ``weight_names`` order (stored names such as ``'conv1_1/kernel:0'``), layers without weights included; groups or
+    datasets the attributes do not list follow the listed ones.  ``attrs``: the attributes of the group holding the layers
+    (``layer_names``, ``backend``, ``keras_version``).  ``root_attrs``: a full-model file's root attributes (``model_config``,
+    ``training_config``, ...); ``{}`` for a weights file, whose root is the layer group.  ``optimizer_weights``: a full-model
+    file's ``/optimizer_weights`` as ``[(name, array), ...]``.  Attributes this reader cannot decode (variable-length strings)
+    are not kept."""
+
+    def __init__(self, layers, attrs, root_attrs=None, full_model=False, optimizer_weights=()):
+        self.layers, self.attrs = layers, attrs
+        self.root_attrs, self.full_model, self.optimizer_weights = dict(root_attrs or {}), full_model, list(optimizer_weights)
+
+    def weights(self):
+        """``{'conv1_1/kernel': array, ...}`` in layer and weight order (``read_keras_weights``)."""
+        return {keras_weight_key(layer, n): np.ascontiguousarray(a) for layer, _, items in self.layers for n, a in items}
+
+
+def read_keras_file(path):
+    """-> ``KerasFile``: the layers, weights and attributes of a Keras weights file (``/<layer>/<layer>/kernel:0``,
+    ``model.save_weights``) or of a full-model file (``/model_weights/...``, ``model.save``), in the file's order."""
+    with open(path, 'rb') as f:
+        datasets, attrs = _Reader(f.read()).walk()
+    full = '/model_weights' in attrs and '/model_weights' not in datasets
+    top = '/model_weights' if full else ''
+    groups = [p[len(top) + 1:] for p in attrs if p not in datasets and p.startswith(top + '/') and '/' not in p[len(top) + 1:]]
+    groups = [g for g in groups if g]
+    top_attrs = attrs.get(top or '/', {})
+    layers = []
+    for layer in _in_listed_order(_names(top_attrs.get('layer_names')), groups):
+        g = top + '/' + layer
+        stored = {p[len(g) + 1:]: a for p, a in datasets.items() if p.startswith(g + '/')}
+        gattrs = attrs[g]
+        layers.append((layer, gattrs, [(n, stored[n]) for n in _in_listed_order(_names(gattrs.get('weight_names')), list(stored))]))
+    return KerasFile(layers, top_attrs, attrs.get('/', {}) if full else {}, full, _optimizer_weights(datasets, attrs, path) if full else ())
+
+
+def read_keras_weights(path):
+    """Keras weight names -> arrays: ``{'conv1_1/kernel': ..., 'conv1_1/bias': ..., 'conv4_3_norm/gamma': ...}``, in the
+    file's ``layer_names`` / ``weight_names`` order.
+
+    Handles both layouts Keras writes: a weights file (``/<layer>/<layer>/kernel:0``, ``model.save_weights``) and a full model
+    file (``/model_weights/<layer>/<layer>/kernel:0``, ``model.save``).  The names are ``keras_weight_key``'s."""
+    return read_keras_file(path).weights()
+
+
 # =================================================================================================
-# writer (test fixture generator): superblock v0, old-style groups, v1 object headers, contiguous float datasets,
-# fixed-length string attributes -- the same structures h5py's default writes
+# writer (model.save / save_weights, rewrites of a read file, test fixtures): superblock v0, old-style groups, v1 object
+# headers, contiguous or chunked datasets, fixed-length string attributes -- the same structures h5py's default writes
 # =================================================================================================
+def _little_endian(a):
+    """The writer's datatype messages say little endian; a big-endian array read from another file is converted."""
+    return a.astype(a.dtype.newbyteorder('<')) if a.dtype.byteorder == '>' else a
+
+
 class _Writer:
     def __init__(self):
         self.buf = bytearray(b'\x00' * 96)              # superblock v0 = 56 bytes + 40-byte root symbol table entry
@@ -397,7 +461,7 @@ class _Writer:
         return struct.pack('<BBB5x', 1, len(shape), 0) + b''.join(struct.pack('<Q', int(s)) for s in shape)
 
     def _attr_msg(self, name, value):
-        value = np.asarray(value)
+        value = _little_endian(np.asarray(value))
         nm = name.encode() + b'\x00'
         t, s = self._dtype_msg(value.dtype), self._space_msg(value.shape)
         pad = lambda x: x + b'\x00' * (-len(x) % 8)      # noqa: E731
@@ -405,7 +469,7 @@ class _Writer:
 
     def dataset_chunked(self, arr, chunks, gzip=True, shuffle=True):
         """Chunked layout (one B-tree leaf), optionally shuffle + deflate filtered -- what ``compression='gzip'`` produces."""
-        arr = np.ascontiguousarray(arr)
+        arr = _little_endian(np.ascontiguousarray(arr))
         rank, esize = arr.ndim, arr.dtype.itemsize
         keys = []
         grid = [range(0, s, c) for s, c in zip(arr.shape, chunks)]
@@ -444,7 +508,7 @@ class _Writer:
         return self._header(msgs)
 
     def dataset(self, arr):
-        arr = np.ascontiguousarray(arr).reshape(np.shape(arr))     # a scalar stays a scalar (Keras' iterations:0)
+        arr = _little_endian(np.ascontiguousarray(arr).reshape(np.shape(arr)))     # a scalar stays a scalar (Keras' iterations:0)
         data = self._alloc(max(arr.nbytes, 1))
         self.buf[data:data + arr.nbytes] = arr.tobytes()
         layout = struct.pack('<BBQQ', 3, 1, data, arr.nbytes)
@@ -502,63 +566,86 @@ def read_optimizer_weights(path):
     attribute (Keras' ``optimizer.get_weights()`` order); ``[]`` when the file has none."""
     with open(path, 'rb') as f:
         datasets, attrs = _Reader(f.read()).walk()
-    names = attrs.get('/optimizer_weights', {}).get('weight_names')
-    if names is None:
-        return []
-    out = []
-    for n in np.atleast_1d(names):
-        n = bytes(n).decode('utf-8')
-        if '/optimizer_weights/' + n not in datasets:
-            raise ValueError('%s: optimizer weight %s is listed in weight_names but not stored' % (path, n))
-        out.append((n, datasets['/optimizer_weights/' + n]))
-    return out
+    return _optimizer_weights(datasets, attrs, path)
 
 
 def _tree(w, items):
-    """[('a/b/name', array), ...] -> the links of one group: datasets for plain names, nested groups for 'a/...' prefixes."""
+    """[('a/b/name', array or object header address), ...] -> the links of one group: datasets for plain names (an address is
+    a dataset already written), nested groups for 'a/...' prefixes."""
     links, sub = [], {}
-    for name, arr in items:
+    for name, obj in items:
         head, _, rest = name.partition('/')
         if rest:
-            sub.setdefault(head, []).append((rest, arr))
+            sub.setdefault(head, []).append((rest, obj))
         else:
-            links.append((head, w.dataset(np.asarray(arr))))
+            links.append((head, obj if isinstance(obj, int) else w.dataset(np.asarray(obj))))
     return links + [(head, w.group(_tree(w, part))[0]) for head, part in sub.items()]
+
+
+def _write(path, source, chunked=()):
+    """``source`` (a ``KerasFile``) -> an HDF5 file: its layers, weights and attributes as given; the weights whose
+    ``keras_weight_key`` is in ``chunked`` are stored chunked with shuffle + gzip filters."""
+    w = _Writer()
+    top = []
+    for layer, gattrs, items in source.layers:
+        objs = [(n, w.dataset_chunked(a, tuple(max(1, (d + 1) // 2) for d in np.shape(a))) if keras_weight_key(layer, n) in chunked else a)
+                for n, a in items]
+        top.append((layer, w.group(_tree(w, objs), attrs=gattrs)[0]))
+    if source.full_model:
+        links = [('model_weights', w.group(top, attrs=source.attrs)[0])]
+        if source.optimizer_weights:
+            names = np.array([n.encode() for n, _ in source.optimizer_weights])
+            links.append(('optimizer_weights', w.group(_tree(w, source.optimizer_weights), attrs={'weight_names': names})[0]))
+        root, bt, heap = w.group(links, attrs=source.root_attrs or None)
+    else:
+        root, bt, heap = w.group(top, attrs=source.attrs)
+    w.finish(root, bt, heap, path)
+
+
+def write_keras_file(path, source, replace=None, include_optimizer=None):
+    """Write the ``KerasFile`` ``source`` (``read_keras_file``) to ``path``: the same layers in the same order, the same
+    ``weight_names`` and attributes, with the weights named in ``replace`` (``{'conv4_3_norm_mbox_conf/kernel': array, ...}``,
+    ``keras_weight_key`` names) stored with the shape and dtype of the new array, and every other dataset as it was.
+
+    A full-model file keeps its ``training_config`` and ``/optimizer_weights`` when nothing is replaced and loses them
+    otherwise, since an optimizer state does not fit re-shaped weights; ``include_optimizer=True`` with replaced weights raises
+    ``ValueError``, ``include_optimizer=False`` drops them always.  Only the weights file layout and ``/model_weights`` are
+    written; other groups of a full-model file are not."""
+    replace = dict(replace or {})
+    replaced = bool(replace)
+    layers = []
+    for layer, gattrs, items in source.layers:
+        layers.append((layer, gattrs, [(n, replace.pop(keras_weight_key(layer, n), a)) for n, a in items]))
+    if replace:
+        raise ValueError('%s: no such weights in the source file: %s' % (path, sorted(replace)))
+    keep = (not replaced) if include_optimizer is None else bool(include_optimizer)
+    if keep and replaced and source.full_model:
+        raise ValueError('the training_config and optimizer weights of %s do not fit the replaced weights: write the file with '
+                         'include_optimizer=False' % path)
+    root_attrs = dict(source.root_attrs)
+    if not keep:
+        root_attrs.pop('training_config', None)
+    _write(path, KerasFile(layers, source.attrs, root_attrs, source.full_model, source.optimizer_weights if keep else ()))
 
 
 def write_keras_weights(path, weights, full_model=False, chunked=(), root_attrs=None, optimizer_weights=()):
     """``weights``: ``{'conv1_1/kernel': array, 'conv1_1/bias': array, ...}`` -> an HDF5 file with the layout of
-    ``model.save_weights`` (``/<layer>/<layer>/kernel:0`` datasets, ``layer_names`` / ``weight_names`` attributes); with
-    ``full_model`` everything sits below ``/model_weights`` like in ``model.save``; the weights named in ``chunked`` are stored
-    chunked with shuffle + gzip filters; ``root_attrs`` (name -> bytes / array) become attributes of the root group, where
-    ``model.save`` keeps ``model_config``.  ``optimizer_weights`` (full model only): ``[(name, array), ...]`` stored below
-    ``/optimizer_weights`` -- a name's '/' parts become nested groups -- with their order in its ``weight_names`` attribute."""
-    w = _Writer()
-    layers = {}
+    ``model.save_weights`` (``/<layer>/<layer>/kernel:0`` datasets, ``layer_names`` / ``weight_names`` attributes, layers in
+    the order of ``weights``); with ``full_model`` everything sits below ``/model_weights`` like in ``model.save``; the weights
+    named in ``chunked`` are stored chunked with shuffle + gzip filters; ``root_attrs`` (name -> bytes / array) become
+    attributes of the root group, where ``model.save`` keeps ``model_config``.  ``optimizer_weights`` (full model only):
+    ``[(name, array), ...]`` stored below ``/optimizer_weights`` -- a name's '/' parts become nested groups -- with their order
+    in its ``weight_names`` attribute.  ``write_keras_file`` rewrites a file read with ``read_keras_file`` in its own order."""
+    per_layer = {}
     for k, v in weights.items():
         layer, name = k.split('/', 1)
-        layers.setdefault(layer, []).append((name, np.asarray(v)))
-    top = []
-    for layer, items in layers.items():
-        inner = [(n + ':0', w.dataset_chunked(a, tuple(max(1, (d + 1) // 2) for d in a.shape)) if (layer + '/' + n) in chunked else w.dataset(a))
-                 for n, a in items]
-        inner_hdr, _, _ = w.group(inner)
-        names = np.array([(layer + '/' + n + ':0').encode() for n, _ in items])
-        outer_hdr, _, _ = w.group([(layer, inner_hdr)], attrs={'weight_names': names})
-        top.append((layer, outer_hdr))
-    attrs = {'layer_names': np.array([l.encode() for l in layers]), 'backend': np.array(b'tensorflow'), 'keras_version': np.array(b'2.1.4')}
-    if full_model:
-        mw, _, _ = w.group(top, attrs=attrs)
-        ra = {k: (np.array(v) if isinstance(v, (bytes, str)) else np.asarray(v)) for k, v in (root_attrs or {}).items()}
-        links = [('model_weights', mw)]
-        if optimizer_weights:
-            names = np.array([n.encode() for n, _ in optimizer_weights])
-            links.append(('optimizer_weights', w.group(_tree(w, optimizer_weights), attrs={'weight_names': names})[0]))
-        root, bt, heap = w.group(links, attrs=ra or None)
-    else:
+        per_layer.setdefault(layer, []).append((layer + '/' + name + ':0', np.asarray(v)))
+    layers = [(layer, {'weight_names': np.array([n.encode() for n, _ in items])}, items) for layer, items in per_layer.items()]
+    attrs = {'layer_names': np.array([l.encode() for l in per_layer]), 'backend': np.array(b'tensorflow'), 'keras_version': np.array(b'2.1.4')}
+    ra = {k: (np.array(v) if isinstance(v, (bytes, str)) else np.asarray(v)) for k, v in (root_attrs or {}).items()}
+    if not full_model:
         if optimizer_weights:
             raise ValueError('optimizer weights belong to a full-model file')
-        if root_attrs:
-            attrs.update({k: (np.array(v) if isinstance(v, (bytes, str)) else np.asarray(v)) for k, v in root_attrs.items()})
-        root, bt, heap = w.group(top, attrs=attrs)
-    w.finish(root, bt, heap, path)
+        attrs.update(ra)
+        ra = {}
+    _write(path, KerasFile(layers, attrs, ra, full_model, optimizer_weights), chunked)
