@@ -148,6 +148,7 @@ int ssdk_iou(ssdk_ctx* ctx, const double* boxes1_dev, int m, const double* boxes
  *             SSDExpand = negative patch origin without filter / clip, SSDRandomCrop = filter + clip)
  *   FLIP_H    a0=image width   FLIP_V  a0=image height                  (object_detection_2d_geometric_ops.py:186,194)
  *   RESIZE    a0=in_height a1=in_width a2=out_height a3=out_width; flags bit0: drop degenerate boxes afterwards (:88-100)
+ *   RESIZE_INTERP  the same arithmetic as RESIZE (its image half takes all five cv2 interpolation codes)
  *   FILTER    flags bit0: drop degenerate boxes (xmax <= xmin or ymax <= ymin), bit1: drop boxes with area < a0
  *             (BoxFilter, object_detection_2d_image_boxes_validation_utils.py:155-165; also DataGenerator's
  *             degenerate_box_handling='remove')
@@ -173,7 +174,9 @@ typedef enum { SSDK_BOXOP_END = 0, SSDK_BOXOP_CROP_PAD = 1, SSDK_BOXOP_FLIP_H = 
                 * box kernel skips them */
                SSDK_BOXOP_TO_FLOAT32 = 16, SSDK_BOXOP_TO_UINT8 = 17, SSDK_BOXOP_BRIGHTNESS = 18, SSDK_BOXOP_CONTRAST = 19,
                SSDK_BOXOP_SATURATION = 20, SSDK_BOXOP_HUE = 21, SSDK_BOXOP_RGB2HSV = 22, SSDK_BOXOP_HSV2RGB = 23,
-               SSDK_BOXOP_CHANNEL_SWAP = 24 } ssdk_box_op_kind;
+               SSDK_BOXOP_CHANNEL_SWAP = 24,
+               /* 25: RESIZE with every interpolation mode of ResizeRandomInterp; boxes as RESIZE */
+               SSDK_BOXOP_RESIZE_INTERP = SSDK_BOXOP_CHANNEL_SWAP + 1 } ssdk_box_op_kind;
 typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
@@ -189,6 +192,10 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
  *   CROP_PAD  flags bits 8-31: background R, G, B bytes (0 = black, as CropPad's default; SSDExpand uses 123,117,104)
  *   RESIZE    flags bits 8-15: cv2 interpolation code, INTER_NEAREST = 0 or INTER_LINEAR = 1 (an exact 2x linear downscale
  *             takes INTER_AREA's fast path, as cv2 does); any other code is an error
+ *   RESIZE_INTERP  RESIZE that also takes INTER_CUBIC = 2, INTER_AREA = 3 and INTER_LANCZOS4 = 4, OpenCV 4.13's own resize
+ *             code bit for bit (cubic and Lanczos4: 11-bit coefficient tables, 4 or 8 clamped taps per axis; area: its three
+ *             paths, integer factors, other downscales and upscales); IPP's INTER_CUBIC, which cv2 wheels built with IPP use
+ *             by default, differs from it in the last bit at a few pixels in 10^5
  *   TRANSLATE flags bits 8-31: background; an integer shift, composed like a pad / crop
  *   SCALE     flags bits 8-31: background; the bilinear warp, cv2's fixed-point scheme bit for bit
  *   ROTATE    an exact signed axis permutation (cv2's fixed-point map is checked on the host to have fraction 0 everywhere),

@@ -55,7 +55,8 @@ BOXOP_END, BOXOP_CROP_PAD, BOXOP_FLIP_H, BOXOP_FLIP_V, BOXOP_RESIZE, BOXOP_FILTE
 BOXOP_TRANSLATE, BOXOP_SCALE, BOXOP_ROTATE, BOXOP_OVERLAP, BOXOP_CLIP = range(6, 11)
 (BOXOP_TO_FLOAT32, BOXOP_TO_UINT8, BOXOP_BRIGHTNESS, BOXOP_CONTRAST, BOXOP_SATURATION, BOXOP_HUE, BOXOP_RGB2HSV, BOXOP_HSV2RGB,
  BOXOP_CHANNEL_SWAP) = range(16, 25)         # photometric ops: images only (ssdk_assemble_images)
-INTER_NEAREST, INTER_LINEAR = 0, 1          # cv2's codes, in RESIZE's flag bits 8-15 (ssdk_assemble_images)
+BOXOP_RESIZE_INTERP = 25                    # RESIZE with all five cv2 modes (the boxes as RESIZE)
+INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = range(5)   # cv2's codes, in flag bits 8-15
 
 
 class LossWsLayout(C.Structure):

@@ -13,11 +13,13 @@
 //   box_pack_kernel    one CTA per image: rows to their final place.
 // The image half of the same op lists (ssdk_assemble_images) is at the end of the file: ConvertTo3Channels
 // (object_detection_2d_photometric_ops.py:88-108), the image arithmetic of CropPad (:266-313) and Flip, and uint8 cv2.resize
-// (INTER_NEAREST / INTER_LINEAR) and uint8 cv2.warpAffine (Translate / Scale / Rotate, geometric_ops.py:233-737) in one launch,
+// (INTER_NEAREST / INTER_LINEAR; RESIZE_INTERP also INTER_CUBIC / INTER_AREA / INTER_LANCZOS4, restated in tests/resize_reference.py)
+// and uint8 cv2.warpAffine (Translate / Scale / Rotate, geometric_ops.py:233-737) in one launch,
 // restated in oracle/imageops.py and oracle/warpops.py; the box half of Translate / Scale / Rotate and BoxFilter's overlap test is in oracle/boxops.py.
 //   image_assemble_kernel  one CTA per (output row, image): every output pixel is traced back through the resize to at most
 //                          four canvas taps, and each tap through the composed crop / pad / flip map to a source pixel or to
 //                          the background colour.  No intermediate image exists.
+//   image_assemble_kernel_wide  the same for batches with cubic, Lanczos4 or area taps (4 x 4, 8 x 8 or the area window).
 //   photometric_kernel     the photometric prefix of the op lists (ConvertDataType, Brightness, Contrast, Saturation, Hue,
 //                          ConvertColor RGB <-> HSV, ChannelSwap; object_detection_2d_photometric_ops.py), one launch in front of
 //                          image_assemble_kernel: uint8 in, uint8 h x w x 3 out, restated in oracle/photoops.py.
@@ -25,6 +27,7 @@
 #include "common.cuh"
 #include "rn.cuh"
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <vector>
 
@@ -111,7 +114,7 @@ __global__ void __launch_bounds__(kBoxThreads) box_ops_kernel(const void* __rest
           const double nx0 = op.a0 - x1, nx1 = op.a0 - x0; x0 = nx0; x1 = nx1;
         } else if (op.op == SSDK_BOXOP_FLIP_V) {
           const double ny0 = op.a0 - y1, ny1 = op.a0 - y0; y0 = ny0; y1 = ny1;
-        } else if (op.op == SSDK_BOXOP_RESIZE) {             // np.round(labels * (out / in), decimals=0)
+        } else if (op.op == SSDK_BOXOP_RESIZE || op.op == SSDK_BOXOP_RESIZE_INTERP) {   // np.round(labels * (out / in), decimals=0)
           const double sy = op.a2 / op.a0, sx = op.a3 / op.a1;
           y0 = rint(y0 * sy); y1 = rint(y1 * sy); x0 = rint(x0 * sx); x1 = rint(x1 * sx);
           if (op.flags & 1) valid = valid && (x1 > x0) && (y1 > y0);
@@ -233,6 +236,10 @@ namespace {
 
 constexpr int kImgThreads = 128;
 enum { kImgCopy = 0, kImgNearest = 1, kImgLinear = 2, kImgArea2 = 3, kImgWarp = 4 };
+// The modes only RESIZE_INTERP reaches; they run in image_assemble_kernel_wide, so that batches without them keep the
+// instantiations (and registers) of image_assemble_kernel.
+enum WideMode { kWideCubic = 5, kWideLanczos4 = 6, kWideArea = 7, kWideAreaInt = 8, kWideAreaUp = 9 };
+inline bool is_wide(int mode) { return mode >= kWideCubic; }
 
 // An integer map from a canvas to the image it is drawn from: canvas (r, c) -> (o0 + m00 * r + m01 * c, o1 + m10 * r + m11 * c),
 // a translation and a signed axis permutation.  Canvas rows [v0, v1) x columns [v2, v3) come from that image; every other canvas
@@ -251,7 +258,7 @@ struct ImgDesc {
   IntMap pre;                  // canvas -> source
   IntMap post;                 // output -> SCALE output (kImgWarp only)
   int bg;                      // background R | G << 8 | B << 16
-  int mode;                    // kImgCopy / kImgNearest / kImgLinear / kImgArea2 / kImgWarp
+  int mode;                    // kImgCopy / kImgNearest / kImgLinear / kImgArea2 / kImgWarp / kWideCubic .. kWideAreaUp
   double scale_y, scale_x;     // RESIZE: cv2's 1 / (out / in), float64
   double m[6];                 // SCALE: cv2's inverted matrix, float64
 };
@@ -303,10 +310,174 @@ __device__ __forceinline__ void warp_px(const uint8_t* __restrict__ src, const I
   for (int k = 0; k < 3; ++k) v[k] = (p00[k] * w00 + p01[k] * w01 + p10[k] * w10 + p11[k] * w11 + (1 << 14)) >> 15;
 }
 
-// kWarp: the batch has a SCALE; batches without one run an instantiation that carries no warp code (fewer registers).
-template <bool kWarp>
-__global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8_t* __restrict__ src, const ImgDesc* __restrict__ descs,
-                                                                     int out_h, int out_w, float* __restrict__ out) {
+// The column half of cv2's linear resize (INTER_LINEAR, and INTER_AREA when it upscales) for a column with first tap s and
+// fraction f, rows r0 / r1 with coefficients b0 / b1: columns past either border take the edge pixel with weight 2048.
+__device__ __forceinline__ void linear_cols(const uint8_t* __restrict__ src, const ImgDesc& d, int r0, int r1, int b0, int b1, int s, float f,
+                                            int v[3]) {
+  if (s < 0) { s = 0; f = 0.f; }
+  if (s >= d.cw - 1) { s = d.cw - 1; f = 0.f; }
+  const int c1 = min(s + 1, d.cw - 1);
+  const int a0 = coef11(__fsub_rn(1.f, f)), a1 = coef11(f);
+  int p01[3], p10[3], p11[3];
+  canvas_px(src, d, r0, s, v); canvas_px(src, d, r0, c1, p01);
+  canvas_px(src, d, r1, s, p10); canvas_px(src, d, r1, c1, p11);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int S0 = v[k] * a0 + p01[k] * a1, S1 = p10[k] * a0 + p11[k] * a1;      // horizontal pass, int
+    const int t = (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2;  // cv2's vertical pass on 8-bit
+    v[k] = min(max(t, 0), 255);
+  }
+}
+
+// cv2's INTER_AREA coordinate when an axis upscales (resize's area_mode, both axes): s = floor(d * scale),
+// f = (float)((d + 1) - (s + 1) * inv_scale), then f <= 0 ? 0 : f - floor(f).
+__device__ __forceinline__ void area_coord(int dst, double scale, double inv, int& s, float& f) {
+  s = (int)floor(__dmul_rn((double)dst, scale));
+  const float fx = __double2float_rn(__dsub_rn((double)(dst + 1), __dmul_rn((double)(s + 1), inv)));
+  f = fx <= 0.f ? 0.f : __fsub_rn(fx, floorf(fx));
+}
+
+// interpolateCubic (A = -0.75) in float32, every step rounded, then saturate_cast<short>(c * 2048).
+__device__ __forceinline__ void cubic_coefs(float x, int c[8]) {
+  const float A = -0.75f, x1 = __fadd_rn(x, 1.f), mx = __fsub_rn(1.f, x);
+  const float k0 = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(A, x1), 5 * A), x1), 8 * A), x1), 4 * A);
+  const float k1 = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2, x), A + 3), x), x), 1.f);
+  const float k2 = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(A + 2, mx), A + 3), mx), mx), 1.f);
+  const float k3 = __fsub_rn(__fsub_rn(__fsub_rn(1.f, k0), k1), k2);
+  c[0] = coef11(k0); c[1] = coef11(k1); c[2] = coef11(k2); c[3] = coef11(k3);
+}
+
+// interpolateLanczos4: float32 coefficients from float64 sin / cos, normalised by their float32 sum, then saturate_cast<short>(c *
+// 2048).  CUDA's sin / cos are within an ulp of the C library's; a difference would have to survive two roundings to float32
+// and one to 11 bits to show.
+__device__ __forceinline__ void lanczos_coefs(float x, int c[8]) {
+  if (x < 1.1920928955078125e-7f) {                               // FLT_EPSILON
+#pragma unroll
+    for (int i = 0; i < 8; ++i) c[i] = i == 3 ? 2048 : 0;
+    return;
+  }
+  const double kPi = 3.14159265358979323846, s45 = 0.70710678118654752440084436210485;
+  const double cs[8][2] = {{1, 0}, {-s45, -s45}, {0, 1}, {s45, -s45}, {-1, 0}, {s45, s45}, {0, -1}, {-s45, s45}};
+  const float x3 = __fadd_rn(x, 3.f);
+  const double y0 = __dmul_rn(__dmul_rn(-(double)x3, kPi), 0.25);
+  double s0, c0;
+  sincos(y0, &s0, &c0);
+  float k[8], sum = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const double y = __dmul_rn(__dmul_rn(-(double)__fsub_rn(x3, (float)i), kPi), 0.25);
+    k[i] = __double2float_rn(__ddiv_rn(__dadd_rn(__dmul_rn(cs[i][0], s0), __dmul_rn(cs[i][1], c0)), __dmul_rn(y, y)));
+    sum = __fadd_rn(sum, k[i]);
+  }
+  sum = __fdiv_rn(1.f, sum);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) c[i] = coef11(__fmul_rn(k[i], sum));
+}
+
+// One axis of cv2's INTER_AREA downscale (computeResizeAreaTab) for output index d: source indices lo..hi, weight a_first at
+// s1 - 1 (if lo < s1), a_mid on s1 .. s2 - 1, a_last at s2 (if hi == s2); float64 geometry, float32 weights.
+struct AreaSpan { int lo, hi, s1, s2; float a_first, a_mid, a_last; };
+__device__ __forceinline__ AreaSpan area_span(int d, int n_in, double scale) {
+  const double f1 = __dmul_rn((double)d, scale), f2 = __dadd_rn(f1, scale);
+  const double cell = fmin(scale, __dsub_rn((double)n_in, f1));
+  int s2 = min((int)floor(f2), n_in - 1);
+  const int s1 = min((int)ceil(f1), s2);
+  AreaSpan a;
+  a.s1 = s1; a.s2 = s2;
+  a.lo = __dsub_rn((double)s1, f1) > 1e-3 ? s1 - 1 : s1;
+  a.hi = __dsub_rn(f2, (double)s2) > 1e-3 ? s2 : s2 - 1;
+  a.a_first = __double2float_rn(__ddiv_rn(__dsub_rn((double)s1, f1), cell));
+  a.a_mid = __double2float_rn(__ddiv_rn(1.0, cell));
+  a.a_last = __double2float_rn(__ddiv_rn(fmin(fmin(__dsub_rn(f2, (double)s2), 1.0), cell), cell));
+  return a;
+}
+__device__ __forceinline__ float area_weight(const AreaSpan& a, int t) {
+  return t < a.s1 ? a.a_first : t < a.s2 ? a.a_mid : a.a_last;
+}
+
+// The vertical pass of cv2's INTER_CUBIC on 8-bit (VResizeCubic): elements of a row (column * 3 + channel) below the last whole
+// 8-lane block run VResizeCubicVec_32s8u, float32 sums S3*b3, then S2*b2 + that, ... each step rounded, rounded half to even;
+// the remaining elements take the integer sum (+ 2^21) >> 22.  INTER_LANCZOS4 has no vector body: integer sums throughout.
+// kTaps = 4 (cubic) or 8 (Lanczos4); taps are clamped to the canvas in both axes and keep their fraction.
+template <int kTaps>
+__device__ __forceinline__ void kernel_px(const uint8_t* __restrict__ src, const ImgDesc& d, int sy, const int* b, int dx, int vec_end,
+                                          int v[3]) {
+  int s; float f;
+  linear_coord(dx, d.scale_x, s, f);
+  int a[8];
+  if (kTaps == 4) cubic_coefs(f, a); else lanczos_coefs(f, a);
+  int isum[3] = {0, 0, 0};
+  float fsum[3] = {0.f, 0.f, 0.f};
+#pragma unroll 1
+  for (int k = kTaps - 1; k >= 0; --k) {
+    const int r = min(max(sy - kTaps / 2 + 1 + k, 0), d.ch - 1);
+    int D[3] = {0, 0, 0};
+#pragma unroll
+    for (int j = 0; j < kTaps; ++j) {
+      int p[3];
+      canvas_px(src, d, r, min(max(s - kTaps / 2 + 1 + j, 0), d.cw - 1), p);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) D[c] += p[c] * a[j];              // horizontal pass, int
+    }
+    const float bf = __fmul_rn((float)b[k], 1.f / (1 << 22));
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      isum[c] += D[c] * b[k];
+      const float t = __fmul_rn((float)D[c], bf);
+      fsum[c] = k == kTaps - 1 ? t : __fadd_rn(t, fsum[c]);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int t = kTaps == 4 && dx * 3 + c < vec_end ? __float2int_rn(fsum[c]) : (isum[c] + (1 << 21)) >> 22;
+    v[c] = min(max(t, 0), 255);
+  }
+}
+
+// cv2's INTER_AREA downscale by non-integer factors (resizeArea_): per source row of the window, buf = sum of S * alpha over
+// the columns (float32, in column order); sum = beta0 * buf0, then sum += beta * buf; rounded half to even.
+__device__ __forceinline__ void area_px(const uint8_t* __restrict__ src, const ImgDesc& d, const AreaSpan& ys, int dx, int v[3]) {
+  const AreaSpan xs = area_span(dx, d.cw, d.scale_x);
+  float acc[3] = {0.f, 0.f, 0.f};
+  for (int r = ys.lo; r <= ys.hi; ++r) {
+    float buf[3] = {0.f, 0.f, 0.f};
+    for (int c = xs.lo; c <= xs.hi; ++c) {
+      const float alpha = area_weight(xs, c);
+      int p[3];
+      canvas_px(src, d, r, c, p);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) buf[k] = __fadd_rn(buf[k], __fmul_rn((float)p[k], alpha));
+    }
+    const float beta = area_weight(ys, r);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) acc[k] = r == ys.lo ? __fmul_rn(beta, buf[k]) : __fadd_rn(acc[k], __fmul_rn(beta, buf[k]));
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = min(max(__float2int_rn(acc[k]), 0), 255);
+}
+
+// cv2's INTER_AREA downscale by integer factors other than 2 x 2 (ResizeAreaFast_Invoker's scalar loop): the int sum of the
+// fy x fx block times float32 1 / (fx * fy), rounded half to even.
+__device__ __forceinline__ void area_int_px(const uint8_t* __restrict__ src, const ImgDesc& d, int dy, int dx, int v[3]) {
+  const int fy = __double2int_rn(d.scale_y), fx = __double2int_rn(d.scale_x);
+  int sum[3] = {0, 0, 0};
+  for (int r = dy * fy; r < dy * fy + fy; ++r)
+    for (int c = dx * fx; c < dx * fx + fx; ++c) {
+      int p[3];
+      canvas_px(src, d, r, c, p);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) sum[k] += p[k];
+    }
+  const float scale = __fdiv_rn(1.f, (float)(fx * fy));
+#pragma unroll
+  for (int k = 0; k < 3; ++k) v[k] = min(max(__float2int_rn(__fmul_rn((float)sum[k], scale)), 0), 255);
+}
+
+// kWarp: the batch has a SCALE; kWide: it has a RESIZE_INTERP with cubic, Lanczos4 or area taps.  Batches without them run an
+// instantiation that carries none of that code (fewer registers).
+template <bool kWarp, bool kWide>
+__device__ __forceinline__ void assemble_row(const uint8_t* __restrict__ src, const ImgDesc* __restrict__ descs, int out_h, int out_w,
+                                             float* __restrict__ out) {
   const int b = blockIdx.y, dy = blockIdx.x;
   const ImgDesc d = descs[b];
   float* orow = out + ((size_t)b * out_h + dy) * (size_t)out_w * 3;
@@ -314,14 +485,27 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8
   int r0 = dy, r1 = dy, b0 = 2048, b1 = 0;
   if (d.mode == kImgNearest) {
     r0 = min((int)floor(__dmul_rn((double)dy, d.scale_y)), d.ch - 1);
-  } else if (d.mode == kImgLinear) {
+  } else if (d.mode == kImgLinear || (kWide && d.mode == kWideAreaUp)) {
     int s; float f;
-    linear_coord(dy, d.scale_y, s, f);
+    if (d.mode == kImgLinear) linear_coord(dy, d.scale_y, s, f);
+    else area_coord(dy, d.scale_y, (double)out_h / (double)d.ch, s, f);
     r0 = min(max(s, 0), d.ch - 1); r1 = min(max(s + 1, 0), d.ch - 1);
     b0 = coef11(__fsub_rn(1.f, f)); b1 = coef11(f);
   } else if (d.mode == kImgArea2) {
     r0 = 2 * dy; r1 = 2 * dy + 1;
   }
+  int kb[8] = {0, 0, 0, 0, 0, 0, 0, 0};                           // cubic / Lanczos4 row coefficients; r0 = first row
+  AreaSpan ys{};
+  if (kWide) {
+    if (d.mode == kWideCubic || d.mode == kWideLanczos4) {
+      float f;
+      linear_coord(dy, d.scale_y, r0, f);
+      if (d.mode == kWideCubic) cubic_coefs(f, kb); else lanczos_coefs(f, kb);
+    } else if (d.mode == kWideArea) {
+      ys = area_span(dy, d.ch, d.scale_y);
+    }
+  }
+  const int vec_end = out_w * 3 / 8 * 8;
   for (int dx = threadIdx.x; dx < out_w; dx += kImgThreads) {
     int v[3];
     if (d.mode == kImgCopy) {
@@ -341,26 +525,33 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8
       canvas_px(src, d, r1, 2 * dx, q); canvas_px(src, d, r1, 2 * dx + 1, r);
 #pragma unroll
       for (int k = 0; k < 3; ++k) v[k] = (v[k] + p[k] + q[k] + r[k] + 2) >> 2;
+    } else if (kWide && d.mode == kWideCubic) {
+      kernel_px<4>(src, d, r0, kb, dx, vec_end, v);
+    } else if (kWide && d.mode == kWideLanczos4) {
+      kernel_px<8>(src, d, r0, kb, dx, vec_end, v);
+    } else if (kWide && d.mode == kWideArea) {
+      area_px(src, d, ys, dx, v);
+    } else if (kWide && d.mode == kWideAreaInt) {
+      area_int_px(src, d, dy, dx, v);
     } else {
-      // columns past either border take the edge pixel with weight 2048
       int s; float f;
-      linear_coord(dx, d.scale_x, s, f);
-      if (s < 0) { s = 0; f = 0.f; }
-      if (s >= d.cw - 1) { s = d.cw - 1; f = 0.f; }
-      const int c1 = min(s + 1, d.cw - 1);
-      const int a0 = coef11(__fsub_rn(1.f, f)), a1 = coef11(f);
-      int p01[3], p10[3], p11[3];
-      canvas_px(src, d, r0, s, v); canvas_px(src, d, r0, c1, p01);
-      canvas_px(src, d, r1, s, p10); canvas_px(src, d, r1, c1, p11);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const int S0 = v[k] * a0 + p01[k] * a1, S1 = p10[k] * a0 + p11[k] * a1;      // horizontal pass, int
-        const int t = (((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2;  // cv2's vertical pass on 8-bit
-        v[k] = min(max(t, 0), 255);
-      }
+      if (kWide && d.mode == kWideAreaUp) area_coord(dx, d.scale_x, (double)out_w / (double)d.cw, s, f);
+      else linear_coord(dx, d.scale_x, s, f);
+      linear_cols(src, d, r0, r1, b0, b1, s, f, v);
     }
     orow[dx * 3 + 0] = (float)v[0]; orow[dx * 3 + 1] = (float)v[1]; orow[dx * 3 + 2] = (float)v[2];
   }
+}
+
+template <bool kWarp>
+__global__ void __launch_bounds__(kImgThreads) image_assemble_kernel(const uint8_t* __restrict__ src, const ImgDesc* __restrict__ descs,
+                                                                     int out_h, int out_w, float* __restrict__ out) {
+  assemble_row<kWarp, false>(src, descs, out_h, out_w, out);
+}
+template <bool kWarp>
+__global__ void __launch_bounds__(kImgThreads) image_assemble_kernel_wide(const uint8_t* __restrict__ src, const ImgDesc* __restrict__ descs,
+                                                                          int out_h, int out_w, float* __restrict__ out) {
+  assemble_row<kWarp, true>(src, descs, out_h, out_w, out);
 }
 
 // ---- the photometric prefix ----
@@ -555,7 +746,8 @@ int compose_photo(int b, const ssdk_box_op* ops, int max_ops, PhotoDesc* out) {
     const ssdk_box_op& op = ops[(size_t)b * max_ops + i];
     if (op.op == SSDK_BOXOP_END) break;
     if (!is_photo(op.op)) {
-      geometric = geometric || (op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE && op.op != SSDK_BOXOP_FILTER);
+      geometric = geometric || (op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE && op.op != SSDK_BOXOP_FILTER) ||
+                  op.op == SSDK_BOXOP_RESIZE_INTERP;
       continue;
     }
     SSDK_REQUIRE(!geometric, "ssdk_assemble_images: image %d, op %d: photometric ops must come before every op that changes the "
@@ -694,6 +886,17 @@ bool rotate_op(long long h, long long w, double angle, IntOp& op) {
   return true;
 }
 
+// Which of cv2.resize's INTER_AREA paths a ch x cw -> rh x rw resize takes: integer factors in both axes (to within DBL_EPSILON
+// of 1 / (out / in)) take ResizeAreaFast (2 x 2 its vector rule), other downscales resizeArea_, and a resize that upscales
+// either axis is linear with area coordinates.
+int area_mode(long long ch, long long cw, long long rh, long long rw) {
+  const double sx = 1.0 / ((double)rw / (double)cw), sy = 1.0 / ((double)rh / (double)ch);
+  if (!(sx >= 1 && sy >= 1)) return kWideAreaUp;
+  const double ix = std::nearbyint(sx), iy = std::nearbyint(sy);
+  if (!(std::fabs(sx - ix) < DBL_EPSILON && std::fabs(sy - iy) < DBL_EPSILON)) return kWideArea;
+  return ix == 2 && iy == 2 ? kImgArea2 : kWideAreaInt;
+}
+
 // Compose image b's op list into its descriptor; every check the entry point documents.
 int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_op* ops, int max_ops, int out_h, int out_w, ImgDesc* out) {
   const int h = hwc[3 * b], w = hwc[3 * b + 1], c = hwc[3 * b + 2];
@@ -712,7 +915,8 @@ int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_o
     if (op.op == SSDK_BOXOP_END) break;
     if (op.op == SSDK_BOXOP_FILTER || op.op == SSDK_BOXOP_OVERLAP || op.op == SSDK_BOXOP_CLIP) continue;   // boxes only
     if (is_photo(op.op)) continue;                                  // run by photometric_kernel (compose_photo)
-    SSDK_REQUIRE(op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE, "ssdk_assemble_images: image %d, op %d: unknown op code %d", b, i, op.op);
+    SSDK_REQUIRE((op.op >= SSDK_BOXOP_CROP_PAD && op.op <= SSDK_BOXOP_ROTATE) || op.op == SSDK_BOXOP_RESIZE_INTERP,
+                 "ssdk_assemble_images: image %d, op %d: unknown op code %d", b, i, op.op);
     SSDK_REQUIRE(!resized, "ssdk_assemble_images: image %d, op %d: the RESIZE must be the last op that changes the image", b, i);
     const long long ch = cur->h, cw = cur->w;
     const int col = (int)(((unsigned)op.flags >> 8) & 0xFFFFFFu);
@@ -755,10 +959,15 @@ int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_o
         SSDK_REQUIRE(is_int(op.a2) && is_int(op.a3) && op.a2 > 0 && op.a3 > 0, "ssdk_assemble_images: image %d, op %d: RESIZE needs a "
                      "positive integer output size", b, i);
         const int interp = (op.flags >> 8) & 255;
-        SSDK_REQUIRE(interp == 0 || interp == 1, "ssdk_assemble_images: image %d, op %d: interpolation mode %d is not supported "
-                     "(INTER_NEAREST = 0 and INTER_LINEAR = 1 are)", b, i, interp);
+        if (op.op == SSDK_BOXOP_RESIZE)
+          SSDK_REQUIRE(interp == 0 || interp == 1, "ssdk_assemble_images: image %d, op %d: interpolation mode %d is not supported "
+                       "(INTER_NEAREST = 0 and INTER_LINEAR = 1 are)", b, i, interp);
+        else
+          SSDK_REQUIRE(interp <= 4, "ssdk_assemble_images: image %d, op %d: interpolation mode %d is not supported (RESIZE_INTERP "
+                       "takes INTER_NEAREST = 0, INTER_LINEAR = 1, INTER_CUBIC = 2, INTER_AREA = 3 and INTER_LANCZOS4 = 4)", b, i, interp);
         resized = true; rh = (long long)op.a2; rw = (long long)op.a3;
         mode = interp == 0 ? kImgNearest : kImgLinear;
+        if (interp >= 2) mode = interp == 2 ? kWideCubic : interp == 3 ? kWideArea : kWideLanczos4;
         continue;
       }
       SSDK_REQUIRE(op.a1 == (double)ch && op.a2 == (double)cw, "ssdk_assemble_images: image %d, op %d: SCALE of a %gx%g image, but the "
@@ -792,6 +1001,7 @@ int compose_image(int b, const long long* offs, const int* hwc, const ssdk_box_o
                  "ssdk_assemble_images: image %d: canvas too large", b);
   if (resized && rh == ch && rw == cw) mode = kImgCopy;            // cv2.resize to the same size is a copy
   else if (mode == kImgLinear && ch == 2 * rh && cw == 2 * rw) mode = kImgArea2;
+  else if (mode == kWideArea) mode = area_mode(ch, cw, rh, rw);
   ImgDesc& d = *out;
   d.src_off = offs[b]; d.h = h; d.w = w; d.c = c;
   d.ch = (int)ch; d.cw = (int)cw;
@@ -860,6 +1070,10 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
     if (rc) return rc;
   }
   const bool warp = std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; });
+  const bool wide = std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return is_wide(d.mode); });
+  if (wide)
+    return launch(ctx, warp ? image_assemble_kernel_wide<true> : image_assemble_kernel_wide<false>, dim3(out_h, B), kImgThreads, 0,
+                  stream, src_dev, d_dev, out_h, out_w, out_dev);
   return launch(ctx, warp ? image_assemble_kernel<true> : image_assemble_kernel<false>, dim3(out_h, B), kImgThreads, 0, stream,
                 src_dev, d_dev, out_h, out_w, out_dev);
 }

@@ -19,6 +19,9 @@ one list moves the boxes and produces the image batch; ``assemble_training_batch
 - ``flip(width_or_height, dim)``: ``Flip``;
 - ``resize(..., interpolation_mode=1)``: uint8 ``cv2.resize`` with ``INTER_NEAREST`` (0) or ``INTER_LINEAR`` (1), bit-exact
   to OpenCV 4.13 (``oracle/imageops.py`` restates it); nothing that changes the image may follow it;
+- ``resize_interp(..., interpolation_mode)``: the same step with every mode ``ResizeRandomInterp`` draws, ``INTER_CUBIC`` (2),
+  ``INTER_AREA`` (3) and ``INTER_LANCZOS4`` (4) too, bit-exact to OpenCV 4.13's own resize code (``tests/resize_reference.py``
+  restates the three); its boxes are ``resize``'s;
 - ``translate`` / ``scale`` / ``rotate``: ``Translate`` / ``Scale`` / ``Rotate`` (``geometric_ops.py:233-737``), uint8
   ``cv2.warpAffine`` with ``INTER_LINEAR`` and ``BORDER_CONSTANT``, bit-exact to OpenCV 4.13.  ``translate`` and ``rotate``
   (90 / 180 / 270) are exact integer maps; ``scale`` is a bilinear warp.  A list holds at most one resampling step
@@ -36,10 +39,10 @@ sequence one call of the reference class runs, box filter and clipping included,
 ``DataAugmentationConstantInputSize`` (SSD7: translate -> zoom in -> flip, or zoom out -> translate -> flip) and
 ``DataAugmentationSatellite`` (flips -> rotate -> patch -> resize) are one op list per image.
 
-Not covered: ``Gamma`` (the reference's raises), histogram equalisation, conversion to GRAY, other interpolation modes (``INTER_CUBIC``, ``INTER_LANCZOS4``, ``INTER_AREA`` apart from
-cv2's own exact-2x linear path), a second resampling step, the random samplers (``RandomTranslate`` / ``RandomScale``'s draws,
-``ImageValidator`` retries, ``RandomPatch``), JPEG decoding.  The random decisions of a chain (which patch, flip or not, which
-factor, which photometric op with which delta) stay with the caller, as for the boxes."""
+Not covered: ``Gamma`` (the reference's raises), histogram equalisation, conversion to GRAY, a second resampling step, JPEG
+decoding.  The random decisions of a chain (which patch, flip or not, which factor, which photometric op with which delta) are
+the caller's: ``data_augmentation_chain_original_ssd`` draws them for the original SSD chain, in the reference's ``np.random``
+order, and ``DataGenerator.generate`` runs them; the SSD7, variable-input-size and satellite chains' samplers are not restated."""
 import ctypes as C
 
 import numpy as np
@@ -77,6 +80,16 @@ def resize(in_height, in_width, out_height, out_width, drop_degenerate=True, int
         raise ValueError('`interpolation_mode` must be a cv2 interpolation code')
     return (_ffi.BOXOP_RESIZE, (1 if drop_degenerate else 0) | (mode << 8), float(in_height), float(in_width), float(out_height),
             float(out_width))
+
+
+def resize_interp(in_height, in_width, out_height, out_width, interpolation_mode, drop_degenerate=True):
+    """``Resize`` with any of the five cv2 codes ``ResizeRandomInterp`` draws from: ``INTER_NEAREST`` (0), ``INTER_LINEAR`` (1),
+    ``INTER_CUBIC`` (2), ``INTER_AREA`` (3), ``INTER_LANCZOS4`` (4).  The boxes are ``resize``'s."""
+    mode = int(interpolation_mode)
+    if not 0 <= mode <= 4:
+        raise ValueError('`interpolation_mode` must be one of the cv2 codes 0-4')
+    return (_ffi.BOXOP_RESIZE_INTERP, (1 if drop_degenerate else 0) | (mode << 8), float(in_height), float(in_width),
+            float(out_height), float(out_width))
 
 
 def box_filter(check_degenerate=True, min_area=None):

@@ -1,0 +1,261 @@
+"""``DataGenerator`` (the reference's object_detection_2d_data_generator.py): a dataset of images and labels, and ``generate()``,
+which yields training batches assembled on the device.
+
+Per batch, the host does what only the host can: the shuffle (``sklearn.utils.shuffle``'s permutation, drawn from the global
+``np.random``), the batch slice, dropping images without boxes, and the random draws of the augmentation planners
+(``data_augmentation_chain_original_ssd``), which turn each image into one op list.  Images are decoded with PIL on a small
+thread pool ahead of the batch that needs them (or taken from memory).  The device then runs one assembly per batch:
+``ssdk_assemble_images`` for the pixels, ``ssdk_assemble_batch`` for the boxes and the encoder on its output
+(``batch_assembly.assemble_training_batch``), so ``'processed_images'`` and ``'encoded_labels'`` are the float32 CUDA tensors
+``train_on_batch`` takes.
+
+The reference checks the processed boxes for degenerate ones after the chain.  When every op list of a batch ends in a
+degenerate-box filter (``Resize`` with one, as in ``SSDDataAugmentation``), no box can be degenerate and nothing is checked;
+otherwise the processed boxes are read back once and the reference's ``'remove'`` / ``'warn'`` rules are applied to them.
+
+Not covered: HDF5 datasets, the XML / CSV / JSON parsers, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
+transformations other than the planners of this package."""
+import os
+import pickle
+import warnings
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+
+from . import batch_assembly as ba
+from .. import _ffi
+from ..eval_utils.dataset_predict import load_image
+from .object_detection_2d_geometric_ops import DevicePlanner
+
+_DECODE_THREADS = 8
+_DECODE_AHEAD = 2                      # batches decoded ahead of the one being assembled
+
+
+class DegenerateBatchError(Exception):
+    """An error indicating that an empty batch was produced."""
+
+
+class DatasetError(Exception):
+    """An error indicating that something is wrong with the dataset."""
+
+
+def _load_list(value, name):
+    if value is None or isinstance(value, (list, tuple)):
+        return value
+    if isinstance(value, str):
+        with open(value, 'rb') as f:
+            return pickle.load(f)
+    raise ValueError('`%s` must be either a Python list/tuple or a string representing the path to a pickled file containing a '
+                     'list/tuple. The value you passed is neither of the two.' % name)
+
+
+def shuffle_together(objects):
+    """``sklearn.utils.shuffle(*objects)`` written back in place: one permutation from the global ``np.random``
+    (``np.random.shuffle(np.arange(n))``) applied to every list / array."""
+    perm = np.arange(len(objects[0]))
+    np.random.shuffle(perm)
+    for o in objects:
+        o[:] = [o[i] for i in perm] if isinstance(o, list) else o[perm]
+
+
+def _has_degenerate(labels, fmt):
+    return bool(np.any(labels[:, fmt['xmax']] - labels[:, fmt['xmin']] <= 0) or np.any(labels[:, fmt['ymax']] - labels[:, fmt['ymin']] <= 0))
+
+
+def _ends_degenerate_free(ops):
+    """Whether the list leaves no degenerate box: its last op that moves or filters boxes is a degenerate-box filter (an
+    overlap test or a photometric op after it changes no box)."""
+    for code, flags in ((o[0], o[1]) for o in reversed(ops)):
+        if code in (_ffi.BOXOP_RESIZE, _ffi.BOXOP_RESIZE_INTERP, _ffi.BOXOP_FILTER):
+            return bool(flags & 1)
+        if code != _ffi.BOXOP_OVERLAP and not _ffi.BOXOP_TO_FLOAT32 <= code <= _ffi.BOXOP_CHANNEL_SWAP:
+            return False
+    return False
+
+
+class DataGenerator:
+    """A dataset of images (files, or arrays in memory) with their labels, image ids and evaluation-neutral flags."""
+
+    def __init__(self, load_images_into_memory=False, hdf5_dataset_path=None, filenames=None, filenames_type='text', images_dir=None,
+                 labels=None, image_ids=None, eval_neutral=None, labels_output_format=('class_id', 'xmin', 'ymin', 'xmax', 'ymax'),
+                 verbose=True):
+        if hdf5_dataset_path is not None:
+            raise NotImplementedError('HDF5 datasets are not supported; pass `filenames` (and `labels`)')
+        self.labels_output_format = labels_output_format
+        self.labels_format = {k: labels_output_format.index(k) for k in ('class_id', 'xmin', 'ymin', 'xmax', 'ymax')}
+        self.dataset_size = 0
+        self.load_images_into_memory = load_images_into_memory
+        self.images = None
+        self.hdf5_dataset = None
+        self.filenames = None
+        if filenames is not None:
+            if isinstance(filenames, (list, tuple)):
+                self.filenames = list(filenames)
+            elif isinstance(filenames, str):
+                if filenames_type == 'pickle':
+                    with open(filenames, 'rb') as f:
+                        self.filenames = pickle.load(f)
+                elif filenames_type == 'text':
+                    with open(filenames) as f:
+                        self.filenames = [os.path.join(images_dir, line.strip()) for line in f]
+                else:
+                    raise ValueError("`filenames_type` can be either 'text' or 'pickle'.")
+            else:
+                raise ValueError('`filenames` must be either a Python list/tuple or a string representing a filepath (to a pickled '
+                                 'or text file). The value you passed is neither of the two.')
+            self.dataset_size = len(self.filenames)
+            self.dataset_indices = np.arange(self.dataset_size, dtype=np.int32)
+            if load_images_into_memory:
+                with ThreadPoolExecutor(_DECODE_THREADS) as pool:
+                    self.images = list(pool.map(load_image, self.filenames))
+        self.labels = _load_list(labels, 'labels')
+        self.image_ids = _load_list(image_ids, 'image_ids')
+        self.eval_neutral = _load_list(eval_neutral, 'eval_neutral')
+
+    def get_dataset(self):
+        return self.filenames, self.labels, self.image_ids, self.eval_neutral
+
+    def get_dataset_size(self):
+        return self.dataset_size
+
+    def generate(self, batch_size=32, shuffle=True, transformations=[], label_encoder=None, returns={'processed_images', 'encoded_labels'},
+                 keep_images_without_gt=False, degenerate_box_handling='remove'):
+        """Yields batches indefinitely, as the reference's ``generate`` (same arguments and return order), from a device assembly
+        of each batch.  ``transformations``: planners of this package (``SSDDataAugmentation``, its parts, ``Resize``,
+        ``ResizeRandomInterp``, ``RandomFlip``, ``ConvertTo3Channels``); after them every image of a batch must have one size.
+        ``'processed_images'`` is a float32 CUDA tensor ``(B, H, W, 3)``; ``'encoded_labels'`` the float32 CUDA ``y_true``;
+        ``'processed_labels'`` a list of float64 arrays read back from the device."""
+        if self.dataset_size == 0:
+            raise DatasetError('Cannot generate batches because you did not load a dataset.')
+        for r in ('matched_anchors', 'inverse_transform'):
+            if r in returns:
+                raise NotImplementedError("the '%s' return is not supported" % r)
+        for t in transformations:
+            if not isinstance(t, DevicePlanner):
+                raise NotImplementedError('transformation %r is not one the device generator knows; use the planners of '
+                                          'ssd_keras_b200.data_generator' % (t,))
+        if self.labels is not None and self.labels_format != {'class_id': 0, 'xmin': 1, 'ymin': 2, 'xmax': 3, 'ymax': 4}:
+            raise NotImplementedError("the device generator takes labels as ('class_id', 'xmin', 'ymin', 'xmax', 'ymax')")
+        if degenerate_box_handling not in ('remove', 'warn'):
+            raise ValueError("`degenerate_box_handling` must be either 'remove' or 'warn'")
+        if self.labels is None:
+            if any(r in returns for r in ('encoded_labels', 'processed_labels', 'original_labels')):
+                warnings.warn('Since no labels were given, none of the label returns are possible; they will be `None`.')
+        elif label_encoder is None and 'encoded_labels' in returns:
+            warnings.warn("Since no label encoder was given, 'encoded_labels' is not possible; it will be `None`.")
+        for t in transformations:
+            t.labels_format = self.labels_format
+        with ThreadPoolExecutor(_DECODE_THREADS) as pool:
+            for batch in self.plan_batches(batch_size, shuffle, transformations, keep_images_without_gt, pool):
+                batch_X, batch_y, keep, ops, out_hw = (batch[k] for k in ('images', 'labels', 'keep', 'ops', 'out_hw'))
+                batch_filenames, batch_image_ids, batch_eval_neutral = batch['filenames'], batch['image_ids'], batch['eval_neutral']
+                batch_original_images = [np.copy(x) for x in batch_X] if 'original_images' in returns else None
+                batch_original_labels = [np.copy(y) for y in batch_y] if 'original_labels' in returns and batch_y is not None else None
+                if batch_y is not None and keep and not all(_ends_degenerate_free(o) for o in ops):
+                    keep, ops = self._degenerate_check(batch_X, batch_y, keep, ops, degenerate_box_handling, keep_images_without_gt)
+                if not keep:
+                    raise DegenerateBatchError('You produced an empty batch.')
+
+                def pick(lst):
+                    return None if lst is None else [lst[i] for i in keep]
+                X_in, y_in = [batch_X[i] for i in keep], pick(batch_y)
+                if batch_y is not None and label_encoder is not None:
+                    X, y_enc = ba.assemble_training_batch(label_encoder, X_in, y_in, ops, out_hw[0], out_hw[1])
+                else:
+                    X, y_enc = ba.assemble_images_device(X_in, ops, out_hw[0], out_hw[1]), None
+                processed = None
+                if 'processed_labels' in returns and batch_y is not None:
+                    gt, offs = ba.assemble_batch_device(y_in, ops)[:2]
+                    gt, offs = gt.cpu().numpy().astype(np.float64), offs.cpu().numpy()
+                    processed = [gt[offs[b]:offs[b + 1]] for b in range(len(keep))]
+                ret = []
+                if 'processed_images' in returns: ret.append(X)
+                if 'encoded_labels' in returns: ret.append(y_enc)
+                if 'processed_labels' in returns: ret.append(processed)
+                if 'filenames' in returns: ret.append(pick(batch_filenames))
+                if 'image_ids' in returns: ret.append(pick(batch_image_ids))
+                if 'evaluation-neutral' in returns: ret.append(pick(batch_eval_neutral))
+                if 'original_images' in returns: ret.append(pick(batch_original_images))
+                if 'original_labels' in returns: ret.append(pick(batch_original_labels))
+                yield ret
+
+    def plan_batches(self, batch_size, shuffle, transformations, keep_images_without_gt, pool=None):
+        """The host half of ``generate``: shuffles, slices, drops the images without boxes and draws every kept image's op
+        list, in the reference's ``np.random`` order.  Yields dicts with the batch's ``images``, ``labels`` (arrays),
+        ``filenames``, ``image_ids``, ``eval_neutral``, the indices ``keep`` of the images that go on, their ``ops`` and the
+        common output size ``out_hw``."""
+        if shuffle:
+            self._shuffle()
+        current = 0
+        ahead = {}
+        while True:
+            if current >= self.dataset_size:
+                current = 0
+                if shuffle:
+                    ahead.clear()
+                    self._shuffle()
+            for k in range(_DECODE_AHEAD + 1 if pool is not None else 1):
+                lo = current + k * batch_size
+                if lo < self.dataset_size and lo not in ahead:
+                    ahead[lo] = self._fetch(pool, lo, batch_size)
+            batch_X = [a.result() if hasattr(a, 'result') else a for a in ahead.pop(current)]
+            sl = slice(current, current + batch_size)
+            batch_y = [np.array(y) for y in self.labels[sl]] if self.labels is not None else None
+            current += batch_size
+            keep, ops, out_hw = [], [], None
+            for i, x in enumerate(batch_X):
+                labels = batch_y[i] if batch_y is not None else None
+                if labels is not None and labels.size == 0 and not keep_images_without_gt:
+                    continue                                       # no draws for an image without boxes
+                o, h, w = [], x.shape[0], x.shape[1]
+                for t in transformations:
+                    o_t, h, w, labels = t.plan(h, w, labels)
+                    o += o_t
+                if out_hw is None:
+                    out_hw = (h, w)
+                elif out_hw != (h, w):
+                    raise DegenerateBatchError('You produced an empty batch. This might be because the images in the batch vary in '
+                                               'their size and/or number of channels. Note that after all transformations (if any '
+                                               'were given) have been applied to all images in the batch, all images must be '
+                                               'homogenous in size along all axes.')
+                keep.append(i)
+                ops.append(o)
+            yield dict(images=batch_X, labels=batch_y, keep=keep, ops=ops, out_hw=out_hw,
+                       filenames=list(self.filenames[sl]) if self.filenames is not None else None,
+                       image_ids=list(self.image_ids[sl]) if self.image_ids is not None else None,
+                       eval_neutral=list(self.eval_neutral[sl]) if self.eval_neutral is not None else None)
+
+    def _shuffle(self):
+        objects = [self.dataset_indices]
+        for o in (self.filenames, self.labels, self.image_ids, self.eval_neutral):
+            if o is not None:
+                objects.append(o)
+        shuffle_together(objects)
+
+    def _fetch(self, pool, lo, batch_size):
+        idx = self.dataset_indices[lo:lo + batch_size]
+        if self.images is not None:
+            return [self.images[i] for i in idx]
+        names = self.filenames[lo:lo + batch_size]
+        return [pool.submit(load_image, f) for f in names] if pool is not None else [load_image(f) for f in names]
+
+    def _degenerate_check(self, batch_X, batch_y, keep, ops, handling, keep_images_without_gt):
+        """The reference's check on the processed boxes (one read-back): 'warn' warns, 'remove' filters the degenerate boxes and
+        drops the images it empties (unless ``keep_images_without_gt``); the filter joins the image's op list."""
+        gt, offs = ba.assemble_batch_device([batch_y[i] for i in keep], ops)[:2]
+        gt, offs = gt.cpu().numpy(), offs.cpu().numpy()
+        new_keep, new_ops = [], []
+        for b, (i, o) in enumerate(zip(keep, ops)):
+            labels = gt[offs[b]:offs[b + 1]]
+            if _has_degenerate(labels, {'xmin': 1, 'ymin': 2, 'xmax': 3, 'ymax': 4}):
+                if handling == 'warn':
+                    warnings.warn('Detected degenerate ground truth bounding boxes for batch item {} with bounding boxes {}, i.e. '
+                                  'bounding boxes where xmax <= xmin and/or ymax <= ymin.'.format(i, labels))
+                else:
+                    o = o + [ba.box_filter(check_degenerate=True)]
+                    survivors = (labels[:, 3] > labels[:, 1]) & (labels[:, 4] > labels[:, 2])
+                    if not survivors.any() and not keep_images_without_gt:
+                        continue
+            new_keep.append(i)
+            new_ops.append(o)
+        return new_keep, new_ops
