@@ -41,8 +41,8 @@ sequence one call of the reference class runs, box filter and clipping included,
 
 Not covered: ``Gamma`` (the reference's raises), histogram equalisation, conversion to GRAY, a second resampling step, JPEG
 decoding.  The random decisions of a chain (which patch, flip or not, which factor, which photometric op with which delta) are
-the caller's: ``data_augmentation_chain_original_ssd`` draws them for the original SSD chain, in the reference's ``np.random``
-order, and ``DataGenerator.generate`` runs them; the SSD7, variable-input-size and satellite chains' samplers are not restated."""
+the caller's: the planners of ``data_augmentation_chain_original_ssd``, ``_constant_input_size`` (SSD7), ``_variable_input_size``
+and ``_satellite`` draw them in the reference's order, and ``DataGenerator.generate`` runs them."""
 import ctypes as C
 
 import numpy as np
@@ -221,8 +221,9 @@ _BOX_FILTER_DEFAULTS = dict(check_overlap=True, check_min_area=True, check_degen
 def box_filter_ops(spec, img_height, img_width):
     """The ops of one ``BoxFilter.__call__`` (validation_utils.py:147-232) against an ``img_height x img_width`` image: the
     degenerate / minimum-area test, then the overlap test (all three are ANDed there, so the order does not matter).  ``spec``
-    is a dict of ``BoxFilter``'s keyword arguments (its defaults fill the rest) or any object with those attributes, a
-    reference ``BoxFilter`` included; ``None`` gives no ops.  Fixed bounds only (no ``BoundGenerator``)."""
+    is a ``BoxFilter`` (``object_detection_2d_image_boxes_validation_utils``, or the reference's), a dict of ``BoxFilter``'s
+    keyword arguments (its defaults fill the rest) or any object with those attributes; ``None`` gives no ops.  Fixed bounds
+    only (no ``BoundGenerator``)."""
     if spec is None:
         return []
     if isinstance(spec, dict):

@@ -11,6 +11,7 @@ import numpy as np
 
 from . import batch_assembly as ba
 from .object_detection_2d_geometric_ops import DEFAULT_LABELS_FORMAT, DevicePlanner, RandomFlip, ResizeRandomInterp
+from .object_detection_2d_image_boxes_validation_utils import iou_with_image
 
 _DEGENERATE_ONLY = dict(check_overlap=False, check_min_area=False, check_degenerate=True)
 
@@ -36,19 +37,6 @@ def _origin(img_height, img_width, patch_height, patch_width):
     x_range = img_width - patch_width
     patch_xmin = np.random.randint(0, x_range + 1) if x_range >= 0 else np.random.randint(x_range, 1)
     return patch_ymin, patch_xmin, patch_height, patch_width
-
-
-def _iou_with_image(labels, img_height, img_width, fmt):
-    """``bounding_box_utils.iou(np.array([0, 0, w, h]), boxes, coords='corners', mode='element-wise', border_pixels='half')``."""
-    boxes = labels[:, [fmt['xmin'], fmt['ymin'], fmt['xmax'], fmt['ymax']]]
-    image = np.array([[0, 0, img_width, img_height]])
-    min_xy = np.maximum(image[:, [0, 1]], boxes[:, [0, 1]])
-    max_xy = np.minimum(image[:, [2, 3]], boxes[:, [2, 3]])
-    side_lengths = np.maximum(0, max_xy - min_xy)
-    intersection = side_lengths[:, 0] * side_lengths[:, 1]
-    image_area = (image[:, 2] - image[:, 0]) * (image[:, 3] - image[:, 1])
-    box_areas = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1])
-    return intersection / (image_area + box_areas - intersection)
 
 
 class SSDPhotometricDistortions(DevicePlanner):
@@ -108,7 +96,7 @@ class SSDRandomCrop(DevicePlanner):
         new_labels = np.copy(labels)
         new_labels[:, [fmt['ymin'], fmt['ymax']]] -= patch_ymin
         new_labels[:, [fmt['xmin'], fmt['xmax']]] -= patch_xmin
-        ious = _iou_with_image(new_labels, patch_height, patch_width, fmt)
+        ious = iou_with_image(new_labels[:, [fmt['xmin'], fmt['ymin'], fmt['xmax'], fmt['ymax']]], patch_height, patch_width)
         return np.count_nonzero((ious > lower) * (ious <= upper)) >= 1
 
     def plan(self, img_height, img_width, labels):

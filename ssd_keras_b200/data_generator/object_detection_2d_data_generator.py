@@ -1,20 +1,24 @@
 """``DataGenerator`` (the reference's object_detection_2d_data_generator.py): a dataset of images and labels, and ``generate()``,
 which yields training batches assembled on the device.
 
+``parse_csv`` reads a dataset from a CSV of boxes, as the reference's does (the XML and JSON parsers are not restated).
+
 Per batch, the host does what only the host can: the shuffle (``sklearn.utils.shuffle``'s permutation, drawn from the global
-``np.random``), the batch slice, dropping images without boxes, and the random draws of the augmentation planners
-(``data_augmentation_chain_original_ssd``), which turn each image into one op list.  Images are decoded with PIL on a small
+``np.random``), the batch slice, dropping images without boxes, and the random draws of the augmentation planners (the
+``data_augmentation_chain_*`` modules and their parts), which turn each image into one op list.  Images are decoded with PIL on a small
 thread pool ahead of the batch that needs them (or taken from memory).  The device then runs one assembly per batch:
 ``ssdk_assemble_images`` for the pixels, ``ssdk_assemble_batch`` for the boxes and the encoder on its output
 (``batch_assembly.assemble_training_batch``), so ``'processed_images'`` and ``'encoded_labels'`` are the float32 CUDA tensors
 ``train_on_batch`` takes.
 
 The reference checks the processed boxes for degenerate ones after the chain.  When every op list of a batch ends in a
-degenerate-box filter (``Resize`` with one, as in ``SSDDataAugmentation``), no box can be degenerate and nothing is checked;
-otherwise the processed boxes are read back once and the reference's ``'remove'`` / ``'warn'`` rules are applied to them.
+degenerate-box filter (``Resize`` with one, as in ``SSDDataAugmentation`` and the variable-input-size and satellite chains), no
+box can be degenerate and nothing is checked; otherwise (the SSD7 chain's lists end in a flip, or in the clip of a translation
+or zoom) the processed boxes are read back once and the reference's ``'remove'`` / ``'warn'`` rules are applied to them.
 
-Not covered: HDF5 datasets, the XML / CSV / JSON parsers, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
+Not covered: HDF5 datasets, the XML and JSON parsers, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
 transformations other than the planners of this package."""
+import csv
 import os
 import pickle
 import warnings
@@ -112,6 +116,54 @@ class DataGenerator:
         self.image_ids = _load_list(image_ids, 'image_ids')
         self.eval_neutral = _load_list(eval_neutral, 'eval_neutral')
 
+    def parse_csv(self, images_dir, labels_filename, input_format, include_classes='all', random_sample=False, ret=False, verbose=True):
+        """The reference's ``parse_csv``: one box per CSV row (after a header), its first six columns named by ``input_format``
+        (``'image_name'``, ``'class_id'``, ``'xmin'``, ``'xmax'``, ``'ymin'``, ``'ymax'``).  Rows of ``include_classes`` are sorted
+        (by file name, then by the label values), grouped by file into int64 label arrays in ``labels_output_format`` order, and
+        the image id is the file name up to its first dot.  ``random_sample``: each image is kept if ``np.random.uniform(0, 1)
+        >= 1 - random_sample``, one draw per image in file order.  With ``ret``, returns ``(images, filenames, labels,
+        image_ids)``."""
+        self.images_dir = images_dir
+        self.labels_filename = labels_filename
+        self.input_format = input_format
+        self.include_classes = include_classes
+        if self.labels_filename is None or self.input_format is None:
+            raise ValueError("`labels_filename` and/or `input_format` have not been set yet. You need to pass them as arguments.")
+        self.filenames = []
+        self.image_ids = []
+        self.labels = []
+        data = []
+        with open(self.labels_filename, newline='') as csvfile:
+            csvread = csv.reader(csvfile, delimiter=',')
+            next(csvread)
+            for row in csvread:
+                if self.include_classes == 'all' or int(row[self.input_format.index('class_id')].strip()) in self.include_classes:
+                    box = [row[self.input_format.index('image_name')].strip()]
+                    for element in self.labels_output_format:
+                        box.append(int(row[self.input_format.index(element)].strip()))
+                    data.append(box)
+        data = sorted(data)
+        groups = []                                          # (file name, its boxes) in sorted order
+        for box in data:
+            if not groups or box[0] != groups[-1][0]:
+                groups.append((box[0], []))
+            groups[-1][1].append(box[1:])
+        if not groups:
+            raise IndexError('list index out of range')      # the reference reads data[0]
+        for current_file, current_labels in groups:
+            if random_sample and not np.random.uniform(0, 1) >= (1 - random_sample):
+                continue
+            self.labels.append(np.stack(current_labels, axis=0))
+            self.filenames.append(os.path.join(self.images_dir, current_file))
+            self.image_ids.append(current_file.split('.')[0])
+        self.dataset_size = len(self.filenames)
+        self.dataset_indices = np.arange(self.dataset_size, dtype=np.int32)
+        if self.load_images_into_memory:
+            with ThreadPoolExecutor(_DECODE_THREADS) as pool:
+                self.images = list(pool.map(load_image, self.filenames))
+        if ret:
+            return self.images, self.filenames, self.labels, self.image_ids
+
     def get_dataset(self):
         return self.filenames, self.labels, self.image_ids, self.eval_neutral
 
@@ -121,8 +173,9 @@ class DataGenerator:
     def generate(self, batch_size=32, shuffle=True, transformations=[], label_encoder=None, returns={'processed_images', 'encoded_labels'},
                  keep_images_without_gt=False, degenerate_box_handling='remove'):
         """Yields batches indefinitely, as the reference's ``generate`` (same arguments and return order), from a device assembly
-        of each batch.  ``transformations``: planners of this package (``SSDDataAugmentation``, its parts, ``Resize``,
-        ``ResizeRandomInterp``, ``RandomFlip``, ``ConvertTo3Channels``); after them every image of a batch must have one size.
+        of each batch.  ``transformations``: planners of this package (the three training chains, ``SSDDataAugmentation`` and
+        their parts: ``Resize``, ``ResizeRandomInterp``, ``RandomFlip``, ``RandomTranslate``, ``RandomScale``, ``RandomRotate``,
+        ``RandomPatch``, ``ConvertTo3Channels``); after them every image of a batch must have one size.
         ``'processed_images'`` is a float32 CUDA tensor ``(B, H, W, 3)``; ``'encoded_labels'`` the float32 CUDA ``y_true``;
         ``'processed_labels'`` a list of float64 arrays read back from the device."""
         if self.dataset_size == 0:
