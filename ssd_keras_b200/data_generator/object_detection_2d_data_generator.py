@@ -1,7 +1,8 @@
 """``DataGenerator`` (the reference's object_detection_2d_data_generator.py): a dataset of images and labels, and ``generate()``,
 which yields training batches assembled on the device.
 
-``parse_csv`` reads a dataset from a CSV of boxes, as the reference's does (the XML and JSON parsers are not restated).
+``parse_csv`` (a CSV of boxes), ``parse_xml`` (Pascal VOC annotations) and ``parse_json`` (MS COCO annotations) read a dataset as
+the reference's do, with the same attributes and return values; ``save_dataset`` pickles the parsed lists for the constructor.
 
 Per batch, the host does what only the host can: the shuffle (``sklearn.utils.shuffle``'s permutation, drawn from the global
 ``np.random``), the batch slice, dropping images without boxes, and the random draws of the augmentation planners (the
@@ -16,12 +17,15 @@ degenerate-box filter (``Resize`` with one, as in ``SSDDataAugmentation`` and th
 box can be degenerate and nothing is checked; otherwise (the SSD7 chain's lists end in a flip, or in the clip of a translation
 or zoom) the processed boxes are read back once and the reference's ``'remove'`` / ``'warn'`` rules are applied to them.
 
-Not covered: HDF5 datasets, the XML and JSON parsers, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
+Not covered: HDF5 datasets, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
 transformations other than the planners of this package."""
 import csv
+import json
 import os
 import pickle
 import warnings
+import xml.etree.ElementTree as ET
+from collections import defaultdict
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -51,6 +55,14 @@ def _load_list(value, name):
             return pickle.load(f)
     raise ValueError('`%s` must be either a Python list/tuple or a string representing the path to a pickled file containing a '
                      'list/tuple. The value you passed is neither of the two.' % name)
+
+
+def _text(element):
+    """BeautifulSoup's ``.text``: the text of the element and all its descendants.  A tag that was not found (``None``) raises
+    ``AttributeError``, as the reference's ``.text`` on BeautifulSoup's ``None`` does."""
+    if element is None:
+        raise AttributeError("'NoneType' object has no attribute 'text'")
+    return ''.join(element.itertext())
 
 
 def shuffle_together(objects):
@@ -107,11 +119,7 @@ class DataGenerator:
             else:
                 raise ValueError('`filenames` must be either a Python list/tuple or a string representing a filepath (to a pickled '
                                  'or text file). The value you passed is neither of the two.')
-            self.dataset_size = len(self.filenames)
-            self.dataset_indices = np.arange(self.dataset_size, dtype=np.int32)
-            if load_images_into_memory:
-                with ThreadPoolExecutor(_DECODE_THREADS) as pool:
-                    self.images = list(pool.map(load_image, self.filenames))
+            self._index_dataset()
         self.labels = _load_list(labels, 'labels')
         self.image_ids = _load_list(image_ids, 'image_ids')
         self.eval_neutral = _load_list(eval_neutral, 'eval_neutral')
@@ -156,13 +164,147 @@ class DataGenerator:
             self.labels.append(np.stack(current_labels, axis=0))
             self.filenames.append(os.path.join(self.images_dir, current_file))
             self.image_ids.append(current_file.split('.')[0])
+        self._index_dataset()
+        if ret:
+            return self.images, self.filenames, self.labels, self.image_ids
+
+    def parse_xml(self, images_dirs, image_set_filenames, annotations_dirs=[],
+                  classes=['background', 'aeroplane', 'bicycle', 'bird', 'boat', 'bottle', 'bus', 'car', 'cat', 'chair', 'cow',
+                           'diningtable', 'dog', 'horse', 'motorbike', 'person', 'pottedplant', 'sheep', 'sofa', 'train', 'tvmonitor'],
+                  include_classes='all', exclude_truncated=False, exclude_difficult=False, ret=False, verbose=True):
+        """The reference's Pascal VOC parser.  Per image directory, the ids are the stripped lines of its image-set file (strings)
+        and the file names ``<id>.jpg``; without ``annotations_dirs``, ``labels`` and ``eval_neutral`` are ``None``.  Otherwise
+        each ``<id>.xml`` gives one box per ``object`` element in document order: ``[class_id, xmin, ymin, xmax, ymax]`` as Python
+        ints in ``labels_output_format`` order (class ids index ``classes``), and its ``difficult`` flag as a bool in
+        ``eval_neutral``.  ``include_classes`` is tested on the class id before ``exclude_truncated`` and ``exclude_difficult``.
+
+        The reference reads the files with BeautifulSoup; here ``xml.etree.ElementTree`` does its lookups: the first ``folder``
+        of the document, an object's direct ``name`` / ``pose`` / ``truncated`` / ``difficult`` / ``bndbox`` children (so the
+        ``<part>`` children of VOC person objects never match), the first ``xmin`` ... under ``bndbox``, and an element's text
+        as that of all its descendants.  A missing tag raises ``AttributeError``, an unknown class name or a non-integer
+        number ``ValueError``.  With ``ret``, returns ``(images, filenames, labels, image_ids, eval_neutral)``."""
+        self.images_dirs = images_dirs
+        self.annotations_dirs = annotations_dirs
+        self.image_set_filenames = image_set_filenames
+        self.classes = classes
+        self.include_classes = include_classes
+        self.filenames = []
+        self.image_ids = []
+        self.labels = []
+        self.eval_neutral = []
+        if not annotations_dirs:
+            self.labels = None
+            self.eval_neutral = None
+            annotations_dirs = [None] * len(images_dirs)
+        for images_dir, image_set_filename, annotations_dir in zip(images_dirs, image_set_filenames, annotations_dirs):
+            with open(image_set_filename) as f:
+                image_ids = [line.strip() for line in f]
+            self.image_ids += image_ids
+            for image_id in image_ids:
+                filename = image_id + '.jpg'
+                self.filenames.append(os.path.join(images_dir, filename))
+                if annotations_dir is None:
+                    continue
+                root = ET.parse(os.path.join(annotations_dir, image_id + '.xml')).getroot()
+                folder = _text(next(root.iter('folder'), None))
+                boxes, eval_neutr = [], []
+                for obj in root.iter('object'):
+                    class_name = _text(obj.find('name'))
+                    class_id = self.classes.index(class_name)
+                    if self.include_classes != 'all' and class_id not in self.include_classes:
+                        continue
+                    pose = _text(obj.find('pose'))
+                    truncated = int(_text(obj.find('truncated')))
+                    if exclude_truncated and truncated == 1:
+                        continue
+                    difficult = int(_text(obj.find('difficult')))
+                    if exclude_difficult and difficult == 1:
+                        continue
+                    bndbox = obj.find('bndbox')
+                    xmin, ymin, xmax, ymax = (int(_text(bndbox.find('.//' + k))) for k in ('xmin', 'ymin', 'xmax', 'ymax'))
+                    item = {'folder': folder, 'image_name': filename, 'image_id': image_id, 'class_name': class_name,
+                            'class_id': class_id, 'pose': pose, 'truncated': truncated, 'difficult': difficult,
+                            'xmin': xmin, 'ymin': ymin, 'xmax': xmax, 'ymax': ymax}
+                    boxes.append([item[k] for k in self.labels_output_format])
+                    eval_neutr.append(bool(difficult))
+                self.labels.append(boxes)
+                self.eval_neutral.append(eval_neutr)
+        self._index_dataset()
+        if ret:
+            return self.images, self.filenames, self.labels, self.image_ids, self.eval_neutral
+
+    def parse_json(self, images_dirs, annotations_filenames, ground_truth_available=False, include_classes='all', ret=False,
+                   verbose=True):
+        """The reference's MS COCO parser.  The class maps come from the first annotations file's ``categories``, in its order:
+        ``cats_to_names`` (COCO id -> name), ``classes_to_names`` (``'background'`` then the names), ``cats_to_classes`` (COCO id
+        -> consecutive id from 1) and ``classes_to_cats``.  Per file, its ``images`` give the file names and the image ids
+        (the JSON ints).  With ``ground_truth_available``, each image's ``annotations`` whose original category id is in
+        ``include_classes`` give the boxes ``[class_id, x, y, x + w, y + h]`` in ``labels_output_format`` order, the JSON's
+        numbers as they are; otherwise ``labels`` is ``None``.  ``eval_neutral`` is left as it is.  With ``ret``, returns
+        ``(images, filenames, labels, image_ids)``."""
+        self.images_dirs = images_dirs
+        self.annotations_filenames = annotations_filenames
+        self.include_classes = include_classes
+        self.filenames = []
+        self.image_ids = []
+        self.labels = [] if ground_truth_available else None
+        with open(annotations_filenames[0]) as f:
+            categories = json.load(f)['categories']
+        self.cats_to_names = {}
+        self.classes_to_names = ['background']
+        self.cats_to_classes = {}
+        self.classes_to_cats = {}
+        for i, cat in enumerate(categories):
+            self.cats_to_names[cat['id']] = cat['name']
+            self.classes_to_names.append(cat['name'])
+            self.cats_to_classes[cat['id']] = i + 1
+            self.classes_to_cats[i + 1] = cat['id']
+        for images_dir, annotations_filename in zip(self.images_dirs, self.annotations_filenames):
+            with open(annotations_filename) as f:
+                annotations = json.load(f)
+            if ground_truth_available:
+                image_ids_to_annotations = defaultdict(list)
+                for annotation in annotations['annotations']:
+                    image_ids_to_annotations[annotation['image_id']].append(annotation)
+            for img in annotations['images']:
+                self.filenames.append(os.path.join(images_dir, img['file_name']))
+                self.image_ids.append(img['id'])
+                if not ground_truth_available:
+                    continue
+                boxes = []
+                for annotation in image_ids_to_annotations[img['id']]:
+                    cat_id = annotation['category_id']
+                    if self.include_classes != 'all' and cat_id not in self.include_classes:
+                        continue
+                    class_id = self.cats_to_classes[cat_id]
+                    xmin, ymin, width, height = (annotation['bbox'][k] for k in range(4))
+                    item = {'image_name': img['file_name'], 'image_id': img['id'], 'class_id': class_id,
+                            'xmin': xmin, 'ymin': ymin, 'xmax': xmin + width, 'ymax': ymin + height}
+                    boxes.append([item[k] for k in self.labels_output_format])
+                self.labels.append(boxes)
+        self._index_dataset()
+        if ret:
+            return self.images, self.filenames, self.labels, self.image_ids
+
+    def _index_dataset(self):
+        """What every way of loading a dataset ends with: its size and indices, and its images decoded into memory when
+        ``load_images_into_memory`` is set."""
         self.dataset_size = len(self.filenames)
         self.dataset_indices = np.arange(self.dataset_size, dtype=np.int32)
         if self.load_images_into_memory:
             with ThreadPoolExecutor(_DECODE_THREADS) as pool:
                 self.images = list(pool.map(load_image, self.filenames))
-        if ret:
-            return self.images, self.filenames, self.labels, self.image_ids
+
+    def save_dataset(self, filenames_path='filenames.pkl', labels_path=None, image_ids_path=None, eval_neutral_path=None):
+        """Pickles ``filenames`` and, for each path given, ``labels``, ``image_ids`` and ``eval_neutral``, so that a slow parse
+        is done once: the constructor reads the files back (``filenames_type='pickle'``, ``labels=``, ``image_ids=``,
+        ``eval_neutral=``)."""
+        with open(filenames_path, 'wb') as f:
+            pickle.dump(self.filenames, f)
+        for path, value in ((labels_path, self.labels), (image_ids_path, self.image_ids), (eval_neutral_path, self.eval_neutral)):
+            if path is not None:
+                with open(path, 'wb') as f:
+                    pickle.dump(value, f)
 
     def get_dataset(self):
         return self.filenames, self.labels, self.image_ids, self.eval_neutral
