@@ -277,6 +277,30 @@ def n_steps_wgrad(plan, products):
     return per_unit * per + ks
 
 
+def direct_wgrad_rows(B, Ho, sm_count):
+    """train.cu, the launch of wgrad_direct_kernel / wgrad_direct3x3_kernel -> (rows_per_block, grid, rows of the last block):
+    each block owns ceil(B Ho / (8 SMs)) consecutive output rows (image-major)."""
+    rows = B * Ho
+    rpb = max(1, -(-rows // (8 * sm_count)))
+    grid = -(-rows // rpb)
+    return rpb, grid, rows - (grid - 1) * rpb
+
+
+def n_steps_wgrad_direct(B, Ho, Wo, cout, fast, sm_count):
+    """Roundings behind one element of the direct weight gradient, in the kernels' summation order (section 4): a thread adds
+    its products over the block's rows in fp32 (wgrad_direct3x3_kernel: every 256 / (cout / 2)-th pixel of a row, the pixel
+    lanes then meet in shared-memory atomics; wgrad_direct_kernel: every pixel, one add into shared memory), and each block adds
+    its sum into the flat gradient with one fp32 atomic.  A sum whose partial sums are formed this way loses at most
+    (longest chain of roundings) * 2**-24 * sum |term|, so this count replaces the B Ho Wo + 1 of one flat sum."""
+    rpb, grid, _ = direct_wgrad_rows(B, Ho, sm_count)
+    if fast:
+        lanes = 256 // (cout // 2)
+        per_thread = rpb * -(-Wo // lanes)
+    else:
+        lanes, per_thread = 1, rpb * Wo
+    return per_thread + lanes + grid + 1
+
+
 def _dconv_tap(dz, w, t, in_hw, stride, dil, pads, c0=0, c1=None):
     """Contribution of tap t (dZ channels [c0, c1)) to the data gradient: dz (B,Ho,Wo,Cout) x w[kh,kw,:,c0:c1]^T scattered
     onto the (B,H,W,Cin) input grid."""
@@ -287,7 +311,7 @@ def _dconv_tap(dz, w, t, in_hw, stride, dil, pads, c0=0, c1=None):
     B, Ho, Wo, _ = dz.shape
     H, W = in_hw
     out = np.zeros((B, H + 2 * (pt + dil * KH + stride), W + 2 * (pl + dil * KW + stride), cin))
-    v = np.einsum('bhwo,co->bhwc', np.asarray(dz[..., c0:c1], np.float64), np.asarray(w[kh, kw, :, c0:c1], np.float64))
+    v = np.asarray(dz[..., c0:c1], np.float64) @ np.asarray(w[kh, kw, :, c0:c1], np.float64).T
     y0, x0 = kh * dil, kw * dil                                    # padded-input position of output (0, 0) under this tap
     out[:, y0:y0 + stride * (Ho - 1) + 1:stride, x0:x0 + stride * (Wo - 1) + 1:stride] += v
     return out[:, pt:pt + H, pl:pl + W]
@@ -363,7 +387,7 @@ def _wgrad_tap(x, dz, t, KH, KW, stride, dil, pads, pix=None):
     xp = np.pad(np.asarray(x, np.float64), ((0, 0), (pt, pb + stride + dil * KH), (pl, pr + stride + dil * KW), (0, 0)))
     win = xp[:, kh * dil:kh * dil + stride * (Ho - 1) + 1:stride, kw * dil:kw * dil + stride * (Wo - 1) + 1:stride]
     d = np.asarray(dz, np.float64) if pix is None else np.asarray(dz, np.float64) * pix[..., None]
-    return np.einsum('bhwc,bhwo->oc', win, d)
+    return np.tensordot(d, win, axes=([0, 1, 2], [0, 1, 2]))         # one BLAS product: full-size layers stay cheap
 
 
 def wgrad_ref(x, dz, KH, KW, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', perturb=()):
@@ -386,14 +410,12 @@ def wgrad_ref(x, dz, KH, KW, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', 
     taps = KH * KW
     geo = dict(KH=KH, KW=KW, stride=stride, dil=dil, pads=pads)
 
-    def full(pix=None, c=None, skip_tap=None, which=None):
+    def full(pix=None, skip_tap=None, which=None):
         out = np.zeros((dz[0].shape[-1], taps, xs[0].shape[-1]))
         for a, d in (terms if which is None else which):
             for t in range(taps):
                 if t != skip_tap:
                     out[:, t] += _wgrad_tap(a, d, t, pix=pix, **geo)
-        if c is not None:
-            out[:, :, c] = 0.0
         return out
     ref = full()
     A = full(which=[(np.abs(a), np.abs(d)) for a, d in terms])
@@ -404,7 +426,8 @@ def wgrad_ref(x, dz, KH, KW, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', 
         elif p[0] == 'tap':
             out[p] = full(skip_tap=p[1])
         elif p[0] == 'kblock':
-            out[p] = full(c=slice(64 * p[1], 64 * p[1] + 64))
+            out[p] = ref.copy()
+            out[p][:, :, 64 * p[1]:64 * p[1] + 64] = 0.0
         elif p[0] == 'pixels':
             pix = np.ones(dz[0].shape[:3])
             pix[p[1], p[2]:p[2] + p[4], p[3]:p[3] + p[5]] = 0

@@ -305,6 +305,33 @@ def test_repacked_planes_hold_the_updated_master(prec):
 # ------------------------------------------------------------------------------------------------------------------------------
 # training-phase forward launches
 # ------------------------------------------------------------------------------------------------------------------------------
+def bn_pass_ratios(name, p, g, info, bn_layers, before, z_prev, store):
+    """Judges the BatchNormalization layers after forward pass p: the stored output against bn_fwd_ref of the z the pass
+    normalised, the moving statistics against their recurrence from `before` ({layer: (mean, var)} read before the pass).
+    z_prev ({layer: z of the previous pass}) is updated.  -> (max ratio, {perturbation: max ratio})."""
+    ratio, pr = 0.0, {}
+    for i in bn_layers:
+        inf = info[i]
+        z = g.read_bn_input(i)
+        planes = g.planes(i)
+        a = tb._fval(planes, inf)
+        mm, mv = g.bn_stats(i, inf['C'])
+        perts = [('biased',), ('no_eps',)] + ([('acc',)] if i in z_prev else [])
+        ref, A, kap, st, sb, pv = opexact.bn_fwd_ref(z, inf['bn_gamma'], inf['bn_beta'], before[i][0], before[i][1], act=inf['act'],
+                                                     z_prev=z_prev.get(i), perturb=perts)
+        bnd = kap * A + opexact.UNIT[store] * np.abs(ref)
+        got_st = {'mean': mm, 'var': mv}
+        r = max(opexact.err_ratio(a, ref, bnd), opexact.state_ratio(got_st, st, sb))
+        assert r <= 1.0, (name, p, i, r)
+        ratio = max(ratio, r)
+        for k, (ap, sp) in pv.items():
+            pr[k] = max(pr.get(k, 0.0), opexact.err_ratio(a, ap, bnd), opexact.state_ratio(got_st, sp, sb))
+        for o in cc.outside(planes, inf['H'], inf['W'], inf['C']):
+            assert not np.any(o), (name, p, i, 'border / padding channels not zero')
+        z_prev[i] = z
+    return ratio, pr
+
+
 @pytest.mark.parametrize('case', BN_CASES, ids=[c['name'] for c in BN_CASES])
 def test_batchnorm_forward_and_moving_statistics_over_three_passes(case):
     bc = tb.bcase(case['name'], case['B'], case['H'], case['W'], 16, case['layers'], {}, prec=case['prec'])
@@ -321,26 +348,7 @@ def test_batchnorm_forward_and_moving_statistics_over_three_passes(case):
             x = (rng.standard_normal((case['B'], case['H'], case['W'], 16)) * (0.1, 0.06, 0.15)[p] + 0.05 * p).astype(np.float32)
             before = {i: g.bn_stats(i, info[i]['C']) for i in bn_layers}
             g.forward(x)
-            ratio, pr = 0.0, {}
-            for i in bn_layers:
-                inf = info[i]
-                z = g.read_bn_input(i)
-                planes = g.planes(i)
-                a = tb._fval(planes, inf)
-                mm, mv = g.bn_stats(i, inf['C'])
-                perts = [('biased',), ('no_eps',)] + ([('acc',)] if i in z_prev else [])
-                ref, A, kap, st, sb, pv = opexact.bn_fwd_ref(z, inf['bn_gamma'], inf['bn_beta'], before[i][0], before[i][1], act=inf['act'],
-                                                             z_prev=z_prev.get(i), perturb=perts)
-                bnd = kap * A + opexact.UNIT[store] * np.abs(ref)
-                got_st = {'mean': mm, 'var': mv}
-                r = max(opexact.err_ratio(a, ref, bnd), opexact.state_ratio(got_st, st, sb))
-                assert r <= 1.0, (case['name'], p, i, r)
-                ratio = max(ratio, r)
-                for k, (ap, sp) in pv.items():
-                    pr[k] = max(pr.get(k, 0.0), opexact.err_ratio(a, ap, bnd), opexact.state_ratio(got_st, sp, sb))
-                for o in cc.outside(planes, inf['H'], inf['W'], inf['C']):
-                    assert not np.any(o), (case['name'], p, i, 'border / padding channels not zero')
-                z_prev[i] = z
+            ratio, pr = bn_pass_ratios(case['name'], p, g, info, bn_layers, before, z_prev, store)
             _judge(dict(test='bn_forward', case=case['name'], pass_=p), ratio, pr)
     finally:
         g.close()
