@@ -176,7 +176,9 @@ typedef enum { SSDK_BOXOP_END = 0, SSDK_BOXOP_CROP_PAD = 1, SSDK_BOXOP_FLIP_H = 
                SSDK_BOXOP_SATURATION = 20, SSDK_BOXOP_HUE = 21, SSDK_BOXOP_RGB2HSV = 22, SSDK_BOXOP_HSV2RGB = 23,
                SSDK_BOXOP_CHANNEL_SWAP = 24,
                /* 25: RESIZE with every interpolation mode of ResizeRandomInterp; boxes as RESIZE */
-               SSDK_BOXOP_RESIZE_INTERP = SSDK_BOXOP_CHANNEL_SWAP + 1 } ssdk_box_op_kind;
+               SSDK_BOXOP_RESIZE_INTERP = SSDK_BOXOP_CHANNEL_SWAP + 1,
+               /* 26: a photometric op outside the 16-24 range: HistogramEqualization of channel 2; images only */
+               SSDK_BOXOP_EQUALIZE_V = SSDK_BOXOP_RESIZE_INTERP + 1 } ssdk_box_op_kind;
 typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
@@ -213,8 +215,12 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
  *                            32-pixel vector loop and rounds in the scalar loop that finishes each row: columns >= w / 32 * 32
  *                            round, the others truncate
  *   CHANNEL_SWAP a0..a2=order  image[:, :, order]
- * Gamma, histogram equalisation and conversions to GRAY are not covered; the random draws stay with the caller (an op that a
- * draw skipped is absent from the list).
+ *   EQUALIZE_V               HistogramEqualization (:397-411): image[:, :, 2] = cv2.equalizeHist(image[:, :, 2]) on the uint8
+ *                            state, OpenCV 4.13's LUT bit for bit.  The image's histogram is taken where the op stands: the
+ *                            stages before it run in one photometric_kernel pass, equalize_hist_kernel and equalize_lut_kernel
+ *                            build the image's table, and the next pass starts by applying it
+ * Gamma and conversions to GRAY are not covered; the random draws stay with the caller (an op that a draw skipped is absent
+ * from the list).
  * src_dev: the B uint8 images packed back to back, image b at bytes src_offsets_host[b] .. src_offsets_host[b+1] (host, [B+1]),
  * of shape src_hwc_host[3b..3b+2] = h, w, c with c in {1, 3, 4}.  ops_host: [B*max_ops] on the HOST (a list ends at
  * SSDK_BOXOP_END or after max_ops entries).  out_dev: [B*out_h*out_w*3] float32.
@@ -226,8 +232,9 @@ int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, con
  * a RESIZE (after a SCALE they are applied to its output); the final size out_h x out_w; a supported interpolation code; and one
  * background colour per list: every pad or translate that brings in background, every SCALE, and a ROTATE whose map leaves
  * the source (black) must agree (bands of different colours are not represented).  Photometric ops: all of them before the
- * first op that changes the image geometry; at most 16; BRIGHTNESS / CONTRAST / SATURATION / HUE only between a TO_FLOAT32 and
- * the next TO_UINT8, the colour conversions and the end of the prefix only in the uint8 state; factors > 0, -180 <= hue delta
+ * first op that changes the image geometry; at most 16, of which at most 4 EQUALIZE_V; BRIGHTNESS / CONTRAST / SATURATION / HUE
+ * only between a TO_FLOAT32 and the next TO_UINT8, the colour conversions, EQUALIZE_V (cv2.equalizeHist takes 8-bit images
+ * only) and the end of the prefix only in the uint8 state; factors > 0, -180 <= hue delta
  * <= 180 (the reference's own ValueErrors), brightness delta finite, the swap order a permutation of (0, 1, 2).
  * Images with photometric ops are written, converted to 3 channels, to a scratch buffer owned by the context (grown when needed,
  * freed with the context) and assembled from there; the others are read from src_dev as before, and a call without photometric

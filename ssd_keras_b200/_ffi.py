@@ -56,6 +56,8 @@ BOXOP_TRANSLATE, BOXOP_SCALE, BOXOP_ROTATE, BOXOP_OVERLAP, BOXOP_CLIP = range(6,
 (BOXOP_TO_FLOAT32, BOXOP_TO_UINT8, BOXOP_BRIGHTNESS, BOXOP_CONTRAST, BOXOP_SATURATION, BOXOP_HUE, BOXOP_RGB2HSV, BOXOP_HSV2RGB,
  BOXOP_CHANNEL_SWAP) = range(16, 25)         # photometric ops: images only (ssdk_assemble_images)
 BOXOP_RESIZE_INTERP = 25                    # RESIZE with all five cv2 modes (the boxes as RESIZE)
+BOXOP_EQUALIZE_V = 26                       # photometric: cv2.equalizeHist of channel 2 (images only)
+PHOTO_OPS = frozenset(range(BOXOP_TO_FLOAT32, BOXOP_CHANNEL_SWAP + 1)) | {BOXOP_EQUALIZE_V}
 INTER_NEAREST, INTER_LINEAR, INTER_CUBIC, INTER_AREA, INTER_LANCZOS4 = range(5)   # cv2's codes, in flag bits 8-15
 
 

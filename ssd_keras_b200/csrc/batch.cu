@@ -23,6 +23,11 @@
 //   photometric_kernel     the photometric prefix of the op lists (ConvertDataType, Brightness, Contrast, Saturation, Hue,
 //                          ConvertColor RGB <-> HSV, ChannelSwap; object_detection_2d_photometric_ops.py), one launch in front of
 //                          image_assemble_kernel: uint8 in, uint8 h x w x 3 out, restated in oracle/photoops.py.
+//   equalize_hist_kernel   HistogramEqualization (EQUALIZE_V, cv2.equalizeHist of channel 2) cuts an image's prefix into
+//   equalize_lut_kernel    passes of photometric_kernel: after a pass, the first adds each image's channel-2 histogram into
+//                          a 256-bin one per image (a shared-memory histogram per CTA, one atomic per bin), the second (one
+//                          CTA per image) scans it into cv2's table, and the next pass starts by applying that table.
+//                          Restated in tests/equalize_reference.py.
 // The file is compiled with --fmad=false; the float64 resize coordinates also spell their roundings out (__dmul_rn / __dadd_rn).
 #include "common.cuh"
 #include "rn.cuh"
@@ -558,14 +563,19 @@ __global__ void __launch_bounds__(kImgThreads) image_assemble_kernel_wide(const 
 constexpr int kPhotoThreads = 256;
 constexpr int kPhotoMaxStages = 16;
 constexpr int kPhotoGroupsPerThread = 4;       // groups of 4 pixels a thread takes, when the grid is sized for the largest image
+constexpr int kPhotoMaxEqualize = 4;           // EQUALIZE_V stages per list: each one is another pass
 
 struct PhotoStage { int op; float a; };        // CHANNEL_SWAP keeps its order in op bits 8-13
 struct PhotoDesc {
   long long src_off;                           // the image in the packed source buffer
   long long dst_off;                           // its 3-channel result in the scratch buffer, 16-byte aligned
   int n_px, w, c, n_stages;
+  int lut, pad_;                               // the equalisation table an EQUALIZE_V stage applies (-1: none)
   PhotoStage st[kPhotoMaxStages];
 };
+
+// One equalisation: the pass output it is taken from (3-channel, 16-byte aligned, in the scratch buffer) and its table slot.
+struct EqDesc { long long off; int n_px, slot; };
 
 // The aligned 32-bit word at q, of which only the bytes inside the image [lo, hi) may be read (the packed images start and end
 // at arbitrary byte offsets); bytes outside read as 0.
@@ -619,10 +629,11 @@ __device__ __forceinline__ void hsv2rgb_px(float p[3], bool round) {
 
 // One CTA column per image with photometric ops (blockIdx.y); a thread takes groups of 4 pixels: 4 * c source bytes from aligned
 // words (any source alignment), 12 result bytes as three aligned words.  A pixel is carried as three float32 values, which hold
-// the uint8 state exactly; the stage list is uniform across the CTA.
+// the uint8 state exactly; the stage list is uniform across the CTA.  luts: the equalisation tables (passes after the first).
 __global__ void __launch_bounds__(kPhotoThreads) photometric_kernel(const uint8_t* __restrict__ src, const PhotoDesc* __restrict__ descs,
-                                                                    uint8_t* __restrict__ dst) {
+                                                                    const uint8_t* __restrict__ luts, uint8_t* __restrict__ dst) {
   __shared__ int s_sdiv[256], s_hdiv[256];
+  __shared__ uint8_t s_lut[256];
   __shared__ PhotoDesc s_d;
   if (threadIdx.x < sizeof(PhotoDesc) / 4)
     reinterpret_cast<int*>(&s_d)[threadIdx.x] = reinterpret_cast<const int*>(descs + blockIdx.y)[threadIdx.x];
@@ -630,6 +641,8 @@ __global__ void __launch_bounds__(kPhotoThreads) photometric_kernel(const uint8_
     const int i = threadIdx.x;                                    // rint(N / i) = (2N + i) / (2i): neither quotient has a tie
     s_sdiv[i] = i ? (2 * (255 << 12) + i) / (2 * i) : 0;
     s_hdiv[i] = i ? (2 * ((180 << 12) / 6) + i) / (2 * i) : 0;
+    const int lut = descs[blockIdx.y].lut;
+    if (lut >= 0) s_lut[i] = luts[(size_t)lut * 256 + i];
   }
   __syncthreads();
   const int n_px = s_d.n_px, w = s_d.w, c = s_d.c, n_stages = s_d.n_stages;
@@ -717,6 +730,10 @@ __global__ void __launch_bounds__(kPhotoThreads) photometric_kernel(const uint8_
           }
           break;
         }
+        case SSDK_BOXOP_EQUALIZE_V:                               // LUT_V: the first stage of a pass, channel 2 through the table
+#pragma unroll                                                    // equalize_lut_kernel built from the previous pass's output
+          for (int j = 0; j < 4; ++j) p[j][2] = (float)s_lut[(int)p[j][2]];
+          break;
         default: break;                                           // TO_FLOAT32: the values are float32 already
       }
     }
@@ -736,12 +753,76 @@ __global__ void __launch_bounds__(kPhotoThreads) photometric_kernel(const uint8_
   }
 }
 
-bool is_photo(int code) { return code >= SSDK_BOXOP_TO_FLOAT32 && code <= SSDK_BOXOP_CHANNEL_SWAP; }
+// ---- histogram equalisation between passes ----
+constexpr int kEqThreads = 256;                // one thread per bin in the histogram and the table
+
+// Channel 2 of each image's pass output into its 256-bin histogram (hist[slot], zeroed by the caller): a CTA counts in shared
+// memory and adds its non-zero bins once.  A thread takes groups of 4 pixels, 12 bytes as three aligned words.
+__global__ void __launch_bounds__(kEqThreads) equalize_hist_kernel(const uint8_t* __restrict__ img, const EqDesc* __restrict__ descs,
+                                                                   int* __restrict__ hist) {
+  __shared__ int s_h[256];
+  s_h[threadIdx.x] = 0;
+  const EqDesc d = descs[blockIdx.y];
+  __syncthreads();
+  const uint8_t* p = img + d.off;
+  const int groups = (d.n_px + 3) >> 2;
+  for (int grp = blockIdx.x * kEqThreads + threadIdx.x; grp < groups; grp += gridDim.x * kEqThreads) {
+    if (grp * 4 + 4 <= d.n_px) {                                  // bytes 2, 5, 8 and 11 of the group
+      const uint32_t* q = reinterpret_cast<const uint32_t*>(p + (size_t)grp * 12);
+      const uint32_t w0 = q[0], w1 = q[1], w2 = q[2];
+      atomicAdd(&s_h[(w0 >> 16) & 255u], 1); atomicAdd(&s_h[(w1 >> 8) & 255u], 1);
+      atomicAdd(&s_h[w2 & 255u], 1); atomicAdd(&s_h[w2 >> 24], 1);
+    } else {                                                      // the last, partial group
+      for (int j = grp * 4; j < d.n_px; ++j) atomicAdd(&s_h[p[(size_t)j * 3 + 2]], 1);
+    }
+  }
+  __syncthreads();
+  const int v = s_h[threadIdx.x];
+  if (v) atomicAdd(&hist[(size_t)d.slot * 256 + threadIdx.x], v);
+}
+
+// One CTA per equalisation: cv2.equalizeHist's table from the histogram (OpenCV 4.13, histogram.cpp).  i0 is the first
+// non-empty bin; if it holds every pixel the channel becomes i0, otherwise scale = 255.f / (total - hist[i0]) in float32,
+// lut[i0] = 0 and lut[i] = saturate_cast<uchar>((float)sum_i * scale) with sum_i = hist[i0 + 1] + ... + hist[i]: the int sum
+// rounded to float32, the product rounded, then rounded half to even.
+__global__ void __launch_bounds__(kEqThreads) equalize_lut_kernel(const EqDesc* __restrict__ descs, const int* __restrict__ hist,
+                                                                  uint8_t* __restrict__ luts) {
+  __shared__ int s_c[256];
+  __shared__ int s_i0;
+  const EqDesc d = descs[blockIdx.x];
+  const int t = threadIdx.x;
+  const int h = hist[(size_t)d.slot * 256 + t];
+  s_c[t] = h;
+  if (t == 0) s_i0 = 256;
+  __syncthreads();
+  if (h) atomicMin(&s_i0, t);
+  for (int off = 1; off < 256; off <<= 1) {                       // inclusive scan
+    const int v = t >= off ? s_c[t - off] : 0;
+    __syncthreads();
+    s_c[t] += v;
+    __syncthreads();
+  }
+  const int i0 = s_i0, h0 = s_c[i0];                              // nothing before i0, so its prefix sum is hist[i0]
+  int v;
+  if (h0 == d.n_px) {
+    v = i0;
+  } else if (t <= i0) {
+    v = 0;                                                        // below i0 no pixel reads the table
+  } else {
+    const float scale = __fdiv_rn(255.f, __int2float_rn(d.n_px - h0));
+    v = min(max(__float2int_rn(__fmul_rn(__int2float_rn(s_c[t] - h0), scale)), 0), 255);
+  }
+  luts[(size_t)d.slot * 256 + t] = (uint8_t)v;
+}
+
+bool is_photo(int code) {
+  return (code >= SSDK_BOXOP_TO_FLOAT32 && code <= SSDK_BOXOP_CHANNEL_SWAP) || code == SSDK_BOXOP_EQUALIZE_V;
+}
 
 // The photometric prefix of image b's op list -> its stages; every check the entry point documents.
 int compose_photo(int b, const ssdk_box_op* ops, int max_ops, PhotoDesc* out) {
   bool geometric = false, is_float = false;
-  int n = 0;
+  int n = 0, n_eq = 0;
   for (int i = 0; i < max_ops; ++i) {
     const ssdk_box_op& op = ops[(size_t)b * max_ops + i];
     if (op.op == SSDK_BOXOP_END) break;
@@ -759,6 +840,11 @@ int compose_photo(int b, const ssdk_box_op* ops, int max_ops, PhotoDesc* out) {
       case SSDK_BOXOP_TO_UINT8: is_float = false; break;
       case SSDK_BOXOP_RGB2HSV: case SSDK_BOXOP_HSV2RGB:
         SSDK_REQUIRE(!is_float, "ssdk_assemble_images: image %d, op %d: a colour conversion needs a uint8 image (TO_UINT8 first)", b, i);
+        break;
+      case SSDK_BOXOP_EQUALIZE_V:
+        SSDK_REQUIRE(!is_float, "ssdk_assemble_images: image %d, op %d: EQUALIZE_V needs a uint8 image (cv2.equalizeHist takes 8-bit "
+                     "images only; TO_UINT8 first)", b, i);
+        SSDK_REQUIRE(++n_eq <= kPhotoMaxEqualize, "ssdk_assemble_images: image %d: more than %d EQUALIZE_V ops", b, kPhotoMaxEqualize);
         break;
       case SSDK_BOXOP_CHANNEL_SWAP: {
         const double o[3] = {op.a0, op.a1, op.a2};
@@ -1022,10 +1108,11 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
   SSDK_REQUIRE(out_h > 0 && out_w > 0, "ssdk_assemble_images: output size %dx%d must be positive", out_h, out_w);
   SSDK_REQUIRE(max_ops >= 0 && (max_ops == 0 || ops_host), "ssdk_assemble_images: ops_host is NULL");
   std::vector<ImgDesc> descs(B);
-  std::vector<PhotoDesc> photo;                                   // the images with photometric ops
-  std::vector<int> photo_image;
+  std::vector<PhotoDesc> photo;                                   // the images with photometric ops: their whole stage lists
+  std::vector<int> photo_image, photo_eq;                         // ... their batch index and EQUALIZE_V count
+  std::vector<long long> photo_alt;                               // ... a second result buffer when they equalise
   long long photo_bytes = 0;
-  int photo_groups = 0;
+  int photo_groups = 0, max_eq = 0;
   for (int b = 0; b < B; ++b) {
     PhotoDesc p{};
     int rc = compose_photo(b, ops_host, max_ops, &p);
@@ -1035,39 +1122,96 @@ extern "C" int ssdk_assemble_images(ssdk_ctx* ctx, const uint8_t* src_dev, const
     if (!p.n_stages) continue;
     const long long n_px = (long long)descs[b].h * descs[b].w;
     SSDK_REQUIRE(n_px < (1LL << 31) - 4, "ssdk_assemble_images: image %d is too large for the photometric ops", b);
+    const long long region = (n_px * 3 + 15) / 16 * 16;
+    const int n_eq = (int)std::count_if(p.st, p.st + p.n_stages, [](const PhotoStage& s) { return s.op == SSDK_BOXOP_EQUALIZE_V; });
     p.src_off = descs[b].src_off; p.dst_off = photo_bytes;
-    p.n_px = (int)n_px; p.w = descs[b].w; p.c = descs[b].c;
-    photo_bytes += (n_px * 3 + 15) / 16 * 16;
+    p.n_px = (int)n_px; p.w = descs[b].w; p.c = descs[b].c; p.lut = -1;
+    photo_bytes += region;
+    photo_alt.push_back(n_eq ? photo_bytes : -1);                 // equalising images alternate between two buffers
+    if (n_eq) photo_bytes += region;
     photo_groups = std::max(photo_groups, (int)((n_px + 3) / 4));
-    photo.push_back(p); photo_image.push_back(b);
+    photo.push_back(p); photo_image.push_back(b); photo_eq.push_back(n_eq);
+    max_eq = std::max(max_eq, n_eq);
+  }
+  // Pass k of photometric_kernel runs the stages between an image's k-th and (k+1)-th EQUALIZE_V (pass 0 from the source, the
+  // others from the previous pass's output, starting with the table of the equalisation between them); pass k reads buffer
+  // (k - 1) % 2 and writes buffer k % 2.  Equalisation k of every image that has one is taken from pass k - 1's output.
+  std::vector<PhotoDesc> passes;                                  // pass 0's descriptors, then pass 1's, ...
+  std::vector<EqDesc> eqs;                                        // equalisation 1's, then 2's, ...
+  std::vector<int> pass_n(max_eq + 1, 0), pass_groups(max_eq + 1, 0);
+  for (int k = 0; k <= max_eq; ++k) {
+    for (size_t i = 0; i < photo.size(); ++i) {
+      if (photo_eq[i] < k) continue;
+      const PhotoDesc& full = photo[i];
+      const long long buf[2] = {full.dst_off, photo_alt[i]};
+      PhotoDesc p = full;
+      p.n_stages = 0;
+      int seen = 0;
+      for (int s = 0; s < full.n_stages; ++s) {                   // pass k > 0 starts with its EQUALIZE_V: the table
+        seen += full.st[s].op == SSDK_BOXOP_EQUALIZE_V;
+        if (seen == k) p.st[p.n_stages++] = full.st[s];
+      }
+      if (k > 0) {
+        eqs.push_back(EqDesc{buf[(k - 1) % 2], full.n_px, (int)eqs.size()});
+        p.lut = eqs.back().slot;
+        p.src_off = buf[(k - 1) % 2];                             // relative to the scratch buffer until it is placed
+        p.c = 3;
+      }
+      p.dst_off = buf[k % 2];
+      passes.push_back(p);
+      ++pass_n[k];
+      pass_groups[k] = std::max(pass_groups[k], (p.n_px + 3) / 4);
+    }
   }
   cudaStream_t stream = (cudaStream_t)stream_;
   const size_t img_bytes = sizeof(ImgDesc) * (size_t)B;
-  const size_t bytes = img_bytes + sizeof(PhotoDesc) * photo.size();
+  const size_t pass_bytes = sizeof(PhotoDesc) * passes.size();
+  const size_t bytes = img_bytes + pass_bytes + sizeof(EqDesc) * eqs.size();
   int rc = ctx->img_desc_ws.ensure(bytes);
   if (rc) return rc;
+  const long long hist_off = photo_bytes, lut_off = hist_off + (long long)eqs.size() * 256 * (long long)sizeof(int);
   if (!photo.empty()) {
-    rc = ctx->photo_ws.ensure((size_t)photo_bytes);
+    rc = ctx->photo_ws.ensure((size_t)(lut_off + (long long)eqs.size() * 256));
     if (rc) return rc;
-    // image_assemble_kernel addresses every image as src_dev + src_off: the images in the scratch buffer get their distance
-    // from src_dev (both are device addresses of one flat address space)
+    // image_assemble_kernel and the passes after the first address every image as src_dev + src_off: the images in the
+    // scratch buffer get their distance from src_dev (both are device addresses of one flat address space)
+    const long long rel = (long long)reinterpret_cast<uintptr_t>(ctx->photo_ws.ptr) - (long long)reinterpret_cast<uintptr_t>(src_dev);
     for (size_t k = 0; k < photo.size(); ++k) {
       ImgDesc& d = descs[photo_image[k]];
-      d.src_off = (long long)(reinterpret_cast<uintptr_t>(ctx->photo_ws.ptr) + (uintptr_t)photo[k].dst_off) - (long long)reinterpret_cast<uintptr_t>(src_dev);
+      d.src_off = rel + (photo_eq[k] % 2 ? photo_alt[k] : photo[k].dst_off);
       d.c = 3;
     }
+    for (size_t k = photo.size(); k < passes.size(); ++k) passes[k].src_off += rel;
   }
   // descriptors: pinned staging -> workspace, asynchronous; the host waits only if the upload from the same staging buffer,
   // four calls ago, is still queued
-  rc = ctx->img_desc_ring.upload(ctx->img_desc_ws.ptr, stream, {{descs.data(), img_bytes}, {photo.data(), bytes - img_bytes}});
+  rc = ctx->img_desc_ring.upload(ctx->img_desc_ws.ptr, stream, {{descs.data(), img_bytes}, {passes.data(), pass_bytes},
+                                                                {eqs.data(), bytes - img_bytes - pass_bytes}});
   if (rc) return rc;
   const ImgDesc* d_dev = reinterpret_cast<const ImgDesc*>(ctx->img_desc_ws.ptr);
   if (!photo.empty()) {
+    uint8_t* ws = static_cast<uint8_t*>(ctx->photo_ws.ptr);
+    const PhotoDesc* pass_dev = reinterpret_cast<const PhotoDesc*>(static_cast<const unsigned char*>(ctx->img_desc_ws.ptr) + img_bytes);
+    const EqDesc* eq_dev = reinterpret_cast<const EqDesc*>(static_cast<const unsigned char*>(ctx->img_desc_ws.ptr) + img_bytes + pass_bytes);
+    const uint8_t* luts = ws + lut_off;
+    int* hist = reinterpret_cast<int*>(ws + hist_off);
+    if (!eqs.empty()) SSDK_CHECK_CUDA(cudaMemsetAsync(hist, 0, eqs.size() * 256 * sizeof(int), stream));
     const int gx = std::max(1, std::min(ceil_div(photo_groups, kPhotoThreads * kPhotoGroupsPerThread), 65535));
     rc = launch(ctx, photometric_kernel, dim3(gx, (unsigned)photo.size()), kPhotoThreads, 0, stream,
-                src_dev, reinterpret_cast<const PhotoDesc*>(static_cast<const unsigned char*>(ctx->img_desc_ws.ptr) + img_bytes),
-                static_cast<uint8_t*>(ctx->photo_ws.ptr));
+                src_dev, pass_dev, luts, ws);
     if (rc) return rc;
+    pass_dev += photo.size();
+    for (int k = 1; k <= max_eq; ++k) {                           // equalisation k, then the pass that starts with its table
+      const int gk = std::max(1, std::min(ceil_div(pass_groups[k], kPhotoThreads * kPhotoGroupsPerThread), 65535));
+      rc = launch(ctx, equalize_hist_kernel, dim3(gk, (unsigned)pass_n[k]), kEqThreads, 0, stream, (const uint8_t*)ws, eq_dev, hist);
+      if (rc) return rc;
+      rc = launch(ctx, equalize_lut_kernel, pass_n[k], kEqThreads, 0, stream, eq_dev, (const int*)hist, ws + lut_off);
+      if (rc) return rc;
+      rc = launch(ctx, photometric_kernel, dim3(gk, (unsigned)pass_n[k]), kPhotoThreads, 0, stream, src_dev, pass_dev, luts, ws);
+      if (rc) return rc;
+      eq_dev += pass_n[k];
+      pass_dev += pass_n[k];
+    }
   }
   const bool warp = std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return d.mode == kImgWarp; });
   const bool wide = std::any_of(descs.begin(), descs.end(), [](const ImgDesc& d) { return is_wide(d.mode); });

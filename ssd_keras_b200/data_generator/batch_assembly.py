@@ -30,17 +30,17 @@ one list moves the boxes and produces the image batch; ``assemble_training_batch
   border is black;
 - ``box_filter``, ``overlap_filter``, ``clip``: boxes only;
 - the photometric ops (``convert_dtype``, ``brightness``, ``contrast``, ``saturation``, ``hue``, ``convert_color``,
-  ``channel_swap``; ``object_detection_2d_photometric_ops.py``) come before every geometric op, as in all three training chains,
-  and run as a uint8 pre-pass on the device, bit-exact to NumPy and to OpenCV 4.13's uint8 ``cv2.cvtColor`` on a CPU with AVX2
-  (``oracle/photoops.py`` restates them).  ``photometric_ops`` returns ``SSDPhotometricDistortions``' two sequences.
+  ``channel_swap``, ``equalize_hist``; ``object_detection_2d_photometric_ops.py``) come before every geometric op, as in all
+  three training chains, and run as a uint8 pre-pass on the device, bit-exact to NumPy and to OpenCV 4.13's uint8
+  ``cv2.cvtColor`` on a CPU with AVX2 (``oracle/photoops.py`` restates them) and ``cv2.equalizeHist``
+  (``tests/equalize_reference.py``).  ``photometric_ops`` returns ``SSDPhotometricDistortions``' two sequences.
 
 ``translate_ops`` / ``scale_ops`` / ``rotate_ops`` / ``crop_pad_ops`` / ``resize_ops`` / ``box_filter_ops`` return the whole op
 sequence one call of the reference class runs, box filter and clipping included, so the geometric halves of
 ``DataAugmentationConstantInputSize`` (SSD7: translate -> zoom in -> flip, or zoom out -> translate -> flip) and
 ``DataAugmentationSatellite`` (flips -> rotate -> patch -> resize) are one op list per image.
 
-Not covered: ``Gamma`` (the reference's raises), histogram equalisation, conversion to GRAY, a second resampling step, JPEG
-decoding.  The random decisions of a chain (which patch, flip or not, which factor, which photometric op with which delta) are
+Not covered: ``Gamma`` (the reference's raises), conversion to GRAY, a second resampling step, JPEG decoding.  The random decisions of a chain (which patch, flip or not, which factor, which photometric op with which delta) are
 the caller's: the planners of ``data_augmentation_chain_original_ssd``, ``_constant_input_size`` (SSD7), ``_variable_input_size``
 and ``_satellite`` draw them in the reference's order, and ``DataGenerator.generate`` runs them."""
 import ctypes as C
@@ -193,6 +193,12 @@ def channel_swap(order):
     if sorted(order) != [0, 1, 2]:
         raise ValueError('`order` must be a permutation of (0, 1, 2)')
     return (_ffi.BOXOP_CHANNEL_SWAP, 0, float(order[0]), float(order[1]), float(order[2]), 0.0)
+
+
+def equalize_hist():
+    """``HistogramEqualization`` (photometric_ops.py:397-411): ``image[:, :, 2] = cv2.equalizeHist(image[:, :, 2])`` on a uint8
+    image (HSV in the reference's intent; nothing checks it), OpenCV 4.13's table bit for bit."""
+    return (_ffi.BOXOP_EQUALIZE_V, 0, 0.0, 0.0, 0.0, 0.0)
 
 
 def photometric_ops(sequence, brightness=None, contrast=None, saturation=None, hue=None, channel_swap=None):

@@ -84,9 +84,25 @@ def _ends_degenerate_free(ops):
     for code, flags in ((o[0], o[1]) for o in reversed(ops)):
         if code in (_ffi.BOXOP_RESIZE, _ffi.BOXOP_RESIZE_INTERP, _ffi.BOXOP_FILTER):
             return bool(flags & 1)
-        if code != _ffi.BOXOP_OVERLAP and not _ffi.BOXOP_TO_FLOAT32 <= code <= _ffi.BOXOP_CHANNEL_SWAP:
+        if code != _ffi.BOXOP_OVERLAP and code not in _ffi.PHOTO_OPS:
             return False
     return False
+
+
+_GEOMETRIC_OPS = frozenset(range(_ffi.BOXOP_CROP_PAD, _ffi.BOXOP_ROTATE + 1)) - {_ffi.BOXOP_FILTER} | {_ffi.BOXOP_RESIZE_INTERP}
+
+
+def _check_photometric_prefix(ops, transformations, owners):
+    """The device runs an image's photometric ops before its geometry: refuse a list where one follows an op that changes the
+    image geometry, naming both transformations."""
+    first_geometric = None
+    for o, k in zip(ops, owners):
+        if o[0] in _GEOMETRIC_OPS and first_geometric is None:
+            first_geometric = k
+        elif o[0] in _ffi.PHOTO_OPS and first_geometric is not None:
+            raise ValueError('the photometric transformation %r comes after %r, which changes the image geometry; the device runs '
+                             'the photometric ops of an image first, so they must come before every crop, pad, flip, resize, '
+                             'translation, scale and rotation' % (transformations[k], transformations[first_geometric]))
 
 
 class DataGenerator:
@@ -316,8 +332,9 @@ class DataGenerator:
                  keep_images_without_gt=False, degenerate_box_handling='remove'):
         """Yields batches indefinitely, as the reference's ``generate`` (same arguments and return order), from a device assembly
         of each batch.  ``transformations``: planners of this package (the three training chains, ``SSDDataAugmentation`` and
-        their parts: ``Resize``, ``ResizeRandomInterp``, ``RandomFlip``, ``RandomTranslate``, ``RandomScale``, ``RandomRotate``,
-        ``RandomPatch``, ``ConvertTo3Channels``); after them every image of a batch must have one size.
+        the classes of the op modules: ``object_detection_2d_geometric_ops``, ``_patch_sampling_ops`` and ``_photometric_ops``),
+        in any order that puts the photometric ops of an image before its first crop, pad, flip, resize, translation, scale or
+        rotation (``ValueError`` otherwise); after them every image of a batch must have one size.
         ``'processed_images'`` is a float32 CUDA tensor ``(B, H, W, 3)``; ``'encoded_labels'`` the float32 CUDA ``y_true``;
         ``'processed_labels'`` a list of float64 arrays read back from the device."""
         if self.dataset_size == 0:
@@ -402,10 +419,12 @@ class DataGenerator:
                 labels = batch_y[i] if batch_y is not None else None
                 if labels is not None and labels.size == 0 and not keep_images_without_gt:
                     continue                                       # no draws for an image without boxes
-                o, h, w = [], x.shape[0], x.shape[1]
-                for t in transformations:
+                o, owners, h, w = [], [], x.shape[0], x.shape[1]
+                for k, t in enumerate(transformations):
                     o_t, h, w, labels = t.plan(h, w, labels)
                     o += o_t
+                    owners += [k] * len(o_t)
+                _check_photometric_prefix(o, transformations, owners)
                 if out_hw is None:
                     out_hw = (h, w)
                 elif out_hw != (h, w):

@@ -1,7 +1,8 @@
-"""The geometric ops of the training chains as planners for ``DataGenerator.generate``: ``Resize``, ``ResizeRandomInterp``,
-``RandomFlip``, ``RandomTranslate``, ``RandomScale`` and ``RandomRotate`` (the reference's object_detection_2d_geometric_ops.py).
-Each one draws what the reference draws, from the global ``np.random`` in the same order (``RandomRotate``'s angle from
-Python's ``random``, as there), and returns the op records of ``batch_assembly`` that the device runs for it.
+"""The geometric ops as planners for ``DataGenerator.generate``: ``Resize``, ``ResizeRandomInterp``, ``Flip``, ``RandomFlip``,
+``Translate``, ``RandomTranslate``, ``Scale``, ``RandomScale``, ``Rotate`` and ``RandomRotate`` (the reference's
+object_detection_2d_geometric_ops.py), each random one built on its deterministic one, as there.  Each one draws what the
+reference draws, from the global ``np.random`` in the same order (``RandomRotate``'s angle from Python's ``random``, as there),
+and returns the op records of ``batch_assembly`` that the device runs for it.
 
 A planner's ``plan(img_height, img_width, labels)`` returns ``(ops, img_height, img_width, labels)``: the records, the image
 size after them, and the host's copy of the labels where a later draw still depends on them (``None`` once the boxes are the
@@ -124,8 +125,29 @@ class ResizeRandomInterp(DevicePlanner):
         return self.resize.plan(img_height, img_width, labels)
 
 
+class Flip(DevicePlanner):
+    """``Flip(dim)``: the image mirrored horizontally or vertically, the boxes with it."""
+
+    def __init__(self, dim='horizontal', labels_format=DEFAULT_LABELS_FORMAT):
+        if dim not in {'horizontal', 'vertical'}:
+            raise ValueError("`dim` can be one of 'horizontal' and 'vertical'.")
+        self.dim = dim
+        self.labels_format = labels_format
+
+    def plan(self, img_height, img_width, labels):
+        xmin, ymin, xmax, ymax = box_columns(self.labels_format)
+        size = img_width if self.dim == 'horizontal' else img_height
+        if labels is not None:
+            labels = np.copy(labels)
+            if self.dim == 'horizontal':
+                labels[:, [xmin, xmax]] = img_width - labels[:, [xmax, xmin]]
+            else:
+                labels[:, [ymin, ymax]] = img_height - labels[:, [ymax, ymin]]
+        return [ba.flip(size, self.dim)], img_height, img_width, labels
+
+
 class RandomFlip(DevicePlanner):
-    """``RandomFlip(dim, prob)``: flips when ``np.random.uniform(0, 1) >= 1 - prob``."""
+    """``RandomFlip(dim, prob)``: ``Flip`` when ``np.random.uniform(0, 1) >= 1 - prob``."""
 
     def __init__(self, dim='horizontal', prob=0.5, labels_format=DEFAULT_LABELS_FORMAT):
         if dim not in {'horizontal', 'vertical'}:
@@ -133,20 +155,38 @@ class RandomFlip(DevicePlanner):
         self.dim = dim
         self.prob = prob
         self.labels_format = labels_format
+        self.flip = Flip(dim=dim, labels_format=labels_format)
 
     def plan(self, img_height, img_width, labels):
         p = np.random.uniform(0, 1)
         if p >= (1.0 - self.prob):
-            xmin, ymin, xmax, ymax = box_columns(self.labels_format)
-            size = img_width if self.dim == 'horizontal' else img_height
-            if labels is not None:
-                labels = np.copy(labels)
-                if self.dim == 'horizontal':
-                    labels[:, [xmin, xmax]] = img_width - labels[:, [xmax, xmin]]
-                else:
-                    labels[:, [ymin, ymax]] = img_height - labels[:, [ymax, ymin]]
-            return [ba.flip(size, self.dim)], img_height, img_width, labels
+            self.flip.labels_format = self.labels_format
+            return self.flip.plan(img_height, img_width, labels)
         return [], img_height, img_width, labels
+
+
+class Translate(DevicePlanner):
+    """``Translate(dy, dx, clip_boxes, box_filter, background)``: a shift by ``int(round(h * dy))`` rows and
+    ``int(round(w * dx))`` columns, then ``box_filter`` against the image and the clip."""
+
+    def __init__(self, dy, dx, clip_boxes=True, box_filter=None, background=(0, 0, 0), labels_format=DEFAULT_LABELS_FORMAT):
+        check_box_filter(box_filter)
+        self.dy_rel = dy
+        self.dx_rel = dx
+        self.clip_boxes = clip_boxes
+        self.box_filter = box_filter
+        self.background = background
+        self.labels_format = labels_format
+
+    def plan(self, img_height, img_width, labels):
+        ops = ba.translate_ops(img_height, img_width, self.dy_rel, self.dx_rel, self.box_filter, self.clip_boxes, self.background)
+        if labels is not None:
+            xmin, ymin, xmax, ymax = box_columns(self.labels_format)
+            labels = np.copy(labels)
+            labels[:, [xmin, xmax]] += int(round(img_width * self.dx_rel))
+            labels[:, [ymin, ymax]] += int(round(img_height * self.dy_rel))
+            labels = filter_and_clip(labels, self.box_filter, self.clip_boxes, img_height, img_width, self.labels_format)
+        return ops, img_height, img_width, labels
 
 
 class RandomTranslate(DevicePlanner):
@@ -164,7 +204,6 @@ class RandomTranslate(DevicePlanner):
         if dy_minmax[0] < 0 or dx_minmax[0] < 0:
             raise ValueError("It must be `dy_minmax[0] >= 0` and `dx_minmax[0] >= 0`.")
         check_image_validator(image_validator)
-        check_box_filter(box_filter)
         self.dy_minmax = dy_minmax
         self.dx_minmax = dx_minmax
         self.prob = prob
@@ -174,16 +213,13 @@ class RandomTranslate(DevicePlanner):
         self.n_trials_max = n_trials_max
         self.background = background
         self.labels_format = labels_format
+        self.translate = Translate(dy=0, dx=0, clip_boxes=clip_boxes, box_filter=box_filter, background=background,
+                                   labels_format=labels_format)
 
     def _translate(self, img_height, img_width, dy, dx, labels):
-        ops = ba.translate_ops(img_height, img_width, dy, dx, self.box_filter, self.clip_boxes, self.background)
-        if labels is not None:
-            xmin, ymin, xmax, ymax = box_columns(self.labels_format)
-            labels = np.copy(labels)
-            labels[:, [xmin, xmax]] += int(round(img_width * dx))
-            labels[:, [ymin, ymax]] += int(round(img_height * dy))
-            labels = filter_and_clip(labels, self.box_filter, self.clip_boxes, img_height, img_width, self.labels_format)
-        return ops, img_height, img_width, labels
+        self.translate.dy_rel, self.translate.dx_rel = dy, dx
+        self.translate.labels_format = self.labels_format
+        return self.translate.plan(img_height, img_width, labels)
 
     def plan(self, img_height, img_width, labels):
         if not np.random.uniform(0, 1) >= (1.0 - self.prob):
@@ -206,6 +242,29 @@ class RandomTranslate(DevicePlanner):
         return [], img_height, img_width, labels
 
 
+class Scale(DevicePlanner):
+    """``Scale(factor, clip_boxes, box_filter, background)``: a zoom by ``factor`` about the image centre, same output size,
+    then ``box_filter`` against the image and the clip."""
+
+    def __init__(self, factor, clip_boxes=True, box_filter=None, background=(0, 0, 0), labels_format=DEFAULT_LABELS_FORMAT):
+        if factor <= 0:
+            raise ValueError("It must be `factor > 0`.")
+        check_box_filter(box_filter)
+        self.factor = factor
+        self.clip_boxes = clip_boxes
+        self.box_filter = box_filter
+        self.background = background
+        self.labels_format = labels_format
+
+    def plan(self, img_height, img_width, labels):
+        ops = ba.scale_ops(img_height, img_width, self.factor, self.box_filter, self.clip_boxes, self.background)
+        if labels is not None:
+            M = rotation_matrix_2d(img_width / 2, img_height / 2, 0, self.factor)
+            labels = filter_and_clip(move_corners(labels, M, self.labels_format), self.box_filter, self.clip_boxes, img_height,
+                                     img_width, self.labels_format)
+        return ops, img_height, img_width, labels
+
+
 class RandomScale(DevicePlanner):
     """``RandomScale``: with probability ``prob``, up to ``max(1, n_trials_max)`` zoom factors in ``[min_factor, max_factor]``
     about the image centre until ``image_validator`` accepts the scaled boxes; the first accepted factor runs as ``Scale``.  If
@@ -216,7 +275,6 @@ class RandomScale(DevicePlanner):
         if not (0 < min_factor <= max_factor):
             raise ValueError("It must be `0 < min_factor <= max_factor`.")
         check_image_validator(image_validator)
-        check_box_filter(box_filter)
         self.min_factor = min_factor
         self.max_factor = max_factor
         self.prob = prob
@@ -226,14 +284,12 @@ class RandomScale(DevicePlanner):
         self.n_trials_max = n_trials_max
         self.background = background
         self.labels_format = labels_format
+        self.scale = Scale(factor=1.0, clip_boxes=clip_boxes, box_filter=box_filter, background=background, labels_format=labels_format)
 
     def _scale(self, img_height, img_width, factor, labels):
-        ops = ba.scale_ops(img_height, img_width, factor, self.box_filter, self.clip_boxes, self.background)
-        if labels is not None:
-            M = rotation_matrix_2d(img_width / 2, img_height / 2, 0, factor)
-            labels = filter_and_clip(move_corners(labels, M, self.labels_format), self.box_filter, self.clip_boxes, img_height,
-                                     img_width, self.labels_format)
-        return ops, img_height, img_width, labels
+        self.scale.factor = factor
+        self.scale.labels_format = self.labels_format
+        return self.scale.plan(img_height, img_width, labels)
 
     def plan(self, img_height, img_width, labels):
         if not np.random.uniform(0, 1) >= (1.0 - self.prob):
@@ -250,9 +306,30 @@ class RandomScale(DevicePlanner):
         return [], img_height, img_width, labels
 
 
+class Rotate(DevicePlanner):
+    """``Rotate(angle)``: counter-clockwise by 90, 180 or 270 degrees; the output is w x h for 90 and 270."""
+
+    def __init__(self, angle, labels_format=DEFAULT_LABELS_FORMAT):
+        if angle not in {90, 180, 270}:
+            raise ValueError("`angle` must be in the set {90, 180, 270}.")
+        self.angle = angle
+        self.labels_format = labels_format
+
+    def plan(self, img_height, img_width, labels):
+        M, h_new, w_new = rotate_geometry(img_height, img_width, self.angle)
+        if labels is not None:
+            xmin, ymin, xmax, ymax = box_columns(self.labels_format)
+            labels = move_corners(labels, M, self.labels_format)
+            if self.angle in (90, 180):
+                labels[:, [ymax, ymin]] = labels[:, [ymin, ymax]]
+            if self.angle in (180, 270):
+                labels[:, [xmax, xmin]] = labels[:, [xmin, xmax]]
+        return ba.rotate_ops(img_height, img_width, self.angle), h_new, w_new, labels
+
+
 class RandomRotate(DevicePlanner):
-    """``RandomRotate``: with probability ``prob`` (``np.random``), a counter-clockwise rotation by an angle drawn with Python's
-    ``random.choice(angles)``; the output is w x h for 90 and 270 degrees."""
+    """``RandomRotate``: with probability ``prob`` (``np.random``), ``Rotate`` by an angle drawn with Python's
+    ``random.choice(angles)``."""
 
     def __init__(self, angles=(90, 180, 270), prob=0.5, labels_format=DEFAULT_LABELS_FORMAT):
         for angle in angles:
@@ -261,17 +338,11 @@ class RandomRotate(DevicePlanner):
         self.angles = list(angles)
         self.prob = prob
         self.labels_format = labels_format
+        self.rotate = Rotate(angle=90, labels_format=labels_format)
 
     def plan(self, img_height, img_width, labels):
         if not np.random.uniform(0, 1) >= (1.0 - self.prob):
             return [], img_height, img_width, labels
-        angle = random.choice(self.angles)
-        M, h_new, w_new = rotate_geometry(img_height, img_width, angle)
-        if labels is not None:
-            xmin, ymin, xmax, ymax = box_columns(self.labels_format)
-            labels = move_corners(labels, M, self.labels_format)
-            if angle in (90, 180):
-                labels[:, [ymax, ymin]] = labels[:, [ymin, ymax]]
-            if angle in (180, 270):
-                labels[:, [xmax, xmin]] = labels[:, [xmin, xmax]]
-        return ba.rotate_ops(img_height, img_width, angle), h_new, w_new, labels
+        self.rotate.angle = random.choice(self.angles)
+        self.rotate.labels_format = self.labels_format
+        return self.rotate.plan(img_height, img_width, labels)

@@ -1,5 +1,11 @@
-"""The photometric ops of the training chains as planners for ``DataGenerator.generate`` (the reference's
-object_detection_2d_photometric_ops.py).
+"""The photometric ops as planners for ``DataGenerator.generate`` (the reference's object_detection_2d_photometric_ops.py):
+``ConvertColor`` (RGB <-> HSV), ``ConvertDataType``, ``ConvertTo3Channels``, ``Brightness``, ``Contrast``, ``Saturation``,
+``Hue``, ``ChannelSwap``, ``HistogramEqualization`` and their random forms.  The device runs them as a prefix of each image's
+op list: they must come before every op that changes the image geometry, which ``generate()`` checks when it plans a batch.
+Like the reference classes, ``Brightness`` / ``Contrast`` / ``Saturation`` / ``Hue`` expect a float32 image
+(``ConvertDataType('float32')`` first, HSV for the last two), and the colour conversions and ``HistogramEqualization`` a uint8
+one; the list must end in uint8.  Not covered: conversion to GRAY (``NotImplementedError`` when planned) and ``Gamma`` /
+``RandomGamma``, whose ``__call__`` fails in the reference.
 
 ``ConvertTo3Channels``: the device converts every image to 3 channels first (gray is replicated, RGBA drops alpha), so it adds
 no op.
@@ -17,6 +23,124 @@ from .object_detection_2d_geometric_ops import DevicePlanner
 
 class ConvertTo3Channels(DevicePlanner):
     def plan(self, img_height, img_width, labels):
+        return [], img_height, img_width, labels
+
+
+class ConvertColor(DevicePlanner):
+    """``ConvertColor(current, to)``: uint8 ``cv2.cvtColor`` between RGB and HSV; ``current == to`` leaves the image alone."""
+
+    def __init__(self, current='RGB', to='HSV', keep_3ch=True):
+        if not ((current in {'RGB', 'HSV'}) and (to in {'RGB', 'HSV', 'GRAY'})):
+            raise NotImplementedError
+        self.current = current
+        self.to = to
+        self.keep_3ch = keep_3ch
+
+    def plan(self, img_height, img_width, labels):
+        if self.to == 'GRAY':
+            raise NotImplementedError('ConvertColor to GRAY is not supported on the device')
+        return ([] if self.current == self.to else [ba.convert_color(self.current, self.to)]), img_height, img_width, labels
+
+
+class ConvertDataType(DevicePlanner):
+    """``ConvertDataType(to)``: ``astype(float32)``, or ``np.round`` and ``astype(uint8)``."""
+
+    def __init__(self, to='uint8'):
+        if not (to == 'uint8' or to == 'float32'):
+            raise ValueError("`to` can be either of 'uint8' or 'float32'.")
+        self.to = to
+
+    def plan(self, img_height, img_width, labels):
+        return [ba.convert_dtype(self.to)], img_height, img_width, labels
+
+
+class _Photometric(DevicePlanner):
+    """A deterministic op: ``op(value)``, the value in the attribute ``value_name``."""
+
+    def plan(self, img_height, img_width, labels):
+        return [self.op(getattr(self, self.value_name))], img_height, img_width, labels
+
+
+class Brightness(_Photometric):
+    """``Brightness(delta)``: ``np.clip(image + delta, 0, 255)`` on an RGB float32 image."""
+    op, value_name = staticmethod(ba.brightness), 'delta'
+
+    def __init__(self, delta):
+        self.delta = delta
+
+
+class Contrast(_Photometric):
+    """``Contrast(factor)``: ``np.clip(127.5 + factor * (image - 127.5), 0, 255)`` on an RGB float32 image."""
+    op, value_name = staticmethod(ba.contrast), 'factor'
+
+    def __init__(self, factor):
+        if factor <= 0.0:
+            raise ValueError("It must be `factor > 0`.")
+        self.factor = factor
+
+
+class Saturation(_Photometric):
+    """``Saturation(factor)``: the S channel of an HSV float32 image times ``factor``, clipped."""
+    op, value_name = staticmethod(ba.saturation), 'factor'
+
+    def __init__(self, factor):
+        if factor <= 0.0:
+            raise ValueError("It must be `factor > 0`.")
+        self.factor = factor
+
+
+class Hue(_Photometric):
+    """``Hue(delta)``: ``(H + delta) % 180`` on the H channel of an HSV float32 image."""
+    op, value_name = staticmethod(ba.hue), 'delta'
+
+    def __init__(self, delta):
+        if not (-180 <= delta <= 180):
+            raise ValueError("`delta` must be in the closed interval `[-180, 180]`.")
+        self.delta = delta
+
+
+class ChannelSwap(_Photometric):
+    """``ChannelSwap(order)``: ``image[:, :, order]``."""
+    op, value_name = staticmethod(ba.channel_swap), 'order'
+
+    def __init__(self, order):
+        self.order = order
+
+
+class HistogramEqualization(DevicePlanner):
+    """``HistogramEqualization()``: ``cv2.equalizeHist`` of channel 2 (V of an HSV image) on a uint8 image.  The reference's
+    writes into its input, so with images held in memory a 3-channel dataset image it receives directly is changed for later
+    epochs; the device leaves the dataset alone."""
+
+    def plan(self, img_height, img_width, labels):
+        return [ba.equalize_hist()], img_height, img_width, labels
+
+
+class RandomHistogramEqualization(DevicePlanner):
+    """``HistogramEqualization`` when ``np.random.uniform(0, 1) >= 1 - prob``."""
+
+    def __init__(self, prob=0.5):
+        self.prob = prob
+        self.equalize = HistogramEqualization()
+
+    def plan(self, img_height, img_width, labels):
+        if np.random.uniform(0, 1) >= (1.0 - self.prob):
+            return self.equalize.plan(img_height, img_width, labels)
+        return [], img_height, img_width, labels
+
+
+class RandomChannelSwap(DevicePlanner):
+    """With ``np.random.uniform(0, 1) >= 1 - prob``, ``ChannelSwap`` to one of the five other orders, ``np.random.randint(5)``."""
+
+    def __init__(self, prob=0.5):
+        self.prob = prob
+        self.permutations = ((0, 2, 1), (1, 0, 2), (1, 2, 0), (2, 0, 1), (2, 1, 0))
+        self.swap_channels = ChannelSwap(order=(0, 1, 2))
+
+    def plan(self, img_height, img_width, labels):
+        if np.random.uniform(0, 1) >= (1.0 - self.prob):
+            self.swap_channels.order = self.permutations[np.random.randint(5)]
+            return self.swap_channels.plan(img_height, img_width, labels)
         return [], img_height, img_width, labels
 
 
