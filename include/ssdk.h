@@ -183,7 +183,8 @@ typedef struct { int op; int flags; double a0, a1, a2, a3; } ssdk_box_op;
 /* gt_in_dev [total_in*5] float32 (gt_in_f64 = 0) or float64 (1) rows (class, xmin, ymin, xmax, ymax), offsets_in_dev [B+1]; ops_dev [B*max_ops] (a list ends at
  * SSDK_BOXOP_END or after max_ops entries; max_ops = 0: pack only).  Outputs: gt_out_dev [<= total_in*5], offsets_out_dev [B+1],
  * out_stats_dev (optional) [2] = total number of boxes left, largest per-image count.  Everything stays on the device: feed
- * the result to ssdk_encode with device offsets and total_in / the input's largest count as upper bounds. */
+ * the result to ssdk_encode with device offsets and total_in / the input's largest count as upper bounds.  The calls of one
+ * context share a workspace: a call's kernels wait for those of the previous call, on whatever stream it ran. */
 int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_in_f64, const int* offsets_in_dev, int B, int total_in,
                         const ssdk_box_op* ops_dev, int max_ops, float* gt_out_dev, int* offsets_out_dev, int* out_stats_dev,
                         void* stream);

@@ -222,6 +222,10 @@ extern "C" int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_
   SSDK_REQUIRE(total_in == 0 || gt_in_dev, "ssdk_assemble_batch: gt_in_dev is NULL");
   SSDK_REQUIRE(max_ops == 0 || ops_dev, "ssdk_assemble_batch: ops_dev is NULL");
   cudaStream_t stream = (cudaStream_t)stream_;
+  // Calls may come on different streams (the data generator reads boxes back on a side stream while the training step runs):
+  // each one's kernels wait for the previous call's, which used the same box_ws.
+  if (ctx->box_ws_done) SSDK_CHECK_CUDA(cudaStreamWaitEvent(stream, ctx->box_ws_done, 0));
+  else SSDK_CHECK_CUDA(cudaEventCreateWithFlags(&ctx->box_ws_done, cudaEventDisableTiming));
   const size_t need = (size_t)(total_in > 0 ? total_in : 1) * 5 * sizeof(float) + (size_t)B * sizeof(int) + 256;
   int rc = ctx->box_ws.ensure(need);
   if (rc) return rc;
@@ -231,7 +235,10 @@ extern "C" int ssdk_assemble_batch(ssdk_ctx* ctx, const void* gt_in_dev, int gt_
   if (rc) return rc;
   rc = launch(ctx, box_offsets_kernel, 1, 1024, 0, stream, counts, B, offsets_out_dev, out_stats_dev);
   if (rc) return rc;
-  return launch(ctx, box_pack_kernel, B, kBoxThreads, 0, stream, tmp, offsets_in_dev, offsets_out_dev, gt_out_dev);
+  rc = launch(ctx, box_pack_kernel, B, kBoxThreads, 0, stream, tmp, offsets_in_dev, offsets_out_dev, gt_out_dev);
+  if (rc) return rc;
+  SSDK_CHECK_CUDA(cudaEventRecord(ctx->box_ws_done, stream));
+  return SSDK_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -108,6 +108,7 @@ struct ssdk_ctx {
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for
   int loss_parity = 0;          // which of its two histogram sets the next loss call uses (the other one is being cleared)
   ssdk::Scratch box_ws;         // ssdk_assemble_batch: transformed boxes and per-image counts
+  cudaEvent_t box_ws_done = nullptr;  // recorded after the last ssdk_assemble_batch: box_ws is free once it has completed
   ssdk::Scratch img_desc_ws;    // ssdk_assemble_images: per-image and photometric descriptors
   ssdk::Scratch photo_ws;       // ssdk_assemble_images: images after the photometric pre-pass
   cudaDeviceProp prop{};

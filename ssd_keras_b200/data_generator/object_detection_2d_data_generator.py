@@ -16,6 +16,9 @@ The reference checks the processed boxes for degenerate ones after the chain.  W
 degenerate-box filter (``Resize`` with one, as in ``SSDDataAugmentation`` and the variable-input-size and satellite chains), no
 box can be degenerate and nothing is checked; otherwise (the SSD7 chain's lists end in a flip, or in the clip of a translation
 or zoom) the processed boxes are read back once and the reference's ``'remove'`` / ``'warn'`` rules are applied to them.
+That read-back, and the one of ``'processed_labels'``, run on a side stream of their own: they wait for the box work they
+need, not for a training step or prediction still running on the caller's stream, so ``fit_generator`` can plan and assemble
+the next batch while the device trains on the current one.
 
 Not covered: HDF5 datasets, ``'matched_anchors'`` and ``'inverse_transform'`` returns, and
 transformations other than the planners of this package."""
@@ -103,6 +106,18 @@ def _check_photometric_prefix(ops, transformations, owners):
             raise ValueError('the photometric transformation %r comes after %r, which changes the image geometry; the device runs '
                              'the photometric ops of an image first, so they must come before every crop, pad, flip, resize, '
                              'translation, scale and rotation' % (transformations[k], transformations[first_geometric]))
+
+
+def _read_boxes(labels, ops, side):
+    """The boxes of ``labels`` after ``ops``, read back to the host: float32 ``(N, 5)`` rows and ``(B+1,)`` offsets.  The work
+    runs on ``side``, a stream held in a list that the first call fills: it starts once the previous box assembly has
+    finished (``ssdk_assemble_batch`` orders its calls) and the host waits for nothing else on the device."""
+    import torch
+    if not side:
+        side.append(torch.cuda.Stream())
+    with torch.cuda.stream(side[0]):
+        gt, offs = ba.assemble_batch_device(labels, ops)[:2]
+        return gt.cpu().numpy(), offs.cpu().numpy()
 
 
 class DataGenerator:
@@ -357,6 +372,7 @@ class DataGenerator:
             warnings.warn("Since no label encoder was given, 'encoded_labels' is not possible; it will be `None`.")
         for t in transformations:
             t.labels_format = self.labels_format
+        side = []                              # the stream of the box read-backs, made by the first one
         with ThreadPoolExecutor(_DECODE_THREADS) as pool:
             for batch in self.plan_batches(batch_size, shuffle, transformations, keep_images_without_gt, pool):
                 batch_X, batch_y, keep, ops, out_hw = (batch[k] for k in ('images', 'labels', 'keep', 'ops', 'out_hw'))
@@ -364,7 +380,7 @@ class DataGenerator:
                 batch_original_images = [np.copy(x) for x in batch_X] if 'original_images' in returns else None
                 batch_original_labels = [np.copy(y) for y in batch_y] if 'original_labels' in returns and batch_y is not None else None
                 if batch_y is not None and keep and not all(_ends_degenerate_free(o) for o in ops):
-                    keep, ops = self._degenerate_check(batch_X, batch_y, keep, ops, degenerate_box_handling, keep_images_without_gt)
+                    keep, ops = self._degenerate_check(batch_X, batch_y, keep, ops, degenerate_box_handling, keep_images_without_gt, side)
                 if not keep:
                     raise DegenerateBatchError('You produced an empty batch.')
 
@@ -377,9 +393,8 @@ class DataGenerator:
                     X, y_enc = ba.assemble_images_device(X_in, ops, out_hw[0], out_hw[1]), None
                 processed = None
                 if 'processed_labels' in returns and batch_y is not None:
-                    gt, offs = ba.assemble_batch_device(y_in, ops)[:2]
-                    gt, offs = gt.cpu().numpy().astype(np.float64), offs.cpu().numpy()
-                    processed = [gt[offs[b]:offs[b + 1]] for b in range(len(keep))]
+                    gt, offs = _read_boxes(y_in, ops, side)
+                    processed = [gt[offs[b]:offs[b + 1]].astype(np.float64) for b in range(len(keep))]
                 ret = []
                 if 'processed_images' in returns: ret.append(X)
                 if 'encoded_labels' in returns: ret.append(y_enc)
@@ -453,11 +468,11 @@ class DataGenerator:
         names = self.filenames[lo:lo + batch_size]
         return [pool.submit(load_image, f) for f in names] if pool is not None else [load_image(f) for f in names]
 
-    def _degenerate_check(self, batch_X, batch_y, keep, ops, handling, keep_images_without_gt):
-        """The reference's check on the processed boxes (one read-back): 'warn' warns, 'remove' filters the degenerate boxes and
-        drops the images it empties (unless ``keep_images_without_gt``); the filter joins the image's op list."""
-        gt, offs = ba.assemble_batch_device([batch_y[i] for i in keep], ops)[:2]
-        gt, offs = gt.cpu().numpy(), offs.cpu().numpy()
+    def _degenerate_check(self, batch_X, batch_y, keep, ops, handling, keep_images_without_gt, side):
+        """The reference's check on the processed boxes (one read-back, see ``_read_boxes``): 'warn' warns, 'remove' filters the
+        degenerate boxes and drops the images it empties (unless ``keep_images_without_gt``); the filter joins the image's op
+        list."""
+        gt, offs = _read_boxes([batch_y[i] for i in keep], ops, side)
         new_keep, new_ops = [], []
         for b, (i, o) in enumerate(zip(keep, ops)):
             labels = gt[offs[b]:offs[b + 1]]

@@ -399,14 +399,29 @@ class SSDModel(KerasTrainingMixin):
         y = self.forward_device(images)
         return y if self.decoder is None else self.decoder(y)
 
+    def _device_batch(self, x):
+        """A CUDA image batch as the forward pass takes it: float32 (B, H, W, C) of this model's input size on the current
+        device.  Anything else raises ``ValueError`` (a host batch is converted by the callers instead)."""
+        import torch
+        want = (self.img_height, self.img_width, self.img_channels)
+        if x.dtype != torch.float32:
+            raise ValueError('a CUDA image batch must be float32, got %s' % (x.dtype,))
+        if x.device != torch.device('cuda', torch.cuda.current_device()):
+            raise ValueError('the CUDA image batch is on %s, but this model runs on cuda:%d' % (x.device, torch.cuda.current_device()))
+        if x.dim() != 4 or tuple(x.shape[1:]) != want:
+            raise ValueError('a CUDA image batch must have the shape (B, %d, %d, %d), got %s' % (want + (tuple(x.shape),)))
+        return x
+
     def predict_stream(self, batches, post=None):
-        """Generator over HOST batches -> HOST results, in order, software-pipelined: while the kernels of batch i run, batch
+        """Generator over image batches -> HOST results, in order, software-pipelined: while the kernels of batch i run, batch
         i+1 is already on its way to the device (copy stream) and the host is still reading the result of batch i-1; the host
         only ever waits for the device->host copy of the PREVIOUS batch, so the GPU does not idle between batches (what Keras'
         ``predict_generator`` does with its queue of prefetched batches; the reference drives its models that way in
         eval_utils/average_precision_evaluator.py:373-380).
 
-        batches: iterable of float32 (B,H,W,3) pinned CPU tensors (used as they are) or ndarrays (pinned here, one host copy).
+        batches: iterable of float32 (B,H,W,3) pinned CPU tensors (used as they are), ndarrays (pinned here, one host copy) or
+                 float32 CUDA tensors on the current device, such as ``DataGenerator.generate``'s ``'processed_images'``.  A
+                 CUDA batch is used where it lies, after the work already enqueued on the current stream: no copy, no staging.
         post:    optional function applied to the device result of each batch before it is downloaded (e.g. an all-gather).
         Yields pinned CPU tensors out of three rotating buffers owned by the model (allocating pinned memory costs milliseconds,
         so it happens once per result shape): a yielded tensor is overwritten when two more batches have gone through this model."""
@@ -420,6 +435,8 @@ class SSDModel(KerasTrainingMixin):
         slots = self._pin_slots                         # pinned result buffers, rotated
 
         def upload(hb):
+            if torch.is_tensor(hb) and hb.is_cuda:
+                return self._device_batch(hb), None, None
             if not torch.is_tensor(hb):
                 hb = torch.from_numpy(np.ascontiguousarray(hb, dtype=np.float32))
             if not hb.is_pinned():
@@ -443,8 +460,9 @@ class SSDModel(KerasTrainingMixin):
             for hb in it:                               # issue the NEXT upload before this batch's kernels
                 nxt = upload(hb)
                 break
-            main.wait_event(ev)
-            x.record_stream(main)
+            if ev is not None:
+                main.wait_event(ev)
+                x.record_stream(main)
             out = self.predict_device(x)
             if post is not None:
                 out = post(out)
@@ -467,8 +485,8 @@ class SSDModel(KerasTrainingMixin):
 
     def predict_generator(self, generator, steps=None):
         """Keras' ``Model.predict_generator``: pulls ``steps`` batches (all of them if None) from ``generator`` -- each an image
-        batch or a tuple whose first element is one -- and returns the concatenated predictions as one ndarray.  The batches are
-        pipelined through :meth:`predict_stream`."""
+        batch or a tuple or list whose first element is one, as ``DataGenerator.generate`` yields them -- and returns the
+        concatenated predictions as one ndarray.  The batches are pipelined through :meth:`predict_stream`."""
         import itertools
 
         def images():
@@ -481,11 +499,21 @@ class SSDModel(KerasTrainingMixin):
         return np.concatenate(outs, axis=0)
 
     def predict(self, x, batch_size=None):
-        """Keras-style: ndarray (N,H,W,3) -> ndarray ((N,P,C+12) in 'training' mode, (N,top_k,6) otherwise)."""
-        x = np.asarray(x, dtype=np.float32)
+        """Keras-style: ndarray (N,H,W,3) -> ndarray ((N,P,C+12) in 'training' mode, (N,top_k,6) otherwise).  ``x`` may also be a
+        float32 CUDA tensor, such as a batch of ``DataGenerator.generate``: it is sliced on the device, and the result is the
+        one its host copy gives."""
+        import torch
+        if torch.is_tensor(x) and x.is_cuda:
+            x = self._device_batch(x)
+        else:
+            x = np.asarray(x, dtype=np.float32)
         bs = batch_size or x.shape[0]
         outs = [r.numpy().copy() for r in self.predict_stream(x[i:i + bs] for i in range(0, x.shape[0], bs))]
         return np.concatenate(outs, axis=0)
+
+    def predict_on_batch(self, x):
+        """Keras' ``predict_on_batch``: the predictions of one batch, host or CUDA, as ``predict`` returns them."""
+        return self.predict(x)
 
     def read_layer(self, name, batch):
         """Activation of a layer after the last forward with this batch size, float32 ndarray (B,h,w,c)."""

@@ -2,7 +2,13 @@
 ``ssd7_training.ipynb:153-156, 330-340``): ``compile(optimizer, loss)``, ``train_on_batch``, ``test_on_batch``,
 ``fit_generator(generator, steps_per_epoch, epochs, callbacks, validation_data, validation_steps, initial_epoch)`` and
 ``evaluate_generator`` -- thin host code over ``SSDTrainer`` (encode-free: the generator yields ``(images, y_encoded)`` exactly as
-the reference's ``DataGenerator.generate(..., label_encoder=SSDInputEncoder, returns={'processed_images', 'encoded_labels'})``)."""
+the reference's ``DataGenerator.generate(..., label_encoder=SSDInputEncoder, returns={'processed_images', 'encoded_labels'})``).
+
+A step is two halves: enqueueing its device work (``_enqueue_train_step`` / ``_enqueue_test_step``, which return the per-image
+loss tensor without waiting) and reading the mean loss as a float (``_read_loss``, which waits for the step).
+``train_on_batch`` / ``test_on_batch`` run them back to back.  ``fit_generator`` and ``evaluate_generator`` pull the next batch
+from the generator between the two, so that the host work of batch i+1 (the shuffle, the augmentation draws, decoding and
+packing) runs while the device computes step i, as Keras' generator queue lets it."""
 import numpy as np
 
 
@@ -11,6 +17,15 @@ class History:
 
     def __init__(self):
         self.epoch, self.history = [], {}
+
+
+def _pull(it):
+    """The next ``(x, y)`` of a generator, or the exception pulling it raised: a loop that pulls a batch ahead raises it where a
+    serial loop would have pulled that batch, after the steps and callbacks before it."""
+    try:
+        return next(it)[:2]
+    except Exception as e:                               # noqa: BLE001 -- re-raised by the step that needs the batch
+        return e
 
 
 def _call(callbacks, name, *args):
@@ -146,29 +161,61 @@ class KerasTrainingMixin:
             return a.to(device='cuda', dtype=torch.float32).contiguous()
         return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).cuda()
 
-    def train_on_batch(self, x, y):
-        """One optimizer step on ``(x, y)``; returns the scalar Keras reports: the mean over the batch of ``compute_loss``."""
+    def _enqueue_train_step(self, x, y):
+        """Enqueues forward, loss, backward and update of one optimizer step on ``(x, y)`` on the current stream; returns the
+        per-image loss, a CUDA tensor (B,), without waiting for the device."""
         if self._compiled is None:
             raise RuntimeError('You must compile a model before training/testing. Use `model.compile(optimizer, loss)`.')
         xd, yd = self._to_cuda(x), self._to_cuda(y)
-        loss = self._trainer_for(int(xd.shape[0])).train_on_batch(xd, yd)
-        return float(loss.mean().item())
+        return self._trainer_for(int(xd.shape[0])).train_on_batch(xd, yd)
 
-    def test_on_batch(self, x, y):
-        """The same scalar without an update, in the inference phase (moving BatchNormalization statistics), like Keras."""
+    def _enqueue_test_step(self, x, y):
+        """Enqueues the inference-phase forward and loss of ``(x, y)``; returns the per-image loss tensor (B,) without waiting."""
         if self._compiled is None:
             raise RuntimeError('You must compile a model before training/testing. Use `model.compile(optimizer, loss)`.')
         xd, yd = self._to_cuda(x), self._to_cuda(y)
         if self.decoder is not None:
             raise ValueError("test_on_batch needs the raw predictions: build the model with mode='training'")
-        return float(self._compiled[1].compute_loss(yd, self.forward_device(xd)).mean().item())
+        return self._compiled[1].compute_loss(yd, self.forward_device(xd))
+
+    @staticmethod
+    def _read_loss(loss):
+        """The scalar Keras reports for a step: the mean over the batch of its per-image loss, as a float (waits for the step)."""
+        return float(loss.mean().item())
+
+    def train_on_batch(self, x, y):
+        """One optimizer step on ``(x, y)``; returns the scalar Keras reports: the mean over the batch of ``compute_loss``."""
+        return self._read_loss(self._enqueue_train_step(x, y))
+
+    def test_on_batch(self, x, y):
+        """The same scalar without an update, in the inference phase (moving BatchNormalization statistics), like Keras."""
+        return self._read_loss(self._enqueue_test_step(x, y))
+
+    def _split_step(self, public, enqueue):
+        """``(enqueue, read)`` for the steps of the generator loops.  A ``train_on_batch`` / ``test_on_batch`` that a subclass or
+        the caller has replaced is what Keras' loops call, so it is called whole in the enqueue's place and its float read as
+        it is."""
+        fn = getattr(self, public)
+        if getattr(fn, '__func__', None) is getattr(KerasTrainingMixin, public):
+            return enqueue, self._read_loss
+        return fn, float
 
     def evaluate_generator(self, generator, steps):
+        """Keras' ``evaluate_generator``: the mean over the images of ``steps`` batches of ``test_on_batch``'s loss.  The next
+        batch is pulled from ``generator`` while the device computes the loss of the current one."""
+        enqueue, read = self._split_step('test_on_batch', self._enqueue_test_step)
         it = iter(generator)
+        steps = int(steps)
         tot, n = 0.0, 0
-        for _ in range(int(steps)):
-            x, y = next(it)[:2]
-            tot += self.test_on_batch(x, y) * len(x)
+        batch = next(it)[:2] if steps > 0 else None
+        for step in range(steps):
+            if isinstance(batch, Exception):
+                raise batch
+            x, y = batch
+            pending = enqueue(x, y)
+            if step + 1 < steps:
+                batch = _pull(it)
+            tot += read(pending) * len(x)
             n += len(x)
         return tot / max(n, 1)
 
@@ -177,19 +224,36 @@ class KerasTrainingMixin:
         """Keras' loop: ``epochs - initial_epoch`` epochs of ``steps_per_epoch`` batches from ``generator`` (an endless iterator of
         ``(images, y_encoded)``), the epoch's mean loss in ``history['loss']``, the validation loss in ``history['val_loss']``.
         Callbacks are duck-typed: ``set_model``, ``on_train_begin/end(logs)``, ``on_epoch_begin/end(epoch, logs)``,
-        ``on_batch_end(batch, logs)`` are called where present; a callback may set ``model.optimizer.lr`` or ``model.stop_training``."""
+        ``on_batch_end(batch, logs)`` are called where present; a callback may set ``model.optimizer.lr`` or ``model.stop_training``.
+
+        Each step but the last of an epoch runs as: enqueue step i on the device, pull batch i+1 from ``generator``, read the
+        loss of step i, call ``on_batch_end(i)``.  The host therefore plans and assembles batch i+1 while the device trains on
+        batch i; the learning rate a callback sets in ``on_batch_end(i)`` is the one step i+1 uses, as in a serial loop.  The
+        last step of an epoch pulls nothing ahead, so validation and the next epoch find ``generator`` where a serial loop
+        leaves it (the training and validation generators may be one object).  Every step trains on the batch, with the
+        learning rate, that a serial ``train_on_batch`` loop gives it, and the callbacks and history see what they see
+        there, with one difference: when a callback stops training in the middle of an epoch, the batch after the last one
+        trained has already been pulled and is not trained on (Keras' queue does the same)."""
         callbacks = list(callbacks or [])
         hist = History()
         _call(callbacks, 'set_model', self)
         self.stop_training = False
         _call(callbacks, 'on_train_begin', {})
+        enqueue, read = self._split_step('train_on_batch', self._enqueue_train_step)
         it = iter(generator)
+        steps = int(steps_per_epoch)
         for epoch in range(int(initial_epoch), int(epochs)):
             _call(callbacks, 'on_epoch_begin', epoch, {})
             tot, n = 0.0, 0
-            for step in range(int(steps_per_epoch)):
-                x, y = next(it)[:2]
-                l = self.train_on_batch(x, y)
+            batch = next(it)[:2] if steps > 0 else None
+            for step in range(steps):
+                if isinstance(batch, Exception):
+                    raise batch
+                x, y = batch
+                pending = enqueue(x, y)
+                if step + 1 < steps:
+                    batch = _pull(it)
+                l = read(pending)
                 tot += l * len(x)
                 n += len(x)
                 _call(callbacks, 'on_batch_end', step, {'loss': l, 'size': len(x)})
