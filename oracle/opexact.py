@@ -165,7 +165,7 @@ def _tap64(x, w, t, stride, dil, pads, c0=0, c1=None):
     Ho = (xp.shape[1] - dil * (KH - 1) - 1) // stride + 1
     Wo = (xp.shape[2] - dil * (KW - 1) - 1) // stride + 1
     win = xp[:, kh * dil:kh * dil + stride * (Ho - 1) + 1:stride, kw * dil:kw * dil + stride * (Wo - 1) + 1:stride, c0:c1]
-    return np.einsum('bhwc,co->bhwo', win, np.asarray(w[kh, kw, c0:c1], np.float64))
+    return np.einsum('bhwc,co->bhwo', win, np.asarray(w[kh, kw, c0:c1], np.float64), optimize=True)    # a BLAS product
 
 
 def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3', act=None, bn_scale=None, bn_shift=None,
@@ -178,7 +178,8 @@ def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3',
     perturb: perturbations for the sensitivity checks, each a tuple -- ('cross',) drops hi*lo; ('tap', t) drops tap t;
     ('taps', t0, t1) drops taps [t0, t1) (one 64-column K block of conv_first_kernel: 16 taps x 4 channels);
     ('kblock', t, kb) drops input channels [64 kb, 64 kb + 64) of tap t; ('kcols', k0, k1) drops the columns [k0, k1) of an
-    im2col row (k = tap * cin + c); ('bias', o) drops output channel o's bias.
+    im2col row (k = tap * cin + c); ('bias', o) drops output channel o's bias; ('bias_live',) drops the largest |bias| of the
+    output channels the activation does not zero everywhere (a ReLU channel that is zero on every pixel hides its bias).
     A perturbed reference differs from y_ref by the dropped products only; it is judged with the unperturbed bound."""
     geo = dict(stride=stride, dil=dil, pads=pads)
     if mode == 'fp32':
@@ -214,10 +215,15 @@ def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3',
     A = A + np.abs(b)
     if bn_scale is not None:
         A = A * np.abs(np.asarray(bn_scale, np.float64)) + np.abs(np.asarray(bn_shift, np.float64))
+    y = epilogue(z, b)
     out = {}
     for p in perturb:
         bp, dz = b, 0.0
-        if p[0] == 'cross':
+        if p[0] == 'bias_live':
+            live = np.any(y != 0, axis=tuple(range(y.ndim - 1)))
+            bp = b.copy()
+            bp[int(np.argmax(np.abs(b) * live))] = 0.0
+        elif p[0] == 'cross':
             dz = conv64(terms[1][0], terms[1][1], **geo)
         elif p[0] == 'tap':
             dz = sum(_tap64(a, k, p[1], **geo) for a, k in terms)
@@ -233,7 +239,7 @@ def conv_ref(x, w, bias=None, stride=1, dil=1, pads=(0, 0, 0, 0), mode='bf16x3',
             bp = b.copy()
             bp[p[1]] = 0.0
         out[p] = epilogue(z - dz, bp)
-    return epilogue(z, b), A, out
+    return y, A, out
 
 
 def bound(y_ref, A, n_steps, store):
@@ -759,7 +765,7 @@ def bn_fwd_ref(z, gamma, beta, mmean, mvar, act=None, eps=1e-3, momentum=0.99, z
 def l2norm_fwd_ref(x, gamma, perturb=()):
     """L2Normalization forward (l2norm_kernel, l2norm8_kernel) -> (y_ref, kappa * |y_ref|, {perturbation: y'}), float64; add
     unit |y_ref| of the store (section 9).  x: the layer's input as stored (hi + lo).  perturb: ('no_gamma',);
-    ('gamma_shift',) channel c takes gamma[c + 1]."""
+    ('gamma_shift',) channel c takes gamma[c + 1]; ('gamma_at', c) only channel c takes gamma[c + 1]."""
     x = _f64(x)
     gm = _f64(gamma)
     Cc = x.shape[-1]
@@ -771,6 +777,10 @@ def l2norm_fwd_ref(x, gamma, perturb=()):
             out[p] = x * s
         elif p == ('gamma_shift',):
             out[p] = x * s * np.roll(gm, -1)
+        elif p[0] == 'gamma_at':
+            g2 = gm.copy()
+            g2[p[1]] = gm[(p[1] + 1) % Cc]
+            out[p] = x * s * g2
     return y, ((Cc + 1) / 2.0 + 8) * U32 * np.abs(y), out
 
 

@@ -98,6 +98,9 @@ HEAD_CASES = [
     # unfused: fp32 logits, then head_finalize_kernel
     head_case('unfused_no_head_fusion', 2, 10, 9, 64, 4, 21, HF(128, 1, fused=0), env={'SSDK_NO_HEAD_FUSION': '1'}),
     head_case('unfused_8boxes_bf16x3', 2, 6, 7, 136, 8, 21, HF(128, 1, fused=0, n_tiles_n=2)),
+    # SSD512's COCO heads: 4 boxes x 85 columns span several n-tiles; head_finalize_kernel makes three lane passes per row
+    head_case('unfused_81classes_4boxes_bf16x3', 2, 6, 7, 64, 4, 81, HF(128, 1, fused=0, n_tiles_n=3)),
+    head_case('unfused_81classes_4boxes_bf16', 2, 6, 7, 64, 4, 81, HF(256, 0, fused=0, n_tiles_n=2), prec='bf16'),
 ]
 
 
@@ -355,11 +358,16 @@ def case_data(case, seed):
 
 
 def n_steps_of(plan, taps, cin):
-    if plan['kernel'] in ('gemm', 'im2col_gemm'):
-        return opexact.n_steps_gemm(taps if plan['kernel'] == 'gemm' else 1, plan['kblocks'])
+    """The k-steps on one accumulator of the forward kernel a plan names (oracle/opexact.py, section 1)."""
+    if plan['kernel'] in ('gemm', 'gemm_swap'):
+        return opexact.n_steps_gemm(taps, plan['kblocks'])
+    if plan['kernel'] == 'im2col_gemm':
+        return opexact.n_steps_gemm(1, plan['kblocks'])
     if plan['kernel'] == 'first_tc':
         return opexact.n_steps_first(plan['kblocks'], plan['split'])
-    return opexact.n_steps_direct(taps, cin)
+    if plan['kernel'] == 'direct':
+        return opexact.n_steps_direct(taps, cin)
+    raise ValueError('no k-step count for the forward kernel %r' % (plan['kernel'],))
 
 
 def perturbations(plan, taps, cin, split_products, bias):

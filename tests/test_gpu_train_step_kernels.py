@@ -67,8 +67,11 @@ POOL_CASES = [
 ]
 
 # L2Normalization: l2norm8_kernel needs C % 8 == 0, C <= 512 and no padding channels; the other two take l2norm_kernel
+# l2norm8_kernel holds channels (k * 32 + lane) * 8 ... + 7 in register half k: C = 512 fills both halves (conv4_3_norm), C = 264
+# puts only lane 0 in the second half
 L2_CASES = [dict(name='l2norm8_c32', C=32, kernel='l2norm8'), dict(name='l2norm_c20_padded', C=20, kernel='l2norm'),
-            dict(name='l2norm_c520_wide', C=520, kernel='l2norm')]
+            dict(name='l2norm_c520_wide', C=520, kernel='l2norm'), dict(name='l2norm8_c512_both_halves', C=512, kernel='l2norm8'),
+            dict(name='l2norm8_c264_second_half_lane0', C=264, kernel='l2norm8')]
 
 PRE_CASES = [dict(name='mean_only', mean=(123.0, 117.0, 104.0), stddev=None, swap=None),
              dict(name='mean_std', mean=(127.5, 110.25, 99.0), stddev=(127.5, 63.0, 58.395), swap=None),
@@ -411,7 +414,9 @@ def test_l2norm_forward_within_bound(case, prec):
         out = g.planes(1)
         assert l2norm_kernel_of(Cc, g.planes(0)[0].shape[-1]) == case['kernel'] and out[0].shape[-1] == g.planes(0)[0].shape[-1]
         got = tb._fval(out, dict(H=H, W=W, C=Cc))
-        ref, err, pv = opexact.l2norm_fwd_ref(xv, gamma, perturb=[('no_gamma',), ('gamma_shift',)])
+        # a gamma taken from the next channel at the first and the last channel of the second register half
+        perts = [('no_gamma',), ('gamma_shift',)] + [('gamma_at', c) for c in (256, Cc - 1) if Cc > 256]
+        ref, err, pv = opexact.l2norm_fwd_ref(xv, gamma, perturb=perts)
         store = 'split' if prec == 'bf16x3' else 'bf16'
         bnd = np.maximum(err + opexact.UNIT[store] * np.abs(ref), np.finfo(np.float64).tiny)
         _judge(dict(test='l2norm_forward', case=case['name'], prec=prec, kernel=case['kernel']), opexact.err_ratio(got, ref, bnd),

@@ -119,6 +119,22 @@ def test_perturbed_references_equal_recomputed_ones():
     assert np.allclose(pert[('bias', 3)], want, rtol=1e-12, atol=1e-12)
 
 
+def test_live_bias_perturbation_skips_channels_the_relu_zeroes():
+    """('bias_live',) drops the largest |bias| among the channels with a non-zero output: a ReLU channel that is zero on every
+    pixel would hide a dropped bias from any comparison."""
+    rng = np.random.default_rng(4)
+    x = rng.standard_normal((1, 5, 5, 16)).astype(np.float32)
+    w = (rng.standard_normal((3, 3, 16, 8)) * 0.1).astype(np.float32)
+    w[..., 3] = 0.0
+    b = np.array([0.3, -0.2, 0.1, -50.0, 0.05, 0.0, 0.2, -0.1], np.float32)      # channel 3 is zero with or without its bias
+    geo = dict(pads=(1, 1, 1, 1), act='relu')
+    y, _, pert = opexact.conv_ref(x, w, b, perturb=[('bias_live',), ('bias', 3)], **geo)
+    assert not np.any(y[..., 3]) and np.array_equal(pert[('bias', 3)], y)
+    b2 = b.copy()
+    b2[0] = 0
+    assert np.array_equal(pert[('bias_live',)], opexact.conv_ref(x, w, b2, **geo)[0])
+
+
 def test_softmax_bound_accepts_fp32_softmax_and_rejects_a_shifted_logit():
     rng = np.random.default_rng(5)
     z = rng.standard_normal((3, 50, 21)) * 4
@@ -172,6 +188,8 @@ def test_head_case_table_reaches_every_variant():
     unfused = [(c, e) for c, e in hv if not e['head_fused']]
     assert any(c['env'].get('SSDK_NO_HEAD_FUSION') == '1' for c, e in unfused)
     assert any(c['nb'] * (c['C'] + 4) == 200 and c['prec'] == 'bf16x3' and not c['env'] for c, e in unfused)
+    # head_finalize_kernel with more than 64 classes (three lane passes per row), 4 boxes x 85 columns, both precisions
+    assert {c['prec'] for c, e in unfused if c['C'] > 64 and c['nb'] * (c['C'] + 4) == 340} == {'bf16x3', 'bf16'}
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -589,14 +607,14 @@ def test_bn_forward_reference_emulation_and_perturbations(act):
         mm, mv, z_prev = gst['mean'], gst['var'], z
 
 
-@pytest.mark.parametrize('Cc', [32, 20, 520])
+@pytest.mark.parametrize('Cc', [32, 20, 520, 264, 512])
 def test_l2norm_forward_reference_emulation_and_perturbations(Cc):
     rng = np.random.default_rng(Cc)
     x = rng.standard_normal((2, 3, 4, Cc)).astype(np.float32)
     x[0, 1, 1] = 0
     x[1, 2, 3] = (rng.standard_normal(Cc) * 1e-8).astype(np.float32)
     gamma = rng.uniform(0.5, 20, Cc).astype(np.float32)
-    ref, err, pv = opexact.l2norm_fwd_ref(x, gamma, perturb=[('no_gamma',), ('gamma_shift',)])
+    ref, err, pv = opexact.l2norm_fwd_ref(x, gamma, perturb=[('no_gamma',), ('gamma_shift',)] + [('gamma_at', c) for c in (256, Cc - 1) if Cc > 256])
     xt = torch.from_numpy(x.astype(np.float64))
     want = xt * torch.rsqrt(torch.clamp((xt * xt).sum(-1, keepdim=True), min=float(np.float32(1e-12)))) * torch.from_numpy(gamma.astype(np.float64))
     np.testing.assert_allclose(ref, want.numpy(), rtol=1e-12, atol=0)
@@ -677,6 +695,9 @@ def test_train_step_case_tables_reach_every_variant():
     assert any(c['H'] == 75 and c['pads'] == (0, 0, 1, 1) for c in ts.POOL_CASES)
     ks = {ts.l2norm_kernel_of(c['C'], -(-c['C'] // 8) * 8): c['C'] for c in ts.L2_CASES}
     assert set(ks) == {'l2norm8', 'l2norm'} and {20, 520} <= {c['C'] for c in ts.L2_CASES}
+    # l2norm8_kernel's second register half: full (C = 512) and lane 0 alone (C = 264)
+    l2n8 = {c['C'] for c in ts.L2_CASES if ts.l2norm_kernel_of(c['C'], -(-c['C'] // 8) * 8) == 'l2norm8'}
+    assert {264, 512} <= l2n8 and all(c['kernel'] == ts.l2norm_kernel_of(c['C'], -(-c['C'] // 8) * 8) for c in ts.L2_CASES)
     # BatchNormalization: ELU / ReLU / none, C = 24 and 136, both precisions, both branches of bn_grid
     bn = [(c, x) for c in ts.BN_CASES for x in c['layers'] if x['bn']]
     assert {x['act'] for _, x in bn} == {'elu', 'relu', None} and {24, 136} <= {x['cout'] for _, x in bn}
