@@ -442,6 +442,28 @@ int ssdk_ssd_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true_dev, const
                         const int* ties_all_dev /* [world], phase 4 */, int rank, const float* upstream_dev,
                         float* out_loss_dev, int* out_stats_dev, float* out_grad_dev, void* stream);
 
+/* Softmax focal loss (Lin et al., arXiv:1708.02002) on SSDLoss's layout: y_true / y_pred (B,P,C+12) float32, columns [0, C) the
+ * class values (y_pred: the heads' softmax probabilities), [C, C+4) the offsets, the last 8 without loss.  Per box
+ *   cls = sum_c y_true[c] w_c (1 - q_c)^gamma (-log max(q_c, 1e-15)),  w_0 = 1 - focal_alpha, w_c = focal_alpha (c >= 1),
+ *   pos = max_{c=1..C-1} y_true[c],  loc = SSDLoss's smooth-L1 of the offsets;
+ * per image L_b = global_B (sum_p cls + alpha sum_p loc pos) / max(1, N), N = sum of pos over the whole (global) batch.
+ * out_loss_dev [B] float32 (optional); out_grad_dev [B*P*(C+12)] (optional, not both NULL): d(sum_b u_b L_b) / d y_pred, u_b =
+ * upstream_dev[b] or 1/global_B when upstream_dev is NULL (the Keras batch mean); the clamp passes no gradient below 1e-15,
+ * gamma (1-q)^(gamma-1) log q is taken as 0 at q = 1 (its limit), the last 8 columns get 0.  gamma < 0 and focal_alpha outside
+ * [0, 1] are refused (SSDK_ERR_INVALID) before any launch.  Reductions run in a fixed order (no float atomics): the result is
+ * bit-reproducible.  csrc/focal_loss.cu.
+ *   ssdk_focal_loss        single process: both phases (global_B = B).
+ *   ssdk_focal_loss_phase  a batch sharded over ranks.  count_dev: one int64, N in 32.32 fixed point (the sum over the rows of
+ *                          llrint(pos * 2^32)).  Zero it; phase 0 adds this rank's rows; all-reduce (sum) it over the ranks;
+ *                          phase 1 writes this rank's losses and / or gradient rows, normalised by the global N and global_B.
+ *                          The per-image losses and gradient rows are bit-identical to one ssdk_focal_loss on the whole batch. */
+int ssdk_focal_loss(ssdk_ctx* ctx, const float* y_true_dev, const float* y_pred_dev, int B, int P, int n_classes_total,
+                    float gamma, float focal_alpha, float alpha, const float* upstream_dev, float* out_loss_dev,
+                    float* out_grad_dev, void* stream);
+int ssdk_focal_loss_phase(ssdk_ctx* ctx, int phase, const float* y_true_dev, const float* y_pred_dev, int B, int P,
+                          int n_classes_total, float gamma, float focal_alpha, float alpha, long long* count_dev, int global_B,
+                          const float* upstream_dev, float* out_loss_dev, float* out_grad_dev, void* stream);
+
 /* Read-only views of the loss kernel, for tests and diagnostics.
  *   ssdk_ssd_loss_plan  the launch a call with these arguments would make (want_grad: ssdk_ssd_loss with out_grad_dev, or
  *                       phase 4 with a gradient; cooperative: ssdk_ssd_loss, 0 = ssdk_ssd_loss_phase), or the error that

@@ -20,6 +20,7 @@ def _exports():
     from .keras_layers.keras_layer_DecodeDetections import DecodeDetections
     from .keras_layers.keras_layer_DecodeDetectionsFast import DecodeDetectionsFast
     from .keras_loss_function.keras_ssd_loss import SSDLoss
+    from .keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
     from .ssd_encoder_decoder.ssd_input_encoder import SSDInputEncoder, DegenerateBoxError
     from .ssd_encoder_decoder.ssd_output_decoder import decode_detections, decode_detections_fast
     from .bounding_box_utils.bounding_box_utils import iou, convert_coordinates, intersection_area
@@ -29,7 +30,7 @@ def _exports():
 
 
 _NAMES = ('ssd_300', 'ssd_512', 'build_model', 'ssd_7', 'AnchorBoxes', 'L2Normalization', 'DecodeDetections',
-          'DecodeDetectionsFast', 'SSDLoss', 'SSDInputEncoder', 'DegenerateBoxError', 'decode_detections',
+          'DecodeDetectionsFast', 'SSDLoss', 'SSDFocalLoss', 'SSDInputEncoder', 'DegenerateBoxError', 'decode_detections',
           'decode_detections_fast', 'iou', 'convert_coordinates', 'intersection_area', 'match_bipartite_greedy', 'match_multi',
           'SSDTrainer')
 

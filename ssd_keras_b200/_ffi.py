@@ -186,6 +186,8 @@ SIGNATURES = {
     'ssdk_ssd_loss': (_i, [_p, _p, _p, _i, _i, _i, _i, _i, _f, _p, _p, _p, _p, _p]),
     'ssdk_ssd_loss_ws_layout': (_i, [_i, _i, C.POINTER(LossWsLayout)]),
     'ssdk_ssd_loss_phase': (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _f, _p, _i, _p, _i, _p, _p, _p, _p, _p]),
+    'ssdk_focal_loss': (_i, [_p, _p, _p, _i, _i, _i, _f, _f, _f, _p, _p, _p, _p]),
+    'ssdk_focal_loss_phase': (_i, [_p, _i, _p, _p, _i, _i, _i, _f, _f, _f, _p, _i, _p, _p, _p, _p]),
     'ssdk_ssd_loss_plan': (_i, [_p, _p, _p, _i, _i, _i, _i, _i, C.POINTER(LossPlan)]),
     'ssdk_ssd_loss_read_box_losses': (_i, [_p, _p, _i, _i, _p, _p, _p]),
     'ssdk_l2_normalize': (_i, [_p, _p, _ll, _i, _p, _p, _p]),

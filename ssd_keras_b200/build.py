@@ -25,6 +25,7 @@ SOURCES = {
     'encode.cu': ['--fmad=false'],
     'decode.cu': ['--fmad=false'],
     'loss.cu': ['--fmad=false'],
+    'focal_loss.cu': ['--fmad=false'],
     'batch.cu': ['--fmad=false'],
     'evaluate.cu': ['--fmad=false'],
     'cocoeval.cu': ['--fmad=false'],

@@ -39,7 +39,7 @@ extern "C" int ssdk_ctx_create(int device, ssdk_ctx** out) {
 
 extern "C" int ssdk_ctx_destroy(ssdk_ctx* ctx) {
   if (!ctx) return SSDK_OK;
-  for (Scratch* w : {&ctx->decode_ws, &ctx->nms_ws, &ctx->loss_ws, &ctx->box_ws, &ctx->img_desc_ws, &ctx->photo_ws}) w->release();
+  for (Scratch* w : {&ctx->decode_ws, &ctx->nms_ws, &ctx->loss_ws, &ctx->focal_ws, &ctx->box_ws, &ctx->img_desc_ws, &ctx->photo_ws}) w->release();
   ctx->img_desc_ring.release();
   if (ctx->box_ws_done) cudaEventDestroy(ctx->box_ws_done);
   delete ctx;

@@ -107,6 +107,7 @@ struct ssdk_ctx {
   ssdk::Scratch loss_ws;        // the SSD loss
   long long loss_ws_shape = -1; // (B, P) the loss workspace is laid out for
   int loss_parity = 0;          // which of its two histogram sets the next loss call uses (the other one is being cleared)
+  ssdk::Scratch focal_ws;       // the focal loss: its count, ticket and tile partials
   ssdk::Scratch box_ws;         // ssdk_assemble_batch: transformed boxes and per-image counts
   cudaEvent_t box_ws_done = nullptr;  // recorded after the last ssdk_assemble_batch: box_ws is free once it has completed
   ssdk::Scratch img_desc_ws;    // ssdk_assemble_images: per-image and photometric descriptors

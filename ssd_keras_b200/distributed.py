@@ -177,3 +177,39 @@ def ssd_loss_global(y_true, y_pred, neg_pos_ratio=3, n_neg_min=0, alpha=1.0, gro
         run.ties_all.copy_(run.ties)
     run.phase(4)
     return (run.loss, run.grad, run.stats) if return_grad else run.loss
+
+
+def focal_loss_global(y_true, y_pred, gamma=2.0, focal_alpha=0.25, alpha=1.0, group=None, return_grad=False, grad_out=None):
+    """``SSDFocalLoss.compute_loss`` for a batch that is sharded over the ranks of ``group``: its normaliser, the number of
+    positives, runs over the WHOLE batch.  Every rank holds ``(B_local, P, C+12)`` shards (equal ``B_local``, rank order = image
+    order): ``ssdk_focal_loss_phase`` phase 0 counts this rank's positives into one int64 (32.32 fixed point), one all-reduce
+    sums it, phase 1 writes the losses and / or the gradient.  Returns the ``(B_local,)`` losses of this rank's images, bit for
+    bit the entries one process computes for them on the whole batch, and with ``return_grad`` ``(loss, d(mean over the global
+    batch)/d y_pred of this shard)``, written into ``grad_out`` when given.  Without an initialised process group this is the
+    single-rank result."""
+    import torch
+    import torch.distributed as dist
+    from . import _ffi
+    on = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
+    world = dist.get_world_size(group) if on else 1
+    yt = y_true.to(device='cuda', dtype=torch.float32).contiguous()
+    yp = y_pred.to(device='cuda', dtype=torch.float32).contiguous()
+    B, P, W = yp.shape
+    dev = yp.device
+    count = torch.zeros((1,), dtype=torch.int64, device=dev)
+    loss = torch.empty((B,), dtype=torch.float32, device=dev)
+    grad = None
+    if return_grad:
+        grad = torch.empty_like(yp) if grad_out is None else grad_out
+        assert grad.shape == yp.shape and grad.dtype == torch.float32 and grad.is_contiguous()
+    lib, ctx = _ffi.lib(), _ffi.context(dev.index)
+    cfg = (float(gamma), float(focal_alpha), float(alpha))
+
+    def phase(i):
+        _ffi.check(lib.ssdk_focal_loss_phase(ctx, i, _ffi.dptr(yt), _ffi.dptr(yp), B, P, W - 12, *cfg, _ffi.dptr(count), world * B,
+                                             _ffi.dptr(None), _ffi.dptr(loss), _ffi.dptr(grad), _ffi.stream_ptr()))
+    phase(0)
+    if on:
+        dist.all_reduce(count, group=group)
+    phase(1)
+    return (loss, grad) if return_grad else loss

@@ -49,8 +49,10 @@ class KerasTrainingMixin:
 
     def compile(self, optimizer, loss=None, **kwargs):
         """``optimizer``: ``ssd_keras_b200.optimizers.SGD`` / ``Adam`` (or any object with their attributes, or 'sgd' / 'adam');
-        ``loss``: ``SSDLoss(...).compute_loss`` (the bound method, as in the reference) or the ``SSDLoss`` object."""
+        ``loss``: ``SSDLoss(...).compute_loss`` (the bound method, as in the reference) or the ``SSDLoss`` object, or the same of
+        an ``SSDFocalLoss``."""
         from .. import optimizers
+        from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
         from ..keras_loss_function.keras_ssd_loss import SSDLoss
         if kwargs:
             raise TypeError('compile() got unsupported arguments: %s' % sorted(kwargs))
@@ -62,17 +64,19 @@ class KerasTrainingMixin:
         if kind not in ('sgd', 'adam') or not hasattr(optimizer, 'lr'):
             raise ValueError('unsupported optimizer %r: SGD (lr, momentum) and Adam (lr, beta_1, beta_2, epsilon) are implemented' % (optimizer,))
         owner = getattr(loss, '__self__', loss)
-        if not isinstance(owner, SSDLoss):
-            raise ValueError('loss must be SSDLoss(...).compute_loss (keras_loss_function/keras_ssd_loss.py:98): the training step '
-                             'computes that loss and its gradient on the device')
+        if not isinstance(owner, (SSDLoss, SSDFocalLoss)):
+            raise ValueError('loss must be SSDLoss(...).compute_loss (keras_loss_function/keras_ssd_loss.py:98) or '
+                             'SSDFocalLoss(...).compute_loss: the training step computes that loss and its gradient on the device')
         self.optimizer, self._compiled = optimizer, (kind, owner)
         self._fit_trainer = None
         self._pending_opt_state = None
 
     # -- the training half of a full-model file (Keras' training_config and /optimizer_weights) --------------------------------
     def _training_config(self):
-        """Keras' ``training_config`` root attribute of ``model.save``, with the ``SSDLoss`` parameters load_model rebuilds the
-        loss from when ``custom_objects`` does not bring it."""
+        """Keras' ``training_config`` root attribute of ``model.save``, with the ``SSDLoss`` parameters (``'ssd_loss'``) or the
+        ``SSDFocalLoss`` parameters (``'ssd_focal_loss'``) load_model rebuilds the loss from when ``custom_objects`` does not bring
+        it."""
+        from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
         kind, lossobj = self._compiled
         o = self.optimizer
         if kind == 'sgd':
@@ -82,8 +86,12 @@ class KerasTrainingMixin:
             opt = {'class_name': 'Adam', 'config': {'lr': float(o.lr), 'beta_1': float(getattr(o, 'beta_1', 0.9)),
                                                     'beta_2': float(getattr(o, 'beta_2', 0.999)), 'decay': 0.0,
                                                     'epsilon': float(getattr(o, 'epsilon', 1e-8)), 'amsgrad': False}}
-        return {'optimizer_config': opt, 'loss': 'compute_loss', 'metrics': [], 'sample_weight_mode': None, 'loss_weights': None,
-                'ssd_loss': {'neg_pos_ratio': lossobj.neg_pos_ratio, 'n_neg_min': lossobj.n_neg_min, 'alpha': lossobj.alpha}}
+        out = {'optimizer_config': opt, 'loss': 'compute_loss', 'metrics': [], 'sample_weight_mode': None, 'loss_weights': None}
+        if isinstance(lossobj, SSDFocalLoss):
+            out['ssd_focal_loss'] = lossobj.config()
+        else:
+            out['ssd_loss'] = {'neg_pos_ratio': lossobj.neg_pos_ratio, 'n_neg_min': lossobj.n_neg_min, 'alpha': lossobj.alpha}
+        return out
 
     def _optimizer_weights(self):
         """``[(name, array), ...]`` for ``/optimizer_weights`` in Keras' order -- ``iterations:0``, then each slot in the trainer's
@@ -102,6 +110,7 @@ class KerasTrainingMixin:
         """``load_model``'s ``compile=True``: compile with the stored optimizer and learning rate, and keep the stored optimizer
         state (checked against this model) for the trainer of the next step."""
         from .. import optimizers
+        from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
         from ..keras_loss_function.keras_ssd_loss import SSDLoss
         from ..training import check_optimizer_state
         oc = config['optimizer_config']
@@ -113,8 +122,11 @@ class KerasTrainingMixin:
         else:
             raise ValueError('training_config names the optimizer %r: SGD and Adam are implemented' % (oc['class_name'],))
         loss = (custom_objects or {}).get('compute_loss')
-        if not isinstance(getattr(loss, '__self__', None), SSDLoss):
-            loss = SSDLoss(**config['ssd_loss']).compute_loss
+        if not isinstance(getattr(loss, '__self__', None), (SSDLoss, SSDFocalLoss)):
+            if 'ssd_focal_loss' in config:
+                loss = SSDFocalLoss(**config['ssd_focal_loss']).compute_loss
+            else:
+                loss = SSDLoss(**config['ssd_loss']).compute_loss
         self.compile(optimizer=opt, loss=loss)
         if not opt_weights:
             return
@@ -144,9 +156,8 @@ class KerasTrainingMixin:
                 raise ValueError('this model has been training on batches of %d images; a batch of %d would need its own optimizer '
                                  'state (the reference generator yields constant-size batches)' % (t.batch, batch))
             o = self.optimizer
-            t = SSDTrainer(self, batch, lr=o.lr, momentum=getattr(o, 'momentum', 0.0), neg_pos_ratio=lossobj.neg_pos_ratio,
-                           n_neg_min=lossobj.n_neg_min, alpha=lossobj.alpha, optimizer=kind, beta_1=getattr(o, 'beta_1', 0.9),
-                           beta_2=getattr(o, 'beta_2', 0.999), epsilon=getattr(o, 'epsilon', 1e-8))
+            t = SSDTrainer(self, batch, lr=o.lr, momentum=getattr(o, 'momentum', 0.0), optimizer=kind, beta_1=getattr(o, 'beta_1', 0.9),
+                           beta_2=getattr(o, 'beta_2', 0.999), epsilon=getattr(o, 'epsilon', 1e-8), loss=lossobj)
             if self._pending_opt_state is not None:
                 t.set_optimizer_state(self._pending_opt_state)
                 self._pending_opt_state = None
