@@ -619,8 +619,9 @@ int ssdk_model_layer_plan(const ssdk_model* m, int layer, ssdk_layer_plan* out);
  * Training step (BASELINE config 3).  Replaces what Keras/TensorFlow do for the reference in model.fit_generator:
  * autodiff of the graph (models/keras_ssd300.py:263-419) and of SSDLoss (keras_ssd_loss.py:98-211), the kernel_regularizer
  * l2(l2_reg) (models/keras_ssd300.py:274), SGD(lr, momentum) (ssd300_training.ipynb:169) and Adam (ssd7_training.ipynb:153).
- *   ssdk_train_backward_begin / _layers  after ssdk_model_forward on the same images: loss + gradients of every kernel /
- *                        bias / gamma into one flat float32 buffer (so that a single NCCL all-reduce covers it).
+ *   ssdk_train_backward_layers  after ssdk_model_forward on the same images, from the d loss / d y_pred a loss entry point
+ *                        (ssdk_ssd_loss, ssdk_focal_loss or their phases) wrote: gradients of every kernel / bias / gamma into
+ *                        one flat float32 buffer (so that a single NCCL all-reduce covers it).
  *   ssdk_train_apply     g = grad*grad_scale + 2*l2*w (kernels only); v = momentum*v - lr*g; w += v; re-pack the bf16 planes.
  * Parameter order in the flat buffer: layers in graph order, for each conv [kernel as (cout, kh, kw, cin) | bias | BatchNorm
  * gamma | BatchNorm beta], for each head [fused kernel (n_boxes*(C+4), 3, 3, cin) | fused bias], for L2Normalization [gamma].
@@ -642,18 +643,11 @@ int ssdk_trainer_param_span(const ssdk_trainer* t, int layer, int which, long lo
 int ssdk_trainer_grad_shape(const ssdk_trainer* t, int layer, int* out_hp, int* out_wp, int* out_cs, int* out_pad);
 int ssdk_trainer_read_grad(ssdk_trainer* t, int layer, float* out_dev, void* stream);
 int ssdk_trainer_read_grad_planes(ssdk_trainer* t, int layer, uint16_t* hi_dev, uint16_t* lo_dev, void* stream);
-/* The backward pass in pieces, so that the gradient exchange can overlap it:
- *   ssdk_train_backward_begin   loss (out_loss_dev [B], optional) + d loss / d y_pred (kept inside the trainer), gradient
- *                               buffer cleared;
- *   ssdk_train_backward_layers  layers hi .. lo (graph indices, top down, consecutive calls cover n_layers-1 .. 0).  In stream
- *                               order after the call the parameter gradients of exactly these layers are final, so their
- *                               span of the flat buffer (ssdk_trainer_param_span) can be all-reduced on another stream while the
- *                               lower layers are still being differentiated.  dypred_dev NULL = the trainer's own; otherwise
- *                               d loss / d y_pred, (B,P,C+12) float32, that the caller computed (the multi-GPU
- *                               global-batch-exact loss, whose phases run between NCCL collectives, see ssdk_ssd_loss_phase),
- *                               and a pass that starts at the top layer clears the gradient buffer first. */
-int ssdk_train_backward_begin(ssdk_trainer* t, const float* y_true_dev, const float* y_pred_dev, int neg_pos_ratio, int n_neg_min,
-                              float alpha, float* out_loss_dev, void* stream);
+/* The backward pass in pieces, so that the gradient exchange can overlap it: layers hi .. lo (graph indices, top down,
+ * consecutive calls cover n_layers-1 .. 0) from dypred_dev, d loss / d y_pred (B,P,C+12) float32, which the caller's loss
+ * wrote (required).  A pass that starts at the top layer clears the gradient buffer first.  In stream order after the call the
+ * parameter gradients of exactly these layers are final, so their span of the flat buffer (ssdk_trainer_param_span) can be
+ * all-reduced on another stream while the lower layers are still being differentiated. */
 int ssdk_train_backward_layers(ssdk_trainer* t, const float* dypred_dev, int hi, int lo, void* stream);
 int ssdk_train_apply(ssdk_trainer* t, float lr, float momentum, float l2_reg, float grad_scale, void* stream);
 /* Adam as Keras applies it (ssd7_training.ipynb:153: Adam(lr=0.001, beta_1=0.9, beta_2=0.999, epsilon=1e-08, decay=0.0)):

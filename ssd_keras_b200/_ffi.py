@@ -214,7 +214,6 @@ SIGNATURES = {
     'ssdk_trainer_grad_shape': (_i, [_p, _i, c_int_p, c_int_p, c_int_p, c_int_p]),
     'ssdk_trainer_read_grad': (_i, [_p, _i, _p, _p]),
     'ssdk_trainer_read_grad_planes': (_i, [_p, _i, _p, _p, _p]),
-    'ssdk_train_backward_begin': (_i, [_p, _p, _p, _i, _i, _f, _p, _p]),
     'ssdk_train_backward_layers': (_i, [_p, _p, _i, _i, _p]),
     'ssdk_train_apply': (_i, [_p, _f, _f, _f, _f, _p]),
     'ssdk_train_apply_adam': (_i, [_p, _f, _f, _f, _f, _f, _f, _i, _p]),

@@ -423,7 +423,6 @@ struct ssdk_trainer {
   // the trainer; [1] Adam second moment, made by the first Adam update
   float* state[2] = {nullptr, nullptr};
   __nv_bfloat16 *xT_hi = nullptr, *xT_lo = nullptr, *dyT_hi = nullptr, *dyT_lo = nullptr;   // scratch, sized for the largest layer
-  float* dypred = nullptr;                  // [B*P*(C+12)]
   std::vector<char> written;                // backward pass state: which activations already hold a partial gradient
   std::vector<void*> allocs;
 };
@@ -649,7 +648,6 @@ int plan_trainer(ssdk_trainer* t, float* flat_grad_dev) {
   const int n = (int)m->layers.size();
   t->tl.resize(n);
   int rc = plan_params(t, flat_grad_dev); if (rc) return rc;
-  rc = dev_alloc(t->allocs, &t->dypred, (size_t)m->B * m->P * (m->Ctot + 12), true); if (rc) return rc;
   rc = alloc_grad_planes(t); if (rc) return rc;
   // in the backward pass's order: does the producer's gradient buffer already hold a contribution?
   std::vector<char> written(n, 0);
@@ -775,27 +773,16 @@ int backward_layers(ssdk_trainer* t, const float* dypred, int hi, int lo, cudaSt
 
 }  // namespace
 
-// Loss (optional) and d loss / d y_pred from one launch of the fused loss kernel; clears the gradient buffer.
-extern "C" int ssdk_train_backward_begin(ssdk_trainer* t, const float* y_true, const float* y_pred, int neg_pos_ratio, int n_neg_min,
-                                         float alpha, float* out_loss, void* stream_) {
-  SSDK_REQUIRE(t && y_true && y_pred, "ssdk_train_backward_begin: NULL argument");
-  ssdk_model* m = t->m;
-  ssdk_ctx* ctx = m->ctx;
-  SSDK_CHECK_CUDA(cudaMemsetAsync(t->grad, 0, (size_t)t->n_params * sizeof(float), (cudaStream_t)stream_));
-  return ssdk_ssd_loss(ctx, y_true, y_pred, m->B, m->P, m->Ctot, neg_pos_ratio, n_neg_min, alpha, nullptr, out_loss, nullptr, t->dypred, stream_);
-}
-
 // The backward pass of layers hi, hi-1, ..., lo (graph indices; a full pass is n_layers-1 .. 0 in one or several calls, top
 // down).  When it returns (stream order), the parameter gradients of exactly these layers are final -- their span of the
-// flat buffer can be all-reduced while the lower layers are still being differentiated.  dypred_dev NULL: the gradient
-// ssdk_train_backward_begin left in the trainer; otherwise d loss / d y_pred provided by the caller (the buffer is cleared
-// when the pass starts at the top layer).
+// flat buffer can be all-reduced while the lower layers are still being differentiated.  dypred_dev: d loss / d y_pred, which
+// the caller's loss wrote; a pass that starts at the top layer clears the gradient buffer first.
 extern "C" int ssdk_train_backward_layers(ssdk_trainer* t, const float* dypred_dev, int hi, int lo, void* stream_) {
-  SSDK_REQUIRE(t, "ssdk_train_backward_layers: NULL trainer");
+  SSDK_REQUIRE(t && dypred_dev, "ssdk_train_backward_layers: NULL argument");
   const int n = (int)t->m->layers.size();
   SSDK_REQUIRE(hi < n && lo >= 0 && lo <= hi, "ssdk_train_backward_layers: bad layer range [%d, %d] of %d layers", lo, hi, n);
-  if (dypred_dev && hi == n - 1) SSDK_CHECK_CUDA(cudaMemsetAsync(t->grad, 0, (size_t)t->n_params * sizeof(float), (cudaStream_t)stream_));
-  return backward_layers(t, dypred_dev ? dypred_dev : t->dypred, hi, lo, (cudaStream_t)stream_);
+  if (hi == n - 1) SSDK_CHECK_CUDA(cudaMemsetAsync(t->grad, 0, (size_t)t->n_params * sizeof(float), (cudaStream_t)stream_));
+  return backward_layers(t, dypred_dev, hi, lo, (cudaStream_t)stream_);
 }
 
 namespace {

@@ -112,9 +112,9 @@ def all_reduce_buckets_(flat_grad, buckets, produce, group=None):
 class GlobalLossRun:
     """One rank's side of the phase-wise loss (``ssdk_ssd_loss_phase``): owns the workspace and exposes the tensors that have
     to be reduced between the phases.  ``ssd_loss_global`` drives it with torch.distributed; the single-GPU tests drive several
-    instances and add the tensors by hand."""
+    instances and add the tensors by hand.  With ``return_grad`` the gradient goes to ``grad_out`` when given."""
 
-    def __init__(self, y_true, y_pred, neg_pos_ratio, n_neg_min, alpha, world, rank, return_grad):
+    def __init__(self, y_true, y_pred, neg_pos_ratio, n_neg_min, alpha, world, rank, return_grad, grad_out=None):
         import ctypes as C
         import torch
         from . import _ffi
@@ -134,7 +134,10 @@ class GlobalLossRun:
         self.ties_all = torch.zeros((self.world,), dtype=torch.int32, device=dev)
         self.loss = torch.empty((self.B,), dtype=torch.float32, device=dev)
         self.stats = torch.zeros((4,), dtype=torch.int32, device=dev)
-        self.grad = torch.empty_like(self.yp) if return_grad else None
+        self.grad = None
+        if return_grad:
+            self.grad = torch.empty_like(self.yp) if grad_out is None else grad_out
+            assert self.grad.shape == self.yp.shape and self.grad.dtype == torch.float32 and self.grad.is_contiguous()
 
     def phase(self, i):
         from . import _ffi
@@ -147,7 +150,7 @@ class GlobalLossRun:
                                                   _ffi.dptr(self.grad if final else None), _ffi.stream_ptr()))
 
 
-def ssd_loss_global(y_true, y_pred, neg_pos_ratio=3, n_neg_min=0, alpha=1.0, group=None, return_grad=False):
+def ssd_loss_global(y_true, y_pred, neg_pos_ratio=3, n_neg_min=0, alpha=1.0, group=None, return_grad=False, grad_out=None):
     """Global-batch-exact ``SSDLoss.compute_loss`` for a batch that is sharded over the ranks of ``group`` (SURVEY section 8e(ii)).
 
     The reference's ``n_positive`` (keras_ssd_loss.py:143) and its hard-negative top-k (:179-183) run over the WHOLE batch.
@@ -155,13 +158,14 @@ def ssd_loss_global(y_true, y_pred, neg_pos_ratio=3, n_neg_min=0, alpha=1.0, gro
     one by one and the integer counts / histograms in its workspace are summed with all-reduces in between (2 x int64, then
     two histograms of 67 584 int32), ties at the k-th value are resolved by GLOBAL flat index via an all-gather of one int per
     rank.  Returns the ``(B_local,)`` losses of this rank's images -- exactly the entries the single-process reference
-    computes for them -- and, with ``return_grad``, ``(loss, d(mean over the global batch)/d y_pred of this shard, stats)``.
-    Without an initialised process group this is the single-rank result (phases run back to back)."""
+    computes for them -- and, with ``return_grad``, ``(loss, d(mean over the global batch)/d y_pred of this shard, stats)``,
+    the gradient written into ``grad_out`` when given.  Without an initialised process group this is the single-rank result
+    (phases run back to back)."""
     import torch.distributed as dist
     on = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
     world = dist.get_world_size(group) if on else 1
     rank = dist.get_rank(group) if on else 0
-    run = GlobalLossRun(y_true, y_pred, neg_pos_ratio, n_neg_min, alpha, world, rank, return_grad)
+    run = GlobalLossRun(y_true, y_pred, neg_pos_ratio, n_neg_min, alpha, world, rank, return_grad, grad_out)
     run.phase(0)
     if on:
         dist.all_reduce(run.counts, group=group)

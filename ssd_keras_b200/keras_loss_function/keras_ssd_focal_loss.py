@@ -10,44 +10,13 @@ no batch-global top-k is needed.  The localisation term, the positives and the n
 import math
 
 from .. import _ffi
-from .keras_ssd_loss import _as_cuda
+from .keras_ssd_loss import KernelLoss
 
 
-def _make_fn():
-    import torch
-
-    class _SSDFocalLossFn(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, y_true, y_pred, gamma, focal_alpha, alpha):
-            B, P, W = y_pred.shape
-            out = torch.empty((B,), dtype=torch.float32, device=y_pred.device)
-            _ffi.check(_ffi.lib().ssdk_focal_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
-                                                  W - 12, gamma, focal_alpha, alpha, _ffi.dptr(None), _ffi.dptr(out),
-                                                  _ffi.dptr(None), _ffi.stream_ptr()))
-            ctx.save_for_backward(y_true, y_pred)
-            ctx.cfg = (gamma, focal_alpha, alpha)
-            return out
-
-        @staticmethod
-        def backward(ctx, grad_out):
-            y_true, y_pred = ctx.saved_tensors
-            B, P, W = y_pred.shape
-            g = torch.empty_like(y_pred)
-            up = grad_out.to(dtype=torch.float32).contiguous()
-            _ffi.check(_ffi.lib().ssdk_focal_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P,
-                                                  W - 12, *ctx.cfg, _ffi.dptr(up), _ffi.dptr(None), _ffi.dptr(g),
-                                                  _ffi.stream_ptr()))
-            return None, g, None, None, None
-
-    return _SSDFocalLossFn
-
-
-_FN = None
-
-
-class SSDFocalLoss:
+class SSDFocalLoss(KernelLoss):
     """``gamma``: the focusing exponent (0 gives the weighted log-loss); ``focal_alpha``: the weight of the object classes, the
     background's being ``1 - focal_alpha``; ``alpha``: the weight of the localisation term, as in ``SSDLoss``."""
+    config_key = 'ssd_focal_loss'
 
     def __init__(self, gamma=2.0, focal_alpha=0.25, alpha=1.0):
         if not (float(gamma) >= 0 and math.isfinite(float(gamma))):
@@ -62,15 +31,14 @@ class SSDFocalLoss:
         """The constructor's arguments, as ``model.save`` stores them."""
         return {'gamma': self.gamma, 'focal_alpha': self.focal_alpha, 'alpha': self.alpha}
 
-    def compute_loss(self, y_true, y_pred):
-        """(B,P,C+12) x2 -> (B,) float32 CUDA tensor."""
-        global _FN
-        if _FN is None:
-            _FN = _make_fn()
-        yt, yp = _as_cuda(y_true), _as_cuda(y_pred)
-        if yt.shape != yp.shape or yt.dim() != 3 or yt.shape[-1] < 14:
-            raise ValueError("y_true and y_pred must both have shape (batch, #boxes, #classes + 12) with at least two classes, "
-                             "got %s and %s" % (tuple(yt.shape), tuple(yp.shape)))
-        if yt.device != yp.device:
-            raise ValueError("y_true and y_pred must live on the same device")
-        return _FN.apply(yt, yp, self.gamma, self.focal_alpha, self.alpha)
+    def _launch(self, y_true, y_pred, upstream, out_loss, out_grad):
+        B, P, W = y_pred.shape
+        _ffi.check(_ffi.lib().ssdk_focal_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P, W - 12,
+                                              self.gamma, self.focal_alpha, self.alpha, _ffi.dptr(upstream), _ffi.dptr(out_loss),
+                                              _ffi.dptr(out_grad), _ffi.stream_ptr()))
+
+    def _global(self, y_true, y_pred, grad_out, group):
+        from ..distributed import focal_loss_global
+        loss, _ = focal_loss_global(y_true, y_pred, self.gamma, self.focal_alpha, self.alpha, group=group, return_grad=True,
+                                    grad_out=grad_out)
+        return loss

@@ -52,8 +52,7 @@ class KerasTrainingMixin:
         ``loss``: ``SSDLoss(...).compute_loss`` (the bound method, as in the reference) or the ``SSDLoss`` object, or the same of
         an ``SSDFocalLoss``."""
         from .. import optimizers
-        from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
-        from ..keras_loss_function.keras_ssd_loss import SSDLoss
+        from ..keras_loss_function.keras_ssd_loss import KernelLoss
         if kwargs:
             raise TypeError('compile() got unsupported arguments: %s' % sorted(kwargs))
         if isinstance(optimizer, str):
@@ -64,7 +63,7 @@ class KerasTrainingMixin:
         if kind not in ('sgd', 'adam') or not hasattr(optimizer, 'lr'):
             raise ValueError('unsupported optimizer %r: SGD (lr, momentum) and Adam (lr, beta_1, beta_2, epsilon) are implemented' % (optimizer,))
         owner = getattr(loss, '__self__', loss)
-        if not isinstance(owner, (SSDLoss, SSDFocalLoss)):
+        if not isinstance(owner, KernelLoss):
             raise ValueError('loss must be SSDLoss(...).compute_loss (keras_loss_function/keras_ssd_loss.py:98) or '
                              'SSDFocalLoss(...).compute_loss: the training step computes that loss and its gradient on the device')
         self.optimizer, self._compiled = optimizer, (kind, owner)
@@ -73,10 +72,9 @@ class KerasTrainingMixin:
 
     # -- the training half of a full-model file (Keras' training_config and /optimizer_weights) --------------------------------
     def _training_config(self):
-        """Keras' ``training_config`` root attribute of ``model.save``, with the ``SSDLoss`` parameters (``'ssd_loss'``) or the
-        ``SSDFocalLoss`` parameters (``'ssd_focal_loss'``) load_model rebuilds the loss from when ``custom_objects`` does not bring
+        """Keras' ``training_config`` root attribute of ``model.save``, with the loss's parameters under its ``config_key``
+        (``'ssd_loss'`` or ``'ssd_focal_loss'``), which load_model rebuilds the loss from when ``custom_objects`` does not bring
         it."""
-        from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
         kind, lossobj = self._compiled
         o = self.optimizer
         if kind == 'sgd':
@@ -87,10 +85,7 @@ class KerasTrainingMixin:
                                                     'beta_2': float(getattr(o, 'beta_2', 0.999)), 'decay': 0.0,
                                                     'epsilon': float(getattr(o, 'epsilon', 1e-8)), 'amsgrad': False}}
         out = {'optimizer_config': opt, 'loss': 'compute_loss', 'metrics': [], 'sample_weight_mode': None, 'loss_weights': None}
-        if isinstance(lossobj, SSDFocalLoss):
-            out['ssd_focal_loss'] = lossobj.config()
-        else:
-            out['ssd_loss'] = {'neg_pos_ratio': lossobj.neg_pos_ratio, 'n_neg_min': lossobj.n_neg_min, 'alpha': lossobj.alpha}
+        out[lossobj.config_key] = lossobj.config()
         return out
 
     def _optimizer_weights(self):
@@ -111,7 +106,7 @@ class KerasTrainingMixin:
         state (checked against this model) for the trainer of the next step."""
         from .. import optimizers
         from ..keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
-        from ..keras_loss_function.keras_ssd_loss import SSDLoss
+        from ..keras_loss_function.keras_ssd_loss import KernelLoss, SSDLoss
         from ..training import check_optimizer_state
         oc = config['optimizer_config']
         c = oc['config']
@@ -122,11 +117,9 @@ class KerasTrainingMixin:
         else:
             raise ValueError('training_config names the optimizer %r: SGD and Adam are implemented' % (oc['class_name'],))
         loss = (custom_objects or {}).get('compute_loss')
-        if not isinstance(getattr(loss, '__self__', None), (SSDLoss, SSDFocalLoss)):
-            if 'ssd_focal_loss' in config:
-                loss = SSDFocalLoss(**config['ssd_focal_loss']).compute_loss
-            else:
-                loss = SSDLoss(**config['ssd_loss']).compute_loss
+        if not isinstance(getattr(loss, '__self__', None), KernelLoss):
+            cls = next((c for c in (SSDFocalLoss, SSDLoss) if c.config_key in config), SSDLoss)
+            loss = cls(**config[cls.config_key]).compute_loss
         self.compile(optimizer=opt, loss=loss)
         if not opt_weights:
             return

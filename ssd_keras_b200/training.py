@@ -1,8 +1,8 @@
 """Training step on H100: what ``model.compile(optimizer=SGD(lr, momentum), loss=SSDLoss().compute_loss)`` +
-``train_on_batch`` do in the reference (``ssd300_training.ipynb:169-173``), through ``ssdk_train_backward_begin`` /
-``ssdk_train_backward_layers`` / ``ssdk_train_apply`` (``csrc/train.cu``).  Data-parallel: every rank runs the same step on
-its shard and the flat gradient buffer is summed with ONE NCCL all-reduce before the update (replica-local loss, SURVEY.md
-section 8e(i)).
+``train_on_batch`` do in the reference (``ssd300_training.ipynb:169-173``): the loss writes d loss / d y_pred into a buffer of
+the trainer's (``KernelLoss.loss_and_grad``), then ``ssdk_train_backward_layers`` / ``ssdk_train_apply`` (``csrc/train.cu``).
+Data-parallel: every rank runs the same step on its shard and the flat gradient buffer is summed with ONE NCCL all-reduce
+before the update (replica-local loss, SURVEY.md section 8e(i)).
 """
 import ctypes as C
 import weakref
@@ -36,23 +36,21 @@ def check_optimizer_state(model, optimizer, state):
 
 
 class SSDTrainer:
-    def __init__(self, model, batch_size, lr=1e-3, momentum=0.9, l2_regularization=None, neg_pos_ratio=3, n_neg_min=0,
-                 alpha=1.0, loss_mode='replica', optimizer='sgd', beta_1=0.9, beta_2=0.999, epsilon=1e-8, loss=None):
-        """``loss_mode``: 'replica' -- every rank applies the reference loss to its own shard (what Keras data-parallel replicas
-        compute, SURVEY 8e(i)); 'global' -- n_positive and the hard-negative top-k run over the whole sharded batch, so that N
-        ranks reproduce the single-process reference on the full batch (8e(ii), ``distributed.ssd_loss_global``).
-        ``loss``: an ``SSDLoss`` (its parameters replace neg_pos_ratio, n_neg_min and alpha) or an ``SSDFocalLoss``, whose
-        gradient the step writes into a buffer of the trainer's own and hands to the backward pass (with 'global', its number
-        of positives runs over the whole sharded batch, ``distributed.focal_loss_global``); None is ``SSDLoss`` with the
-        parameters above."""
-        from .keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
-        from .keras_loss_function.keras_ssd_loss import SSDLoss
-        if loss is not None and not isinstance(loss, (SSDLoss, SSDFocalLoss)):
+    def __init__(self, model, batch_size, lr=1e-3, momentum=0.9, l2_regularization=None, loss_mode='replica', optimizer='sgd',
+                 beta_1=0.9, beta_2=0.999, epsilon=1e-8, loss=None):
+        """``loss``: an ``SSDLoss`` or an ``SSDFocalLoss`` (any ``KernelLoss``); None is ``SSDLoss()``.  Each step it writes
+        d loss / d y_pred into a buffer of the trainer's, from which the backward pass starts.
+        ``loss_mode``: 'replica' -- every rank applies the loss to its own shard (what Keras data-parallel replicas compute,
+        SURVEY 8e(i)); 'global' -- the loss's batch-global quantities (SSDLoss: n_positive and the hard-negative top-k; the
+        focal loss: n_positive) run over the whole sharded batch, so that N ranks reproduce the single-process loss on the full
+        batch (8e(ii), ``distributed.ssd_loss_global`` / ``focal_loss_global``)."""
+        import torch
+        from .keras_loss_function.keras_ssd_loss import KernelLoss, SSDLoss
+        if loss is None:
+            loss = SSDLoss()
+        if not isinstance(loss, KernelLoss):
             raise ValueError('loss must be an SSDLoss or an SSDFocalLoss, got %r' % (loss,))
-        if isinstance(loss, SSDLoss):
-            neg_pos_ratio, n_neg_min, alpha = loss.neg_pos_ratio, loss.n_neg_min, loss.alpha
-        self.focal = loss if isinstance(loss, SSDFocalLoss) else None
-        self._dy = None                          # d loss / d y_pred of the focal loss (B, P, C+12)
+        self.loss = loss
         if loss_mode not in ('replica', 'global'):
             raise ValueError("loss_mode must be 'replica' or 'global'")
         if optimizer not in ('sgd', 'adam'):
@@ -61,12 +59,11 @@ class SSDTrainer:
         self.optimizer, self.beta_1, self.beta_2, self.epsilon = optimizer, float(beta_1), float(beta_2), float(epsilon)
         self.iterations = 0                      # optimiser steps taken (Adam's bias correction)
         self._n_slots = 1                        # optimiser state slots on the device: Adam's v is made by its first update
-        import torch
         self.model = model
         self.batch = int(batch_size)
         self.lr, self.momentum = float(lr), float(momentum)
         self.l2 = float(model.l2_regularization if l2_regularization is None else l2_regularization)
-        self.neg_pos_ratio, self.n_neg_min, self.alpha = int(neg_pos_ratio), int(n_neg_min), float(alpha)
+        self._dy = torch.empty((self.batch, model.n_boxes_total, model.n_classes + 12), dtype=torch.float32, device='cuda')
         # the flat gradient buffer is a torch tensor so that torch.distributed can all-reduce it in place
         self.n_params = self._count_trainable(model)
         self.grad = torch.zeros((self.n_params,), dtype=torch.float32, device='cuda')
@@ -131,38 +128,13 @@ class SSDTrainer:
             raise ValueError('images and y_true must be CUDA tensors')
 
     def _loss_and_dy(self, images, y_true):
-        """forward + loss; leaves d loss / d y_pred ready for the layer-wise backward.  Returns (loss, y_pred, dy or None)."""
+        """forward + loss; leaves d loss / d y_pred in ``self._dy`` for the layer-wise backward.  Returns (loss, y_pred, dy)."""
         import torch
         self._attach()
         self._check_batch(images, y_true)
         y_pred = self.model.forward_device(images, training=True)
         y_true = y_true.to(dtype=torch.float32).contiguous()
-        if self.focal is not None:
-            return self._focal_loss_and_dy(y_true, y_pred)
-        if self.loss_mode == 'global':
-            from .distributed import ssd_loss_global
-            loss, dy, _ = ssd_loss_global(y_true, y_pred, self.neg_pos_ratio, self.n_neg_min, self.alpha, return_grad=True)
-            return loss, y_pred, dy
-        loss = torch.empty((self.batch,), dtype=torch.float32, device=images.device)
-        _ffi.check(_ffi.lib().ssdk_train_backward_begin(self.handle, _ffi.dptr(y_true), _ffi.dptr(y_pred), self.neg_pos_ratio,
-                                                        self.n_neg_min, self.alpha, _ffi.dptr(loss), _ffi.stream_ptr()))
-        return loss, y_pred, None
-
-    def _focal_loss_and_dy(self, y_true, y_pred):
-        import torch
-        f = self.focal
-        if self._dy is None or self._dy.shape != y_pred.shape:
-            self._dy = torch.empty_like(y_pred)
-        if self.loss_mode == 'global':
-            from .distributed import focal_loss_global
-            loss, _ = focal_loss_global(y_true, y_pred, f.gamma, f.focal_alpha, f.alpha, return_grad=True, grad_out=self._dy)
-            return loss, y_pred, self._dy
-        B, P, W = y_pred.shape
-        loss = torch.empty((B,), dtype=torch.float32, device=y_pred.device)
-        _ffi.check(_ffi.lib().ssdk_focal_loss(_ffi.context(y_pred.device.index), _ffi.dptr(y_true), _ffi.dptr(y_pred), B, P, W - 12,
-                                              f.gamma, f.focal_alpha, f.alpha, _ffi.dptr(None), _ffi.dptr(loss), _ffi.dptr(self._dy),
-                                              _ffi.stream_ptr()))
-        return loss, y_pred, self._dy
+        return self.loss.loss_and_grad(y_true, y_pred, self._dy, self.loss_mode), y_pred, self._dy
 
     def _backward_layers(self, dy, hi, lo):
         _ffi.check(_ffi.lib().ssdk_train_backward_layers(self.handle, _ffi.dptr(dy), int(hi), int(lo), _ffi.stream_ptr()))

@@ -7,8 +7,8 @@ and bound of tests/focal_reference.py, call by call:
   loads, which give the float4 path's bits), upstream with zero and negative entries, the clamp's edges and q = 1, no positives;
 - two calls are bit-identical, and 1, 2 and 4 emulated ranks through ssdk_focal_loss_phase give the single launch's bits;
 - refused parameters raise ValueError before any launch;
-- training: the dy the trainer hands to the backward pass is the kernel's gradient, an SSD7 fit_generator run lowers the loss,
-  and save -> load_model -> fit_generator(initial_epoch=...) resumes.
+- training: the dy the trainer hands to the backward pass is the loss kernel's gradient, for SSDLoss and the focal loss in both
+  loss modes, an SSD7 fit_generator run lowers the loss, and save -> load_model -> fit_generator(initial_epoch=...) resumes.
 Ratios go to SSDK_KERNEL_ERRORS_LOG (conv_cases.log_ratio).
 """
 import itertools
@@ -259,24 +259,49 @@ def _batches(m, B, n, seed):
             for i in range(n)]
 
 
-@pytest.mark.parametrize('loss_mode', ['replica', 'global'])
-def test_trainer_hands_the_kernel_gradient_to_the_backward_pass(loss_mode):
+def _single_launch(lossobj, yt_d, yp_d):
+    """The loss's own ssdk_ssd_loss / ssdk_focal_loss call with the loss, a gradient output and no upstream -> (loss, grad)."""
     import torch
+    from ssd_keras_b200 import _ffi
     from ssd_keras_b200.keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
+    if isinstance(lossobj, SSDFocalLoss):
+        return run_focal('fwd_bwd', yt_d, yp_d, (lossobj.gamma, lossobj.focal_alpha, lossobj.alpha))
+    B, P, W = yp_d.shape
+    loss = torch.full((B,), np.nan, dtype=torch.float32, device='cuda')
+    grad = torch.full_like(yp_d, np.nan)
+    d = _ffi.dptr
+    _ffi.check(_ffi.lib().ssdk_ssd_loss(_ffi.context(), d(yt_d), d(yp_d), B, P, W - 12, lossobj.neg_pos_ratio, lossobj.n_neg_min,
+                                        lossobj.alpha, None, d(loss), None, d(grad), _ffi.stream_ptr()))
+    torch.cuda.synchronize()
+    return loss.cpu().numpy(), grad.cpu().numpy()
+
+
+@pytest.mark.parametrize('loss_mode', ['replica', 'global'])
+@pytest.mark.parametrize('loss_name', ['ssd', 'focal'])
+def test_trainer_hands_the_kernel_gradient_to_the_backward_pass(loss_name, loss_mode):
+    """Either loss writes d loss / d y_pred into the trainer's buffer: the bits of its own single launch, which the backward pass
+    then reads.  A NULL d loss / d y_pred is refused before the gradient buffer is touched."""
+    import torch
+    from ssd_keras_b200 import _ffi
+    from ssd_keras_b200.keras_loss_function.keras_ssd_focal_loss import SSDFocalLoss
+    from ssd_keras_b200.keras_loss_function.keras_ssd_loss import SSDLoss
     from ssd_keras_b200.training import SSDTrainer
     m = _ssd7()
-    f = SSDFocalLoss(gamma=2.0, focal_alpha=0.25, alpha=1.0)
-    tr = SSDTrainer(m, 2, lr=1e-3, loss=f, loss_mode=loss_mode, optimizer='adam')
+    lossobj = SSDLoss(neg_pos_ratio=3, n_neg_min=0, alpha=1.0) if loss_name == 'ssd' else SSDFocalLoss(gamma=2.0, focal_alpha=0.25)
+    tr = SSDTrainer(m, 2, lr=1e-3, loss=lossobj, loss_mode=loss_mode, optimizer='adam')
     x, y = _batches(m, 2, 1, seed=4)[0]
     xd, yd = torch.from_numpy(x).cuda(), torch.from_numpy(y).cuda()
     loss, y_pred, dy = tr._loss_and_dy(xd, yd)
     assert dy is tr._dy
     y_pred = y_pred.clone()
-    want_loss, want_grad = run_focal('fwd_bwd', yd, y_pred, (f.gamma, f.focal_alpha, f.alpha))
+    want_loss, want_grad = _single_launch(lossobj, yd, y_pred)
     assert np.array_equal(_bits(loss.cpu().numpy()), _bits(want_loss)) and np.array_equal(_bits(dy.cpu().numpy()), _bits(want_grad))
     tr._backward_layers(dy, len(m.specs) - 1, 0)
     g = tr.grad.cpu().numpy()
     assert np.all(np.isfinite(g)) and np.any(g != 0)
+    with pytest.raises(ValueError, match='NULL'):
+        _ffi.check(_ffi.lib().ssdk_train_backward_layers(tr.handle, None, len(m.specs) - 1, 0, _ffi.stream_ptr()))
+    assert np.array_equal(_bits(tr.grad.cpu().numpy()), _bits(g))
 
 
 def test_fit_generator_with_focal_loss_trains_and_resumes(tmp_path):
@@ -299,6 +324,6 @@ def test_fit_generator_with_focal_loss_trains_and_resumes(tmp_path):
     lossobj = m2._compiled[1]
     assert isinstance(lossobj, SSDFocalLoss) and lossobj.config() == focal.config()
     t2 = m2._trainer_for(4)
-    assert t2.focal is lossobj and t2.iterations == st0['iterations'] == 12
+    assert t2.loss is lossobj and t2.iterations == st0['iterations'] == 12
     h2 = m2.fit_generator(itertools.cycle(data), steps_per_epoch=2, epochs=7, initial_epoch=6)
     assert h2.epoch == [6] and np.isfinite(h2.history['loss'][0]) and t2.iterations == 14

@@ -1,6 +1,6 @@
 """GPU parity tests for the training step (SURVEY.md A16 / BASELINE config 3): loss, every gradient and the SGD-momentum
-update of ``ssdk_train_backward_begin`` / ``_layers`` / ``ssdk_train_apply`` against float64 torch autograd over the same
-layer specs (oracle/graph.py) on identical weights, images and encoded ground truth.
+update of ``SSDLoss.loss_and_grad`` / ``ssdk_train_backward_layers`` / ``ssdk_train_apply`` against float64 torch autograd
+over the same layer specs (oracle/graph.py) on identical weights, images and encoded ground truth.
 
 Tolerance: the backward GEMMs run in the same bf16x3 mode as the forward pass (~16 significant bits per product, fp32
 accumulation); gradients are compared at 2e-3 of the tensor's max magnitude (measured 5e-6 .. 2e-4; 1e-3 where one ReLU

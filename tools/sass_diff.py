@@ -63,7 +63,8 @@ def compile_tree(tree, objdir, nvcc):
             return src, None
         obj = os.path.join(objdir, src.replace('.cu', '.o'))
         log = _run([nvcc, '-Xptxas', '-v'] + ARCH + COMMON + SOURCES[src] + ['-c', path, '-o', obj])
-        warnings = collections.Counter(_norm(l) for l in log.splitlines() if _WARNING.search(l))
+        # host-compiler warnings name the source by its path in the tree: compare them without it
+        warnings = collections.Counter(_norm(l.replace(tree + os.sep, '')) for l in log.splitlines() if _WARNING.search(l))
         return src, (_per_function(_run([cuobjdump, '-sass', obj]), _FUNC_SASS),
                      _per_function(_run([cuobjdump, '-res-usage', obj]), _FUNC_RES), warnings)
 
