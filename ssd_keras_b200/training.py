@@ -127,14 +127,15 @@ class SSDTrainer:
         if not (images.is_cuda and y_true.is_cuda):
             raise ValueError('images and y_true must be CUDA tensors')
 
-    def _loss_and_dy(self, images, y_true):
-        """forward + loss; leaves d loss / d y_pred in ``self._dy`` for the layer-wise backward.  Returns (loss, y_pred, dy)."""
+    def _loss_and_dy(self, images, y_true, group=None):
+        """forward + loss; leaves d loss / d y_pred in ``self._dy`` for the layer-wise backward.  Returns (loss, y_pred, dy).
+        ``group``: the process group a 'global' loss reduces its batch-global quantities over (None: the default group)."""
         import torch
         self._attach()
         self._check_batch(images, y_true)
         y_pred = self.model.forward_device(images, training=True)
         y_true = y_true.to(dtype=torch.float32).contiguous()
-        return self.loss.loss_and_grad(y_true, y_pred, self._dy, self.loss_mode), y_pred, self._dy
+        return self.loss.loss_and_grad(y_true, y_pred, self._dy, self.loss_mode, group=group), y_pred, self._dy
 
     def _backward_layers(self, dy, hi, lo):
         _ffi.check(_ffi.lib().ssdk_train_backward_layers(self.handle, _ffi.dptr(dy), int(hi), int(lo), _ffi.stream_ptr()))
@@ -185,7 +186,7 @@ class SSDTrainer:
         bucketed exchange is used from 4 ranks on."""
         import torch.distributed as dist
         on = dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1
-        loss, _, dy = self._loss_and_dy(images, y_true)
+        loss, _, dy = self._loss_and_dy(images, y_true, group)
         if not on:
             self._backward_layers(dy, len(self.model.specs) - 1, 0)
             self.apply(1.0)
